@@ -10,7 +10,9 @@ latents).  `value` times device-resident inputs; `e2e` times the public API
 (ns2vc_b200.api.sample_latents) from pinned host tensors to a host result, copies inside the timed
 region.  Weak scaling over GPUs (independent utterances per rank, SURVEY.md §8e).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR: the last timed step's latents as DIR/latents.npy (float32 [B, 100, T]; inputs are seeded).
 """
 from __future__ import annotations
 
@@ -40,7 +42,7 @@ SURVEY_BYTES_CFG2 = 3.20e9
 def workload_cfg(n_gpus):
     return {"workload": f"cfg2: B={B}/GPU, C=100, T={T}, S={S}, {NFE}-step DPM-Solver++(2M) multistep time_uniform, x_start UNet1D (66.08M params)",
             "global_batch": B * n_gpus, "nfe": NFE, "parallelism": f"utterance-shard x{n_gpus} (one all-gather of latents)" if n_gpus > 1 else "single GPU",
-            "l2_policy": "per-forward weight stream (264 MB packed bf16 hi/lo + 2.9 GB activations) exceeds the 126 MB L2; no explicit flush"}
+            "l2_policy": "per-forward weight stream (264 MB packed bf16 hi/lo + 2.9 GB activations) exceeds the 50 MB L2; no explicit flush"}
 
 
 def flops_per_forward(cfg, Bn, Tn, Sn, gemm_only=False):
@@ -67,7 +69,7 @@ def read_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured (MEASURED_PEAKS.json, sustained bf16)"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "src": "NVIDIA H100 SXM data sheet (dense BF16, 700 W card; not reached)"}
 
 
 class ClockSampler:
@@ -207,7 +209,7 @@ def run_reference(args, rank, world):
     with torch.no_grad():
         sampler_oracle.dpmpp_2m(fn, sch, inp["x"], NFE)
     full_dt = time.perf_counter() - t1
-    sample = f"{per_step} of {NFE} denoiser calls (UNet forward + x0 round trip) per step at B={B},T={T},S={S}; reference CPU path via the oracle port (reference is pure PyTorch; /root/reference is absent on the GPU box)"
+    sample = f"{per_step} of {NFE} denoiser calls (UNet forward + x0 round trip) per step at B={B},T={T},S={S}; reference CPU path via the oracle port (the reference is pure PyTorch)"
     print(json.dumps({"impl": "reference", "metric": METRIC, "value": val, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
                       "warmup": args.warmup, "ms_per_step": 1e3 * dt / args.steps, "higher_is_better": True, "scaling": "weak",
                       "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": workload_cfg(args.gpus),
@@ -282,20 +284,6 @@ def bench_pre_model(unet, dev, hin, nfe, with_cpu):
     return res
 
 
-def ncu_traffic(kernel):
-    """Average DRAM bytes per launch of `kernel` from the committed ncu launch list (profiles/)."""
-    p = os.path.join(REPO, "profiles", "r02_traffic.json")
-    if not os.path.exists(p):
-        p = os.path.join(REPO, "profiles", "r01_traffic.json")
-    if not os.path.exists(p):
-        return None
-    tab = json.load(open(p))
-    pref = "gemm_tc_kernel" if kernel == "gemm_tc" else "attn_v2_kernel"
-    n = sum(v["launches"] for k, v in tab.items() if k.startswith(pref))
-    tot = sum(v["launches"] * v["dram_bytes_per_launch"] for k, v in tab.items() if k.startswith(pref))
-    return tot / n if n else None
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -303,6 +291,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--nfe", type=int, default=NFE, help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's latents as DIR/latents.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -357,6 +346,8 @@ def main():
             return gathered.to("cpu", non_blocking=False) if rank == 0 else out[:1, :1, :1].cpu()
         return out.cpu()
 
+    last = {}
+
     def timed(fn, K, W, sample_clocks=False):
         for _ in range(W):
             fn()
@@ -368,7 +359,7 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(K):
-            fn()
+            last["out"] = fn()
         e1.record()
         torch.cuda.synchronize(dev)
         clocks = cs.stop() if cs else None
@@ -380,6 +371,11 @@ def main():
         return float(ms.item()), clocks
 
     ms, clocks = timed(run_device, args.steps, args.warmup, sample_clocks=True)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        lat = (gathered if world > 1 else last["out"]).float().cpu().numpy()
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), lat)
     # kernel launches per run, counted from the engine's own launch programs (one memset node per
     # forward is not a kernel and is subtracted; +1 sampler-update kernel per step)
     cnt = DenoiserSession(unet, content_d, prompt_d, mask_d)
@@ -455,13 +451,11 @@ def main():
         else:
             ach = fl_gemm / (dom_ms * 1e-3) / 1e12
             alg = f"{fl_gemm / 1e9:.1f} GFLOP conv+linear per forward (algorithmic, SURVEY 8d; the 3xBF16 split issues 3x this on the tensor pipe); all gemm_tc instantiations"
-        traffic = ncu_traffic(dom)
         whole = survey_flops(B, T, S)
         ms_fwd = ms / args.steps / nfe
         t_hbm = SURVEY_BYTES_CFG2 / (peaks["hbm_gbs"] * 1e9) * 1e3
         t_tc = whole / (peaks["tflops"] * 1e12) * 1e3
         out["roofline"] = {"kernel": dom, "bound": "tensor", "achieved": ach, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"],
-                           "traffic": traffic, "traffic_unit": "DRAM bytes per launch (ncu dram__bytes_read+write, cold-cache capture, profiles/r02_ncu_launches.md)",
                            "algorithmic": alg, "peak_source": peaks["src"], "issued_tflops": 3 * ach if dom == "gemm_tc" else ach,
                            "frac_issued": (3 * ach if dom == "gemm_tc" else ach) / peaks["tflops"],
                            "kernel_ms_per_forward": dom_ms, "launch_avg_us": 1e3 * dom_ms / dom_n,
@@ -471,7 +465,7 @@ def main():
                                     "binding": "hbm" if t_hbm >= t_tc else "tensor", "frac_vs_binding": max(t_hbm, t_tc) / ms_fwd,
                                     "achieved_tflops": whole / (ms_fwd * 1e-3) / 1e12, "achieved_gbs": SURVEY_BYTES_CFG2 / (ms_fwd * 1e-3) / 1e9,
                                     "note": "SURVEY.md 8(d) constants: 40.20 GFLOP per sample-step (321.6 per cfg2 step), 3.20 GB ideal-fusion bytes; graded against the tighter (larger-time) bound"},
-                           "note": "the step is a chain of dependent launches (PDL-linked, one CUDA graph): launches of <= 148 tiles are bound by per-launch latency (TMA round trip, epilogue stores at L2 bandwidth), not by the pipe's FLOP rate"}
+                           "note": "the step is a chain of dependent launches (PDL-linked, one CUDA graph): launches of <= 132 tiles are bound by per-launch latency (TMA round trip, epilogue stores at L2 bandwidth), not by the pipe's FLOP rate"}
         out["kernels"] = kernels
         out["forward_span_us"] = span_us
         # ---- cfg3 (BASELINE.json configs[2]): B=4, T=2048, UniPC bh2 at the reference default of 30 steps and at 50, same process

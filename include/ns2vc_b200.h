@@ -1,4 +1,4 @@
-/* ns2vc_b200 — C-ABI of the B200-native NS2VC denoiser hot path.
+/* ns2vc_b200 — C-ABI of the H100-native NS2VC denoiser hot path.
  *
  * The reference (adelacvg/NS2VC) is pure Python/PyTorch and defines no FFI; its boundary for this
  * path is the Python object graph (SURVEY.md §8b).  This header is the C boundary the Python
@@ -63,7 +63,7 @@ int ns2vc_unet_weight_info(const ns2vc_unet* h, int i, const char** name, int64_
 /* Copy one parameter (device fp32, contiguous) into the handle: load_state_dict per key. */
 int ns2vc_unet_load_weight(ns2vc_unet* h, const char* key, const float* dptr, const int64_t* shape, int ndim,
                            ns2vc_stream stream);
-/* Pack every contraction weight into the tcgen05 operand layout (bf16 hi/lo, swizzled tiles);
+/* Pack every contraction weight into the wgmma operand layout (bf16 hi/lo, swizzled tiles);
  * fails if any key is missing (strict load, reference inference/infer_tool.py:27). */
 int ns2vc_unet_finalize(ns2vc_unet* h, ns2vc_stream stream);
 

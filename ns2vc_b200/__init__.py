@@ -1,4 +1,4 @@
-"""ns2vc_b200 — B200-native (sm_100a) implementation of the NS2VC diffusion-denoiser hot path.
+"""ns2vc_b200 — H100-native (sm_90a) implementation of the NS2VC diffusion-denoiser hot path.
 
 Drop-in surface (same names as the reference):
     ns2vc_b200.unet.UNet1DConditionModel          <- unet1d/unet_1d_condition.py
@@ -19,7 +19,7 @@ __version__ = "0.1.0"
 
 def install() -> None:
     """Make ``unet1d.unet_1d_condition``, ``sampler.dpm_solver`` and ``sampler.uni_pc`` resolve to
-    the B200 implementations (call before ``import model`` in the reference tree).  The reference's
+    the CUDA implementations (call before ``import model`` in the reference tree).  The reference's
     own ``unet1d`` / ``sampler`` packages stay importable for their other submodules
     (``model.py:6`` imports ``unet1d.embeddings``); only the three hot-path modules are aliased."""
     import importlib
@@ -50,7 +50,7 @@ def install() -> None:
 
 
 def install_pre_model(model_module=None) -> None:
-    """Make the reference's ``model.Pre_model`` (defined inside ``model.py`` itself, :328) the B200 implementation: call after
+    """Make the reference's ``model.Pre_model`` (defined inside ``model.py`` itself, :328) the CUDA implementation: call after
     ``import model`` and before ``NaturalSpeech2(cfg)`` is constructed (``model.py:451`` looks the class up by its global name)."""
     from .pre_model import Pre_model
     if model_module is None:

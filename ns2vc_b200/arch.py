@@ -65,10 +65,10 @@ class UNetConfig:
             raise ValueError("Must provide the same number of `block_out_channels` as `down_block_types`.")
         for t in self.down_block_types:
             if t not in SUPPORTED_DOWN:
-                raise ValueError(f"{t} is not supported by the B200 denoiser (supported: {SUPPORTED_DOWN})")
+                raise ValueError(f"{t} is not supported by this denoiser (supported: {SUPPORTED_DOWN})")
         for t in self.up_block_types:
             if t not in SUPPORTED_UP:
-                raise ValueError(f"{t} is not supported by the B200 denoiser (supported: {SUPPORTED_UP})")
+                raise ValueError(f"{t} is not supported by this denoiser (supported: {SUPPORTED_UP})")
         if self.mid_block_type not in SUPPORTED_MID:
             raise ValueError(f"unknown mid_block_type : {self.mid_block_type}")
         if self.resnet_time_scale_shift not in ("default", "scale_shift"):

@@ -5,7 +5,7 @@
 // over 16-key chunks with exp2f and the scale*log2(e) folded into q.
 // Self-attention: k/v come from the fused QKV buffer; cross-attention: from the per-utterance
 // K/V cache with the additive mask bias (0 / -10000, NOT -inf: reference unet_1d_condition.py:817).
-#include "gemm_common.cuh"
+#include "flash_mma.cuh"
 #include "tc_common.cuh"
 #include "launch.cuh"
 #include <math.h>
@@ -125,24 +125,19 @@ static int launch_attention_simt(const AttnOp& op, cudaStream_t st) {
 
 
 // =============================================================================================
-// tcgen05 flash attention (product path).
-//   CTA = 128 queries of one (batch, head); key tiles of 64.
-//   S[128x64] = Q K^T and O_tile[128xdh] = P V run on the tensor cores with TMEM accumulators,
-//   each as three bf16 MMAs over hi/lo splits (fp32-level products, see gemm_tc.cu); the online
-//   softmax runs on warps 0-3 (one query row per thread = one TMEM lane), exp2 with the softmax
-//   scale and log2(e) folded into Q.  Q/K/V are read as fp32 rows (fused QKV buffer or the
-//   cross-attention K/V cache), split on the fly and written as K-major SWIZZLE_128B operand
-//   images (V transposed so that keys are the MMA K dimension).  96 KB smem -> 2 CTAs / SM.
+// Tensor-core flash attention for fp32 q / k / v (head dims the v2 kernel does not take, and long biased key rows).
+//   CTA = 128 queries of one (batch, head), 8 warps of 16 query rows; key tiles of 64.  Q/K/V are read as fp32 rows
+//   (fused QKV buffer or the cross-attention K/V cache), split on the fly into bf16 hi/lo and written as SWIZZLE_128B row
+//   images [rows][64 channels]; S = Q K^T and O += P V then run on the tensor cores (flash_mma.cuh), exp2 with the softmax
+//   scale and log2(e) folded into Q.  The next tile's global loads are in flight while the current one is computed.
 // =============================================================================================
 constexpr int AQ = 128, AKT = 64;
 constexpr int kAttnTcThreads = 256;
 constexpr int kOffQ = 0;                 // Q hi [128][64] bf16, lo follows
 constexpr int kOffK = 32768;             // K hi [64][64], lo follows
-constexpr int kOffV = kOffK + 16384;     // V^T hi [64 d][64 keys], lo follows
-constexpr int kOffP = kOffV + 16384;     // P hi [128][64], lo follows
-constexpr int kOffBias = kOffP + 32768;  // 64 floats
-constexpr int kOffBar = kOffBias + 256;
-constexpr int kAttnSmem = kOffBar + 64 + 1024 /*row max / row sum exchange*/ + 1024 /*alignment slack*/;
+constexpr int kOffV = kOffK + 16384;     // V hi [64 keys][64], lo follows
+constexpr int kOffBias = kOffV + 16384;  // 64 floats
+constexpr int kAttnSmem = kOffBias + 256 + 1024 /*alignment slack*/;
 
 __device__ __forceinline__ void load8(const float* p, bool row_ok, int d0, int dh, bool vec, float* v) {
 #pragma unroll
@@ -158,13 +153,11 @@ __device__ __forceinline__ void load8(const float* p, bool row_ok, int d0, int d
 }
 
 template <int DHP>
-__global__ void __launch_bounds__(kAttnTcThreads, 2) attn_tc_kernel(const AttnOp op) {
+__global__ void __launch_bounds__(kAttnTcThreads, 1) attn_tc_kernel(const AttnOp op) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - raw);
-  const uint32_t bar_s = base + kOffBar, bar_o = base + kOffBar + 8;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + kOffBar + 16);
   float* bias_s = reinterpret_cast<float*>(smem + kOffBias);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -177,8 +170,6 @@ __global__ void __launch_bounds__(kAttnTcThreads, 2) attn_tc_kernel(const AttnOp
   const bool vv = ((op.v_ld | (h * dh)) & 3) == 0 && (dh & 7) == 0;
 
   span_begin(op.span);
-  if (tid == 0) { mbar_init(bar_s, 1); mbar_init(bar_o, 1); mbar_fence_init(); }
-  if (warp == 4) tmem_alloc(smem_u32((const void*)tmem_slot), 128);
   pdl_trigger();
   pdl_wait();
 
@@ -216,21 +207,14 @@ __global__ void __launch_bounds__(kAttnTcThreads, 2) attn_tc_kernel(const AttnOp
       const int i = tid + u * kAttnTcThreads;
       if (i < AKT * CK) {
         const int key = i / CK, ck = i % CK;
+        const int off = key * 128 + ((ck ^ (key & 7)) << 4);
         uint4 hi, lo;
         split8(kreg[u], hi, lo);
-        const int off = key * 128 + ((ck ^ (key & 7)) << 4);
         *reinterpret_cast<uint4*>(smem + kOffK + off) = hi;
         *reinterpret_cast<uint4*>(smem + kOffK + 8192 + off) = lo;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {                      // V^T: row = d, column = key
-          const int d = ck * 8 + j;
-          const float x = vreg[u][j];
-          const __nv_bfloat16 xh = __float2bfloat16_rn(x);
-          const __nv_bfloat16 xl = __float2bfloat16_rn(x - __bfloat162float(xh));
-          const int voff = d * 128 + (((key >> 3) ^ (d & 7)) << 4) + (key & 7) * 2;
-          *reinterpret_cast<__nv_bfloat16*>(smem + kOffV + voff) = xh;
-          *reinterpret_cast<__nv_bfloat16*>(smem + kOffV + 8192 + voff) = xl;
-        }
+        split8(vreg[u], hi, lo);
+        *reinterpret_cast<uint4*>(smem + kOffV + off) = hi;
+        *reinterpret_cast<uint4*>(smem + kOffV + 8192 + off) = lo;
       }
     }
     if (tid < AKT) {
@@ -239,145 +223,20 @@ __global__ void __launch_bounds__(kAttnTcThreads, 2) attn_tc_kernel(const AttnOp
     }
   };
 
-  load_kv(0);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tO = tmem_base + 64;
-  constexpr uint32_t idS = umma_idesc_bf16(128, AKT);
-  constexpr uint32_t idO = umma_idesc_bf16(128, DHP);
-  const uint32_t sQ = base + kOffQ, sK = base + kOffK, sV = base + kOffV, sP = base + kOffP;
-
-  // Softmax on all 8 warps: warp w works on TMEM lane quarter (w & 3); warps 0-3 take score columns
-  // 0-31 and the first half of the head dim, warps 4-7 columns 32-63 and the second half.  The two
-  // threads of a row exchange their partial row maxima through shared memory (one 64-thread named
-  // barrier per tile) and their partial row sums once at the end.
-  constexpr int OH = DHP / 2;                              // output columns per thread
-  float o[OH];
-#pragma unroll
-  for (int d = 0; d < OH; ++d) o[d] = 0.f;
-  float m_run = -INFINITY, l_run = 0.f;
-  const int qtr = warp & 3, hf = warp >> 2;
-  const int r = qtr * 32 + lane;                           // query row / TMEM lane
-  const uint32_t lane_base = ((uint32_t)(qtr * 32)) << 16;
-  float* xch = reinterpret_cast<float*>(smem + kOffBias + 256 + 64);   // [2][128] exchange buffer (after bias + barriers)
+  const uint32_t sQ = base + kOffQ, sK = base + kOffK, sV = base + kOffV;
+  FlashWarp<DHP, 128, false> fw;
   const int ntiles = (op.Tk + AKT - 1) / AKT;
-
+  load_kv(0);
   for (int j = 0; j < ntiles; ++j) {
-    const uint32_t par = (uint32_t)(j & 1);
     store_kv(j * AKT);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    if (tid == 128) {
-      tc_fence_after();
-#pragma unroll
-      for (int k = 0; k < DHP / 16; ++k) {
-        const uint64_t qh = umma_desc(sQ + k * 32), ql = umma_desc(sQ + 16384 + k * 32);
-        const uint64_t kh = umma_desc(sK + k * 32), kl = umma_desc(sK + 8192 + k * 32);
-        umma_bf16(tS, qh, kh, idS, k != 0 ? 1u : 0u);
-        umma_bf16(tS, qh, kl, idS, 1u);
-        umma_bf16(tS, ql, kh, idS, 1u);
-      }
-      umma_commit(bar_s);
-    }
-    if (j + 1 < ntiles) load_kv((j + 1) * AKT);            // global loads overlap the MMA + softmax
-    mbar_wait(bar_s, par);
-    tc_fence_after();
-    float sv[32];
-    tmem_ld32(tS + lane_base + hf * 32, sv);
-    float mt = -INFINITY;
-#pragma unroll
-    for (int c = 0; c < 32; ++c) { sv[c] += bias_s[hf * 32 + c]; mt = fmaxf(mt, sv[c]); }
-    xch[hf * 128 + r] = mt;
-    asm volatile("bar.sync %0, 64;" ::"r"(1 + qtr) : "memory");          // the two warps of this lane quarter
-    const float m_new = fmaxf(m_run, fmaxf(mt, xch[(hf ^ 1) * 128 + r]));
-    const float corr = exp2f(m_run - m_new);
-    float lt = 0.f;
-#pragma unroll
-    for (int c = 0; c < 32; ++c) { sv[c] = exp2f(sv[c] - m_new); lt += sv[c]; }
-#pragma unroll
-    for (int c8 = 0; c8 < 4; ++c8) {
-      uint4 hi, lo;
-      split8(sv + 8 * c8, hi, lo);
-      const int ck = hf * 4 + c8;
-      const int off = r * 128 + ((ck ^ (r & 7)) << 4);
-      *reinterpret_cast<uint4*>(smem + kOffP + off) = hi;
-      *reinterpret_cast<uint4*>(smem + kOffP + 16384 + off) = lo;
-    }
-    l_run = l_run * corr + lt;
-    m_run = m_new;
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    if (tid == 128) {
-      tc_fence_after();
-#pragma unroll
-      for (int k = 0; k < AKT / 16; ++k) {
-        const uint64_t ph = umma_desc(sP + k * 32), pl = umma_desc(sP + 16384 + k * 32);
-        const uint64_t vh = umma_desc(sV + k * 32), vl = umma_desc(sV + 8192 + k * 32);
-        umma_bf16(tO, ph, vh, idO, k != 0 ? 1u : 0u);
-        umma_bf16(tO, ph, vl, idO, 1u);
-        umma_bf16(tO, pl, vh, idO, 1u);
-      }
-      umma_commit(bar_o);
-    }
-    mbar_wait(bar_o, par);                                 // every thread: K / V^T / P smem is free again
-    tc_fence_after();
-    {
-      float ot[8];
-#pragma unroll
-      for (int d0 = 0; d0 < OH; d0 += 8) {
-        tmem_ld8(tO + lane_base + hf * OH + d0, ot);
-#pragma unroll
-        for (int d = 0; d < 8; ++d) o[d0 + d] = o[d0 + d] * corr + ot[d];
-      }
-    }
+    __syncthreads();                                       // Q (first tile), K, V and the bias row are in shared memory
+    if (j == 0) fw.load_q(sQ, sQ + 16384, 16 * warp, lane);
+    if (j + 1 < ntiles) load_kv((j + 1) * AKT);            // global loads overlap the MMAs + softmax
+    fw.tile(sK, sK + 8192, sV, sV + 8192, bias_s, 1.0f, AKT, lane);
+    __syncthreads();                                       // every warp is done with K / V before the next store
   }
-
-  // total row sum = the two halves' partial sums
-  xch[hf * 128 + r] = l_run;
-  asm volatile("bar.sync %0, 64;" ::"r"(1 + qtr) : "memory");
-  const float l_tot = l_run + xch[(hf ^ 1) * 128 + r];
-  if (q0 + r < op.Tq) {
-    const float inv = 1.0f / l_tot;
-    const long long orow = (long long)b * op.Tq + q0 + r;
-    const int dbase = hf * OH;                              // first head-dim column of this thread
-    if (op.out) {
-      float* po = op.out + orow * op.out_ld + h * dh;
-      for (int d = 0; d < OH; ++d) if (dbase + d < dh) po[dbase + d] = o[d] * inv;
-    }
-    if (op.out_hi) {
-      __nv_bfloat16* ph = op.out_hi + orow * op.out_split_ld + h * dh + dbase;
-      __nv_bfloat16* pl = op.out_lo + orow * op.out_split_ld + h * dh + dbase;
-      if ((dh & 15) == 0 && ((op.out_split_ld | (h * dh)) & 7) == 0) {
-#pragma unroll
-        for (int d0 = 0; d0 < OH; d0 += 8) {
-          float v[8];
-#pragma unroll
-          for (int d = 0; d < 8; ++d) v[d] = o[d0 + d] * inv;
-          uint4 hi, lo;
-          split8(v, hi, lo);
-          *reinterpret_cast<uint4*>(ph + d0) = hi;
-          *reinterpret_cast<uint4*>(pl + d0) = lo;
-        }
-      } else {
-#pragma unroll
-        for (int d = 0; d < OH; ++d)
-          if (dbase + d < dh) {
-            const float v = o[d] * inv;
-            const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-            ph[d] = hi;
-            pl[d] = __float2bfloat16_rn(v - __bfloat162float(hi));
-          }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
+  fw.store(op, b, h, q0 + 16 * warp, lane);
   span_end(op.span);
-  if (warp == 4) tmem_dealloc(tmem_base, 128);
 }
 
 template <int DHP>

@@ -1,23 +1,13 @@
-// tcgen05 flash attention, v2 (product path): TMA-fed and warp-specialised.
+// Flash attention, v2 (product path): TMA-fed and warp-specialised, sm_90a.
 //   out = softmax(q k^T * dh^-0.5 + bias) v      (reference attention_processor.py:1025-1036)
 //
 // CTA = 128 queries of one (batch, head); key tiles of 64; 288 threads:
-//   warp 0      one elected thread (elect.sync) is TMA producer and MMA issuer at once.  Producer: Q once, then a ring of
-//               {K_hi, K_lo, V_hi, V_lo} tiles.  q / k / v are the bf16 hi/lo "split" tensors the projection GEMMs'
-//               epilogues wrote (token-major), so a tile is a plain 3-D box {head channels, 64 keys, 1 batch} - no
-//               conversion, no transpose.  MMA issuer: S[128x64] = Q K^T (A, B K-major) and O_tile[128xdh] = P V with V
-//               as an MN-major B operand (dh contiguous, keys = MMA K dimension), each as 3 bf16 MMAs over the hi/lo
-//               splits, fp32 accumulators in TMEM.  x_hi*[y_hi ; y_lo] is one instruction of twice the N (two TMEM column
-//               groups), x_lo*y_hi a second one: 2 MMAs per k-step instead of 3.  The ring stage of tile j-1 is refilled
-//               right before PV(j) is issued (PV(j-1) has retired by then: the softmax warps waited for it).
-//   warps 1-8   online softmax, two threads per query row (32 score columns and dh/2 output columns
-//               each): exp2 with scale*log2(e) folded into one FFMA, P written as a SWIZZLE_128B A operand.
-// The roles only meet through mbarriers: S(j+1) is issued as soon as the softmax warps have
-// pulled S(j) out of TMEM, and P(j) V(j) runs under softmax(j+1), so neither MMA latency nor a
-// CTA-wide barrier sits on the per-tile critical path.
-// Shared-memory rows of the Q/K/V tiles are `PB` bytes wide (32/64/128 = the TMA box width and the
-// UMMA swizzle mode), so a dh=16 head moves 32 B per key instead of a padded 128 B row.
-#include "gemm_common.cuh"
+//   warp 0      one elected thread is the TMA producer: Q once, then a ring of {K_hi, K_lo, V_hi, V_lo} tiles, plain 3-D
+//               boxes of the hi/lo "split" tensors the projection GEMMs wrote (no conversion, no transpose).
+//   warps 1-8   16 query rows each (flash_mma.cuh); a warp hands a ring stage back as soon as it is done with it.
+// Shared-memory rows of the Q/K/V tiles are `PB` bytes wide (32/64/128 = the TMA box width and swizzle mode), so a dh=16
+// head moves 32 B per key instead of a padded 128 B row.
+#include "flash_mma.cuh"
 #include "tc_common.cuh"
 #include "launch.cuh"
 #include <math.h>
@@ -28,63 +18,23 @@ namespace ns2vc {
 namespace {
 
 constexpr int kQ = 128, kKeys = 64;
-constexpr int kThreadsV2 = 288;                          // warp 0: TMA producer + MMA issuer (one elected thread); warps 1-8: softmax
+constexpr int kThreadsV2 = 288;                          // warp 0: TMA producer (one elected thread); warps 1-8: 16 query rows each
 
 template <int DHP, int PB, bool PF16, bool BIAS> struct ACfg {
   static constexpr int NST = (PB == 128) ? 2 : 3;
   static constexpr int kQBytes = kQ * PB;            // Q hi (lo follows)
   static constexpr int kTBytes = kKeys * PB;         // one K or V tile (hi or lo)
   static constexpr int kStageBytes = 4 * kTBytes;    // K_hi | K_lo | V_hi | V_lo
-  static constexpr int kPBytes = kQ * 128;           // P [128 x 64] 16-bit: fp16 (PF16), or bf16 hi with lo following
   static constexpr int kOffQ = 0;
-  static constexpr int kOffP = 2 * kQBytes;
-  static constexpr int kOffKV = kOffP + (PF16 ? 1 : 2) * kPBytes;
+  static constexpr int kOffKV = 2 * kQBytes;
   static constexpr int kOffBar = kOffKV + NST * kStageBytes;
-  static constexpr int kOffXch = kOffBar + 256;      // [3: parity 0 / parity 1 / row sums][2 halves][128 rows] floats
-  static constexpr int kOffBias = kOffXch + 3072;    // additive bias * log2(e) (or -inf past Tk) for up to kBiasKeys keys
-  static constexpr int kBiasKeys = (PB == 32) ? 768 : 1024;   // d_h = 16: 3 KB so that the biased (cross-attention) variant also fits 4 CTAs / SM
+  static constexpr int kOffBias = kOffBar + 256;     // additive bias * log2(e) (or -inf past Tk) for up to kBiasKeys keys
+  static constexpr int kBiasKeys = (PB == 32) ? 768 : 1024;
   static constexpr int kSmem = kOffBias + (BIAS ? 4 * kBiasKeys : 0) + 1024 /*alignment slack*/;
-  static constexpr int NO = PB / 2;                  // channels per V tile row = width of one O column group
-  // TMEM: S = x_hi*[y_hi ; y_lo] lands in two column groups when the K tiles are issued as one N = 128 operand (SC);
-  // for 32-byte head rows (dh = 16) S stays three plain N = 64 MMAs so that 128 columns (-> 3 CTAs / SM) suffice.
-  static constexpr bool SC = (PB != 32);
-  static constexpr int kSCols = SC ? 128 : 64;
-  static constexpr int kOCols = 2 * NO;              // one O buffer: [0,NO) hi*hi + lo*hi, [NO,2NO) hi*lo
-  static constexpr int kTmemCols = (kSCols + 2 * kOCols <= 128) ? 128 : (kSCols + 2 * kOCols <= 256) ? 256 : 512;
-  static constexpr int kBySmem = (kSmem <= 56 * 1024) ? 4 : (kSmem <= 74 * 1024) ? 3 : (kSmem <= 113 * 1024) ? 2 : 1;
-  static constexpr int kMinCtas = (512 / kTmemCols < kBySmem) ? 512 / kTmemCols : kBySmem;
+  // The scores, output and Q fragments of a warp's 16 rows live in registers.  128-byte rows (d_h 48 / 64) need ~150-170 per
+  // thread: one CTA per SM without spills measured faster than two with spills (H100, 741 vs 837 us of attention per forward).
+  static constexpr int kMinCtas = (PB == 128) ? 1 : (kSmem <= 113 * 1024) ? 2 : 1;
 };
-
-// Shared-memory matrix descriptor for a tile whose rows are PB bytes (SWIZZLE_<PB>B), 8-row groups dense.
-template <int PB>
-__device__ __forceinline__ uint64_t desc_pb(uint32_t saddr, uint32_t lbo_bytes) {
-  constexpr uint64_t layout = (PB == 32) ? 6 : (PB == 64) ? 4 : 2;
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)((8 * PB) >> 4) << 32) |
-         (1ull << 46) | (layout << 61);
-}
-
-__device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-
-template <int N>
-__device__ __forceinline__ void tmem_ld_nw(uint32_t taddr, float* v);
-template <>
-__device__ __forceinline__ void tmem_ld_nw<8>(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ long long clk() { long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)); return t; }
-// Per-tile role timeline of CTA (0,0,0) (scripts/trace_attn.py): compiled in only with -DNS2VC_ATTN_TRACE (NVCC_EXTRA of build.sh) -
-// eight predicated stamps per key tile are ~7 % of the softmax loop's issue slots and a live pointer in a 56-register kernel.
-#ifdef NS2VC_ATTN_TRACE
-#define ATRACE(j, slot) do { if (tr && (j) < 16) tr[(j) * 16 + (slot)] = clk(); } while (0)
-#else
-#define ATRACE(j, slot) do { } while (0)
-#endif
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 template <int DHP, int PB, bool BIAS, bool PF16>
 __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCtas) attn_v2_kernel(const __grid_constant__ AttnOp op) {
@@ -95,10 +45,9 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - raw);
   const uint32_t bar0 = base + C::kOffBar;
-  const uint32_t q_full = bar0, s_full = bar0 + 8, s_empty = bar0 + 16, p_full = bar0 + 24, o_full = bar0 + 32;
-  auto kv_full = [&](int s) { return bar0 + 40u + 8u * s; };
-  auto kv_empty = [&](int s) { return bar0 + 40u + 8u * (NST + s); };
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + C::kOffBar + 40 + 16 * NST);
+  const uint32_t q_full = bar0;
+  auto kv_full = [&](int s) { return bar0 + 8u + 8u * s; };
+  auto kv_empty = [&](int s) { return bar0 + 8u + 8u * (NST + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * kQ;
@@ -113,30 +62,19 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
     op.trace[256 + 3 * cta_lin] = gtime_ns();
     op.trace[256 + 3 * cta_lin + 2] = smid;
   }
-#ifdef NS2VC_ATTN_TRACE
-  unsigned long long* tr = (op.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (warp == 0 || (warp == 1 && lane == 0))) ? op.trace : nullptr;
-#endif
   if (tid == 0) {
-    mbar_init(q_full, 1); mbar_init(s_full, 1); mbar_init(s_empty, 256); mbar_init(p_full, 256); mbar_init(o_full, 1);
-    for (int s = 0; s < NST; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); }
+    mbar_init(q_full, 1);
+    for (int s = 0; s < NST; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 8); }
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32((const void*)tmem_slot), C::kTmemCols);
   if (warp == 0 && lane == 0) {
 #pragma unroll
     for (int i = 0; i < 6; ++i) prefetch_tmap(&op.tm[i]);
   }
   pdl_trigger();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tO = tmem_base + C::kSCols;   // O: two buffers of kOCols columns (tile parity)
-  const uint32_t sQ = base + C::kOffQ, sP = base + C::kOffP, sKV = base + C::kOffKV;
+  const uint32_t sQ = base + C::kOffQ, sKV = base + C::kOffKV;
 
-  // Warp 0: ONE elected thread streams the tiles AND issues the MMAs (eight softmax warps + this one = 288 threads, so that
-  // four CTAs fit an SM).  Under elect.sync ptxas issues the uniform-datapath instructions (UTMALDG, UTCHMMA, UTCBAR) back to
-  // back; as two divergent lanes of one warp each of them sat in an ELECT / BRA.U.ANY serialisation loop.
   if (warp == 0) {
     if (elect_one()) {
       auto load_kv = [&](int j) {
@@ -152,84 +90,13 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
       mbar_arrive_expect_tx(q_full, 2u * C::kQBytes);
       tma_load_3d(sQ, &op.tm[0], op.q_c0 + h * dh, q0, b, q_full);
       tma_load_3d(sQ + C::kQBytes, &op.tm[1], op.q_c0 + h * dh, q0, b, q_full);
-      for (int j = 0; j < NST && j < ntiles; ++j) { ATRACE(j, 12); load_kv(j); }
-      // Every product is hi*hi + hi*lo + lo*hi.  The hi and lo tiles of K (and of V) are adjacent in shared memory,
-      // so X_hi x [Y_hi ; Y_lo] is ONE instruction of twice the N whose result lands in two TMEM column groups;
-      // X_lo x Y_hi accumulates into the first group and the softmax warps add the groups.
-      constexpr uint32_t idS2 = umma_idesc_bf16(kQ, 2 * kKeys), idS1 = umma_idesc_bf16(kQ, kKeys);                    // A, B K-major
-      constexpr uint32_t idO2 = umma_idesc_bf16(kQ, 2 * C::NO) | (1u << 16), idO1 = umma_idesc_bf16(kQ, C::NO) | (1u << 16);   // B (= V) MN-major
-      auto issue_S = [&](int j) {
-        const uint32_t kst = sKV + (j % NST) * C::kStageBytes;
-#pragma unroll
-        for (int k = 0; k < DHP / 16; ++k) {
-          const uint64_t qh = desc_pb<PB>(sQ + k * 32, 16), ql = desc_pb<PB>(sQ + C::kQBytes + k * 32, 16);
-          const uint64_t kh = desc_pb<PB>(kst + k * 32, 16);                   // rows [0,64) = K_hi, rows [64,128) = K_lo
-          if (C::SC) {
-            umma_bf16(tS, qh, kh, idS2, k != 0 ? 1u : 0u);
-            umma_bf16(tS, ql, kh, idS1, 1u);
-          } else {
-            const uint64_t kl = desc_pb<PB>(kst + C::kTBytes + k * 32, 16);
-            umma_bf16(tS, qh, kh, idS1, k != 0 ? 1u : 0u);
-            umma_bf16(tS, qh, kl, idS1, 1u);
-            umma_bf16(tS, ql, kh, idS1, 1u);
-          }
-        }
-        umma_commit(s_full);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(kv_full(0), 0);
-      tc_fence_after();
-      issue_S(0);
-      // Refill of the ring stage tile j-1 occupied (with tile j-1+NST), once PV(j-1) has retired.  Three stages: after the
-      // wait for P(j) - the softmax warps waited for PV(j-1) before they stored P(j), so the stage is free without waiting.
-      // Two stages (128-byte head rows): tile j+1 itself goes there, so it is refilled first thing in iteration j.
-      auto refill = [&](int j) {
-        if (j >= 1 && j - 1 + NST < ntiles) {
-          mbar_wait(kv_empty((j - 1) % NST), (uint32_t)(((j - 1) / NST) & 1));
-          ATRACE(j - 1 + NST, 12);
-          load_kv(j - 1 + NST);
-        }
-      };
       for (int j = 0; j < ntiles; ++j) {
-        const uint32_t par = (uint32_t)(j & 1);
-        if (NST < 3) refill(j);
-        if (j + 1 < ntiles) {
-          mbar_wait(kv_full((j + 1) % NST), (uint32_t)(((j + 1) / NST) & 1));
-          mbar_wait(s_empty, par);                          // every softmax thread holds S(j) in registers
-          tc_fence_after();
-          ATRACE(j, 8);
-          issue_S(j + 1);
-          ATRACE(j, 9);
-        }
-        mbar_wait(p_full, par);                             // P(j) is in shared memory, O_tile(j-1) has been read
-        tc_fence_after();
-        ATRACE(j, 10);
-        if (NST >= 3) refill(j);
-        const uint32_t vst = sKV + (j % NST) * C::kStageBytes + 2 * C::kTBytes;
-#pragma unroll
-        for (int k = 0; k < kKeys / 16; ++k) {
-          const uint64_t ph = umma_desc(sP + k * 32);
-          const uint64_t vh = desc_pb<PB>(vst + k * 16 * PB, C::kTBytes);      // channel group 0 = V_hi, group 1 (+LBO) = V_lo
-          if (PF16) {
-            umma_bf16(tO + par * C::kOCols, ph, vh, idO2 & ~((7u << 7) | (7u << 10)), k != 0 ? 1u : 0u);   // A = fp16 P, B = fp16 [V_hi | V_lo] (format fields 0)
-          } else {
-            const uint64_t pl = umma_desc(sP + C::kPBytes + k * 32);
-            umma_bf16(tO + par * C::kOCols, ph, vh, idO2, k != 0 ? 1u : 0u);
-            umma_bf16(tO + par * C::kOCols, pl, vh, idO1, 1u);
-          }
-        }
-        umma_commit(o_full);
-        umma_commit(kv_empty(j % NST));                     // K(j), V(j) consumed
-        ATRACE(j, 11);
+        if (j >= NST) mbar_wait(kv_empty(j % NST), (uint32_t)(((j / NST) & 1) ^ 1));   // every warp is done with tile j - NST
+        load_kv(j);
       }
     }
   } else {
-    // ===================== softmax warps =====================
-    constexpr int OH = DHP / 2;                             // output columns per thread
-    const int qtr = warp & 3, hf = (warp - 1) >> 2;
-    const int r = qtr * 32 + lane;                          // query row = TMEM lane
-    const uint32_t lane_base = ((uint32_t)(qtr * 32)) << 16;
-    float* xch = reinterpret_cast<float*>(smem + C::kOffXch);
+    // ===================== attention warps =====================
     float* bias_s = reinterpret_cast<float*>(smem + C::kOffBias);
     const float qscale = op.scale * 1.4426950408889634f;
     pdl_wait();                                             // the mask bias and the output buffers belong to earlier kernels
@@ -237,168 +104,26 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
       const float* bias = op.bias + (long long)b * op.Tk;
       for (int i = tid - 32; i < ntiles * kKeys; i += 256)
         bias_s[i] = (i < op.Tk) ? __ldg(bias + i) * 1.4426950408889634f : -INFINITY;
-      asm volatile("bar.sync 5, 256;" ::: "memory");
+      asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    float o[OH];
-#pragma unroll
-    for (int d = 0; d < OH; ++d) o[d] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f;
-
-    auto add_o_tile = [&](uint32_t buf, float scale) {      // o = (o + O_tile[buf] (TMEM)) * scale
-      float ot[OH], ou[OH];
-      const uint32_t to = tO + buf * C::kOCols + lane_base + hf * OH;
-#pragma unroll
-      for (int d0 = 0; d0 < OH; d0 += 8) {
-        tmem_ld_nw<8>(to + d0, ot + d0);
-        tmem_ld_nw<8>(to + C::NO + d0, ou + d0);
-      }
-      tmem_wait_ld();
-      const unsigned long long s2 = pk2(scale, scale);
-#pragma unroll
-      for (int d = 0; d < OH; d += 2)
-        upk2(fmul2(fadd2(pk2(o[d], o[d + 1]), fadd2(pk2(ot[d], ot[d + 1]), pk2(ou[d], ou[d + 1]))), s2), o[d], o[d + 1]);
-    };
-
+    FlashWarp<DHP, PB, PF16> fw;
+    const int r0 = 16 * (warp - 1);
+    mbar_wait(q_full, 0);
+    fw.load_q(sQ, sQ + C::kQBytes, r0, lane);
     for (int j = 0; j < ntiles; ++j) {
-      const uint32_t par = (uint32_t)(j & 1);
-      ATRACE(j, 0);
-      mbar_wait_quiet(s_full, par);
-      tc_fence_after();
-      ATRACE(j, 1);
-      float sv[32];
-      if (C::SC) tmem_ld32_sum(tS + lane_base + hf * 32, tS + lane_base + kKeys + hf * 32, sv);
-      else tmem_ld32(tS + lane_base + hf * 32, sv);
-      tc_fence_before();
-      mbar_arrive(s_empty);
-      ATRACE(j, 2);
-      const int kbase = j * kKeys + hf * 32;
-      float mt = -INFINITY;
-      const unsigned long long qs2 = pk2(qscale, qscale);
-      if (BIAS) {
-        const float4* bp = reinterpret_cast<const float4*>(bias_s + kbase);
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          const float4 bb = bp[c4];
-          upk2(ffma2(pk2(sv[4 * c4 + 0], sv[4 * c4 + 1]), qs2, pk2(bb.x, bb.y)), sv[4 * c4 + 0], sv[4 * c4 + 1]);
-          upk2(ffma2(pk2(sv[4 * c4 + 2], sv[4 * c4 + 3]), qs2, pk2(bb.z, bb.w)), sv[4 * c4 + 2], sv[4 * c4 + 3]);
-        }
-#pragma unroll
-        for (int c = 0; c < 32; ++c) mt = fmaxf(mt, sv[c]);
-      } else {
-        if (j == ntiles - 1 && (op.Tk & (kKeys - 1))) {     // keys past Tk were zero-filled by TMA: mask them
-          const int nvalid = op.Tk - kbase;
-#pragma unroll
-          for (int c = 0; c < 32; ++c) if (c >= nvalid) sv[c] = -INFINITY;
-        }
-#pragma unroll
-        for (int c = 0; c < 32; ++c) mt = fmaxf(mt, sv[c]);
-        mt *= qscale;                                       // qscale > 0: max commutes with the scaling
-      }
-      xch[(par * 2 + hf) * 128 + r] = mt;
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + qtr) : "memory");          // the two warps of this lane quarter
-      ATRACE(j, 3);
-      const float m_new = fmaxf(m_run, fmaxf(mt, xch[(par * 2 + (hf ^ 1)) * 128 + r]));
-      const float corr = ex2f(m_run - m_new);
-      const unsigned long long nm2 = pk2(-m_new, -m_new);
-      unsigned long long lt2 = pk2(0.f, 0.f);
-      // PV(j-1) was issued as soon as P(j-1) was complete, i.e. before these warps even picked up S(j): by now it has
-      // retired (the P buffer is free, O_tile(j-1) complete).  Waiting for it HERE lets every 8-column group of P go to
-      // shared memory as soon as it is computed instead of staying live in registers across the wait (the kernel runs
-      // at 56 registers per thread for four CTAs per SM).
-      if (j > 0) {
-        mbar_wait_quiet(o_full, par ^ 1u);
-        tc_fence_after();
-      }
-      ATRACE(j, 5);
-#pragma unroll
-      for (int c8 = 0; c8 < 4; ++c8) {
-        uint32_t ph2[4];
-#pragma unroll
-        for (int c = 8 * c8; c < 8 * c8 + 8; c += 2) {
-          float a, bq;
-          if (BIAS) upk2(fadd2(pk2(sv[c], sv[c + 1]), nm2), a, bq);
-          else upk2(ffma2(pk2(sv[c], sv[c + 1]), qs2, nm2), a, bq);
-          sv[c] = ex2f(a); sv[c + 1] = ex2f(bq);
-          if (PF16) {                                       // the weights ARE the fp16-rounded values: numerator and row sum agree
-            const uint32_t h2 = pack_f16x2(sv[c], sv[c + 1]);
-            ph2[(c >> 1) & 3] = h2;
-            sv[c] = f16lo_to_f32(h2); sv[c + 1] = f16hi_to_f32(h2);
-          }
-          lt2 = fadd2(lt2, pk2(sv[c], sv[c + 1]));
-        }
-        const int ck = hf * 4 + c8;
-        const int off = r * 128 + ((ck ^ (r & 7)) << 4);
-        if (PF16) {
-          *reinterpret_cast<uint4*>(smem + C::kOffP + off) = make_uint4(ph2[0], ph2[1], ph2[2], ph2[3]);
-        } else {
-          uint4 hi, lo;
-          split8(sv + 8 * c8, hi, lo);
-          *reinterpret_cast<uint4*>(smem + C::kOffP + off) = hi;
-          *reinterpret_cast<uint4*>(smem + C::kOffP + C::kPBytes + off) = lo;
-        }
-      }
-      float lt, lt_hi;
-      upk2(lt2, lt, lt_hi);
-      lt += lt_hi;
-      l_run = l_run * corr + lt;
-      m_run = m_new;
-      ATRACE(j, 4);
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(p_full);
-      ATRACE(j, 6);
-      // O_tile(j-1) (the other TMEM buffer than the one PV(j) is about to fill) is relative to the previous running max
-      if (j > 0) add_o_tile(par ^ 1u, corr);
-      ATRACE(j, 7);
+      const int stage = j % NST;
+      mbar_wait_quiet(kv_full(stage), (uint32_t)((j / NST) & 1));
+      const uint32_t kst = sKV + stage * C::kStageBytes;
+      fw.tile(kst, kst + C::kTBytes, kst + 2 * C::kTBytes, kst + 3 * C::kTBytes, BIAS ? bias_s + j * kKeys : nullptr, qscale,
+              op.Tk - j * kKeys, lane);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(kv_empty(stage));
     }
-    mbar_wait_quiet(o_full, (uint32_t)((ntiles - 1) & 1));
-    tc_fence_after();
-    add_o_tile((uint32_t)((ntiles - 1) & 1), 1.0f);
-
-    // total row sum = the two halves' partial sums
-    xch[(4 + hf) * 128 + r] = l_run;
-    asm volatile("bar.sync %0, 64;" ::"r"(1 + qtr) : "memory");
-    const float l_tot = l_run + xch[(4 + (hf ^ 1)) * 128 + r];
-    if (q0 + r < op.Tq) {
-      const float inv = 1.0f / l_tot;
-      const long long orow = (long long)b * op.Tq + q0 + r;
-      const int dbase = hf * OH;
-      if (op.out) {
-        float* po = op.out + orow * op.out_ld + h * dh;
-#pragma unroll
-        for (int d = 0; d < OH; ++d) if (dbase + d < dh) po[dbase + d] = o[d] * inv;
-      }
-      if (op.out_hi) {
-        __nv_bfloat16* ph = op.out_hi + orow * op.out_split_ld + h * dh + dbase;
-        __nv_bfloat16* pl = op.out_lo + orow * op.out_split_ld + h * dh + dbase;
-        if (((op.out_split_ld | (h * dh)) & 7) == 0) {      // dh % 16 == 0 here, so dbase % 8 == 0
-#pragma unroll
-          for (int d0 = 0; d0 < OH; d0 += 8) {
-            float v[8];
-#pragma unroll
-            for (int d = 0; d < 8; ++d) v[d] = o[d0 + d] * inv;
-            uint4 hi, lo;
-            split8(v, hi, lo);
-            *reinterpret_cast<uint4*>(ph + d0) = hi;
-            *reinterpret_cast<uint4*>(pl + d0) = lo;
-          }
-        } else {
-#pragma unroll
-          for (int d = 0; d < OH; ++d) {
-            const float v = o[d] * inv;
-            const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-            ph[d] = hi;
-            pl[d] = __float2bfloat16_rn(v - __bfloat162float(hi));
-          }
-        }
-      }
-    }
+    fw.store(op, b, h, q0 + r0, lane);
   }
-  tc_fence_before();
   __syncthreads();
   span_end(op.span);
   if (op.trace && tid == 0 && cta_lin < 597) op.trace[256 + 3 * cta_lin + 1] = gtime_ns();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
 }
 
 template <int DHP, int PB, bool BIAS, bool PF16>

@@ -1,4 +1,4 @@
-// Shared declarations for the ns2vc_b200 denoiser engine (sm_100a only).
+// Shared declarations for the ns2vc_b200 denoiser engine (sm_90a only).
 //
 // Internal activation layout: TOKEN-MAJOR fp32 [B, T_l, C] ("rows" = B*T_l tokens, channels
 // contiguous).  The reference keeps [B, C, T] and permutes around every transformer block
@@ -40,7 +40,7 @@ const char* get_error();
 // "Split" activations: every GEMM A operand is stored as two bf16 tensors hi = bf16(x),
 // lo = bf16(x - hi), token-major [B, T, ld].  They are written ONCE by the op that produces or
 // normalises the activation (prep kernels below, or a GEMM/attention epilogue) and then read by
-// TMA straight into the swizzled shared-memory image the UMMA wants — for every conv tap and
+// TMA straight into the swizzled shared-memory image wgmma wants — for every conv tap and
 // every N tile — instead of re-running GroupNorm/SiLU in the GEMM's load path.
 // ---------------------------------------------------------------------------------------------
 struct SplitBuf {
@@ -82,7 +82,7 @@ struct alignas(16) PrepOp {      // (16-byte multiples: arrays of descriptors ar
   unsigned long long* span;               // diagnostics
 };
 
-// GEMM / implicit-conv operator (shared by the tcgen05 kernel and the SIMT debug kernel):
+// GEMM / implicit-conv operator (shared by the wgmma kernel and the SIMT debug kernel):
 //
 //   out[b, t, n] = epilogue( sum_seg sum_{c < 64*nkb} A_seg[b, t + tap, c0 + c] * W[kofs_seg + c, n] )
 //
@@ -112,7 +112,7 @@ enum EpiFlags : int {
   EPI_LNFOLD = 256,   // the A operand is the RAW input of a LayerNorm whose gamma is folded into the weights:
                       //   acc <- rstd_row * (acc - mean_row * ln_g[n]);  bias then carries beta.W + bias   (see engine.cu)
   EPI_ROWSTATS = 512, // accumulate per-row sum / sum-of-squares of the fp32 output (LayerNorm statistics for the consumer)
-  // condition encoders (pre_engine.cu; the ENC instantiation of the tcgen05 kernel):
+  // condition encoders (pre_engine.cu; the ENC instantiation of the wgmma kernel):
   EPI_RELU = 1024,    // max(v, 0) after bias / residual              (conv-FFN, reference operations.py:689)
   EPI_ROWMASK = 2048, // v *= rowmask[m] after everything else         (x * (1 - padding_mask), reference operations.py:813, 820)
 };

@@ -1234,7 +1234,7 @@ extern "C" {
 
 const char* ns2vc_last_error(void) { return ns2vc::get_error(); }
 
-const char* ns2vc_build_info(void) { return "ns2vc_b200 sm_100a tcgen05/3xBF16 engine, built " __DATE__ " " __TIME__; }
+const char* ns2vc_build_info(void) { return "ns2vc_b200 sm_90a wgmma/3xBF16 engine, built " __DATE__ " " __TIME__; }
 
 int ns2vc_down_length(int t) { return (t - 1) / 2 + 1; }
 

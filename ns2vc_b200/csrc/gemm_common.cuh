@@ -1,4 +1,4 @@
-// Device helpers shared by the tcgen05 GEMM, the SIMT debug GEMM and the prep kernels.
+// Device helpers shared by the wgmma GEMM, the SIMT debug GEMM and the prep kernels.
 #pragma once
 #include "common.cuh"
 
@@ -33,20 +33,20 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-// Packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 / FMUL2 retire two results per issue slot)
+// fp32 pairs packed in one 64-bit value.  sm_90 has no packed fp32x2 arithmetic: each helper is two scalar operations, which
+// the compiler sees through (the packing is a register-pair move).
 __device__ __forceinline__ unsigned long long pk2(float a, float b) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ void upk2(unsigned long long v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
 __device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+  float a0, a1, b0, b1, c0, c1; upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1); return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1)); }
 __device__ __forceinline__ unsigned long long fadd2(unsigned long long a, unsigned long long b) {
-  unsigned long long d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+  float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1); return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1)); }
 __device__ __forceinline__ unsigned long long fsub2(unsigned long long a, unsigned long long b) {
-  unsigned long long d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+  float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1); return pk2(__fsub_rn(a0, b0), __fsub_rn(a1, b1)); }
 __device__ __forceinline__ unsigned long long fmul2(unsigned long long a, unsigned long long b) {
-  unsigned long long d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+  float a0, a1, b0, b1; upk2(a, a0, a1); upk2(b, b0, b1); return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1)); }
 
 // (a, b) -> packed bf16 hi = rn(a), rn(b) and lo = rn(a - hi_a), rn(b - hi_b): x = hi + lo to ~2^-17 relative.
-// 5 instructions per pair, none on the XU pipe (F2FP pack, two unpack ops, FADD2, F2FP).
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
   hi = pack_bf16x2(a, b);
   const float ha = __uint_as_float(hi << 16), hb = __uint_as_float(hi & 0xffff0000u);
@@ -55,7 +55,7 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   lo = pack_bf16x2(la, lb);
 }
 
-// erf-GELU of two values at once on the packed fp32x2 pipes (same A&S 7.1.26 polynomial as gelu_erf_f)
+// erf-GELU of two values at once (same A&S 7.1.26 polynomial as gelu_erf_f)
 __device__ __forceinline__ unsigned long long gelu_erf2(unsigned long long v2) {
   float a, b;
   upk2(v2, a, b);
@@ -80,7 +80,7 @@ __device__ __forceinline__ unsigned long long gelu_erf2(unsigned long long v2) {
   return fmul2(fmul2(v2, pk2(0.5f, 0.5f)), one_plus);
 }
 
-// silu of a packed pair (FMUL2 / FADD2 / FMUL2 around the four MUFU ops: 3.5 issue slots per element instead of 5)
+// silu of a packed pair
 __device__ __forceinline__ unsigned long long silu2(unsigned long long y2) {
   float z0, z1, e0, e1, r0, r1, d0, d1;
   upk2(fmul2(y2, pk2(-1.4426950408889634f, -1.4426950408889634f)), z0, z1);

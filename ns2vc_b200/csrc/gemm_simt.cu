@@ -1,6 +1,6 @@
-// (1) Weight packing into the tcgen05 B-operand layout (+ optional fp32 copy for the debug GEMM).
+// (1) Weight packing into the wgmma B-operand layout (+ optional fp32 copy for the debug GEMM).
 // (2) SIMT fp32 GEMM over the same GemmOp descriptor.  DEBUG/TEST backend only: it is selected
-//     with NS2VC_GEMM_BACKEND=simt and exists so the tcgen05 kernel can be differentially
+//     with NS2VC_GEMM_BACKEND=simt and exists so the wgmma kernel can be differentially
 //     tested on the device; the product path is gemm_tc.cu.
 #include "gemm_common.cuh"
 
@@ -9,7 +9,7 @@ namespace ns2vc {
 // ---------------------------------------------------------------------------------------------
 // Packed B layout: for k-block kb (64 K-values) and packed column n:
 //     row (kb*Npad + n) is 128 bytes = 64 bf16 along K, whose 16-byte chunks are XOR-swizzled
-//     with (n & 7)  — exactly the shared-memory image of a K-major SWIZZLE_128B UMMA operand,
+//     with (n & 7)  — exactly the shared-memory image of a K-major SWIZZLE_128B wgmma operand,
 //     so one contiguous cp.async.bulk of BN*128 bytes loads a [BN x 64] tile.
 // w_hi = bf16(w), w_lo = bf16(w - float(w_hi))   (3xBF16 split: hi*hi + hi*lo + lo*hi).
 // ---------------------------------------------------------------------------------------------
@@ -51,7 +51,7 @@ int launch_pack_b(const PackSeg& ps, __nv_bfloat16* w_hi, __nv_bfloat16* w_lo, f
                   cudaStream_t st) {
   const long long total = (long long)ps.n_rows * ps.nkb * 64;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   pack_b_kernel<<<blocks, 256, 0, st>>>(ps, w_hi, w_lo, w_f32, Npad);
   cudaError_t e = cudaGetLastError();
@@ -62,7 +62,7 @@ int launch_pack_b(const PackSeg& ps, __nv_bfloat16* w_hi, __nv_bfloat16* w_lo, f
 // ---------------------------------------------------------------------------------------------
 // SIMT debug GEMM: 64x64 tile, BK=16, 256 threads x (4x4) accumulators (x2 for GEGLU).  Reads the
 // same split activations the TMA path reads (A = hi + lo) and the fp32 copy of the weights, so a
-// disagreement with gemm_tc isolates the TMA/UMMA/TMEM machinery.
+// disagreement with gemm_tc isolates the TMA / wgmma machinery.
 // ---------------------------------------------------------------------------------------------
 template <bool GEGLU>
 __global__ void __launch_bounds__(256) gemm_simt_kernel(const __grid_constant__ GemmOp op) {

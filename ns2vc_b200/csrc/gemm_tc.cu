@@ -1,19 +1,11 @@
-// tcgen05 implicit-GEMM kernel for every contraction of the denoiser step (k=3 convs, 1x1 convs,
-// linears), sm_100a.
+// wgmma implicit-GEMM kernel for every contraction of the denoiser step (k=3 convs, 1x1 convs,
+// linears), sm_90a.
 //
-//   D[128 x BN] (fp32, TMEM) += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi          (3xBF16 split)
-//
-// issued as TWO MMAs per 16-wide k-step: A_hi x [B_hi ; B_lo] (one N = 2*BN instruction: the hi and lo
-// weight tiles are adjacent in shared memory, its result lands in two TMEM column groups) and
-// A_lo x B_hi (N = BN, accumulating into the first group); the epilogue adds the two groups.  In a
-// long chain a tcgen05.mma (M = 128, K = 16, SS) costs max(~50, N/2) SM cycles - 114 per k-step at BN = 64 -
-// whether or not consecutive MMAs hit the same accumulator columns (scripts/micro/mma_rate.cu,
-// profiles/r02_mma_rate.txt): folding B_hi | B_lo into one N = 2*BN instruction is what keeps the count down.
+//   D[128 x BN] (fp32, registers) += A_hi*B_hi + A_lo*B_hi + A_hi*B_lo          (3xBF16 split)
 //
 // fp32-level parity with the reference (rtol 1e-3 / atol 1e-4) cannot be met by single-pass
 // bf16/tf32 MMAs (SURVEY.md Appendix D), so both operands are split x = hi + lo (bf16 each) and
-// three kind::f16 MMAs accumulate into the same TMEM tile (the lo*lo term, ~2^-16 relative, is
-// dropped).
+// three bf16 wgmmas accumulate into the same fp32 tile (the lo*lo term, ~2^-16 relative, is dropped).
 //
 // A operand: the pre-normalised "split" activations [B, T, C] (bf16 hi / lo), fetched by TMA
 // (cp.async.bulk.tensor.3d, SWIZZLE_128B) as {64 channels x 128 rows} boxes of ONE batch entry.
@@ -22,12 +14,11 @@
 // once.  Channel concats are just two tensor maps.
 // B operand: weights pre-packed as the swizzled smem image, one cp.async.bulk per hi/lo tile.
 //
-// Persistent CTAs (one per SM at most, 320 threads), each looping over its share of the output tiles:
-//   warp 0     TMA producer (one elected lane): 2-4 stage mbarrier ring running across tiles
-//   warp 1     MMA issuer (one elected lane): tcgen05.mma x8 per k-block into TMEM accumulator buffer (tile & 1)
-//   warps 2-9  epilogue of tile i while the main loop of tile i+1 runs: TMEM -> registers (tcgen05.ld 32x32b)
-//              -> bias / GEGLU / residual -> staged 32x32 chunks -> TMA bulk stores (fp32 token-major, 16-bit hi/lo
-//              split for the next GEMM / attention), or direct channel-major stores for the output head
+// One output tile per CTA, 384 threads:
+//   warp 0      TMA producer (one elected lane): 3-4 stage mbarrier ring
+//   warps 1-3   idle (they keep warps 4-11 aligned to warpgroups)
+//   warps 4-11  two warpgroups (tile rows [0, 64) / [64, 128)): wgmma into registers, parked in shared memory as a fp32 tile;
+//               the epilogue reads it one row per thread -> bias / GEGLU / residual -> TMA bulk stores (fp32, 16-bit hi/lo)
 #include "gemm_common.cuh"
 #include "prep_common.cuh"
 #include "tc_common.cuh"
@@ -41,7 +32,7 @@ namespace ns2vc {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int kEpiWarps = 8;                            // two per SMSP: the epilogue is issue-latency bound
-constexpr int kThreads = (2 + kEpiWarps) * 32;
+constexpr int kThreads = (4 + kEpiWarps) * 32;
 constexpr int kATileBytes = BM * BK * 2;                // 16 KB: one bf16 [128 x 64] A tile (hi or lo)
 
 constexpr int kMaxStages = 4;
@@ -69,20 +60,22 @@ template <int BN_> struct TileCfg {
   static constexpr int BN = BN_;
   static constexpr int kBTileBytes = BN_ * BK * 2;      // one bf16 [BN x 64] B tile (hi or lo)
   static constexpr int kStageBytes = 2 * kATileBytes + 2 * kBTileBytes;
-  // measured r01: 4/3 stages (1 CTA/SM) beat 2 stages (2 CTAs/SM, co-resident with other lanes' kernels): 4.98 vs 5.74 ms/forward
-  static constexpr int kStagesSingle = (BN_ == 128) ? 3 : 4;   // a CTA with one tile: the epilogue stages its output in the idle stage buffers
-  static constexpr int kStagesMulti = (BN_ == 128) ? 2 : 3;    // a CTA with several tiles: dedicated staging area after the stages
-  static constexpr int kOffStagingMulti = kStagesMulti * kStageBytes;
-  static constexpr int kPipeBytes = (kStagesSingle * kStageBytes > kOffStagingMulti + kStagingBytes) ? kStagesSingle * kStageBytes : kOffStagingMulti + kStagingBytes;
+  // once the main loop is done the epilogue uses the idle stage buffers: staging area, then the parked accumulator tile
+  static constexpr int kStagesSingle = (BN_ == 128) ? 3 : 4;
+  static constexpr int kOffAcc = kStagingBytes;
+  static constexpr int kPipeBytes = (kStagesSingle * kStageBytes > kXOffAff + kXAffBytes) ? kStagesSingle * kStageBytes : kXOffAff + kXAffBytes;
   static constexpr int kOffBar = kPipeBytes;
   static constexpr int kOffDesc = kOffBar + 1024;
   static constexpr int kOffLnG = kOffDesc + 3072;         // [8 warps][4][32] floats: folded-LayerNorm g and bias vectors of the warp's chunk
   static constexpr int kSmemBytes = kOffLnG + 4096 + 1024 /*alignment slack*/;
-  static constexpr uint32_t kIdesc = umma_idesc_bf16(BM, BN_);
-  static constexpr uint32_t kIdesc2 = umma_idesc_bf16(BM, 2 * BN_);
 };
 static_assert(TileCfg<64>::kSmemBytes <= 227 * 1024 && TileCfg<128>::kSmemBytes <= 227 * 1024, "shared memory budget");
 static_assert(kXOffAff + kXAffBytes <= TileCfg<64>::kPipeBytes && kPrepSlots * kEpiWarps * 32 >= kXfMaxC, "panel mode: stages + affine table inside the pipeline area");
+// panel mode: the accumulator is parked in the weight ring, behind the area a split-K partner writes its partial tile into
+constexpr int kXOffAcc = kXOffB + 8 * 256 * 16;
+static_assert(kXOffAcc + BM * 64 * 4 <= kXOffAff, "panel mode: parked accumulator inside the weight ring");
+static_assert(TileCfg<64>::kOffAcc + BM * 64 * 4 <= TileCfg<64>::kStagesSingle * TileCfg<64>::kStageBytes &&
+              TileCfg<128>::kOffAcc + BM * 128 * 4 <= TileCfg<128>::kStagesSingle * TileCfg<128>::kStageBytes, "parked accumulator inside the stage buffers");
 
 
 __device__ __forceinline__ float* stage_f32_ptr(uint8_t* st, int row, int c4) {      // 16-byte group c4 (0..7) of row
@@ -183,18 +176,18 @@ __device__ __forceinline__ void emit_chunk(const GemmOp& op, const TMap* tmo, ui
 
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 // panel-mode stamps of the first transform thread of CTA 0: slots 16.. of the 32-slot trace record
-#define XTRACE(i) do { if (op_param.trace && blockIdx.x == 0 && tid == 64) op_param.trace[16 + (i)] = gtime(); } while (0)
+#define XTRACE(i) do { if (op_param.trace && blockIdx.x == 0 && tid == 128) op_param.trace[16 + (i)] = gtime(); } while (0)
 #define TRACE(i) do { if (op.trace && blockIdx.x == 0 && blockIdx.y == 0) op.trace[i] = gtime(); } while (0)
-// epilogue sub-steps of warp 2 / lane 0 of CTA (0,0), SM clock: slots 8..15 of the 16-slot trace record
+// epilogue sub-steps of warp 4 / lane 0 of CTA (0,0), SM clock: slots 8..15 of the 16-slot trace record
 __device__ __forceinline__ long long gclk() { long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)); return t; }
-#define ETRACE(i) do { if (op.trace && blockIdx.x == 0 && blockIdx.y == 0 && warp == 2 && lane == 0) op.trace[8 + (i)] = gclk(); } while (0)
+#define ETRACE(i) do { if (op.trace && blockIdx.x == 0 && blockIdx.y == 0 && warp == 4 && lane == 0) op.trace[8 + (i)] = gclk(); } while (0)
 
 // only the fields in front of the tensor maps are copied to shared memory (the maps are used by address)
 constexpr int kGemmOpHotBytes = (int)offsetof(GemmOp, tmap);
 static_assert(kGemmOpHotBytes % 16 == 0 && kGemmOpHotBytes <= 2688 && sizeof(PrepOp) <= 320, "GemmOp's hot part must fit the shared-memory descriptor copy");
 
 // LNF: instantiation for the consumers of a folded LayerNorm (EPI_LNFOLD); the other GEMMs run the LNF = false code, which
-// keeps the epilogue free of the extra live values (the epilogue is register-bound: 168 per thread at 320 threads).
+// keeps the epilogue free of the extra live values (the epilogue is register-bound).
 // XF: instantiation with the panel-mode paths (GroupNorm of the A operand applied in shared memory; BN = 64, one tile per CTA)
 // ENC: instantiation for the condition encoders (pre_engine.cu): ReLU and the per-row keep mask in the epilogue (EPI_RELU /
 // EPI_ROWMASK); the denoiser's instantiations do not carry that code
@@ -203,7 +196,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   using Cfg = TileCfg<BN_>;
   constexpr int BN = Cfg::BN;
   constexpr int kStageBytes = Cfg::kStageBytes;
-  constexpr int kAccCols = 2 * BN;                          // one accumulator buffer: [0,BN) hi*hi + lo*hi, [BN,2BN) hi*lo
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;             // SWIZZLE_128B atoms need 1024 B alignment
@@ -211,11 +203,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   const uint32_t bar_base = base + Cfg::kOffBar;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kMaxStages + s); };
-  auto acc_full = [&](int a) { return bar_base + 8u * (2 * kMaxStages + a); };
-  auto acc_empty = [&](int a) { return bar_base + 8u * (2 * kMaxStages + 2 + a); };
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + Cfg::kOffBar + 8 * (2 * kMaxStages + 4));
-  // panel mode: A ring = full_bar / empty_bar (0..2) + a_ready (normalised by the 8 epilogue warps); weight ring of its own
-  auto a_ready = [&](int s) { return bar_base + 8u * (16 + s); };
+  // panel mode: A ring = full_bar / empty_bar (0..2); weight ring of its own
   auto b_full = [&](int s) { return bar_base + 8u * (19 + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (21 + s); };
 
@@ -238,20 +226,26 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   }
   const GemmOp& op = *reinterpret_cast<const GemmOp*>(smem + Cfg::kOffDesc);
   const TMap* tmaps = op_param.tmap;
-  // Persistent tile loop: this CTA owns tiles blockIdx.x, blockIdx.x + gridDim.x, ...  (tile = m_tile * n_tiles + n_tile).
-  // A CTA with a single tile keeps all kMaxStages pipeline stages and stages its epilogue output in the (then idle)
-  // stage buffers; a CTA with several tiles gives the last stage(s) up for a dedicated staging area, so that the
-  // epilogue of tile i (TMEM accumulator buffer i & 1) runs under the main loop of tile i + 1.
+  // One tile per CTA (tile = m_tile * n_tiles + n_tile; launch_bn's grid is the tile count): the epilogue stages its output
+  // and parks the accumulator in the stage buffers, which only a CTA without a next tile may do.
   const int tiles_per_batch = (op_param.T_out + BM - 1) / BM;
   const int n_tiles = op_param.N / BN;
-  const int total_tiles = op_param.B * tiles_per_batch * n_tiles;
   // split-K (panel mode only): the `ks` CTAs of a cluster share one tile; kr = this CTA's share of the channel blocks
   const int ks = (XF && op_param.xmode && op_param.ksplit > 1) ? op_param.ksplit : 1;
-  const int kr = (int)blockIdx.x % ks, bid = (int)blockIdx.x / ks, nblk = (int)gridDim.x / ks;
-  const int my_tiles = (total_tiles - bid + nblk - 1) / nblk;
-  const bool multi = my_tiles > 1;
-  const int nst = multi ? Cfg::kStagesMulti : Cfg::kStagesSingle;   // pipeline depth actually used
-  uint8_t* stage_area = smem + (multi ? Cfg::kOffStagingMulti : 0);
+  const int kr = (int)blockIdx.x % ks, bid = (int)blockIdx.x / ks;
+  const int nst = Cfg::kStagesSingle;
+  uint8_t* stage_area = smem;
+  float* acc_tile = reinterpret_cast<float*>(smem + (XF ? kXOffAcc : Cfg::kOffAcc));
+  const int wg = (warp - 4) >> 2;                           // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+  float acc_d[BN / 2];                                      // this thread's part of the warpgroup's m64 x BN accumulator
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc_d[i] = 0.f;
+  // one 16-wide k-step of the 3xBF16 product: A rows [64 wg, 64 wg + 64) at a_hi / a_lo, B rows [0, BN) at b_hi / b_lo
+  auto mma3 = [&](uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+    wgmma_bf16<BN>(acc_d, wg_desc(a_hi), wg_desc(b_hi));
+    wgmma_bf16<BN>(acc_d, wg_desc(a_lo), wg_desc(b_hi));
+    wgmma_bf16<BN>(acc_d, wg_desc(a_hi), wg_desc(b_lo));
+  };
   const int nkb = op_param.nkb_total;
   const bool tr0 = blockIdx.x == 0;
   auto xr_ready = [&]() { return bar_base + 8u * 23; };     // split-K: the first CTA's rings are idle, the partner may write
@@ -260,9 +254,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   span_begin(op_param.span);
 
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(acc_full(a), 1); mbar_init(acc_empty(a), kEpiWarps); }
-    if (XF) { mbar_init(xr_ready(), 1); mbar_init(xr_full(), kEpiWarps); for (int a = 0; a < kXAStages; ++a) mbar_init(a_ready(a), kEpiWarps); for (int a = 0; a < kXBStages; ++a) { mbar_init(b_full(a), 1); mbar_init(b_empty(a), 1); } }
+    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kEpiWarps); }
+    if (XF) { mbar_init(xr_ready(), 1); mbar_init(xr_full(), kEpiWarps); for (int a = 0; a < kXBStages; ++a) { mbar_init(b_full(a), 1); mbar_init(b_empty(a), kEpiWarps); } }
     mbar_fence_init();
   }
   if (warp == 0 && lane == 0) {
@@ -273,31 +266,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     if (op_param.tma_out & 2) { prefetch_tmap(&pm[1]); prefetch_tmap(&pm[2]); }
   }
   pdl_trigger();
-#ifdef NS2VC_TMEM_LATE
-  __syncthreads();                                          // descriptor copy + armed barriers: the TMA producer may go
-  // The tensor-memory allocation (~0.4 us) is needed by the MMA issuer and the epilogue only: it runs AFTER the CTA-wide barrier
-  // and is joined by warps 1-9 alone, so the producer's weight / activation loads are in flight while it completes.
-  uint32_t tmem_base = 0;
-  if (warp >= 1) {
-    if (warp == 2) tmem_alloc(smem_u32((const void*)tmem_slot), 2 * kAccCols);
-    tc_fence_before();
-    asm volatile("bar.sync 2, 288;" ::: "memory");
-    tc_fence_after();
-    tmem_base = *tmem_slot;
-  }
-#else
-  if (warp == 2) tmem_alloc(smem_u32((const void*)tmem_slot), 2 * kAccCols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-#endif
+  __syncthreads();                                          // descriptor copy + armed barriers
   if (tid == 0 && tr0) TRACE(1);
   if constexpr (XF) if (ks > 1) cluster_sync_all();          // split-K: the partner's mbarriers exist before anyone arrives on them remotely
 
   // ============================================================================================================
-  // Panel mode: one tile per CTA (grid == tile count).  warp 0: panels + weight tiles by TMA; warps 2-9: normalise
-  // each panel in place, then (below) the ordinary epilogue; warp 1: three row-shifted views of the panel per tap.
+  // Panel mode: one tile per CTA (grid == tile count).  warp 0: panels + weight tiles by TMA; warps 4-11: normalise
+  // each panel in place, issue the wgmmas over three row-shifted views of the panel per tap, then (below) the ordinary
+  // epilogue.
   // ============================================================================================================
   constexpr bool xpanel = XF;                               // the XF instantiation IS the panel mode (launch_gemm_tc): no plain main loop in it
   if constexpr (XF) {
@@ -344,39 +320,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
         }
       }
-    } else if (warp == 1) {
-      if (elect_one()) {
-        int it = 0, gp = 0;
-        for (int si = 0; si < op.nxs; ++si) {
-          const XSeg& xs = op.xs[si];
-          for (int cb = 0; cb < xs.ncb; ++cb, ++gp) {
-            if (gp < p_lo || gp >= p_hi) continue;
-            const int sa = it % kXAStages, sb = it % kXBStages;
-            mbar_wait(b_full(sb), (uint32_t)((it / kXBStages) & 1));
-            mbar_wait(a_ready(sa), (uint32_t)((it / kXAStages) & 1));
-            if (it == 0 && tr0) TRACE(3);
-            tc_fence_after();
-            const uint32_t a_hi = base + sa * kXAStageBytes, a_lo = a_hi + kPanelBytes, b0 = base + kXOffB + sb * kXBStageBytes;
-            for (int j = 0; j < xs.ntap; ++j) {            // tap j = panel rows [j, j + 128): start address + 128 B per row
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t dah = umma_desc(a_hi + j * 128 + k * 32), dal = umma_desc(a_lo + j * 128 + k * 32);
-                const uint64_t dbh = umma_desc(b0 + j * 2 * Cfg::kBTileBytes + k * 32);
-                umma_bf16(tmem_base, dah, dbh, Cfg::kIdesc2, (it | j | k) != 0 ? 1u : 0u);
-                umma_bf16(tmem_base, dal, dbh, Cfg::kIdesc, 1u);
-              }
-            }
-            umma_commit(empty_bar(sa));
-            umma_commit(b_empty(sb));
-            ++it;
-          }
-        }
-        umma_commit(acc_full(0));
-        if (tr0) TRACE(4);
-      }
-    } else {
-      // ---- transform warps (the epilogue warps; 256 threads) ----
-      const int xt = tid - 64;
+    } else if (warp >= 4) {
+      // ---- transform + MMA warps (the epilogue warps; 256 threads) ----
+      const int xt = tid - 128;
       float* aff = reinterpret_cast<float*>(smem + kXOffAff);
       const PrepOp& pr = *reinterpret_cast<const PrepOp*>(smem + Cfg::kOffDesc + 2688);
       const bool have_aff = op.pre != nullptr;
@@ -463,12 +409,26 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
             fence_proxy_async();
           }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(a_ready(sa));
+          asm volatile("bar.sync 1, 256;" ::: "memory");      // the whole panel is normalised
           if (it == 0) XTRACE(3);
+          const int sb = it % kXBStages;
+          mbar_wait(b_full(sb), (uint32_t)((it / kXBStages) & 1));
+          const uint32_t a_hi = base + sa * kXAStageBytes + wg * 64 * 128, a_lo = a_hi + kPanelBytes, b0 = base + kXOffB + sb * kXBStageBytes;
+          wgmma_fence();
+          for (int j = 0; j < xs.ntap; ++j) {              // tap j = panel rows [j, j + 128): start address + 128 B per row
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+              const uint32_t bh = b0 + j * 2 * Cfg::kBTileBytes + k * 32;
+              mma3(a_hi + j * 128 + k * 32, a_lo + j * 128 + k * 32, bh, bh + Cfg::kBTileBytes);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();                                   // the previous panel's wgmmas have retired: release its buffers
+          if (it > 0 && lane == 0) { mbar_arrive(empty_bar((it - 1) % kXAStages)); mbar_arrive(b_empty((it - 1) % kXBStages)); }
           ++it;
         }
       }
+      wgmma_wait<0>();
       XTRACE(4);
     }
   }
@@ -494,20 +454,18 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       const int npre = npf;
       pdl_wait();
       if (tr0) TRACE(2);
-      int g = 0;                                            // k-block counter across this CTA's tiles
-      for (int it = 0; it < my_tiles; ++it) {
-        const int tile = bid + it * nblk;
-        const int mt = tile / n_tiles, n0 = (tile % n_tiles) * BN;
+      {
+        const int mt = bid / n_tiles, n0 = (bid % n_tiles) * BN;
         const int b = mt / tiles_per_batch, t0 = (mt % tiles_per_batch) * BM;
         int si = 0, kbl = 0;
-        for (int kb = 0; kb < nkb; ++kb, ++g) {
-          const int stage = g % nst;
+        for (int kb = 0; kb < nkb; ++kb) {
+          const int stage = kb % nst;
           const GSeg& s = op.seg[si];
           const uint32_t a_hi = base + stage * kStageBytes;
           const uint32_t a_lo = a_hi + kATileBytes;
           const uint32_t b_hi = a_lo + kATileBytes;
-          if (g >= npre) {
-            if (g >= nst) mbar_wait(empty_bar(stage), (uint32_t)(((g / nst) & 1) ^ 1));
+          if (kb >= npre) {
+            if (kb >= nst) mbar_wait(empty_bar(stage), (uint32_t)(((kb / nst) & 1) ^ 1));
             mbar_arrive_expect_tx(full_bar(stage), 2u * kATileBytes + 2u * Cfg::kBTileBytes);
             const size_t eoff = ((size_t)kb * op.N + n0) * 64;
             bulk_g2s(b_hi, op.w_hi + eoff, Cfg::kBTileBytes, full_bar(stage));
@@ -520,63 +478,58 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if constexpr (!xpanel) if (elect_one()) {
-      int g = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        const uint32_t acc = tmem_base + (uint32_t)((it & 1) * kAccCols);
-        if (it >= 2) { mbar_wait(acc_empty(it & 1), (uint32_t)(((it >> 1) & 1) ^ 1)); tc_fence_after(); }   // epilogue of tile it-2 has drained this buffer
-        for (int kb = 0; kb < nkb; ++kb, ++g) {
-          const int stage = g % nst;
-          mbar_wait(full_bar(stage), (uint32_t)((g / nst) & 1));
-          if (g == 0 && tr0) TRACE(3);
-          tc_fence_after();
-          const uint32_t a_hi = base + stage * kStageBytes;
-          const uint32_t a_lo = a_hi + kATileBytes;
-          const uint32_t b_hi = a_lo + kATileBytes;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t dah = umma_desc(a_hi + k * 32), dal = umma_desc(a_lo + k * 32);
-            const uint64_t dbh = umma_desc(b_hi + k * 32);   // rows [0, BN) = B_hi tile, rows [BN, 2BN) = B_lo tile (adjacent)
-            umma_bf16(acc, dah, dbh, Cfg::kIdesc2, (kb | k) != 0 ? 1u : 0u);
-            umma_bf16(acc, dal, dbh, Cfg::kIdesc, 1u);
-          }
-          umma_commit(empty_bar(stage));                     // frees this smem stage when the MMAs retire
-        }
-        umma_commit(acc_full(it & 1));                       // accumulator complete -> epilogue
-        if (it == 0 && tr0) TRACE(4);
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
+  } else if (warp >= 4) {
+    // ===================== main loop + epilogue (warps 4..11) =====================
     pdl_wait();                                             // residual reads / output writes follow the previous kernel
     __syncwarp();
     const bool leader = elect_one();                        // this warp's bulk-store thread (issues, commits and waits for its groups)
-    const int q = warp & 3;                                 // TMEM lane quarter this warp may access
+    const int q = warp & 3;                                 // row quarter of the tile this warp's epilogue handles
     const int r = q * 32 + lane;
-    const int cc0 = (warp - 2) >> 2;
-    uint8_t* st = stage_area + kStageOff + (warp - 2) * kStagePerWarp;   // this warp's staging area
+    const int cc0 = (warp - 4) >> 2;
+    uint8_t* st = stage_area + kStageOff + (warp - 4) * kStagePerWarp;   // this warp's staging area
     const TMap* tmo = op_param.tmap_out;
     bool staged_once = false;
-    for (int it = 0; it < my_tiles; ++it) {
-      const int tile = bid + it * nblk;
-      const int mt = tile / n_tiles, nt = tile % n_tiles, n0 = nt * BN;
+    {
+      constexpr int it = 0;                                 // the CTA's only tile (tile-parity indexing below)
+      const int mt = bid / n_tiles, nt = bid % n_tiles, n0 = nt * BN;
       const int b = mt / tiles_per_batch, t0 = (mt % tiles_per_batch) * BM;
       const int t = t0 + r;
       const bool mv = t < op.T_out;
       const long long m = (long long)b * op.T_out + t;
-      const uint32_t trow = tmem_base + (uint32_t)((it & 1) * kAccCols) + ((uint32_t)(q * 32) << 16);
+      if constexpr (!xpanel) {
+        for (int kb = 0; kb < nkb; ++kb) {
+          const int stage = kb % nst;
+          mbar_wait(full_bar(stage), (uint32_t)((kb / nst) & 1));
+          if (kb == 0 && tr0 && warp == 4 && lane == 0) TRACE(3);
+          const uint32_t a_hi = base + stage * kStageBytes + wg * 64 * 128;
+          const uint32_t a_lo = a_hi + kATileBytes;
+          const uint32_t b_hi = base + stage * kStageBytes + 2 * kATileBytes;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) mma3(a_hi + k * 32, a_lo + k * 32, b_hi + k * 32, b_hi + Cfg::kBTileBytes + k * 32);
+          wgmma_commit();
+          wgmma_wait<1>();                                   // the previous k-block's wgmmas have retired: release its stage
+          if (kb > 0 && lane == 0) mbar_arrive(empty_bar((kb - 1) % nst));
+        }
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(empty_bar((nkb - 1) % nst));
+        if (it == 0 && tr0 && warp == 4 && lane == 0) TRACE(4);
+      }
+      // once every wgmma of BOTH warpgroups has retired the stage buffers are idle: park the accumulator there
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      acc_park<BN>(acc_tile, acc_d, wg, tid & 127);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc_d[i] = 0.f;
+      asm volatile("bar.sync 1, 256;" ::: "memory");
       const int t_warp0 = t0 + q * 32;                      // first row of this warp's 32-row slab
-      // While the main loop runs these warps have nothing to do: fetch this thread's bias and residual values for
-      // its first 32-column chunk into registers now, so no global-load latency is left on the epilogue's critical path.
+      // bias and residual values of this thread's first 32-column chunk
       float pre[32];                                        // bias + residual of chunk cc0 (plain path); GEGLU: value bias
       float preg[32];                                       // GEGLU: gate bias
       bool pre_ok = false;
       // folded LayerNorm: this row's mean / rstd (sums accumulated by the producer's epilogue) and the g vectors of the
       // warp's first chunk (shared by all rows: parked in shared memory, one column per lane)
       float ln_mu = 0.f, ln_rstd = 1.f;
-      float* sg = reinterpret_cast<float*>(smem + Cfg::kOffLnG) + (warp - 2) * 128;   // g (value | gate) | folded bias (value | gate)
+      float* sg = reinterpret_cast<float*>(smem + Cfg::kOffLnG) + (warp - 4) * 128;   // g (value | gate) | folded bias (value | gate)
       if constexpr (LNF) {
         // LNF instantiation: every per-column vector lives in shared memory (no register copies: the epilogue is register-bound)
         if (mv) ln_row_stats(op, m, ln_mu, ln_rstd);
@@ -633,15 +586,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       }   // !LNF
       float enc_keep = 1.f;
       if constexpr (ENC) if ((op.flags & EPI_ROWMASK) && mv) enc_keep = __ldg(op.rowmask + m);
-      mbar_wait(acc_full(it & 1), (uint32_t)((it >> 1) & 1));
-      if (it == 0 && tr0 && warp == 2 && lane == 0) TRACE(5);
+      if (it == 0 && tr0 && warp == 4 && lane == 0) TRACE(5);
       if (it == 0 && tr0) ETRACE(0);
-      tc_fence_after();
-      auto release_acc = [&]() {                            // this warp has read everything it needs from the accumulator buffer
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(acc_empty(it & 1));
-      };
       auto wait_staging = [&]() {                           // the TMA unit must have read the previous chunk out of the staging area
         if (staged_once && op.tma_out) {
           if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -652,9 +598,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         {
           const int hh = cc0;                               // the two warps of a lane quarter take one half each
           float val[32], gate[32];
-          tmem_ld32_sum(trow + (uint32_t)(hh * 32), trow + (uint32_t)(BN + hh * 32), val);
-          tmem_ld32_sum(trow + (uint32_t)(64 + hh * 32), trow + (uint32_t)(BN + 64 + hh * 32), gate);
-          release_acc();
+          acc_row32<BN>(acc_tile, r, hh * 32, val);
+          acc_row32<BN>(acc_tile, r, 64 + hh * 32, gate);
           const int nbase = nt * 64 + hh * 32;              // logical output column
           if (nbase < op.n_valid) {                         // (uniform across the warp)
             if (!mv) {
@@ -693,13 +638,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
 #pragma unroll 1
         for (int cc = cc0; cc < BN / 32; cc += 2) {         // the two warps of a lane quarter alternate chunks
           float acc[32];
-          tmem_ld32_sum(trow + (uint32_t)(cc * 32), trow + (uint32_t)(BN + cc * 32), acc);
-          if (cc + 2 >= BN / 32) release_acc();
+          acc_row32<BN>(acc_tile, r, cc * 32, acc);
           if (it == 0 && tr0) ETRACE(1);
           if constexpr (XF) if (ks > 1) {
             // split-K: the partner CTA's fp32 partial of this thread's 32 values travels through THIS tile owner's shared
             // memory (its weight ring is idle once its own accumulator is complete): [8 x float4][256 threads]
-            const int te = tid - 64;
+            const int te = tid - 128;
             if (kr != 0) {
               mbar_wait_cluster(xr_ready(), 0);              // the owner has finished its main loop
               const uint32_t rbase = mapa_u32(base + kXOffB, 0);
@@ -710,7 +654,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
               if (lane == 0) mbar_arrive_remote(mapa_u32(xr_full(), 0));
               continue;                                      // no epilogue of its own: the owner stores the tile
             }
-            if (warp == 2 && lane == 0) mbar_arrive_remote(mapa_u32(xr_ready(), 1));   // (acc_full has been waited for: our rings are idle)
+            if (warp == 4 && lane == 0) mbar_arrive_remote(mapa_u32(xr_ready(), 1));   // (our wgmmas have retired: the rings are idle)
             mbar_wait_cluster(xr_full(), 0);
             const float4* xr = reinterpret_cast<const float4*>(smem + kXOffB);
 #pragma unroll
@@ -773,7 +717,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
             wait_staging();
             emit_chunk(op, tmo, st, lane, leader, stage_f32, b, t, t_warp0, m, mv, nbase, acc, true,
-                       (it == 0 && tr0 && warp == 2 && lane == 0) ? op.trace : nullptr);
+                       (it == 0 && tr0 && warp == 4 && lane == 0) ? op.trace : nullptr);
             staged_once = true;
             if (it == 0 && tr0) ETRACE(3);
             if (op.flags & EPI_STATS) {
@@ -796,7 +740,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         if ((op.flags & EPI_STATS) && kr == 0) {            // (a split-K partner has no output of its own)
           asm volatile("bar.sync 1, 256;" ::: "memory");    // the 8 epilogue warps
           if (it == 0 && tr0) ETRACE(5);
-          const int col = tid - 64;                         // 0..127
+          const int col = tid - 128;                        // 0..127
           if (col < BN && n0 + col < op.n_valid) {
             double cs = 0, cq = 0;
 #pragma unroll
@@ -812,14 +756,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     if (op.tma_out && leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
   }
 
-  if (warp == 2 && lane == 0 && tr0) TRACE(6);
+  if (warp == 4 && lane == 0 && tr0) TRACE(6);
   if (tr0) ETRACE(6);
-  tc_fence_before();
   __syncthreads();
   if (tr0) ETRACE(7);
   if (tid == 0 && tr0) TRACE(7);
   span_end(op.span);
-  if (warp == 2) tmem_dealloc(tmem_base, 2 * kAccCols);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -867,7 +809,7 @@ static int encode_one(TMap* out, const __nv_bfloat16* base, const SplitBuf& s, i
 
 int encode_tmaps(GemmOp& op) {
   // Outputs: the epilogue stages each warp's 32 x 32 chunk in shared memory and hands it to the TMA unit
-  // (thread = row straight out of TMEM would cost 32 LSU wavefronts per 128-bit store instruction).
+  // (one thread per row storing straight to global memory would cost 32 LSU wavefronts per 128-bit store instruction).
   op.tma_out = 0;
   if (!(op.flags & EPI_OUT_NCT)) {
     if ((op.flags & EPI_OUT_F32) && op.out && (op.out_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(op.out) & 15) == 0) {
@@ -902,7 +844,7 @@ static int sm_count() {
   if (!n) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -917,8 +859,7 @@ static int launch_bn(const GemmOp& op, cudaStream_t st) {
     attr_set = true;
   }
   const int tiles = op.B * ceil_div(op.T_out, BM) * (op.N / BN_);
-  // persistent: one CTA per SM at most, each looping over its share of the (m, n) tiles; panel mode: one tile per CTA
-  int grid = (XF && op.xmode) ? tiles : (tiles < sm_count() ? tiles : sm_count());
+  int grid = tiles;                                         // one tile per CTA (the epilogue reuses the stage buffers)
   dim3 cluster(1, 1, 1);
   if (XF && op.xmode && op.ksplit > 1) { grid = tiles * op.ksplit; cluster.x = (unsigned)op.ksplit; }   // split-K: the CTAs of a cluster share a tile
   cudaError_t e = launch_kc(gemm_tc_kernel<BN_, LNF, XF, ENC>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmemBytes, st, cluster, op);
@@ -929,7 +870,7 @@ static int launch_bn(const GemmOp& op, cudaStream_t st) {
 int gemm_sm_count() { return sm_count(); }
 
 void plan_gemm(GemmOp& op) {
-  // N tile: 64 wide (more, smaller tiles balance better over the persistent CTAs); the GEGLU epilogue pairs
+  // N tile: 64 wide (more, smaller tiles balance better over the SMs); the GEGLU epilogue pairs
   // value|gate inside a 128-column block and needs BN = 128.
   op.bn = (op.flags & EPI_GEGLU) ? 128 : 64;
 }

@@ -165,7 +165,7 @@ int launch_prep_split(const PrepOp& op, cudaStream_t st) {
   if (op.mode != PREP_RAW && !op.scale && (C % op.gn.G)) { set_error("prep_split: %d channels not divisible by %d groups", C, op.gn.G); return -1; }
   const int total = op.T_dst * (op.out.ld >> 3);
   int bx = (total + 255) / 256;
-  const int cap = (148 * 8 + op.B - 1) / op.B;           // ~8 blocks per SM over the whole grid
+  const int cap = (132 * 8 + op.B - 1) / op.B;           // ~8 blocks per SM over the whole grid
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   const size_t smem = (op.mode != PREP_RAW) ? (size_t)prep_affine_floats(C) * sizeof(float) : 0;
@@ -529,7 +529,7 @@ __global__ void __launch_bounds__(256) dpm_step_kernel(const float* __restrict__
 int launch_dpm_step(const float* x, const float* unet_out, const float* m_prev, const DpmStepCoef& c, float* m_cur,
                     float* x_next, size_t n, int* nan_flag, cudaStream_t st) {
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   launch_k(dpm_step_kernel, dim3(blocks), dim3(256), 0, st, x, unet_out, m_prev, c, m_cur, x_next, n, nan_flag);
   NS_LAUNCH_CHECK();
   return 0;
@@ -583,7 +583,7 @@ int launch_unipc_step(const float* x_prev, const float* x_eval, const float* une
                       const float* m1, const UniPcStepCoef& c, float* m_t, float* x_t, float* x_pred, size_t n,
                       int* nan_flag, cudaStream_t st) {
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   launch_k(unipc_step_kernel, dim3(blocks), dim3(256), 0, st, x_prev, x_eval, unet_out, m0, m1, c, m_t, x_t, x_pred, n, nan_flag);
   NS_LAUNCH_CHECK();
   return 0;

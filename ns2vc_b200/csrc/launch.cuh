@@ -1,7 +1,7 @@
 // Programmatic dependent launch (PDL): every kernel of the step is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, fires griddepcontrol.launch_dependents at its
 // top and executes griddepcontrol.wait before its first access to global memory.  The next
-// kernel's launch latency and prologue (barrier init, TMEM alloc, descriptor fetch) then overlap the
+// kernel's launch latency and prologue (barrier init, descriptor fetch) then overlap the
 // tail of the current one; correctness is unchanged because `wait` returns only after the
 // prerequisite grid has completed and its writes are visible.  NS2VC_PDL=0 disables it.
 #pragma once

@@ -1,5 +1,5 @@
 // Condition-encoder engine: `Pre_model.infer` of the reference (model.py:359-377) as one launch program per (B, T, S) over the
-// denoiser's own kernels - the tcgen05 3xBF16 GEMM (gemm_tc.cu, ENC instantiation for the ReLU / padding-mask epilogues), the
+// denoiser's own kernels - the wgmma 3xBF16 GEMM (gemm_tc.cu, ENC instantiation for the ReLU / padding-mask epilogues), the
 // flash attention kernels (key-padding bias), the LayerNorm split - plus the handful of small kernels in pre_kernels.cu.
 //
 //   g            = ref_enc(refer^T)                      TextTimeEmbedding(100, 100, 1)      model.py:340, 362; embeddings.py:421-434

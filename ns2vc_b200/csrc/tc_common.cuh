@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a primitives used by the tensor-core kernels:
-// mbarrier, TMA (bulk + tensor), tcgen05 (alloc / mma / commit / ld), UMMA descriptors.
+// Thin inline-PTX wrappers for the sm_90a primitives used by the tensor-core kernels:
+// mbarrier, TMA (bulk + tensor), clusters, wgmma and its shared-memory descriptors.
 #pragma once
 #include "common.cuh"
 #include <cstdio>
@@ -49,7 +49,7 @@ __device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) { if (++spins > (1u << 24)) __trap(); }
 }
 // One lane of a CONVERGED warp: ptxas knows that the region guarded by elect.sync runs on a single thread and issues the
-// uniform-datapath instructions (UTCHMMA, UTMALDG, UBLKCP...) directly; behind a `lane == 0` test it wraps every one of them
+// uniform-datapath instructions (UTMALDG, UBLKCP...) directly; behind a `lane == 0` test it wraps every one of them
 // in an ELECT / BRA.U.ANY serialisation loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -57,8 +57,6 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
@@ -119,99 +117,55 @@ __device__ __forceinline__ void prefetch_tmap(const TMap* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem_addr, uint32_t cols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem_addr), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// K-major SWIZZLE_128B wgmma descriptor: [0,14) start>>4 | [16,30) LBO>>4 = 1 (unused) | [32,46) SBO>>4 = 1024>>4 | [62,64) 1 =
+// SWIZZLE_128B.  The swizzle follows the address bits: a start advanced by 32 B (k-step) or by 128-byte rows stays consistent.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {          // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// d[64 x N] (fp32, registers of the warpgroup) += A[64 x 16] * B[N x 16]^T, both bf16 K-major in shared memory.
+// Thread t of the warpgroup holds d[i] = D[16 (t/32) + (t%32)/4 + 8 ((i/2)%2)][8 (i/4) + 2 (t%4) + i%2].
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float* d, uint64_t adesc, uint64_t bdesc);
+#define NS2VC_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define NS2VC_D32(i) NS2VC_D8(i), NS2VC_D8(i + 8), NS2VC_D8(i + 16), NS2VC_D8(i + 24)
+template <>
+__device__ __forceinline__ void wgmma_bf16<64>(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+               "%32, %33, p, 1, 1, 0, 0;\n\t}" : NS2VC_D32(0) : "l"(adesc), "l"(bdesc), "r"(1));
 }
+template <>
+__device__ __forceinline__ void wgmma_bf16<128>(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+               "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+               "%64, %65, p, 1, 1, 0, 0;\n\t}" : NS2VC_D32(0), NS2VC_D32(32) : "l"(adesc), "l"(bdesc), "r"(1));
+}
+#undef NS2VC_D32
+#undef NS2VC_D8
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm100):
-//   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major; 1) | [32,46) SBO>>4 = 1024>>4
-//   [46,48) version = 1 | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1,
-// B=bf16 [10,13)=1, A/B K-major, N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane quarter base + i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// Park a warpgroup's m64 x N accumulator in a [128][N] fp32 shared-memory tile (rows 64 g .. 64 g + 63), 16-byte chunk c of
+// row r stored at chunk c ^ (r & 7): the epilogue then reads one row per thread, 32 consecutive columns, conflict-free.
+template <int N>
+__device__ __forceinline__ void acc_park(float* tile, const float* d, int g, int t) {
+  const int w = t >> 5, l = t & 31;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N / 2; i += 2) {
+    const int r = 64 * g + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3);
+    *reinterpret_cast<float2*>(tile + r * N + ((((c >> 2) ^ (r & 7))) << 2) + (c & 3)) = make_float2(d[i], d[i + 1]);
+  }
 }
-// v[i] = tmem[a + i] + tmem[b + i], i < 32 (both loads in flight before the single wait)
-__device__ __forceinline__ void tmem_ld32_sum(uint32_t ta, uint32_t tb, float* v) {
-  uint32_t r[32], q[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(ta));
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]),
-        "=r"(q[9]), "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15]), "=r"(q[16]),
-        "=r"(q[17]), "=r"(q[18]), "=r"(q[19]), "=r"(q[20]), "=r"(q[21]), "=r"(q[22]), "=r"(q[23]), "=r"(q[24]),
-        "=r"(q[25]), "=r"(q[26]), "=r"(q[27]), "=r"(q[28]), "=r"(q[29]), "=r"(q[30]), "=r"(q[31])
-      : "r"(tb));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// v[i] = row r, column c0 + i of the parked tile, i < 32 (c0 a multiple of 32)
+template <int N>
+__device__ __forceinline__ void acc_row32(const float* tile, int r, int c0, float* v) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) + __uint_as_float(q[i]);
+  for (int j = 0; j < 8; ++j) {
+    const float4 x = *reinterpret_cast<const float4*>(tile + r * N + ((((c0 >> 2) + j) ^ (r & 7)) << 2));
+    v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
+  }
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 }  // namespace ns2vc

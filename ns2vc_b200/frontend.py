@@ -4,9 +4,8 @@
 
 The reference walks the target frames in a Python loop and copies one column per iteration (on a CUDA tensor: one tiny kernel per
 frame - about a thousand launches per slice, the same order as this package's whole first-call overhead for a new shape).  Here the
-SAME walk runs on the host over the same fp32 boundary table and produces an index vector; the copy is one gather (measured on a
-B200, 530 -> 1000 frames: 12.5 ms for the reference-style walk on a CUDA tensor, 0.14 ms here; profiles/r02_shape_churn.txt).  Bit-identical
-output (``tests/test_frontend.py``, against the reference's own function where the reference tree is present).
+SAME walk runs on the host over the same fp32 boundary table and produces an index vector; the copy is one gather.  Bit-identical
+output (``tests/test_frontend.py``, against outputs recorded from the reference's own function).
 
 Drop-in: ``utils.repeat_expand_2d = ns2vc_b200.frontend.repeat_expand_2d`` after ``import utils``.
 """

@@ -7,7 +7,7 @@ results to the sampler (``model.py:631-633, 666-668``).
 Same constructor argument (the ``cfg`` dict with ``phoneme_encoder`` / ``prompt_encoder`` keyword sets), same
 ``state_dict`` key names and shapes (34 923 404 parameters for the shipped configuration, ``demo.ipynb:447``), same
 ``infer(data)`` / ``forward(data)`` signatures and return layouts (``[T, B, C]`` / ``[S, B, C]``).  The math runs in the
-sm_100a engine behind the C-ABI (``include/ns2vc_b200.h``, ``csrc/pre_engine.cu``); this module owns the parameters and
+sm_90a engine behind the C-ABI (``include/ns2vc_b200.h``, ``csrc/pre_engine.cu``); this module owns the parameters and
 marshals pointers.  No CPU path; inference only (the reference's training forward applies dropout and needs autograd).
 """
 from __future__ import annotations
@@ -82,7 +82,7 @@ class Pre_model(nn.Module):
         self.cfg = cfg
         for name in ("phoneme_encoder", "prompt_encoder"):
             if not cfg[name].get("last_ln", True):
-                raise NotImplementedError(f"{name}: last_ln=False is not supported by the B200 condition encoders")
+                raise NotImplementedError(f"{name}: last_ln=False is not supported by these condition encoders")
         shapes = pre_param_shapes(cfg)
         for key, shape in shapes.items():
             owner, leaf = key.rsplit(".", 1)
@@ -153,7 +153,7 @@ class Pre_model(nn.Module):
                 self._handle_device = device
             for key, p in self.state_dict().items():
                 if p.device != device or p.dtype != torch.float32:
-                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; the B200 condition encoders need fp32 parameters on {device}")
+                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; these condition encoders need fp32 parameters on {device}")
                 t = p.detach().contiguous()
                 shape = (C.c_int64 * t.dim())(*t.shape)
                 _lib.check(L.ns2vc_pre_load_weight(self._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
@@ -177,7 +177,7 @@ class Pre_model(nn.Module):
         refer_lengths [B], uv) -> (content [T, B, C_out], audio_prompt [S, B, C_out]); frames past a length are exactly zero."""
         c_padded, refer_padded, _f0, _spec, _wav, lengths, refer_lengths, _uv = data
         if not c_padded.is_cuda:
-            raise RuntimeError("ns2vc_b200.Pre_model has no CPU path: move the module and inputs to a B200 ('cuda')")
+            raise RuntimeError("ns2vc_b200.Pre_model has no CPU path: move the module and inputs to an H100 ('cuda')")
         dev = c_padded.device
         pi, _ph, po, _pl = _enc_args(self.cfg["phoneme_encoder"], 512)
         ri, _rh, ro, _rl = _enc_args(self.cfg["prompt_encoder"], 256)
@@ -212,7 +212,7 @@ class Pre_model(nn.Module):
     def forward(self, data, g=None):
         """``Pre_model.forward`` (model.py:341-359) in eval mode: (content, audio_prompt, lf0, lf0_pred) with lf0 = lf0_pred = 0."""
         if self.training and torch.is_grad_enabled():
-            raise NotImplementedError("the B200 condition encoders run inference only (the reference's training forward applies "
+            raise NotImplementedError("these condition encoders run inference only (the reference's training forward applies "
                                       "dropout and needs autograd): call .eval() under torch.no_grad()")
         content, prompt = self.infer(data)
         return content, prompt, 0, 0

@@ -2,7 +2,7 @@
 
 Same constructor keywords (``unet_1d_condition.py:151-203``), same ``state_dict`` key names and
 shapes (SURVEY.md Appendix B), same ``forward`` signature and ``UNet1DConditionOutput(.sample)``
-return (``:743-757, 1034-1037``).  The math runs in the sm_100a engine behind the C-ABI
+return (``:743-757, 1034-1037``).  The math runs in the sm_90a engine behind the C-ABI
 (``include/ns2vc_b200.h``); this module only owns the parameters and marshals pointers.
 
 There is NO CPU fallback: a forward on CPU tensors, or without the built extension, raises.
@@ -165,7 +165,7 @@ class UNet1DConditionModel(nn.Module):
 
         def _only(name, val, allowed):
             if val not in allowed:
-                raise ValueError(f"`{name}`={val!r} is not supported by the B200 denoiser (supported: {allowed})")
+                raise ValueError(f"`{name}`={val!r} is not supported by this denoiser (supported: {allowed})")
 
         n = len(block_out_channels)
         _only("center_input_sample", center_input_sample, (False,))
@@ -193,7 +193,7 @@ class UNet1DConditionModel(nn.Module):
         _only("class_embeddings_concat", class_embeddings_concat, (False,))
         _only("cross_attention_norm", cross_attention_norm, (None,))
         if norm_num_groups is None:
-            raise ValueError("`norm_num_groups`=None is not supported by the B200 denoiser")
+            raise ValueError("`norm_num_groups`=None is not supported by this denoiser")
         if not isinstance(num_attention_heads, int):
             if len(set(num_attention_heads)) != 1:
                 raise ValueError("per-block `attention_head_dim` tuples must be uniform")
@@ -324,7 +324,7 @@ class UNet1DConditionModel(nn.Module):
                 self._handle_device = device
             for key, p in self.state_dict().items():
                 if p.device != device or p.dtype != torch.float32:
-                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; the B200 denoiser needs fp32 parameters on {device} (module.to('cuda'))")
+                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; this denoiser needs fp32 parameters on {device} (module.to('cuda'))")
                 t = p.detach().contiguous()
                 shape = (C.c_int64 * t.dim())(*t.shape)
                 _lib.check(L.ns2vc_unet_load_weight(self._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
@@ -379,13 +379,13 @@ class UNet1DConditionModel(nn.Module):
                         ("down_block_additional_residuals", down_block_additional_residuals),
                         ("mid_block_additional_residual", mid_block_additional_residual)):
             if v is not None and not (isinstance(v, dict) and not v):
-                raise NotImplementedError(f"`{name}` is not supported by the B200 denoiser")
+                raise NotImplementedError(f"`{name}` is not supported by this denoiser")
         if not sample.is_cuda:
-            raise RuntimeError("ns2vc_b200.UNet1DConditionModel has no CPU path: move the module and inputs to a B200 ('cuda')")
+            raise RuntimeError("ns2vc_b200.UNet1DConditionModel has no CPU path: move the module and inputs to an H100 ('cuda')")
         if torch.is_grad_enabled() and (sample.requires_grad or encoder_hidden_states.requires_grad
                                         or any(p.requires_grad for p in self.parameters())):
             raise NotImplementedError(
-                "backward through the fused sm_100a denoiser is not implemented yet; call under torch.no_grad() "
+                "backward through the fused sm_90a denoiser is not implemented yet; call under torch.no_grad() "
                 "(inference) — training is tracked as SURVEY.md §8(f) rank 2")
         dev = sample.device
         if sample.dim() != 3 or sample.shape[1] != self.cfg.in_channels:

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(L, s), f"{s} declared in include/ns2vc_b200.h but not exported"
     assert set(syms) == set(_lib.SIGNATURES), set(syms) ^ set(_lib.SIGNATURES)
-    assert b"sm_100a" in L.ns2vc_build_info()
+    assert b"sm_90a" in L.ns2vc_build_info()
 
 
 def test_nearest_index_bit_exact(gold):
