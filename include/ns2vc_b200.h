@@ -193,6 +193,49 @@ int ns2vc_pre_tap_info(const ns2vc_pre* h, int i, const char** name, int* rows, 
 int ns2vc_pre_set_tap(ns2vc_pre* h, int i, float* dst);
 int ns2vc_pre_launch_count(const ns2vc_pre* h);   /* kernels launched by the last infer */
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Prompt-mel front end: the recipe of reference inference/infer_tool.py:170-181 (and preprocess.py:27-31, 49-59) per
+ * utterance of a ragged batch - torchaudio Resample(orig, new) (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99),
+ * then MelSpectrogram at the fixed parameters below, then log(max(., 1e-7)).
+ * Same conventions as above: raw device pointers, device int64 lengths, caller-owned outputs, int errors, stream-ordered.
+ * create builds and uploads the handle's tables on the current device; the calls allocate nothing and never synchronise.
+ * A handle is read-only after create: it may serve several streams at once. */
+#define NS2VC_MEL_SAMPLE_RATE 24000   /* Hz                                                                  */
+#define NS2VC_MEL_N_FFT 1024          /* periodic Hann window of n_fft, center=True with reflect padding of  */
+#define NS2VC_MEL_HOP 256             /* n_fft / 2 at each utterance's own ends, one-sided magnitude          */
+#define NS2VC_MEL_N_MELS 100          /* HTK mel scale, 0 .. NS2VC_MEL_F_MAX Hz, norm=None                    */
+#define NS2VC_MEL_F_MAX 12000.0
+#define NS2VC_MEL_LOG_CLIP 1e-7f
+typedef struct ns2vc_resampler ns2vc_resampler;
+typedef struct ns2vc_mel ns2vc_mel;
+/* Host-only, no GPU: torchaudio's output length of Resample(orig, new) for n input samples, ceil(fp32(new * n / orig))
+ * with the ratio reduced by its gcd and the quotient taken in fp64 (NOT the exact integer ceiling); n when orig == new;
+ * -1 on bad arguments. */
+long long ns2vc_resample_out_length(int orig_freq, int new_freq, long long n);
+/* Host-only: the resampler's fp32 phase table [phases][taps] (phases = new / gcd, taps = 2 * width + orig / gcd) as torchaudio
+ * builds it in fp64 and rounds it; table may be NULL to query the sizes.  orig == new has no table (error). */
+int ns2vc_resample_table(int orig_freq, int new_freq, int* phases, int* taps, int* width, float* table);
+/* Host-only: the dense fp32 mel filterbank [513][100] (torchaudio melscale_fbanks at the parameters above). */
+int ns2vc_mel_filterbank(float* fb);
+int ns2vc_resampler_create(int orig_freq, int new_freq, ns2vc_resampler** out);   /* orig == new: a copy */
+void ns2vc_resampler_destroy(ns2vc_resampler* h);
+/* x [B, n] fp32 (batch stride x_bstride floats), lengths [B] int64 device (each <= n; NULL: every row n)
+ *   -> y [B, n_out] (batch stride y_bstride), n_out <= ns2vc_resample_out_length(orig, new, n).  Row b is
+ *   Resample(orig, new)(x[b, :lengths[b]]); samples at or past its output length are exactly 0. */
+int ns2vc_resample(const ns2vc_resampler* h, const float* x, long long x_bstride, long long n, const int64_t* lengths, float* y,
+                   long long y_bstride, long long n_out, int B, ns2vc_stream stream);
+/* window [1024] and fb [513][100]: host fp32 tables, or NULL for the library's own (the periodic Hann window in fp64 rounded to
+ * fp32; ns2vc_mel_filterbank()).  The reference's recipe uses torch's fp32 tables, whose vectorised cosf / powf round some
+ * entries 1 ulp apart from the C library's; a quiet mel band notices that more than the kernel's own rounding, so a caller
+ * matching the reference passes torch.hann_window(1024) and torch's melscale_fbanks (ns2vc_b200.frontend does). */
+int ns2vc_mel_create(const float* window, const float* fb, ns2vc_mel** out);
+void ns2vc_mel_destroy(ns2vc_mel* h);
+/* x [B, n] fp32 at 24 kHz (batch stride x_bstride floats), lengths [B] int64 device (each in (512, n]; NULL: every row n)
+ *   -> mel [B, 100, S] fp32 contiguous, S <= 1 + n / 256: log(max(MelSpectrogram(x[b, :len]), 1e-7)); frames at or past
+ *   1 + lengths[b] / 256 are exactly 0. */
+int ns2vc_log_mel(const ns2vc_mel* h, const float* x, long long x_bstride, long long n, const int64_t* lengths, float* mel, int S,
+                  int B, ns2vc_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -93,6 +93,16 @@ SIGNATURES = {
     "ns2vc_pre_tap_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ns2vc_pre_set_tap": (C.c_int, [_P, C.c_int, _P]),
     "ns2vc_pre_launch_count": (C.c_int, [_P]),
+    # prompt-mel front end (resampler + log-mel spectrogram)
+    "ns2vc_resample_out_length": (C.c_longlong, [C.c_int, C.c_int, C.c_longlong]),
+    "ns2vc_resample_table": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
+    "ns2vc_mel_filterbank": (C.c_int, [_P]),
+    "ns2vc_resampler_create": (C.c_int, [C.c_int, C.c_int, C.POINTER(_P)]),
+    "ns2vc_resampler_destroy": (None, [_P]),
+    "ns2vc_resample": (C.c_int, [_P, _P, C.c_longlong, C.c_longlong, _P, _P, C.c_longlong, C.c_longlong, C.c_int, _P]),
+    "ns2vc_mel_create": (C.c_int, [_P, _P, C.POINTER(_P)]),
+    "ns2vc_mel_destroy": (None, [_P]),
+    "ns2vc_log_mel": (C.c_int, [_P, _P, C.c_longlong, C.c_longlong, _P, _P, C.c_int, C.c_int, _P]),
 }
 
 _lib: Optional[C.CDLL] = None
