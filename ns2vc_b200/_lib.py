@@ -8,6 +8,8 @@ import ctypes as C
 import os
 from typing import Optional
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", os.environ.get("NS2VC_LIB_NAME", "libns2vc_b200.so"))   # (NS2VC_LIB_NAME: A/B builds during development)
 
@@ -133,3 +135,55 @@ def check(rc: int) -> None:
     if rc != 0:
         msg = lib().ns2vc_last_error()
         raise Ns2vcError((msg or b"unknown error").decode("utf-8", "replace") + f" (code {rc})")
+
+
+def engine_handle(mod, prefix: str, device, requirement: str) -> int:
+    """The engine handle of ``mod`` (a module with ``_c_cfg()`` and ``_release()``) on ``device``, with its current parameter
+    values loaded and packed.  ``prefix`` selects the C-ABI (``"ns2vc_unet_"`` / ``"ns2vc_pre_"``).  The handle is created on
+    the device if needed; every state_dict entry is loaded and the weights are finalized again whenever a parameter changed
+    (optimizer step, load_state_dict, .to()).  ``requirement`` ends the error raised for a parameter that is not fp32 on
+    ``device``; ``{device}`` in it is filled in."""
+    # (storage, version) pairs over a cached list of the Parameter objects: the module tree is fixed after construction,
+    # `.to()` / `load_state_dict` / optimizers change storage or bump versions of the SAME objects (the recursive
+    # `self.parameters()` walk on every forward of the generic path was ~1 ms of host time per call)
+    plist = mod.__dict__.get("_plist")
+    if plist is None:
+        plist = mod.__dict__["_plist"] = list(mod.parameters())
+    sig = tuple((p.data_ptr(), p._version) for p in plist)
+    if mod._handle is not None and mod._wsig == sig and mod._handle_device == device:
+        return mod._handle
+    plist = mod.__dict__["_plist"] = list(mod.parameters())     # something changed: re-walk the tree before re-packing
+    sig = tuple((p.data_ptr(), p._version) for p in plist)
+    L = lib()
+    stream = torch.cuda.current_stream(device).cuda_stream
+    with torch.cuda.device(device):
+        if mod._handle is None or mod._handle_device != device:
+            mod._release()
+            h = C.c_void_p()
+            ccfg = mod._c_cfg()
+            check(getattr(L, prefix + "create")(C.byref(ccfg), C.byref(h)))
+            mod._handle = h.value
+            mod._handle_device = device
+        load = getattr(L, prefix + "load_weight")
+        for key, p in mod.state_dict().items():
+            if p.device != device or p.dtype != torch.float32:
+                raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; " + requirement.format(device=device))
+            t = p.detach().contiguous()
+            shape = (C.c_int64 * t.dim())(*t.shape)
+            check(load(mod._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
+        check(getattr(L, prefix + "finalize")(mod._handle, stream))
+    mod._wsig = sig
+    return mod._handle
+
+
+def release_engine(mod, prefix: str) -> bool:
+    """Destroy the engine handle of ``mod``; False if it had none.  Plain ``__dict__`` writes: ``nn.Module.__setattr__`` may
+    already be torn down at interpreter shutdown."""
+    if mod.__dict__.get("_handle") is None:
+        return False
+    try:
+        getattr(lib(), prefix + "destroy")(mod._handle)
+    except Exception:
+        pass
+    mod.__dict__["_handle"] = None
+    return True

@@ -213,6 +213,9 @@ struct PackSeg {
 };
 int launch_pack_b(const PackSeg& ps, __nv_bfloat16* w_hi, __nv_bfloat16* w_lo, float* w_f32, int Npad,
                   cudaStream_t st);
+// g[n] = sum_c gamma_c W[n, c], bf[n] = sum_c beta_c W[n, c] (+ bias[n]) of a [N, C] linear that consumes LayerNorm(gamma, beta)
+// (EPI_LNFOLD; load time, pre_kernels.cu)
+int launch_ln_fold_vec(const float* W, const float* gamma, const float* beta, const float* bias, float* g, float* bf, int N, int C, cudaStream_t st);
 
 int launch_prep_split(const PrepOp& op, cudaStream_t st);
 
@@ -339,7 +342,6 @@ int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int 
 int launch_tbc_weight(const float* w, int k, int cin, int cout, float* o, cudaStream_t st);
 int launch_ffn_taps(const float* const* w, int k, int F, int H, int centre, float scale, float* o, cudaStream_t st);
 int launch_scale_vec(const float* a, float s, float* o, int n, cudaStream_t st);
-int launch_ln_fold_vec(const float* W, const float* gamma, const float* beta, const float* bias, float* g, float* bf, int N, int C, cudaStream_t st);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

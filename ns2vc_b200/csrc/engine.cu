@@ -4,6 +4,7 @@
 // (unet1d/unet_1d_condition.py:421-559, forward :943-1032) — see ns2vc_b200/arch.py for the
 // Python twin that the oracle uses; tests compare the two plan strings.
 #include "common.cuh"
+#include "engine_host.cuh"
 #include "../../include/ns2vc_b200.h"
 
 #include <algorithm>
@@ -11,9 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 using namespace ns2vc;
@@ -26,24 +25,6 @@ struct PlanOp {
   int cin = 0, cout = 0, level = 0;
   int c1 = 0, c2 = 0;       // RESNET: channels of the running tensor and of the concatenated skip
 };
-
-struct WSlot {
-  std::string name;
-  std::vector<int64_t> shape;
-  float* d = nullptr;       // owned fp32 copy
-  bool loaded = false;
-  size_t numel() const { size_t n = 1; for (auto s : shape) n *= (size_t)s; return n; }
-};
-
-struct PackedB {
-  __nv_bfloat16* hi = nullptr;
-  __nv_bfloat16* lo = nullptr;
-  float* f32 = nullptr;
-  int Npad = 0, nkb = 0, n_logical = 0;
-};
-
-inline int pad_to(int v, int m) { return (v + m - 1) / m * m; }
-inline int nkb_of(int c) { return (c + 63) / 64; }
 
 struct ResnetSite {
   std::string p;
@@ -71,33 +52,15 @@ struct XformerSite {
 };
 struct ConvSite { std::string p; int c; PackedB w; };
 
-// One launch of the per-shape program.
-struct Launch {
-  enum Kind { GEMM, ATTN, LN_SPLIT, LN_APPLY, LINEAR, NCT2SPLIT, POOL_CLS, POOL_ATT, MASKBIAS, PREP, MEMSET, TAP } kind;
-  GemmOp gemm;
-  AttnOp attn;
-  LinOp lin;
-  PrepOp prep;
-  SplitBuf split;
-  // generic small args
-  const float* a = nullptr; const float* b = nullptr; const float* c = nullptr; float* o = nullptr;
-  int i0 = 0, i1 = 0, i2 = 0, i3 = 0; float f0 = 0;
-  void* mem = nullptr; size_t mem_bytes = 0;
-  int patch = 0;             // 1: x (forward)  2: t  3: out  4: content  5: prompt  6: mask
-  int tap_index = -1;
-  int reads_film = 0;        // 1: reads the FiLM rows (pointers are rebased when the caller supplies precomputed rows)
-  int time_path = 0;         // 1: timestep path (sinusoid -> MLP -> FiLM rows): skipped when the caller supplies precomputed FiLM rows
-};
-
-struct Arena {           // bump allocator over the caller's workspace (or a dry run when base == nullptr)
-  uint8_t* base = nullptr;
-  size_t off = 0;
-  template <class T> T* get(size_t n) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * sizeof(T);
-    return p;
-  }
+// The launch programs of one (B, T, S, workspace) key.
+struct Program {
+  int B = 0, T = 0, S = 0; void* ws = nullptr;
+  bool has_mask = false;
+  bool cond_ready = false;   // the conditioning program has run for this key since it last became active
+  std::vector<Launch> prog_cond, prog_fwd;
+  float* film_base = nullptr;                             // FiLM rows [B, film_total] (workspace)
+  float* aug = nullptr;                                   // add_embedding output [B, ted] (workspace)
+  TapSet taps;
 };
 
 }  // namespace
@@ -106,8 +69,7 @@ struct ns2vc_unet {
   ns2vc_unet_cfg cfg;
   int ted = 0;                                   // time_embed_dim
   std::vector<PlanOp> plan;
-  std::vector<WSlot> weights;
-  std::unordered_map<std::string, int> windex;
+  WeightRegistry weights;
   bool finalized = false;
   bool simt = false;
   std::string plan_str;
@@ -118,45 +80,30 @@ struct ns2vc_unet {
   PackedB convin_lat, convin_content, conv_out, kv_all;
   int kv_total = 0, k_total = 0, film_total = 0;
   float* film_W = nullptr; float* film_b = nullptr;       // concatenated time_emb_proj
-  float* pool_kv_W = nullptr; float* pool_kv_b = nullptr; // concatenated k_proj | v_proj
-  std::vector<void*> owned;                               // everything to cudaFree
+  PoolKV pool_kv;                                         // concatenated k_proj | v_proj
+  DeviceMem mem;                                          // everything the packed model owns
 
-  // cached program
-  int pB = 0, pT = 0, pS = 0; void* pws = nullptr; bool has_mask = false; bool cond_ready = false;
-  float* aug = nullptr;                                   // add_embedding output [B, ted] of the active program (workspace)
+  // Cached programs, least recently active first; the active one (if any) is progs[active].  Other keys stay cached for the
+  // sub-batch lanes of a multi-stream sampler and for callers that alternate shapes.
+  static constexpr size_t kMaxInactive = 16;
+  std::vector<Program> progs;
+  int active = -1;
   // Per-program STATIC device data (GroupNorm descriptors, nearest-upsample index tables) lives outside the caller's workspace:
   // several shapes may share one workspace, and captured graphs keep reading these tables, so they are only released when the
   // weights are re-packed or the handle is destroyed (~20 KB per shape ever seen)
   std::vector<void*> static_bufs;
-  std::vector<Launch> prog_cond, prog_fwd;
-  std::vector<std::string> tap_names; std::vector<int> tap_level, tap_ch;
-  std::vector<float*> tap_dst;
-  // Inactive programs (other (B,T,S,workspace) keys, e.g. the sub-batch lanes of a multi-stream sampler):
-  // the fields above are the ACTIVE program; activate() swaps them with an entry of this list.
-  struct Stash {
-    int pB, pT, pS; void* pws; bool has_mask, cond_ready;
-    std::vector<Launch> prog_cond, prog_fwd; float* film_base; float* aug;
-    std::vector<std::string> tap_names; std::vector<int> tap_level, tap_ch; std::vector<float*> tap_dst;
-  };
-  std::vector<Stash> stash;
   int last_launches = 0;
   bool profiling = false;
   bool ksplit = true;        // split-K pairs for few-tile panel-mode launches (NS2VC_KSPLIT=0: one CTA per tile)
   bool xf = true;            // GroupNorm(+FiLM)(+SiLU) of the conv / proj_in inputs applied inside the GEMM (panel mode; NS2VC_XF=0: prep launches)
   bool merge_ff = true;      // ff.net.2 + proj_out as one GEMM (NS2VC_MERGE_FF=0: two launches)
-  float* film_base = nullptr;        // FiLM rows of the active program (workspace), and the caller-supplied replacement for one forward
-  const float* film_ext = nullptr;
+  const float* film_ext = nullptr;   // caller-supplied FiLM rows for one forward (replace the active program's film_base)
   bool lnfold = true;        // LayerNorms of the transformer folded into their consumer GEMMs (NS2VC_LNFOLD=0: separate LN kernels)
   unsigned long long* trace = nullptr; int trace_cap = 0;
   unsigned long long* attn_trace = nullptr; int attn_trace_cap = 0;
   unsigned long long* span = nullptr; int span_cap = 0;   // [launch][2] grid spans
   struct ProfRec { int kind; cudaEvent_t a, b; int M, N, K, nseg, ctas; };
   std::vector<ProfRec> prof;
-
-  const float* W(const std::string& n) const {
-    auto it = windex.find(n);
-    return it == windex.end() ? nullptr : weights[it->second].d;
-  }
 };
 
 namespace {
@@ -165,15 +112,6 @@ int level_len(int T, int level) {
   for (int i = 0; i < level; ++i) T = (T - 1) / 2 + 1;
   return T;
 }
-
-void add_w(ns2vc_unet* h, const std::string& n, std::vector<int64_t> shape) {
-  h->windex[n] = (int)h->weights.size();
-  WSlot s; s.name = n; s.shape = std::move(shape);
-  h->weights.push_back(std::move(s));
-}
-void add_conv(ns2vc_unet* h, const std::string& p, int co, int ci, int k) { add_w(h, p + ".weight", {co, ci, k}); add_w(h, p + ".bias", {co}); }
-void add_lin(ns2vc_unet* h, const std::string& p, int co, int ci, bool bias = true) { add_w(h, p + ".weight", {co, ci}); if (bias) add_w(h, p + ".bias", {co}); }
-void add_norm(ns2vc_unet* h, const std::string& p, int c) { add_w(h, p + ".weight", {c}); add_w(h, p + ".bias", {c}); }
 
 void build_plan(ns2vc_unet* h) {
   const ns2vc_unet_cfg& c = h->cfg;
@@ -237,109 +175,67 @@ void build_plan(ns2vc_unet* h) {
 
 void register_weights(ns2vc_unet* h) {
   const ns2vc_unet_cfg& c = h->cfg;
+  WeightRegistry& w = h->weights;
   const int c0 = c.block_out_channels[0], ted = h->ted, xd = c.cross_attention_dim;
-  add_conv(h, "conv_in", c0, c.in_channels, 3);
-  add_lin(h, "time_embedding.linear_1", ted, c0);
-  add_lin(h, "time_embedding.linear_2", ted, ted);
+  w.add_conv("conv_in", c0, c.in_channels, 3);
+  w.add_lin("time_embedding.linear_1", ted, c0);
+  w.add_lin("time_embedding.linear_2", ted, ted);
   if (c.add_embed_text) {
-    add_norm(h, "add_embedding.norm1", xd);
-    add_w(h, "add_embedding.pool.positional_embedding", {1, xd});
-    add_lin(h, "add_embedding.pool.k_proj", xd, xd);
-    add_lin(h, "add_embedding.pool.q_proj", xd, xd);
-    add_lin(h, "add_embedding.pool.v_proj", xd, xd);
-    add_lin(h, "add_embedding.proj", ted, xd);
-    add_norm(h, "add_embedding.norm2", ted);
+    w.add_norm("add_embedding.norm1", xd);
+    w.add("add_embedding.pool.positional_embedding", {1, xd});
+    w.add_lin("add_embedding.pool.k_proj", xd, xd);
+    w.add_lin("add_embedding.pool.q_proj", xd, xd);
+    w.add_lin("add_embedding.pool.v_proj", xd, xd);
+    w.add_lin("add_embedding.proj", ted, xd);
+    w.add_norm("add_embedding.norm2", ted);
   }
   for (auto& o : h->plan) {
     if (o.kind == PlanOp::RESNET) {
       const std::string& p = o.prefix;
-      add_norm(h, p + ".norm1", o.cin);
-      add_conv(h, p + ".conv1", o.cout, o.cin, 3);
-      add_lin(h, p + ".time_emb_proj", c.time_scale_shift ? 2 * o.cout : o.cout, ted);
-      add_norm(h, p + ".norm2", o.cout);
-      add_conv(h, p + ".conv2", o.cout, o.cout, 3);
-      if (o.cin != o.cout) add_conv(h, p + ".conv_shortcut", o.cout, o.cin, 1);
+      w.add_norm(p + ".norm1", o.cin);
+      w.add_conv(p + ".conv1", o.cout, o.cin, 3);
+      w.add_lin(p + ".time_emb_proj", c.time_scale_shift ? 2 * o.cout : o.cout, ted);
+      w.add_norm(p + ".norm2", o.cout);
+      w.add_conv(p + ".conv2", o.cout, o.cout, 3);
+      if (o.cin != o.cout) w.add_conv(p + ".conv_shortcut", o.cout, o.cin, 1);
     } else if (o.kind == PlanOp::XFORMER) {
       const std::string& p = o.prefix; const int cc = o.cout;
-      add_norm(h, p + ".norm", cc);
-      add_conv(h, p + ".proj_in", cc, cc, 1);
+      w.add_norm(p + ".norm", cc);
+      w.add_conv(p + ".proj_in", cc, cc, 1);
       const std::string b = p + ".transformer_blocks.0";
-      add_norm(h, b + ".norm1", cc);
-      add_lin(h, b + ".attn1.to_q", cc, cc, false); add_lin(h, b + ".attn1.to_k", cc, cc, false); add_lin(h, b + ".attn1.to_v", cc, cc, false);
-      add_lin(h, b + ".attn1.to_out.0", cc, cc);
-      add_norm(h, b + ".norm2", cc);
-      add_lin(h, b + ".attn2.to_q", cc, cc, false); add_lin(h, b + ".attn2.to_k", cc, xd, false); add_lin(h, b + ".attn2.to_v", cc, xd, false);
-      add_lin(h, b + ".attn2.to_out.0", cc, cc);
-      add_norm(h, b + ".norm3", cc);
-      add_lin(h, b + ".ff.net.0.proj", 8 * cc, cc);
-      add_lin(h, b + ".ff.net.2", cc, 4 * cc);
-      add_conv(h, p + ".proj_out", cc, cc, 1);
+      w.add_norm(b + ".norm1", cc);
+      w.add_lin(b + ".attn1.to_q", cc, cc, false); w.add_lin(b + ".attn1.to_k", cc, cc, false); w.add_lin(b + ".attn1.to_v", cc, cc, false);
+      w.add_lin(b + ".attn1.to_out.0", cc, cc);
+      w.add_norm(b + ".norm2", cc);
+      w.add_lin(b + ".attn2.to_q", cc, cc, false); w.add_lin(b + ".attn2.to_k", cc, xd, false); w.add_lin(b + ".attn2.to_v", cc, xd, false);
+      w.add_lin(b + ".attn2.to_out.0", cc, cc);
+      w.add_norm(b + ".norm3", cc);
+      w.add_lin(b + ".ff.net.0.proj", 8 * cc, cc);
+      w.add_lin(b + ".ff.net.2", cc, 4 * cc);
+      w.add_conv(p + ".proj_out", cc, cc, 1);
     } else if (o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) {
-      add_conv(h, o.prefix + ".conv", o.cout, o.cin, 3);
+      w.add_conv(o.prefix + ".conv", o.cout, o.cin, 3);
     }
   }
-  add_norm(h, "conv_norm_out", c0);
-  add_conv(h, "conv_out", c.out_channels, c0, 3);
+  w.add_norm("conv_norm_out", c0);
+  w.add_conv("conv_out", c.out_channels, c0, 3);
 }
 
-template <class T>
-int dev_alloc(ns2vc_unet* h, T** p, size_t n, bool zero) {
-  void* q = nullptr;
-  NS_CHECK_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)));
-  if (zero) NS_CHECK_CUDA(cudaMemset(q, 0, std::max<size_t>(n, 1) * sizeof(T)));
-  h->owned.push_back(q);
-  *p = reinterpret_cast<T*>(q);
-  return 0;
-}
-
-int alloc_packed(ns2vc_unet* h, PackedB& pb, int n_logical, int n_packed, int nkb) {
-  pb.n_logical = n_logical;
-  pb.Npad = pad_to(n_packed, 128);
-  pb.nkb = nkb;
-  const size_t elems = (size_t)nkb * pb.Npad * 64;
-  if (dev_alloc(h, &pb.hi, elems, true)) return -2;
-  if (dev_alloc(h, &pb.lo, elems, true)) return -2;
-  if (h->simt) { if (dev_alloc(h, &pb.f32, elems, true)) return -2; }
-  return 0;
-}
-
-// Pack `w` ([n_rows, cin_total, ktaps]) channels [cin0, cin0+ncin) of tap `tap` at k-block kb0, columns n_dst0..
-__global__ void ln_fold_vec_kernel(const float* __restrict__ W, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   const float* __restrict__ bias, float* __restrict__ g, float* __restrict__ bf, int N, int C) {
-  const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (n >= N) return;
-  double sg = 0, sb = 0;                                   // load-time only: accumulate in double
-  for (int c = lane; c < C; c += 32) { const double w = W[(long long)n * C + c]; sg += w * gamma[c]; sb += w * beta[c]; }
-  for (int o = 16; o > 0; o >>= 1) { sg += __shfl_xor_sync(0xffffffffu, sg, o); sb += __shfl_xor_sync(0xffffffffu, sb, o); }
-  if (lane == 0) { g[n] = (float)sg; bf[n] = (float)(sb + (bias ? (double)bias[n] : 0.0)); }
-}
 // g / bf of a [N, C] linear that consumes LayerNorm(gamma, beta) (rows n_dst0.. of the output vectors)
 int ln_fold_vectors(ns2vc_unet* h, const std::string& wname, const std::string& bname, const std::string& norm, int N, int C,
                     float* g, float* bf, int n_dst0, cudaStream_t st) {
-  const float* W = h->W(wname); const float* ga = h->W(norm + ".weight"); const float* be = h->W(norm + ".bias");
+  const float* W = h->weights.W(wname); const float* ga = h->weights.W(norm + ".weight"); const float* be = h->weights.W(norm + ".bias");
   NS_REQUIRE(W && ga && be, "ln fold: %s / %s missing", wname.c_str(), norm.c_str());
-  const float* bias = bname.empty() ? nullptr : h->W(bname);
-  ln_fold_vec_kernel<<<ceil_div(N, 8), 256, 0, st>>>(W, ga, be, bias, g + n_dst0, bf + n_dst0, N, C);
-  NS_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  const float* bias = bname.empty() ? nullptr : h->weights.W(bname);
+  return launch_ln_fold_vec(W, ga, be, bias, g + n_dst0, bf + n_dst0, N, C, st);
 }
 
-int pack_seg_ptr(ns2vc_unet* h, PackedB& pb, const float* w, int n_rows, int cin_total, int ktaps, int tap, int cin0,
-                 int ncin, int n_dst0, int kb0, int geglu_half, cudaStream_t st, const float* cscale = nullptr);
-int pack_seg(ns2vc_unet* h, PackedB& pb, const std::string& wname, int n_rows, int cin_total, int ktaps, int tap, int cin0,
-             int ncin, int n_dst0, int kb0, int geglu_half, cudaStream_t st, const float* cscale = nullptr) {
-  const float* w = h->W(wname);
+// pack_seg() of the registered weight `wname`
+int pack_named(ns2vc_unet* h, PackedB& pb, const std::string& wname, int n_rows, int cin_total, int ktaps, int tap, int cin0,
+               int ncin, int n_dst0, int kb0, int geglu_half, cudaStream_t st, const float* cscale = nullptr) {
+  const float* w = h->weights.W(wname);
   NS_REQUIRE(w != nullptr, "pack: weight %s missing", wname.c_str());
-  return pack_seg_ptr(h, pb, w, n_rows, cin_total, ktaps, tap, cin0, ncin, n_dst0, kb0, geglu_half, st, cscale);
-}
-int pack_seg_ptr(ns2vc_unet* h, PackedB& pb, const float* w, int n_rows, int cin_total, int ktaps, int tap, int cin0,
-                 int ncin, int n_dst0, int kb0, int geglu_half, cudaStream_t st, const float* cscale) {
-  (void)h;
-  PackSeg ps;
-  ps.cscale = cscale;
-  ps.w = w; ps.n_rows = n_rows; ps.cin_total = cin_total; ps.ktaps = ktaps; ps.tap = tap; ps.cin0 = cin0; ps.ncin = ncin;
-  ps.n_dst0 = n_dst0; ps.kb0 = kb0; ps.nkb = nkb_of(ncin); ps.geglu_half = geglu_half;
-  return launch_pack_b(ps, pb.hi, pb.lo, pb.f32, pb.Npad, st);
+  return pack_seg(pb, w, n_rows, cin_total, ktaps, tap, cin0, ncin, n_dst0, kb0, geglu_half, st, cscale);
 }
 
 // Wm[n, k] = sum_c Wp[n, c] W2[c, k]  (load time; double accumulation): the product matrix of ff.net.2 followed by proj_out
@@ -372,14 +268,14 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
   // conv_in: latent part and (hoisted) content part
   {
     const int nl = nkb_of(Cl);
-    if ((rc = alloc_packed(h, h->convin_lat, c0, c0, 3 * nl))) return rc;
+    if ((rc = h->mem.alloc_packed(h->convin_lat, c0, c0, 3 * nl, h->simt))) return rc;
     for (int j = 0; j < 3; ++j)
-      if ((rc = pack_seg(h, h->convin_lat, "conv_in.weight", c0, c.in_channels, 3, j, 0, Cl, 0, j * nl, 0, st))) return rc;
+      if ((rc = pack_named(h, h->convin_lat, "conv_in.weight", c0, c.in_channels, 3, j, 0, Cl, 0, j * nl, 0, st))) return rc;
     if (Cc > 0) {
       const int nc = nkb_of(Cc);
-      if ((rc = alloc_packed(h, h->convin_content, c0, c0, 3 * nc))) return rc;
+      if ((rc = h->mem.alloc_packed(h->convin_content, c0, c0, 3 * nc, h->simt))) return rc;
       for (int j = 0; j < 3; ++j)
-        if ((rc = pack_seg(h, h->convin_content, "conv_in.weight", c0, c.in_channels, 3, j, Cl, Cc, 0, j * nc, 0, st))) return rc;
+        if ((rc = pack_named(h, h->convin_content, "conv_in.weight", c0, c.in_channels, 3, j, Cl, Cc, 0, j * nc, 0, st))) return rc;
     }
   }
   // resnets / transformers / resamplers in plan order
@@ -388,17 +284,17 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
     if (o.kind == PlanOp::RESNET) {
       ResnetSite s; s.p = o.prefix; s.c1 = o.c1; s.c2 = o.c2; s.cin = o.cin; s.cout = o.cout; s.shortcut = o.cin != o.cout;
       const int ni = nkb_of(s.cin), no = nkb_of(s.cout);
-      if ((rc = alloc_packed(h, s.conv1, s.cout, s.cout, 3 * ni))) return rc;
+      if ((rc = h->mem.alloc_packed(s.conv1, s.cout, s.cout, 3 * ni, h->simt))) return rc;
       for (int j = 0; j < 3; ++j)
-        if ((rc = pack_seg(h, s.conv1, s.p + ".conv1.weight", s.cout, s.cin, 3, j, 0, s.cin, 0, j * ni, 0, st))) return rc;
+        if ((rc = pack_named(h, s.conv1, s.p + ".conv1.weight", s.cout, s.cin, 3, j, 0, s.cin, 0, j * ni, 0, st))) return rc;
       const int nsc = s.shortcut ? ni : 0;
-      if ((rc = alloc_packed(h, s.conv2, s.cout, s.cout, 3 * no + nsc))) return rc;
+      if ((rc = h->mem.alloc_packed(s.conv2, s.cout, s.cout, 3 * no + nsc, h->simt))) return rc;
       for (int j = 0; j < 3; ++j)
-        if ((rc = pack_seg(h, s.conv2, s.p + ".conv2.weight", s.cout, s.cout, 3, j, 0, s.cout, 0, j * no, 0, st))) return rc;
+        if ((rc = pack_named(h, s.conv2, s.p + ".conv2.weight", s.cout, s.cout, 3, j, 0, s.cout, 0, j * no, 0, st))) return rc;
       if (s.shortcut)
-        if ((rc = pack_seg(h, s.conv2, s.p + ".conv_shortcut.weight", s.cout, s.cin, 1, 0, 0, s.cin, 0, 3 * no, 0, st))) return rc;
-      if (dev_alloc(h, &s.bias2, s.cout, false)) return -2;
-      add_vec_kernel<<<ceil_div(s.cout, 256), 256, 0, st>>>(h->W(s.p + ".conv2.bias"), s.shortcut ? h->W(s.p + ".conv_shortcut.bias") : nullptr, s.bias2, s.cout);
+        if ((rc = pack_named(h, s.conv2, s.p + ".conv_shortcut.weight", s.cout, s.cin, 1, 0, 0, s.cin, 0, 3 * no, 0, st))) return rc;
+      if (!(s.bias2 = h->mem.alloc<float>(s.cout))) return -2;
+      add_vec_kernel<<<ceil_div(s.cout, 256), 256, 0, st>>>(h->weights.W(s.p + ".conv2.bias"), s.shortcut ? h->weights.W(s.p + ".conv_shortcut.bias") : nullptr, s.bias2, s.cout);
       s.film_off = film_off;
       film_off += c.time_scale_shift ? 2 * s.cout : s.cout;
       h->resnets.push_back(s);
@@ -406,46 +302,46 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       XformerSite x; x.p = o.prefix; x.c = o.cout;
       const int C = x.c, nk = nkb_of(C);
       const std::string b = x.p + ".transformer_blocks.0";
-      if ((rc = alloc_packed(h, x.proj_in, C, C, nk))) return rc;
-      if ((rc = pack_seg(h, x.proj_in, x.p + ".proj_in.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
-      if ((rc = alloc_packed(h, x.qkv, 3 * C, 3 * C, nk))) return rc;
+      if ((rc = h->mem.alloc_packed(x.proj_in, C, C, nk, h->simt))) return rc;
+      if ((rc = pack_named(h, x.proj_in, x.p + ".proj_in.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
+      if ((rc = h->mem.alloc_packed(x.qkv, 3 * C, 3 * C, nk, h->simt))) return rc;
       const char* qkvn[3] = {".attn1.to_q.weight", ".attn1.to_k.weight", ".attn1.to_v.weight"};
       const bool fold = h->lnfold;
       for (int i = 0; i < 3; ++i)
-        if ((rc = pack_seg(h, x.qkv, b + qkvn[i], C, C, 1, 0, 0, C, i * C, 0, 0, st, fold ? h->W(b + ".norm1.weight") : nullptr))) return rc;
+        if ((rc = pack_named(h, x.qkv, b + qkvn[i], C, C, 1, 0, 0, C, i * C, 0, 0, st, fold ? h->weights.W(b + ".norm1.weight") : nullptr))) return rc;
       if (fold) {
-        if (dev_alloc(h, &x.g_qkv, (size_t)3 * C, false) || dev_alloc(h, &x.bf_qkv, (size_t)3 * C, false)) return -2;
-        if (dev_alloc(h, &x.g_q2, (size_t)C, false) || dev_alloc(h, &x.bf_q2, (size_t)C, false)) return -2;
-        if (dev_alloc(h, &x.g_ff1, (size_t)8 * C, false) || dev_alloc(h, &x.bf_ff1, (size_t)8 * C, false)) return -2;
+        if (!(x.g_qkv = h->mem.alloc<float>((size_t)3 * C)) || !(x.bf_qkv = h->mem.alloc<float>((size_t)3 * C))) return -2;
+        if (!(x.g_q2 = h->mem.alloc<float>((size_t)C)) || !(x.bf_q2 = h->mem.alloc<float>((size_t)C))) return -2;
+        if (!(x.g_ff1 = h->mem.alloc<float>((size_t)8 * C)) || !(x.bf_ff1 = h->mem.alloc<float>((size_t)8 * C))) return -2;
         for (int i = 0; i < 3; ++i)
           if ((rc = ln_fold_vectors(h, b + qkvn[i], "", b + ".norm1", C, C, x.g_qkv, x.bf_qkv, i * C, st))) return rc;
         if ((rc = ln_fold_vectors(h, b + ".attn2.to_q.weight", "", b + ".norm2", C, C, x.g_q2, x.bf_q2, 0, st))) return rc;
         if ((rc = ln_fold_vectors(h, b + ".ff.net.0.proj.weight", b + ".ff.net.0.proj.bias", b + ".norm3", 8 * C, C, x.g_ff1, x.bf_ff1, 0, st))) return rc;
       }
-      if ((rc = alloc_packed(h, x.out1, C, C, nk))) return rc;
-      if ((rc = pack_seg(h, x.out1, b + ".attn1.to_out.0.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
-      if ((rc = alloc_packed(h, x.q2, C, C, nk))) return rc;
-      if ((rc = pack_seg(h, x.q2, b + ".attn2.to_q.weight", C, C, 1, 0, 0, C, 0, 0, 0, st, fold ? h->W(b + ".norm2.weight") : nullptr))) return rc;
-      if ((rc = alloc_packed(h, x.out2, C, C, nk))) return rc;
-      if ((rc = pack_seg(h, x.out2, b + ".attn2.to_out.0.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
+      if ((rc = h->mem.alloc_packed(x.out1, C, C, nk, h->simt))) return rc;
+      if ((rc = pack_named(h, x.out1, b + ".attn1.to_out.0.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
+      if ((rc = h->mem.alloc_packed(x.q2, C, C, nk, h->simt))) return rc;
+      if ((rc = pack_named(h, x.q2, b + ".attn2.to_q.weight", C, C, 1, 0, 0, C, 0, 0, 0, st, fold ? h->weights.W(b + ".norm2.weight") : nullptr))) return rc;
+      if ((rc = h->mem.alloc_packed(x.out2, C, C, nk, h->simt))) return rc;
+      if ((rc = pack_named(h, x.out2, b + ".attn2.to_out.0.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
       NS_REQUIRE((4 * C) % 64 == 0, "transformer width %d: 4C must be a multiple of 64", C);
-      if ((rc = alloc_packed(h, x.ff1, 4 * C, 8 * C, nk))) return rc;
-      if ((rc = pack_seg(h, x.ff1, b + ".ff.net.0.proj.weight", 8 * C, C, 1, 0, 0, C, 0, 0, 4 * C, st, fold ? h->W(b + ".norm3.weight") : nullptr))) return rc;
-      if ((rc = alloc_packed(h, x.ff2, C, C, nkb_of(4 * C)))) return rc;
-      if ((rc = pack_seg(h, x.ff2, b + ".ff.net.2.weight", C, 4 * C, 1, 0, 0, 4 * C, 0, 0, 0, st))) return rc;
-      if ((rc = alloc_packed(h, x.proj_out, C, C, nk))) return rc;
-      if ((rc = pack_seg(h, x.proj_out, x.p + ".proj_out.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
+      if ((rc = h->mem.alloc_packed(x.ff1, 4 * C, 8 * C, nk, h->simt))) return rc;
+      if ((rc = pack_named(h, x.ff1, b + ".ff.net.0.proj.weight", 8 * C, C, 1, 0, 0, C, 0, 0, 4 * C, st, fold ? h->weights.W(b + ".norm3.weight") : nullptr))) return rc;
+      if ((rc = h->mem.alloc_packed(x.ff2, C, C, nkb_of(4 * C), h->simt))) return rc;
+      if ((rc = pack_named(h, x.ff2, b + ".ff.net.2.weight", C, 4 * C, 1, 0, 0, 4 * C, 0, 0, 0, st))) return rc;
+      if ((rc = h->mem.alloc_packed(x.proj_out, C, C, nk, h->simt))) return rc;
+      if ((rc = pack_named(h, x.proj_out, x.p + ".proj_out.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
       if (h->merge_ff && fold) {
         // proj_out o ff.net.2 as one operator: K blocks [Wp W2 over the 4C GEGLU channels | Wp over the C residual channels]
-        const float* Wp = h->W(x.p + ".proj_out.weight"); const float* W2 = h->W(b + ".ff.net.2.weight");
+        const float* Wp = h->weights.W(x.p + ".proj_out.weight"); const float* W2 = h->weights.W(b + ".ff.net.2.weight");
         NS_REQUIRE(Wp && W2, "pack: %s feed-forward / proj_out weights missing", x.p.c_str());
         float* Wm = nullptr;
-        if (dev_alloc(h, &Wm, (size_t)C * 4 * C, false) || dev_alloc(h, &x.bias_ff2p, (size_t)C, false)) return -2;
+        if (!(Wm = h->mem.alloc<float>((size_t)C * 4 * C)) || !(x.bias_ff2p = h->mem.alloc<float>((size_t)C))) return -2;
         matmul_nn_kernel<<<dim3(ceil_div(4 * C, 128), C), 128, 0, st>>>(Wp, W2, Wm, C, C, 4 * C);
-        matvec_bias_kernel<<<ceil_div(C, 128), 128, 0, st>>>(Wp, h->W(b + ".ff.net.2.bias"), h->W(x.p + ".proj_out.bias"), x.bias_ff2p, C, C);
-        if ((rc = alloc_packed(h, x.ff2p, C, C, nkb_of(4 * C) + nk))) return rc;
-        if ((rc = pack_seg_ptr(h, x.ff2p, Wm, C, 4 * C, 1, 0, 0, 4 * C, 0, 0, 0, st))) return rc;
-        if ((rc = pack_seg(h, x.ff2p, x.p + ".proj_out.weight", C, C, 1, 0, 0, C, 0, nkb_of(4 * C), 0, st))) return rc;
+        matvec_bias_kernel<<<ceil_div(C, 128), 128, 0, st>>>(Wp, h->weights.W(b + ".ff.net.2.bias"), h->weights.W(x.p + ".proj_out.bias"), x.bias_ff2p, C, C);
+        if ((rc = h->mem.alloc_packed(x.ff2p, C, C, nkb_of(4 * C) + nk, h->simt))) return rc;
+        if ((rc = pack_seg(x.ff2p, Wm, C, 4 * C, 1, 0, 0, 4 * C, 0, 0, 0, st))) return rc;
+        if ((rc = pack_named(h, x.ff2p, x.p + ".proj_out.weight", C, C, 1, 0, 0, C, 0, nkb_of(4 * C), 0, st))) return rc;
       }
       x.kv_off = kv_off;
       kv_off += C;
@@ -453,9 +349,9 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
     } else if (o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) {
       ConvSite s; s.p = o.prefix; s.c = o.cout;
       const int nk = nkb_of(s.c);
-      if ((rc = alloc_packed(h, s.w, s.c, s.c, 3 * nk))) return rc;
+      if ((rc = h->mem.alloc_packed(s.w, s.c, s.c, 3 * nk, h->simt))) return rc;
       for (int j = 0; j < 3; ++j)
-        if ((rc = pack_seg(h, s.w, s.p + ".conv.weight", s.c, s.c, 3, j, 0, s.c, 0, j * nk, 0, st))) return rc;
+        if ((rc = pack_named(h, s.w, s.p + ".conv.weight", s.c, s.c, 3, j, 0, s.c, 0, j * nk, 0, st))) return rc;
       h->resamplers.push_back(s);
     }
   }
@@ -466,37 +362,30 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
   // conv_out
   {
     const int nk = nkb_of(c0);
-    if ((rc = alloc_packed(h, h->conv_out, c.out_channels, c.out_channels, 3 * nk))) return rc;
+    if ((rc = h->mem.alloc_packed(h->conv_out, c.out_channels, c.out_channels, 3 * nk, h->simt))) return rc;
     for (int j = 0; j < 3; ++j)
-      if ((rc = pack_seg(h, h->conv_out, "conv_out.weight", c.out_channels, c0, 3, j, 0, c0, 0, j * nk, 0, st))) return rc;
+      if ((rc = pack_named(h, h->conv_out, "conv_out.weight", c.out_channels, c0, 3, j, 0, c0, 0, j * nk, 0, st))) return rc;
   }
   // all cross-attention K|V projections as one GEMM over the prompt
   if (h->kv_total > 0) {
     const int xd = c.cross_attention_dim;
-    if ((rc = alloc_packed(h, h->kv_all, h->kv_total, h->kv_total, nkb_of(xd)))) return rc;
+    if ((rc = h->mem.alloc_packed(h->kv_all, h->kv_total, h->kv_total, nkb_of(xd), h->simt))) return rc;
     for (auto& x : h->xformers) {
       const std::string b = x.p + ".transformer_blocks.0";
-      if ((rc = pack_seg(h, h->kv_all, b + ".attn2.to_k.weight", x.c, xd, 1, 0, 0, xd, x.kv_off, 0, 0, st))) return rc;
-      if ((rc = pack_seg(h, h->kv_all, b + ".attn2.to_v.weight", x.c, xd, 1, 0, 0, xd, x.v_off, 0, 0, st))) return rc;
+      if ((rc = pack_named(h, h->kv_all, b + ".attn2.to_k.weight", x.c, xd, 1, 0, 0, xd, x.kv_off, 0, 0, st))) return rc;
+      if ((rc = pack_named(h, h->kv_all, b + ".attn2.to_v.weight", x.c, xd, 1, 0, 0, xd, x.v_off, 0, 0, st))) return rc;
     }
   }
   // concatenated FiLM projection [film_total, ted]
-  if (dev_alloc(h, &h->film_W, (size_t)h->film_total * h->ted, false)) return -2;
-  if (dev_alloc(h, &h->film_b, (size_t)h->film_total, false)) return -2;
+  if (!(h->film_W = h->mem.alloc<float>((size_t)h->film_total * h->ted))) return -2;
+  if (!(h->film_b = h->mem.alloc<float>((size_t)h->film_total))) return -2;
   for (auto& s : h->resnets) {
     const int rows = c.time_scale_shift ? 2 * s.cout : s.cout;
-    NS_CHECK_CUDA(cudaMemcpyAsync(h->film_W + (size_t)s.film_off * h->ted, h->W(s.p + ".time_emb_proj.weight"), (size_t)rows * h->ted * 4, cudaMemcpyDeviceToDevice, st));
-    NS_CHECK_CUDA(cudaMemcpyAsync(h->film_b + s.film_off, h->W(s.p + ".time_emb_proj.bias"), (size_t)rows * 4, cudaMemcpyDeviceToDevice, st));
+    NS_CHECK_CUDA(cudaMemcpyAsync(h->film_W + (size_t)s.film_off * h->ted, h->weights.W(s.p + ".time_emb_proj.weight"), (size_t)rows * h->ted * 4, cudaMemcpyDeviceToDevice, st));
+    NS_CHECK_CUDA(cudaMemcpyAsync(h->film_b + s.film_off, h->weights.W(s.p + ".time_emb_proj.bias"), (size_t)rows * 4, cudaMemcpyDeviceToDevice, st));
   }
-  if (c.add_embed_text) {
-    const int xd = c.cross_attention_dim;
-    if (dev_alloc(h, &h->pool_kv_W, (size_t)2 * xd * xd, false)) return -2;
-    if (dev_alloc(h, &h->pool_kv_b, (size_t)2 * xd, false)) return -2;
-    NS_CHECK_CUDA(cudaMemcpyAsync(h->pool_kv_W, h->W("add_embedding.pool.k_proj.weight"), (size_t)xd * xd * 4, cudaMemcpyDeviceToDevice, st));
-    NS_CHECK_CUDA(cudaMemcpyAsync(h->pool_kv_W + (size_t)xd * xd, h->W("add_embedding.pool.v_proj.weight"), (size_t)xd * xd * 4, cudaMemcpyDeviceToDevice, st));
-    NS_CHECK_CUDA(cudaMemcpyAsync(h->pool_kv_b, h->W("add_embedding.pool.k_proj.bias"), (size_t)xd * 4, cudaMemcpyDeviceToDevice, st));
-    NS_CHECK_CUDA(cudaMemcpyAsync(h->pool_kv_b + xd, h->W("add_embedding.pool.v_proj.bias"), (size_t)xd * 4, cudaMemcpyDeviceToDevice, st));
-  }
+  if (c.add_embed_text)
+    if ((rc = concat_pool_kv(h->mem, h->weights, "add_embedding.pool", c.cross_attention_dim, h->pool_kv, st))) return rc;
   NS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -515,45 +404,16 @@ __global__ void nearest_index_kernel(int t_in, int t_out, int* idx) {
   idx[i] = s;
 }
 
-struct Builder {
+struct Builder : ProgramBuilder {
   ns2vc_unet* h;
-  Arena ar;
-  int B, T, S;
-  std::vector<Launch>* out;
-  bool dry;
-  bool taps = false;
-  int err = 0;
+  Builder(ns2vc_unet* h_, void* ws, int B_, std::vector<Launch>* out_)
+      : ProgramBuilder{Arena{(uint8_t*)ws, 0}, B_, ws == nullptr, h_->simt, out_}, h(h_) {}
 
-  SplitBuf split(int Tn, int C) {
-    SplitBuf s{}; s.T = Tn; s.C = C; s.ld = pad_to(C, 8);
-    s.hi = ar.get<__nv_bfloat16>((size_t)B * Tn * s.ld);
-    s.lo = ar.get<__nv_bfloat16>((size_t)B * Tn * s.ld);
-    return s;
-  }
-  // view of a (larger) scratch split as [B, Tn, C]
-  static SplitBuf view(const SplitBuf& base, int Tn, int C) {
-    SplitBuf s = base; s.T = Tn; s.C = C; s.ld = pad_to(C, 8); return s;
-  }
-  GemmOp gemm_base(const PackedB& w, int T_out) {
-    GemmOp g; memset(&g, 0, sizeof(g));
-    g.B = B; g.T_out = T_out;
-    g.w_hi = w.hi; g.w_lo = w.lo; g.w_f32 = w.f32; g.N = w.Npad; g.n_valid = w.n_logical;
-    g.f16_col0 = 0x7fffffff;
-    g.ksplit = 1;
-    return g;
-  }
-  int add_src(GemmOp& g, const SplitBuf& s) { g.src[g.nsrc] = s; return g.nsrc++; }
-  void seg(GemmOp& g, int src, int c0, int nch, int tap) {
-    GSeg& s = g.seg[g.nseg++];
-    s.src = src; s.c0 = c0; s.nkb = nkb_of(nch); s.tap = tap;
-    g.nkb_total += s.nkb;
-  }
   void conv3(GemmOp& g, const SplitBuf& s) {           // k=3, stride 1, pad 1 over one split source
     const int i = add_src(g, s);
     for (int j = 0; j < 3; ++j) seg(g, i, 0, s.C, j - 1);
   }
-  void emit_gemm(GemmOp& g, const PackedB& w, int patch = 0) {
-    Launch l; l.kind = Launch::GEMM; l.patch = patch;
+  void emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
     if (g.xmode && h->ksplit) {
       // few-tile, deep-K launches (the two coarsest levels at B = 8: 64 tiles of 24-64 k-blocks each): two CTAs per tile, each
       // half of the channel blocks; worth it when both halves still have a few panels and all pairs are resident at once
@@ -562,14 +422,8 @@ struct Builder {
       for (int i = 0; i < g.nxs; ++i) panels += g.xs[i].ncb;
       if (2 * tiles <= gemm_sm_count() && panels >= 8) g.ksplit = 2;
     }
-    if (!dry) {
-      if (g.nkb_total != w.nkb) { fprintf(stderr, "ns2vc: internal K mismatch %d vs %d\n", g.nkb_total, w.nkb); abort(); }
-      plan_gemm(g);
-      if (!h->simt) { int rc = encode_tmaps(g); if (rc) err = rc; }
-    }
-    l.gemm = g;
+    Launch& l = ProgramBuilder::emit_gemm(g, w, in);
     if (g.pre_film || (g.flags & EPI_ROWBIAS)) l.reads_film = 1;
-    out->push_back(l);
   }
   // ---- panel mode (GemmOp::xmode): raw split sources normalised inside the GEMM
   void xseg(GemmOp& g, int src, int c0, int nch, int ntap, int kb0, int kb_stride, int xf, int aff_c0) {
@@ -601,11 +455,10 @@ struct Builder {
     // pageable source: the runtime stages it before returning, so the vector may die with the builder
     return cudaMemcpyAsync(aff_dev, aff_host.data(), aff_host.size() * sizeof(PrepOp), cudaMemcpyHostToDevice, st) == cudaSuccess ? 0 : -2;
   }
-  void push(const Launch& l) { out->push_back(l); }
   void emit_prep(const float* s1, int C1, const float* s2, int C2, int T_src, int T_dst, int mode, const float* scale,
                  const float* shift, const SplitBuf& o, const SplitBuf* raw = nullptr, int row_mul = 1, int row_add = 0,
-                 const int* rowmap = nullptr, int patch = 0) {
-    Launch l; l.kind = Launch::PREP; l.patch = patch;
+                 const int* rowmap = nullptr, Launch::Input in = Launch::NONE) {
+    Launch l; l.kind = Launch::PREP; l.input = in;
     PrepOp& p = l.prep; memset(&p, 0, sizeof(p));
     p.src1 = s1; p.ld1 = C1; p.C1 = C1; p.src2 = s2; p.ld2 = C2; p.C2 = C2; p.B = B; p.T_src = T_src; p.T_dst = T_dst;
     p.row_mul = row_mul; p.row_add = row_add; p.rowmap = rowmap; p.mode = mode; p.scale = scale; p.shift = shift; p.out = o;
@@ -624,19 +477,10 @@ struct Builder {
     p.gn.gamma = gamma; p.gn.beta = beta; p.gn.film = film; p.gn.film_ld = film_ld; p.gn.G = h->cfg.norm_num_groups; p.gn.eps = eps;
     p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / p.gn.G));
   }
-  void emit_ln_split(const float* x, int ld, int M, int C, const float* gamma, const float* beta, const SplitBuf& o) {
-    Launch l; l.kind = Launch::LN_SPLIT; l.a = x; l.i0 = ld; l.i1 = M; l.i2 = C; l.f0 = 1e-5f; l.b = gamma; l.c = beta; l.split = o;
-    push(l);
-  }
-  void emit_tap(const std::string& name, const float* src, int level, int C, int Tl) {
-    if (!dry && taps) {
-      Launch l; l.kind = Launch::TAP; l.a = src; l.i0 = B * Tl * C; l.tap_index = (int)h->tap_names.size(); push(l);
-      h->tap_names.push_back(name); h->tap_level.push_back(level); h->tap_ch.push_back(C);
-    }
-  }
 };
 
-int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_out, cudaStream_t st = nullptr) {
+// Builds the programs of (B, T, S, ws) into *prog, or (ws == nullptr) sizes their workspace into *bytes_out.
+int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_out, Program* prog, cudaStream_t st = nullptr) {
   const ns2vc_unet_cfg& c = h->cfg;
   const bool dry = (ws == nullptr);
   const int nlev = c.n_levels;
@@ -647,7 +491,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   for (int l = 0; l < nlev; ++l) Tl[l] = level_len(T, l);
   NS_REQUIRE(Tl[nlev - 1] >= 1 && T >= 1 && B >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
 
-  std::vector<Launch> cond, fwd;
+  Program pg;
   if (!dry) {
     // building a program allocates its static tables and copies them to the device: illegal under stream capture (header contract:
     // run a new shape once eagerly first)
@@ -656,9 +500,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
       set_error("the first call for a new (B=%d, T=%d, S=%d, workspace) builds its launch program and must not run under stream capture", B, T, S);
       return -1;
     }
-    h->tap_names.clear(); h->tap_level.clear(); h->tap_ch.clear();
   }
-  Builder bld{h, Arena{(uint8_t*)ws, 0}, B, T, S, &cond, dry};
+  Builder bld(h, ws, B, &pg.prog_cond);
   Arena& ar = bld.ar;
   {
     const int n_aff = 2 * (int)h->resnets.size() + (int)h->xformers.size() + 2;
@@ -685,12 +528,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   // ---- conditioning scratch
   SplitBuf s_content = (Cc > 0) ? bld.split(T, Cc) : SplitBuf{};
   SplitBuf s_prompt = bld.split(S, xd);
-  float* pn = ar.get<float>((size_t)B * S * xd);
-  float* ptok = ar.get<float>((size_t)B * (S + 1) * xd);
-  float* pq = ar.get<float>((size_t)B * xd);
-  float* pkv = ar.get<float>((size_t)B * (S + 1) * 2 * xd);
-  float* ppool = ar.get<float>((size_t)B * xd);
-  float* pproj = ar.get<float>((size_t)B * ted);
+  TextTimeEmbedding tte;
+  tte.reserve(ar, B, S, xd, ted);
 
   // fp16 softmax weights (one P x [V_hi | V_lo] MMA per k-step) only where enough keys average their 2^-12 rounding out: over a few
   // dozen keys (short prompts, the coarsest levels of short utterances) the weights are a bf16 hi/lo split - those launches are
@@ -700,43 +539,26 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
 
   // ================= conditioning program =================
   if (Cc > 0) {
-    { Launch l; l.kind = Launch::NCT2SPLIT; l.patch = 4; l.i0 = Cc; l.i1 = T; l.split = s_content; cond.push_back(l); }
+    { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::CONTENT; l.i0 = Cc; l.i1 = T; l.split = s_content; bld.out->push_back(l); }
     GemmOp g = bld.gemm_base(h->convin_content, T);
     bld.conv3(g, s_content);
-    g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->W("conv_in.bias"); g.out = P; g.out_ld = c0;
+    g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W("conv_in.bias"); g.out = P; g.out_ld = c0;
     bld.emit_gemm(g, h->convin_content);
   }
-  { Launch l; l.kind = Launch::MASKBIAS; l.patch = 6; l.i0 = B * S; l.o = maskbias; cond.push_back(l); }
+  { Launch l; l.kind = Launch::MASKBIAS; l.input = Launch::MASK; l.i0 = B * S; l.o = maskbias; bld.out->push_back(l); }
   if (h->kv_total > 0) {
-    bld.emit_prep(nullptr, xd, nullptr, 0, S, S, PREP_RAW, nullptr, nullptr, s_prompt, nullptr, 1, 0, nullptr, 5);
-    GemmOp g = bld.gemm_base(h->kv_all, S);
-    const int i = bld.add_src(g, s_prompt);
-    bld.seg(g, i, 0, xd, 0);
+    bld.emit_prep(nullptr, xd, nullptr, 0, S, S, PREP_RAW, nullptr, nullptr, s_prompt, nullptr, 1, 0, nullptr, Launch::PROMPT);
+    GemmOp g = bld.lin(h->kv_all, s_prompt, S);
     g.flags = EPI_OUT_F32 | EPI_OUT_SPLIT; g.out = kvc; g.out_ld = h->kv_total;
     g.out_hi = kvs.hi; g.out_lo = kvs.lo; g.out_split_ld = kvs.ld;
     if (p16(S)) g.f16_col0 = h->k_total;                    // V columns as fp16 hi/lo (attention v2: fp16 softmax weights x fp16 V)
     bld.emit_gemm(g, h->kv_all);
   }
-  if (c.add_embed_text) {
-    // TextTimeEmbedding (embeddings.py:421-434): LN -> AttentionPooling -> Linear -> LN
-    { Launch l; l.kind = Launch::LN_APPLY; l.patch = 5; l.i0 = xd; l.i1 = B * S; l.i2 = xd; l.f0 = 1e-5f;
-      l.b = h->W("add_embedding.norm1.weight"); l.c = h->W("add_embedding.norm1.bias"); l.o = pn; l.i3 = xd; cond.push_back(l); }
-    { Launch l; l.kind = Launch::POOL_CLS; l.a = pn; l.b = h->W("add_embedding.pool.positional_embedding"); l.i0 = S; l.i1 = xd; l.o = ptok; cond.push_back(l); }
-    { Launch l; l.kind = Launch::LINEAR; LinOp& o = l.lin; memset(&o, 0, sizeof(o));
-      o.x = ptok; o.x_ld = (S + 1) * xd; o.M = B; o.K = xd; o.W = h->W("add_embedding.pool.q_proj.weight"); o.bias = h->W("add_embedding.pool.q_proj.bias");
-      o.N = xd; o.out = pq; o.out_ld = xd; cond.push_back(l); }
-    { Launch l; l.kind = Launch::LINEAR; LinOp& o = l.lin; memset(&o, 0, sizeof(o));
-      o.x = ptok; o.x_ld = xd; o.M = B * (S + 1); o.K = xd; o.W = h->pool_kv_W; o.bias = h->pool_kv_b; o.N = 2 * xd; o.out = pkv; o.out_ld = 2 * xd; cond.push_back(l); }
-    { Launch l; l.kind = Launch::POOL_ATT; l.a = pq; l.b = pkv; l.i0 = S + 1; l.i1 = xd; l.i2 = c.add_embed_heads; l.o = ppool; cond.push_back(l); }
-    { Launch l; l.kind = Launch::LINEAR; LinOp& o = l.lin; memset(&o, 0, sizeof(o));
-      o.x = ppool; o.x_ld = xd; o.M = B; o.K = xd; o.W = h->W("add_embedding.proj.weight"); o.bias = h->W("add_embedding.proj.bias"); o.N = ted; o.out = pproj; o.out_ld = ted; cond.push_back(l); }
-    { Launch l; l.kind = Launch::LN_APPLY; l.a = pproj; l.i0 = ted; l.i1 = B; l.i2 = ted; l.f0 = 1e-5f;
-      l.b = h->W("add_embedding.norm2.weight"); l.c = h->W("add_embedding.norm2.bias"); l.o = aug; l.i3 = ted; cond.push_back(l); }
-  }
+  if (c.add_embed_text)   // TextTimeEmbedding of the prompt (embeddings.py:421-434)
+    tte.emit(bld, h->weights, "add_embedding", nullptr, Launch::PROMPT, S, xd, ted, c.add_embed_heads, Launch::POOL_ATT, h->pool_kv, aug);
 
   // ================= forward program =================
-  bld.out = &fwd;
-  bld.taps = true;
+  bld.out = &pg.prog_fwd;
   // per-step small buffers
   SplitBuf s_xin = bld.split(T, Cl);
   float* temb1 = ar.get<float>((size_t)B * ted);
@@ -755,7 +577,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   auto new_stats = [&](int C) { double* p = stat_arena ? stat_arena + stat_used : nullptr; stat_used += (size_t)2 * B * C; return p; };
   auto new_rowstats = [&](size_t nrows) { double* p = stat_arena ? stat_arena + stat_used : nullptr; stat_used += 2 * nrows; return p; };
   auto with_stats = [&](GemmOp& g, double* st_, int C) { g.flags |= EPI_STATS; g.stat_sum = st_; g.stat_sq = st_ ? st_ + (size_t)B * C : nullptr; };
-  { Launch l; l.kind = Launch::MEMSET; l.mem = stat_arena; l.mem_bytes = stat_doubles * sizeof(double); fwd.push_back(l); }
+  bld.emit_memset(stat_arena, stat_doubles * sizeof(double));
   // activation buffers
   size_t max_act = (size_t)B * T * c0, max_cat = 0, max_ff = 1, max_qkv = 1;
   for (auto& o : h->plan) {
@@ -781,16 +603,17 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   const SplitBuf SP_LN = scratch_split(max_act);     // raw (un-normalised) split of the transformer's residual stream (folded LayerNorms)
 
   // entry: x -> split tokens, time path, conv_in
-  { Launch l; l.kind = Launch::NCT2SPLIT; l.patch = 1; l.i0 = Cl; l.i1 = T; l.split = s_xin; fwd.push_back(l); }
-  { Launch l; l.kind = Launch::LINEAR; l.patch = 2; LinOp& o = l.lin; memset(&o, 0, sizeof(o));
-    o.x = nullptr; o.x_ld = 1; o.M = B; o.K = c0; o.W = h->W("time_embedding.linear_1.weight"); o.bias = h->W("time_embedding.linear_1.bias");
-    o.N = ted; o.out = temb1; o.out_ld = ted; o.in_mode = LIN_SINUSOID; o.flip_sin_to_cos = c.flip_sin_to_cos; o.freq_shift = c.freq_shift; o.out_silu = 1; l.time_path = 1; fwd.push_back(l); }
-  { Launch l; l.kind = Launch::LINEAR; LinOp& o = l.lin; memset(&o, 0, sizeof(o));
-    o.x = temb1; o.x_ld = ted; o.M = B; o.K = ted; o.W = h->W("time_embedding.linear_2.weight"); o.bias = h->W("time_embedding.linear_2.bias");
-    o.N = ted; o.out = emb; o.out_ld = ted; if (c.add_embed_text) { o.add = aug; o.add_ld = ted; } l.time_path = 1; fwd.push_back(l); }
+  { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::X; l.i0 = Cl; l.i1 = T; l.split = s_xin; bld.out->push_back(l); }
+  { LinOp o = linear_op(nullptr, 1, B, c0, h->weights.W("time_embedding.linear_1.weight"), h->weights.W("time_embedding.linear_1.bias"), ted, temb1, ted);
+    o.in_mode = LIN_SINUSOID; o.flip_sin_to_cos = c.flip_sin_to_cos; o.freq_shift = c.freq_shift; o.out_silu = 1;
+    bld.emit_linear(o, Launch::T, 1); }
+  { LinOp o = linear_op(temb1, ted, B, ted, h->weights.W("time_embedding.linear_2.weight"), h->weights.W("time_embedding.linear_2.bias"), ted, emb, ted);
+    if (c.add_embed_text) { o.add = aug; o.add_ld = ted; }
+    bld.emit_linear(o, Launch::NONE, 1); }
   if (h->film_total > 0) {
-    Launch l; l.kind = Launch::LINEAR; LinOp& o = l.lin; memset(&o, 0, sizeof(o));
-    o.x = emb; o.x_ld = ted; o.M = B; o.K = ted; o.W = h->film_W; o.bias = h->film_b; o.N = h->film_total; o.out = film; o.out_ld = h->film_total; o.in_mode = LIN_SILU; l.time_path = 1; fwd.push_back(l);
+    LinOp o = linear_op(emb, ted, B, ted, h->film_W, h->film_b, h->film_total, film, h->film_total);
+    o.in_mode = LIN_SILU;
+    bld.emit_linear(o, Launch::NONE, 1);
   }
 
   // An activation that leaves a block: fp32 token-major tensor, its raw bf16 hi/lo split (the A operand of the panel-mode
@@ -823,13 +646,13 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
     GemmOp g = bld.gemm_base(h->convin_lat, T);
     bld.conv3(g, s_xin);
     if (Cc > 0) { g.flags |= EPI_RESIDUAL; g.res = P; g.res_ld = c0; }
-    else { g.flags |= EPI_BIAS; g.bias = h->W("conv_in.bias"); }
+    else { g.flags |= EPI_BIAS; g.bias = h->weights.W("conv_in.bias"); }
     emits_block_out(g, o);
     o.st = new_stats(c0);
     with_stats(g, o.st, c0);
     bld.emit_gemm(g, h->convin_lat);
     cur = o;
-    bld.emit_tap("conv_in", cur.p, 0, c0, T);
+    bld.emit_tap(pg.taps, "conv_in", cur.p, 0, c0, T);
   }
   Act cat2;                                              // pending concat source
   size_t ri = 0, xi = 0, si = 0;
@@ -857,8 +680,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             bld.xseg(g, i0, 0, s.c1, 3, 0, ni, 1, 0);
             if (s.c2) { const int i1 = bld.add_src(g, cat2.sp); bld.xseg(g, i1, 0, s.c2, 3, n1, ni, 1, s.c1); }
             g.pre = bld.affine_desc(cur.st, s.c1, s.c2 ? cat2.st : nullptr, s.c2, TL, PREP_AFFINE_SILU, c.norm_eps,
-                                    h->W(s.p + ".norm1.weight"), h->W(s.p + ".norm1.bias"), 0);
-            g.flags = EPI_BIAS | EPI_OUT_SPLIT; g.bias = h->W(s.p + ".conv1.bias");
+                                    h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), 0);
+            g.flags = EPI_BIAS | EPI_OUT_SPLIT; g.bias = h->weights.W(s.p + ".conv1.bias");
             if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
             g.out_hi = a_h.hi; g.out_lo = a_h.lo; g.out_split_ld = a_h.ld;
             with_stats(g, h1_st, s.cout);
@@ -875,8 +698,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             } else { g.flags |= EPI_RESIDUAL; g.res = s1; g.res_ld = s.c1; }
             const int j0 = bld.add_src(g, a_h);
             bld.xseg(g, j0, 0, s.cout, 3, 0, no, 1, 0);
-            g.pre = bld.affine_desc(h1_st, s.cout, nullptr, 0, TL, PREP_AFFINE_SILU, c.norm_eps, h->W(s.p + ".norm2.weight"),
-                                    h->W(s.p + ".norm2.bias"), h->film_total);
+            g.pre = bld.affine_desc(h1_st, s.cout, nullptr, 0, TL, PREP_AFFINE_SILU, c.norm_eps, h->weights.W(s.p + ".norm2.weight"),
+                                    h->weights.W(s.p + ".norm2.bias"), h->film_total);
             g.pre_film = c.time_scale_shift ? film + s.film_off : nullptr;
             emits_block_out(g, outp);
             with_stats(g, outp.st, s.cout);
@@ -885,19 +708,19 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         } else {
           const SplitBuf a_in = Builder::view(SP_A, TL, s.cin), a_raw = Builder::view(SP_R, TL, s.cin);
           bld.emit_prep_gn(s1, s.c1, cur.st, s2, s.c2, s.c2 ? cat2.st : nullptr, TL, PREP_AFFINE_SILU, c.norm_eps,
-                           h->W(s.p + ".norm1.weight"), h->W(s.p + ".norm1.bias"), nullptr, 0, a_in, s.shortcut ? &a_raw : nullptr);
+                           h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), nullptr, 0, a_in, s.shortcut ? &a_raw : nullptr);
           {
             GemmOp g = bld.gemm_base(s.conv1, TL);
             bld.conv3(g, a_in);
-            g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->W(s.p + ".conv1.bias");
+            g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(s.p + ".conv1.bias");
             if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
             g.out = H1; g.out_ld = s.cout;
             with_stats(g, h1_st, s.cout);
             bld.emit_gemm(g, s.conv1);
           }
           // norm2 (+FiLM scale/shift) + SiLU (reference resnet.py:602-612)
-          bld.emit_prep_gn(H1, s.cout, h1_st, nullptr, 0, nullptr, TL, PREP_AFFINE_SILU, c.norm_eps, h->W(s.p + ".norm2.weight"),
-                           h->W(s.p + ".norm2.bias"), c.time_scale_shift ? film + s.film_off : nullptr, h->film_total, a_h);
+          bld.emit_prep_gn(H1, s.cout, h1_st, nullptr, 0, nullptr, TL, PREP_AFFINE_SILU, c.norm_eps, h->weights.W(s.p + ".norm2.weight"),
+                           h->weights.W(s.p + ".norm2.bias"), c.time_scale_shift ? film + s.film_off : nullptr, h->film_total, a_h);
           {
             GemmOp g = bld.gemm_base(s.conv2, TL);
             bld.conv3(g, a_h);
@@ -910,7 +733,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           }
         }
         cur = outp; cat2 = Act{};
-        bld.emit_tap(s.p, cur.p, o.level, cur.c, TL);
+        bld.emit_tap(pg.taps, s.p, cur.p, o.level, cur.c, TL);
         break;
       }
       case PlanOp::XFORMER: {
@@ -919,9 +742,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         const std::string b = x.p + ".transformer_blocks.0";
         const SplitBuf sx = Builder::view(SP_X, TL, C), satt = Builder::view(SP_ATT, TL, C), sff = Builder::view(SP_FF, TL, 4 * C),
                        sh2 = Builder::view(SP_H, TL, C);
-        auto lin = [&](const PackedB& w, const SplitBuf& in, int nch) { GemmOp g = bld.gemm_base(w, TL); const int i = bld.add_src(g, in); bld.seg(g, i, 0, nch, 0); return g; };
         const bool xin = xf_ok(C, 0);                        // GroupNorm(eps 1e-6) of the block input applied inside proj_in
-        if (!xin) bld.emit_prep_gn(cur.p, C, cur.st, nullptr, 0, nullptr, TL, PREP_AFFINE, 1e-6f, h->W(x.p + ".norm.weight"), h->W(x.p + ".norm.bias"), nullptr, 0, sx);
+        if (!xin) bld.emit_prep_gn(cur.p, C, cur.st, nullptr, 0, nullptr, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), nullptr, 0, sx);
         // Folded LayerNorms: the producer of each LN input also emits its raw bf16 split and the per-row sums; the consumer
         // GEMM runs on the raw split with gamma folded into its weights and applies mean / rstd in its epilogue:
         //   LN(x) W^T = rstd * (x (gamma*W)^T - mean * g) + (beta W^T + bias),   g[n] = sum_c gamma_c W[n,c]
@@ -932,53 +754,51 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         auto emits_ln_input = [&](GemmOp& g, double* rs) { g.flags |= EPI_OUT_SPLIT | EPI_ROWSTATS; g.out_hi = sln.hi; g.out_lo = sln.lo; g.out_split_ld = sln.ld; g.row_stats = rs; };
         auto consumes_ln = [&](GemmOp& g, const double* rs, const float* gv, const float* bf) {
           g.flags |= EPI_LNFOLD | EPI_BIAS; g.ln_stats = rs; g.ln_g = gv; g.bias = bf; g.ln_C = C; g.ln_eps = 1e-5f; };
-        { GemmOp g = xin ? bld.gemm_base(x.proj_in, TL) : lin(x.proj_in, sx, C);
+        { GemmOp g = xin ? bld.gemm_base(x.proj_in, TL) : bld.lin(x.proj_in, sx, TL);
           if (xin) {
             const int i0 = bld.add_src(g, cur.sp);
             bld.xseg(g, i0, 0, C, 1, 0, 0, 1, 0);
-            g.pre = bld.affine_desc(cur.st, C, nullptr, 0, TL, PREP_AFFINE, 1e-6f, h->W(x.p + ".norm.weight"), h->W(x.p + ".norm.bias"), 0);
+            g.pre = bld.affine_desc(cur.st, C, nullptr, 0, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), 0);
           }
-          g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->W(x.p + ".proj_in.bias"); g.out = T0; g.out_ld = C;
+          g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(x.p + ".proj_in.bias"); g.out = T0; g.out_ld = C;
           if (fold) emits_ln_input(g, rs1);
           bld.emit_gemm(g, x.proj_in); }
-        if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->W(b + ".norm1.weight"), h->W(b + ".norm1.bias"), sx);
+        if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->weights.W(b + ".norm1.weight"), h->weights.W(b + ".norm1.bias"), sx);
         const SplitBuf& sn = fold ? sln : sx;                // A operand of the LayerNorm consumers
         const bool av2 = !h->simt && attention_v2_supported(dh, TL, false) && attention_v2_supported(dh, S, true);
         const SplitBuf sqkv = Builder::view(SP_QKV, TL, 3 * C), sq2 = Builder::view(SP_QKV, TL, C);
-        { GemmOp g = lin(x.qkv, sn, C);
+        { GemmOp g = bld.lin(x.qkv, sn, TL);
           if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sqkv.hi; g.out_lo = sqkv.lo; g.out_split_ld = sqkv.ld;
                      if (p16(TL)) g.f16_col0 = 2 * C; }
           else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = 3 * C; }
           if (fold) consumes_ln(g, rs1, x.g_qkv, x.bf_qkv);
           bld.emit_gemm(g, x.qkv); }
-        { Launch l; l.kind = Launch::ATTN; AttnOp& a = l.attn; memset(&a, 0, sizeof(a));
+        { AttnOp a; memset(&a, 0, sizeof(a));
           a.q = QKV; a.q_ld = 3 * C; a.k = QKV + C; a.k_ld = 3 * C; a.v = QKV + 2 * C; a.v_ld = 3 * C;
           a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
           a.B = B; a.H = H; a.Tq = TL; a.Tk = TL; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
-          if (av2) { a.v2 = 1; a.p_split = p16(TL) ? 0 : 1; a.qs = sqkv; a.ks = sqkv; a.vs = sqkv; a.q_c0 = 0; a.k_c0 = C; a.v_c0 = 2 * C;
-                     if (!dry) { int rc = encode_attn_tmaps(a); if (rc) bld.err = rc; } }
-          bld.push(l); }
-        { GemmOp g = lin(x.out1, satt, C); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->W(b + ".attn1.to_out.0.bias"); g.res = T0; g.res_ld = C; g.out = T1; g.out_ld = C;
+          if (av2) { a.v2 = 1; a.p_split = p16(TL) ? 0 : 1; a.qs = sqkv; a.ks = sqkv; a.vs = sqkv; a.q_c0 = 0; a.k_c0 = C; a.v_c0 = 2 * C; }
+          bld.emit_attention(a); }
+        { GemmOp g = bld.lin(x.out1, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn1.to_out.0.bias"); g.res = T0; g.res_ld = C; g.out = T1; g.out_ld = C;
           if (fold) emits_ln_input(g, rs2);
           bld.emit_gemm(g, x.out1); }
-        if (!fold) bld.emit_ln_split(T1, C, (int)rows, C, h->W(b + ".norm2.weight"), h->W(b + ".norm2.bias"), sx);
-        { GemmOp g = lin(x.q2, sn, C);
+        if (!fold) bld.emit_ln_split(T1, C, (int)rows, C, h->weights.W(b + ".norm2.weight"), h->weights.W(b + ".norm2.bias"), sx);
+        { GemmOp g = bld.lin(x.q2, sn, TL);
           if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sq2.hi; g.out_lo = sq2.lo; g.out_split_ld = sq2.ld; }
           else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = C; }
           if (fold) consumes_ln(g, rs2, x.g_q2, x.bf_q2);
           bld.emit_gemm(g, x.q2); }
-        { Launch l; l.kind = Launch::ATTN; AttnOp& a = l.attn; memset(&a, 0, sizeof(a));
+        { AttnOp a; memset(&a, 0, sizeof(a));
           a.q = QKV; a.q_ld = C; a.k = kvc + x.kv_off; a.k_ld = h->kv_total; a.v = kvc + x.v_off; a.v_ld = h->kv_total; a.bias = maskbias;
           a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
-          a.B = B; a.H = H; a.Tq = TL; a.Tk = S; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh); l.i0 = 1 /*cross*/;
-          if (av2) { a.v2 = 1; a.p_split = p16(S) ? 0 : 1; a.qs = sq2; a.ks = kvs; a.vs = kvs; a.q_c0 = 0; a.k_c0 = x.kv_off; a.v_c0 = x.v_off;
-                     if (!dry) { int rc = encode_attn_tmaps(a); if (rc) bld.err = rc; } }
-          bld.push(l); }
-        { GemmOp g = lin(x.out2, satt, C); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->W(b + ".attn2.to_out.0.bias"); g.res = T1; g.res_ld = C; g.out = T0; g.out_ld = C;
+          a.B = B; a.H = H; a.Tq = TL; a.Tk = S; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
+          if (av2) { a.v2 = 1; a.p_split = p16(S) ? 0 : 1; a.qs = sq2; a.ks = kvs; a.vs = kvs; a.q_c0 = 0; a.k_c0 = x.kv_off; a.v_c0 = x.v_off; }
+          bld.emit_attention(a, Launch::MASK); }     // the key-padding bias comes from the call's mask (dropped without one)
+        { GemmOp g = bld.lin(x.out2, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn2.to_out.0.bias"); g.res = T1; g.res_ld = C; g.out = T0; g.out_ld = C;
           if (fold) emits_ln_input(g, rs3);
           bld.emit_gemm(g, x.out2); }
-        if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->W(b + ".norm3.weight"), h->W(b + ".norm3.bias"), sx);
-        { GemmOp g = lin(x.ff1, sn, C); g.flags = EPI_GEGLU | EPI_OUT_SPLIT; g.bias = h->W(b + ".ff.net.0.proj.bias");
+        if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->weights.W(b + ".norm3.weight"), h->weights.W(b + ".norm3.bias"), sx);
+        { GemmOp g = bld.lin(x.ff1, sn, TL); g.flags = EPI_GEGLU | EPI_OUT_SPLIT; g.bias = h->weights.W(b + ".ff.net.0.proj.bias");
           g.out_hi = sff.hi; g.out_lo = sff.lo; g.out_split_ld = sff.ld;
           if (fold) { consumes_ln(g, rs3, x.g_ff1, x.bf_ff1); g.flags &= ~EPI_BIAS; }   // GEGLU reads its (folded) biases through g.bias itself
           bld.emit_gemm(g, x.ff1); }
@@ -992,13 +812,13 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = x.bias_ff2p; g.res = cur.p; g.res_ld = C;
           emits_block_out(g, outp); with_stats(g, outp.st, C); bld.emit_gemm(g, x.ff2p);
         } else {
-          { GemmOp g = lin(x.ff2, sff, 4 * C); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_SPLIT; g.bias = h->W(b + ".ff.net.2.bias"); g.res = T0; g.res_ld = C;
+          { GemmOp g = bld.lin(x.ff2, sff, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_SPLIT; g.bias = h->weights.W(b + ".ff.net.2.bias"); g.res = T0; g.res_ld = C;
             g.out_hi = sh2.hi; g.out_lo = sh2.lo; g.out_split_ld = sh2.ld; bld.emit_gemm(g, x.ff2); }
-          { GemmOp g = lin(x.proj_out, sh2, C); g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = h->W(x.p + ".proj_out.bias"); g.res = cur.p; g.res_ld = C;
+          { GemmOp g = bld.lin(x.proj_out, sh2, TL); g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = h->weights.W(x.p + ".proj_out.bias"); g.res = cur.p; g.res_ld = C;
             emits_block_out(g, outp); with_stats(g, outp.st, C); bld.emit_gemm(g, x.proj_out); }
         }
         cur = outp;
-        bld.emit_tap(x.p, cur.p, o.level, C, TL);
+        bld.emit_tap(pg.taps, x.p, cur.p, o.level, C, TL);
         break;
       }
       case PlanOp::DOWN: {
@@ -1022,11 +842,11 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         GemmOp g = bld.gemm_base(s.w, TL);
         const int ie = bld.add_src(g, ev), io = bld.add_src(g, od);
         bld.seg(g, io, 0, s.c, -1); bld.seg(g, ie, 0, s.c, 0); bld.seg(g, io, 0, s.c, 0);
-        g.flags = EPI_BIAS; g.bias = h->W(s.p + ".conv.bias");
+        g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
         emits_block_out(g, outp); with_stats(g, outp.st, s.c);
         bld.emit_gemm(g, s.w);
         cur = outp;
-        bld.emit_tap(s.p, cur.p, o.level, s.c, TL);
+        bld.emit_tap(pg.taps, s.p, cur.p, o.level, s.c, TL);
         break;
       }
       case PlanOp::UP: {
@@ -1045,11 +865,11 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         outp.st = new_stats(s.c);
         GemmOp g = bld.gemm_base(s.w, TL);
         bld.conv3(g, up);
-        g.flags = EPI_BIAS; g.bias = h->W(s.p + ".conv.bias");
+        g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
         emits_block_out(g, outp); with_stats(g, outp.st, s.c);
         bld.emit_gemm(g, s.w);
         cur = outp;
-        bld.emit_tap(s.p, cur.p, o.level, s.c, TL);
+        bld.emit_tap(pg.taps, s.p, cur.p, o.level, s.c, TL);
         break;
       }
     }
@@ -1061,35 +881,33 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
     if (xf_ok(c0, 0)) {
       const int i0 = bld.add_src(g, cur.sp);
       bld.xseg(g, i0, 0, c0, 3, 0, nkb_of(c0), 1, 0);
-      g.pre = bld.affine_desc(cur.st, c0, nullptr, 0, T, PREP_AFFINE_SILU, c.norm_eps, h->W("conv_norm_out.weight"), h->W("conv_norm_out.bias"), 0);
+      g.pre = bld.affine_desc(cur.st, c0, nullptr, 0, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), 0);
     } else {
-      bld.emit_prep_gn(cur.p, c0, cur.st, nullptr, 0, nullptr, T, PREP_AFFINE_SILU, c.norm_eps, h->W("conv_norm_out.weight"), h->W("conv_norm_out.bias"), nullptr, 0, a_h);
+      bld.emit_prep_gn(cur.p, c0, cur.st, nullptr, 0, nullptr, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), nullptr, 0, a_h);
       bld.conv3(g, a_h);
     }
-    g.flags = EPI_BIAS | EPI_OUT_NCT; g.bias = h->W("conv_out.bias"); g.out = nullptr;
-    bld.emit_gemm(g, h->conv_out, 3);
+    g.flags = EPI_BIAS | EPI_OUT_NCT; g.bias = h->weights.W("conv_out.bias"); g.out = nullptr;
+    bld.emit_gemm(g, h->conv_out, Launch::OUT);
   }
   if (!bld.err && bld.upload_affine(st)) { set_error("affine descriptor upload failed"); return -2; }
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
-    h->prog_cond = std::move(cond);
-    h->prog_fwd = std::move(fwd);
-    h->tap_dst.assign(h->tap_names.size(), nullptr);
-    h->pB = B; h->pT = T; h->pS = S; h->pws = ws; h->cond_ready = false;
-    h->film_base = film; h->aug = aug;
+    pg.B = B; pg.T = T; pg.S = S; pg.ws = ws;
+    pg.film_base = film; pg.aug = aug;
+    *prog = std::move(pg);
   }
   return 0;
 }
 
-int run_program(ns2vc_unet* h, std::vector<Launch>& prog, const float* x, long long x_bstride, const float* t, float* out,
-                const float* content, long long content_bstride, const float* prompt, const uint8_t* mask, cudaStream_t st) {
+int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& prog, const float* x, long long x_bstride, const float* t,
+                float* out, const float* content, long long content_bstride, const float* prompt, const uint8_t* mask, cudaStream_t st) {
   int rc = 0, count = 0, gemm_idx = 0, attn_idx = 0;
   // Precomputed FiLM rows (ns2vc_unet_time_table): the timestep path of this forward is skipped and every reader is rebased.
   const float* film_ext = h->film_ext;
-  auto rebase = [&](const float* p) { return (film_ext && p) ? film_ext + (p - h->film_base) : p; };
-  for (size_t li = 0; li < prog.size(); ++li) {
-    Launch& l = prog[li];
+  auto rebase = [&](const float* p) { return (film_ext && p) ? film_ext + (p - pg.film_base) : p; };
+  const Runner run{h->simt, pg.B, &pg.taps, st};
+  for (const Launch& l : prog) {
     if (film_ext && l.time_path) continue;
     cudaEvent_t ev_a = nullptr, ev_b = nullptr;
     const bool prof = h->profiling && l.kind != Launch::TAP;
@@ -1097,77 +915,56 @@ int run_program(ns2vc_unet* h, std::vector<Launch>& prog, const float* x, long l
       cudaEventCreate(&ev_a); cudaEventCreate(&ev_b);
       cudaEventRecord(ev_a, st);
     }
+    unsigned long long* span = (h->span && count < h->span_cap) ? h->span + 2 * count : nullptr;
     switch (l.kind) {
       case Launch::GEMM: {
-        if (l.patch == 3 || h->trace || h->span || (film_ext && l.reads_film)) {
+        const bool to_out = l.input == Launch::OUT;
+        if (to_out || h->trace || h->span || (film_ext && l.reads_film)) {
           GemmOp g = l.gemm;
-          if (l.patch == 3) g.out = out;
+          if (to_out) g.out = out;
           if (film_ext && l.reads_film) {
             g.rowbias = rebase(g.rowbias);
             g.pre_film = rebase(g.pre_film);
           }
-          if (h->span && count < h->span_cap) g.span = h->span + 2 * count;
+          if (span) g.span = span;
           if (h->trace && gemm_idx < h->trace_cap) g.trace = h->trace + 32 * gemm_idx;
           ++gemm_idx;
-          rc = h->simt ? launch_gemm_simt(g, st) : launch_gemm_tc(g, st);
+          rc = run.gemm(g);
         } else {
-          rc = h->simt ? launch_gemm_simt(l.gemm, st) : launch_gemm_tc(l.gemm, st);
+          rc = run.gemm(l.gemm);
         }
         break;
       }
       case Launch::ATTN: {
         AttnOp a = l.attn;
-        if (l.i0 == 1 && !h->has_mask) a.bias = nullptr;
-        if (h->span && count < h->span_cap) a.span = h->span + 2 * count;
+        if (l.input == Launch::MASK && !pg.has_mask) a.bias = nullptr;
+        if (span) a.span = span;
         if (h->attn_trace && attn_idx < h->attn_trace_cap) a.trace = h->attn_trace + 2048 * attn_idx;
         ++attn_idx;
-        rc = (a.v2 && !h->simt) ? launch_attention_v2(a, st) : launch_attention(a, st, h->simt);
-        break;
-      }
-      case Launch::LN_SPLIT: rc = launch_ln_split(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.split, st, (h->span && count < h->span_cap) ? h->span + 2 * count : nullptr); break;
-      case Launch::LN_APPLY: {
-        const float* src = (l.patch == 5) ? prompt : l.a;
-        rc = launch_ln_apply(src, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.o, l.i3, st);
-        break;
-      }
-      case Launch::LINEAR: {
-        LinOp o = l.lin;
-        if (l.patch == 2) o.x = t;
-        rc = launch_small_linear(o, st);
+        rc = run.attn(a);
         break;
       }
       case Launch::NCT2SPLIT: {
-        const float* src = (l.patch == 1) ? x : content;
-        const long long bs = (l.patch == 1) ? x_bstride : content_bstride;
-        const bool warm = l.patch == 1 && film_ext != nullptr;
-        rc = launch_nct_to_split(src, bs, h->pB, l.i0, l.i1, l.split, st, warm ? film_ext : nullptr, warm ? (long long)h->pB * h->film_total * 4 : 0);
+        const bool fwd = l.input == Launch::X;
+        const bool warm = fwd && film_ext != nullptr;
+        rc = launch_nct_to_split(fwd ? x : content, fwd ? x_bstride : content_bstride, pg.B, l.i0, l.i1, l.split, st, warm ? film_ext : nullptr,
+                                 warm ? (long long)pg.B * h->film_total * 4 : 0);
         break;
       }
       case Launch::PREP: {
         PrepOp p = l.prep;
-        if (l.patch == 5) p.src1 = prompt;
+        if (l.input == Launch::PROMPT) p.src1 = prompt;
         if (film_ext && l.reads_film) p.gn.film = rebase(p.gn.film);
-        if (h->span && count < h->span_cap) p.span = h->span + 2 * count;
+        if (span) p.span = span;
         rc = launch_prep_split(p, st);
         break;
       }
-      case Launch::MEMSET: {
-        cudaError_t e = cudaMemsetAsync(l.mem, 0, l.mem_bytes, st);
-        if (e != cudaSuccess) { set_error("memset failed: %s", cudaGetErrorString(e)); rc = -2; }
-        break;
-      }
-      case Launch::POOL_CLS: rc = launch_pool_class_token(l.a, l.b, h->pB, l.i0, l.i1, l.o, st); break;
-      case Launch::POOL_ATT: rc = launch_pool_attend(l.a, l.b, h->pB, l.i0, l.i1, l.i2, l.o, st); break;
+      case Launch::POOL_ATT: rc = launch_pool_attend(l.a, l.b, pg.B, l.i0, l.i1, l.i2, l.o, st); break;
       case Launch::MASKBIAS:
         if (mask) rc = launch_mask_bias(mask, l.i0, l.o, st); else --count;
         break;
-      case Launch::TAP:
-        --count;
-        if (l.tap_index >= 0 && l.tap_index < (int)h->tap_dst.size() && h->tap_dst[l.tap_index]) {
-          cudaError_t e = cudaMemcpyAsync(h->tap_dst[l.tap_index], l.a, (size_t)l.i0 * sizeof(float), cudaMemcpyDeviceToDevice, st);
-          if (e != cudaSuccess) { set_error("tap copy failed: %s", cudaGetErrorString(e)); rc = -2; }
-        }
-        break;
+      case Launch::TAP: --count; rc = run.run(l); break;
+      default: rc = run.run(l, l.input == Launch::PROMPT ? prompt : l.input == Launch::T ? t : nullptr, span); break;
     }
     if (prof) {
       cudaEventRecord(ev_b, st);
@@ -1184,45 +981,38 @@ int run_program(ns2vc_unet* h, std::vector<Launch>& prog, const float* x, long l
   return 0;
 }
 
-void stash_active(ns2vc_unet* h) {
-  if (!h->pws) return;
-  ns2vc_unet::Stash s;
-  // programs of different shapes may share one workspace (the caller's grow-only scratch buffer): the conditioning a stashed
-  // program prepared is gone once another program has run there, so it must be prepared again when it comes back
-  s.pB = h->pB; s.pT = h->pT; s.pS = h->pS; s.pws = h->pws; s.has_mask = h->has_mask; s.cond_ready = false;
-  s.prog_cond = std::move(h->prog_cond); s.prog_fwd = std::move(h->prog_fwd); s.film_base = h->film_base; s.aug = h->aug;
-  s.tap_names = std::move(h->tap_names); s.tap_level = std::move(h->tap_level); s.tap_ch = std::move(h->tap_ch); s.tap_dst = std::move(h->tap_dst);
-  h->prog_cond.clear(); h->prog_fwd.clear(); h->tap_names.clear(); h->tap_level.clear(); h->tap_ch.clear(); h->tap_dst.clear();
-  h->pB = h->pT = h->pS = 0; h->pws = nullptr; h->cond_ready = false;
-  if (h->stash.size() >= 16) h->stash.erase(h->stash.begin());   // bounded: drop the oldest program (it owns no device memory: everything lives in its workspace)
-  h->stash.push_back(std::move(s));
-}
-
 void drop_all_programs(ns2vc_unet* h) {
-  h->stash.clear();
+  h->progs.clear();
+  h->active = -1;
   for (void* p : h->static_bufs) cudaFree(p);
   h->static_bufs.clear();
-  h->prog_cond.clear(); h->prog_fwd.clear();
-  h->pB = h->pT = h->pS = 0; h->pws = nullptr; h->cond_ready = false;
 }
 
-// Make the program for (B,T,S,ws) the active one; returns 1 if it already existed, 0 if built now.
+// Make the program for (B,T,S,ws) the active one, building it if it is not cached.
 int ensure_program(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st) {
   NS_REQUIRE(h->finalized, "ns2vc_unet_finalize() has not been called");
   NS_REQUIRE(ws != nullptr, "workspace is NULL");
-  if (h->pB == B && h->pT == T && h->pS == S && h->pws == ws) return 0;
-  stash_active(h);
-  for (size_t i = 0; i < h->stash.size(); ++i) {
-    ns2vc_unet::Stash& s = h->stash[i];
-    if (s.pB == B && s.pT == T && s.pS == S && s.pws == ws) {
-      h->pB = s.pB; h->pT = s.pT; h->pS = s.pS; h->pws = s.pws; h->has_mask = s.has_mask; h->cond_ready = s.cond_ready;
-      h->prog_cond = std::move(s.prog_cond); h->prog_fwd = std::move(s.prog_fwd); h->film_base = s.film_base; h->aug = s.aug;
-      h->tap_names = std::move(s.tap_names); h->tap_level = std::move(s.tap_level); h->tap_ch = std::move(s.tap_ch); h->tap_dst = std::move(s.tap_dst);
-      h->stash.erase(h->stash.begin() + i);
-      return 0;
-    }
+  auto is = [&](const Program& p) { return p.B == B && p.T == T && p.S == S && p.ws == ws; };
+  if (h->active >= 0) {
+    if (is(h->progs[h->active])) return 0;
+    // programs of different shapes may share one workspace (the caller's grow-only scratch buffer): the conditioning an inactive
+    // program prepared is gone once another program has run there, so it must be prepared again when it comes back
+    h->progs[h->active].cond_ready = false;
+    h->active = -1;
   }
-  return build_programs(h, B, T, S, ws, nullptr, st);
+  auto it = std::find_if(h->progs.begin(), h->progs.end(), is);
+  if (it != h->progs.end()) {
+    std::rotate(it, it + 1, h->progs.end());             // most recently active last
+  } else {
+    Program p;
+    const int rc = build_programs(h, B, T, S, ws, nullptr, &p, st);
+    if (rc) return rc;
+    // bounded: drop the least recently active program (it owns no device memory: everything lives in its workspace)
+    if (h->progs.size() > ns2vc_unet::kMaxInactive) h->progs.erase(h->progs.begin());
+    h->progs.push_back(std::move(p));
+  }
+  h->active = (int)h->progs.size() - 1;
+  return 0;
 }
 
 }  // namespace
@@ -1284,45 +1074,36 @@ int ns2vc_unet_create(const ns2vc_unet_cfg* cfg, ns2vc_unet** out) {
 
 void ns2vc_unet_destroy(ns2vc_unet* h) {
   if (!h) return;
-  for (auto& w : h->weights) if (w.d) cudaFree(w.d);
-  for (void* p : h->owned) cudaFree(p);
+  h->weights.release();
+  h->mem.release();
   drop_all_programs(h);
   delete h;
 }
 
-int ns2vc_unet_num_weights(const ns2vc_unet* h) { return h ? (int)h->weights.size() : -1; }
+int ns2vc_unet_num_weights(const ns2vc_unet* h) { return h ? h->weights.size() : -1; }
 
 int ns2vc_unet_weight_info(const ns2vc_unet* h, int i, const char** name, int64_t shape[4], int* ndim) {
-  NS_REQUIRE(h && i >= 0 && i < (int)h->weights.size(), "weight index %d out of range", i);
-  const WSlot& w = h->weights[i];
-  if (name) *name = w.name.c_str();
-  if (ndim) *ndim = (int)w.shape.size();
-  if (shape) for (size_t k = 0; k < w.shape.size() && k < 4; ++k) shape[k] = w.shape[k];
-  return 0;
+  NS_REQUIRE(h, "weight index %d out of range", i);
+  return h->weights.info(i, name, shape, ndim);
 }
 
 int ns2vc_unet_load_weight(ns2vc_unet* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream) {
   NS_REQUIRE(h && key && dptr, "null argument");
-  auto it = h->windex.find(key);
-  NS_REQUIRE(it != h->windex.end(), "Unexpected key in state_dict: %s", key);
-  WSlot& w = h->weights[it->second];
-  NS_REQUIRE(ndim == (int)w.shape.size(), "size mismatch for %s: expected %d dims, got %d", key, (int)w.shape.size(), ndim);
-  for (int k = 0; k < ndim; ++k) NS_REQUIRE(shape[k] == w.shape[k], "size mismatch for %s at dim %d: expected %lld, got %lld", key, k, (long long)w.shape[k], (long long)shape[k]);
-  if (!w.d) NS_CHECK_CUDA(cudaMalloc(&w.d, w.numel() * sizeof(float)));
-  NS_CHECK_CUDA(cudaMemcpyAsync(w.d, dptr, w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  w.loaded = true;
+  const int rc = h->weights.load(key, dptr, shape, ndim, (cudaStream_t)stream);
+  if (rc) return rc;
   h->finalized = false;
   return 0;
 }
 
 int ns2vc_unet_finalize(ns2vc_unet* h, ns2vc_stream stream) {
   NS_REQUIRE(h, "null handle");
-  for (auto& w : h->weights) NS_REQUIRE(w.loaded, "Missing key in state_dict: %s", w.name.c_str());
+  int rc = h->weights.require_all_loaded();
+  if (rc) return rc;
   // (re)pack: drop previous packed buffers
-  for (void* p : h->owned) cudaFree(p);
-  h->owned.clear(); h->resnets.clear(); h->xformers.clear(); h->resamplers.clear();
+  h->mem.release();
+  h->resnets.clear(); h->xformers.clear(); h->resamplers.clear();
   drop_all_programs(h);
-  int rc = pack_all(h, (cudaStream_t)stream);
+  rc = pack_all(h, (cudaStream_t)stream);
   if (rc) return rc;
   h->finalized = true;
   return 0;
@@ -1331,7 +1112,7 @@ int ns2vc_unet_finalize(ns2vc_unet* h, ns2vc_stream stream) {
 int ns2vc_unet_workspace_bytes(const ns2vc_unet* h, int B, int T, int S, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
   NS_REQUIRE(h->finalized, "ns2vc_unet_finalize() has not been called");
-  return build_programs(const_cast<ns2vc_unet*>(h), B, T, S, nullptr, bytes);
+  return build_programs(const_cast<ns2vc_unet*>(h), B, T, S, nullptr, bytes, nullptr);
 }
 
 int ns2vc_unet_prepare_cond(ns2vc_unet* h, const float* content, long long content_bstride, const float* prompt, const uint8_t* mask,
@@ -1341,10 +1122,11 @@ int ns2vc_unet_prepare_cond(ns2vc_unet* h, const float* content, long long conte
   if (rc) return rc;
   const int Cc = h->cfg.in_channels - h->cfg.latent_channels;
   NS_REQUIRE(Cc == 0 || content != nullptr, "content is NULL but the model has %d content channels", Cc);
-  h->has_mask = mask != nullptr;
-  rc = run_program(h, h->prog_cond, nullptr, 0, nullptr, nullptr, content, content_bstride, prompt, mask, (cudaStream_t)stream);
+  Program& pg = h->progs[h->active];
+  pg.has_mask = mask != nullptr;
+  rc = run_program(h, pg, pg.prog_cond, nullptr, 0, nullptr, nullptr, content, content_bstride, prompt, mask, (cudaStream_t)stream);
   if (rc) return rc;
-  h->cond_ready = true;
+  pg.cond_ready = true;
   return 0;
 }
 
@@ -1353,8 +1135,9 @@ int ns2vc_unet_forward(ns2vc_unet* h, const float* x, long long x_bstride, const
   NS_REQUIRE(h && x && t && out, "null argument");
   int rc0 = ensure_program(h, B, T, S, ws, (cudaStream_t)stream);
   if (rc0) return rc0;
-  NS_REQUIRE(h->cond_ready, "ns2vc_unet_prepare_cond() must be called with the same (B,T,S,workspace) before forward");
-  return run_program(h, h->prog_fwd, x, x_bstride, t, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
+  const Program& pg = h->progs[h->active];
+  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond() must be called with the same (B,T,S,workspace) before forward");
+  return run_program(h, pg, pg.prog_fwd, x, x_bstride, t, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int ns2vc_unet_film_width(const ns2vc_unet* h) { return h ? h->film_total : -1; }
@@ -1369,7 +1152,8 @@ int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float*
   NS_REQUIRE(n_rows > 0 && n_rows % B == 0, "time table: %d rows is not a multiple of the batch %d", n_rows, B);
   int rc = ensure_program(h, B, T, S, ws, (cudaStream_t)stream);
   if (rc) return rc;
-  NS_REQUIRE(h->cond_ready || !h->cfg.add_embed_text, "ns2vc_unet_prepare_cond() must precede ns2vc_unet_time_table() (the pooled prompt embedding is added to every row)");
+  const Program& pg = h->progs[h->active];
+  NS_REQUIRE(pg.cond_ready || !h->cfg.add_embed_text, "ns2vc_unet_prepare_cond() must precede ns2vc_unet_time_table() (the pooled prompt embedding is added to every row)");
   const ns2vc_unet_cfg& c = h->cfg;
   const int ted = h->ted, c0 = c.block_out_channels[0];
   float* film = table;
@@ -1379,12 +1163,12 @@ int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float*
   // reference embeddings.py:24-64, 157-218 (sinusoid -> linear_1 -> SiLU -> linear_2), unet_1d_condition.py:869-883 (+ aug_emb),
   // resnet.py:619-629 (time_emb_proj of SiLU(emb) for all 22 resnets at once)
   { LinOp o; memset(&o, 0, sizeof(o));
-    o.x = t_rows; o.x_ld = 1; o.M = n_rows; o.K = c0; o.W = h->W("time_embedding.linear_1.weight"); o.bias = h->W("time_embedding.linear_1.bias");
+    o.x = t_rows; o.x_ld = 1; o.M = n_rows; o.K = c0; o.W = h->weights.W("time_embedding.linear_1.weight"); o.bias = h->weights.W("time_embedding.linear_1.bias");
     o.N = ted; o.out = temb1; o.out_ld = ted; o.in_mode = LIN_SINUSOID; o.flip_sin_to_cos = c.flip_sin_to_cos; o.freq_shift = c.freq_shift; o.out_silu = 1;
     if ((rc = launch_small_linear(o, st))) return rc; }
   { LinOp o; memset(&o, 0, sizeof(o));
-    o.x = temb1; o.x_ld = ted; o.M = n_rows; o.K = ted; o.W = h->W("time_embedding.linear_2.weight"); o.bias = h->W("time_embedding.linear_2.bias");
-    o.N = ted; o.out = emb; o.out_ld = ted; if (c.add_embed_text) { o.add = h->aug; o.add_ld = ted; o.add_rows = B; }
+    o.x = temb1; o.x_ld = ted; o.M = n_rows; o.K = ted; o.W = h->weights.W("time_embedding.linear_2.weight"); o.bias = h->weights.W("time_embedding.linear_2.bias");
+    o.N = ted; o.out = emb; o.out_ld = ted; if (c.add_embed_text) { o.add = pg.aug; o.add_ld = ted; o.add_rows = B; }
     if ((rc = launch_small_linear(o, st))) return rc; }
   if (h->film_total > 0) {
     LinOp o; memset(&o, 0, sizeof(o));
@@ -1399,10 +1183,11 @@ int ns2vc_unet_forward_film(ns2vc_unet* h, const float* x, long long x_bstride, 
   NS_REQUIRE(h && x && film_rows && out, "null argument");
   int rc0 = ensure_program(h, B, T, S, ws, (cudaStream_t)stream);
   if (rc0) return rc0;
-  NS_REQUIRE(h->cond_ready, "ns2vc_unet_prepare_cond() must be called with the same (B,T,S,workspace) before forward");
+  const Program& pg = h->progs[h->active];
+  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond() must be called with the same (B,T,S,workspace) before forward");
   NS_REQUIRE(h->film_total > 0, "the model has no FiLM rows");
   h->film_ext = film_rows;
-  const int rc = run_program(h, h->prog_fwd, x, x_bstride, nullptr, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
+  const int rc = run_program(h, pg, pg.prog_fwd, x, x_bstride, nullptr, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
   h->film_ext = nullptr;
   return rc;
 }
@@ -1434,18 +1219,14 @@ int ns2vc_mask_bias(const uint8_t* mask, int n, float* bias, ns2vc_stream stream
   return launch_mask_bias(mask, n, bias, (cudaStream_t)stream);
 }
 
-int ns2vc_unet_num_taps(const ns2vc_unet* h) { return h ? (int)h->tap_names.size() : -1; }
+int ns2vc_unet_num_taps(const ns2vc_unet* h) { return h ? (h->active >= 0 ? h->progs[h->active].taps.size() : 0) : -1; }
 int ns2vc_unet_tap_info(const ns2vc_unet* h, int i, const char** name, int* level, int* channels) {
-  NS_REQUIRE(h && i >= 0 && i < (int)h->tap_names.size(), "tap index %d out of range", i);
-  if (name) *name = h->tap_names[i].c_str();
-  if (level) *level = h->tap_level[i];
-  if (channels) *channels = h->tap_ch[i];
-  return 0;
+  NS_REQUIRE(h && h->active >= 0, "tap index %d out of range", i);
+  return h->progs[h->active].taps.info(i, name, level, channels);
 }
 int ns2vc_unet_set_tap(ns2vc_unet* h, int i, float* dst) {
-  NS_REQUIRE(h && i >= 0 && i < (int)h->tap_dst.size(), "tap index %d out of range", i);
-  h->tap_dst[i] = dst;
-  return 0;
+  NS_REQUIRE(h && h->active >= 0, "tap index %d out of range", i);
+  return h->progs[h->active].taps.set(i, dst);
 }
 int ns2vc_unet_set_attn_trace(ns2vc_unet* h, unsigned long long* dbuf, int n_launches) {
   if (!h) return -1;
@@ -1463,9 +1244,9 @@ int ns2vc_unet_set_span_trace(ns2vc_unet* h, unsigned long long* dbuf, int n_lau
   return 0;
 }
 int ns2vc_unet_launch_kind(const ns2vc_unet* h, int i) {
-  if (!h || i < 0) return -1;
+  if (!h || i < 0 || h->active < 0) return -1;
   int c = 0;
-  for (auto& l : h->prog_fwd) {
+  for (auto& l : h->progs[h->active].prog_fwd) {
     if (l.kind == Launch::TAP) continue;
     if (c == i) return (int)l.kind;
     ++c;
@@ -1477,12 +1258,12 @@ int ns2vc_unet_set_profiling(ns2vc_unet* h, int on) {
   h->profiling = on != 0;
   return 0;
 }
-int ns2vc_profile_num_kinds(void) { return 11; }
-const char* ns2vc_profile_kind_name(int k) {
-  static const char* names[] = {"gemm_tc", "attention", "ln_split", "ln_apply", "small_linear", "nct_to_split",     // = Launch::Kind order
-                               "pool_class_token", "pool_attend", "mask_bias", "prep_split", "memset"};
-  return (k >= 0 && k < 11) ? names[k] : "";
-}
+// the denoiser's profiled kinds: every Launch::Kind before TAP (taps are copies, not kernels)
+static const char* const kKindNames[] = {"gemm_tc", "attention", "ln_split", "ln_apply", "small_linear", "nct_to_split",   // = Launch::Kind order
+                                         "pool_class_token", "pool_attend", "mask_bias", "prep_split", "memset"};
+static_assert(sizeof(kKindNames) / sizeof(kKindNames[0]) == Launch::TAP, "one profile name per Launch::Kind before TAP");
+int ns2vc_profile_num_kinds(void) { return Launch::TAP; }
+const char* ns2vc_profile_kind_name(int k) { return (k >= 0 && k < Launch::TAP) ? kKindNames[k] : ""; }
 int ns2vc_unet_profile_read(ns2vc_unet* h, int kind, double* ms_total, long long* launches) {
   NS_REQUIRE(h && ms_total && launches, "null argument");
   double ms = 0; long long n = 0;

@@ -1,0 +1,347 @@
+// Host-side machinery shared by the two engines (engine.cu: the denoiser, pre_engine.cu: the condition encoders): the weight
+// registry, owned device memory and weight packing, the launch record, the program-builder base, the runner of the launch
+// kinds both engines use, the taps, and the TextTimeEmbedding both engines contain.
+#pragma once
+#include "common.cuh"
+
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <unordered_map>
+#include <vector>
+
+namespace ns2vc {
+
+struct PackedB {
+  __nv_bfloat16* hi = nullptr;
+  __nv_bfloat16* lo = nullptr;
+  float* f32 = nullptr;
+  int Npad = 0, nkb = 0, n_logical = 0;
+};
+
+inline int pad_to(int v, int m) { return (v + m - 1) / m * m; }
+inline int nkb_of(int c) { return (c + 63) / 64; }
+
+struct Arena {           // bump allocator over the caller's workspace (or a dry run when base == nullptr)
+  uint8_t* base = nullptr;
+  size_t off = 0;
+  template <class T> T* get(size_t n) {
+    off = (off + 255) & ~(size_t)255;
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += n * sizeof(T);
+    return p;
+  }
+};
+
+// The reference state_dict: keys and shapes in registration order (the order the C-ABI lists them), each with an owned fp32 copy.
+struct WeightRegistry {
+  struct Slot {
+    std::string name;
+    std::vector<int64_t> shape;
+    float* d = nullptr;
+    bool loaded = false;
+    size_t numel() const { size_t n = 1; for (auto s : shape) n *= (size_t)s; return n; }
+  };
+  std::vector<Slot> slots;
+  std::unordered_map<std::string, int> index;
+
+  void add(const std::string& n, std::vector<int64_t> shape) {
+    index[n] = (int)slots.size();
+    Slot s; s.name = n; s.shape = std::move(shape);
+    slots.push_back(std::move(s));
+  }
+  void add_conv(const std::string& p, int co, int ci, int k) { add(p + ".weight", {co, ci, k}); add(p + ".bias", {co}); }
+  void add_lin(const std::string& p, int co, int ci, bool bias = true) { add(p + ".weight", {co, ci}); if (bias) add(p + ".bias", {co}); }
+  void add_norm(const std::string& p, int c) { add(p + ".weight", {c}); add(p + ".bias", {c}); }
+
+  const float* W(const std::string& n) const {
+    auto it = index.find(n);
+    return it == index.end() ? nullptr : slots[it->second].d;
+  }
+  int size() const { return (int)slots.size(); }
+
+  int load(const char* key, const float* dptr, const int64_t* shape, int ndim, cudaStream_t st) {
+    auto it = index.find(key);
+    NS_REQUIRE(it != index.end(), "Unexpected key in state_dict: %s", key);
+    Slot& w = slots[it->second];
+    NS_REQUIRE(ndim == (int)w.shape.size(), "size mismatch for %s: expected %d dims, got %d", key, (int)w.shape.size(), ndim);
+    for (int k = 0; k < ndim; ++k) NS_REQUIRE(shape[k] == w.shape[k], "size mismatch for %s at dim %d: expected %lld, got %lld", key, k, (long long)w.shape[k], (long long)shape[k]);
+    if (!w.d) NS_CHECK_CUDA(cudaMalloc(&w.d, w.numel() * sizeof(float)));
+    NS_CHECK_CUDA(cudaMemcpyAsync(w.d, dptr, w.numel() * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    w.loaded = true;
+    return 0;
+  }
+  int info(int i, const char** name, int64_t shape[4], int* ndim) const {
+    NS_REQUIRE(i >= 0 && i < size(), "weight index %d out of range", i);
+    const Slot& w = slots[i];
+    if (name) *name = w.name.c_str();
+    if (ndim) *ndim = (int)w.shape.size();
+    if (shape) for (size_t k = 0; k < w.shape.size() && k < 4; ++k) shape[k] = w.shape[k];
+    return 0;
+  }
+  int require_all_loaded() const {
+    for (auto& w : slots) NS_REQUIRE(w.loaded, "Missing key in state_dict: %s", w.name.c_str());
+    return 0;
+  }
+  void release() {
+    for (auto& w : slots) if (w.d) { cudaFree(w.d); w.d = nullptr; }
+  }
+};
+
+// Device memory owned by the packed model (freed together when the weights are re-packed or the handle is destroyed).
+struct DeviceMem {
+  std::vector<void*> ptrs;
+  // nullptr on failure (the error is set)
+  template <class T> T* alloc(size_t n, bool zero = false) {
+    void* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T));
+    if (e == cudaSuccess && zero) {
+      e = cudaMemset(q, 0, std::max<size_t>(n, 1) * sizeof(T));
+      if (e != cudaSuccess) cudaFree(q);
+    }
+    if (e != cudaSuccess) { set_error("device allocation of %zu bytes failed: %s", n * sizeof(T), cudaGetErrorString(e)); return nullptr; }
+    ptrs.push_back(q);
+    return reinterpret_cast<T*>(q);
+  }
+  // n_logical output columns of which the first n_packed (padded to 128) are stored, nkb 64-channel k-blocks
+  int alloc_packed(PackedB& pb, int n_logical, int n_packed, int nkb, bool with_f32) {
+    pb.n_logical = n_logical;
+    pb.Npad = pad_to(n_packed, 128);
+    pb.nkb = nkb;
+    const size_t elems = (size_t)nkb * pb.Npad * 64;
+    if (!(pb.hi = alloc<__nv_bfloat16>(elems, true)) || !(pb.lo = alloc<__nv_bfloat16>(elems, true))) return -2;
+    if (with_f32 && !(pb.f32 = alloc<float>(elems, true))) return -2;
+    return 0;
+  }
+  void release() {
+    for (void* p : ptrs) cudaFree(p);
+    ptrs.clear();
+  }
+};
+
+// Pack `w` ([n_rows, cin_total, ktaps] fp32, device) channels [cin0, cin0+ncin) of tap `tap` at k-block kb0, columns n_dst0..
+inline int pack_seg(PackedB& pb, const float* w, int n_rows, int cin_total, int ktaps, int tap, int cin0, int ncin, int n_dst0,
+                    int kb0, int geglu_half, cudaStream_t st, const float* cscale = nullptr) {
+  PackSeg ps;
+  ps.cscale = cscale;
+  ps.w = w; ps.n_rows = n_rows; ps.cin_total = cin_total; ps.ktaps = ktaps; ps.tap = tap; ps.cin0 = cin0; ps.ncin = ncin;
+  ps.n_dst0 = n_dst0; ps.kb0 = kb0; ps.nkb = nkb_of(ncin); ps.geglu_half = geglu_half;
+  return launch_pack_b(ps, pb.hi, pb.lo, pb.f32, pb.Npad, st);
+}
+
+// AttentionPooling's k_proj | v_proj as one [2R, R] operator (and its [2R] bias): one small linear over every token
+struct PoolKV { float* W = nullptr; float* b = nullptr; };
+inline int concat_pool_kv(DeviceMem& mem, const WeightRegistry& w, const std::string& pool, int R, PoolKV& kv, cudaStream_t st) {
+  if (!(kv.W = mem.alloc<float>((size_t)2 * R * R)) || !(kv.b = mem.alloc<float>((size_t)2 * R))) return -2;
+  NS_CHECK_CUDA(cudaMemcpyAsync(kv.W, w.W(pool + ".k_proj.weight"), (size_t)R * R * 4, cudaMemcpyDeviceToDevice, st));
+  NS_CHECK_CUDA(cudaMemcpyAsync(kv.W + (size_t)R * R, w.W(pool + ".v_proj.weight"), (size_t)R * R * 4, cudaMemcpyDeviceToDevice, st));
+  NS_CHECK_CUDA(cudaMemcpyAsync(kv.b, w.W(pool + ".k_proj.bias"), (size_t)R * 4, cudaMemcpyDeviceToDevice, st));
+  NS_CHECK_CUDA(cudaMemcpyAsync(kv.b + R, w.W(pool + ".v_proj.bias"), (size_t)R * 4, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+// One launch of a per-shape program.
+struct Launch {
+  // The denoiser's kinds keep their numbers: ns2vc_unet_launch_kind() and ns2vc_profile_kind_name() expose them.  The
+  // condition encoders' own kinds follow TAP.
+  enum Kind { GEMM, ATTN, LN_SPLIT, LN_APPLY, LINEAR, NCT2SPLIT, POOL_CLS, POOL_ATT, MASKBIAS, PREP, MEMSET, TAP,
+              SEQMASK, ENC_INPUT, LN_MASK, NCT2TOK, POOL_ATT_WIDE } kind;
+  // The call argument a launch reads or writes instead of a program buffer; each engine resolves them in its run_program.
+  enum Input { NONE,
+               X, T, OUT, CONTENT, PROMPT, MASK,                               // ns2vc_unet_prepare_cond / _forward
+               C, REFER, LENGTHS, REFER_LENGTHS, CONTENT_OUT, PROMPT_OUT       // ns2vc_pre_infer
+  } input = NONE;
+  GemmOp gemm;
+  AttnOp attn;
+  LinOp lin;
+  PrepOp prep;
+  SplitBuf split;
+  // generic small args
+  const float* a = nullptr; const float* b = nullptr; const float* c = nullptr; const float* d = nullptr;
+  float* o = nullptr; float* o2 = nullptr;
+  int i0 = 0, i1 = 0, i2 = 0, i3 = 0; float f0 = 0;
+  void* mem = nullptr; size_t mem_bytes = 0;
+  int tap_index = -1;
+  int reads_film = 0;        // denoiser: reads the FiLM rows (pointers are rebased when the caller supplies precomputed rows)
+  int time_path = 0;         // denoiser: timestep path (sinusoid -> MLP -> FiLM rows): skipped when the caller supplies precomputed FiLM rows
+};
+
+// Named activations a program can copy out after the launch that produced them (diagnostics: per-layer parity tests).
+struct TapSet {
+  std::vector<std::string> names;
+  std::vector<int> rows, ch;   // rows: the level (denoiser) or the row count per batch entry (condition encoders)
+  std::vector<float*> dst;
+  int add(const std::string& name, int r, int c) {
+    names.push_back(name); rows.push_back(r); ch.push_back(c); dst.push_back(nullptr);
+    return (int)names.size() - 1;
+  }
+  int size() const { return (int)names.size(); }
+  int info(int i, const char** name, int* r, int* c) const {
+    NS_REQUIRE(i >= 0 && i < size(), "tap index %d out of range", i);
+    if (name) *name = names[i].c_str();
+    if (r) *r = rows[i];
+    if (c) *c = ch[i];
+    return 0;
+  }
+  int set(int i, float* p) {
+    NS_REQUIRE(i >= 0 && i < size(), "tap index %d out of range", i);
+    dst[i] = p;
+    return 0;
+  }
+  int copy(const Launch& l, cudaStream_t st) const {
+    if (l.tap_index >= 0 && l.tap_index < size() && dst[l.tap_index]) {
+      cudaError_t e = cudaMemcpyAsync(dst[l.tap_index], l.a, (size_t)l.i0 * sizeof(float), cudaMemcpyDeviceToDevice, st);
+      if (e != cudaSuccess) { set_error("tap copy failed: %s", cudaGetErrorString(e)); return -2; }
+    }
+    return 0;
+  }
+};
+
+// Builds a launch program over a workspace arena (a dry run sizes the workspace: no device work, no tensor maps).
+struct ProgramBuilder {
+  Arena ar;
+  int B;
+  bool dry;
+  bool simt;
+  std::vector<Launch>* out;
+  int err = 0;
+
+  SplitBuf split(int Tn, int C) {
+    SplitBuf s{}; s.T = Tn; s.C = C; s.ld = pad_to(C, 8);
+    s.hi = ar.get<__nv_bfloat16>((size_t)B * Tn * s.ld);
+    s.lo = ar.get<__nv_bfloat16>((size_t)B * Tn * s.ld);
+    return s;
+  }
+  // view of a (larger) scratch split as [B, Tn, C]
+  static SplitBuf view(const SplitBuf& base, int Tn, int C) {
+    SplitBuf s = base; s.T = Tn; s.C = C; s.ld = pad_to(C, 8); return s;
+  }
+  GemmOp gemm_base(const PackedB& w, int T_out) {
+    GemmOp g; memset(&g, 0, sizeof(g));
+    g.B = B; g.T_out = T_out;
+    g.w_hi = w.hi; g.w_lo = w.lo; g.w_f32 = w.f32; g.N = w.Npad; g.n_valid = w.n_logical;
+    g.f16_col0 = 0x7fffffff;
+    g.ksplit = 1;
+    return g;
+  }
+  int add_src(GemmOp& g, const SplitBuf& s) { g.src[g.nsrc] = s; return g.nsrc++; }
+  void seg(GemmOp& g, int src, int c0, int nch, int tap) {
+    GSeg& s = g.seg[g.nseg++];
+    s.src = src; s.c0 = c0; s.nkb = nkb_of(nch); s.tap = tap;
+    g.nkb_total += s.nkb;
+  }
+  // a linear layer: one unshifted segment over all channels of `in`
+  GemmOp lin(const PackedB& w, const SplitBuf& in, int T_out) {
+    GemmOp g = gemm_base(w, T_out);
+    seg(g, add_src(g, in), 0, in.C, 0);
+    return g;
+  }
+  Launch& emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
+    Launch l; l.kind = Launch::GEMM; l.input = in;
+    if (!dry) {
+      if (g.nkb_total != w.nkb) { set_error("internal: K mismatch %d vs %d", g.nkb_total, w.nkb); err = -1; }
+      plan_gemm(g);
+      if (!simt) { const int rc = encode_tmaps(g); if (rc) err = rc; }
+    }
+    l.gemm = g;
+    out->push_back(l);
+    return out->back();
+  }
+  void emit_attention(const AttnOp& a, Launch::Input in = Launch::NONE) {
+    Launch l; l.kind = Launch::ATTN; l.input = in; l.attn = a;
+    if (a.v2 && !dry) { const int rc = encode_attn_tmaps(l.attn); if (rc) err = rc; }
+    out->push_back(l);
+  }
+  void emit_ln_split(const float* x, int ld, int M, int C, const float* gamma, const float* beta, const SplitBuf& o) {
+    Launch l; l.kind = Launch::LN_SPLIT; l.a = x; l.i0 = ld; l.i1 = M; l.i2 = C; l.f0 = 1e-5f; l.b = gamma; l.c = beta; l.split = o;
+    out->push_back(l);
+  }
+  void emit_ln_apply(const float* x, Launch::Input in, int M, int C, const float* gamma, const float* beta, float* y) {
+    Launch l; l.kind = Launch::LN_APPLY; l.input = in; l.a = x; l.i0 = C; l.i1 = M; l.i2 = C; l.f0 = 1e-5f; l.b = gamma; l.c = beta;
+    l.o = y; l.i3 = C;
+    out->push_back(l);
+  }
+  void emit_linear(const LinOp& o, Launch::Input in = Launch::NONE, int time_path = 0) {
+    Launch l; l.kind = Launch::LINEAR; l.input = in; l.lin = o; l.time_path = time_path;
+    out->push_back(l);
+  }
+  void emit_memset(void* p, size_t bytes) {
+    Launch l; l.kind = Launch::MEMSET; l.mem = p; l.mem_bytes = bytes;
+    out->push_back(l);
+  }
+  // copy-out point of a named activation ([B, rows, C] fp32): only in real programs, whose taps can be read
+  void emit_tap(TapSet& taps, const std::string& name, const float* src, int tap_rows, int C, int rows) {
+    if (dry) return;
+    Launch l; l.kind = Launch::TAP; l.a = src; l.i0 = B * rows * C; l.tap_index = taps.add(name, tap_rows, C);
+    out->push_back(l);
+  }
+};
+
+inline LinOp linear_op(const float* x, int x_ld, int M, int K, const float* W, const float* bias, int N, float* y, int y_ld) {
+  LinOp o; memset(&o, 0, sizeof(o));
+  o.x = x; o.x_ld = x_ld; o.M = M; o.K = K; o.W = W; o.bias = bias; o.N = N; o.out = y; o.out_ld = y_ld;
+  return o;
+}
+
+// TextTimeEmbedding (reference embeddings.py:421-434) over a token-major [B, S, R] input `x` (or the call argument `x_in`):
+//   LayerNorm -> AttentionPooling (class token; q of the class token, k|v of every token as one [2R, R] operator) -> Linear
+//   to E channels -> LayerNorm into `y` [B, E].
+// The scratch buffers are placed by reserve() so that each engine keeps its own workspace layout.
+struct TextTimeEmbedding {
+  float* norm = nullptr; float* tok = nullptr; float* q = nullptr; float* kv = nullptr; float* pool = nullptr; float* proj = nullptr;
+  void reserve(Arena& ar, int B, int S, int R, int E) {
+    norm = ar.get<float>((size_t)B * S * R);
+    tok = ar.get<float>((size_t)B * (S + 1) * R);
+    q = ar.get<float>((size_t)B * R);
+    kv = ar.get<float>((size_t)B * (S + 1) * 2 * R);
+    pool = ar.get<float>((size_t)B * R);
+    proj = ar.get<float>((size_t)B * E);
+  }
+  // `attend`: POOL_ATT (denoiser) or POOL_ATT_WIDE (condition encoders) - their sums run in different orders
+  void emit(ProgramBuilder& bld, const WeightRegistry& w, const std::string& p, const float* x, Launch::Input x_in, int S, int R,
+            int E, int heads, Launch::Kind attend, const PoolKV& pkv, float* y) const {
+    const int B = bld.B;
+    bld.emit_ln_apply(x, x_in, B * S, R, w.W(p + ".norm1.weight"), w.W(p + ".norm1.bias"), norm);
+    { Launch l; l.kind = Launch::POOL_CLS; l.a = norm; l.b = w.W(p + ".pool.positional_embedding"); l.i0 = S; l.i1 = R; l.o = tok; bld.out->push_back(l); }
+    bld.emit_linear(linear_op(tok, (S + 1) * R, B, R, w.W(p + ".pool.q_proj.weight"), w.W(p + ".pool.q_proj.bias"), R, q, R));
+    bld.emit_linear(linear_op(tok, R, B * (S + 1), R, pkv.W, pkv.b, 2 * R, kv, 2 * R));
+    { Launch l; l.kind = attend; l.a = q; l.b = kv; l.i0 = S + 1; l.i1 = R; l.i2 = heads; l.o = pool; bld.out->push_back(l); }
+    bld.emit_linear(linear_op(pool, R, B, R, w.W(p + ".proj.weight"), w.W(p + ".proj.bias"), E, proj, E));
+    bld.emit_ln_apply(proj, Launch::NONE, B, E, w.W(p + ".norm2.weight"), w.W(p + ".norm2.bias"), y);
+  }
+};
+
+// Runs the launch kinds both engines use.  GEMM / ATTN launch the op they are given: the record's own or a copy the caller
+// patched.  `in` replaces the recorded input of LN_APPLY and LINEAR when the launch reads a call argument.
+struct Runner {
+  bool simt;
+  int B;
+  const TapSet* taps;
+  cudaStream_t st;
+
+  int gemm(const GemmOp& g) const { return simt ? launch_gemm_simt(g, st) : launch_gemm_tc(g, st); }
+  int attn(const AttnOp& a) const { return (a.v2 && !simt) ? launch_attention_v2(a, st) : launch_attention(a, st, simt); }
+  int run(const Launch& l, const float* in = nullptr, unsigned long long* span = nullptr) const {
+    switch (l.kind) {
+      case Launch::GEMM: return gemm(l.gemm);
+      case Launch::ATTN: return attn(l.attn);
+      case Launch::LN_SPLIT: return launch_ln_split(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.split, st, span);
+      case Launch::LN_APPLY: return launch_ln_apply(in ? in : l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.o, l.i3, st);
+      case Launch::LINEAR: {
+        LinOp o = l.lin;
+        if (in) o.x = in;
+        return launch_small_linear(o, st);
+      }
+      case Launch::POOL_CLS: return launch_pool_class_token(l.a, l.b, B, l.i0, l.i1, l.o, st);
+      case Launch::MEMSET: {
+        const cudaError_t e = cudaMemsetAsync(l.mem, 0, l.mem_bytes, st);
+        if (e != cudaSuccess) { set_error("memset failed: %s", cudaGetErrorString(e)); return -2; }
+        return 0;
+      }
+      case Launch::TAP: return taps->copy(l, st);
+      default: set_error("internal: launch kind %d is not a shared kind", (int)l.kind); return -1;
+    }
+  }
+};
+
+}  // namespace ns2vc

@@ -194,8 +194,8 @@ int launch_ffn_taps(const float* const* w, int k, int F, int H, int centre, floa
   return 0;
 }
 // g[n] = sum_c gamma_c W[n, c],  bf[n] = sum_c beta_c W[n, c] (+ bias[n]): the vectors of a LayerNorm folded into its consumer
-// GEMM (EPI_LNFOLD; load time, double accumulation)
-__global__ void pre_ln_fold_kernel(const float* __restrict__ W, const float* __restrict__ gamma, const float* __restrict__ beta,
+// GEMM (EPI_LNFOLD; load time, double accumulation).  Used by both engines.
+__global__ void ln_fold_vec_kernel(const float* __restrict__ W, const float* __restrict__ gamma, const float* __restrict__ beta,
                                    const float* __restrict__ bias, float* __restrict__ g, float* __restrict__ bf, int N, int C) {
   const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (n >= N) return;
@@ -205,7 +205,7 @@ __global__ void pre_ln_fold_kernel(const float* __restrict__ W, const float* __r
   if (lane == 0) { g[n] = (float)sg; bf[n] = (float)(sb + (bias ? (double)bias[n] : 0.0)); }
 }
 int launch_ln_fold_vec(const float* W, const float* gamma, const float* beta, const float* bias, float* g, float* bf, int N, int C, cudaStream_t st) {
-  pre_ln_fold_kernel<<<ceil_div(N, 8), 256, 0, st>>>(W, gamma, beta, bias, g, bf, N, C);
+  ln_fold_vec_kernel<<<ceil_div(N, 8), 256, 0, st>>>(W, gamma, beta, bias, g, bf, N, C);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }

@@ -117,12 +117,7 @@ class Pre_model(nn.Module):
         return c
 
     def _release(self):
-        if self.__dict__.get("_handle") is not None:
-            try:
-                _lib.lib().ns2vc_pre_destroy(self._handle)
-            except Exception:
-                pass
-            self.__dict__["_handle"] = None
+        if _lib.release_engine(self, "ns2vc_pre_"):
             self.__dict__["_ws"] = None
 
     def __del__(self):
@@ -133,33 +128,7 @@ class Pre_model(nn.Module):
 
     def engine(self, device: torch.device) -> int:
         """Opaque engine handle with the current parameter values packed (re-packed when a parameter changed)."""
-        L = _lib.lib()
-        plist = self.__dict__.get("_plist")
-        if plist is None:
-            plist = self.__dict__["_plist"] = list(self.parameters())
-        sig = tuple((p.data_ptr(), p._version) for p in plist)
-        if self._handle is not None and self._wsig == sig and self._handle_device == device:
-            return self._handle
-        plist = self.__dict__["_plist"] = list(self.parameters())
-        sig = tuple((p.data_ptr(), p._version) for p in plist)
-        stream = torch.cuda.current_stream(device).cuda_stream
-        with torch.cuda.device(device):
-            if self._handle is None or self._handle_device != device:
-                self._release()
-                h = C.c_void_p()
-                ccfg = self._c_cfg()
-                _lib.check(L.ns2vc_pre_create(C.byref(ccfg), C.byref(h)))
-                self._handle = h.value
-                self._handle_device = device
-            for key, p in self.state_dict().items():
-                if p.device != device or p.dtype != torch.float32:
-                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; these condition encoders need fp32 parameters on {device}")
-                t = p.detach().contiguous()
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(L.ns2vc_pre_load_weight(self._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
-            _lib.check(L.ns2vc_pre_finalize(self._handle, stream))
-        self._wsig = sig
-        return self._handle
+        return _lib.engine_handle(self, "ns2vc_pre_", device, "these condition encoders need fp32 parameters on {device}")
 
     def workspace(self, B: int, T: int, S: int, device: torch.device) -> torch.Tensor:
         n = C.c_size_t()

@@ -283,13 +283,7 @@ class UNet1DConditionModel(nn.Module):
         return c
 
     def _release(self):
-        if self.__dict__.get("_handle") is not None:
-            try:
-                _lib.lib().ns2vc_unet_destroy(self._handle)
-            except Exception:
-                pass
-            # plain __dict__ writes: nn.Module.__setattr__ may already be torn down at interpreter shutdown
-            self.__dict__["_handle"] = None
+        if _lib.release_engine(self, "ns2vc_unet_"):
             self.__dict__["_ws"] = {}
 
     def __del__(self):
@@ -301,37 +295,11 @@ class UNet1DConditionModel(nn.Module):
     def engine(self, device: torch.device) -> int:
         """Opaque engine handle with the current parameter values packed for the tensor cores
         (re-packed when any parameter changed: optimizer step, load_state_dict, .to())."""
-        L = _lib.lib()
-        # 701 (storage, version) pairs over a cached list of the Parameter objects: the module tree is fixed after construction,
-        # `.to()` / `load_state_dict` / optimizers change storage or bump versions of the SAME objects (the recursive
-        # `self.parameters()` walk on every forward of the generic path was ~1 ms of host time per call)
-        plist = self.__dict__.get("_plist")
-        if plist is None:
-            plist = self.__dict__["_plist"] = list(self.parameters())
-        sig = tuple((p.data_ptr(), p._version) for p in plist)
-        if self._handle is not None and self._wsig == sig and self._handle_device == device:
-            return self._handle
-        plist = self.__dict__["_plist"] = list(self.parameters())     # something changed: re-walk the tree before re-packing
-        sig = tuple((p.data_ptr(), p._version) for p in plist)
-        stream = torch.cuda.current_stream(device).cuda_stream
-        with torch.cuda.device(device):
-            if self._handle is None or self._handle_device != device:
-                self._release()
-                h = C.c_void_p()
-                ccfg = self._c_cfg()
-                _lib.check(L.ns2vc_unet_create(C.byref(ccfg), C.byref(h)))
-                self._handle = h.value
-                self._handle_device = device
-            for key, p in self.state_dict().items():
-                if p.device != device or p.dtype != torch.float32:
-                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; this denoiser needs fp32 parameters on {device} (module.to('cuda'))")
-                t = p.detach().contiguous()
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(L.ns2vc_unet_load_weight(self._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
-            _lib.check(L.ns2vc_unet_finalize(self._handle, stream))
-        self._wsig = sig
-        self._ws_need = {}
-        return self._handle
+        sig = self._wsig
+        h = _lib.engine_handle(self, "ns2vc_unet_", device, "this denoiser needs fp32 parameters on {device} (module.to('cuda'))")
+        if self._wsig is not sig:       # (re)loaded: the workspace sizes are asked again
+            self._ws_need = {}
+        return h
 
     def workspace(self, B: int, T: int, S: int, device: torch.device) -> torch.Tensor:
         """ONE grow-only scratch buffer per module, shared by every shape (the CLI feeds a different T per slice: a fresh

@@ -138,6 +138,35 @@ def test_forward_is_deterministic_and_batch_independent(full_model):
     assert torch.isfinite(a).all()
 
 
+def test_return_to_a_cached_program_reproduces_it(full_model):
+    """Shape A, then a smaller shape B, then A again on one module and one shared workspace: the return to A reactivates A's
+    cached program, whose conditioning must be prepared again because B has run in the same workspace since."""
+    m, _ = full_model
+    dev = torch.device("cuda", 0)
+    shapes = {"A": (2, 256, 64), "B": (1, 128, 32)}
+    inps = {k: make_inputs(*v, ragged=True, seed=90 + i) for i, (k, v) in enumerate(shapes.items())}
+    pool = m.workspace(*shapes["A"], dev).data_ptr()
+    ns = NoiseScheduleVP("discrete", betas=linear_betas(1000))
+
+    def forward(k):
+        x, ehs, mask = unet_inputs(inps[k])
+        t = torch.linspace(11.5, 870.25, x.shape[0], device="cuda")
+        with torch.no_grad():
+            return m(x, t, ehs, encoder_attention_mask=mask).sample.clone()
+
+    def dpm10(k):
+        return _session(m, inps[k]).sample_dpmpp_2m(inps[k]["x"].cuda(), ns, torch.linspace(1.0, 1e-3, 11)).clone()
+
+    a0 = forward("A")
+    forward("B")
+    assert torch.equal(forward("A"), a0)
+    s0 = dpm10("A")
+    dpm10("B")
+    assert torch.equal(dpm10("A"), s0)
+    assert torch.isfinite(a0).all() and torch.isfinite(s0).all()
+    assert m.workspace(*shapes["B"], dev).data_ptr() == pool, "both shapes must run in the same workspace"
+
+
 # ------------------------------------------------------------------ sampler kernels: bit-exact
 def _rt(x, o, a, s):
     noise = (x - a * o) / s
