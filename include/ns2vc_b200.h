@@ -120,6 +120,33 @@ int ns2vc_unipc_step(const float* x_prev, const float* x_eval, const float* unet
                      const ns2vc_unipc_coef* c, float* m_t, float* x_t, float* x_pred, size_t n, int* nan_flag,
                      ns2vc_stream stream);
 
+/* DDPM p_sample (model.py:535-542) and DDIM (model.py:586-601) steps after the denoiser returned x0 = x_start.
+ * UNLIKE the two entries above, `c` is a DEVICE pointer to one coefficient struct, read by the kernel: a captured chunk of
+ * steps then serves every chunk of a long run (the host refills a device window of structs before each replay).
+ * x, x0, noise, x_next: n fp32 device values; x_next may equal x (in place).  noise is not read when the step adds none
+ * (add_noise == 0 / last != 0) and may then be NULL.  nan_flag as for ns2vc_dpm_step (NaN in the step's input x). */
+typedef struct ns2vc_ddpm_coef {
+  float c_x0;                 /* posterior_mean_coef1[t]                                                      */
+  float c_x;                  /* posterior_mean_coef2[t]                                                      */
+  float c_noise;              /* exp(0.5 * posterior_log_variance_clipped[t])                                 */
+  int add_noise;              /* t > 0; otherwise x_next = mean + 0.0f (the reference adds exp(.) * 0.)      */
+} ns2vc_ddpm_coef;
+/* x_next = (c_x0*x0 + c_x*x) + c_noise*noise */
+int ns2vc_ddpm_step(const float* x, const float* x0, const float* noise, const ns2vc_ddpm_coef* c, float* x_next, size_t n,
+                    int* nan_flag, ns2vc_stream stream);
+
+typedef struct ns2vc_ddim_coef {
+  float sqrt_recip;           /* sqrt_recip_alphas_cumprod[t]                                                 */
+  float sqrt_recipm1;         /* sqrt_recipm1_alphas_cumprod[t]                                               */
+  float sqrt_alpha_next;      /* alphas_cumprod[t_next].sqrt()                                                */
+  float c;                    /* (1 - alpha_next - sigma**2).sqrt()                                           */
+  float sigma;                /* eta * ((1 - alpha/alpha_next) * (1 - alpha_next) / (1 - alpha)).sqrt()       */
+  int last;                   /* t_next < 0: x_next = x0                                                      */
+} ns2vc_ddim_coef;
+/* pn = (sqrt_recip*x - x0) / sqrt_recipm1 ; x_next = (x0*sqrt_alpha_next + c*pn) + sigma*noise (also at eta = 0) */
+int ns2vc_ddim_step(const float* x, const float* x0, const float* noise, const ns2vc_ddim_coef* c, float* x_next, size_t n,
+                    int* nan_flag, ns2vc_stream stream);
+
 /* Bit-exact index helpers (host, no GPU): nearest-neighbour source index of F.interpolate(size=)
  * (reference resnet.py:160) and the stride-2 conv length rule (resnet.py:200). */
 int ns2vc_nearest_index(int t_in, int t_out, int* idx /* [t_out] */);

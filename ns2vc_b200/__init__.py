@@ -6,6 +6,7 @@ Drop-in surface (same names as the reference):
     ns2vc_b200.uni_pc.{NoiseScheduleVP, model_wrapper, UniPC}            <- sampler/uni_pc.py
     ns2vc_b200.pre_model.Pre_model                <- model.py:328-377 (condition encoders; ``install_pre_model(model)``)
     ns2vc_b200.frontend.repeat_expand_2d          <- utils.py:482-496 (feature stretch in front of the encoders)
+    ns2vc_b200.diffusion.{p_sample_loop, ddim_sample} <- model.py:544-603 (DDPM / DDIM; ``install_diffusion(model)``)
 ``ns2vc_b200.install()`` aliases those module paths so the reference's model.py / infer.py import
 them unchanged (see INTEGRATION.md).
 """
@@ -58,3 +59,15 @@ def install_pre_model(model_module=None) -> None:
     if model_module is None or not hasattr(model_module, "Pre_model"):
         raise RuntimeError("install_pre_model: import the reference's model.py first (or pass the module)")
     model_module.Pre_model = Pre_model
+
+
+def install_diffusion(model_module=None) -> None:
+    """Make the reference's ``NaturalSpeech2.p_sample_loop`` / ``.ddim_sample`` (``sample_method='ddpm'`` / ``'ddim'``, model.py:544-603)
+    take the fused DDPM / DDIM loops when the denoiser is our UNet (``ns2vc_b200.diffusion``); call after ``import model``."""
+    from . import diffusion
+    if model_module is None:
+        model_module = sys.modules.get("model")
+    if model_module is None or not hasattr(model_module, "NaturalSpeech2"):
+        raise RuntimeError("install_diffusion: import the reference's model.py first (or pass the module)")
+    model_module.NaturalSpeech2.p_sample_loop = diffusion.p_sample_loop
+    model_module.NaturalSpeech2.ddim_sample = diffusion.ddim_sample

@@ -44,6 +44,15 @@ class UniPcCoef(C.Structure):
                 ("n_c_x", C.c_float), ("n_c_m", C.c_float), ("nab", C.c_float), ("nrk", C.c_float), ("pred_order", C.c_int)]
 
 
+class DdpmCoef(C.Structure):
+    _fields_ = [("c_x0", C.c_float), ("c_x", C.c_float), ("c_noise", C.c_float), ("add_noise", C.c_int)]
+
+
+class DdimCoef(C.Structure):
+    _fields_ = [("sqrt_recip", C.c_float), ("sqrt_recipm1", C.c_float), ("sqrt_alpha_next", C.c_float), ("c", C.c_float),
+                ("sigma", C.c_float), ("last", C.c_int)]
+
+
 # symbol -> (restype, argtypes); also the export list checked by tests/test_abi.py
 _P = C.c_void_p
 SIGNATURES = {
@@ -64,6 +73,8 @@ SIGNATURES = {
     "ns2vc_unet_forward_film": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_dpm_step": (C.c_int, [_P, _P, _P, C.POINTER(DpmCoef), _P, _P, C.c_size_t, _P, _P]),
     "ns2vc_unipc_step": (C.c_int, [_P, _P, _P, _P, _P, C.POINTER(UniPcCoef), _P, _P, _P, C.c_size_t, _P, _P]),
+    "ns2vc_ddpm_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P, _P]),     # (the coefficient struct is a device pointer)
+    "ns2vc_ddim_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P, _P]),
     "ns2vc_mask_bias": (C.c_int, [_P, C.c_int, _P, _P]),
     "ns2vc_nearest_index": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "ns2vc_down_length": (C.c_int, [C.c_int]),

@@ -155,3 +155,87 @@ def unipc_bh2_table(ns: NoiseScheduleVP, ts: torch.Tensor, variant: str = "bh2")
         st.pred_order = p_order
         out.append(st)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------- DDPM / DDIM
+def diffusion_buffers(timesteps: int = 1000) -> dict:
+    """The schedule buffers of ``NaturalSpeech2.__init__`` (reference model.py:456-498): computed in fp64 from the linear beta
+    schedule, then each cast to fp32 as ``register_buffer`` does."""
+    scale = 1000 / timesteps
+    betas = torch.linspace(scale * 0.0001, scale * 0.02, timesteps, dtype=torch.float64)
+    alphas = 1. - betas
+    alphas_cumprod = torch.cumprod(alphas, dim=0)
+    alphas_cumprod_prev = torch.nn.functional.pad(alphas_cumprod[:-1], (1, 0), value=1.)
+    posterior_variance = betas * (1. - alphas_cumprod_prev) / (1. - alphas_cumprod)
+    f32 = lambda v: v.to(torch.float32)
+    return {
+        "betas": f32(betas),
+        "alphas_cumprod": f32(alphas_cumprod),
+        "sqrt_recip_alphas_cumprod": f32(torch.sqrt(1. / alphas_cumprod)),
+        "sqrt_recipm1_alphas_cumprod": f32(torch.sqrt(1. / alphas_cumprod - 1)),
+        "posterior_log_variance_clipped": f32(torch.log(posterior_variance.clamp(min=1e-20))),
+        "posterior_mean_coef1": f32(betas * torch.sqrt(alphas_cumprod_prev) / (1. - alphas_cumprod)),
+        "posterior_mean_coef2": f32((1. - alphas_cumprod_prev) * torch.sqrt(alphas) / (1. - alphas_cumprod)),
+    }
+
+
+@dataclass
+class DdpmStep:
+    t_input: float      # model time: the integer timestep t
+    c_x0: float         # posterior_mean_coef1[t]
+    c_x: float          # posterior_mean_coef2[t]
+    c_noise: float      # (0.5 * posterior_log_variance_clipped[t]).exp()
+    add_noise: bool     # t > 0
+
+
+def ddpm_table(buffers: dict, timesteps: List[int]) -> List[DdpmStep]:
+    """One p_sample step (reference model.py:535-542) per integer t of a descending list (999 .. 0 for ``p_sample_loop``).
+    The scalars are the fp32 buffer entries and the reference's fp32 ops on them (one-element CPU tensors: the reference's
+    [B, 1, 1] extracts take the same scalar path)."""
+    c1, c2, lv = buffers["posterior_mean_coef1"], buffers["posterior_mean_coef2"], buffers["posterior_log_variance_clipped"]
+    out = []
+    for t in timesteps:
+        t = int(t)
+        out.append(DdpmStep(t_input=float(t), c_x0=_f(c1[t]), c_x=_f(c2[t]), c_noise=_f((0.5 * lv[t:t + 1]).exp()), add_noise=t > 0))
+    return out
+
+
+def ddim_time_pairs(total: int, sampling_timesteps: int) -> List[tuple]:
+    """(time, time_next) pairs of ``ddim_sample`` (reference model.py:570-572): an fp32 linspace truncated by ``.int()``, which
+    differs from exact integer arithmetic for some counts (26, 52, 60, ...)."""
+    times = torch.linspace(-1, total - 1, steps=sampling_timesteps + 1)
+    times = list(reversed(times.int().tolist()))
+    return list(zip(times[:-1], times[1:]))
+
+
+@dataclass
+class DdimStep:
+    t_input: float
+    time: int
+    time_next: int
+    alpha: float = 0.0
+    alpha_next: float = 0.0
+    sqrt_recip: float = 0.0       # sqrt_recip_alphas_cumprod[time]
+    sqrt_recipm1: float = 0.0     # sqrt_recipm1_alphas_cumprod[time]
+    sqrt_alpha_next: float = 0.0
+    c: float = 0.0
+    sigma: float = 0.0
+    last: bool = False            # time_next < 0: the step returns x0
+
+
+def ddim_table(buffers: dict, total: int, sampling_timesteps: int, eta: float = 0.0) -> List[DdimStep]:
+    """The scalars of every ``ddim_sample`` pair (reference model.py:579-601), fp32 torch scalars in the reference's op order."""
+    ac, sr, srm1 = buffers["alphas_cumprod"], buffers["sqrt_recip_alphas_cumprod"], buffers["sqrt_recipm1_alphas_cumprod"]
+    out = []
+    for time, time_next in ddim_time_pairs(total, sampling_timesteps):
+        st = DdimStep(t_input=float(time), time=time, time_next=time_next, sqrt_recip=_f(sr[time]), sqrt_recipm1=_f(srm1[time]))
+        if time_next < 0:
+            st.last = True
+        else:
+            alpha, alpha_next = ac[time], ac[time_next]
+            sigma = eta * ((1 - alpha / alpha_next) * (1 - alpha_next) / (1 - alpha)).sqrt()
+            c = (1 - alpha_next - sigma ** 2).sqrt()
+            st.alpha, st.alpha_next, st.sqrt_alpha_next = _f(alpha), _f(alpha_next), _f(alpha_next.sqrt())
+            st.c, st.sigma = _f(c), _f(sigma)
+        out.append(st)
+    return out

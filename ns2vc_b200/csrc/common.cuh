@@ -330,6 +330,23 @@ int launch_unipc_step(const float* x_prev, const float* x_eval, const float* une
                       const float* m1, const UniPcStepCoef& c, float* m_t, float* x_t, float* x_pred, size_t n,
                       int* nan_flag, cudaStream_t st);
 
+// DDPM / DDIM steps: the coefficient struct is read from DEVICE memory (layout of ns2vc_ddpm_coef / ns2vc_ddim_coef)
+struct DdpmStepCoef {   // x_next = (c_x0*x0 + c_x*x) + (add_noise ? c_noise*noise : 0)
+  float c_x0, c_x;             // posterior_mean_coef1[t], posterior_mean_coef2[t]
+  float c_noise;               // exp(0.5 * posterior_log_variance_clipped[t])
+  int add_noise;               // t > 0
+};
+int launch_ddpm_step(const float* x, const float* x0, const float* noise, const DdpmStepCoef* c, float* x_next, size_t n,
+                     int* nan_flag, cudaStream_t st);
+
+struct DdimStepCoef {   // pn = (sqrt_recip*x - x0)/sqrt_recipm1 ; x_next = (x0*sqrt_alpha_next + c*pn) + sigma*noise, or x0 if last
+  float sqrt_recip, sqrt_recipm1;
+  float sqrt_alpha_next, c, sigma;
+  int last;                    // the pair (t, -1)
+};
+int launch_ddim_step(const float* x, const float* x0, const float* noise, const DdimStepCoef* c, float* x_next, size_t n,
+                     int* nan_flag, cudaStream_t st);
+
 // ---------------------------------------------------------------------------------------------
 // Condition encoders (pre_kernels.cu; program in pre_engine.cu)
 // ---------------------------------------------------------------------------------------------

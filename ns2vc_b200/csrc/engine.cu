@@ -1214,6 +1214,23 @@ int ns2vc_unipc_step(const float* x_prev, const float* x_eval, const float* unet
   return launch_unipc_step(x_prev, x_eval, unet_out, m0, m1, k, m_t, x_t, x_pred, n, nan_flag, (cudaStream_t)stream);
 }
 
+static_assert(sizeof(ns2vc_ddpm_coef) == sizeof(DdpmStepCoef) && offsetof(ns2vc_ddpm_coef, add_noise) == offsetof(DdpmStepCoef, add_noise),
+              "ns2vc_ddpm_coef and DdpmStepCoef must share one layout (the kernel reads the caller's struct from device memory)");
+static_assert(sizeof(ns2vc_ddim_coef) == sizeof(DdimStepCoef) && offsetof(ns2vc_ddim_coef, last) == offsetof(DdimStepCoef, last),
+              "ns2vc_ddim_coef and DdimStepCoef must share one layout (the kernel reads the caller's struct from device memory)");
+
+int ns2vc_ddpm_step(const float* x, const float* x0, const float* noise, const ns2vc_ddpm_coef* c, float* x_next, size_t n,
+                    int* nan_flag, ns2vc_stream stream) {
+  NS_REQUIRE(x && x0 && c && x_next, "null argument");
+  return launch_ddpm_step(x, x0, noise, reinterpret_cast<const DdpmStepCoef*>(c), x_next, n, nan_flag, (cudaStream_t)stream);
+}
+
+int ns2vc_ddim_step(const float* x, const float* x0, const float* noise, const ns2vc_ddim_coef* c, float* x_next, size_t n,
+                    int* nan_flag, ns2vc_stream stream) {
+  NS_REQUIRE(x && x0 && c && x_next, "null argument");
+  return launch_ddim_step(x, x0, noise, reinterpret_cast<const DdimStepCoef*>(c), x_next, n, nan_flag, (cudaStream_t)stream);
+}
+
 int ns2vc_mask_bias(const uint8_t* mask, int n, float* bias, ns2vc_stream stream) {
   NS_REQUIRE(mask && bias && n >= 0, "bad argument");
   return launch_mask_bias(mask, n, bias, (cudaStream_t)stream);

@@ -589,4 +589,66 @@ int launch_unipc_step(const float* x_prev, const float* x_eval, const float* une
   return 0;
 }
 
+// DDPM p_sample and DDIM steps (model.py:535-542, 586-601).  The scalars are read from device memory (one struct per step), so a
+// captured chunk of steps serves any window of a run: the host refills the coefficient window before each replay.  x_next may
+// be x itself (each element is read before it is written), which keeps a run's latents in one buffer.
+__global__ void __launch_bounds__(256) ddpm_step_kernel(const float* x, const float* __restrict__ x0, const float* __restrict__ noise,
+                                                        const DdpmStepCoef* __restrict__ cp, float* x_next, size_t n, int* nan_flag) {
+  pdl_trigger();
+  pdl_wait();
+  const DdpmStepCoef c = *cp;
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  bool bad = false;
+  for (; i < n; i += stride) {
+    const float xv = x[i];
+    bad |= (xv != xv);                                     // NaN guard of the denoiser input (model.py:404)
+    // q_posterior mean (:509-512), then mean + exp(0.5 * logvar) * noise; at t == 0 the reference adds exp(.) * 0. (:540-541)
+    const float mean = __fadd_rn(__fmul_rn(c.c_x0, x0[i]), __fmul_rn(c.c_x, xv));
+    x_next[i] = __fadd_rn(mean, c.add_noise ? __fmul_rn(c.c_noise, noise[i]) : 0.0f);
+  }
+  if (bad && nan_flag) atomicOr(nan_flag, 1);
+}
+int launch_ddpm_step(const float* x, const float* x0, const float* noise, const DdpmStepCoef* c, float* x_next, size_t n,
+                     int* nan_flag, cudaStream_t st) {
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  launch_k(ddpm_step_kernel, dim3(blocks), dim3(256), 0, st, x, x0, noise, c, x_next, n, nan_flag);
+  NS_LAUNCH_CHECK();
+  return 0;
+}
+
+__global__ void __launch_bounds__(256) ddim_step_kernel(const float* x, const float* __restrict__ x0, const float* __restrict__ noise,
+                                                        const DdimStepCoef* __restrict__ cp, float* x_next, size_t n, int* nan_flag) {
+  pdl_trigger();
+  pdl_wait();
+  const DdimStepCoef c = *cp;
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  bool bad = false;
+  for (; i < n; i += stride) {
+    const float xv = x[i];
+    bad |= (xv != xv);                                     // NaN guard of the denoiser input (model.py:404)
+    const float x0v = x0[i];
+    if (c.last) {                                          // the pair (t, -1): img = x_start (:589-592)
+      x_next[i] = x0v;
+      continue;
+    }
+    // predict_noise_from_start (:498-503), then x0 * sqrt(a_next) + c * pred_noise + sigma * noise (:599-601); the sigma term is
+    // kept at eta = 0: it decides the sign of zero results
+    const float pn = __fdiv_rn(__fsub_rn(__fmul_rn(c.sqrt_recip, xv), x0v), c.sqrt_recipm1);
+    const float r = __fadd_rn(__fmul_rn(x0v, c.sqrt_alpha_next), __fmul_rn(c.c, pn));
+    x_next[i] = __fadd_rn(r, __fmul_rn(c.sigma, noise[i]));
+  }
+  if (bad && nan_flag) atomicOr(nan_flag, 1);
+}
+int launch_ddim_step(const float* x, const float* x0, const float* noise, const DdimStepCoef* c, float* x_next, size_t n,
+                     int* nan_flag, cudaStream_t st) {
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  launch_k(ddim_step_kernel, dim3(blocks), dim3(256), 0, st, x, x0, noise, c, x_next, n, nan_flag);
+  NS_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace ns2vc

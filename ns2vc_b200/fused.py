@@ -92,6 +92,9 @@ class DenoiserSession:
         self.nan_flag = torch.zeros((1,), dtype=torch.int32, device=self.dev)
         self.ws = unet.workspace(self.B, self.T, self.S, self.dev)     # the module's shared grow-only scratch buffer
         self._graphs = collections.OrderedDict()
+        self._chains = collections.OrderedDict()             # DDPM / DDIM runs: device coefficient + time tables
+        self._chunk_graphs = collections.OrderedDict()       # captured DDPM / DDIM chunks, by (kind, noise draws)
+        self._chunk = None                                   # their static windows (allocated on the first such run)
         self._wsig = unet._wsig
         self.set_cond(content_BCT, prompt_BSC, prompt_mask)
 
@@ -201,13 +204,17 @@ class DenoiserSession:
             # same exception type as the reference's per-call guard (model.py:404)
             raise AssertionError("NaN in the denoiser input during the fused sampling run (reference model.py:404)")
 
-    def _run(self, kind, x_T, ns, ts, first_out, extra):
-        assert self.Cl == self.Co, "x_start parameterisation needs out_channels == latent channels"
+    def _sync_engine(self):
         if self.unet._wsig != self._wsig:                  # weights were re-packed: captured graphs are stale
             self._graphs.clear()
+            self._chunk_graphs.clear()
             self.h = self.unet.engine(self.dev)
             self._wsig = self.unet._wsig
             self._prepared = False
+
+    def _run(self, kind, x_T, ns, ts, first_out, extra):
+        assert self.Cl == self.Co, "x_start parameterisation needs out_channels == latent channels"
+        self._sync_engine()
         self.x_in.copy_(x_T, non_blocking=True)
         use_first = first_out is not None
         if use_first:
@@ -260,6 +267,154 @@ class DenoiserSession:
                      first_out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """UniPC multistep order 2, data prediction, lower_order_final (uni_pc.py:606-658)."""
         return self._run("unipc", x_T, ns, ts, first_out, variant)
+
+    # ------------------------------------------------------------------ DDPM / DDIM: chunked replay
+    # A 1000-step DDPM run as one graph would hold ~1000 x 205 nodes and its FiLM table 1000 x B rows, so these runs go in chunks
+    # of CHUNK steps.  One chunk = the FiLM rows of its CHUNK x B evaluation times (read from a static time window) + per step
+    # (UNet forward + noise draw + step kernel reading its scalars from a static coefficient window); x stays in one static
+    # buffer (the step kernels update it in place).  Before each chunk the host refills both windows with stream-ordered D2D
+    # copies from the run's full device tables, so one captured chunk is replayed for every full chunk of every run of that
+    # sampler, plus one capture for the final chunk (a different noise-draw pattern and, usually, length).
+    CHUNK = 50                                               # steps per chunk: the node count of a 50-step DPM-Solver graph
+
+    def _chunk_buffers(self):
+        if self._chunk is None:
+            f32 = dict(dtype=torch.float32, device=self.dev)
+            K, B = self.CHUNK, self.B
+            self._chunk = {
+                "tvals": torch.empty((K * B,), **f32),
+                "coef": torch.empty((K * 32,), dtype=torch.uint8, device=self.dev),
+                "table": torch.empty(int(self.L.ns2vc_unet_time_table_floats(self.h, K * B)), **f32),
+                "film_width": int(self.L.ns2vc_unet_film_width(self.h)),
+                "x": torch.empty((B, self.Cl, self.T), **f32),
+                "x0": torch.empty((B, self.Co, self.T), **f32),
+                "noise": torch.empty((B, self.Cl, self.T), **f32),
+            }
+        return self._chunk
+
+    def _chain_step(self, kind, coef_ptr, noise_ptr):
+        cb = self._chunk
+        x = cb["x"]
+        fn = self.L.ns2vc_ddpm_step if kind == "ddpm" else self.L.ns2vc_ddim_step
+        with torch.cuda.device(self.dev):
+            _lib.check(fn(x.data_ptr(), cb["x0"].data_ptr(), noise_ptr, coef_ptr, x.data_ptr(), x.numel(), self.nan_flag.data_ptr(),
+                          self._stream()))
+
+    def _chunk_body(self, kind, draws, noise, j, csize):
+        """Steps j .. j+len(draws)-1 of a run, scalars and times from the windows.  noise: the injected [N, B, C, T] tensor or
+        None (draw ``randn_like(x)`` on the default generator where ``draws`` says the reference draws)."""
+        cb = self._chunk
+        L, B, fw = len(draws), self.B, cb["film_width"]
+        self.time_table(cb["tvals"][:L * B], cb["table"])
+        for k in range(L):
+            self.forward(cb["x"], None, cb["x0"], film_rows=cb["table"][k * B * fw:(k + 1) * B * fw])
+            if noise is not None:
+                nz = noise[j + k].data_ptr()
+            elif draws[k]:
+                nz = cb["noise"].normal_().data_ptr()      # = torch.randn_like(x): empty_like(x).normal_()
+            else:
+                nz = None
+            self._chain_step(kind, cb["coef"].data_ptr() + k * csize, nz)
+
+    def _chain(self, kind, x_T, key, make_steps, first_out, noise):
+        assert self.Cl == self.Co, "x_start parameterisation needs out_channels == latent channels"
+        self._sync_engine()
+        ent = self._chains.get(key)
+        if ent is None:
+            steps = make_steps()
+            if kind == "ddpm":
+                arr = (_lib.DdpmCoef * len(steps))(*[_lib.DdpmCoef(s.c_x0, s.c_x, s.c_noise, int(s.add_noise)) for s in steps])
+                draws = tuple(s.add_noise for s in steps)
+            else:
+                arr = (_lib.DdimCoef * len(steps))(*[_lib.DdimCoef(s.sqrt_recip, s.sqrt_recipm1, s.sqrt_alpha_next, s.c, s.sigma,
+                                                                   int(s.last)) for s in steps])
+                draws = tuple(not s.last for s in steps)
+            ent = {"n": len(steps), "draws": draws, "csize": C.sizeof(arr) // len(steps),
+                   "coef": torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev),
+                   "tvals": torch.tensor([[s.t_input] * self.B for s in steps], dtype=torch.float32).reshape(-1).to(self.dev),
+                   "runs": 0}
+            self._chains[key] = ent
+            while len(self._chains) > self.MAX_GRAPHS:
+                self._chains.popitem(last=False)
+        else:
+            self._chains.move_to_end(key)
+        N, B, csize = ent["n"], self.B, ent["csize"]
+        if noise is not None:
+            if tuple(noise.shape) != (N, B, self.Cl, self.T):
+                raise ValueError(f"noise must be [{N}, {B}, {self.Cl}, {self.T}] (one tensor per step), got {tuple(noise.shape)}")
+            noise = noise.to(self.dev, torch.float32).contiguous()
+        else:
+            ent["runs"] += 1
+        use_graph = noise is None and os.environ.get("NS2VC_GRAPH", "1") != "0" and ent["runs"] >= self.CAPTURE_AFTER
+        cb = self._chunk_buffers()
+        cb["x"].copy_(x_T, non_blocking=True)
+        self.nan_flag.zero_()
+        self.prepare()
+        j = 0
+        if first_out is not None:                          # step 0 was evaluated by the caller: its update runs on its own
+            cb["x0"].copy_(first_out, non_blocking=True)
+            nz = noise[0].data_ptr() if noise is not None else (cb["noise"].normal_().data_ptr() if ent["draws"][0] else None)
+            self._chain_step(kind, ent["coef"].data_ptr(), nz)
+            j = 1
+        while j < N:
+            L = min(self.CHUNK, N - j)
+            cb["tvals"][:L * B].copy_(ent["tvals"][j * B:(j + L) * B], non_blocking=True)
+            cb["coef"][:L * csize].copy_(ent["coef"][j * csize:(j + L) * csize], non_blocking=True)
+            draws = ent["draws"][j:j + L]
+            if not use_graph:
+                self._chunk_body(kind, draws, noise, j, csize)
+            else:
+                gkey = (kind, draws)
+                g = self._chunk_graphs.get(gkey)
+                if g is None:
+                    torch.cuda.synchronize(self.dev)
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        self._chunk_body(kind, draws, None, j, csize)
+                    self._chunk_graphs[gkey] = g
+                    while len(self._chunk_graphs) > 2 * self.MAX_GRAPHS:
+                        self._chunk_graphs.popitem(last=False)
+                else:
+                    self._chunk_graphs.move_to_end(gkey)
+                g.replay()
+            j += L
+        res = cb["x"].clone()
+        self._check_nan()
+        return res
+
+    def sample_ddpm(self, x_T: torch.Tensor, timesteps=None, noise: Optional[torch.Tensor] = None,
+                    first_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """DDPM ancestral sampling, one ``p_sample`` (reference model.py:535-542) per integer t of ``timesteps`` (descending;
+        default 999 .. 0: ``p_sample_loop``, :544-561).  Noise: ``torch.randn_like(x)`` on the device's default generator for every
+        step with t > 0, in the reference's order, or the injected ``noise`` [N, B, C, T] (row k for step k; the run is then
+        eager).  ``first_out``: the model output at timesteps[0] if the caller already evaluated it."""
+        buf = _diffusion_buffers()
+        total = buf["betas"].shape[0]
+        ts = tuple(range(total - 1, -1, -1)) if timesteps is None else tuple(int(t) for t in timesteps)
+        if not ts or any(not 0 <= t < total for t in ts):
+            raise ValueError(f"timesteps must be a non-empty list of integers in [0, {total})")
+        return self._chain("ddpm", x_T, ("ddpm", ts), lambda: coefs.ddpm_table(buf, ts), first_out, noise)
+
+    def sample_ddim(self, x_T: torch.Tensor, sampling_timesteps: int, eta: float = 0.0, noise: Optional[torch.Tensor] = None,
+                    first_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """DDIM (reference ``ddim_sample``, model.py:563-603) over ``sampling_timesteps`` pairs with ``ddim_sampling_eta = eta``.
+        Noise: ``torch.randn_like(x)`` once per pair except the last (also at eta = 0, as the reference draws it), or the
+        injected ``noise`` [N, B, C, T]."""
+        buf = _diffusion_buffers()
+        total = buf["betas"].shape[0]
+        S, eta = int(sampling_timesteps), float(eta)
+        if S < 1:
+            raise ValueError("sampling_timesteps must be >= 1")
+        return self._chain("ddim", x_T, ("ddim", S, eta), lambda: coefs.ddim_table(buf, total, S, eta), first_out, noise)
+
+
+_BUFFERS = {}
+
+
+def _diffusion_buffers(timesteps: int = 1000) -> dict:
+    if timesteps not in _BUFFERS:
+        _BUFFERS[timesteps] = coefs.diffusion_buffers(timesteps)
+    return _BUFFERS[timesteps]
 
 
 def get_session(unet: UNet1DConditionModel, content_BCT, prompt_BSC, prompt_mask, T=None) -> DenoiserSession:
