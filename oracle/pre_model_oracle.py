@@ -71,7 +71,7 @@ def conv_ffn(sd: SD, p: str, x_tbc: Tensor) -> Tensor:
 
 def enc_sa_layer(sd: SD, p: str, x_tbc: Tensor, pad_mask_bt: Tensor) -> Tensor:
     """EncSALayer.forward (operations.py:798-821), eval mode (dropout off)."""
-    keep = (1 - pad_mask_bt.float()).transpose(0, 1)[..., None]
+    keep = (1 - pad_mask_bt.to(x_tbc.dtype)).transpose(0, 1)[..., None]
     r = x_tbc
     x = F.layer_norm(x_tbc, (x_tbc.shape[-1],), sd[p + ".layer_norm1.weight"], sd[p + ".layer_norm1.bias"], 1e-5)
     x = self_attention(sd, p + ".self_attn", x, pad_mask_bt)
@@ -84,7 +84,7 @@ def enc_sa_layer(sd: SD, p: str, x_tbc: Tensor, pad_mask_bt: Tensor) -> Tensor:
 
 def _encoder(sd: SD, p: str, x_tbc: Tensor, lengths: Tensor, n_layers: int, tap=None) -> Tensor:
     pad = ~sequence_mask(lengths, x_tbc.shape[0]).to(torch.bool)           # [B, T], True = padding
-    keep = (1 - pad.float()).transpose(0, 1)[..., None]
+    keep = (1 - pad.to(x_tbc.dtype)).transpose(0, 1)[..., None]
     x = conv_layer(sd, p + ".pre", x_tbc, pad) * keep
     if tap is not None:
         tap[p + ".pre"] = x.clone()

@@ -72,7 +72,7 @@ def text_time_embedding(sd, p: str, ehs: torch.Tensor, num_heads: int) -> torch.
     v = shape(F.linear(x, sd[p + ".pool.v_proj.weight"], sd[p + ".pool.v_proj.bias"]))
     scale = 1 / math.sqrt(math.sqrt(dph))
     weight = torch.einsum("bct,bcs->bts", q * scale, k * scale)
-    weight = torch.softmax(weight.float(), dim=-1)
+    weight = torch.softmax(weight.to(torch.promote_types(weight.dtype, torch.float32)), dim=-1)   # fp32 as the reference; fp64 stays fp64
     a = torch.einsum("bts,bcs->bct", weight, v)
     a = a.reshape(bs, -1, 1).transpose(1, 2)[:, 0, :]
     a = F.linear(a, sd[p + ".proj.weight"], sd[p + ".proj.bias"])
@@ -148,8 +148,6 @@ def unet_forward(sd: Dict[str, torch.Tensor], cfg: UNetConfig, sample: torch.Ten
     ehs_mask bool [B,S] (True = keep).  Returns [B,Cout,T].  ``tap(name, tensor)`` observes
     intermediate activations (channel-major, as in the reference)."""
     tap = tap or (lambda n, t: None)
-    groups, heads = cfg.norm_num_groups, cfg.num_heads
-    ss = cfg.resnet_time_scale_shift == "scale_shift"
     mask_bias = None
     if ehs_mask is not None:
         # unet_1d_condition.py:816-818
@@ -175,26 +173,38 @@ def unet_forward(sd: Dict[str, torch.Tensor], cfg: UNetConfig, sample: torch.Ten
     tap("conv_in", h)
     skips = []
     for op in build_plan(cfg):
-        if op.kind == "push":
-            skips.append(h)
-        elif op.kind == "pop_cat":
-            h = torch.cat([h, skips.pop()], dim=1)
-        elif op.kind == "resnet":
-            h = resnet_block(sd, op.prefix, h, emb, groups, cfg.norm_eps, ss)
+        h = block_forward(sd, cfg, op, h, skips, emb, ehs, mask_bias)
+        if op.prefix:
             tap(op.prefix, h)
-        elif op.kind == "xformer":
-            h = transformer(sd, op.prefix, h, ehs, mask_bias, groups, heads)
-            tap(op.prefix, h)
-        elif op.kind == "down":
-            h = F.conv1d(h, sd[op.prefix + ".conv.weight"], sd[op.prefix + ".conv.bias"], stride=2, padding=1)
-            tap(op.prefix, h)
-        elif op.kind == "up":
-            # forced-size nearest upsample to the next skip's length (unet_1d_condition.py:789-797,
-            # 1009-1010; resnet.py:160)
-            h = F.interpolate(h, size=skips[-1].shape[2:], mode="nearest")
-            h = F.conv1d(h, sd[op.prefix + ".conv.weight"], sd[op.prefix + ".conv.bias"], padding=1)
-            tap(op.prefix, h)
-    h = F.group_norm(h, groups, sd["conv_norm_out.weight"], sd["conv_norm_out.bias"], cfg.norm_eps)
+    return head_forward(sd, cfg, h)
+
+
+def block_forward(sd, cfg: UNetConfig, op, h: torch.Tensor, skips: list, emb: torch.Tensor, ehs: torch.Tensor,
+                  mask_bias: Optional[torch.Tensor]) -> torch.Tensor:
+    """One op of ``build_plan(cfg)`` on the running tensor ``h``; 'push' / 'pop_cat' update the skip list in place.
+    Returns the new running tensor."""
+    groups, heads = cfg.norm_num_groups, cfg.num_heads
+    if op.kind == "push":
+        skips.append(h)
+    elif op.kind == "pop_cat":
+        h = torch.cat([h, skips.pop()], dim=1)
+    elif op.kind == "resnet":
+        h = resnet_block(sd, op.prefix, h, emb, groups, cfg.norm_eps, cfg.resnet_time_scale_shift == "scale_shift")
+    elif op.kind == "xformer":
+        h = transformer(sd, op.prefix, h, ehs, mask_bias, groups, heads)
+    elif op.kind == "down":
+        h = F.conv1d(h, sd[op.prefix + ".conv.weight"], sd[op.prefix + ".conv.bias"], stride=2, padding=1)
+    elif op.kind == "up":
+        # forced-size nearest upsample to the next skip's length (unet_1d_condition.py:789-797,
+        # 1009-1010; resnet.py:160)
+        h = F.interpolate(h, size=skips[-1].shape[2:], mode="nearest")
+        h = F.conv1d(h, sd[op.prefix + ".conv.weight"], sd[op.prefix + ".conv.bias"], padding=1)
+    return h
+
+
+def head_forward(sd, cfg: UNetConfig, h: torch.Tensor) -> torch.Tensor:
+    """The output head after the plan: conv_norm_out -> SiLU -> conv_out."""
+    h = F.group_norm(h, cfg.norm_num_groups, sd["conv_norm_out.weight"], sd["conv_norm_out.bias"], cfg.norm_eps)
     h = F.silu(h)
     return F.conv1d(h, sd["conv_out.weight"], sd["conv_out.bias"], padding=1)
 
