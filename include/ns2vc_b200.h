@@ -78,6 +78,17 @@ int ns2vc_unet_workspace_bytes(const ns2vc_unet* h, int B, int T, int S, size_t*
 int ns2vc_unet_prepare_cond(ns2vc_unet* h, const float* content, long long content_bstride, const float* prompt,
                             const uint8_t* mask, int B, int T, int S, void* ws, ns2vc_stream stream);
 
+/* The same for a ragged batch: utterance b has content_lengths[b] <= T frames and prompt_lengths[b] <= S prompt frames
+ * (int64 [B] device arrays; values are clamped to [1, T] / [1, S]).  It selects the RAGGED program of (B, T, S, workspace),
+ * whose tables these lengths fill: the ns2vc_unet_forward / _forward_film / _time_table calls that follow run it, and
+ * row b of their output equals utterance b run alone on x[b, :, :T_b], content[b, :, :T_b], prompt[b, :S_b] (no mask).
+ * Output frames >= T_b are exact zeros; input values past the lengths are never read.  Lengths may change between calls
+ * without a rebuild (one program and one captured graph serve every length vector).  The padded program of the same key
+ * is untouched: ns2vc_unet_prepare_cond selects it again. */
+int ns2vc_unet_prepare_cond_ragged(ns2vc_unet* h, const float* content, long long content_bstride, const float* prompt,
+                                   const int64_t* content_lengths, const int64_t* prompt_lengths, int B, int T, int S, void* ws,
+                                   ns2vc_stream stream);
+
 /* UNet1DConditionModel.forward (unet_1d_condition.py:743-1037) given prepared conditioning.
  *   x [B, latent_channels, T] fp32 (batch stride x_bstride floats), t [B] fp32 -> out [B, out_channels, T] */
 int ns2vc_unet_forward(ns2vc_unet* h, const float* x, long long x_bstride, const float* t, float* out, int B, int T,

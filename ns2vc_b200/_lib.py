@@ -66,6 +66,7 @@ SIGNATURES = {
     "ns2vc_unet_finalize": (C.c_int, [_P, _P]),
     "ns2vc_unet_workspace_bytes": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "ns2vc_unet_prepare_cond": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_unet_prepare_cond_ragged": (C.c_int, [_P, _P, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_unet_forward": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_unet_film_width": (C.c_int, [_P]),
     "ns2vc_unet_time_table_floats": (C.c_size_t, [_P, C.c_int]),

@@ -8,11 +8,11 @@ sampled with the fused loop, and the result is returned on the requested device.
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
-from .fused import get_session
+from .fused import check_lengths, get_session
 from .schedule import NoiseScheduleVP
 from .synth import linear_betas
 from .unet import UNet1DConditionModel
@@ -38,11 +38,21 @@ def sample_latents(unet: UNet1DConditionModel, x_T: torch.Tensor, content_TBC: t
                    prompt_lengths: Optional[torch.Tensor], steps: Optional[int] = None, method: str = "dpmsolver",
                    device: Optional[torch.device] = None, out_device: Optional[torch.device] = None,
                    noise_schedule: Optional[NoiseScheduleVP] = None, skip_type: str = "time_uniform", eta: float = 0.0,
-                   noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   noise: Optional[torch.Tensor] = None, content_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``method``: ``"dpmsolver"`` / ``"unipc"`` (``steps`` solver steps, default 50), ``"ddim"`` (``steps`` = the reference's
     ``sampling_timesteps``, default 100 as in ``sample()``; ``eta`` = ``ddim_sampling_eta``) or ``"ddpm"`` (``p_sample_loop``: every
     timestep 999 .. 0; ``steps`` may be left unset or be 1000).  DDPM / DDIM draw their noise with ``torch.randn_like`` on the
-    device's default generator, in the reference's order, unless ``noise`` [N, B, 100, T] (one tensor per step) is given."""
+    device's default generator, in the reference's order, unless ``noise`` [N, B, 100, T] (one tensor per step) is given.
+
+    ``content_lengths`` [B] (opt-in): sample a ragged batch.  Row b of the result is then utterance b sampled alone on
+    x_T[b, :, :T_b], content[:T_b, b], prompt[:S_b, b] with S_b = ``prompt_lengths[b]`` (S when None), and its frames >= T_b
+    are 0; values past the lengths are never read.  Without it the batch keeps the reference's padded semantics, in which
+    ``prompt_lengths`` is the cross-attention mask and every row sees the whole padded T.  See ``DenoiserSession`` for the
+    DDPM / DDIM noise of a ragged batch."""
+    if content_lengths is not None:
+        content_lengths = check_lengths(content_lengths, x_T.shape[0], x_T.shape[2], "content_lengths")
+        if prompt_lengths is not None:
+            prompt_lengths = check_lengths(prompt_lengths, x_T.shape[0], prompt_SBC.shape[0], "prompt_lengths")
     if method not in ("dpmsolver", "unipc", "ddpm", "ddim"):
         raise ValueError(f"unknown method {method!r} (dpmsolver | unipc | ddpm | ddim)")
     if method in ("ddpm", "ddim"):
@@ -63,9 +73,12 @@ def sample_latents(unet: UNet1DConditionModel, x_T: torch.Tensor, content_TBC: t
     content = content_TBC.to(dev, torch.float32, non_blocking=nb).permute(1, 2, 0)
     prompt = prompt_SBC.to(dev, torch.float32, non_blocking=nb).permute(1, 0, 2)
     mask = None
-    if prompt_lengths is not None:
-        mask = sequence_mask(prompt_lengths.to(dev, non_blocking=nb), prompt_SBC.shape[0])
-    sess = get_session(unet, content, prompt, mask)
+    if content_lengths is not None:
+        sess = get_session(unet, content, prompt, None, content_lengths=content_lengths, prompt_lengths=prompt_lengths)
+    else:
+        if prompt_lengths is not None:
+            mask = sequence_mask(prompt_lengths.to(dev, non_blocking=nb), prompt_SBC.shape[0])
+        sess = get_session(unet, content, prompt, mask)
     if method == "ddpm":
         out = sess.sample_ddpm(x, noise=noise)
         return out.to(out_device) if out_device is not None else out
@@ -89,14 +102,71 @@ def sample_latents(unet: UNet1DConditionModel, x_T: torch.Tensor, content_TBC: t
 def sample_from_features(pre_model, unet: UNet1DConditionModel, x_T: torch.Tensor, c_padded: torch.Tensor, refer_padded: torch.Tensor,
                          lengths: torch.Tensor, refer_lengths: torch.Tensor, steps: Optional[int] = None, method: str = "dpmsolver",
                          device: Optional[torch.device] = None, out_device: Optional[torch.device] = None, eta: float = 0.0,
-                         noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+                         noise: Optional[torch.Tensor] = None, per_utterance: bool = False) -> torch.Tensor:
     """The device part of ``NaturalSpeech2.sample`` before the vocoder (reference model.py:606-686): ``pre_model.infer`` (condition
     encoders) followed by the sampling run.  c_padded [B, 256, T] (ContentVec features), refer_padded [B, 100, S] (mel prompt),
     lengths / refer_lengths [B]; host tensors are copied to the device.  Returns the mel latents [B, 100, T].  ``steps``, ``method``,
-    ``eta`` and ``noise`` as for ``sample_latents``."""
+    ``eta`` and ``noise`` as for ``sample_latents``.  ``per_utterance=True`` samples the encoders' output as ragged utterances
+    (``sample_latents(content_lengths=lengths, prompt_lengths=refer_lengths)``): row b of the sampling equals ``sample_latents`` on
+    row b of ``pre_model.infer``'s output alone.  The encoders themselves run on the padded batch as the reference runs them,
+    so their row b need not equal utterance b encoded alone; for that, encode per utterance and use ``sample_utterances``.
+    The default keeps the padded semantics."""
     dev = torch.device(device) if device is not None else next(unet.parameters()).device
     data = (c_padded.to(dev, torch.float32, non_blocking=True), refer_padded.to(dev, torch.float32, non_blocking=True), None, None, None,
             lengths.to(dev, non_blocking=True), refer_lengths.to(dev, non_blocking=True), None)
     content, prompt = pre_model.infer(data)
     return sample_latents(unet, x_T, content, prompt, data[6], steps=steps, method=method, device=dev, out_device=out_device, eta=eta,
-                          noise=noise)
+                          noise=noise, content_lengths=lengths if per_utterance else None)
+
+
+Utterance = Tuple[torch.Tensor, torch.Tensor, torch.Tensor]
+
+
+def batch_plan(lengths: Sequence[int], max_batch: int) -> List[List[int]]:
+    """Indices of the utterances grouped into batches of at most ``max_batch``, longest first (so each batch pads to a
+    length close to its rows').  Ties keep the input order."""
+    if max_batch < 1:
+        raise ValueError("max_batch must be >= 1")
+    order = sorted(range(len(lengths)), key=lambda i: -int(lengths[i]))
+    return [order[i:i + max_batch] for i in range(0, len(order), max_batch)]
+
+
+def pad_batch(items: Sequence[Utterance], idx: Sequence[int]):
+    """Pads utterances ``items[i]`` (x_T [Cl, T_b], content [T_b, Cc], prompt [S_b, D]) for i in ``idx`` into one ragged batch:
+    x_T [B, Cl, T], content [T, B, Cc], prompt [S, B, D] (zeros past each length), content lengths [B], prompt lengths [B]."""
+    xs, cs, ps = [items[i][0] for i in idx], [items[i][1] for i in idx], [items[i][2] for i in idx]
+    tl = torch.tensor([x.shape[-1] for x in xs], dtype=torch.int64)
+    sl = torch.tensor([p.shape[0] for p in ps], dtype=torch.int64)
+    T, S, B = int(tl.max()), int(sl.max()), len(idx)
+    x = xs[0].new_zeros((B, xs[0].shape[0], T))
+    c = cs[0].new_zeros((T, B, cs[0].shape[1]))
+    p = ps[0].new_zeros((S, B, ps[0].shape[1]))
+    for j in range(B):
+        x[j, :, :xs[j].shape[-1]] = xs[j]
+        c[:cs[j].shape[0], j] = cs[j]
+        p[:ps[j].shape[0], j] = ps[j]
+    return x, c, p, tl, sl
+
+
+@torch.no_grad()
+def sample_utterances(unet: UNet1DConditionModel, items: Sequence[Utterance], steps: Optional[int] = None, method: str = "dpmsolver",
+                      max_batch: int = 8, device: Optional[torch.device] = None, out_device: Optional[torch.device] = None,
+                      noise_schedule: Optional[NoiseScheduleVP] = None, eta: float = 0.0) -> List[torch.Tensor]:
+    """Samples a list of utterances of different lengths, ``(x_T [100, T_b], content [T_b, C], prompt [S_b, C])`` each, in
+    ragged batches of at most ``max_batch`` (longest first) and returns their latents [100, T_b] in input order.  Each result
+    equals ``sample_latents`` on that utterance alone (DDPM / DDIM: up to the noise draws, see ``DenoiserSession``).
+    The slices of one file (the reference CLI's ``infer.py`` loop) go in as one call."""
+    for k, (x, c, p) in enumerate(items):
+        if x.dim() != 2 or c.dim() != 2 or p.dim() != 2 or x.shape[1] != c.shape[0]:
+            raise ValueError(f"utterance {k}: expected x_T [C, T_b], content [T_b, C] and prompt [S_b, C], got "
+                             f"{tuple(x.shape)}, {tuple(c.shape)}, {tuple(p.shape)}")
+        if x.shape[1] < 1 or p.shape[0] < 1:
+            raise ValueError(f"utterance {k}: empty content or prompt")
+    out: List[Optional[torch.Tensor]] = [None] * len(items)
+    for idx in batch_plan([x.shape[1] for x, _, _ in items], max_batch):
+        x, c, p, tl, sl = pad_batch(items, idx)
+        lat = sample_latents(unet, x, c, p, sl, steps=steps, method=method, device=device, out_device=out_device,
+                             noise_schedule=noise_schedule, eta=eta, content_lengths=tl)
+        for j, i in enumerate(idx):
+            out[i] = lat[j, :, :int(tl[j])]
+    return out

@@ -36,7 +36,9 @@ template <int DHP, int PB, bool PF16, bool BIAS> struct ACfg {
   static constexpr int kMinCtas = (PB == 128) ? 1 : (kSmem <= 113 * 1024) ? 2 : 1;
 };
 
-template <int DHP, int PB, bool BIAS, bool PF16>
+// RAGK: per-entry key counts (op.key_len, the denoiser's ragged self-attention): entry b runs exactly the key tiles, and the tail
+// mask, of a run over its own keys alone
+template <int DHP, int PB, bool BIAS, bool PF16, bool RAGK = false>
 __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCtas) attn_v2_kernel(const __grid_constant__ AttnOp op) {
   using C = ACfg<DHP, PB, PF16, BIAS>;
   constexpr int NST = C::NST;
@@ -87,10 +89,12 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
         tma_load_3d(dst + 3 * C::kTBytes, &op.tm[5], op.v_c0 + h * dh, j * kKeys, b, kv_full(stage));
       };
       pdl_wait();                                           // q / k / v are the previous kernels' outputs
+      int nt = ntiles;
+      if constexpr (RAGK) nt = min(ntiles, (((__ldg(op.key_len + b) - 1) >> op.key_shift) + kKeys) / kKeys);
       mbar_arrive_expect_tx(q_full, 2u * C::kQBytes);
       tma_load_3d(sQ, &op.tm[0], op.q_c0 + h * dh, q0, b, q_full);
       tma_load_3d(sQ + C::kQBytes, &op.tm[1], op.q_c0 + h * dh, q0, b, q_full);
-      for (int j = 0; j < ntiles; ++j) {
+      for (int j = 0; j < nt; ++j) {
         if (j >= NST) mbar_wait(kv_empty(j % NST), (uint32_t)(((j / NST) & 1) ^ 1));   // every warp is done with tile j - NST
         load_kv(j);
       }
@@ -100,6 +104,8 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
     float* bias_s = reinterpret_cast<float*>(smem + C::kOffBias);
     const float qscale = op.scale * 1.4426950408889634f;
     pdl_wait();                                             // the mask bias and the output buffers belong to earlier kernels
+    int tk = op.Tk, nt = ntiles;
+    if constexpr (RAGK) { tk = min(tk, ((__ldg(op.key_len + b) - 1) >> op.key_shift) + 1); nt = (tk + kKeys - 1) / kKeys; }
     if (BIAS) {                                             // additive mask bias * log2(e); -inf past Tk
       const float* bias = op.bias + (long long)b * op.Tk;
       for (int i = tid - 32; i < ntiles * kKeys; i += 256)
@@ -110,12 +116,12 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
     const int r0 = 16 * (warp - 1);
     mbar_wait(q_full, 0);
     fw.load_q(sQ, sQ + C::kQBytes, r0, lane);
-    for (int j = 0; j < ntiles; ++j) {
+    for (int j = 0; j < nt; ++j) {
       const int stage = j % NST;
       mbar_wait_quiet(kv_full(stage), (uint32_t)((j / NST) & 1));
       const uint32_t kst = sKV + stage * C::kStageBytes;
       fw.tile(kst, kst + C::kTBytes, kst + 2 * C::kTBytes, kst + 3 * C::kTBytes, BIAS ? bias_s + j * kKeys : nullptr, qscale,
-              op.Tk - j * kKeys, lane);
+              (RAGK ? tk : op.Tk) - j * kKeys, lane);
       __syncwarp();
       if (lane == 0) mbar_arrive(kv_empty(stage));
     }
@@ -126,24 +132,24 @@ __global__ void __launch_bounds__(kThreadsV2, ACfg<DHP, PB, PF16, BIAS>::kMinCta
   if (op.trace && tid == 0 && cta_lin < 597) op.trace[256 + 3 * cta_lin + 1] = gtime_ns();
 }
 
-template <int DHP, int PB, bool BIAS, bool PF16>
+template <int DHP, int PB, bool BIAS, bool PF16, bool RAGK = false>
 int launch_v2b(const AttnOp& op, cudaStream_t st) {
   using C = ACfg<DHP, PB, PF16, BIAS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_v2_kernel<DHP, PB, BIAS, PF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem);
+    cudaError_t e = cudaFuncSetAttribute(attn_v2_kernel<DHP, PB, BIAS, PF16, RAGK>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem);
     if (e != cudaSuccess) { set_error("attention v2: cannot set %d B dynamic smem: %s", C::kSmem, cudaGetErrorString(e)); return -2; }
     // ask for the largest shared-memory carve-out: the CTA count per SM is what the smem budget above was sized for
-    cudaFuncSetAttribute(attn_v2_kernel<DHP, PB, BIAS, PF16>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(attn_v2_kernel<DHP, PB, BIAS, PF16, RAGK>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (getenv("NS2VC_DEBUG")) {
       int nb = 0;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, attn_v2_kernel<DHP, PB, BIAS, PF16>, kThreadsV2, (size_t)C::kSmem);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, attn_v2_kernel<DHP, PB, BIAS, PF16, RAGK>, kThreadsV2, (size_t)C::kSmem);
       fprintf(stderr, "ns2vc: attn_v2<%d,%d,bias=%d,f16=%d> smem %d B, planned %d CTAs/SM, occupancy API says %d\n", DHP, PB, (int)BIAS, (int)PF16, C::kSmem, C::kMinCtas, nb);
     }
     attr_set = true;
   }
   dim3 grid(ceil_div(op.Tq, kQ), op.H, op.B);
-  cudaError_t e = launch_k(attn_v2_kernel<DHP, PB, BIAS, PF16>, grid, dim3(kThreadsV2), (size_t)C::kSmem, st, op);
+  cudaError_t e = launch_k(attn_v2_kernel<DHP, PB, BIAS, PF16, RAGK>, grid, dim3(kThreadsV2), (size_t)C::kSmem, st, op);
   if (e != cudaSuccess) { set_error("attention v2 launch failed: %s", cudaGetErrorString(e)); return -2; }
   return 0;
 }
@@ -152,6 +158,10 @@ int launch_v2b(const AttnOp& op, cudaStream_t st) {
 bool p_fp16() { return attention_v2_p_fp16(); }
 template <int DHP, int PB>
 int launch_v2(const AttnOp& op, cudaStream_t st) {
+  if (op.key_len) {
+    if (op.bias) { set_error("attention v2: per-entry key counts take no additive bias"); return -1; }
+    return (p_fp16() && !op.p_split) ? launch_v2b<DHP, PB, false, true, true>(op, st) : launch_v2b<DHP, PB, false, false, true>(op, st);
+  }
   if (op.bias) {
     if (ceil_div(op.Tk, kKeys) * kKeys > ACfg<DHP, PB, true, true>::kBiasKeys) { set_error("attention v2: %d biased keys exceed the staged-bias capacity", op.Tk); return -1; }
     return (p_fp16() && !op.p_split) ? launch_v2b<DHP, PB, true, true>(op, st) : launch_v2b<DHP, PB, true, false>(op, st);

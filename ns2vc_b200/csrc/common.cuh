@@ -80,6 +80,10 @@ struct alignas(16) PrepOp {      // (16-byte multiples: arrays of descriptors ar
   SplitBuf out;                           // transformed
   SplitBuf raw;                           // optional second output without the transform (hi == nullptr: none)
   unsigned long long* span;               // diagnostics
+  // ragged programs: per-utterance lengths [B] at level 0 (nullptr: every row of T_dst is valid).  Output rows
+  // t >= ((row_len[b] - 1) >> len_shift) + 1 are written as zeros and the GroupNorm statistics count only the valid rows; a
+  // nearest upsample (rowmap set) derives each entry's source rows from its own lengths at levels len_shift + 1 and len_shift.
+  const int* row_len; int len_shift;
 };
 
 // GEMM / implicit-conv operator (shared by the wgmma kernel and the SIMT debug kernel):
@@ -180,6 +184,10 @@ struct GemmOp {
   const PrepOp* pre;           // GroupNorm parameters of the normalised segments (device memory; only the affine part is used)
   const float* pre_film;       // FiLM rows read by that affine (nullptr: none) - kept here because they change per forward
   const float* rowmask;        // EPI_ROWMASK: [B*T_out] keep factor (1 = frame inside the utterance, 0 = padding)
+  // Ragged programs (the RAG instantiation): per-utterance lengths [B] at level 0, or nullptr.  Rows t >= ((row_len[b] - 1) >>
+  // len_shift) + 1 of the output are stored as exact zeros, and panel-mode rows past that length read as the conv's zero padding.
+  const int* row_len;
+  int len_shift;
   // ---- tensor maps last: the TMA unit reads them by address (kernel-parameter space); the kernel copies only the fields
   // ---- before them into shared memory (kGemmOpHotBytes)
   TMap tmap[2 * kMaxSrc];      // [2*i] = hi, [2*i+1] = lo of src[i]; box = {64 ch, 128 rows, 1} (130 rows for a panel-mode k=3 source)
@@ -245,6 +253,8 @@ struct AttnOp {
   int q_c0, k_c0, v_c0;
   int v2;                         // 1: launch the v2 kernel (needs dh % 16 == 0 and encode_attn_tmaps())
   int pb;                         // byte width of the Q/K/V TMA boxes = shared-memory row pitch (32 / 64 / 128)
+  const int* key_len;             // v2, the denoiser's ragged programs: per-entry lengths [B] at level 0 (nullptr: Tk keys).  Entry b attends
+  int key_shift;                  // over its first ((key_len[b] - 1) >> key_shift) + 1 keys only; later key tiles are not even loaded
   int p_split;                    // 1: softmax weights as a bf16 hi/lo split whatever NS2VC_ATTN_P says (V must then be a bf16 split too).  The
                                   // condition encoders attend over a few dozen keys: the 2^-12 rounding of fp16 weights does not average out there
   TMap tm[6];                     // q hi, q lo (box pb x 128 rows), k hi, k lo, v hi, v lo (box pb x 64 rows)
@@ -275,8 +285,9 @@ int launch_nct_to_tokens(const float* x, long long bstride, int B, int C, int T,
                          cudaStream_t st);
 // [B, C, T] fp32 -> split token-major [B, T, out.ld] (channels >= C zero-filled up to out.ld)
 // warm / warm_bytes: optional region prefetched into L2 by the same launch (the step's FiLM rows)
+// row_len: per-entry valid frames [B] (ragged programs): frames past them are written as zeros
 int launch_nct_to_split(const float* x, long long bstride, int B, int C, int T, SplitBuf out, cudaStream_t st, const void* warm = nullptr,
-                        long long warm_bytes = 0);
+                        long long warm_bytes = 0, const int* row_len = nullptr);
 // token-major [B, T, ld] -> [B, C, T]
 int launch_tokens_to_nct(const float* x, int ld, int B, int C, int T, float* out, cudaStream_t st);
 
@@ -296,11 +307,23 @@ struct LinOp {
 int launch_small_linear(const LinOp& op, cudaStream_t st);
 
 // AttentionPooling pieces (reference embeddings.py:499-546)
+// lens: per-entry prompt lengths [B] (ragged programs: pool over the first lens[b] frames only), or nullptr (all S)
 int launch_pool_class_token(const float* xn /*[B,S,C] LN'd*/, const float* pos /*[C]*/, int B, int S, int C,
-                            float* tokens /*[B,S+1,C]: row0 = class token, rows 1.. = xn*/, cudaStream_t st);
+                            float* tokens /*[B,S+1,C]: row0 = class token, rows 1.. = xn*/, cudaStream_t st, const int* lens = nullptr);
 int launch_pool_attend(const float* q /*[B,C]*/, const float* kv /*[B,S+1,2C] k|v*/, int B, int S1, int C, int heads,
-                       float* out /*[B,C]*/, cudaStream_t st);
+                       float* out /*[B,C]*/, cudaStream_t st, const int* lens = nullptr);
 int launch_mask_bias(const uint8_t* mask, int n, float* bias, cudaStream_t st);
+
+// Ragged programs: per-utterance lengths -> the device tables the program reads (written by ns2vc_unet_prepare_cond_ragged).
+constexpr int kRagMaxLevels = 8;
+struct RaggedTables {
+  int B, T, S, nlev;
+  int* lens;                          // [2B]: content lengths | prompt lengths, clamped to [1, T] / [1, S]
+  float* prompt_bias;                 // [B, S]: 0 / -inf key bias of the cross-attention
+  float* key_bias[kRagMaxLevels];     // [B, Tl] 0 / -inf key bias of the self-attention at level l (nullptr: no transformer there)
+  int Tl[kRagMaxLevels];
+};
+int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st);
 
 // Fused sampler steps (element-wise, bit-exact op order; see kernels_misc.cu)
 struct DpmStepCoef {   // DPM-Solver++(2M): one post-UNet step
@@ -361,5 +384,15 @@ int launch_ffn_taps(const float* const* w, int k, int F, int H, int centre, floa
 int launch_scale_vec(const float* a, float s, float* o, int n, cudaStream_t st);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// Source row of output row i of F.interpolate(size=t_out, mode='nearest') from t_in rows: ATen nearest_idx (UpSample.h), with
+// IEEE fp32 division / product / floor as ns2vc_nearest_index() on the host.  In fp32 this is NOT always i >> 1 when t_out is
+// 2 t_in - 1 (e.g. t_in = 2095, t_out = 4189, i = 4187 -> 2094): a table depends on both lengths.
+__device__ __forceinline__ int nearest_src_index(int i, int t_in, int t_out) {
+  if (t_out == t_in) return i;
+  if (t_out == 2 * t_in) return i >> 1;
+  const float scale = __fdiv_rn((float)t_in, (float)t_out);
+  return min((int)floorf(__fmul_rn((float)i, scale)), t_in - 1);
+}
 
 }  // namespace ns2vc

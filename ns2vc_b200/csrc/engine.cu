@@ -52,9 +52,11 @@ struct XformerSite {
 };
 struct ConvSite { std::string p; int c; PackedB w; };
 
-// The launch programs of one (B, T, S, workspace) key.
+// The launch programs of one (B, T, S, ragged, workspace) key.
 struct Program {
   int B = 0, T = 0, S = 0; void* ws = nullptr;
+  bool ragged = false;       // per-utterance content / prompt lengths (ns2vc_unet_prepare_cond_ragged)
+  RaggedTables rt{};         // ragged: the length and key-bias tables (static buffer) its prepare_cond fills
   bool has_mask = false;
   bool cond_ready = false;   // the conditioning program has run for this key since it last became active
   std::vector<Launch> prog_cond, prog_fwd;
@@ -397,11 +399,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
 __global__ void nearest_index_kernel(int t_in, int t_out, int* idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= t_out) return;
-  int s;
-  if (t_out == t_in) s = i;
-  else if (t_out == 2 * t_in) s = i >> 1;
-  else { const float scale = __fdiv_rn((float)t_in, (float)t_out); s = min((int)floorf(__fmul_rn((float)i, scale)), t_in - 1); }
-  idx[i] = s;
+  idx[i] = nearest_src_index(i, t_in, t_out);
 }
 
 struct Builder : ProgramBuilder {
@@ -435,9 +433,10 @@ struct Builder : ProgramBuilder {
   }
   // GroupNorm parameters of a panel-mode GEMM (statistics of up to two concatenated producers), parked in the workspace
   const PrepOp* affine_desc(const double* st1, int C1, const double* st2, int C2, int Tn, int mode, float eps, const float* gamma,
-                            const float* beta, int film_ld) {
+                            const float* beta, int film_ld, int level) {
     PrepOp p; memset(&p, 0, sizeof(p));
     p.C1 = C1; p.C2 = C2; p.B = B; p.T_src = Tn; p.T_dst = Tn; p.mode = mode;
+    p.row_len = rag_lens; p.len_shift = level;
     p.gn.sum1 = st1; p.gn.sq1 = st1 ? st1 + (size_t)B * C1 : nullptr;
     p.gn.sum2 = st2; p.gn.sq2 = st2 ? st2 + (size_t)B * C2 : nullptr;
     p.gn.gamma = gamma; p.gn.beta = beta; p.gn.film_ld = film_ld; p.gn.G = h->cfg.norm_num_groups; p.gn.eps = eps;
@@ -448,6 +447,7 @@ struct Builder : ProgramBuilder {
     return aff_dev ? aff_dev + (aff_host.size() - 1) : reinterpret_cast<const PrepOp*>(uintptr_t(16));   // (dry run: any non-null value)
   }
   std::vector<PrepOp> aff_host; PrepOp* aff_dev = nullptr; int aff_cap = 0;
+  const int* rag_lens = nullptr;                           // ragged programs: content lengths [B] (device), else nullptr
   Arena sar;                                               // the program's static buffer (see ns2vc_unet::static_bufs)
   void reserve_affine(int n) { aff_cap = n; aff_dev = sar.get<PrepOp>((size_t)n); aff_host.reserve(n); }
   int upload_affine(cudaStream_t st) {
@@ -479,8 +479,10 @@ struct Builder : ProgramBuilder {
   }
 };
 
-// Builds the programs of (B, T, S, ws) into *prog, or (ws == nullptr) sizes their workspace into *bytes_out.
-int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_out, Program* prog, cudaStream_t st = nullptr) {
+// Builds the programs of (B, T, S, ragged, ws) into *prog, or (ws == nullptr) sizes their workspace into *bytes_out.
+// A ragged program takes no more workspace than the padded one: its tables live in the program's static buffer.
+int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_out, Program* prog, cudaStream_t st = nullptr,
+                   bool ragged = false) {
   const ns2vc_unet_cfg& c = h->cfg;
   const bool dry = (ws == nullptr);
   const int nlev = c.n_levels;
@@ -490,6 +492,9 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   std::vector<int> Tl(nlev);
   for (int l = 0; l < nlev; ++l) Tl[l] = level_len(T, l);
   NS_REQUIRE(Tl[nlev - 1] >= 1 && T >= 1 && B >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
+  NS_REQUIRE(!ragged || (!h->simt && nlev <= kRagMaxLevels), "ragged programs need the wgmma backend and at most %d levels", kRagMaxLevels);
+  std::vector<bool> xf_level(nlev, false);                 // levels with a transformer (their self-attention needs a key bias)
+  for (auto& o : h->plan) if (o.kind == PlanOp::XFORMER) xf_level[o.level] = true;
 
   Program pg;
   if (!dry) {
@@ -507,6 +512,10 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
     const int n_aff = 2 * (int)h->resnets.size() + (int)h->xformers.size() + 2;
     size_t sbytes = 1024 + (size_t)n_aff * sizeof(PrepOp);
     for (auto& o : h->plan) if (o.kind == PlanOp::UP) sbytes += 256 + (size_t)Tl[o.level] * sizeof(int);
+    if (ragged) {
+      sbytes += 512 + (size_t)2 * B * sizeof(int) + (size_t)B * S * sizeof(float);
+      for (int l = 0; l < nlev; ++l) if (xf_level[l]) sbytes += 256 + (size_t)B * Tl[l] * sizeof(float);
+    }
     if (!dry) {
       void* sb = nullptr;
       NS_CHECK_CUDA(cudaMalloc(&sb, sbytes));
@@ -514,7 +523,21 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
       bld.sar = Arena{(uint8_t*)sb, 0};
     }
     bld.reserve_affine(n_aff);
+    if (ragged) {
+      pg.ragged = true;
+      RaggedTables& rt = pg.rt;
+      rt.B = B; rt.T = T; rt.S = S; rt.nlev = nlev;
+      rt.lens = bld.sar.get<int>((size_t)2 * B);
+      rt.prompt_bias = bld.sar.get<float>((size_t)B * S);
+      for (int l = 0; l < nlev; ++l) { rt.Tl[l] = Tl[l]; rt.key_bias[l] = xf_level[l] ? bld.sar.get<float>((size_t)B * Tl[l]) : nullptr; }
+      bld.rag_lens = rt.lens;
+    }
   }
+  // ragged programs: content lengths (every level derives its own: ceil(T_b / 2^l)) and prompt lengths
+  const int* lens = pg.rt.lens;
+  const int* plens = lens ? lens + B : nullptr;
+  auto rag = [&](GemmOp& g, int level) { g.row_len = lens; g.len_shift = level; };
+  auto rag_prep = [&](const int* len, int level) { PrepOp& p = bld.out->back().prep; p.row_len = len; p.len_shift = level; };
 
   // ---- persistent conditioning buffers
   float* P = (Cc > 0) ? ar.get<float>((size_t)B * T * c0) : nullptr;      // conv_in(content) + bias
@@ -542,7 +565,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
 
   // ================= conditioning program =================
   if (Cc > 0) {
-    { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::CONTENT; l.i0 = Cc; l.i1 = T; l.split = s_content; bld.out->push_back(l); }
+    { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::CONTENT; l.i0 = Cc; l.i1 = T; l.split = s_content; l.lens = lens; bld.out->push_back(l); }
     GemmOp g = bld.gemm_base(h->convin_content, T);
     bld.conv3(g, s_content);
     g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W("conv_in.bias"); g.out = P; g.out_ld = c0;
@@ -551,13 +574,14 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   { Launch l; l.kind = Launch::MASKBIAS; l.input = Launch::MASK; l.i0 = B * S; l.o = maskbias; bld.out->push_back(l); }
   if (h->kv_total > 0) {
     bld.emit_prep(nullptr, xd, nullptr, 0, S, S, PREP_RAW, nullptr, nullptr, s_prompt, nullptr, 1, 0, nullptr, Launch::PROMPT);
+    rag_prep(plens, 0);                                    // (ragged: prompt frames past S_b are zeros, so is their K / V)
     GemmOp g = bld.lin(h->kv_all, s_prompt, S);
     g.flags = EPI_OUT_F32 | EPI_OUT_SPLIT; g.out = kvc; g.out_ld = h->kv_total;
     g.out_hi = kvs.hi; g.out_lo = kvs.lo; g.out_split_ld = kvs.ld;   // (V stays a bf16 split: cross-attention weights are split)
     bld.emit_gemm(g, h->kv_all);
   }
   if (c.add_embed_text)   // TextTimeEmbedding of the prompt (embeddings.py:421-434)
-    tte.emit(bld, h->weights, "add_embedding", nullptr, Launch::PROMPT, S, xd, ted, c.add_embed_heads, Launch::POOL_ATT, h->pool_kv, aug);
+    tte.emit(bld, h->weights, "add_embedding", nullptr, Launch::PROMPT, S, xd, ted, c.add_embed_heads, Launch::POOL_ATT, h->pool_kv, aug, plens);
 
   // ================= forward program =================
   bld.out = &pg.prog_fwd;
@@ -605,7 +629,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   const SplitBuf SP_LN = scratch_split(max_act);     // raw (un-normalised) split of the transformer's residual stream (folded LayerNorms)
 
   // entry: x -> split tokens, time path, conv_in
-  { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::X; l.i0 = Cl; l.i1 = T; l.split = s_xin; bld.out->push_back(l); }
+  { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::X; l.i0 = Cl; l.i1 = T; l.split = s_xin; l.lens = lens; bld.out->push_back(l); }
   { LinOp o = linear_op(nullptr, 1, B, c0, h->weights.W("time_embedding.linear_1.weight"), h->weights.W("time_embedding.linear_1.bias"), ted, temb1, ted);
     o.in_mode = LIN_SINUSOID; o.flip_sin_to_cos = c.flip_sin_to_cos; o.freq_shift = c.freq_shift; o.out_silu = 1;
     bld.emit_linear(o, Launch::T, 1); }
@@ -652,6 +676,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
     emits_block_out(g, o);
     o.st = new_stats(c0);
     with_stats(g, o.st, c0);
+    rag(g, 0);
     bld.emit_gemm(g, h->convin_lat);
     cur = o;
     bld.emit_tap(pg.taps, "conv_in", cur.p, 0, c0, T);
@@ -682,11 +707,12 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             bld.xseg(g, i0, 0, s.c1, 3, 0, ni, 1, 0);
             if (s.c2) { const int i1 = bld.add_src(g, cat2.sp); bld.xseg(g, i1, 0, s.c2, 3, n1, ni, 1, s.c1); }
             g.pre = bld.affine_desc(cur.st, s.c1, s.c2 ? cat2.st : nullptr, s.c2, TL, PREP_AFFINE_SILU, c.norm_eps,
-                                    h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), 0);
+                                    h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), 0, o.level);
             g.flags = EPI_BIAS | EPI_OUT_SPLIT; g.bias = h->weights.W(s.p + ".conv1.bias");
             if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
             g.out_hi = a_h.hi; g.out_lo = a_h.lo; g.out_split_ld = a_h.ld;
             with_stats(g, h1_st, s.cout);
+            rag(g, o.level);
             bld.emit_gemm(g, s.conv1);
           }
           {
@@ -701,16 +727,18 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             const int j0 = bld.add_src(g, a_h);
             bld.xseg(g, j0, 0, s.cout, 3, 0, no, 1, 0);
             g.pre = bld.affine_desc(h1_st, s.cout, nullptr, 0, TL, PREP_AFFINE_SILU, c.norm_eps, h->weights.W(s.p + ".norm2.weight"),
-                                    h->weights.W(s.p + ".norm2.bias"), h->film_total);
+                                    h->weights.W(s.p + ".norm2.bias"), h->film_total, o.level);
             g.pre_film = c.time_scale_shift ? film + s.film_off : nullptr;
             emits_block_out(g, outp);
             with_stats(g, outp.st, s.cout);
+            rag(g, o.level);
             bld.emit_gemm(g, s.conv2);
           }
         } else {
           const SplitBuf a_in = Builder::view(SP_A, TL, s.cin), a_raw = Builder::view(SP_R, TL, s.cin);
           bld.emit_prep_gn(s1, s.c1, cur.st, s2, s.c2, s.c2 ? cat2.st : nullptr, TL, PREP_AFFINE_SILU, c.norm_eps,
                            h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), nullptr, 0, a_in, s.shortcut ? &a_raw : nullptr);
+          rag_prep(lens, o.level);
           {
             GemmOp g = bld.gemm_base(s.conv1, TL);
             bld.conv3(g, a_in);
@@ -718,11 +746,13 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
             g.out = H1; g.out_ld = s.cout;
             with_stats(g, h1_st, s.cout);
+            rag(g, o.level);
             bld.emit_gemm(g, s.conv1);
           }
           // norm2 (+FiLM scale/shift) + SiLU (reference resnet.py:602-612)
           bld.emit_prep_gn(H1, s.cout, h1_st, nullptr, 0, nullptr, TL, PREP_AFFINE_SILU, c.norm_eps, h->weights.W(s.p + ".norm2.weight"),
                            h->weights.W(s.p + ".norm2.bias"), c.time_scale_shift ? film + s.film_off : nullptr, h->film_total, a_h);
+          rag_prep(lens, o.level);
           {
             GemmOp g = bld.gemm_base(s.conv2, TL);
             bld.conv3(g, a_h);
@@ -731,6 +761,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             else { g.flags |= EPI_RESIDUAL; g.res = s1; g.res_ld = s.c1; }
             emits_block_out(g, outp);
             with_stats(g, outp.st, s.cout);
+            rag(g, o.level);
             bld.emit_gemm(g, s.conv2);
           }
         }
@@ -745,7 +776,10 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         const SplitBuf sx = Builder::view(SP_X, TL, C), satt = Builder::view(SP_ATT, TL, C), sff = Builder::view(SP_FF, TL, 4 * C),
                        sh2 = Builder::view(SP_H, TL, C);
         const bool xin = xf_ok(C, 0);                        // GroupNorm(eps 1e-6) of the block input applied inside proj_in
-        if (!xin) bld.emit_prep_gn(cur.p, C, cur.st, nullptr, 0, nullptr, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), nullptr, 0, sx);
+        if (!xin) {
+          bld.emit_prep_gn(cur.p, C, cur.st, nullptr, 0, nullptr, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), nullptr, 0, sx);
+          rag_prep(lens, o.level);
+        }
         // Folded LayerNorms: the producer of each LN input also emits its raw bf16 split and the per-row sums; the consumer
         // GEMM runs on the raw split with gamma folded into its weights and applies mean / rstd in its epilogue:
         //   LN(x) W^T = rstd * (x (gamma*W)^T - mean * g) + (beta W^T + bias),   g[n] = sum_c gamma_c W[n,c]
@@ -760,10 +794,11 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           if (xin) {
             const int i0 = bld.add_src(g, cur.sp);
             bld.xseg(g, i0, 0, C, 1, 0, 0, 1, 0);
-            g.pre = bld.affine_desc(cur.st, C, nullptr, 0, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), 0);
+            g.pre = bld.affine_desc(cur.st, C, nullptr, 0, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), 0, o.level);
           }
           g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(x.p + ".proj_in.bias"); g.out = T0; g.out_ld = C;
           if (fold) emits_ln_input(g, rs1);
+          rag(g, o.level);
           bld.emit_gemm(g, x.proj_in); }
         if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->weights.W(b + ".norm1.weight"), h->weights.W(b + ".norm1.bias"), sx);
         const SplitBuf& sn = fold ? sln : sx;                // A operand of the LayerNorm consumers
@@ -779,6 +814,9 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           a.q = QKV; a.q_ld = 3 * C; a.k = QKV + C; a.k_ld = 3 * C; a.v = QKV + 2 * C; a.v_ld = 3 * C;
           a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
           a.B = B; a.H = H; a.Tq = TL; a.Tk = TL; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
+          // ragged: v2 attends over each entry's own keys (per-entry key count); the fp32 kernel takes a 0 / -inf key bias
+          if (ragged && av2) { a.key_len = lens; a.key_shift = o.level; }
+          else if (ragged) a.bias = pg.rt.key_bias[o.level];
           if (av2) { a.v2 = 1; a.p_split = p16(TL) ? 0 : 1; a.qs = sqkv; a.ks = sqkv; a.vs = sqkv; a.q_c0 = 0; a.k_c0 = C; a.v_c0 = 2 * C; }
           bld.emit_attention(a); }
         { GemmOp g = bld.lin(x.out1, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn1.to_out.0.bias"); g.res = T0; g.res_ld = C; g.out = T1; g.out_ld = C;
@@ -795,7 +833,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
           a.B = B; a.H = H; a.Tq = TL; a.Tk = S; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
           if (av2) { a.v2 = 1; a.p_split = 1; a.qs = sq2; a.ks = kvs; a.vs = kvs; a.q_c0 = 0; a.k_c0 = x.kv_off; a.v_c0 = x.v_off; }
-          bld.emit_attention(a, Launch::MASK); }     // the key-padding bias comes from the call's mask (dropped without one)
+          if (ragged) { a.bias = pg.rt.prompt_bias; bld.emit_attention(a); }   // the prompt-length bias of the ragged tables
+          else bld.emit_attention(a, Launch::MASK); }     // the key-padding bias comes from the call's mask (dropped without one)
         { GemmOp g = bld.lin(x.out2, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn2.to_out.0.bias"); g.res = T1; g.res_ld = C; g.out = T0; g.out_ld = C;
           if (fold) emits_ln_input(g, rs3);
           bld.emit_gemm(g, x.out2); }
@@ -812,12 +851,12 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           const int i0 = bld.add_src(g, sff); bld.seg(g, i0, 0, 4 * C, 0);
           const int i1 = bld.add_src(g, sln); bld.seg(g, i1, 0, C, 0);          // raw split of the residual stream, written by out2's epilogue
           g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = x.bias_ff2p; g.res = cur.p; g.res_ld = C;
-          emits_block_out(g, outp); with_stats(g, outp.st, C); bld.emit_gemm(g, x.ff2p);
+          emits_block_out(g, outp); with_stats(g, outp.st, C); rag(g, o.level); bld.emit_gemm(g, x.ff2p);
         } else {
           { GemmOp g = bld.lin(x.ff2, sff, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_SPLIT; g.bias = h->weights.W(b + ".ff.net.2.bias"); g.res = T0; g.res_ld = C;
             g.out_hi = sh2.hi; g.out_lo = sh2.lo; g.out_split_ld = sh2.ld; bld.emit_gemm(g, x.ff2); }
           { GemmOp g = bld.lin(x.proj_out, sh2, TL); g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = h->weights.W(x.p + ".proj_out.bias"); g.res = cur.p; g.res_ld = C;
-            emits_block_out(g, outp); with_stats(g, outp.st, C); bld.emit_gemm(g, x.proj_out); }
+            emits_block_out(g, outp); with_stats(g, outp.st, C); rag(g, o.level); bld.emit_gemm(g, x.proj_out); }
         }
         cur = outp;
         bld.emit_tap(pg.taps, x.p, cur.p, o.level, C, TL);
@@ -846,6 +885,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         bld.seg(g, io, 0, s.c, -1); bld.seg(g, ie, 0, s.c, 0); bld.seg(g, io, 0, s.c, 0);
         g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
         emits_block_out(g, outp); with_stats(g, outp.st, s.c);
+        rag(g, o.level);
         bld.emit_gemm(g, s.w);
         cur = outp;
         bld.emit_tap(pg.taps, s.p, cur.p, o.level, s.c, TL);
@@ -863,12 +903,16 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         }
         const SplitBuf up = Builder::view(SP_A, TL, s.c);
         bld.emit_prep(cur.p, s.c, nullptr, 0, Tin, TL, PREP_RAW, nullptr, nullptr, up, nullptr, 1, 0, map_d);
+        // ragged: each entry's rows come from its OWN (T_b,l+1 -> T_b,l) nearest rule (the padded table can differ from it in
+        // fp32), and rows past the entry's length at this level are zeros
+        rag_prep(lens, o.level);
         Act outp = next_out(followed_by_push(pi), TL, s.c);
         outp.st = new_stats(s.c);
         GemmOp g = bld.gemm_base(s.w, TL);
         bld.conv3(g, up);
         g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
         emits_block_out(g, outp); with_stats(g, outp.st, s.c);
+        rag(g, o.level);
         bld.emit_gemm(g, s.w);
         cur = outp;
         bld.emit_tap(pg.taps, s.p, cur.p, o.level, s.c, TL);
@@ -883,12 +927,14 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
     if (xf_ok(c0, 0)) {
       const int i0 = bld.add_src(g, cur.sp);
       bld.xseg(g, i0, 0, c0, 3, 0, nkb_of(c0), 1, 0);
-      g.pre = bld.affine_desc(cur.st, c0, nullptr, 0, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), 0);
+      g.pre = bld.affine_desc(cur.st, c0, nullptr, 0, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), 0, 0);
     } else {
       bld.emit_prep_gn(cur.p, c0, cur.st, nullptr, 0, nullptr, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), nullptr, 0, a_h);
+      rag_prep(lens, 0);
       bld.conv3(g, a_h);
     }
     g.flags = EPI_BIAS | EPI_OUT_NCT; g.bias = h->weights.W("conv_out.bias"); g.out = nullptr;
+    rag(g, 0);                                             // (ragged: output frames past T_b are exact zeros)
     bld.emit_gemm(g, h->conv_out, Launch::OUT);
   }
   if (!bld.err && bld.upload_affine(st)) { set_error("affine descriptor upload failed"); return -2; }
@@ -950,7 +996,7 @@ int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& pro
         const bool fwd = l.input == Launch::X;
         const bool warm = fwd && film_ext != nullptr;
         rc = launch_nct_to_split(fwd ? x : content, fwd ? x_bstride : content_bstride, pg.B, l.i0, l.i1, l.split, st, warm ? film_ext : nullptr,
-                                 warm ? (long long)pg.B * h->film_total * 4 : 0);
+                                 warm ? (long long)pg.B * h->film_total * 4 : 0, l.lens);
         break;
       }
       case Launch::PREP: {
@@ -961,7 +1007,7 @@ int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& pro
         rc = launch_prep_split(p, st);
         break;
       }
-      case Launch::POOL_ATT: rc = launch_pool_attend(l.a, l.b, pg.B, l.i0, l.i1, l.i2, l.o, st); break;
+      case Launch::POOL_ATT: rc = launch_pool_attend(l.a, l.b, pg.B, l.i0, l.i1, l.i2, l.o, st, l.lens); break;
       case Launch::MASKBIAS:
         if (mask) rc = launch_mask_bias(mask, l.i0, l.o, st); else --count;
         break;
@@ -990,11 +1036,11 @@ void drop_all_programs(ns2vc_unet* h) {
   h->static_bufs.clear();
 }
 
-// Make the program for (B,T,S,ws) the active one, building it if it is not cached.
-int ensure_program(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st) {
+// Make the program for (B,T,S,ragged,ws) the active one, building it if it is not cached.
+int ensure_program(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st, bool ragged = false) {
   NS_REQUIRE(h->finalized, "ns2vc_unet_finalize() has not been called");
   NS_REQUIRE(ws != nullptr, "workspace is NULL");
-  auto is = [&](const Program& p) { return p.B == B && p.T == T && p.S == S && p.ws == ws; };
+  auto is = [&](const Program& p) { return p.B == B && p.T == T && p.S == S && p.ws == ws && p.ragged == ragged; };
   if (h->active >= 0) {
     if (is(h->progs[h->active])) return 0;
     // programs of different shapes may share one workspace (the caller's grow-only scratch buffer): the conditioning an inactive
@@ -1007,7 +1053,7 @@ int ensure_program(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st
     std::rotate(it, it + 1, h->progs.end());             // most recently active last
   } else {
     Program p;
-    const int rc = build_programs(h, B, T, S, ws, nullptr, &p, st);
+    const int rc = build_programs(h, B, T, S, ws, nullptr, &p, st, ragged);
     if (rc) return rc;
     // bounded: drop the least recently active program (it owns no device memory: everything lives in its workspace)
     if (h->progs.size() > ns2vc_unet::kMaxInactive) h->progs.erase(h->progs.begin());
@@ -1015,6 +1061,22 @@ int ensure_program(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st
   }
   h->active = (int)h->progs.size() - 1;
   return 0;
+}
+
+// forward / forward_film / time_table run the variant the last prepare_cond of this (B,T,S,ws) chose: ragged or padded.  When
+// another key has run since, neither variant is prepared any more; the call then takes the variant that is cached (the ragged
+// one only if it is the sole one), so that it fails on the missing prepare_cond without building a program for nothing.
+int ensure_program_for_call(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st) {
+  auto key = [&](const Program& p) { return p.B == B && p.T == T && p.S == S && p.ws == ws; };
+  bool ragged = false;
+  if (h->active >= 0 && key(h->progs[h->active])) {
+    ragged = h->progs[h->active].ragged;
+  } else {
+    bool have_padded = false, have_ragged = false;
+    for (const Program& p : h->progs) if (key(p)) (p.ragged ? have_ragged : have_padded) = true;
+    ragged = have_ragged && !have_padded;
+  }
+  return ensure_program(h, B, T, S, ws, st, ragged);
 }
 
 }  // namespace
@@ -1132,13 +1194,32 @@ int ns2vc_unet_prepare_cond(ns2vc_unet* h, const float* content, long long conte
   return 0;
 }
 
+int ns2vc_unet_prepare_cond_ragged(ns2vc_unet* h, const float* content, long long content_bstride, const float* prompt,
+                                   const int64_t* content_lengths, const int64_t* prompt_lengths, int B, int T, int S, void* ws,
+                                   ns2vc_stream stream) {
+  NS_REQUIRE(h && prompt && content_lengths && prompt_lengths, "null argument");
+  int rc = ensure_program(h, B, T, S, ws, (cudaStream_t)stream, true);
+  if (rc) return rc;
+  const int Cc = h->cfg.in_channels - h->cfg.latent_channels;
+  NS_REQUIRE(Cc == 0 || content != nullptr, "content is NULL but the model has %d content channels", Cc);
+  Program& pg = h->progs[h->active];
+  pg.has_mask = false;                                     // (the cross-attention reads the ragged program's prompt-length bias)
+  rc = launch_ragged_tables(reinterpret_cast<const long long*>(content_lengths), reinterpret_cast<const long long*>(prompt_lengths), pg.rt,
+                            (cudaStream_t)stream);
+  if (rc) return rc;
+  rc = run_program(h, pg, pg.prog_cond, nullptr, 0, nullptr, nullptr, content, content_bstride, prompt, nullptr, (cudaStream_t)stream);
+  if (rc) return rc;
+  pg.cond_ready = true;
+  return 0;
+}
+
 int ns2vc_unet_forward(ns2vc_unet* h, const float* x, long long x_bstride, const float* t, float* out, int B, int T, int S, void* ws,
                        ns2vc_stream stream) {
   NS_REQUIRE(h && x && t && out, "null argument");
-  int rc0 = ensure_program(h, B, T, S, ws, (cudaStream_t)stream);
+  int rc0 = ensure_program_for_call(h, B, T, S, ws, (cudaStream_t)stream);
   if (rc0) return rc0;
   const Program& pg = h->progs[h->active];
-  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond() must be called with the same (B,T,S,workspace) before forward");
+  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond%s() must be called with the same (B,T,S,workspace) before forward", pg.ragged ? "_ragged" : "");
   return run_program(h, pg, pg.prog_fwd, x, x_bstride, t, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
 }
 
@@ -1152,7 +1233,7 @@ size_t ns2vc_unet_time_table_floats(const ns2vc_unet* h, int n_rows) {
 int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float* table, int B, int T, int S, void* ws, ns2vc_stream stream) {
   NS_REQUIRE(h && t_rows && table, "null argument");
   NS_REQUIRE(n_rows > 0 && n_rows % B == 0, "time table: %d rows is not a multiple of the batch %d", n_rows, B);
-  int rc = ensure_program(h, B, T, S, ws, (cudaStream_t)stream);
+  int rc = ensure_program_for_call(h, B, T, S, ws, (cudaStream_t)stream);
   if (rc) return rc;
   const Program& pg = h->progs[h->active];
   NS_REQUIRE(pg.cond_ready || !h->cfg.add_embed_text, "ns2vc_unet_prepare_cond() must precede ns2vc_unet_time_table() (the pooled prompt embedding is added to every row)");
@@ -1183,10 +1264,10 @@ int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float*
 int ns2vc_unet_forward_film(ns2vc_unet* h, const float* x, long long x_bstride, const float* film_rows, float* out, int B, int T, int S,
                             void* ws, ns2vc_stream stream) {
   NS_REQUIRE(h && x && film_rows && out, "null argument");
-  int rc0 = ensure_program(h, B, T, S, ws, (cudaStream_t)stream);
+  int rc0 = ensure_program_for_call(h, B, T, S, ws, (cudaStream_t)stream);
   if (rc0) return rc0;
   const Program& pg = h->progs[h->active];
-  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond() must be called with the same (B,T,S,workspace) before forward");
+  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond%s() must be called with the same (B,T,S,workspace) before forward", pg.ragged ? "_ragged" : "");
   NS_REQUIRE(h->film_total > 0, "the model has no FiLM rows");
   h->film_ext = film_rows;
   const int rc = run_program(h, pg, pg.prog_fwd, x, x_bstride, nullptr, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);

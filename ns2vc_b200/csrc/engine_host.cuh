@@ -164,6 +164,7 @@ struct Launch {
   int tap_index = -1;
   int reads_film = 0;        // denoiser: reads the FiLM rows (pointers are rebased when the caller supplies precomputed rows)
   int time_path = 0;         // denoiser: timestep path (sinusoid -> MLP -> FiLM rows): skipped when the caller supplies precomputed FiLM rows
+  const int* lens = nullptr; // denoiser's ragged programs: per-entry lengths [B] of NCT2SPLIT frames / pooled prompt frames
 };
 
 // Named activations a program can copy out after the launch that produced them (diagnostics: per-layer parity tests).
@@ -297,15 +298,17 @@ struct TextTimeEmbedding {
     pool = ar.get<float>((size_t)B * R);
     proj = ar.get<float>((size_t)B * E);
   }
-  // `attend`: POOL_ATT (denoiser) or POOL_ATT_WIDE (condition encoders) - their sums run in different orders
+  // `attend`: POOL_ATT (denoiser) or POOL_ATT_WIDE (condition encoders) - their sums run in different orders.
+  // `lens`: per-entry prompt lengths [B] (the denoiser's ragged programs pool over each entry's own frames), or nullptr.
   void emit(ProgramBuilder& bld, const WeightRegistry& w, const std::string& p, const float* x, Launch::Input x_in, int S, int R,
-            int E, int heads, Launch::Kind attend, const PoolKV& pkv, float* y) const {
+            int E, int heads, Launch::Kind attend, const PoolKV& pkv, float* y, const int* lens = nullptr) const {
     const int B = bld.B;
     bld.emit_ln_apply(x, x_in, B * S, R, w.W(p + ".norm1.weight"), w.W(p + ".norm1.bias"), norm);
-    { Launch l; l.kind = Launch::POOL_CLS; l.a = norm; l.b = w.W(p + ".pool.positional_embedding"); l.i0 = S; l.i1 = R; l.o = tok; bld.out->push_back(l); }
+    { Launch l; l.kind = Launch::POOL_CLS; l.a = norm; l.b = w.W(p + ".pool.positional_embedding"); l.i0 = S; l.i1 = R; l.o = tok; l.lens = lens;
+      bld.out->push_back(l); }
     bld.emit_linear(linear_op(tok, (S + 1) * R, B, R, w.W(p + ".pool.q_proj.weight"), w.W(p + ".pool.q_proj.bias"), R, q, R));
     bld.emit_linear(linear_op(tok, R, B * (S + 1), R, pkv.W, pkv.b, 2 * R, kv, 2 * R));
-    { Launch l; l.kind = attend; l.a = q; l.b = kv; l.i0 = S + 1; l.i1 = R; l.i2 = heads; l.o = pool; bld.out->push_back(l); }
+    { Launch l; l.kind = attend; l.a = q; l.b = kv; l.i0 = S + 1; l.i1 = R; l.i2 = heads; l.o = pool; l.lens = lens; bld.out->push_back(l); }
     bld.emit_linear(linear_op(pool, R, B, R, w.W(p + ".proj.weight"), w.W(p + ".proj.bias"), E, proj, E));
     bld.emit_ln_apply(proj, Launch::NONE, B, E, w.W(p + ".norm2.weight"), w.W(p + ".norm2.bias"), y);
   }
@@ -332,7 +335,7 @@ struct Runner {
         if (in) o.x = in;
         return launch_small_linear(o, st);
       }
-      case Launch::POOL_CLS: return launch_pool_class_token(l.a, l.b, B, l.i0, l.i1, l.o, st);
+      case Launch::POOL_CLS: return launch_pool_class_token(l.a, l.b, B, l.i0, l.i1, l.o, st, l.lens);
       case Launch::MEMSET: {
         const cudaError_t e = cudaMemsetAsync(l.mem, 0, l.mem_bytes, st);
         if (e != cudaSuccess) { set_error("memset failed: %s", cudaGetErrorString(e)); return -2; }

@@ -191,7 +191,9 @@ static_assert(kGemmOpHotBytes % 16 == 0 && kGemmOpHotBytes <= 2688 && sizeof(Pre
 // XF: instantiation with the panel-mode paths (GroupNorm of the A operand applied in shared memory; BN = 64, one tile per CTA)
 // ENC: instantiation for the condition encoders (pre_engine.cu): ReLU and the per-row keep mask in the epilogue (EPI_RELU /
 // EPI_ROWMASK); the denoiser's instantiations do not carry that code
-template <int BN_, bool LNF, bool XF, bool ENC = false>
+// RAG: instantiation for the denoiser's ragged programs (GemmOp::row_len): rows past each utterance's length at this level are
+// stored as exact zeros, and in panel mode they read as the conv's zero padding and drop out of the GroupNorm statistics
+template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmOp op_param) {
   using Cfg = TileCfg<BN_>;
   constexpr int BN = Cfg::BN;
@@ -340,10 +342,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       for (int si = 0; si < op.nxs; ++si) {
         const XSeg& xs = op.xs[si];
         const int rows = xs.ntap == 3 ? kPanelRows : BM, tfirst = xt0 + (xs.ntap == 3 ? -1 : 0);
-        const int Tsrc = op.src[xs.src].T;
+        int Tsrc = op.src[xs.src].T;
+        if constexpr (RAG) Tsrc = min(Tsrc, ragged_rows(op.row_len, xb, op.len_shift));   // (panel sources sit at the output's level)
         if (xs.xf && !aff_done && gp < p_hi && gp + xs.ncb > p_lo) {   // (only if some of this segment's panels are this CTA's)
           for (int c = C + xt; c < ((C + 63) & ~63); c += 256) { aff[c] = 0.f; aff[kXfMaxC + c] = 0.f; }   // padding channels of the last block
-          prep_affine(pr, xb, C, kXfMaxC, aff, pg, pbv, fs, fbv, xt, 256, sync256);
+          prep_affine<RAG>(pr, xb, C, kXfMaxC, aff, pg, pbv, fs, fbv, xt, 256, sync256);
           aff_done = true;
           XTRACE(1);
         }
@@ -496,6 +499,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       const int t = t0 + r;
       const bool mv = t < op.T_out;
       const long long m = (long long)b * op.T_out + t;
+      bool rv = mv;                                         // row inside its utterance (RAG: stored as zeros otherwise)
+      if constexpr (RAG) rv = mv && t < ragged_rows(op.row_len, b, op.len_shift);
       if constexpr (!xpanel) {
         for (int kb = 0; kb < nkb; ++kb) {
           const int stage = kb % nst;
@@ -602,7 +607,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           acc_row32<BN>(acc_tile, r, 64 + hh * 32, gate);
           const int nbase = nt * 64 + hh * 32;              // logical output column
           if (nbase < op.n_valid) {                         // (uniform across the warp)
-            if (!mv) {
+            if (!rv) {
 #pragma unroll
               for (int j = 0; j < 32; ++j) val[j] = 0.f;
             } else if (pre_ok) {                            // biases were fetched before the accumulator wait
@@ -668,7 +673,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           if (cvalid) {
             const bool fullc = nbase + 32 <= op.n_valid;
             bool enc_hot = ENC && mv;                       // (the out-of-line path applies ReLU / mask itself: epi_value)
-            if (!mv) {
+            if (!rv) {
 #pragma unroll
               for (int j = 0; j < 32; ++j) acc[j] = 0.f;
             } else if (cc == cc0 && pre_ok) {
@@ -849,12 +854,12 @@ static int sm_count() {
   return n;
 }
 
-template <int BN_, bool LNF, bool XF, bool ENC = false>
+template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false>
 static int launch_bn(const GemmOp& op, cudaStream_t st) {
   using Cfg = TileCfg<BN_>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN_, LNF, XF, ENC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN_, LNF, XF, ENC, RAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) { set_error("gemm_tc: cannot set %d B dynamic smem: %s", Cfg::kSmemBytes, cudaGetErrorString(e)); return -2; }
     attr_set = true;
   }
@@ -862,7 +867,7 @@ static int launch_bn(const GemmOp& op, cudaStream_t st) {
   int grid = tiles;                                         // one tile per CTA (the epilogue reuses the stage buffers)
   dim3 cluster(1, 1, 1);
   if (XF && op.xmode && op.ksplit > 1) { grid = tiles * op.ksplit; cluster.x = (unsigned)op.ksplit; }   // split-K: the CTAs of a cluster share a tile
-  cudaError_t e = launch_kc(gemm_tc_kernel<BN_, LNF, XF, ENC>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmemBytes, st, cluster, op);
+  cudaError_t e = launch_kc(gemm_tc_kernel<BN_, LNF, XF, ENC, RAG>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmemBytes, st, cluster, op);
   if (e != cudaSuccess) { set_error("gemm_tc launch failed: %s", cudaGetErrorString(e)); return -2; }
   return 0;
 }
@@ -878,6 +883,11 @@ void plan_gemm(GemmOp& op) {
 int launch_gemm_tc(const GemmOp& op, cudaStream_t st) {
   if (op.N % 128) { set_error("gemm_tc: packed N=%d is not a multiple of 128", op.N); return -1; }
   const bool lnf = (op.flags & EPI_LNFOLD) != 0;
+  const bool rag = op.row_len != nullptr;
+  if (rag && (lnf || op.bn != 64 || (op.flags & (EPI_GEGLU | EPI_RELU | EPI_ROWMASK)))) {
+    set_error("gemm_tc: ragged row masks need a plain 64-wide tile without a folded LayerNorm");
+    return -1;
+  }
   if (op.flags & (EPI_RELU | EPI_ROWMASK)) {
     if (lnf || op.xmode || op.bn != 64 || (op.flags & EPI_GEGLU)) { set_error("gemm_tc: ReLU / row-mask epilogues need a plain 64-wide tile"); return -1; }
     if ((op.flags & EPI_ROWMASK) && !op.rowmask) { set_error("gemm_tc: EPI_ROWMASK without a mask"); return -1; }
@@ -888,12 +898,13 @@ int launch_gemm_tc(const GemmOp& op, cudaStream_t st) {
     if (lnf || op.bn != 64 || op.nxs < 1 || op.nxs > kMaxXSeg) { set_error("gemm_tc: panel mode needs a plain 64-wide tile and 1..%d segments", kMaxXSeg); return -1; }
     if (op.pre == nullptr) { set_error("gemm_tc: panel mode without GroupNorm parameters"); return -1; }
     if (op.ksplit != 1 && op.ksplit != 2) { set_error("gemm_tc: ksplit must be 1 or 2"); return -1; }
-    return launch_bn<64, false, true>(op, st);
+    return rag ? launch_bn<64, false, true, false, true>(op, st) : launch_bn<64, false, true>(op, st);
   }
   if (op.nkb_total <= 0) { set_error("gemm_tc: empty K"); return -1; }
   if ((op.bn == 128) != ((op.flags & EPI_GEGLU) != 0)) { set_error("gemm_tc: the 128-wide tile is the GEGLU instantiation (plan_gemm)"); return -1; }
   if (op.bn == 128) return lnf ? launch_bn<128, true, false>(op, st) : launch_bn<128, false, false>(op, st);
   if (op.bn != 64) { set_error("gemm_tc: plan_gemm() was not called"); return -1; }
+  if (rag) return launch_bn<64, false, false, false, true>(op, st);
   return lnf ? launch_bn<64, true, false>(op, st) : launch_bn<64, false, false>(op, st);
 }
 

@@ -131,6 +131,8 @@ int launch_ln_apply(const float* x, int ld, int M, int C, float eps, const float
 // row (two 16-byte loads, 16-byte hi + lo stores); rows may be remapped (stride-2 decimation for
 // the downsample convs, nearest-upsample index table).
 // ---------------------------------------------------------------------------------------------
+// RAG: ragged programs (op.row_len): rows past the entry's length are zeros, the GroupNorm counts only the valid rows
+template <bool RAG>
 __global__ void __launch_bounds__(256) prep_split_kernel(PrepOp op) {
   span_begin(op.span);
   pdl_trigger();
@@ -147,14 +149,14 @@ __global__ void __launch_bounds__(256) prep_split_kernel(PrepOp op) {
   // the first chunk's loads are in flight while the block derives the GroupNorm affine
   PrepChunk k0;
   const bool have = i < total;
-  if (have) prep_load_at(op, b, C, i / chunks, i % chunks, k0);
+  if (have) prep_load_at<RAG>(op, b, C, i / chunks, i % chunks, k0);
   float fs[kPrepSlots], fb[kPrepSlots];
   prep_fetch_film(op, op.gn.film, b, C, fs, fb, threadIdx.x, blockDim.x);
-  prep_affine(op, b, C, C, aff, pg, pb, fs, fb, threadIdx.x, blockDim.x, BlockSync());
+  prep_affine<RAG>(op, b, C, C, aff, pg, pb, fs, fb, threadIdx.x, blockDim.x, BlockSync());
   if (have) prep_finish(op, b, C, aff, k0);
   for (i += stride; i < total; i += stride) {
     PrepChunk k;
-    prep_load_at(op, b, C, i / chunks, i % chunks, k);
+    prep_load_at<RAG>(op, b, C, i / chunks, i % chunks, k);
     prep_finish(op, b, C, aff, k);
   }
   span_end(op.span);
@@ -170,7 +172,8 @@ int launch_prep_split(const PrepOp& op, cudaStream_t st) {
   if (bx < 1) bx = 1;
   const size_t smem = (op.mode != PREP_RAW) ? (size_t)prep_affine_floats(C) * sizeof(float) : 0;
   if (smem > 48 * 1024 || (op.mode != PREP_RAW && !op.scale && (C > kPrepSlots * 256 || op.gn.G > 64))) { set_error("prep_split: C=%d too large", C); return -1; }
-  cudaError_t e = launch_k(prep_split_kernel, dim3(bx, op.B), dim3(256), smem, st, op);
+  cudaError_t e = op.row_len ? launch_k(prep_split_kernel<true>, dim3(bx, op.B), dim3(256), smem, st, op)
+                             : launch_k(prep_split_kernel<false>, dim3(bx, op.B), dim3(256), smem, st, op);
   if (e != cudaSuccess) { set_error("prep_split launch failed: %s", cudaGetErrorString(e)); return -2; }
   return 0;
 }
@@ -264,9 +267,10 @@ int launch_ln_split(const float* x, int ld, int M, int C, float eps, const float
   return 0;
 }
 
-// [B, C, T] fp32 -> split token-major [B, T, out.ld]; 32x32 smem transpose, zero-fills c >= C.
+// [B, C, T] fp32 -> split token-major [B, T, out.ld]; 32x32 smem transpose, zero-fills c >= C (RAG: and t >= row_len[b]).
+template <bool RAG>
 __global__ void nct_to_split_kernel(const float* __restrict__ x, long long bstride, int C, int T, SplitBuf out,
-                                    const char* warm, long long warm_bytes) {
+                                    const char* warm, long long warm_bytes, const int* __restrict__ row_len) {
   pdl_trigger();
   // first kernel of a forward: pull this step's FiLM rows (a slice of the run's timestep table, cold in L2) towards L2 so that
   // the 22 conv2 launches that read them later do not each wait for HBM
@@ -279,9 +283,11 @@ __global__ void nct_to_split_kernel(const float* __restrict__ x, long long bstri
   const int b = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   const float* xb = x + (long long)b * bstride;
+  int Tv = T;
+  if constexpr (RAG) Tv = min(T, __ldg(row_len + b));
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     int c = c0 + i, t = t0 + threadIdx.x;
-    tile[i][threadIdx.x] = (c < C && t < T) ? xb[(long long)c * T + t] : 0.f;
+    tile[i][threadIdx.x] = (c < C && t < Tv) ? xb[(long long)c * T + t] : 0.f;
   }
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -296,9 +302,10 @@ __global__ void nct_to_split_kernel(const float* __restrict__ x, long long bstri
   }
 }
 int launch_nct_to_split(const float* x, long long bstride, int B, int C, int T, SplitBuf out, cudaStream_t st, const void* warm,
-                        long long warm_bytes) {
+                        long long warm_bytes, const int* row_len) {
   dim3 grid(ceil_div(T, 32), ceil_div(out.ld, 32), B), block(32, 8);
-  launch_k(nct_to_split_kernel, grid, block, 0, st, x, bstride, C, T, out, (const char*)warm, warm_bytes);
+  if (row_len) launch_k(nct_to_split_kernel<true>, grid, block, 0, st, x, bstride, C, T, out, (const char*)warm, warm_bytes, row_len);
+  else launch_k(nct_to_split_kernel<false>, grid, block, 0, st, x, bstride, C, T, out, (const char*)warm, warm_bytes, row_len);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -423,32 +430,39 @@ int launch_small_linear(const LinOp& op, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 // AttentionPooling pieces (reference embeddings.py:499-546); once per utterance.
 // ---------------------------------------------------------------------------------------------
+// RAG: the class token is the mean over the entry's first lens[b] frames (the utterance's own prompt)
+template <bool RAG>
 __global__ void pool_class_token_kernel(const float* __restrict__ xn, const float* __restrict__ pos, int S, int C,
-                                        float* __restrict__ tokens) {
+                                        float* __restrict__ tokens, const int* __restrict__ lens) {
   const int b = blockIdx.x;
+  const int Sb = RAG ? lens[b] : S;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float s = 0.f;
-    for (int t = 0; t < S; ++t) s += xn[((long long)b * S + t) * C + c];
-    tokens[((long long)b * (S + 1)) * C + c] = s / (float)S + pos[c];
+    for (int t = 0; t < Sb; ++t) s += xn[((long long)b * S + t) * C + c];
+    tokens[((long long)b * (S + 1)) * C + c] = s / (float)Sb + pos[c];
     for (int t = 0; t < S; ++t) tokens[((long long)b * (S + 1) + 1 + t) * C + c] = xn[((long long)b * S + t) * C + c];
   }
 }
-int launch_pool_class_token(const float* xn, const float* pos, int B, int S, int C, float* tokens, cudaStream_t st) {
-  pool_class_token_kernel<<<B, 256, 0, st>>>(xn, pos, S, C, tokens);
+int launch_pool_class_token(const float* xn, const float* pos, int B, int S, int C, float* tokens, cudaStream_t st, const int* lens) {
+  if (lens) pool_class_token_kernel<true><<<B, 256, 0, st>>>(xn, pos, S, C, tokens, lens);
+  else pool_class_token_kernel<false><<<B, 256, 0, st>>>(xn, pos, S, C, tokens, lens);
   NS_LAUNCH_CHECK();
   return 0;
 }
 
 // one warp per (b, head): softmax over S1 keys of (q*s).(k*s), s = dph^-1/4; out = sum_j w_j v_j
+// RAG: over the class token and the entry's first lens[b] frames only
+template <bool RAG>
 __global__ void pool_attend_kernel(const float* __restrict__ q, const float* __restrict__ kv, int S1, int C, int heads,
-                                   float* __restrict__ out) {
+                                   float* __restrict__ out, const int* __restrict__ lens) {
   const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const int K1 = RAG ? lens[b] + 1 : S1;                 // keys attended (kv rows keep the stride S1)
   const int dph = C / heads;
   const int lane = threadIdx.x;
   const float sc = 1.0f / sqrtf(sqrtf((float)dph));
   const float* qh = q + (long long)b * C + h * dph;
   float mx = -INFINITY;
-  for (int j = lane; j < S1; j += 32) {
+  for (int j = lane; j < K1; j += 32) {
     const float* kr = kv + ((long long)b * S1 + j) * 2 * C + h * dph;
     float s = 0.f;
     for (int d = 0; d < dph; ++d) s += (qh[d] * sc) * (kr[d] * sc);
@@ -458,7 +472,7 @@ __global__ void pool_attend_kernel(const float* __restrict__ q, const float* __r
   float den = 0.f;
   float acc[16];
   for (int d = 0; d < 16; ++d) acc[d] = 0.f;
-  for (int j = lane; j < S1; j += 32) {
+  for (int j = lane; j < K1; j += 32) {
     const float* kr = kv + ((long long)b * S1 + j) * 2 * C + h * dph;
     float s = 0.f;
     for (int d = 0; d < dph; ++d) s += (qh[d] * sc) * (kr[d] * sc);
@@ -473,9 +487,10 @@ __global__ void pool_attend_kernel(const float* __restrict__ q, const float* __r
     if (lane == 0) out[(long long)b * C + h * dph + d] = a / den;
   }
 }
-int launch_pool_attend(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st) {
+int launch_pool_attend(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st, const int* lens) {
   if (C % heads || C / heads > 16) { set_error("pool_attend: dim/head %d/%d unsupported", C, heads); return -1; }
-  pool_attend_kernel<<<B * heads, 32, 0, st>>>(q, kv, S1, C, heads, out);
+  if (lens) pool_attend_kernel<true><<<B * heads, 32, 0, st>>>(q, kv, S1, C, heads, out, lens);
+  else pool_attend_kernel<false><<<B * heads, 32, 0, st>>>(q, kv, S1, C, heads, out, lens);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -487,6 +502,27 @@ __global__ void mask_bias_kernel(const uint8_t* __restrict__ mask, int n, float*
 }
 int launch_mask_bias(const uint8_t* mask, int n, float* bias, cudaStream_t st) {
   mask_bias_kernel<<<ceil_div(n, 256), 256, 0, st>>>(mask, n, bias);
+  NS_LAUNCH_CHECK();
+  return 0;
+}
+
+// Ragged programs: one block per batch entry turns its content / prompt lengths into the program's tables.  The key biases are
+// -inf (not the reference mask's -10000): the attention kernels already stage -inf for keys past Tk, so a masked key contributes
+// exactly 0 to the online softmax, and the staged bias row of a short utterance equals that of the utterance run alone.
+__global__ void ragged_tables_kernel(const long long* __restrict__ clen, const long long* __restrict__ plen, RaggedTables r) {
+  const int b = blockIdx.x;
+  const int T = (int)min(max(clen[b], 1LL), (long long)r.T), S = (int)min(max(plen[b], 1LL), (long long)r.S);
+  if (threadIdx.x == 0) { r.lens[b] = T; r.lens[r.B + b] = S; }
+  for (int s = threadIdx.x; s < r.S; s += blockDim.x) r.prompt_bias[(long long)b * r.S + s] = s < S ? 0.f : -INFINITY;
+  for (int l = 0; l < r.nlev; ++l) {
+    if (!r.key_bias[l]) continue;
+    const int Tl = r.Tl[l], tb = ((T - 1) >> l) + 1;
+    for (int t = threadIdx.x; t < Tl; t += blockDim.x) r.key_bias[l][(long long)b * Tl + t] = t < tb ? 0.f : -INFINITY;
+  }
+}
+int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st) {
+  if (r.nlev > kRagMaxLevels) { set_error("ragged tables: %d levels", r.nlev); return -1; }
+  ragged_tables_kernel<<<r.B, 256, 0, st>>>(content_lengths, prompt_lengths, r);
   NS_LAUNCH_CHECK();
   return 0;
 }

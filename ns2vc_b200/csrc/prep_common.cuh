@@ -10,14 +10,26 @@ namespace ns2vc {
 struct PrepChunk { float v[8]; int t, c0; bool rowok; };
 constexpr int kPrepSlots = 4;                              // per-thread channel slots of the affine: C <= kPrepSlots * blockDim.x
 
-// Fetch 8 channels [ck*8, ck*8+8) of output row t (zero outside the sources).
+// Valid rows of batch entry b in a ragged program: ceil(len / 2^shift), the stride-2 conv length rule applied `shift` times
+__device__ __forceinline__ int ragged_rows(const int* len, int b, int shift) { return ((__ldg(len + b) - 1) >> shift) + 1; }
+
+// Fetch 8 channels [ck*8, ck*8+8) of output row t (zero outside the sources; RAG: also past the entry's length).
+template <bool RAG = false>
 __device__ __forceinline__ void prep_load_at(const PrepOp& op, int b, int C, int t, int ck, PrepChunk& k) {
   k.t = t;
   k.c0 = ck * 8;
-  const int ts = op.rowmap ? __ldg(op.rowmap + t) : t * op.row_mul + op.row_add;
+  int ts;
+  if constexpr (RAG) {
+    // nearest upsample (rowmap set): this entry's own rule from its length one level down (len_shift + 1) to its length here
+    ts = op.rowmap ? nearest_src_index(t, ragged_rows(op.row_len, b, op.len_shift + 1), ragged_rows(op.row_len, b, op.len_shift))
+                   : t * op.row_mul + op.row_add;
+  } else {
+    ts = op.rowmap ? __ldg(op.rowmap + t) : t * op.row_mul + op.row_add;
+  }
 #pragma unroll
   for (int j = 0; j < 8; ++j) k.v[j] = 0.f;
   k.rowok = ts >= 0 && ts < op.T_src;
+  if constexpr (RAG) k.rowok = k.rowok && t < ragged_rows(op.row_len, b, op.len_shift);
   if (k.rowok && k.c0 < C) {
     const int c0 = k.c0;
     const bool in1 = c0 < op.C1;
@@ -96,7 +108,8 @@ __device__ __forceinline__ void prep_fetch_film(const PrepOp& op, const float* f
 // aff[2*Cs .. 2*Cs + 2G) as scratch).  GroupNorm finalise from the per-channel sums the producer epilogues accumulated
 // (reference nn.GroupNorm: biased variance over T x C/G elements; resnet.py:536,557, transformer_1d.py:134), then
 // (1 + scale) / shift of the FiLM row (resnet.py:627-629).  Called by every thread of the group; ends with sync().
-template <class Sync>
+// RAG: the statistics cover the entry's valid rows only (the producers stored zeros past them): n = rows_b x C/G.
+template <bool RAG = false, class Sync>
 __device__ __forceinline__ void prep_affine(const PrepOp& op, int b, int C, int Cs, float* aff, const float* pg, const float* pb,
                                             const float* fs, const float* fb, int tid, int nthr, Sync sync) {
   if (op.mode == PREP_RAW) return;
@@ -116,7 +129,9 @@ __device__ __forceinline__ void prep_affine(const PrepOp& op, int b, int C, int 
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
       if ((tid & 31) == 0) {
-        const double inv = g.inv_n != 0.0 ? g.inv_n : 1.0 / ((double)op.T_src * cpg);   // (a double division is ~0.1 us on the launch's critical path)
+        double inv;
+        if constexpr (RAG) inv = 1.0 / ((double)ragged_rows(op.row_len, b, op.len_shift) * cpg);
+        else inv = g.inv_n != 0.0 ? g.inv_n : 1.0 / ((double)op.T_src * cpg);   // (a double division is ~0.1 us on the launch's critical path)
         const double mean = s * inv;
         double var = q * inv - mean * mean;
         if (var < 0) var = 0;

@@ -59,13 +59,21 @@ class DenoiserSession:
 
     The reference asserts ``not isnan(x)`` on the host before every denoiser call (model.py:404: one
     device->host sync per step).  Here the sampler-step kernel accumulates a device flag and the host checks
-    it ONCE after the run, raising the same ``AssertionError``."""
+    it ONCE after the run, raising the same ``AssertionError``.
+
+    Ragged batches: with ``content_lengths`` [B] (and optionally ``prompt_lengths`` [B], default S; no ``prompt_mask``)
+    the session runs the engine's ragged program, for every sampling method.  Row b of a result is then utterance b
+    sampled alone on x_T[b, :, :T_b], content[b, :, :T_b], prompt[b, :S_b]; its frames >= T_b are exactly 0 and input
+    values past the lengths are never read.  x_T's padding is zeroed on entry and the denoiser output is zero there, so
+    the DPM-Solver++ / UniPC state stays zero in the padding.  DDPM / DDIM noise is still ``randn_like`` over the padded
+    [B, C, T] tensor (the default generator advances as for one padded call, not as for B separate runs): a row equals its
+    B = 1 run when the caller injects the per-row noise (``noise``), or with the deterministic samplers."""
 
     MAX_GRAPHS = 4                                           # LRU bound of captured loops per session
     CAPTURE_AFTER = 3                                        # the loop is captured on its third run, replayed from the fourth
 
     def __init__(self, unet: UNet1DConditionModel, content_BCT: Optional[torch.Tensor], prompt_BSC: torch.Tensor,
-                 prompt_mask: Optional[torch.Tensor], T: Optional[int] = None):
+                 prompt_mask: Optional[torch.Tensor], T: Optional[int] = None, content_lengths=None, prompt_lengths=None):
         if not prompt_BSC.is_cuda:
             raise RuntimeError("DenoiserSession needs CUDA tensors (no CPU path)")
         self.unet = unet
@@ -84,6 +92,15 @@ class DenoiserSession:
         self.content = torch.empty((self.B, self.Cc, self.T), **f32) if self.Cc > 0 else None
         self.prompt = torch.empty((self.B, self.S, unet.cfg.cross_attention_dim), **f32)
         self.mask = torch.empty((self.B, self.S), dtype=torch.uint8, device=self.dev) if prompt_mask is not None else None
+        self.ragged = content_lengths is not None
+        if self.ragged:
+            if prompt_mask is not None:
+                raise ValueError("a ragged session takes prompt_lengths, not a prompt mask")
+            self.clen = torch.empty((self.B,), dtype=torch.int64, device=self.dev)
+            self.plen = torch.empty((self.B,), dtype=torch.int64, device=self.dev)
+            self.keep = torch.empty((self.B, 1, self.T), dtype=torch.bool, device=self.dev)   # frame t < T_b
+        elif prompt_lengths is not None:
+            raise ValueError("prompt_lengths applies to ragged sessions (content_lengths); pass a prompt mask instead")
         self.L = _lib.lib()
         self.h = unet.engine(self.dev)
         self.Cl, self.Co = unet.latent_channels, unet.cfg.out_channels
@@ -96,10 +113,18 @@ class DenoiserSession:
         self._chunk_graphs = collections.OrderedDict()       # captured DDPM / DDIM chunks, by (kind, noise draws)
         self._chunk = None                                   # their static windows (allocated on the first such run)
         self._wsig = unet._wsig
-        self.set_cond(content_BCT, prompt_BSC, prompt_mask)
+        self.set_cond(content_BCT, prompt_BSC, prompt_mask, content_lengths, prompt_lengths)
 
-    def set_cond(self, content_BCT, prompt_BSC, prompt_mask):
-        """Copy a new utterance batch (same shapes) into the static buffers."""
+    def set_cond(self, content_BCT, prompt_BSC, prompt_mask, content_lengths=None, prompt_lengths=None):
+        """Copy a new utterance batch (same shapes; for a ragged session, new lengths) into the static buffers."""
+        if (content_lengths is not None) != self.ragged:
+            raise ValueError("content_lengths must be given exactly when the session is ragged")
+        if self.ragged:
+            cl = check_lengths(content_lengths, self.B, self.T, "content_lengths")
+            pl = check_lengths(prompt_lengths, self.B, self.S, "prompt_lengths") if prompt_lengths is not None else [self.S] * self.B
+            self.clen.copy_(torch.tensor(cl, dtype=torch.int64), non_blocking=False)
+            self.plen.copy_(torch.tensor(pl, dtype=torch.int64), non_blocking=False)
+            self.keep.copy_(torch.arange(self.T, device=self.dev)[None, None, :] < self.clen[:, None, None])
         if self.content is not None:
             self.content.copy_(content_BCT, non_blocking=True)
         self.prompt.copy_(prompt_BSC, non_blocking=True)
@@ -113,6 +138,15 @@ class DenoiserSession:
         return torch.cuda.current_stream(self.dev).cuda_stream
 
     def prepare(self):
+        if self.ragged:
+            with torch.cuda.device(self.dev):
+                _lib.check(self.L.ns2vc_unet_prepare_cond_ragged(
+                    self.h, self.content.data_ptr() if self.content is not None else None,
+                    (self.Cc * self.T) if self.content is not None else 0, self.prompt.data_ptr(), self.clen.data_ptr(),
+                    self.plen.data_ptr(), self.B, self.T, self.S, self.ws.data_ptr(), self._stream()))
+            self._prepared = True
+            self.unet.__dict__["_cond_owner"] = self
+            return
         with torch.cuda.device(self.dev):
             _lib.check(self.L.ns2vc_unet_prepare_cond(
                 self.h, self.content.data_ptr() if self.content is not None else None,
@@ -199,6 +233,12 @@ class DenoiserSession:
         res = self._body_dpm(ent, use_first) if kind == "dpm" else self._body_unipc(ent, use_first)
         return res.clone()
 
+    def _unpad(self, x: torch.Tensor) -> torch.Tensor:
+        """Ragged sessions: zero every frame past its utterance's length (in place; NaN-safe)."""
+        if self.ragged:
+            x.masked_fill_(~self.keep, 0.0)
+        return x
+
     def _check_nan(self):
         if int(self.nan_flag.item()) != 0:
             # same exception type as the reference's per-call guard (model.py:404)
@@ -215,7 +255,7 @@ class DenoiserSession:
     def _run(self, kind, x_T, ns, ts, first_out, extra):
         assert self.Cl == self.Co, "x_start parameterisation needs out_channels == latent channels"
         self._sync_engine()
-        self.x_in.copy_(x_T, non_blocking=True)
+        self._unpad(self.x_in.copy_(x_T, non_blocking=True))
         use_first = first_out is not None
         if use_first:
             self.first_out.copy_(first_out, non_blocking=True)
@@ -253,7 +293,7 @@ class DenoiserSession:
             self.unet.__dict__["_cond_owner"] = self
             res = ent["out"].clone()
         self._check_nan()
-        return res
+        return self._unpad(res)
 
     # ------------------------------------------------------------------ public samplers
     def sample_dpmpp_2m(self, x_T: torch.Tensor, ns, ts: torch.Tensor, lower_order_final: bool = True,
@@ -347,7 +387,7 @@ class DenoiserSession:
             ent["runs"] += 1
         use_graph = noise is None and os.environ.get("NS2VC_GRAPH", "1") != "0" and ent["runs"] >= self.CAPTURE_AFTER
         cb = self._chunk_buffers()
-        cb["x"].copy_(x_T, non_blocking=True)
+        self._unpad(cb["x"].copy_(x_T, non_blocking=True))
         self.nan_flag.zero_()
         self.prepare()
         j = 0
@@ -380,7 +420,7 @@ class DenoiserSession:
             j += L
         res = cb["x"].clone()
         self._check_nan()
-        return res
+        return self._unpad(res)
 
     def sample_ddpm(self, x_T: torch.Tensor, timesteps=None, noise: Optional[torch.Tensor] = None,
                     first_out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -408,6 +448,17 @@ class DenoiserSession:
         return self._chain("ddim", x_T, ("ddim", S, eta), lambda: coefs.ddim_table(buf, total, S, eta), first_out, noise)
 
 
+def check_lengths(lengths, B: int, limit: int, name: str) -> list:
+    """Per-utterance lengths as a list of B ints in [1, limit]; ValueError otherwise."""
+    vals = [int(v) for v in (lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
+    if len(vals) != B:
+        raise ValueError(f"{name} must have {B} entries, got {len(vals)}")
+    bad = [v for v in vals if not 1 <= v <= limit]
+    if bad:
+        raise ValueError(f"{name} must lie in [1, {limit}], got {bad}")
+    return vals
+
+
 _BUFFERS = {}
 
 
@@ -417,22 +468,25 @@ def _diffusion_buffers(timesteps: int = 1000) -> dict:
     return _BUFFERS[timesteps]
 
 
-def get_session(unet: UNet1DConditionModel, content_BCT, prompt_BSC, prompt_mask, T=None) -> DenoiserSession:
-    """Session cache per (B, T, S, mask?) on the module: captured graphs and static buffers are reused
-    across utterance batches of the same shape."""
+def get_session(unet: UNet1DConditionModel, content_BCT, prompt_BSC, prompt_mask, T=None, content_lengths=None,
+                prompt_lengths=None) -> DenoiserSession:
+    """Session cache per (B, T, S, mask?, ragged?) on the module: captured graphs and static buffers are reused
+    across utterance batches of the same shape (a ragged session across any lengths)."""
     B, S = prompt_BSC.shape[0], prompt_BSC.shape[1]
     Tn = content_BCT.shape[2] if content_BCT is not None else T
-    key = (B, Tn, S, prompt_mask is not None, str(prompt_BSC.device))
+    ragged = content_lengths is not None
+    key = (B, Tn, S, prompt_mask is not None, str(prompt_BSC.device)) + (("ragged",) if ragged else ())
     cache = unet.__dict__.setdefault("_sessions", {})
     sess = cache.get(key)
     if sess is None or sess.h != unet.engine(prompt_BSC.device):
         while len(cache) >= 8:                               # bounded: oldest shape first (dicts keep insertion order)
             cache.pop(next(iter(cache)))
-        sess = DenoiserSession(unet, content_BCT, prompt_BSC, prompt_mask, T=T)
+        sess = DenoiserSession(unet, content_BCT, prompt_BSC, prompt_mask, T=T, content_lengths=content_lengths,
+                               prompt_lengths=prompt_lengths)
         cache = unet.__dict__.setdefault("_sessions", {})     # (the workspace may have grown and dropped the old sessions)
         cache[key] = sess
     else:
-        sess.set_cond(content_BCT, prompt_BSC, prompt_mask)
+        sess.set_cond(content_BCT, prompt_BSC, prompt_mask, content_lengths, prompt_lengths)
     return sess
 
 
