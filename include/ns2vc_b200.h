@@ -274,6 +274,40 @@ void ns2vc_mel_destroy(ns2vc_mel* h);
 int ns2vc_log_mel(const ns2vc_mel* h, const float* x, long long x_bstride, long long n, const int64_t* lengths, float* mel, int S,
                   int B, ns2vc_stream stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Vocoder: `Vocos.decode` (vocos/pretrained.py) of the mel configuration the reference loads (charactr/vocos-mel-24khz,
+ * model.py:689-691): VocosBackbone (vocos/models.py: Conv1d embed k=7, LayerNorm, ConvNeXtBlocks of vocos/modules.py, final
+ * LayerNorm; no AdaLayerNorm) and ISTFTHead (vocos/heads.py: Linear to n_fft + 2, exp / clip 100 / phase, the "same"-padded
+ * ISTFT of vocos/spectral_ops.py).  A ragged batch decodes row b as if it were decoded alone on its first lengths[b] frames.
+ * Same conventions as the encoders: raw device pointers, caller-owned workspace, stream-ordered, int errors; the first call for
+ * a new (B, T, workspace) builds the launch program on the host, later calls allocate nothing and may be captured. */
+typedef struct ns2vc_voc ns2vc_voc;
+typedef struct ns2vc_voc_cfg {       /* VocosBackbone(input_channels, dim, intermediate_dim, num_layers) + ISTFTHead(dim, n_fft,  */
+  int input_channels, dim, intermediate_dim, num_layers, n_fft, hop_length;   /* hop_length, padding="same")                     */
+} ns2vc_voc_cfg;
+/* Only the "same" padding and no AdaLayerNorm exist here; the configuration must have n_fft = 4 hop_length (a power of two,
+ * 64 .. 2048), dim a multiple of 128 up to 1024 and intermediate_dim a multiple of 64. */
+int ns2vc_voc_create(const ns2vc_voc_cfg* cfg, ns2vc_voc** out);
+void ns2vc_voc_destroy(ns2vc_voc* h);
+int ns2vc_voc_num_weights(const ns2vc_voc* h);                                  /* backbone.* / head.* keys of Vocos.state_dict() */
+int ns2vc_voc_weight_info(const ns2vc_voc* h, int i, const char** name, int64_t shape[4], int* ndim);
+int ns2vc_voc_load_weight(ns2vc_voc* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream);
+int ns2vc_voc_finalize(ns2vc_voc* h, ns2vc_stream stream);                      /* strict: fails on a missing key                   */
+int ns2vc_voc_workspace_bytes(const ns2vc_voc* h, int B, int T, size_t* bytes);
+/* Vocos.decode: mel [B, input_channels, T] fp32 (row-contiguous, batch stride mel_bstride floats), lengths [B] int64 device or
+ * NULL (every row T; values are clamped into [1, T]) -> audio [B, T * hop_length] fp32.  Row b equals the row decoded alone on
+ * mel[b, :, :lengths[b]]; its samples >= lengths[b] * hop_length are exactly 0 and mel frames past lengths[b] are never read. */
+int ns2vc_voc_decode(ns2vc_voc* h, const float* mel, long long mel_bstride, const int64_t* lengths, float* audio, int B, int T,
+                     void* ws, ns2vc_stream stream);
+/* The head's ISTFT stage alone: head_out [B, T, n_fft + 2] fp32 token-major (log-magnitudes, then phases) -> audio as above. */
+int ns2vc_voc_istft(ns2vc_voc* h, const float* head_out, const int64_t* lengths, float* audio, int B, int T, ns2vc_stream stream);
+/* Diagnostics for the parity tests: activations after backbone.norm, each convnext block, final_layer_norm ([B, T, dim]) and
+ * head.out ([B, T, channels] with channels = n_fft + 2 rounded up to a multiple of 4: columns past n_fft + 2 are padding). */
+int ns2vc_voc_num_taps(const ns2vc_voc* h);
+int ns2vc_voc_tap_info(const ns2vc_voc* h, int i, const char** name, int* rows, int* channels);
+int ns2vc_voc_set_tap(ns2vc_voc* h, int i, float* dst);
+int ns2vc_voc_launch_count(const ns2vc_voc* h);   /* kernels launched by the last decode */
+
 #ifdef __cplusplus
 }
 #endif

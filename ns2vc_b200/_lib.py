@@ -33,6 +33,11 @@ class PreCfg(C.Structure):
                 ("ref_dim", C.c_int), ("ref_heads", C.c_int), ("n_heads", C.c_int), ("ffn_kernel", C.c_int)]
 
 
+class VocCfg(C.Structure):
+    _fields_ = [("input_channels", C.c_int), ("dim", C.c_int), ("intermediate_dim", C.c_int), ("num_layers", C.c_int),
+                ("n_fft", C.c_int), ("hop_length", C.c_int)]
+
+
 class DpmCoef(C.Structure):
     _fields_ = [("alpha_s", C.c_float), ("sigma_s", C.c_float), ("c_x", C.c_float), ("c_m", C.c_float),
                 ("c_d", C.c_float), ("inv_r0", C.c_float), ("order", C.c_int)]
@@ -107,6 +112,20 @@ SIGNATURES = {
     "ns2vc_pre_tap_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ns2vc_pre_set_tap": (C.c_int, [_P, C.c_int, _P]),
     "ns2vc_pre_launch_count": (C.c_int, [_P]),
+    # vocoder (Vocos.decode)
+    "ns2vc_voc_create": (C.c_int, [C.POINTER(VocCfg), C.POINTER(_P)]),
+    "ns2vc_voc_destroy": (None, [_P]),
+    "ns2vc_voc_num_weights": (C.c_int, [_P]),
+    "ns2vc_voc_weight_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
+    "ns2vc_voc_load_weight": (C.c_int, [_P, C.c_char_p, _P, C.POINTER(C.c_int64), C.c_int, _P]),
+    "ns2vc_voc_finalize": (C.c_int, [_P, _P]),
+    "ns2vc_voc_workspace_bytes": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ns2vc_voc_decode": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_voc_istft": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P]),
+    "ns2vc_voc_num_taps": (C.c_int, [_P]),
+    "ns2vc_voc_tap_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "ns2vc_voc_set_tap": (C.c_int, [_P, C.c_int, _P]),
+    "ns2vc_voc_launch_count": (C.c_int, [_P]),
     # prompt-mel front end (resampler + log-mel spectrogram)
     "ns2vc_resample_out_length": (C.c_longlong, [C.c_int, C.c_int, C.c_longlong]),
     "ns2vc_resample_table": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
@@ -151,7 +170,7 @@ def check(rc: int) -> None:
 
 def engine_handle(mod, prefix: str, device, requirement: str) -> int:
     """The engine handle of ``mod`` (a module with ``_c_cfg()`` and ``_release()``) on ``device``, with its current parameter
-    values loaded and packed.  ``prefix`` selects the C-ABI (``"ns2vc_unet_"`` / ``"ns2vc_pre_"``).  The handle is created on
+    values loaded and packed.  ``prefix`` selects the C-ABI (``"ns2vc_unet_"`` / ``"ns2vc_pre_"`` / ``"ns2vc_voc_"``).  The handle is created on
     the device if needed; every state_dict entry is loaded and the weights are finalized again whenever a parameter changed
     (optimizer step, load_state_dict, .to()).  ``requirement`` ends the error raised for a parameter that is not fp32 on
     ``device``; ``{device}`` in it is filled in."""

@@ -1,4 +1,4 @@
-"""Public convenience API: host tensors in, sampled latents out (what bench.py's ``e2e`` leg times).
+"""Public convenience API: host tensors in, sampled latents out (what bench.py's ``e2e`` leg times), and latents to waveforms.
 
 ``sample_latents`` is the batched equivalent of the sampling block of ``NaturalSpeech2.sample``
 (reference model.py:620-686) after ``pre_model.infer``: it takes the condition tensors in the
@@ -169,4 +169,27 @@ def sample_utterances(unet: UNet1DConditionModel, items: Sequence[Utterance], st
                              noise_schedule=noise_schedule, eta=eta, content_lengths=tl)
         for j, i in enumerate(idx):
             out[i] = lat[j, :, :int(tl[j])]
+    return out
+
+
+@torch.no_grad()
+def decode_utterances(vocoder, latents: Sequence[torch.Tensor], max_batch: int = 8) -> List[torch.Tensor]:
+    """Decodes a list of mel latents [C, T_b] of different lengths (what ``sample_utterances`` returns) with a
+    ``vocoder.Vocos`` in ragged batches of at most ``max_batch`` (longest first) and returns the waveforms [T_b * hop_length]
+    in input order.  Each equals ``vocoder.decode`` of that latent alone."""
+    C = vocoder.cfg["input_channels"]
+    for k, x in enumerate(latents):
+        if x.dim() != 2 or x.shape[0] != C or x.shape[1] < 1:
+            raise ValueError(f"latent {k}: expected [{C}, T_b] with T_b >= 1, got {tuple(x.shape)}")
+    dev = next(vocoder.parameters()).device
+    hop = vocoder.hop_length
+    out: List[Optional[torch.Tensor]] = [None] * len(latents)
+    for idx in batch_plan([x.shape[1] for x in latents], max_batch):
+        tl = [int(latents[i].shape[1]) for i in idx]
+        mel = torch.zeros((len(idx), C, max(tl)), dtype=torch.float32, device=dev)
+        for j, i in enumerate(idx):
+            mel[j, :, :tl[j]] = latents[i]
+        audio = vocoder.decode(mel, torch.tensor(tl, dtype=torch.int64))
+        for j, i in enumerate(idx):
+            out[i] = audio[j, :tl[j] * hop]
     return out

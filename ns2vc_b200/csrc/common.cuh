@@ -119,6 +119,8 @@ enum EpiFlags : int {
   // condition encoders (pre_engine.cu; the ENC instantiation of the wgmma kernel):
   EPI_RELU = 1024,    // max(v, 0) after bias / residual              (conv-FFN, reference operations.py:689)
   EPI_ROWMASK = 2048, // v *= rowmask[m] after everything else         (x * (1 - padding_mask), reference operations.py:813, 820)
+  // vocoder (vocoder.cu; the VOC instantiation of the wgmma kernel):
+  EPI_GELU = 4096,    // gelu_erf(v) after bias / residual             (ConvNeXtBlock pwconv1 -> act, vocos/modules.py)
 };
 
 // One panel segment of a panel-mode GEMM: `ncb` 64-channel blocks of one raw split source

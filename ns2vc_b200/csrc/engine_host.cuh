@@ -1,6 +1,6 @@
-// Host-side machinery shared by the two engines (engine.cu: the denoiser, pre_engine.cu: the condition encoders): the weight
-// registry, owned device memory and weight packing, the launch record, the program-builder base, the runner of the launch
-// kinds both engines use, the taps, and the TextTimeEmbedding both engines contain.
+// Host-side machinery shared by the engines (engine.cu: the denoiser, pre_engine.cu: the condition encoders, vocoder.cu: the
+// vocoder): the weight registry, owned device memory and weight packing, the launch record, the program-builder base, the
+// runner of the launch kinds the engines share, the taps, and the TextTimeEmbedding of the first two.
 #pragma once
 #include "common.cuh"
 
@@ -143,13 +143,15 @@ inline int concat_pool_kv(DeviceMem& mem, const WeightRegistry& w, const std::st
 // One launch of a per-shape program.
 struct Launch {
   // The denoiser's kinds keep their numbers: ns2vc_unet_launch_kind() and ns2vc_profile_kind_name() expose them.  The
-  // condition encoders' own kinds follow TAP.
+  // condition encoders' own kinds follow TAP, the vocoder's follow theirs.
   enum Kind { GEMM, ATTN, LN_SPLIT, LN_APPLY, LINEAR, NCT2SPLIT, POOL_CLS, POOL_ATT, MASKBIAS, PREP, MEMSET, TAP,
-              SEQMASK, ENC_INPUT, LN_MASK, NCT2TOK, POOL_ATT_WIDE } kind;
+              SEQMASK, ENC_INPUT, LN_MASK, NCT2TOK, POOL_ATT_WIDE,
+              VOC_LENS, VOC_NORM, VOC_ISTFT } kind;
   // The call argument a launch reads or writes instead of a program buffer; each engine resolves them in its run_program.
   enum Input { NONE,
                X, T, OUT, CONTENT, PROMPT, MASK,                               // ns2vc_unet_prepare_cond / _forward
-               C, REFER, LENGTHS, REFER_LENGTHS, CONTENT_OUT, PROMPT_OUT       // ns2vc_pre_infer
+               C, REFER, LENGTHS, REFER_LENGTHS, CONTENT_OUT, PROMPT_OUT,      // ns2vc_pre_infer
+               MEL, AUDIO                                                     // ns2vc_voc_decode
   } input = NONE;
   GemmOp gemm;
   AttnOp attn;

@@ -134,7 +134,7 @@ __device__ __forceinline__ void ln_row_stats(const GemmOp& op, long long m, floa
 
 // Epilogue for one accumulator value at (m = b*T_out + t, logical column n).  For GEGLU the caller
 // passes the value accumulator in `acc` and the gate accumulator in `acc_gate`.
-template <bool LNF = true>
+template <bool LNF = true, bool VOC = false>
 __device__ __forceinline__ float epi_value(const GemmOp& op, int b, long long m, int n, float acc, float acc_gate) {
   if (LNF && (op.flags & EPI_LNFOLD)) {
     float mu, rstd;
@@ -151,6 +151,7 @@ __device__ __forceinline__ float epi_value(const GemmOp& op, int b, long long m,
   }
   if (op.flags & EPI_ROWBIAS) v += __ldg(op.rowbias + (long long)b * op.rowbias_ld + n);
   if (op.flags & EPI_RESIDUAL) v += __ldg(op.res + m * op.res_ld + n);
+  if (VOC && (op.flags & EPI_GELU)) v = gelu_erf_f(v);
   if (op.flags & EPI_RELU) v = fmaxf(v, 0.f);
   if (op.flags & EPI_ROWMASK) v *= __ldg(op.rowmask + m);
   return v;

@@ -89,13 +89,13 @@ __device__ __forceinline__ float* stage_f32_ptr(uint8_t* st, int row, int c4) { 
 
 // Element-wise epilogue (bias / GEGLU / row bias / residual / folded LayerNorm) of this thread's parked row; gate values of a
 // GEGLU chunk are parked as plain [32 rows][32] floats behind the fp32 chunk (the 16-bit staging area).
-template <bool LNF>
+template <bool LNF, bool VOC = false>
 __device__ __noinline__ void epi_cold(const GemmOp& op, int b, long long m, int nbase, uint8_t* st, int lane, bool with_gate) {
 #pragma unroll 1
   for (int j = 0; j < 32; ++j) {
     float* pv = stage_f32_ptr(st, lane, j >> 2) + (j & 3);
     const float g = with_gate ? reinterpret_cast<const float*>(st + 4096)[lane * 32 + j] : 0.f;
-    *pv = (nbase + j < op.n_valid) ? epi_value<LNF>(op, b, m, nbase + j, *pv, g) : 0.f;
+    *pv = (nbase + j < op.n_valid) ? epi_value<LNF, VOC>(op, b, m, nbase + j, *pv, g) : 0.f;
   }
 }
 // Element-wise stores of this thread's parked row in the layout(s) `flags` asks for (channel-major, fp32 or split rows).
@@ -193,7 +193,8 @@ static_assert(kGemmOpHotBytes % 16 == 0 && kGemmOpHotBytes <= 2688 && sizeof(Pre
 // EPI_ROWMASK); the denoiser's instantiations do not carry that code
 // RAG: instantiation for the denoiser's ragged programs (GemmOp::row_len): rows past each utterance's length at this level are
 // stored as exact zeros, and in panel mode they read as the conv's zero padding and drop out of the GroupNorm statistics
-template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false>
+// VOC: instantiation for the vocoder (vocoder.cu): the erf-GELU epilogue of ConvNeXt's pwconv1 (EPI_GELU)
+template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false, bool VOC = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmOp op_param) {
   using Cfg = TileCfg<BN_>;
   constexpr int BN = Cfg::BN;
@@ -673,6 +674,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           if (cvalid) {
             const bool fullc = nbase + 32 <= op.n_valid;
             bool enc_hot = ENC && mv;                       // (the out-of-line path applies ReLU / mask itself: epi_value)
+            bool voc_hot = VOC;                             // (likewise the GELU)
             if (!rv) {
 #pragma unroll
               for (int j = 0; j < 32; ++j) acc[j] = 0.f;
@@ -698,9 +700,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             } else {                                        // cold: partial chunk / row bias / unaligned residual - out of line
               wait_staging();
               park_row(st, lane, acc);
-              epi_cold<LNF>(op, b, m, nbase, st, lane, false);
+              epi_cold<LNF, VOC>(op, b, m, nbase, st, lane, false);
               fetch_row(st, lane, acc);
               enc_hot = false;
+              voc_hot = false;
+            }
+            if constexpr (VOC) if (voc_hot && (op.flags & EPI_GELU)) {
+#pragma unroll
+              for (int j = 0; j < 32; j += 2) upk2(gelu_erf2(pk2(acc[j], acc[j + 1])), acc[j], acc[j + 1]);
             }
             if constexpr (ENC) if (enc_hot) {
               if (op.flags & EPI_RELU) {
@@ -854,12 +861,12 @@ static int sm_count() {
   return n;
 }
 
-template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false>
+template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false, bool VOC = false>
 static int launch_bn(const GemmOp& op, cudaStream_t st) {
   using Cfg = TileCfg<BN_>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN_, LNF, XF, ENC, RAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN_, LNF, XF, ENC, RAG, VOC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) { set_error("gemm_tc: cannot set %d B dynamic smem: %s", Cfg::kSmemBytes, cudaGetErrorString(e)); return -2; }
     attr_set = true;
   }
@@ -867,7 +874,7 @@ static int launch_bn(const GemmOp& op, cudaStream_t st) {
   int grid = tiles;                                         // one tile per CTA (the epilogue reuses the stage buffers)
   dim3 cluster(1, 1, 1);
   if (XF && op.xmode && op.ksplit > 1) { grid = tiles * op.ksplit; cluster.x = (unsigned)op.ksplit; }   // split-K: the CTAs of a cluster share a tile
-  cudaError_t e = launch_kc(gemm_tc_kernel<BN_, LNF, XF, ENC, RAG>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmemBytes, st, cluster, op);
+  cudaError_t e = launch_kc(gemm_tc_kernel<BN_, LNF, XF, ENC, RAG, VOC>, dim3(grid), dim3(kThreads), (size_t)Cfg::kSmemBytes, st, cluster, op);
   if (e != cudaSuccess) { set_error("gemm_tc launch failed: %s", cudaGetErrorString(e)); return -2; }
   return 0;
 }
@@ -887,6 +894,14 @@ int launch_gemm_tc(const GemmOp& op, cudaStream_t st) {
   if (rag && (lnf || op.bn != 64 || (op.flags & (EPI_GEGLU | EPI_RELU | EPI_ROWMASK)))) {
     set_error("gemm_tc: ragged row masks need a plain 64-wide tile without a folded LayerNorm");
     return -1;
+  }
+  if (op.flags & EPI_GELU) {
+    if (lnf || rag || op.xmode || op.bn != 64 || (op.flags & (EPI_GEGLU | EPI_RELU | EPI_ROWMASK))) {
+      set_error("gemm_tc: the GELU epilogue needs a plain 64-wide tile without a folded LayerNorm, ReLU or row mask");
+      return -1;
+    }
+    if (op.nkb_total <= 0) { set_error("gemm_tc: empty K"); return -1; }
+    return launch_bn<64, false, false, false, false, true>(op, st);
   }
   if (op.flags & (EPI_RELU | EPI_ROWMASK)) {
     if (lnf || op.xmode || op.bn != 64 || (op.flags & EPI_GEGLU)) { set_error("gemm_tc: ReLU / row-mask epilogues need a plain 64-wide tile"); return -1; }

@@ -76,6 +76,52 @@ def make_pre_state_dict(cfg: dict, seed: int = 0) -> Dict[str, torch.Tensor]:
     return sd
 
 
+VOCOS_REGIMES = ("init", "trained_like", "clip", "large_phase", "ln_offset")
+
+
+def make_vocos_state_dict(seed: int = 0, regime: str = "init", input_channels: int = 100, dim: int = 512, intermediate_dim: int = 1536,
+                          num_layers: int = 8, n_fft: int = 1024) -> Dict[str, torch.Tensor]:
+    """Synthetic ``Vocos`` weights keyed by parameter name.  Regimes:
+
+    init          the package's own init (trunc-normal std 0.02 conv / linear weights, zero biases, layer scale 1 / num_layers,
+                  LayerNorms 1 / 0, periodic Hann window)
+    trained_like  biases 0.05 N(0,1), LayerNorms 1 + 0.1 N / 0.1 N, layer scale U(0.05, 1); head log-magnitude bias -3 + 0.5 N,
+                  phase bias U(-20, 20) rad
+    clip          trained_like with log-magnitude biases of +6 on a quarter of the bins (exp > 100: clipped) and +200 on a
+                  twentieth (exp overflows fp32 to +inf before the clip)
+    large_phase   trained_like with the phase rows of head.out (weights and bias) x 100: sin / cos range reduction
+    ln_offset     trained_like with embed bias + 30: the backbone LayerNorm's row statistics at |mean| >> std
+    """
+    from .vocoder import vocos_init, vocos_param_shapes
+    if regime not in VOCOS_REGIMES:
+        raise ValueError(f"unknown regime {regime!r} ({' | '.join(VOCOS_REGIMES)})")
+    nb = n_fft // 2 + 1
+    sd: Dict[str, torch.Tensor] = {}
+    for name, shape in vocos_param_shapes(input_channels, dim, intermediate_dim, num_layers, n_fft).items():
+        g = torch.Generator().manual_seed(_seed_for(name, seed))
+        t = vocos_init(name, shape, num_layers, generator=g)
+        leaf = name.rsplit(".", 1)[-1]
+        if regime != "init" and not name.endswith("istft.window"):
+            if leaf == "gamma":
+                t = 0.05 + 0.95 * torch.rand(shape, generator=g)
+            elif ".norm." in name or "final_layer_norm" in name:
+                t = t + 0.1 * torch.randn(shape, generator=g)
+            elif name == "head.out.bias":
+                t = torch.cat([-3.0 + 0.5 * torch.randn((nb,), generator=g), 40.0 * torch.rand((nb,), generator=g) - 20.0])
+                if regime == "clip":
+                    u = torch.rand((nb,), generator=g)
+                    t[:nb][u < 0.25] = 6.0
+                    t[:nb][u < 0.05] = 200.0
+            elif leaf == "bias":
+                t = 0.05 * torch.randn(shape, generator=g)
+            if regime == "large_phase" and name.startswith("head.out."):
+                t[nb:] *= 100.0
+            if regime == "ln_offset" and name == "backbone.embed.bias":
+                t = t + 30.0
+        sd[name] = t.to(torch.float32).contiguous()
+    return sd
+
+
 def make_pre_inputs(B: int, T: int, S: int, content_ch: int = 256, ragged: bool = False, seed: int = 0) -> Dict[str, torch.Tensor]:
     """Synthetic `Pre_model.infer` inputs: c ~ N(0,1) [B, 256, T] (ContentVec features), refer ~ N(0,1) [B, 100, S] (mel prompt)."""
     g = torch.Generator().manual_seed(seed + 11)
