@@ -560,8 +560,10 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   // Only self-attention uses fp16 weights.  Cross-attention keeps the split whatever its key count: a key count cannot see how
   // sharp the prompt attention is, and with fp16 weights in both attentions, scores of std ~4 (tests/test_numerics_fp64.py,
   // regime 'sharp' at B=4, T=1024, S=256) put the output at 1.51x the elementwise tolerance against fp64 on an H100.
+  // Ragged programs never use them: entry b of a self-attention attends over its own T_b,l keys, known only on the device, and
+  // one built program serves every length vector, so the padded T_l says nothing about how many keys average the rounding.
   constexpr int kFp16MinKeys = 256;
-  auto p16 = [&](int keys) { return attention_v2_p_fp16() && keys >= kFp16MinKeys; };
+  auto p16 = [&](int keys) { return !ragged && attention_v2_p_fp16() && keys >= kFp16MinKeys; };
 
   // ================= conditioning program =================
   if (Cc > 0) {

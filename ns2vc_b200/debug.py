@@ -2,7 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Tuple
+from typing import Any, Callable, Dict, Optional, Tuple
 
 import torch
 
@@ -10,33 +10,48 @@ from . import _lib
 from .arch import level_lengths
 
 
-def forward_with_taps(unet, sample: torch.Tensor, timestep, ehs: torch.Tensor,
-                      mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
-    """Returns (output [B,Cout,T], {op name: activation [B,C,T_level]}) — activations converted from the
-    engine's token-major layout to the reference's channel-major layout."""
+def run_with_taps(unet, device: torch.device, B: int, T: int, run: Callable[[], Any]) -> Tuple[Any, Dict[str, torch.Tensor]]:
+    """Sets every tap of the engine's ACTIVE program (B, T: its batch and frame count), calls ``run()``, clears the taps.
+    ``run`` must execute that program (the module call of the same shape, or ``DenoiserSession.forward`` of the session that
+    prepared it) without building another one first.  Returns (run's result, {op name: activation [B,C,T_level]}) —
+    activations converted from the engine's token-major layout to the reference's channel-major layout; fresh buffers, so a
+    tap the program does not write is left uninitialised."""
     L = _lib.lib()
-    dev = sample.device
-    with torch.no_grad():
-        unet(sample, timestep, ehs, encoder_attention_mask=mask)      # builds the program for this shape
-        h = unet.engine(dev)
-        B, _, T = sample.shape
-        Tl = level_lengths(T, len(unet.cfg.block_out_channels))
-        n = L.ns2vc_unet_num_taps(h)
-        bufs, names = [], []
+    h = unet.engine(device)
+    Tl = level_lengths(T, len(unet.cfg.block_out_channels))
+    n = L.ns2vc_unet_num_taps(h)
+    bufs, names = [], []
+    try:
         for i in range(n):
             name, lvl, ch = C.c_char_p(), C.c_int(), C.c_int()
             _lib.check(L.ns2vc_unet_tap_info(h, i, C.byref(name), C.byref(lvl), C.byref(ch)))
-            buf = torch.empty((B, Tl[lvl.value], ch.value), dtype=torch.float32, device=dev)
+            buf = torch.empty((B, Tl[lvl.value], ch.value), dtype=torch.float32, device=device)
             _lib.check(L.ns2vc_unet_set_tap(h, i, buf.data_ptr()))
             bufs.append(buf)
             names.append(name.value.decode())
-        try:
-            out = unet(sample, timestep, ehs, encoder_attention_mask=mask).sample
-            torch.cuda.synchronize(dev)
-        finally:
-            for i in range(n):
-                L.ns2vc_unet_set_tap(h, i, None)
-    return out, {k: v.permute(0, 2, 1).contiguous() for k, v in zip(names, bufs)}
+        with torch.no_grad():
+            res = run()
+        torch.cuda.synchronize(device)
+    finally:
+        for i in range(n):
+            L.ns2vc_unet_set_tap(h, i, None)
+    return res, {k: v.permute(0, 2, 1).contiguous() for k, v in zip(names, bufs)}
+
+
+def forward_with_taps(unet, sample: torch.Tensor, timestep, ehs: torch.Tensor,
+                      mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """Module call (the padded program) with taps: (output [B,Cout,T], {op name: activation [B,C,T_level]})."""
+    with torch.no_grad():
+        unet(sample, timestep, ehs, encoder_attention_mask=mask)      # builds the program for this shape
+    B, _, T = sample.shape
+    return run_with_taps(unet, sample.device, B, T, lambda: unet(sample, timestep, ehs, encoder_attention_mask=mask).sample)
+
+
+def session_forward_with_taps(sess, x: torch.Tensor, t: torch.Tensor) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """``DenoiserSession.forward`` (its padded or ragged program) with taps: (output [B,Cout,T], taps as above)."""
+    out = torch.empty((sess.B, sess.Co, sess.T), dtype=torch.float32, device=sess.dev)
+    sess.forward(x, t, out)                                            # builds and prepares the session's program
+    return run_with_taps(sess.unet, sess.dev, sess.B, sess.T, lambda: (sess.forward(x, t, out), out)[1])
 
 
 def profile_forward(unet, steps_fn, device, dump_csv: Optional[str] = None) -> Dict[str, Tuple[float, int]]:
