@@ -308,6 +308,41 @@ int ns2vc_voc_tap_info(const ns2vc_voc* h, int i, const char** name, int* rows, 
 int ns2vc_voc_set_tap(ns2vc_voc* h, int i, float* dst);
 int ns2vc_voc_launch_count(const ns2vc_voc* h);   /* kernels launched by the last decode */
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Content encoder: the units of `utils.get_hubert_content` (ContentVec, a fairseq HubertModel of extractor_mode "default",
+ * layer_norm_first False, no conv biases): `extract_features(source, padding_mask = all False, output_layer = num_layers)` then
+ * `final_proj`.  The feature encoder's convs are fairseq's default [(C, 10, 5)] + [(C, 3, 2)] * 4 + [(C, 2, 2)] * 2.  A ragged
+ * batch computes row b as if it were run alone on its first lengths[b] samples.  Same conventions as the vocoder. */
+typedef struct ns2vc_cv ns2vc_cv;
+typedef struct ns2vc_cv_cfg {        /* ContentVec legacy: 512, 768, 3072, 12, 12, 128, 16, 256 */
+  int conv_dim, embed_dim, ffn_dim, num_layers, num_heads, pos_conv_kernel, pos_conv_groups, final_dim;
+} ns2vc_cv_cfg;
+/* Rejected: conv_dim or embed_dim not a multiple of 128 up to 1024, a head dim other than 16 / 32 / 48 / 64, ffn_dim not a
+ * multiple of 64, final_dim not a multiple of 4, positional-conv groups wider than 64 channels or not a multiple of 4, and
+ * pos_conv_kernel not a multiple of 16 up to 128. */
+int ns2vc_cv_create(const ns2vc_cv_cfg* cfg, ns2vc_cv** out);
+void ns2vc_cv_destroy(ns2vc_cv* h);
+int ns2vc_cv_num_weights(const ns2vc_cv* h);     /* HubertModel.state_dict() keys without mask_emb / label_embs_concat, in its order */
+int ns2vc_cv_weight_info(const ns2vc_cv* h, int i, const char** name, int64_t shape[4], int* ndim);
+int ns2vc_cv_load_weight(ns2vc_cv* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream);
+int ns2vc_cv_finalize(ns2vc_cv* h, ns2vc_stream stream);   /* strict: fails on a missing key; folds the weight norm and q's scaling */
+int ns2vc_cv_workspace_bytes(const ns2vc_cv* h, int B, int N, size_t* bytes);
+/* Frames of n samples (0 below 400): T = floor((T - k) / s) + 1 through the seven convs. */
+int ns2vc_cv_num_frames(long long n);
+/* wav [B, N] fp32 at 16 kHz (batch stride wav_bstride floats), lengths [B] int64 device or NULL (every row N; values are clamped
+ * into [400, N]) -> units [B, T, final_dim] fp32 with T = ns2vc_cv_num_frames(N), frames [B] int64 device (or NULL): each row's
+ * frame count.  Row b equals the row run alone on wav[b, :lengths[b]]; its frames >= frames[b] are exactly 0 and samples past
+ * lengths[b] are never read. */
+int ns2vc_cv_extract(ns2vc_cv* h, const float* wav, long long wav_bstride, const int64_t* lengths, float* units, int64_t* frames, int B, int N,
+                     void* ws, ns2vc_stream stream);
+/* Diagnostics for the parity tests: activations ([B, rows, C] fp32) after each conv of the feature encoder, layer_norm,
+ * post_extract_proj, the positional conv's residual sum, encoder.layer_norm, each layer's self_attn_layer_norm and output, and
+ * final_proj. */
+int ns2vc_cv_num_taps(const ns2vc_cv* h);
+int ns2vc_cv_tap_info(const ns2vc_cv* h, int i, const char** name, int* rows, int* channels);
+int ns2vc_cv_set_tap(ns2vc_cv* h, int i, float* dst);
+int ns2vc_cv_launch_count(const ns2vc_cv* h);   /* kernels launched by the last extract */
+
 #ifdef __cplusplus
 }
 #endif

@@ -38,6 +38,11 @@ class VocCfg(C.Structure):
                 ("n_fft", C.c_int), ("hop_length", C.c_int)]
 
 
+class CvCfg(C.Structure):
+    _fields_ = [("conv_dim", C.c_int), ("embed_dim", C.c_int), ("ffn_dim", C.c_int), ("num_layers", C.c_int), ("num_heads", C.c_int),
+                ("pos_conv_kernel", C.c_int), ("pos_conv_groups", C.c_int), ("final_dim", C.c_int)]
+
+
 class DpmCoef(C.Structure):
     _fields_ = [("alpha_s", C.c_float), ("sigma_s", C.c_float), ("c_x", C.c_float), ("c_m", C.c_float),
                 ("c_d", C.c_float), ("inv_r0", C.c_float), ("order", C.c_int)]
@@ -126,6 +131,20 @@ SIGNATURES = {
     "ns2vc_voc_tap_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ns2vc_voc_set_tap": (C.c_int, [_P, C.c_int, _P]),
     "ns2vc_voc_launch_count": (C.c_int, [_P]),
+    # content encoder (ContentVec / HubertModel units)
+    "ns2vc_cv_create": (C.c_int, [C.POINTER(CvCfg), C.POINTER(_P)]),
+    "ns2vc_cv_destroy": (None, [_P]),
+    "ns2vc_cv_num_weights": (C.c_int, [_P]),
+    "ns2vc_cv_weight_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
+    "ns2vc_cv_load_weight": (C.c_int, [_P, C.c_char_p, _P, C.POINTER(C.c_int64), C.c_int, _P]),
+    "ns2vc_cv_finalize": (C.c_int, [_P, _P]),
+    "ns2vc_cv_workspace_bytes": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ns2vc_cv_num_frames": (C.c_int, [C.c_longlong]),
+    "ns2vc_cv_extract": (C.c_int, [_P, _P, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_cv_num_taps": (C.c_int, [_P]),
+    "ns2vc_cv_tap_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "ns2vc_cv_set_tap": (C.c_int, [_P, C.c_int, _P]),
+    "ns2vc_cv_launch_count": (C.c_int, [_P]),
     # prompt-mel front end (resampler + log-mel spectrogram)
     "ns2vc_resample_out_length": (C.c_longlong, [C.c_int, C.c_int, C.c_longlong]),
     "ns2vc_resample_table": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
@@ -170,7 +189,7 @@ def check(rc: int) -> None:
 
 def engine_handle(mod, prefix: str, device, requirement: str) -> int:
     """The engine handle of ``mod`` (a module with ``_c_cfg()`` and ``_release()``) on ``device``, with its current parameter
-    values loaded and packed.  ``prefix`` selects the C-ABI (``"ns2vc_unet_"`` / ``"ns2vc_pre_"`` / ``"ns2vc_voc_"``).  The handle is created on
+    values loaded and packed.  ``prefix`` selects the C-ABI (``"ns2vc_unet_"`` / ``"ns2vc_pre_"`` / ``"ns2vc_voc_"`` / ``"ns2vc_cv_"``).  The handle is created on
     the device if needed; every state_dict entry is loaded and the weights are finalized again whenever a parameter changed
     (optimizer step, load_state_dict, .to()).  ``requirement`` ends the error raised for a parameter that is not fp32 on
     ``device``; ``{device}`` in it is filled in."""

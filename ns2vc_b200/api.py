@@ -193,3 +193,32 @@ def decode_utterances(vocoder, latents: Sequence[torch.Tensor], max_batch: int =
         for j, i in enumerate(idx):
             out[i] = audio[j, :tl[j] * hop]
     return out
+
+
+def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Optional[Sequence[int]] = None,
+                       max_batch: int = 8) -> List[torch.Tensor]:
+    """Content units of a list of 1-D 16 kHz waveforms of different lengths with a ``content.ContentVec``, in ragged batches of
+    at most ``max_batch`` (longest first).  Returns [final_dim, T_b] per waveform in input order (each equals
+    ``get_hubert_content`` of that waveform alone), or, with ``target_frames``, [final_dim, target_frames[b]] through
+    ``frontend.repeat_expand_2d``: the ``c`` that ``Svc.get_unit_f0_code`` builds (its target is the f0 length, N24 // 256)."""
+    from .content import MIN_SAMPLES
+    from .frontend import repeat_expand_2d
+    for k, w in enumerate(wavs16k):
+        if w.dim() != 1 or w.shape[0] < MIN_SAMPLES:
+            raise ValueError(f"waveform {k}: expected a 1-D tensor of at least {MIN_SAMPLES} samples, got {tuple(w.shape)}")
+    if target_frames is not None and len(target_frames) != len(wavs16k):
+        raise ValueError(f"target_frames has {len(target_frames)} entries for {len(wavs16k)} waveforms")
+    dev = next(model.parameters()).device
+    out: List[Optional[torch.Tensor]] = [None] * len(wavs16k)
+    for idx in batch_plan([int(w.shape[0]) for w in wavs16k], max_batch):
+        nl = [int(wavs16k[i].shape[0]) for i in idx]
+        wav = torch.zeros((len(idx), max(nl)), dtype=torch.float32, device=dev)
+        for j, i in enumerate(idx):
+            wav[j, :nl[j]] = wavs16k[i]
+        with torch.no_grad():
+            units, frames = model.extract(wav, torch.tensor(nl, dtype=torch.int64))
+        fl = frames.tolist()
+        for j, i in enumerate(idx):
+            c = units[j, :fl[j]].t()
+            out[i] = c if target_frames is None else repeat_expand_2d(c, int(target_frames[i]))
+    return out

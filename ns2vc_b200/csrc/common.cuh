@@ -119,7 +119,8 @@ enum EpiFlags : int {
   // condition encoders (pre_engine.cu; the ENC instantiation of the wgmma kernel):
   EPI_RELU = 1024,    // max(v, 0) after bias / residual              (conv-FFN, reference operations.py:689)
   EPI_ROWMASK = 2048, // v *= rowmask[m] after everything else         (x * (1 - padding_mask), reference operations.py:813, 820)
-  // vocoder (vocoder.cu; the VOC instantiation of the wgmma kernel):
+                      //   (VOC instantiation: rows whose rowmask is 0 are stored as exact zeros)
+  // vocoder (vocoder.cu) and content encoder (content.cu; the VOC instantiation of the wgmma kernel):
   EPI_GELU = 4096,    // gelu_erf(v) after bias / residual             (ConvNeXtBlock pwconv1 -> act, vocos/modules.py)
 };
 
@@ -384,6 +385,12 @@ int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int 
 int launch_tbc_weight(const float* w, int k, int cin, int cout, float* o, cudaStream_t st);
 int launch_ffn_taps(const float* const* w, int k, int F, int H, int centre, float scale, float* o, cudaStream_t st);
 int launch_scale_vec(const float* a, float s, float* o, int n, cudaStream_t st);
+
+// LayerNorm (eps) of token-major [B, T, C] rows (vocoder.cu's voc_norm_kernel; C a multiple of 128 up to 1024), optionally after
+// a 7-tap depthwise conv (dw: [C][8] taps and bias).  Rows at or past len[b] (int64 [B], clamped into [1, T]; nullptr: T) read
+// and store 0.  Outputs: fp32 `out` and / or the bf16 hi/lo `split`.
+int launch_voc_norm(const float* x, int B, int T, int C, const float* dw, const float* gamma, const float* beta, float eps, const long long* len,
+                    float* out, const SplitBuf& split, cudaStream_t st);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

@@ -194,6 +194,7 @@ static_assert(kGemmOpHotBytes % 16 == 0 && kGemmOpHotBytes <= 2688 && sizeof(Pre
 // RAG: instantiation for the denoiser's ragged programs (GemmOp::row_len): rows past each utterance's length at this level are
 // stored as exact zeros, and in panel mode they read as the conv's zero padding and drop out of the GroupNorm statistics
 // VOC: instantiation for the vocoder (vocoder.cu): the erf-GELU epilogue of ConvNeXt's pwconv1 (EPI_GELU)
+// and of the content encoder (content.cu), whose row mask (EPI_ROWMASK) stores the rows a zero keep factor marks as exact zeros
 template <int BN_, bool LNF, bool XF, bool ENC = false, bool RAG = false, bool VOC = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmOp op_param) {
   using Cfg = TileCfg<BN_>;
@@ -502,6 +503,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       const long long m = (long long)b * op.T_out + t;
       bool rv = mv;                                         // row inside its utterance (RAG: stored as zeros otherwise)
       if constexpr (RAG) rv = mv && t < ragged_rows(op.row_len, b, op.len_shift);
+      if constexpr (VOC) if (op.flags & EPI_ROWMASK) rv = mv && __ldg(op.rowmask + m) != 0.f;   // (content.cu: exact zeros past a row's frames)
       if constexpr (!xpanel) {
         for (int kb = 0; kb < nkb; ++kb) {
           const int stage = kb % nst;
@@ -896,10 +898,11 @@ int launch_gemm_tc(const GemmOp& op, cudaStream_t st) {
     return -1;
   }
   if (op.flags & EPI_GELU) {
-    if (lnf || rag || op.xmode || op.bn != 64 || (op.flags & (EPI_GEGLU | EPI_RELU | EPI_ROWMASK))) {
-      set_error("gemm_tc: the GELU epilogue needs a plain 64-wide tile without a folded LayerNorm, ReLU or row mask");
+    if (lnf || rag || op.xmode || op.bn != 64 || (op.flags & (EPI_GEGLU | EPI_RELU))) {
+      set_error("gemm_tc: the GELU epilogue needs a plain 64-wide tile without a folded LayerNorm or ReLU");
       return -1;
     }
+    if ((op.flags & EPI_ROWMASK) && !op.rowmask) { set_error("gemm_tc: EPI_ROWMASK without a mask"); return -1; }
     if (op.nkb_total <= 0) { set_error("gemm_tc: empty K"); return -1; }
     return launch_bn<64, false, false, false, false, true>(op, st);
   }

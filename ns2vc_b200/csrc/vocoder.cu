@@ -285,6 +285,9 @@ __global__ void voc_layer_scale_kernel(const float* __restrict__ W, const float*
   if (i % K == 0) bo[n] = (float)((double)gamma[n] * (double)bias[n]);
 }
 
+}  // namespace
+
+// (also the content encoder's LayerNorms: content.cu)
 int launch_voc_norm(const float* x, int B, int T, int C, const float* dw, const float* gamma, const float* beta, float eps, const long long* len,
                     float* out, const SplitBuf& split, cudaStream_t st) {
   const dim3 grid(ceil_div(T, kNormRows), B), block(C / 4);
@@ -294,7 +297,6 @@ int launch_voc_norm(const float* x, int B, int T, int C, const float* dw, const 
   return 0;
 }
 
-}  // namespace
 }  // namespace ns2vc
 
 using namespace ns2vc;

@@ -167,3 +167,72 @@ def linear_betas(timesteps: int = 1000) -> torch.Tensor:
     float64 linspace cast to float32 by ``register_buffer``."""
     scale = 1000 / timesteps
     return torch.linspace(scale * 0.0001, scale * 0.02, timesteps, dtype=torch.float64).to(torch.float32)
+
+
+CONTENTVEC_REGIMES = ("init", "trained_like", "sharp", "large_v", "ln_offset")
+CONTENTVEC_SMALL = dict(conv_dim=128, embed_dim=128, ffn_dim=256, num_layers=2, num_heads=2, pos_conv_kernel=16, pos_conv_groups=4,
+                        final_dim=32)
+
+
+def make_contentvec_state_dict(seed: int = 0, regime: str = "init", **cfg) -> Dict[str, torch.Tensor]:
+    """Synthetic fairseq ``HubertModel`` weights (ContentVec's configuration unless ``cfg`` overrides it), fairseq-named, in one
+    of five regimes:
+
+    * ``init``: fairseq's initialisation (Kaiming-normal convs, N(0, 0.02) linears, zero biases, unit LayerNorms, the positional
+      conv N(0, sqrt(4 / (K D))) with g = ||v||);
+    * ``trained_like``: perturbed norms and biases, and a ``final_proj`` whose output has unit scale (the dataset's ``.soft.pt``
+      units have mean -0.02 and std 1.0);
+    * ``sharp``: q and k scaled to an attention-score std of about 4;
+    * ``large_v``: v_proj x 256 and out_proj x 1/256;
+    * ``ln_offset``: ``trained_like`` with a +100 offset on four residual channels (post_extract_proj, out_proj and fc2 biases),
+      so that every post-LN sees rows whose mean is far from their spread."""
+    from .content import CONTENTVEC, contentvec_param_shapes
+    if regime not in CONTENTVEC_REGIMES:
+        raise ValueError(f"unknown regime {regime!r}")
+    c = {**CONTENTVEC, **cfg}
+    D, K = c["embed_dim"], c["pos_conv_kernel"]
+    g = torch.Generator().manual_seed(1000 + seed)
+    sd: Dict[str, torch.Tensor] = {}
+    trained = regime != "init"
+    for k, shape in contentvec_param_shapes(**c).items():
+        leaf = k.rsplit(".", 1)[-1]
+        if k.startswith("feature_extractor.conv_layers.") and k.endswith(".0.weight"):
+            t = torch.randn(shape, generator=g) * math.sqrt(2.0 / (shape[1] * shape[2]))
+        elif k == "encoder.pos_conv.0.weight_v":
+            t = torch.randn(shape, generator=g) * math.sqrt(4.0 / (K * D))
+        elif k == "encoder.pos_conv.0.weight_g":
+            continue                                           # after weight_v: g = ||v|| per tap (weight_norm's initial value)
+        elif "norm" in k or k.startswith("feature_extractor.conv_layers.0.2."):
+            if leaf == "weight":
+                t = 1.0 + (0.1 * torch.randn(shape, generator=g) if trained else torch.zeros(shape))
+            else:
+                t = 0.1 * torch.randn(shape, generator=g) if trained else torch.zeros(shape)
+        elif leaf == "bias":
+            t = 0.02 * torch.randn(shape, generator=g) if trained else torch.zeros(shape)
+        else:
+            t = 0.02 * torch.randn(shape, generator=g)
+        sd[k] = t
+    v = sd["encoder.pos_conv.0.weight_v"]
+    sd["encoder.pos_conv.0.weight_g"] = v.pow(2).sum(dim=(0, 1), keepdim=True).sqrt() * (1.5 if trained else 1.0)
+    sd = {k: sd[k] for k in contentvec_param_shapes(**c)}     # registry order
+    if trained:
+        sd["final_proj.weight"] = torch.randn(sd["final_proj.weight"].shape, generator=g) / math.sqrt(D)
+        sd["final_proj.bias"] = torch.full_like(sd["final_proj.bias"], -0.02)
+    for i in range(c["num_layers"]):
+        p = f"encoder.layers.{i}.self_attn."
+        if regime == "sharp":
+            s = 2.0 / math.sqrt(D) / 0.02
+            sd[p + "q_proj.weight"] = sd[p + "q_proj.weight"] * s
+            sd[p + "k_proj.weight"] = sd[p + "k_proj.weight"] * s
+        if regime == "large_v":
+            sd[p + "v_proj.weight"] = sd[p + "v_proj.weight"] * 256.0
+            sd[p + "v_proj.bias"] = sd[p + "v_proj.bias"] * 256.0
+            sd[p + "out_proj.weight"] = sd[p + "out_proj.weight"] / 256.0
+    if regime == "ln_offset":
+        ch = torch.tensor([3, 17, 40, D - 1])
+        for k in ["post_extract_proj.bias"] + [f"encoder.layers.{i}.{m}.bias" for i in range(c["num_layers"])
+                                               for m in ("self_attn.out_proj", "fc2")]:
+            t = sd[k].clone()
+            t[ch] += 100.0
+            sd[k] = t
+    return {k: t.to(torch.float32).contiguous() for k, t in sd.items()}
