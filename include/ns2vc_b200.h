@@ -225,6 +225,11 @@ int ns2vc_pre_workspace_bytes(const ns2vc_pre* h, int B, int T, int S, size_t* b
  *      views of the same values: model.py:145, 189).                                                                        */
 int ns2vc_pre_infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths,
                     float* content, float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream);
+/* Ragged batch, same arguments: row b equals ns2vc_pre_infer of c[b, :, :T_b], refer[b, :, :S_b] alone (B = 1, T = T_b, S = S_b),
+ * T_b = lengths[b] in [1, T], S_b = refer_lengths[b] in [1, S]; frames past T_b / S_b are exactly 0 and input values there are
+ * never read.  A second program per (B, T, S, workspace); the workspace size above serves both. */
+int ns2vc_pre_infer_ragged(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths,
+                           float* content, float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream);
 /* Diagnostics for the parity tests: per-layer activations (token-major [B, rows, channels]; rows = 1 for the speaker vector). */
 int ns2vc_pre_num_taps(const ns2vc_pre* h);
 int ns2vc_pre_tap_info(const ns2vc_pre* h, int i, const char** name, int* rows, int* channels);

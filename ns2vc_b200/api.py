@@ -109,7 +109,8 @@ def sample_from_features(pre_model, unet: UNet1DConditionModel, x_T: torch.Tenso
     ``eta`` and ``noise`` as for ``sample_latents``.  ``per_utterance=True`` samples the encoders' output as ragged utterances
     (``sample_latents(content_lengths=lengths, prompt_lengths=refer_lengths)``): row b of the sampling equals ``sample_latents`` on
     row b of ``pre_model.infer``'s output alone.  The encoders themselves run on the padded batch as the reference runs them,
-    so their row b need not equal utterance b encoded alone; for that, encode per utterance and use ``sample_utterances``.
+    so their row b need not equal utterance b encoded alone; for that, encode with ``pre_model.infer(data, per_utterance=True)``
+    and sample with ``sample_latents(content_lengths=...)`` (or convert whole waveforms with ``convert_utterances``).
     The default keeps the padded semantics."""
     dev = torch.device(device) if device is not None else next(unet.parameters()).device
     data = (c_padded.to(dev, torch.float32, non_blocking=True), refer_padded.to(dev, torch.float32, non_blocking=True), None, None, None,
@@ -222,3 +223,11 @@ def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Op
             c = units[j, :fl[j]].t()
             out[i] = c if target_frames is None else repeat_expand_2d(c, int(target_frames[i]))
     return out
+
+
+def __getattr__(name):
+    # waveform-to-waveform conversion lives in convert.py, which builds on this module
+    if name in ("convert_utterances", "convert_slices"):
+        from . import convert
+        return getattr(convert, name)
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -1,0 +1,233 @@
+"""Waveform-to-waveform conversion of a file's voice slices in ragged batches: the device part of ``Svc.infer``
+(reference ``inference/infer_tool.py:141-206``) and the slicing loop of the CLI (``infer.py:99-141``) around it.
+
+Per utterance the chain is ``Svc.get_unit_f0_code`` + ``NaturalSpeech2.sample``:
+
+1. resample the input to 24 kHz (``frontend.resample``): N24 samples;
+2. T = N24 // 256, the frame count of ``compute_f0_parselmouth`` (``utils.py:159-160``).  f0 itself is not read by the model
+   (``model.py:349-375``) and the transposition only scales f0, so neither enters here;
+3. resample 24 -> 16 kHz, ContentVec units (``content.ContentVec.extract``), stretched to T frames (``repeat_expand_2d``);
+4. the condition encoders (``Pre_model.infer(per_utterance=True)``);
+5. UniPC (30 steps, what ``Svc.infer`` runs) or DPM-Solver++ (40 steps) from x_T ~ N(0, 1) [1, 100, T];
+6. the vocoder (``Vocos.decode``): T * 256 samples at 24 kHz.
+
+Every stage runs on a ragged batch in which row b equals utterance b run alone, so a file's slices convert together and each
+result equals that slice's own conversion.  Every length is computed on the host from the input sizes.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Optional, Sequence, Union
+
+import numpy as np
+import torch
+
+from . import frontend
+from .api import batch_plan, sample_latents
+from .content import MIN_SAMPLES, num_frames
+
+TARGET_SR = 24000        # config data.sampling_rate: the rate of the converted audio
+HOP = 256                # config data.hop_length
+CONTENT_SR = 16000       # ContentVec's input rate (infer_tool.py:162)
+LATENT_CH = 100
+DEFAULT_STEPS = {"unipc": 30, "dpmsolver": 40}       # model.py:654-686 / :620-653
+
+
+def frame_plan(n: int, sr: int) -> Dict[str, int]:
+    """Host lengths of one utterance of n samples at ``sr``: 24 kHz samples ``n24``, frames ``T`` (= the f0 length), 16 kHz samples
+    ``n16`` and ContentVec frames ``units`` (stretched to T afterwards)."""
+    n24 = frontend.resample_out_length(sr, TARGET_SR, n)
+    n16 = frontend.resample_out_length(TARGET_SR, CONTENT_SR, n24)
+    return dict(n24=n24, T=n24 // HOP, n16=n16, units=num_frames(n16))
+
+
+def _check_method(method: str, steps: Optional[int]) -> int:
+    if method in ("ddpm", "ddim"):
+        raise ValueError(f"method {method!r}: its per-step noise of a ragged batch is drawn over the padded tensor, so a slice would "
+                         "not equal its own conversion; use 'unipc' or 'dpmsolver'")
+    if method not in DEFAULT_STEPS:
+        raise ValueError(f"unknown method {method!r} (unipc | dpmsolver)")
+    return DEFAULT_STEPS[method] if steps is None else int(steps)
+
+
+def _check_inputs(wavs: Sequence[torch.Tensor], sr: int, prompt, x_T) -> List[Dict[str, int]]:
+    if len(wavs) == 0:
+        raise ValueError("wavs is empty")
+    if int(sr) <= 0:
+        raise ValueError(f"bad sample rate {sr}")
+    plans = []
+    for k, w in enumerate(wavs):
+        if not isinstance(w, torch.Tensor) or w.dim() != 1:
+            raise ValueError(f"waveform {k}: expected a 1-D (mono) tensor, got {tuple(getattr(w, 'shape', ()))}")
+        p = frame_plan(int(w.shape[0]), sr)
+        if p["T"] < 1 or p["n16"] < MIN_SAMPLES:
+            raise ValueError(f"waveform {k}: {w.shape[0]} samples at {sr} Hz are too short ({p['n24']} at 24 kHz, {p['n16']} at 16 kHz; "
+                             f"one frame needs {HOP} and {MIN_SAMPLES})")
+        plans.append(p)
+    prompts = list(prompt) if isinstance(prompt, (list, tuple)) else [prompt] * len(wavs)
+    if len(prompts) != len(wavs):
+        raise ValueError(f"{len(prompts)} prompts for {len(wavs)} waveforms")
+    for k, p in enumerate(prompts):
+        if p.dim() != 2 or p.shape[0] != LATENT_CH or p.shape[1] < 1:
+            raise ValueError(f"prompt {k}: expected a mel [{LATENT_CH}, S], got {tuple(p.shape)}")
+    if x_T is not None:
+        if len(x_T) != len(wavs):
+            raise ValueError(f"{len(x_T)} x_T tensors for {len(wavs)} waveforms")
+        for k, (x, p) in enumerate(zip(x_T, plans)):
+            if tuple(x.shape) not in ((1, LATENT_CH, p["T"]), (LATENT_CH, p["T"])):
+                raise ValueError(f"x_T {k}: expected [1, {LATENT_CH}, {p['T']}], got {tuple(x.shape)}")
+    return plans
+
+
+@torch.no_grad()
+def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence[torch.Tensor],
+                  x_T: Sequence[torch.Tensor], method: str = "unipc", steps: Optional[int] = None) -> Dict[str, List[torch.Tensor]]:
+    """Converts ``wavs`` (1-D, at ``sr``) as ONE ragged batch, each with its prompt mel [100, S_b] and x_T [1, 100, T_b], and returns
+    every stage per utterance, unpadded: ``units`` [D, units_b], ``c`` [D, T_b] (stretched), ``content`` [T_b, C], ``prompt``
+    [S_b, C] (the encoders' outputs), ``latent`` [100, T_b] and ``audio`` [T_b * 256]."""
+    steps = _check_method(method, steps)
+    plans = _check_inputs(wavs, sr, list(prompts), list(x_T))
+    dev = next(unet.parameters()).device
+    B = len(wavs)
+    n = [int(w.shape[0]) for w in wavs]
+    n24, tl = [p["n24"] for p in plans], [p["T"] for p in plans]
+    n16, nu = [p["n16"] for p in plans], [p["units"] for p in plans]
+    sl = [int(p.shape[1]) for p in prompts]
+    T, S = max(tl), max(sl)
+    wav = torch.zeros((B, max(n)), dtype=torch.float32, device=dev)
+    for j, w in enumerate(wavs):
+        wav[j, :n[j]] = w.to(dev, torch.float32)
+    w24, _ = frontend.resample(wav, sr, TARGET_SR, torch.tensor(n, dtype=torch.int64))
+    w16, _ = frontend.resample(w24, TARGET_SR, CONTENT_SR, torch.tensor(n24, dtype=torch.int64))
+    units_all, _ = content_model.extract(w16, torch.tensor(n16, dtype=torch.int64))
+    D = units_all.shape[2]
+    units = [units_all[j, :nu[j]].t() for j in range(B)]
+    c = torch.zeros((B, D, T), dtype=torch.float32, device=dev)
+    cs = []
+    for j in range(B):
+        cs.append(frontend.repeat_expand_2d(units[j], tl[j]))
+        c[j, :, :tl[j]] = cs[j]
+    refer = torch.zeros((B, LATENT_CH, S), dtype=torch.float32, device=dev)
+    for j, p in enumerate(prompts):
+        refer[j, :, :sl[j]] = p.to(dev, torch.float32)
+    tl_h, sl_h = torch.tensor(tl, dtype=torch.int64), torch.tensor(sl, dtype=torch.int64)
+    content, prompt = pre_model.infer((c, refer, None, None, None, tl_h, sl_h, None), per_utterance=True)
+    x = torch.zeros((B, LATENT_CH, T), dtype=torch.float32, device=dev)
+    for j, xt in enumerate(x_T):
+        x[j, :, :tl[j]] = xt.reshape(LATENT_CH, tl[j]).to(dev, torch.float32)
+    lat = sample_latents(unet, x, content, prompt, sl_h, steps=steps, method=method, device=dev, content_lengths=tl_h)
+    audio = vocoder.decode(lat, tl_h)
+    return dict(units=units, c=cs, content=[content[:tl[j], j] for j in range(B)], prompt=[prompt[:sl[j], j] for j in range(B)],
+                latent=[lat[j, :, :tl[j]] for j in range(B)], audio=[audio[j, :tl[j] * HOP] for j in range(B)])
+
+
+@torch.no_grad()
+def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int,
+                       prompt: Union[torch.Tensor, Sequence[torch.Tensor]], method: str = "unipc", steps: Optional[int] = None,
+                       max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+    """Converts 1-D float32 waveforms at ``sr`` with one prompt mel [100, S] (or one per waveform) and returns one 24 kHz
+    waveform [T_b * 256] per input, in input order, T_b = resample_out_length(sr, 24000, len) // 256.  The waveforms run in
+    ragged batches of at most ``max_batch`` (longest first); each result equals that waveform converted alone.
+
+    ``x_T`` (one [1, 100, T_b] per waveform) defaults to ``torch.randn((1, 100, T_b), device=dev)`` drawn per waveform in input
+    order before any batching: the shape and order in which ``Svc.infer`` draws it once per slice (``model.py:633-635``), so after
+    the same ``torch.manual_seed`` each waveform gets the reference CLI's x_T."""
+    steps = _check_method(method, steps)
+    plans = _check_inputs(wavs, sr, prompt, x_T)
+    prompts = list(prompt) if isinstance(prompt, (list, tuple)) else [prompt] * len(wavs)
+    dev = next(unet.parameters()).device
+    if x_T is None:
+        x_T = [torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans]
+    out: List[Optional[torch.Tensor]] = [None] * len(wavs)
+    for idx in batch_plan([int(w.shape[0]) for w in wavs], max_batch):
+        r = convert_batch(content_model, pre_model, unet, vocoder, [wavs[i] for i in idx], sr, [prompts[i] for i in idx],
+                          [x_T[i] for i in idx], method, steps)
+        for j, i in enumerate(idx):
+            out[i] = r["audio"][j]
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------ slicing (infer.py)
+def pad_array(arr: np.ndarray, target_length: int) -> np.ndarray:
+    """Centres ``arr`` in zeros up to ``target_length`` (longer arrays are returned as they are)."""
+    if arr.shape[0] >= target_length:
+        return arr
+    w = target_length - arr.shape[0]
+    return np.pad(arr, (w // 2, w - w // 2), "constant", constant_values=(0, 0))
+
+
+def split_list_by_n(x, n: int, pre: int = 0) -> list:
+    """Pieces of n samples, each but the first starting ``pre`` samples early (the cross-fade overlap)."""
+    return [x[i - pre if i - pre >= 0 else i: i + n] for i in range(0, len(x), n)]
+
+
+def _plan_slices(audio_data, audio_sr: int, pad_seconds: float, clip_seconds: float, linear_gradient: float):
+    """The voice sub-slices to convert, padded with ``pad_seconds`` of zeros at the input rate, in the CLI's order."""
+    per_size, lg_size = int(clip_seconds * audio_sr), int(linear_gradient * audio_sr)
+    pad_len = int(audio_sr * pad_seconds)
+    subs = []
+    for slice_tag, data in audio_data:
+        if slice_tag:
+            continue
+        for dat in (split_list_by_n(data, per_size, lg_size) if per_size != 0 else [data]):
+            subs.append(np.concatenate([np.zeros([pad_len]), dat, np.zeros([pad_len])]))
+    return subs
+
+
+def stitch(audio_data, audio_sr: int, converted: Sequence[np.ndarray], pad_seconds: float = 0.5, clip_seconds: float = 0,
+           linear_gradient: float = 0, linear_gradient_retain: float = 0.75) -> np.ndarray:
+    """Assembles a file from the conversions of its voice sub-slices (``converted``, 24 kHz, in ``_plan_slices`` order) as
+    ``infer.py:99-141`` does: silence as zeros, the ``pad_seconds`` trim, ``pad_array`` to each piece's length and the linear
+    cross-fade between the pieces of a forced split.  float64."""
+    per_size = int(clip_seconds * audio_sr)
+    lg_size = int(linear_gradient * audio_sr)
+    lg_size_r = int(lg_size * linear_gradient_retain)
+    lg_size_c_l = (lg_size - lg_size_r) // 2
+    lg_size_c_r = lg_size - lg_size_r - lg_size_c_l
+    lg = np.linspace(0, 1, lg_size_r) if lg_size != 0 else 0
+    lgr = linear_gradient_retain
+    trim = int(TARGET_SR * pad_seconds)
+    chunks: List[np.ndarray] = []
+    it = iter(converted)
+
+    def flat() -> np.ndarray:
+        a = np.concatenate(chunks) if chunks else np.zeros(0)
+        chunks[:] = [a]
+        return a
+
+    for slice_tag, data in audio_data:
+        length = int(np.ceil(len(data) / audio_sr * TARGET_SR))
+        if slice_tag:
+            chunks.append(pad_array(np.zeros(length), length))
+            continue
+        for k, dat in enumerate(split_list_by_n(data, per_size, lg_size) if per_size != 0 else [data]):
+            per_length = int(np.ceil(len(dat) / audio_sr * TARGET_SR)) if clip_seconds != 0 else length
+            _audio = pad_array(np.asarray(next(it))[trim:-trim], per_length)
+            if lg_size != 0 and k != 0:
+                audio = flat()
+                lg1 = audio[-(lg_size_r + lg_size_c_r):-lg_size_c_r] if lgr != 1 else audio[-lg_size:]
+                lg2 = _audio[lg_size_c_l:lg_size_c_l + lg_size_r] if lgr != 1 else _audio[0:lg_size]
+                lg_pre = lg1 * (1 - lg) + lg2 * lg
+                chunks[:] = [audio[0:-(lg_size_r + lg_size_c_r)] if lgr != 1 else audio[0:-lg_size], lg_pre]
+                _audio = _audio[lg_size_c_l + lg_size_r:] if lgr != 1 else _audio[lg_size:]
+            chunks.append(_audio)
+    return flat().astype(np.float64)
+
+
+@torch.no_grad()
+def convert_slices(content_model, pre_model, unet, vocoder, audio_data, audio_sr: int, prompt: torch.Tensor, pad_seconds: float = 0.5,
+                   clip_seconds: float = 0, linear_gradient: float = 0, linear_gradient_retain: float = 0.75, method: str = "unipc",
+                   steps: Optional[int] = None, max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None) -> np.ndarray:
+    """Converts one file given as ``slicer.chunks2audio``'s list of (is_silence, samples) at ``audio_sr`` with one prompt mel
+    [100, S] and returns the float64 24 kHz array ``infer.py`` writes for it.  Every voice sub-slice goes through one
+    ``convert_utterances`` call (``x_T``, if given, holds one tensor per sub-slice in order); stitching is ``stitch``."""
+    _check_method(method, steps)
+    if int(TARGET_SR * pad_seconds) <= 0:
+        raise ValueError(f"pad_seconds={pad_seconds} trims no sample at {TARGET_SR} Hz, and the reference's [0:-0] trim would leave "
+                         "every slice empty")
+    subs = _plan_slices(audio_data, audio_sr, pad_seconds, clip_seconds, linear_gradient)
+    converted = []
+    if subs:
+        outs = convert_utterances(content_model, pre_model, unet, vocoder, [torch.from_numpy(s.astype(np.float32)) for s in subs],
+                                  audio_sr, prompt, method=method, steps=steps, max_batch=max_batch, x_T=x_T)
+        converted = [o.cpu().numpy() for o in outs]
+    return stitch(audio_data, audio_sr, converted, pad_seconds, clip_seconds, linear_gradient, linear_gradient_retain)

@@ -230,9 +230,10 @@ int launch_ln_fold_vec(const float* W, const float* gamma, const float* beta, co
 
 int launch_prep_split(const PrepOp& op, cudaStream_t st);
 
-// LayerNorm + split in one pass (one warp per row): out = ((x-mean)*rstd*gamma + beta) as bf16 hi/lo
+// LayerNorm + split in one pass (one warp per row): out = ((x-mean)*rstd*gamma + beta) as bf16 hi/lo; rows with keep[row] == 0
+// store zeros when `keep` is given
 int launch_ln_split(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta,
-                    SplitBuf out, cudaStream_t st, unsigned long long* span = nullptr);
+                    SplitBuf out, cudaStream_t st, unsigned long long* span = nullptr, const float* keep = nullptr);
 
 // ---------------------------------------------------------------------------------------------
 // Attention
@@ -376,12 +377,12 @@ int launch_ddim_step(const float* x, const float* x0, const float* noise, const 
 // ---------------------------------------------------------------------------------------------
 // Condition encoders (pre_kernels.cu; program in pre_engine.cu)
 // ---------------------------------------------------------------------------------------------
-int launch_seq_mask(const long long* len, int B, int T, float* keep, float* kbias, cudaStream_t st);
+int launch_seq_mask(const long long* len, int B, int T, float* keep, float* kbias, cudaStream_t st, int* ilen = nullptr);
 int launch_enc_input(const float* x, long long bstride, const float* rowbias, const float* keep, int B, int C, int T, float* out, int ld,
                      cudaStream_t st);
 int launch_ln_mask(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta, const float* keep, float* y, int y_ld,
                    cudaStream_t st);
-int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st);
+int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st, const int* lens = nullptr);
 int launch_tbc_weight(const float* w, int k, int cin, int cout, float* o, cudaStream_t st);
 int launch_ffn_taps(const float* const* w, int k, int F, int H, int centre, float scale, float* o, cudaStream_t st);
 int launch_scale_vec(const float* a, float s, float* o, int n, cudaStream_t st);

@@ -330,7 +330,7 @@ struct Runner {
     switch (l.kind) {
       case Launch::GEMM: return gemm(l.gemm);
       case Launch::ATTN: return attn(l.attn);
-      case Launch::LN_SPLIT: return launch_ln_split(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.split, st, span);
+      case Launch::LN_SPLIT: return launch_ln_split(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.split, st, span, l.d);   // d: row keep factors, or nullptr
       case Launch::LN_APPLY: return launch_ln_apply(in ? in : l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.o, l.i3, st);
       case Launch::LINEAR: {
         LinOp o = l.lin;

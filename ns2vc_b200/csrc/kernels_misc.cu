@@ -179,9 +179,12 @@ int launch_prep_split(const PrepOp& op, cudaStream_t st) {
 }
 
 // LayerNorm + split: one warp per row, two-pass statistics in registers (C <= 1024).
+// KEEP: rows with keep[row] == 0 store hi = lo = 0 (the condition encoders' ragged programs: a k > 1 conv over the split then
+// reads zeros past an entry's length, as an unpadded run reads its zero padding).
+template <bool KEEP>
 __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__ x, int ld, int M, int C, float eps,
                                                        const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                       SplitBuf out, unsigned long long* span) {
+                                                       SplitBuf out, unsigned long long* span, const float* __restrict__ keep) {
   span_begin(span);
   pdl_trigger();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -239,6 +242,7 @@ __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__
     }
   }
   const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)C + eps);
+  const bool live = !KEEP || keep[row] != 0.f;
   const int ochunks = out.ld >> 3;
 #pragma unroll
   for (int k = 0; k < kMaxChunks; ++k) {
@@ -249,7 +253,7 @@ __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int c = c0 + j;
-        y[j] = (c < C) ? (v[k][j] - mean) * rstd * gm[k][j] + bt[k][j] : 0.f;
+        y[j] = (c < C && live) ? (v[k][j] - mean) * rstd * gm[k][j] + bt[k][j] : 0.f;
       }
       uint4 hi, lo;
       split8(y, hi, lo);
@@ -260,9 +264,10 @@ __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__
   span_end(span);
 }
 int launch_ln_split(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta, SplitBuf out,
-                    cudaStream_t st, unsigned long long* span) {
+                    cudaStream_t st, unsigned long long* span, const float* keep) {
   if (C > 1024 || (out.ld & 7) || out.ld > 1024) { set_error("ln_split: C=%d / pitch %d unsupported", C, out.ld); return -1; }
-  launch_k(ln_split_kernel, dim3(ceil_div(M, 8)), dim3(256), 0, st, x, ld, M, C, eps, gamma, beta, out, span);
+  if (keep) launch_k(ln_split_kernel<true>, dim3(ceil_div(M, 8)), dim3(256), 0, st, x, ld, M, C, eps, gamma, beta, out, span, keep);
+  else launch_k(ln_split_kernel<false>, dim3(ceil_div(M, 8)), dim3(256), 0, st, x, ld, M, C, eps, gamma, beta, out, span, keep);
   NS_LAUNCH_CHECK();
   return 0;
 }

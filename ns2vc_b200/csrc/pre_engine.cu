@@ -59,7 +59,7 @@ struct ns2vc_pre {
   EncSite phone, prompt;
   PoolKV ref_kv;                                       // ref_enc.pool k_proj | v_proj as one [2R, R] operator
   // cached program
-  int pB = 0, pT = 0, pS = 0; void* pws = nullptr;
+  int pB = 0, pT = 0, pS = 0; void* pws = nullptr; bool pR = false;
   std::vector<Launch> prog;
   TapSet taps;
   int last_launches = 0;
@@ -163,8 +163,10 @@ int pack_encoder(ns2vc_pre* h, EncSite& e, const std::string& p, int cin, int H,
 // The call arguments of one encoder: its lengths, its [B, C, T] input and its [B, T, C_out] output.
 struct EncIo { Launch::Input lengths, in, out; };
 
-// One encoder over Tn frames.
-void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSite& e, int Tn, EncIo io, const float* spk, double*& stat_cur) {
+// One encoder over Tn frames.  `ragged`: LN2's split is 0 on rows past the entry's length, so the conv-FFN reads zeros there as
+// an unpadded run reads its zero padding.  `ilens`: where SEQMASK also writes the lengths as int [B], clamped to [1, Tn], or nullptr.
+void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSite& e, int Tn, EncIo io, const float* spk, double*& stat_cur,
+                   bool ragged, int* ilens) {
   Arena& ar = bld.ar;
   const WeightRegistry& w = h->weights;
   const int B = bld.B, H = e.H, F = 4 * H, k = h->cfg.ffn_kernel, heads = h->cfg.n_heads, dh = H / heads;
@@ -185,7 +187,7 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
     g.flags |= EPI_LNFOLD | EPI_BIAS; g.ln_stats = rs; g.ln_g = gv; g.bias = bf; g.ln_C = H; g.ln_eps = 1e-5f; };
   auto masked = [&](GemmOp& g) { g.flags |= EPI_ROWMASK; g.rowmask = keep; };
 
-  { Launch l; l.kind = Launch::SEQMASK; l.input = io.lengths; l.i0 = Tn; l.o = keep; l.o2 = kbias; bld.out->push_back(l); }
+  { Launch l; l.kind = Launch::SEQMASK; l.input = io.lengths; l.i0 = Tn; l.o = keep; l.o2 = kbias; l.mem = ilens; bld.out->push_back(l); }
   { Launch l; l.kind = Launch::ENC_INPUT; l.input = io.in; l.b = spk; l.c = keep; l.i0 = e.cin; l.i1 = Tn; l.o = X0; l.i2 = ldin; bld.out->push_back(l); }
   bld.emit_ln_split(X0, ldin, (int)M, e.cin, w.W(e.p + ".pre.layer_norm.weight"), w.W(e.p + ".pre.layer_norm.bias"), s_in);
   double* rs = new_rowstats();
@@ -216,6 +218,7 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
       masked(g);
       bld.emit_gemm(g, ls.out); }
     bld.emit_ln_split(XB, H, (int)M, H, w.W(b + ".layer_norm2.weight"), w.W(b + ".layer_norm2.bias"), s_y);
+    if (ragged) bld.out->back().d = keep;
     { GemmOp g = bld.gemm_base(ls.ffn1, Tn);
       const int src = bld.add_src(g, s_y);
       for (int j = 0; j < k - 1; ++j) bld.seg(g, src, 0, H, j + 1 - (k - 1) / 2);     // row offsets -3 .. +4 for k = 9
@@ -237,7 +240,10 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
     l.b = w.W(e.p + ".layer_norm.weight"); l.c = w.W(e.p + ".layer_norm.bias"); l.d = keep; bld.out->push_back(l); }
 }
 
-int build_program(ns2vc_pre* h, int B, int T, int S, void* ws, size_t* bytes_out) {
+// `ragged`: row b is the utterance c[b, :, :T_b], refer[b, :, :S_b] encoded alone (ns2vc_pre_infer_ragged).  Besides the masked
+// LN2 splits, ref_enc pools over each entry's 1 + S_b tokens; the prompt encoder runs first so that its SEQMASK launch writes the
+// int prompt lengths ref_enc reads.  Same launches as the padded program.
+int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size_t* bytes_out) {
   const ns2vc_pre_cfg& c = h->cfg;
   const bool dry = ws == nullptr;
   NS_REQUIRE(B >= 1 && T >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
@@ -250,7 +256,9 @@ int build_program(ns2vc_pre* h, int B, int T, int S, void* ws, size_t* bytes_out
   double* stat_arena = ar.get<double>(stat_doubles);
   double* stat_cur = stat_arena;
   bld.emit_memset(stat_arena, stat_doubles * sizeof(double));
-  // ---- ref_enc: TextTimeEmbedding over ALL S prompt frames (the reference does not mask them: model.py:362)
+  int* plens = ragged ? ar.get<int>(B) : nullptr;
+  if (ragged) build_encoder(h, bld, taps, h->prompt, S, {Launch::REFER_LENGTHS, Launch::REFER, Launch::PROMPT_OUT}, nullptr, stat_cur, true, plens);
+  // ---- ref_enc: TextTimeEmbedding over ALL S prompt frames (the reference does not mask them: model.py:362), or S_b when ragged
   const int R = c.ref_dim;
   float* rt = ar.get<float>((size_t)B * S * R);
   TextTimeEmbedding tte;
@@ -258,19 +266,19 @@ int build_program(ns2vc_pre* h, int B, int T, int S, void* ws, size_t* bytes_out
   float* g = ar.get<float>((size_t)B * R);
   float* spk = ar.get<float>((size_t)B * c.phone_hidden);
   { Launch l; l.kind = Launch::NCT2TOK; l.input = Launch::REFER; l.i0 = R; l.i1 = S; l.o = rt; prog.push_back(l); }
-  tte.emit(bld, h->weights, "ref_enc", rt, Launch::NONE, S, R, R, c.ref_heads, Launch::POOL_ATT_WIDE, h->ref_kv, g);
+  tte.emit(bld, h->weights, "ref_enc", rt, Launch::NONE, S, R, R, c.ref_heads, Launch::POOL_ATT_WIDE, h->ref_kv, g, plens);
   bld.emit_tap(taps, "ref_enc", g, 1, R, 1);
   // spk_proj: Conv1d(100, hidden, 1) on g [B, 100, 1] (model.py:123, 127)
   bld.emit_linear(linear_op(g, R, B, R, h->weights.W("phoneme_encoder.spk_proj.weight"), h->weights.W("phoneme_encoder.spk_proj.bias"),
                             c.phone_hidden, spk, c.phone_hidden));
-  build_encoder(h, bld, taps, h->prompt, S, {Launch::REFER_LENGTHS, Launch::REFER, Launch::PROMPT_OUT}, nullptr, stat_cur);
-  build_encoder(h, bld, taps, h->phone, T, {Launch::LENGTHS, Launch::C, Launch::CONTENT_OUT}, spk, stat_cur);
+  if (!ragged) build_encoder(h, bld, taps, h->prompt, S, {Launch::REFER_LENGTHS, Launch::REFER, Launch::PROMPT_OUT}, nullptr, stat_cur, false, nullptr);
+  build_encoder(h, bld, taps, h->phone, T, {Launch::LENGTHS, Launch::C, Launch::CONTENT_OUT}, spk, stat_cur, ragged, nullptr);
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
     h->prog = std::move(prog);
     h->taps = std::move(taps);
-    h->pB = B; h->pT = T; h->pS = S; h->pws = ws;
+    h->pB = B; h->pT = T; h->pS = S; h->pws = ws; h->pR = ragged;
   }
   return 0;
 }
@@ -282,7 +290,7 @@ int run_program(ns2vc_pre* h, const float* c, const float* refer, const long lon
   const Runner run{h->simt, B, &h->taps, st};
   for (const Launch& l : h->prog) {
     switch (l.kind) {
-      case Launch::SEQMASK: rc = launch_seq_mask(l.input == Launch::LENGTHS ? lengths : refer_lengths, B, l.i0, l.o, l.o2, st); break;
+      case Launch::SEQMASK: rc = launch_seq_mask(l.input == Launch::LENGTHS ? lengths : refer_lengths, B, l.i0, l.o, l.o2, st, (int*)l.mem); break;
       case Launch::ENC_INPUT: {
         const float* src = l.input == Launch::C ? c : refer;
         rc = launch_enc_input(src, (long long)l.i0 * l.i1, l.b, l.c, B, l.i0, l.i1, l.o, l.i2, st);
@@ -290,7 +298,7 @@ int run_program(ns2vc_pre* h, const float* c, const float* refer, const long lon
       }
       case Launch::LN_MASK: rc = launch_ln_mask(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.d, l.input == Launch::CONTENT_OUT ? content : prompt, l.i2, st); break;
       case Launch::NCT2TOK: rc = launch_nct_to_tokens(refer, (long long)l.i0 * l.i1, B, l.i0, l.i1, l.o, l.i0, l.i0, st); break;
-      case Launch::POOL_ATT_WIDE: rc = launch_pool_attend_wide(l.a, l.b, B, l.i0, l.i1, l.i2, l.o, st); break;
+      case Launch::POOL_ATT_WIDE: rc = launch_pool_attend_wide(l.a, l.b, B, l.i0, l.i1, l.i2, l.o, st, l.lens); break;
       case Launch::TAP: --count; rc = run.run(l); break;
       default: rc = run.run(l); break;
     }
@@ -354,7 +362,7 @@ int ns2vc_pre_finalize(ns2vc_pre* h, ns2vc_stream stream) {
   int rc = h->weights.require_all_loaded();
   if (rc) return rc;
   h->mem.release();
-  h->prog.clear(); h->pB = h->pT = h->pS = 0; h->pws = nullptr;
+  h->prog.clear(); h->pB = h->pT = h->pS = 0; h->pws = nullptr; h->pR = false;
   const ns2vc_pre_cfg& c = h->cfg;
   cudaStream_t st = (cudaStream_t)stream;
   rc = pack_encoder(h, h->phone, "phoneme_encoder", c.phone_in, c.phone_hidden, c.phone_out, c.phone_layers, true, st);
@@ -370,20 +378,40 @@ int ns2vc_pre_finalize(ns2vc_pre* h, ns2vc_stream stream) {
 int ns2vc_pre_workspace_bytes(const ns2vc_pre* h, int B, int T, int S, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
   NS_REQUIRE(h->finalized, "ns2vc_pre_finalize() has not been called");
-  return build_program(const_cast<ns2vc_pre*>(h), B, T, S, nullptr, bytes);
+  // one workspace serves both programs of a shape
+  size_t padded = 0, ragged = 0;
+  int rc = build_program(const_cast<ns2vc_pre*>(h), B, T, S, false, nullptr, &padded);
+  if (!rc) rc = build_program(const_cast<ns2vc_pre*>(h), B, T, S, true, nullptr, &ragged);
+  if (!rc) *bytes = std::max(padded, ragged);
+  return rc;
 }
 
-int ns2vc_pre_infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content,
-                    float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream) {
+}  // extern "C"
+
+namespace {
+int infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content, float* prompt,
+          int B, int T, int S, void* ws, bool ragged, cudaStream_t st) {
   NS_REQUIRE(h && c && refer && lengths && refer_lengths && content && prompt, "null argument");
   NS_REQUIRE(h->finalized, "ns2vc_pre_finalize() has not been called");
   NS_REQUIRE(ws != nullptr, "workspace is NULL");
-  if (!(h->pB == B && h->pT == T && h->pS == S && h->pws == ws)) {
-    const int rc = build_program(h, B, T, S, ws, nullptr);
+  if (!(h->pB == B && h->pT == T && h->pS == S && h->pws == ws && h->pR == ragged)) {
+    const int rc = build_program(h, B, T, S, ragged, ws, nullptr);
     if (rc) return rc;
   }
-  return run_program(h, c, refer, reinterpret_cast<const long long*>(lengths), reinterpret_cast<const long long*>(refer_lengths), content, prompt,
-                     (cudaStream_t)stream);
+  return run_program(h, c, refer, reinterpret_cast<const long long*>(lengths), reinterpret_cast<const long long*>(refer_lengths), content, prompt, st);
+}
+}  // namespace
+
+extern "C" {
+
+int ns2vc_pre_infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content,
+                    float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream) {
+  return infer(h, c, refer, lengths, refer_lengths, content, prompt, B, T, S, ws, false, (cudaStream_t)stream);
+}
+
+int ns2vc_pre_infer_ragged(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content,
+                           float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream) {
+  return infer(h, c, refer, lengths, refer_lengths, content, prompt, B, T, S, ws, true, (cudaStream_t)stream);
 }
 
 int ns2vc_pre_num_taps(const ns2vc_pre* h) { return h ? h->taps.size() : -1; }

@@ -32,17 +32,20 @@ __device__ __forceinline__ float wmax(float v) {
 
 // sequence_mask (reference modules/commons.py:149-153): keep[b, t] = t < len[b]; the attention's key-padding bias uses the
 // denoiser's finite form (1 - keep) * -10000 instead of -inf (operations.py:412-421): exp(-10000 - max) is exactly 0 in fp32
-// as long as one key is valid (lengths >= 1), so the softmax weights are identical.
-__global__ void seq_mask_kernel(const long long* __restrict__ len, int B, int T, float* __restrict__ keep, float* __restrict__ kbias) {
+// as long as one key is valid (lengths >= 1), so the softmax weights are identical.  `ilen` (ragged programs, or nullptr): the
+// lengths as int [B], clamped to [1, T], for the kernels that take per-entry key counts.
+__global__ void seq_mask_kernel(const long long* __restrict__ len, int B, int T, float* __restrict__ keep, float* __restrict__ kbias,
+                                int* __restrict__ ilen) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * T) return;
   const int b = i / T, t = i - b * T;
   const float k = ((long long)t < len[b]) ? 1.f : 0.f;
   keep[i] = k;
   kbias[i] = (1.0f - k) * -10000.0f;
+  if (ilen && t == 0) ilen[b] = (int)max(1LL, min((long long)T, len[b]));
 }
-int launch_seq_mask(const long long* len, int B, int T, float* keep, float* kbias, cudaStream_t st) {
-  seq_mask_kernel<<<ceil_div(B * T, 256), 256, 0, st>>>(len, B, T, keep, kbias);
+int launch_seq_mask(const long long* len, int B, int T, float* keep, float* kbias, cudaStream_t st, int* ilen) {
+  seq_mask_kernel<<<ceil_div(B * T, 256), 256, 0, st>>>(len, B, T, keep, kbias, ilen);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }
@@ -104,18 +107,21 @@ int launch_ln_mask(const float* x, int ld, int M, int C, float eps, const float*
 
 // AttentionPooling attend step for any head width (reference unet1d/embeddings.py:521-546; `ref_enc` has ONE head of 100
 // channels): one block per (b, head); scores of the S1 keys in shared memory, softmax, then one thread per output channel.
+// RAG: over the class token and the entry's first lens[b] frames only (kv rows keep the stride S1).
+template <bool RAG>
 __global__ void __launch_bounds__(256) pool_attend_wide_kernel(const float* __restrict__ q, const float* __restrict__ kv, int S1, int C, int heads,
-                                                               float* __restrict__ out) {
+                                                               float* __restrict__ out, const int* __restrict__ lens) {
   extern __shared__ float sc_[];                            // [S1] scores -> weights
   __shared__ float red[8];
   __shared__ float bcast;
   const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const int K1 = RAG ? lens[b] + 1 : S1;
   const int dph = C / heads;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float s4 = 1.0f / sqrtf(sqrtf((float)dph));
   const float* qh = q + (long long)b * C + h * dph;
   float mx = -INFINITY;
-  for (int j = tid; j < S1; j += 256) {
+  for (int j = tid; j < K1; j += 256) {
     const float* kr = kv + ((long long)b * S1 + j) * 2 * C + h * dph;
     float s = 0.f;
     for (int d = 0; d < dph; ++d) s += (qh[d] * s4) * (kr[d] * s4);
@@ -129,7 +135,7 @@ __global__ void __launch_bounds__(256) pool_attend_wide_kernel(const float* __re
   __syncthreads();
   mx = bcast;
   float den = 0.f;
-  for (int j = tid; j < S1; j += 256) { const float p = expf(sc_[j] - mx); sc_[j] = p; den += p; }
+  for (int j = tid; j < K1; j += 256) { const float p = expf(sc_[j] - mx); sc_[j] = p; den += p; }
   den = wsum(den);
   __syncthreads();
   if (lane == 0) red[warp] = den;
@@ -139,15 +145,16 @@ __global__ void __launch_bounds__(256) pool_attend_wide_kernel(const float* __re
   den = bcast;
   for (int d = tid; d < dph; d += 256) {
     float a = 0.f;
-    for (int j = 0; j < S1; ++j) a += sc_[j] * kv[((long long)b * S1 + j) * 2 * C + C + h * dph + d];
+    for (int j = 0; j < K1; ++j) a += sc_[j] * kv[((long long)b * S1 + j) * 2 * C + C + h * dph + d];
     out[(long long)b * C + h * dph + d] = a / den;
   }
 }
-int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st) {
+int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st, const int* lens) {
   if (heads < 1 || C % heads) { set_error("pool_attend: dim/heads %d/%d unsupported", C, heads); return -1; }
   const size_t smem = (size_t)S1 * sizeof(float);
   if (smem > 48 * 1024) { set_error("pool_attend: %d keys do not fit the score buffer", S1); return -1; }
-  pool_attend_wide_kernel<<<B * heads, 256, smem, st>>>(q, kv, S1, C, heads, out);
+  if (lens) pool_attend_wide_kernel<true><<<B * heads, 256, smem, st>>>(q, kv, S1, C, heads, out, lens);
+  else pool_attend_wide_kernel<false><<<B * heads, 256, smem, st>>>(q, kv, S1, C, heads, out, lens);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }

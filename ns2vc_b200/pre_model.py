@@ -141,9 +141,14 @@ class Pre_model(nn.Module):
 
     # ------------------------------------------------------------------ reference API
     @torch.no_grad()
-    def infer(self, data, auto_predict_f0=None):
+    def infer(self, data, auto_predict_f0=None, per_utterance: bool = False):
         """``Pre_model.infer`` (model.py:360-377): data = (c_padded [B, C, T], refer_padded [B, 100, S], f0, spec, wav, lengths [B],
-        refer_lengths [B], uv) -> (content [T, B, C_out], audio_prompt [S, B, C_out]); frames past a length are exactly zero."""
+        refer_lengths [B], uv) -> (content [T, B, C_out], audio_prompt [S, B, C_out]); frames past a length are exactly zero.
+
+        The default runs the padded batch as the reference does: ``ref_enc`` pools over all S prompt frames and the conv-FFN of
+        a short row reads the batch's padding.  ``per_utterance=True`` runs a ragged batch instead: row b equals ``infer`` of
+        ``c_padded[b:b+1, :, :lengths[b]]``, ``refer_padded[b:b+1, :, :refer_lengths[b]]`` alone, and input values past the
+        lengths (which must lie in [1, T] / [1, S]) are never read."""
         c_padded, refer_padded, _f0, _spec, _wav, lengths, refer_lengths, _uv = data
         if not c_padded.is_cuda:
             raise RuntimeError("ns2vc_b200.Pre_model has no CPU path: move the module and inputs to an H100 ('cuda')")
@@ -166,14 +171,19 @@ class Pre_model(nn.Module):
         len_r = refer_lengths.to(dev, torch.int64).contiguous()
         if len_c.shape != (B,) or len_r.shape != (B,):
             raise ValueError("lengths / refer_lengths must be [B]")
+        if per_utterance:
+            from .fused import check_lengths
+            check_lengths(lengths, B, T, "lengths")
+            check_lengths(refer_lengths, B, S, "refer_lengths")
         L = _lib.lib()
         h = self.engine(dev)
         ws = self.workspace(B, T, S, dev)
         content = torch.empty((B, T, po), dtype=torch.float32, device=dev)
         prompt = torch.empty((B, S, ro), dtype=torch.float32, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
+        run = L.ns2vc_pre_infer_ragged if per_utterance else L.ns2vc_pre_infer
         with torch.cuda.device(dev):
-            _lib.check(L.ns2vc_pre_infer(h, c.data_ptr(), refer.data_ptr(), len_c.data_ptr(), len_r.data_ptr(), content.data_ptr(),
+            _lib.check(run(h, c.data_ptr(), refer.data_ptr(), len_c.data_ptr(), len_r.data_ptr(), content.data_ptr(),
                                          prompt.data_ptr(), B, T, S, ws.data_ptr(), stream))
         # the reference's layouts are the [T, B, C] / [S, B, C] views of the same values (model.py:147, 189)
         return content.transpose(0, 1).to(c_padded.dtype), prompt.transpose(0, 1).to(c_padded.dtype)
@@ -187,13 +197,13 @@ class Pre_model(nn.Module):
         return content, prompt, 0, 0
 
     # diagnostics for the parity tests -------------------------------------------------------
-    def taps(self, data) -> Dict[str, torch.Tensor]:
+    def taps(self, data, per_utterance: bool = False) -> Dict[str, torch.Tensor]:
         """Per-layer activations of one ``infer`` (token-major [B, rows, C]; the speaker vector as [B, 1, 100])."""
         c_padded, refer_padded = data[0], data[1]
         dev = c_padded.device
         B, _, T = c_padded.shape
         S = refer_padded.shape[2]
-        self.infer(data)                                       # builds the program for this shape
+        self.infer(data, per_utterance=per_utterance)          # builds the program for this shape
         L = _lib.lib()
         h = self._handle
         bufs = {}
@@ -204,7 +214,7 @@ class Pre_model(nn.Module):
             _lib.check(L.ns2vc_pre_set_tap(h, i, t.data_ptr()))
             bufs[name.value.decode()] = t
         try:
-            self.infer(data)
+            self.infer(data, per_utterance=per_utterance)
             torch.cuda.synchronize(dev)
         finally:
             for i in range(L.ns2vc_pre_num_taps(h)):
