@@ -348,6 +348,18 @@ int ns2vc_cv_tap_info(const ns2vc_cv* h, int i, const char** name, int* rows, in
 int ns2vc_cv_set_tap(ns2vc_cv* h, int i, float* dst);
 int ns2vc_cv_launch_count(const ns2vc_cv* h);   /* kernels launched by the last extract */
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Live conversion: the SOLA (synchronized overlap-add) join of one sliding-window tick, per slot b of B (one CTA each).
+ *   seg     [B, Nb + Nc + Ns] fp32 (batch stride seg_bstride floats): the end of the tick's converted window
+ *   tail    [B, Nc] fp32 contiguous, in place: the samples kept from the last tick; on return seg[b, k + Nb : k + Nb + Nc]
+ *   fade_in [Nc] fp32: the cross-fade's rising half (the caller's table; ns2vc_b200.stream builds sin^2(pi/2 i/(Nc-1)))
+ *   out     [B, Nb] fp32 contiguous, offset [B] int32: the emitted block and the chosen k
+ * k maximises sum_i seg[k+i] tail[i] / sqrt(sum_i seg[k+i]^2 + 1e-8) over k in [0, Ns] (i < Nc), both sums in fp64 in a fixed
+ * order, the lowest k on ties (an all-zero tail gives 0).  out[i] = seg[k+i], cross-faded with tail[i] for i < Nc.
+ * Needs Nb >= Nc and (2 Nc + Ns) * 4 bytes <= 47 KB.  Stream-ordered, allocates nothing, capturable. */
+int ns2vc_stream_sola(const float* seg, long long seg_bstride, float* tail, const float* fade_in, float* out, int* offset, int B,
+                      int Nb, int Nc, int Ns, ns2vc_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -156,6 +156,8 @@ SIGNATURES = {
     "ns2vc_mel_create": (C.c_int, [_P, _P, C.POINTER(_P)]),
     "ns2vc_mel_destroy": (None, [_P]),
     "ns2vc_log_mel": (C.c_int, [_P, _P, C.c_longlong, C.c_longlong, _P, _P, C.c_int, C.c_int, _P]),
+    # live conversion (SOLA join of one tick)
+    "ns2vc_stream_sola": (C.c_int, [_P, C.c_longlong, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

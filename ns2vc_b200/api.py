@@ -226,8 +226,11 @@ def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Op
 
 
 def __getattr__(name):
-    # waveform-to-waveform conversion lives in convert.py, which builds on this module
+    # waveform-to-waveform conversion lives in convert.py and live conversion in stream.py; both build on this module
     if name in ("convert_utterances", "convert_slices"):
         from . import convert
         return getattr(convert, name)
+    if name == "StreamConverter":
+        from . import stream
+        return stream.StreamConverter
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")
