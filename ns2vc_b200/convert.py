@@ -20,8 +20,9 @@ from typing import Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
-from . import frontend
+from . import frontend, shard
 from .api import batch_plan, sample_latents
 from .content import MIN_SAMPLES, num_frames
 
@@ -123,18 +124,25 @@ def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.
 @torch.no_grad()
 def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int,
                        prompt: Union[torch.Tensor, Sequence[torch.Tensor]], method: str = "unipc", steps: Optional[int] = None,
-                       max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+                       max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None,
+                       group: Optional[dist.ProcessGroup] = None) -> List[torch.Tensor]:
     """Converts 1-D float32 waveforms at ``sr`` with one prompt mel [100, S] (or one per waveform) and returns one 24 kHz
     waveform [T_b * 256] per input, in input order, T_b = resample_out_length(sr, 24000, len) // 256.  The waveforms run in
     ragged batches of at most ``max_batch`` (longest first); each result equals that waveform converted alone.
 
     ``x_T`` (one [1, 100, T_b] per waveform) defaults to ``torch.randn((1, 100, T_b), device=dev)`` drawn per waveform in input
     order before any batching: the shape and order in which ``Svc.infer`` draws it once per slice (``model.py:633-635``), so after
-    the same ``torch.manual_seed`` each waveform gets the reference CLI's x_T."""
+    the same ``torch.manual_seed`` each waveform gets the reference CLI's x_T.
+
+    With a process ``group`` of more than one rank (one process per GPU, each with its models on its own device, every rank
+    making the same call) the waveforms are shared out by ``shard.plan_batches`` and every rank returns the full list; see
+    ``_convert_sharded``."""
     steps = _check_method(method, steps)
     plans = _check_inputs(wavs, sr, prompt, x_T)
     prompts = list(prompt) if isinstance(prompt, (list, tuple)) else [prompt] * len(wavs)
     dev = next(unet.parameters()).device
+    if group is not None and dist.get_world_size(group) > 1:
+        return _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts, plans, method, steps, max_batch, x_T, group, dev)
     if x_T is None:
         x_T = [torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans]
     out: List[Optional[torch.Tensor]] = [None] * len(wavs)
@@ -144,6 +152,25 @@ def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[t
         for j, i in enumerate(idx):
             out[i] = r["audio"][j]
     return out
+
+
+def _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts, plans, method, steps, max_batch, x_T, group,
+                     dev) -> List[torch.Tensor]:
+    """``convert_utterances`` over the ranks of ``group``: each rank runs its batches of ``shard.plan_batches`` through
+    ``convert_batch`` and ``shard.run_sharded`` gathers the audio of all ranks (one status exchange, one all-gather).
+
+    The default x_T: every rank draws all of them, in input order on its own device, and keeps its own, so each waveform gets
+    the x_T of the one-GPU call and every rank's generator ends where that call leaves it.  The ranks' CUDA generators must
+    therefore start equal, which one all-gather of their seed and offset checks first."""
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    plan = shard.plan_batches(plans, [int(p.shape[1]) for p in prompts], world, max_batch)
+    if x_T is None:
+        shard.check_generator(torch.cuda.default_generators[dev.index], group, dev)
+        mine = {i for b in plan[rank] for i in b}
+        x_T = [x if i in mine else None for i, x in enumerate([torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans])]
+    return shard.run_sharded(lambda idx: convert_batch(content_model, pre_model, unet, vocoder, [wavs[i] for i in idx], sr,
+                                                       [prompts[i] for i in idx], [x_T[i] for i in idx], method, steps)["audio"],
+                             plan, [p["T"] * HOP for p in plans], group, dev)
 
 
 # ------------------------------------------------------------------------------------------------------------ slicing (infer.py)
@@ -216,10 +243,12 @@ def stitch(audio_data, audio_sr: int, converted: Sequence[np.ndarray], pad_secon
 @torch.no_grad()
 def convert_slices(content_model, pre_model, unet, vocoder, audio_data, audio_sr: int, prompt: torch.Tensor, pad_seconds: float = 0.5,
                    clip_seconds: float = 0, linear_gradient: float = 0, linear_gradient_retain: float = 0.75, method: str = "unipc",
-                   steps: Optional[int] = None, max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None) -> np.ndarray:
+                   steps: Optional[int] = None, max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None,
+                   group: Optional[dist.ProcessGroup] = None) -> np.ndarray:
     """Converts one file given as ``slicer.chunks2audio``'s list of (is_silence, samples) at ``audio_sr`` with one prompt mel
     [100, S] and returns the float64 24 kHz array ``infer.py`` writes for it.  Every voice sub-slice goes through one
-    ``convert_utterances`` call (``x_T``, if given, holds one tensor per sub-slice in order); stitching is ``stitch``."""
+    ``convert_utterances`` call (``x_T``, if given, holds one tensor per sub-slice in order); stitching is ``stitch``.  With a
+    ``group`` of more than one rank, the sub-slices are shared out over its ranks and every rank returns the stitched file."""
     _check_method(method, steps)
     if int(TARGET_SR * pad_seconds) <= 0:
         raise ValueError(f"pad_seconds={pad_seconds} trims no sample at {TARGET_SR} Hz, and the reference's [0:-0] trim would leave "
@@ -228,6 +257,6 @@ def convert_slices(content_model, pre_model, unet, vocoder, audio_data, audio_sr
     converted = []
     if subs:
         outs = convert_utterances(content_model, pre_model, unet, vocoder, [torch.from_numpy(s.astype(np.float32)) for s in subs],
-                                  audio_sr, prompt, method=method, steps=steps, max_batch=max_batch, x_T=x_T)
+                                  audio_sr, prompt, method=method, steps=steps, max_batch=max_batch, x_T=x_T, group=group)
         converted = [o.cpu().numpy() for o in outs]
     return stitch(audio_data, audio_sr, converted, pad_seconds, clip_seconds, linear_gradient, linear_gradient_retain)
