@@ -360,6 +360,18 @@ int ns2vc_cv_launch_count(const ns2vc_cv* h);   /* kernels launched by the last 
 int ns2vc_stream_sola(const float* seg, long long seg_bstride, float* tail, const float* fade_in, float* out, int* offset, int B,
                       int Nb, int Nc, int Ns, ns2vc_stream stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Silence slicer: framewise RMS, librosa 0.10 feature.rms(y, frame_length=win, hop_length=hop) with center=True and
+ * pad_mode="constant", bit for bit (numpy's pairwise float32 sum of each squared frame, divided by win in float32, IEEE sqrt).
+ * Host-only: the frame count 1 + (n + 2 (win/2) - win) / hop of a row of n samples, or -1 for bad arguments (hop or win < 1,
+ * a padded length n + 2 (win/2) shorter than win, or a win too long for the kernel's unrolled pairwise sum, about 32768). */
+long long ns2vc_slice_rms_frames(long long n, int hop, int win);
+/* wav [B, *] fp32 (batch stride wav_bstride floats), lengths [B] int64 device, hop_win [B, 2] int32 device (row b's hop and
+ * win, each accepted by ns2vc_slice_rms_frames) -> rms [B, F] fp32 contiguous: frame f of row b, 0 for f at or past that
+ * row's frame count.  Samples past lengths[b] are never read.  Stream-ordered, allocates nothing, capturable. */
+int ns2vc_slice_rms(const float* wav, long long wav_bstride, const int64_t* lengths, const int* hop_win, float* rms, int F, int B,
+                    ns2vc_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -158,6 +158,9 @@ SIGNATURES = {
     "ns2vc_log_mel": (C.c_int, [_P, _P, C.c_longlong, C.c_longlong, _P, _P, C.c_int, C.c_int, _P]),
     # live conversion (SOLA join of one tick)
     "ns2vc_stream_sola": (C.c_int, [_P, C.c_longlong, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    # silence slicer (framewise RMS)
+    "ns2vc_slice_rms_frames": (C.c_longlong, [C.c_longlong, C.c_int, C.c_int]),
+    "ns2vc_slice_rms": (C.c_int, [_P, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

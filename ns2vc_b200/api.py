@@ -227,7 +227,7 @@ def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Op
 
 def __getattr__(name):
     # waveform-to-waveform conversion lives in convert.py and live conversion in stream.py; both build on this module
-    if name in ("convert_utterances", "convert_slices"):
+    if name in ("convert_utterances", "convert_slices", "convert_files"):
         from . import convert
         return getattr(convert, name)
     if name == "StreamConverter":

@@ -13,10 +13,13 @@ Per utterance the chain is ``Svc.get_unit_f0_code`` + ``NaturalSpeech2.sample``:
 
 Every stage runs on a ragged batch in which row b equals utterance b run alone, so a file's slices convert together and each
 result equals that slice's own conversion.  Every length is computed on the host from the input sizes.
+
+``convert_files`` is the whole CLI: a list of files, each cut at its silences by ``slicer.cut_batch``, against a list of
+reference voices, with every voice sub-slice of every (file, voice) pair in shared ragged batches.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional, Sequence, Union
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -260,3 +263,94 @@ def convert_slices(content_model, pre_model, unet, vocoder, audio_data, audio_sr
                                   audio_sr, prompt, method=method, steps=steps, max_batch=max_batch, x_T=x_T, group=group)
         converted = [o.cpu().numpy() for o in outs]
     return stitch(audio_data, audio_sr, converted, pad_seconds, clip_seconds, linear_gradient, linear_gradient_retain)
+
+
+# ------------------------------------------------------------------------------------------------------------ the CLI (infer.py)
+def voice_mels(voices: Sequence[Tuple[object, int]], dev: torch.device) -> List[torch.Tensor]:
+    """The prompt mel [100, S_v] of each reference recording ``(wav, sr)``: ``frontend.log_mel_spectrogram`` in one ragged
+    batch per rate.  A 2-D wav [channels, N] gives its channel 0, the channel ``model.py:610-611`` keeps."""
+    from .slicer import _mono
+    wavs, srs = [], []
+    for k, v in enumerate(voices):
+        if not isinstance(v, (tuple, list)) or len(v) != 2:
+            raise ValueError(f"voice {k}: expected a (wav, sr) pair")
+        w = torch.as_tensor(v[0])
+        wavs.append(_mono(w[0] if w.dim() == 2 else w, f"voice {k}"))
+        srs.append(int(v[1]))
+    out: List[Optional[torch.Tensor]] = [None] * len(wavs)
+    for sr in dict.fromkeys(srs):
+        idx = [i for i, s in enumerate(srs) if s == sr]
+        n = [int(wavs[i].shape[0]) for i in idx]
+        x = torch.zeros((len(idx), max(n)), dtype=torch.float32, device=dev)
+        for j, i in enumerate(idx):
+            x[j, :n[j]] = wavs[i].to(dev)
+        mel, frames = frontend.log_mel_spectrogram(x, sr, torch.tensor(n, dtype=torch.int64))
+        for j, (i, s) in enumerate(zip(idx, frames.tolist())):
+            out[i] = mel[j, :, :s]
+    return out
+
+
+def _files_x_T(sub_T: Sequence[Sequence[int]], n_voices: int, dev) -> List[List[List[torch.Tensor]]]:
+    """x_T[f][v][k] = ``torch.randn((1, 100, sub_T[f][k]), device=dev)`` drawn in the CLI's nested order: file, then voice, then
+    sub-slice (``infer.py:77, 92, 99-122``; ``Svc.infer`` draws once per call)."""
+    return [[[torch.randn((1, LATENT_CH, T), device=dev) for T in Ts] for _ in range(n_voices)] for Ts in sub_T]
+
+
+@torch.no_grad()
+def convert_files(content_model, pre_model, unet, vocoder, files: Sequence[Tuple[object, int]], voices: Sequence[Tuple[object, int]],
+                  slice_db: float = -40, pad_seconds: float = 0.5, clip_seconds: float = 0, linear_gradient: float = 0,
+                  linear_gradient_retain: float = 0.75, method: str = "unipc", steps: Optional[int] = None, max_batch: int = 8,
+                  x_T: Optional[Sequence[Sequence[Sequence[torch.Tensor]]]] = None,
+                  group: Optional[dist.ProcessGroup] = None) -> List[List[np.ndarray]]:
+    """The reference CLI (``infer.py:58-145``): every file of ``files`` converted with every voice of ``voices``.  Returns
+    ``out[f][v]``, the float64 24 kHz array ``infer.py`` writes for file f and voice v.
+
+    ``files`` are ``(wav, sr)`` pairs of 1-D float32 samples (as ``librosa.load(sr=None)`` returns them); each is cut at its
+    silences by ``slicer.cut_batch`` (``slice_db``, min_len 5000 ms, as ``infer.py:83`` calls ``slicer.cut``; one RMS launch for
+    all files) and split into voice sub-slices as ``convert_slices`` does.  ``voices`` are ``(wav, sr)`` reference recordings
+    (1-D, or [channels, N] of which channel 0 is used); their prompt mels come from ``voice_mels``.  Every (file, voice,
+    sub-slice) item of one input rate goes through ONE ``convert_utterances`` call, so the slices of different files and voices
+    share ragged batches (files at several rates take one call per rate); each file is stitched per voice by ``stitch``.
+
+    ``x_T`` (``x_T[f][v]``: one [1, 100, T] per voice sub-slice of file f) defaults to ``torch.randn((1, 100, T))`` per item drawn
+    in the CLI's order - file, then voice, then sub-slice - before any conversion, so after the same ``torch.manual_seed`` every
+    slice starts from the reference CLI's noise.  ``group`` is passed to ``convert_utterances``; every rank draws every x_T,
+    after ``shard.check_generator`` has checked that the ranks' generators agree."""
+    from . import slicer
+    _check_method(method, steps)
+    if int(TARGET_SR * pad_seconds) <= 0:
+        raise ValueError(f"pad_seconds={pad_seconds} trims no sample at {TARGET_SR} Hz, and the reference's [0:-0] trim would leave "
+                         "every slice empty")
+    if len(files) == 0 or len(voices) == 0:
+        raise ValueError(f"{len(files)} files and {len(voices)} voices: give at least one of each")
+    for k, f in enumerate(files):
+        if not isinstance(f, (tuple, list)) or len(f) != 2:
+            raise ValueError(f"file {k}: expected a (wav, sr) pair")
+        slicer._mono(f[0], f"file {k}")
+    dev = next(unet.parameters()).device
+    wavs, srs = [f[0] for f in files], [int(f[1]) for f in files]
+    chunks = slicer.cut_batch(wavs, srs, slice_db, 5000, device=dev)
+    audio_data = [slicer.chunks2audio(w, c) for w, c in zip(wavs, chunks)]
+    subs = [_plan_slices(a, sr, pad_seconds, clip_seconds, linear_gradient) for a, sr in zip(audio_data, srs)]
+    sub_T = [[frame_plan(len(s), sr)["T"] for s in ss] for ss, sr in zip(subs, srs)]
+    mels = voice_mels(voices, dev)
+    V = len(voices)
+    if x_T is None:
+        if group is not None and dist.get_world_size(group) > 1:
+            shard.check_generator(torch.cuda.default_generators[dev.index], group, dev)
+        x_T = _files_x_T(sub_T, V, dev)
+    elif len(x_T) != len(files) or any(len(xf) != V or any(len(xv) != len(ss) for xv in xf) for xf, ss in zip(x_T, subs)):
+        raise ValueError("x_T must hold x_T[f][v], one tensor per voice sub-slice of file f, for every file and voice")
+    converted: Dict[Tuple[int, int], List[np.ndarray]] = {(f, v): [] for f in range(len(files)) for v in range(V)}
+    for sr in dict.fromkeys(srs):
+        items = [(f, v, k) for f in range(len(files)) if srs[f] == sr for v in range(V) for k in range(len(subs[f]))]
+        if not items:
+            continue
+        outs = convert_utterances(content_model, pre_model, unet, vocoder,
+                                  [torch.from_numpy(subs[f][k].astype(np.float32)) for f, _, k in items], sr,
+                                  [mels[v] for _, v, _ in items], method=method, steps=steps, max_batch=max_batch,
+                                  x_T=[x_T[f][v][k] for f, v, k in items], group=group)
+        for (f, v, _), o in zip(items, outs):
+            converted[(f, v)].append(o.cpu().numpy())
+    return [[stitch(audio_data[f], srs[f], converted[(f, v)], pad_seconds, clip_seconds, linear_gradient, linear_gradient_retain)
+             for v in range(V)] for f in range(len(files))]
