@@ -1,4 +1,5 @@
-"""ctypes binding of ``libns2vc_b200.so`` (C-ABI declared in ``include/ns2vc_b200.h``).
+"""ctypes binding of ``libns2vc_b200.so`` (C-ABI declared in ``include/ns2vc_b200.h``), and the base class of the modules
+that run in its engines.
 
 There is no CPU fallback: if the library is missing every CUDA entry point raises.
 """
@@ -6,9 +7,10 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional
+from typing import Any, Callable, Dict, Optional, Tuple
 
 import torch
+import torch.nn as nn
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", os.environ.get("NS2VC_LIB_NAME", "libns2vc_b200.so"))   # (NS2VC_LIB_NAME: A/B builds during development)
@@ -193,53 +195,149 @@ def check(rc: int) -> None:
         raise Ns2vcError((msg or b"unknown error").decode("utf-8", "replace") + f" (code {rc})")
 
 
-def engine_handle(mod, prefix: str, device, requirement: str) -> int:
-    """The engine handle of ``mod`` (a module with ``_c_cfg()`` and ``_release()``) on ``device``, with its current parameter
-    values loaded and packed.  ``prefix`` selects the C-ABI (``"ns2vc_unet_"`` / ``"ns2vc_pre_"`` / ``"ns2vc_voc_"`` / ``"ns2vc_cv_"``).  The handle is created on
-    the device if needed; every state_dict entry is loaded and the weights are finalized again whenever a parameter changed
-    (optimizer step, load_state_dict, .to()).  ``requirement`` ends the error raised for a parameter that is not fp32 on
-    ``device``; ``{device}`` in it is filled in."""
-    # (storage, version) pairs over a cached list of the Parameter objects: the module tree is fixed after construction,
-    # `.to()` / `load_state_dict` / optimizers change storage or bump versions of the SAME objects (the recursive
-    # `self.parameters()` walk on every forward of the generic path was ~1 ms of host time per call)
-    plist = mod.__dict__.get("_plist")
-    if plist is None:
-        plist = mod.__dict__["_plist"] = list(mod.parameters())
-    sig = tuple((p.data_ptr(), p._version) for p in plist)
-    if mod._handle is not None and mod._wsig == sig and mod._handle_device == device:
-        return mod._handle
-    plist = mod.__dict__["_plist"] = list(mod.parameters())     # something changed: re-walk the tree before re-packing
-    sig = tuple((p.data_ptr(), p._version) for p in plist)
-    L = lib()
-    stream = torch.cuda.current_stream(device).cuda_stream
-    with torch.cuda.device(device):
-        if mod._handle is None or mod._handle_device != device:
-            mod._release()
-            h = C.c_void_p()
-            ccfg = mod._c_cfg()
-            check(getattr(L, prefix + "create")(C.byref(ccfg), C.byref(h)))
-            mod._handle = h.value
-            mod._handle_device = device
-        load = getattr(L, prefix + "load_weight")
-        for key, p in mod.state_dict().items():
-            if p.device != device or p.dtype != torch.float32:
-                raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; " + requirement.format(device=device))
-            t = p.detach().contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            check(load(mod._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
-        check(getattr(L, prefix + "finalize")(mod._handle, stream))
-    mod._wsig = sig
-    return mod._handle
+class EngineModule(nn.Module):
+    """A module whose parameters run in one of the engines behind the C-ABI.  A subclass sets ``_prefix`` (which C-ABI:
+    ``"ns2vc_unet_"`` / ``"ns2vc_pre_"`` / ``"ns2vc_voc_"`` / ``"ns2vc_cv_"``), ``_cfg_struct`` (its create argument, filled
+    from the ``self.cfg`` dict unless the subclass overrides ``_c_cfg``) and ``_requirement`` (the end of the error raised for a
+    parameter that is not fp32 on the device; ``{device}`` in it is filled in)."""
+    _prefix: str
+    _cfg_struct: type
+    _requirement: str
 
+    def __init__(self) -> None:
+        super().__init__()
+        self._handle: Optional[int] = None
+        self._handle_device = None
+        self._wsig = None
+        self._ws: Optional[torch.Tensor] = None
+        self._ws_need: Dict[Tuple[int, ...], int] = {}
 
-def release_engine(mod, prefix: str) -> bool:
-    """Destroy the engine handle of ``mod``; False if it had none.  Plain ``__dict__`` writes: ``nn.Module.__setattr__`` may
-    already be torn down at interpreter shutdown."""
-    if mod.__dict__.get("_handle") is None:
-        return False
-    try:
-        getattr(lib(), prefix + "destroy")(mod._handle)
-    except Exception:
-        pass
-    mod.__dict__["_handle"] = None
-    return True
+    def _c_cfg(self):
+        c = self._cfg_struct()
+        for k, v in self.cfg.items():
+            setattr(c, k, int(v))
+        return c
+
+    def _fn(self, name: str):
+        return getattr(lib(), self._prefix + name)
+
+    def engine(self, device: torch.device) -> int:
+        """Opaque engine handle on ``device`` with the current parameter values loaded and packed.  The handle is created on
+        the device if needed; every state_dict entry is loaded and the weights are finalized again whenever a parameter
+        changed (optimizer step, load_state_dict, .to())."""
+        # (storage, version) pairs over a cached list of the Parameter objects: the module tree is fixed after construction,
+        # `.to()` / `load_state_dict` / optimizers change storage or bump versions of the SAME objects (the recursive
+        # `self.parameters()` walk on every forward of the generic path was ~1 ms of host time per call)
+        plist = self.__dict__.get("_plist")
+        if plist is None:
+            plist = self.__dict__["_plist"] = list(self.parameters())
+        sig = tuple((p.data_ptr(), p._version) for p in plist)
+        if self._handle is not None and self._wsig == sig and self._handle_device == device:
+            return self._handle
+        plist = self.__dict__["_plist"] = list(self.parameters())     # something changed: re-walk the tree before re-packing
+        sig = tuple((p.data_ptr(), p._version) for p in plist)
+        stream = torch.cuda.current_stream(device).cuda_stream
+        with torch.cuda.device(device):
+            if self._handle is None or self._handle_device != device:
+                self._release()
+                h = C.c_void_p()
+                ccfg = self._c_cfg()
+                check(self._fn("create")(C.byref(ccfg), C.byref(h)))
+                self._handle = h.value
+                self._handle_device = device
+            load = self._fn("load_weight")
+            for key, p in self.state_dict().items():
+                if p.device != device or p.dtype != torch.float32:
+                    raise RuntimeError(f"parameter {key} is {p.dtype} on {p.device}; " + self._requirement.format(device=device))
+                t = p.detach().contiguous()
+                shape = (C.c_int64 * t.dim())(*t.shape)
+                check(load(self._handle, key.encode(), t.data_ptr(), shape, t.dim(), stream))
+            check(self._fn("finalize")(self._handle, stream))
+        self._wsig = sig
+        self._ws_need = {}                  # (re)packed: the workspace sizes are asked again
+        return self._handle
+
+    def _release(self):
+        """Destroy the engine handle and drop the workspace.  Plain ``__dict__`` writes: ``nn.Module.__setattr__`` may already
+        be torn down at interpreter shutdown."""
+        if self.__dict__.get("_handle") is None:
+            return
+        try:
+            self._fn("destroy")(self._handle)
+        except Exception:
+            pass
+        self.__dict__["_handle"] = None
+        self.__dict__["_ws"] = None
+
+    def __del__(self):
+        try:
+            self._release()
+        except Exception:
+            pass
+
+    def workspace(self, *dims_and_device) -> torch.Tensor:
+        """``workspace(*dims, device)``: the scratch buffer of a call of shape ``dims`` (the dims of the engine's
+        ``_workspace_bytes``).  ONE grow-only buffer per module, shared by every shape (the CLI feeds a different T per slice: a
+        fresh multi-hundred-MB allocation per shape was most of a cold call).  Calls are stream-ordered and never concurrent,
+        and every program rebuilds or re-prepares what it keeps there after a shape switch, so shapes can alias the same
+        memory.  Growing it invalidates the captured loops that baked the old pointer (the module's sessions are dropped)."""
+        *dims, device = dims_and_device
+        key = tuple(dims)
+        need = self._ws_need.get(key)
+        if need is None:
+            n = C.c_size_t()
+            check(self._fn("workspace_bytes")(self.engine(device), *dims, C.byref(n)))
+            need = int(n.value)
+            if len(self._ws_need) > 256:
+                self._ws_need.clear()
+            self._ws_need[key] = need
+        ws = self._ws
+        if ws is None or ws.device != device or ws.numel() < need:
+            self.__dict__.get("_sessions", {}).clear()
+            self._ws = ws = None            # (the old buffer is freed before the new one is allocated)
+            self._ws = ws = torch.empty(int(need * 1.25) if need < (8 << 30) else need, dtype=torch.uint8, device=device)
+        return ws
+
+    def launch_count(self) -> int:
+        """Launches of the engine's last run (tap copies not counted); 0 before the first."""
+        return int(self._fn("launch_count")(self._handle)) if self._handle is not None else 0
+
+    def _collect_taps(self, device: torch.device, B: int, run: Callable[[], Any],
+                      rows: Callable[[int], int] = lambda r: r) -> Tuple[Any, Dict[str, torch.Tensor]]:
+        """Sets every tap of the engine's current program to a fresh zeroed [B, rows(r), C] buffer (r, C: the tap's info; r is a
+        row count, or the denoiser's level), calls ``run()`` (which must run that program without building another),
+        synchronises and clears the taps whatever happens.  Returns (run's result, {tap name: buffer}) in the engine's
+        token-major layout."""
+        h = self.engine(device)
+        num, info, set_tap = self._fn("num_taps"), self._fn("tap_info"), self._fn("set_tap")
+        n = num(h)
+        bufs = {}
+        try:
+            for i in range(n):
+                name, r, ch = C.c_char_p(), C.c_int(), C.c_int()
+                check(info(h, i, C.byref(name), C.byref(r), C.byref(ch)))
+                t = torch.zeros((B, rows(r.value), ch.value), dtype=torch.float32, device=device)
+                check(set_tap(h, i, t.data_ptr()))
+                bufs[name.value.decode()] = t
+            with torch.no_grad():
+                res = run()
+            torch.cuda.synchronize(device)
+        finally:
+            for i in range(n):
+                set_tap(h, i, None)
+        return res, bufs
+
+    def _load_checked(self, sd: Dict[str, torch.Tensor], what: str) -> "EngineModule":
+        """Loads ``sd`` (as fp32) after checking it holds exactly this module's keys and shapes; ValueError names the first
+        missing, unexpected or mis-shaped key (``what``: the reference model the state_dict comes from)."""
+        want = self.state_dict()
+        for k in want:
+            if k not in sd:
+                raise ValueError(f"missing key {k} in the {what} state_dict")
+        for k, v in sd.items():
+            if k not in want:
+                raise ValueError(f"unexpected key {k} in the {what} state_dict")
+            if tuple(v.shape) != tuple(want[k].shape):
+                raise ValueError(f"size mismatch for {k}: expected {tuple(want[k].shape)}, got {tuple(v.shape)}")
+        self.load_state_dict({k: v.detach().to(torch.float32) for k, v in sd.items()})
+        return self

@@ -11,7 +11,6 @@ pointers.  No CPU path; inference only.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional, Tuple
 
 import torch
@@ -70,7 +69,9 @@ def _norm_keys(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     return {ren.get(k, k): v for k, v in sd.items()}
 
 
-class ContentVec(nn.Module):
+class ContentVec(_lib.EngineModule):
+    _prefix, _cfg_struct, _requirement = "ns2vc_cv_", _lib.CvCfg, "this content encoder needs fp32 parameters on {device}"
+
     def __init__(self, conv_dim: int = 512, embed_dim: int = 768, ffn_dim: int = 3072, num_layers: int = 12, num_heads: int = 12,
                  pos_conv_kernel: int = 128, pos_conv_groups: int = 16, final_dim: int = 256) -> None:
         super().__init__()
@@ -79,10 +80,6 @@ class ContentVec(nn.Module):
         for key, shape in contentvec_param_shapes(**self.cfg).items():
             init = torch.ones(shape) if key.endswith(("norm.weight", "conv_layers.0.2.weight", "weight_g")) else torch.zeros(shape)
             _insert(self, key, nn.Parameter(init))
-        self._handle: Optional[int] = None
-        self._handle_device = None
-        self._wsig = None
-        self._ws: Optional[torch.Tensor] = None
 
     # ------------------------------------------------------------------ loading
     @classmethod
@@ -112,16 +109,7 @@ class ContentVec(nn.Module):
         final_dim = need("final_proj.weight").shape[0]
         groups = embed_dim // v.shape[1] if v.dim() == 3 and v.shape[1] else 1
         m = cls(int(conv_dim), int(embed_dim), int(ffn_dim), num_layers, int(num_heads), int(v.shape[-1]), int(groups), int(final_dim))
-        want = m.state_dict()
-        for k in want:
-            need(k)
-        for k, t in sd.items():
-            if k not in want:
-                raise ValueError(f"unexpected key {k} in the HubertModel state_dict")
-            if tuple(t.shape) != tuple(want[k].shape):
-                raise ValueError(f"size mismatch for {k}: expected {tuple(want[k].shape)}, got {tuple(t.shape)}")
-        m.load_state_dict({k: t.detach().to(torch.float32) for k, t in sd.items()})
-        return m
+        return m._load_checked(sd, "HubertModel")
 
     @classmethod
     def from_fairseq(cls, obj) -> "ContentVec":
@@ -135,36 +123,6 @@ class ContentVec(nn.Module):
         m = cls.from_state_dict(sd, num_heads=int(heads))
         dev = sd["final_proj.weight"].device
         return m.to(dev)
-
-    # ------------------------------------------------------------------ engine management
-    def _c_cfg(self) -> "_lib.CvCfg":
-        c = _lib.CvCfg()
-        for k, v in self.cfg.items():
-            setattr(c, k, int(v))
-        return c
-
-    def _release(self):
-        if _lib.release_engine(self, "ns2vc_cv_"):
-            self.__dict__["_ws"] = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
-
-    def engine(self, device: torch.device) -> int:
-        """Opaque engine handle with the current parameter values packed (re-packed when a parameter changed)."""
-        return _lib.engine_handle(self, "ns2vc_cv_", device, "this content encoder needs fp32 parameters on {device}")
-
-    def workspace(self, B: int, N: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.lib().ns2vc_cv_workspace_bytes(self.engine(device), B, N, C.byref(n)))
-        need = int(n.value)
-        ws = self._ws
-        if ws is None or ws.device != device or ws.numel() < need:
-            self._ws = ws = torch.empty(int(need * 1.25), dtype=torch.uint8, device=device)
-        return ws
 
     @staticmethod
     def num_frames(n: int) -> int:
@@ -218,27 +176,10 @@ class ContentVec(nn.Module):
     def taps(self, wav: torch.Tensor, lengths=None) -> Dict[str, torch.Tensor]:
         """Activations of one ``extract`` (token-major [B, T_stage, C]) under the oracle's stage names, plus ``"units"``."""
         B, _ = wav.shape
-        dev = wav.device
         self.extract(wav, lengths)                               # builds the program for this shape
-        L = _lib.lib()
-        h = self._handle
-        bufs = {}
-        for i in range(L.ns2vc_cv_num_taps(h)):
-            name, rows, ch = C.c_char_p(), C.c_int(), C.c_int()
-            _lib.check(L.ns2vc_cv_tap_info(h, i, C.byref(name), C.byref(rows), C.byref(ch)))
-            t = torch.zeros((B, rows.value, ch.value), dtype=torch.float32, device=dev)
-            _lib.check(L.ns2vc_cv_set_tap(h, i, t.data_ptr()))
-            bufs[name.value.decode()] = t
-        try:
-            bufs["units"], bufs["frames"] = self.extract(wav, lengths)
-            torch.cuda.synchronize(dev)
-        finally:
-            for i in range(L.ns2vc_cv_num_taps(h)):
-                L.ns2vc_cv_set_tap(h, i, None)
+        (units, frames), bufs = self._collect_taps(wav.device, B, lambda: self.extract(wav, lengths))
+        bufs["units"], bufs["frames"] = units, frames
         return bufs
-
-    def launch_count(self) -> int:
-        return int(_lib.lib().ns2vc_cv_launch_count(self._handle)) if self._handle is not None else 0
 
 
 def get_hubert_content(model: ContentVec, wav_16k_tensor: torch.Tensor) -> torch.Tensor:

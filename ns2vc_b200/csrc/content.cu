@@ -262,24 +262,17 @@ __global__ void cv_qkv_kernel(const float* __restrict__ qw, const float* __restr
 
 using namespace ns2vc;
 
-struct ns2vc_cv {
+struct ns2vc_cv : SingleProgramEngine {
   ns2vc_cv_cfg cfg;
-  WeightRegistry weights;
-  DeviceMem mem;
-  bool finalized = false;
   PackedB conv[kLevels];                                    // conv[1 ..]: the strided convs
   PackedB proj, fin;
   std::vector<PackedB> pos;                                 // per positional-conv group
   std::vector<PackedB> qkv, out, fc1, fc2;
   std::vector<float*> qkv_b;
-  // cached program
-  int pB = 0, pN = 0; void* pws = nullptr;
-  std::vector<Launch> prog;
-  TapSet taps;
+  // what the cached program adds to the shared one
   std::vector<SplitBuf> tap_split;                          // per tap: the split it converts (hi == nullptr: an fp32 tap)
   std::vector<int> tap_rows;                                // per split tap: rows per entry of the split
   LenTables lt{};                                           // the program's length tables (in its workspace)
-  int last_launches = 0;
 };
 
 namespace {
@@ -519,11 +512,10 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
-    h->prog = std::move(prog);
-    h->taps = std::move(taps);
+    h->cp.prog = std::move(prog);
+    h->cp.taps = std::move(taps);
     h->tap_split = std::move(tap_split);
     h->tap_rows = std::move(tap_rows);
-    h->pB = B; h->pN = N; h->pws = ws;
     h->lt = lt;
   }
   return 0;
@@ -539,57 +531,44 @@ int launch_check(cudaError_t e, const char* what) {
 }
 
 int run_program(ns2vc_cv* h, const float* wav, long long bstride, const long long* lengths, float* units, long long* frames_out, cudaStream_t st) {
-  int rc = 0, count = 0;
-  const int B = h->pB, N = h->pN;
+  const int B = h->cp.dims[0], N = h->cp.dims[1];
   const ns2vc_cv_cfg& c = h->cfg;
   const int C0 = c.conv_dim;
   const WeightRegistry& w = h->weights;
   const LenTables& lt = h->lt;
-  const Runner run{false, B, &h->taps, st};
-  for (const Launch& l : h->prog) {
+  return run_cached(h, false, st, [&](const Launch& l) {
     switch ((int)l.kind) {
       case CV_LENS:
-        rc = launch_check(launch_k(cv_lengths_kernel, dim3(ceil_div(B * lt.rows[1], 256)), dim3(256), 0, st, lengths, B, N, lt, frames_out), "cv_lengths");
-        break;
+        return launch_check(launch_k(cv_lengths_kernel, dim3(ceil_div(B * lt.rows[1], 256)), dim3(256), 0, st, lengths, B, N, lt, frames_out), "cv_lengths");
       case CV_GN_STATS:
-        rc = launch_check(launch_k(cv_gn_stats_kernel, dim3(C0 / kStatCh, B), dim3(kStatCh * kStatLanes), 0, st, wav, bstride, lengths, N,
-                                   w.W(conv_key(0) + ".0.weight"), 1e-5f, C0, reinterpret_cast<float2*>(l.o)), "cv_gn_stats");
-        break;
+        return launch_check(launch_k(cv_gn_stats_kernel, dim3(C0 / kStatCh, B), dim3(kStatCh * kStatLanes), 0, st, wav, bstride, lengths, N,
+                                     w.W(conv_key(0) + ".0.weight"), 1e-5f, C0, reinterpret_cast<float2*>(l.o)), "cv_gn_stats");
       case CV_CONV0:
-        rc = launch_check(launch_k(cv_conv0_kernel, dim3(ceil_div(l.i0, kConv0Frames), B), dim3(C0 / 2), 0, st, wav, bstride, lengths, N, l.i0,
-                                   w.W(conv_key(0) + ".0.weight"), reinterpret_cast<const float2*>(l.a), w.W(conv_key(0) + ".2.weight"),
-                                   w.W(conv_key(0) + ".2.bias"), l.split), "cv_conv0");
-        break;
-      case CV_NORM: rc = launch_voc_norm(l.a, B, l.i0, l.i1, nullptr, l.b, l.c, l.f0, lt.frames64, l.o, l.split, st); break;
+        return launch_check(launch_k(cv_conv0_kernel, dim3(ceil_div(l.i0, kConv0Frames), B), dim3(C0 / 2), 0, st, wav, bstride, lengths, N, l.i0,
+                                     w.W(conv_key(0) + ".0.weight"), reinterpret_cast<const float2*>(l.a), w.W(conv_key(0) + ".2.weight"),
+                                     w.W(conv_key(0) + ".2.bias"), l.split), "cv_conv0");
+      case CV_NORM: return launch_voc_norm(l.a, B, l.i0, l.i1, nullptr, l.b, l.c, l.f0, lt.frames64, l.o, l.split, st);
       case CV_POS_WIN:
-        rc = launch_check(launch_k(cv_pos_windows_kernel, dim3(l.split.T, l.i2, B), dim3(kWinTaps * 64 / 8), 0, st, l.a, l.i0, l.i1, l.i2, l.i3,
-                                   c.pos_conv_kernel, (const long long*)lt.frames64, l.split.hi, l.split.lo), "cv_pos_windows");
-        break;
+        return launch_check(launch_k(cv_pos_windows_kernel, dim3(l.split.T, l.i2, B), dim3(kWinTaps * 64 / 8), 0, st, l.a, l.i0, l.i1, l.i2, l.i3,
+                                     c.pos_conv_kernel, (const long long*)lt.frames64, l.split.hi, l.split.lo), "cv_pos_windows");
       case CV_ADD: {
         const long long n4 = (long long)(l.mem_bytes / sizeof(float4));
-        rc = launch_check(launch_k(cv_add_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(l.o),
-                                   reinterpret_cast<const float4*>(l.a), n4), "cv_add");
-        break;
+        return launch_check(launch_k(cv_add_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(l.o),
+                                     reinterpret_cast<const float4*>(l.a), n4), "cv_add");
       }
       case CV_SPLIT_TAP: {
-        --count;
-        float* dst = h->taps.dst[l.tap_index];
+        float* dst = h->cp.taps.dst[l.tap_index];
         if (dst) {
           const long long n = (long long)B * l.i1 * C0;
           cv_split_tap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(h->tap_split[l.tap_index], l.i0, l.i1, C0, dst, n);
           NS_CV_LAUNCH_CHECK();
         }
-        break;
+        return 0;
       }
-      case CV_OUT: NS_CHECK_CUDA(cudaMemcpyAsync(units, l.a, l.mem_bytes, cudaMemcpyDeviceToDevice, st)); break;
-      case Launch::TAP: --count; rc = run.run(l); break;
-      default: rc = run.run(l); break;
+      case CV_OUT: NS_CHECK_CUDA(cudaMemcpyAsync(units, l.a, l.mem_bytes, cudaMemcpyDeviceToDevice, st)); return 0;
+      default: return kSharedKind;
     }
-    if (rc) return rc;
-    ++count;
-  }
-  h->last_launches = count;
-  return 0;
+  });
 }
 
 }  // namespace
@@ -621,39 +600,13 @@ int ns2vc_cv_create(const ns2vc_cv_cfg* cfg, ns2vc_cv** out) {
   return 0;
 }
 
-void ns2vc_cv_destroy(ns2vc_cv* h) {
-  if (!h) return;
-  h->weights.release();
-  h->mem.release();
-  delete h;
-}
-
-int ns2vc_cv_num_weights(const ns2vc_cv* h) { return h ? h->weights.size() : -1; }
-
-int ns2vc_cv_weight_info(const ns2vc_cv* h, int i, const char** name, int64_t shape[4], int* ndim) {
-  NS_REQUIRE(h, "weight index %d out of range", i);
-  return h->weights.info(i, name, shape, ndim);
-}
-
+void ns2vc_cv_destroy(ns2vc_cv* h) { destroy_engine(h); }
+int ns2vc_cv_num_weights(const ns2vc_cv* h) { return num_weights(h); }
+int ns2vc_cv_weight_info(const ns2vc_cv* h, int i, const char** name, int64_t shape[4], int* ndim) { return weight_info(h, i, name, shape, ndim); }
 int ns2vc_cv_load_weight(ns2vc_cv* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream) {
-  NS_REQUIRE(h && key && dptr, "null argument");
-  const int rc = h->weights.load(key, dptr, shape, ndim, (cudaStream_t)stream);
-  if (rc) return rc;
-  h->finalized = false;
-  return 0;
+  return load_weight(h, key, dptr, shape, ndim, (cudaStream_t)stream);
 }
-
-int ns2vc_cv_finalize(ns2vc_cv* h, ns2vc_stream stream) {
-  NS_REQUIRE(h, "null handle");
-  int rc = h->weights.require_all_loaded();
-  if (rc) return rc;
-  h->mem.release();
-  h->prog.clear(); h->pB = h->pN = 0; h->pws = nullptr;
-  if ((rc = pack(h, (cudaStream_t)stream))) return rc;
-  NS_CHECK_CUDA(cudaGetLastError());
-  h->finalized = true;
-  return 0;
-}
+int ns2vc_cv_finalize(ns2vc_cv* h, ns2vc_stream stream) { return finalize_engine(h, [&] { return pack(h, (cudaStream_t)stream); }); }
 
 int ns2vc_cv_workspace_bytes(const ns2vc_cv* h, int B, int N, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
@@ -671,26 +624,16 @@ int ns2vc_cv_num_frames(long long n) {
 int ns2vc_cv_extract(ns2vc_cv* h, const float* wav, long long wav_bstride, const int64_t* lengths, float* units, int64_t* frames, int B, int N,
                      void* ws, ns2vc_stream stream) {
   NS_REQUIRE(h && wav && units, "null argument");
-  NS_REQUIRE(h->finalized, "ns2vc_cv_finalize() has not been called");
-  NS_REQUIRE(ws != nullptr, "workspace is NULL");
   NS_REQUIRE(wav_bstride >= N, "waveform batch stride %lld shorter than a row of %d samples", wav_bstride, N);
-  if (!(h->pB == B && h->pN == N && h->pws == ws)) {
-    const int rc = build_program(h, B, N, ws, nullptr);
-    if (rc) return rc;
-  }
+  const int rc = ensure_program(h, "ns2vc_cv", B, N, 0, false, ws, [&] { return build_program(h, B, N, ws, nullptr); });
+  if (rc) return rc;
   return run_program(h, wav, wav_bstride, reinterpret_cast<const long long*>(lengths), units, reinterpret_cast<long long*>(frames),
                      (cudaStream_t)stream);
 }
 
-int ns2vc_cv_num_taps(const ns2vc_cv* h) { return h ? h->taps.size() : -1; }
-int ns2vc_cv_tap_info(const ns2vc_cv* h, int i, const char** name, int* rows, int* channels) {
-  NS_REQUIRE(h, "tap index %d out of range", i);
-  return h->taps.info(i, name, rows, channels);
-}
-int ns2vc_cv_set_tap(ns2vc_cv* h, int i, float* dst) {
-  NS_REQUIRE(h, "tap index %d out of range", i);
-  return h->taps.set(i, dst);
-}
-int ns2vc_cv_launch_count(const ns2vc_cv* h) { return h ? h->last_launches : -1; }
+int ns2vc_cv_num_taps(const ns2vc_cv* h) { return num_taps(h); }
+int ns2vc_cv_tap_info(const ns2vc_cv* h, int i, const char** name, int* rows, int* channels) { return tap_info(h, i, name, rows, channels); }
+int ns2vc_cv_set_tap(ns2vc_cv* h, int i, float* dst) { return set_tap(h, i, dst); }
+int ns2vc_cv_launch_count(const ns2vc_cv* h) { return launch_count(h); }
 
 }  // extern "C"

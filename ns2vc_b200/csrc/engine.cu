@@ -67,12 +67,10 @@ struct Program {
 
 }  // namespace
 
-struct ns2vc_unet {
+struct ns2vc_unet : EngineBase {
   ns2vc_unet_cfg cfg;
   int ted = 0;                                   // time_embed_dim
   std::vector<PlanOp> plan;
-  WeightRegistry weights;
-  bool finalized = false;
   bool simt = false;
   std::string plan_str;
 
@@ -83,7 +81,6 @@ struct ns2vc_unet {
   int kv_total = 0, k_total = 0, film_total = 0;
   float* film_W = nullptr; float* film_b = nullptr;       // concatenated time_emb_proj
   PoolKV pool_kv;                                         // concatenated k_proj | v_proj
-  DeviceMem mem;                                          // everything the packed model owns
 
   // Cached programs, least recently active first; the active one (if any) is progs[active].  Other keys stay cached for the
   // sub-batch lanes of a multi-stream sampler and for callers that alternate shapes.
@@ -94,7 +91,12 @@ struct ns2vc_unet {
   // several shapes may share one workspace, and captured graphs keep reading these tables, so they are only released when the
   // weights are re-packed or the handle is destroyed (~20 KB per shape ever seen)
   std::vector<void*> static_bufs;
-  int last_launches = 0;
+  void drop_programs() {
+    progs.clear();
+    active = -1;
+    for (void* p : static_bufs) cudaFree(p);
+    static_bufs.clear();
+  }
   bool profiling = false;
   bool ksplit = true;        // split-K pairs for few-tile panel-mode launches (NS2VC_KSPLIT=0: one CTA per tile)
   bool xf = true;            // GroupNorm(+FiLM)(+SiLU) of the conv / proj_in inputs applied inside the GEMM (panel mode; NS2VC_XF=0: prep launches)
@@ -281,6 +283,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
     }
   }
   // resnets / transformers / resamplers in plan order
+  h->resnets.clear(); h->xformers.clear(); h->resamplers.clear();
   int film_off = 0, kv_off = 0;
   for (auto& o : h->plan) {
     if (o.kind == PlanOp::RESNET) {
@@ -388,7 +391,6 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
   }
   if (c.add_embed_text)
     if ((rc = concat_pool_kv(h->mem, h->weights, "add_embedding.pool", c.cross_attention_dim, h->pool_kv, st))) return rc;
-  NS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -1031,13 +1033,6 @@ int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& pro
   return 0;
 }
 
-void drop_all_programs(ns2vc_unet* h) {
-  h->progs.clear();
-  h->active = -1;
-  for (void* p : h->static_bufs) cudaFree(p);
-  h->static_bufs.clear();
-}
-
 // Make the program for (B,T,S,ragged,ws) the active one, building it if it is not cached.
 int ensure_program(ns2vc_unet* h, int B, int T, int S, void* ws, cudaStream_t st, bool ragged = false) {
   NS_REQUIRE(h->finalized, "ns2vc_unet_finalize() has not been called");
@@ -1138,42 +1133,13 @@ int ns2vc_unet_create(const ns2vc_unet_cfg* cfg, ns2vc_unet** out) {
   return 0;
 }
 
-void ns2vc_unet_destroy(ns2vc_unet* h) {
-  if (!h) return;
-  h->weights.release();
-  h->mem.release();
-  drop_all_programs(h);
-  delete h;
-}
-
-int ns2vc_unet_num_weights(const ns2vc_unet* h) { return h ? h->weights.size() : -1; }
-
-int ns2vc_unet_weight_info(const ns2vc_unet* h, int i, const char** name, int64_t shape[4], int* ndim) {
-  NS_REQUIRE(h, "weight index %d out of range", i);
-  return h->weights.info(i, name, shape, ndim);
-}
-
+void ns2vc_unet_destroy(ns2vc_unet* h) { destroy_engine(h); }
+int ns2vc_unet_num_weights(const ns2vc_unet* h) { return num_weights(h); }
+int ns2vc_unet_weight_info(const ns2vc_unet* h, int i, const char** name, int64_t shape[4], int* ndim) { return weight_info(h, i, name, shape, ndim); }
 int ns2vc_unet_load_weight(ns2vc_unet* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream) {
-  NS_REQUIRE(h && key && dptr, "null argument");
-  const int rc = h->weights.load(key, dptr, shape, ndim, (cudaStream_t)stream);
-  if (rc) return rc;
-  h->finalized = false;
-  return 0;
+  return load_weight(h, key, dptr, shape, ndim, (cudaStream_t)stream);
 }
-
-int ns2vc_unet_finalize(ns2vc_unet* h, ns2vc_stream stream) {
-  NS_REQUIRE(h, "null handle");
-  int rc = h->weights.require_all_loaded();
-  if (rc) return rc;
-  // (re)pack: drop previous packed buffers
-  h->mem.release();
-  h->resnets.clear(); h->xformers.clear(); h->resamplers.clear();
-  drop_all_programs(h);
-  rc = pack_all(h, (cudaStream_t)stream);
-  if (rc) return rc;
-  h->finalized = true;
-  return 0;
-}
+int ns2vc_unet_finalize(ns2vc_unet* h, ns2vc_stream stream) { return finalize_engine(h, [&] { return pack_all(h, (cudaStream_t)stream); }); }
 
 int ns2vc_unet_workspace_bytes(const ns2vc_unet* h, int B, int T, int S, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
@@ -1400,6 +1366,6 @@ int ns2vc_unet_profile_reset(ns2vc_unet* h) {
   return 0;
 }
 const char* ns2vc_unet_plan_string(const ns2vc_unet* h) { return h ? h->plan_str.c_str() : ""; }
-int ns2vc_unet_launch_count(const ns2vc_unet* h) { return h ? h->last_launches : -1; }
+int ns2vc_unet_launch_count(const ns2vc_unet* h) { return launch_count(h); }
 
 }  // extern "C"

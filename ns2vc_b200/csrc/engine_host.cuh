@@ -1,6 +1,7 @@
 // Host-side machinery shared by the engines (engine.cu: the denoiser, pre_engine.cu: the condition encoders, vocoder.cu: the
-// vocoder): the weight registry, owned device memory and weight packing, the launch record, the program-builder base, the
-// runner of the launch kinds the engines share, the taps, and the TextTimeEmbedding of the first two.
+// vocoder, content.cu: the content encoder): the weight registry, owned device memory and weight packing, the launch record,
+// the program-builder base, the runner of the launch kinds the engines share, the taps, the TextTimeEmbedding of the first
+// two, and the handle lifecycle (load, finalize, destroy; the cached program and counted run of the single-program engines).
 #pragma once
 #include "common.cuh"
 
@@ -348,5 +349,110 @@ struct Runner {
     }
   }
 };
+
+// What every engine handle holds: the reference state_dict, the device memory of its packed weights, whether the loaded
+// weights are packed, and the number of launches of its last run.  Each handle also has a drop_programs() that forgets the
+// launch programs built over the packed weights.
+struct EngineBase {
+  WeightRegistry weights;
+  DeviceMem mem;
+  bool finalized = false;
+  int last_launches = 0;
+};
+
+// The C-ABI's <engine>_num_weights / _weight_info / _load_weight / _launch_count
+inline int num_weights(const EngineBase* h) { return h ? h->weights.size() : -1; }
+inline int weight_info(const EngineBase* h, int i, const char** name, int64_t shape[4], int* ndim) {
+  NS_REQUIRE(h, "weight index %d out of range", i);
+  return h->weights.info(i, name, shape, ndim);
+}
+inline int load_weight(EngineBase* h, const char* key, const float* dptr, const int64_t* shape, int ndim, cudaStream_t st) {
+  NS_REQUIRE(h && key && dptr, "null argument");
+  const int rc = h->weights.load(key, dptr, shape, ndim, st);
+  if (rc) return rc;
+  h->finalized = false;          // packed from the old values until the next finalize
+  return 0;
+}
+inline int launch_count(const EngineBase* h) { return h ? h->last_launches : -1; }
+
+// <engine>_finalize: (re)packs every loaded weight with the engine's `pack()`, after freeing the previous packing and the
+// programs that point into it.
+template <class Engine, class Pack> int finalize_engine(Engine* h, Pack pack) {
+  NS_REQUIRE(h, "null handle");
+  int rc = h->weights.require_all_loaded();
+  if (rc) return rc;
+  h->mem.release();
+  h->drop_programs();
+  if ((rc = pack())) return rc;
+  NS_CHECK_CUDA(cudaGetLastError());
+  h->finalized = true;
+  return 0;
+}
+
+// <engine>_destroy
+template <class Engine> void destroy_engine(Engine* h) {
+  if (!h) return;
+  h->weights.release();
+  h->mem.release();
+  h->drop_programs();
+  delete h;
+}
+
+// The launch program of the condition encoders, the vocoder and the content encoder: one per handle, for the last shape
+// (B, and up to two more dims: T, S or N), ragged flag and workspace it ran with.
+struct CachedProgram {
+  int dims[3] = {0, 0, 0};
+  bool ragged = false;
+  void* ws = nullptr;
+  std::vector<Launch> prog;
+  TapSet taps;
+};
+
+struct SingleProgramEngine : EngineBase {
+  CachedProgram cp;
+  void drop_programs() { cp = CachedProgram(); }
+};
+
+// The C-ABI's <engine>_num_taps / _tap_info / _set_tap: the taps of the cached program
+inline int num_taps(const SingleProgramEngine* h) { return h ? h->cp.taps.size() : -1; }
+inline int tap_info(const SingleProgramEngine* h, int i, const char** name, int* rows, int* channels) {
+  NS_REQUIRE(h, "tap index %d out of range", i);
+  return h->cp.taps.info(i, name, rows, channels);
+}
+inline int set_tap(SingleProgramEngine* h, int i, float* dst) {
+  NS_REQUIRE(h, "tap index %d out of range", i);
+  return h->cp.taps.set(i, dst);
+}
+
+// Makes h->cp the program of (B, d1, d2, ragged, ws), calling `build()` (which fills cp.prog and cp.taps) unless it already is.
+// `engine`: the C-ABI prefix named in the error of an unfinalized handle.
+template <class Build> int ensure_program(SingleProgramEngine* h, const char* engine, int B, int d1, int d2, bool ragged, void* ws,
+                                          Build build) {
+  NS_REQUIRE(h->finalized, "%s_finalize() has not been called", engine);
+  NS_REQUIRE(ws != nullptr, "workspace is NULL");
+  CachedProgram& cp = h->cp;
+  if (cp.dims[0] == B && cp.dims[1] == d1 && cp.dims[2] == d2 && cp.ragged == ragged && cp.ws == ws) return 0;
+  const int rc = build();
+  if (rc) return rc;
+  cp.dims[0] = B; cp.dims[1] = d1; cp.dims[2] = d2; cp.ragged = ragged; cp.ws = ws;
+  return 0;
+}
+
+// Runs h->cp and records its launch count in h->last_launches.  `own(l)` launches the engine's own kinds and returns
+// kSharedKind for the kinds Runner launches.  Tap copies (the launches with a tap index) are not counted: they are
+// diagnostics, not part of the computation.
+constexpr int kSharedKind = 1;
+template <class Own> int run_cached(SingleProgramEngine* h, bool simt, cudaStream_t st, Own own) {
+  const Runner run{simt, h->cp.dims[0], &h->cp.taps, st};
+  int count = 0;
+  for (const Launch& l : h->cp.prog) {
+    int rc = own(l);
+    if (rc == kSharedKind) rc = run.run(l);
+    if (rc) return rc;
+    if (l.tap_index < 0) ++count;
+  }
+  h->last_launches = count;
+  return 0;
+}
 
 }  // namespace ns2vc

@@ -51,18 +51,11 @@ struct EncSite {
 
 }  // namespace
 
-struct ns2vc_pre {
+struct ns2vc_pre : SingleProgramEngine {
   ns2vc_pre_cfg cfg;
-  WeightRegistry weights;
-  DeviceMem mem;
-  bool finalized = false, simt = false;
+  bool simt = false;
   EncSite phone, prompt;
   PoolKV ref_kv;                                       // ref_enc.pool k_proj | v_proj as one [2R, R] operator
-  // cached program
-  int pB = 0, pT = 0, pS = 0; void* pws = nullptr; bool pR = false;
-  std::vector<Launch> prog;
-  TapSet taps;
-  int last_launches = 0;
 };
 
 namespace {
@@ -158,6 +151,14 @@ int pack_encoder(ns2vc_pre* h, EncSite& e, const std::string& p, int cin, int H,
     if ((rc = launch_ln_fold_vec(wt, go, bo, cb, e.g_out, e.bf_out, cout, H, st))) return rc;
   }
   return 0;
+}
+
+int pack(ns2vc_pre* h, cudaStream_t st) {
+  const ns2vc_pre_cfg& c = h->cfg;
+  int rc;
+  if ((rc = pack_encoder(h, h->phone, "phoneme_encoder", c.phone_in, c.phone_hidden, c.phone_out, c.phone_layers, true, st))) return rc;
+  if ((rc = pack_encoder(h, h->prompt, "prompt_encoder", c.prompt_in, c.prompt_hidden, c.prompt_out, c.prompt_layers, false, st))) return rc;
+  return concat_pool_kv(h->mem, h->weights, "ref_enc.pool", c.ref_dim, h->ref_kv, st);
 }
 
 // The call arguments of one encoder: its lengths, its [B, C, T] input and its [B, T, C_out] output.
@@ -276,37 +277,28 @@ int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
-    h->prog = std::move(prog);
-    h->taps = std::move(taps);
-    h->pB = B; h->pT = T; h->pS = S; h->pws = ws; h->pR = ragged;
+    h->cp.prog = std::move(prog);
+    h->cp.taps = std::move(taps);
   }
   return 0;
 }
 
 int run_program(ns2vc_pre* h, const float* c, const float* refer, const long long* lengths, const long long* refer_lengths, float* content,
                 float* prompt, cudaStream_t st) {
-  int rc = 0, count = 0;
-  const int B = h->pB;
-  const Runner run{h->simt, B, &h->taps, st};
-  for (const Launch& l : h->prog) {
+  const int B = h->cp.dims[0];
+  return run_cached(h, h->simt, st, [&](const Launch& l) {
     switch (l.kind) {
-      case Launch::SEQMASK: rc = launch_seq_mask(l.input == Launch::LENGTHS ? lengths : refer_lengths, B, l.i0, l.o, l.o2, st, (int*)l.mem); break;
+      case Launch::SEQMASK: return launch_seq_mask(l.input == Launch::LENGTHS ? lengths : refer_lengths, B, l.i0, l.o, l.o2, st, (int*)l.mem);
       case Launch::ENC_INPUT: {
         const float* src = l.input == Launch::C ? c : refer;
-        rc = launch_enc_input(src, (long long)l.i0 * l.i1, l.b, l.c, B, l.i0, l.i1, l.o, l.i2, st);
-        break;
+        return launch_enc_input(src, (long long)l.i0 * l.i1, l.b, l.c, B, l.i0, l.i1, l.o, l.i2, st);
       }
-      case Launch::LN_MASK: rc = launch_ln_mask(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.d, l.input == Launch::CONTENT_OUT ? content : prompt, l.i2, st); break;
-      case Launch::NCT2TOK: rc = launch_nct_to_tokens(refer, (long long)l.i0 * l.i1, B, l.i0, l.i1, l.o, l.i0, l.i0, st); break;
-      case Launch::POOL_ATT_WIDE: rc = launch_pool_attend_wide(l.a, l.b, B, l.i0, l.i1, l.i2, l.o, st, l.lens); break;
-      case Launch::TAP: --count; rc = run.run(l); break;
-      default: rc = run.run(l); break;
+      case Launch::LN_MASK: return launch_ln_mask(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.d, l.input == Launch::CONTENT_OUT ? content : prompt, l.i2, st);
+      case Launch::NCT2TOK: return launch_nct_to_tokens(refer, (long long)l.i0 * l.i1, B, l.i0, l.i1, l.o, l.i0, l.i0, st);
+      case Launch::POOL_ATT_WIDE: return launch_pool_attend_wide(l.a, l.b, B, l.i0, l.i1, l.i2, l.o, st, l.lens);
+      default: return kSharedKind;
     }
-    if (rc) return rc;
-    ++count;
-  }
-  h->last_launches = count;
-  return 0;
+  });
 }
 
 }  // namespace
@@ -335,45 +327,13 @@ int ns2vc_pre_create(const ns2vc_pre_cfg* cfg, ns2vc_pre** out) {
   return 0;
 }
 
-void ns2vc_pre_destroy(ns2vc_pre* h) {
-  if (!h) return;
-  h->weights.release();
-  h->mem.release();
-  delete h;
-}
-
-int ns2vc_pre_num_weights(const ns2vc_pre* h) { return h ? h->weights.size() : -1; }
-
-int ns2vc_pre_weight_info(const ns2vc_pre* h, int i, const char** name, int64_t shape[4], int* ndim) {
-  NS_REQUIRE(h, "weight index %d out of range", i);
-  return h->weights.info(i, name, shape, ndim);
-}
-
+void ns2vc_pre_destroy(ns2vc_pre* h) { destroy_engine(h); }
+int ns2vc_pre_num_weights(const ns2vc_pre* h) { return num_weights(h); }
+int ns2vc_pre_weight_info(const ns2vc_pre* h, int i, const char** name, int64_t shape[4], int* ndim) { return weight_info(h, i, name, shape, ndim); }
 int ns2vc_pre_load_weight(ns2vc_pre* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream) {
-  NS_REQUIRE(h && key && dptr, "null argument");
-  const int rc = h->weights.load(key, dptr, shape, ndim, (cudaStream_t)stream);
-  if (rc) return rc;
-  h->finalized = false;
-  return 0;
+  return load_weight(h, key, dptr, shape, ndim, (cudaStream_t)stream);
 }
-
-int ns2vc_pre_finalize(ns2vc_pre* h, ns2vc_stream stream) {
-  NS_REQUIRE(h, "null handle");
-  int rc = h->weights.require_all_loaded();
-  if (rc) return rc;
-  h->mem.release();
-  h->prog.clear(); h->pB = h->pT = h->pS = 0; h->pws = nullptr; h->pR = false;
-  const ns2vc_pre_cfg& c = h->cfg;
-  cudaStream_t st = (cudaStream_t)stream;
-  rc = pack_encoder(h, h->phone, "phoneme_encoder", c.phone_in, c.phone_hidden, c.phone_out, c.phone_layers, true, st);
-  if (rc) return rc;
-  rc = pack_encoder(h, h->prompt, "prompt_encoder", c.prompt_in, c.prompt_hidden, c.prompt_out, c.prompt_layers, false, st);
-  if (rc) return rc;
-  if ((rc = concat_pool_kv(h->mem, h->weights, "ref_enc.pool", c.ref_dim, h->ref_kv, st))) return rc;
-  NS_CHECK_CUDA(cudaGetLastError());
-  h->finalized = true;
-  return 0;
-}
+int ns2vc_pre_finalize(ns2vc_pre* h, ns2vc_stream stream) { return finalize_engine(h, [&] { return pack(h, (cudaStream_t)stream); }); }
 
 int ns2vc_pre_workspace_bytes(const ns2vc_pre* h, int B, int T, int S, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
@@ -392,12 +352,8 @@ namespace {
 int infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content, float* prompt,
           int B, int T, int S, void* ws, bool ragged, cudaStream_t st) {
   NS_REQUIRE(h && c && refer && lengths && refer_lengths && content && prompt, "null argument");
-  NS_REQUIRE(h->finalized, "ns2vc_pre_finalize() has not been called");
-  NS_REQUIRE(ws != nullptr, "workspace is NULL");
-  if (!(h->pB == B && h->pT == T && h->pS == S && h->pws == ws && h->pR == ragged)) {
-    const int rc = build_program(h, B, T, S, ragged, ws, nullptr);
-    if (rc) return rc;
-  }
+  const int rc = ensure_program(h, "ns2vc_pre", B, T, S, ragged, ws, [&] { return build_program(h, B, T, S, ragged, ws, nullptr); });
+  if (rc) return rc;
   return run_program(h, c, refer, reinterpret_cast<const long long*>(lengths), reinterpret_cast<const long long*>(refer_lengths), content, prompt, st);
 }
 }  // namespace
@@ -414,15 +370,9 @@ int ns2vc_pre_infer_ragged(ns2vc_pre* h, const float* c, const float* refer, con
   return infer(h, c, refer, lengths, refer_lengths, content, prompt, B, T, S, ws, true, (cudaStream_t)stream);
 }
 
-int ns2vc_pre_num_taps(const ns2vc_pre* h) { return h ? h->taps.size() : -1; }
-int ns2vc_pre_tap_info(const ns2vc_pre* h, int i, const char** name, int* rows, int* channels) {
-  NS_REQUIRE(h, "tap index %d out of range", i);
-  return h->taps.info(i, name, rows, channels);
-}
-int ns2vc_pre_set_tap(ns2vc_pre* h, int i, float* dst) {
-  NS_REQUIRE(h, "tap index %d out of range", i);
-  return h->taps.set(i, dst);
-}
-int ns2vc_pre_launch_count(const ns2vc_pre* h) { return h ? h->last_launches : -1; }
+int ns2vc_pre_num_taps(const ns2vc_pre* h) { return num_taps(h); }
+int ns2vc_pre_tap_info(const ns2vc_pre* h, int i, const char** name, int* rows, int* channels) { return tap_info(h, i, name, rows, channels); }
+int ns2vc_pre_set_tap(ns2vc_pre* h, int i, float* dst) { return set_tap(h, i, dst); }
+int ns2vc_pre_launch_count(const ns2vc_pre* h) { return launch_count(h); }
 
 }  // extern "C"

@@ -301,11 +301,8 @@ int launch_voc_norm(const float* x, int B, int T, int C, const float* dw, const 
 
 using namespace ns2vc;
 
-struct ns2vc_voc {
+struct ns2vc_voc : SingleProgramEngine {
   ns2vc_voc_cfg cfg;
-  WeightRegistry weights;
-  DeviceMem mem;
-  bool finalized = false;
   PackedB embed, head;
   std::vector<PackedB> pw1, pw2;
   std::vector<float*> b2;                                   // gamma * pwconv2.bias per block
@@ -313,11 +310,6 @@ struct ns2vc_voc {
   float2* tw_half = nullptr; float2* tw_full = nullptr;
   int log2m = 0;
   size_t istft_smem = 0;
-  // cached program
-  int pB = 0, pT = 0; void* pws = nullptr;
-  std::vector<Launch> prog;
-  TapSet taps;
-  int last_launches = 0;
 };
 
 namespace {
@@ -460,34 +452,26 @@ int build_program(ns2vc_voc* h, int B, int T, void* ws, size_t* bytes_out) {
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
-    h->prog = std::move(prog);
-    h->taps = std::move(taps);
-    h->pB = B; h->pT = T; h->pws = ws;
+    h->cp.prog = std::move(prog);
+    h->cp.taps = std::move(taps);
   }
   return 0;
 }
 
 int run_program(ns2vc_voc* h, const float* mel, long long mel_bstride, const long long* lengths, float* audio, cudaStream_t st) {
-  int rc = 0, count = 0;
-  const int B = h->pB, T = h->pT;
-  const Runner run{false, B, &h->taps, st};
-  for (const Launch& l : h->prog) {
+  const int B = h->cp.dims[0], T = h->cp.dims[1];
+  return run_cached(h, false, st, [&](const Launch& l) {
     switch (l.kind) {
       case Launch::VOC_LENS:
         voc_lengths_kernel<<<ceil_div(B * T, 256), 256, 0, st>>>(lengths, B, T, static_cast<int*>(l.mem), l.o);
         NS_VOC_LAUNCH_CHECK();
-        break;
-      case Launch::NCT2SPLIT: rc = launch_nct_to_split(mel, mel_bstride, B, l.i0, l.i1, l.split, st, nullptr, 0, l.lens); break;
-      case Launch::VOC_NORM: rc = launch_voc_norm(l.a, B, l.i0, h->cfg.dim, l.d, l.b, l.c, l.f0, lengths, l.o, l.split, st); break;
-      case Launch::VOC_ISTFT: rc = launch_istft(h, l.a, l.i0, lengths, audio, B, l.i1, st); break;
-      case Launch::TAP: --count; rc = run.run(l); break;
-      default: rc = run.run(l); break;
+        return 0;
+      case Launch::NCT2SPLIT: return launch_nct_to_split(mel, mel_bstride, B, l.i0, l.i1, l.split, st, nullptr, 0, l.lens);
+      case Launch::VOC_NORM: return launch_voc_norm(l.a, B, l.i0, h->cfg.dim, l.d, l.b, l.c, l.f0, lengths, l.o, l.split, st);
+      case Launch::VOC_ISTFT: return launch_istft(h, l.a, l.i0, lengths, audio, B, l.i1, st);
+      default: return kSharedKind;
     }
-    if (rc) return rc;
-    ++count;
-  }
-  h->last_launches = count;
-  return 0;
+  });
 }
 
 }  // namespace
@@ -512,39 +496,13 @@ int ns2vc_voc_create(const ns2vc_voc_cfg* cfg, ns2vc_voc** out) {
   return 0;
 }
 
-void ns2vc_voc_destroy(ns2vc_voc* h) {
-  if (!h) return;
-  h->weights.release();
-  h->mem.release();
-  delete h;
-}
-
-int ns2vc_voc_num_weights(const ns2vc_voc* h) { return h ? h->weights.size() : -1; }
-
-int ns2vc_voc_weight_info(const ns2vc_voc* h, int i, const char** name, int64_t shape[4], int* ndim) {
-  NS_REQUIRE(h, "weight index %d out of range", i);
-  return h->weights.info(i, name, shape, ndim);
-}
-
+void ns2vc_voc_destroy(ns2vc_voc* h) { destroy_engine(h); }
+int ns2vc_voc_num_weights(const ns2vc_voc* h) { return num_weights(h); }
+int ns2vc_voc_weight_info(const ns2vc_voc* h, int i, const char** name, int64_t shape[4], int* ndim) { return weight_info(h, i, name, shape, ndim); }
 int ns2vc_voc_load_weight(ns2vc_voc* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream) {
-  NS_REQUIRE(h && key && dptr, "null argument");
-  const int rc = h->weights.load(key, dptr, shape, ndim, (cudaStream_t)stream);
-  if (rc) return rc;
-  h->finalized = false;
-  return 0;
+  return load_weight(h, key, dptr, shape, ndim, (cudaStream_t)stream);
 }
-
-int ns2vc_voc_finalize(ns2vc_voc* h, ns2vc_stream stream) {
-  NS_REQUIRE(h, "null handle");
-  int rc = h->weights.require_all_loaded();
-  if (rc) return rc;
-  h->mem.release();
-  h->prog.clear(); h->pB = h->pT = 0; h->pws = nullptr;
-  if ((rc = pack(h, (cudaStream_t)stream))) return rc;
-  NS_CHECK_CUDA(cudaGetLastError());
-  h->finalized = true;
-  return 0;
-}
+int ns2vc_voc_finalize(ns2vc_voc* h, ns2vc_stream stream) { return finalize_engine(h, [&] { return pack(h, (cudaStream_t)stream); }); }
 
 int ns2vc_voc_workspace_bytes(const ns2vc_voc* h, int B, int T, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
@@ -555,14 +513,10 @@ int ns2vc_voc_workspace_bytes(const ns2vc_voc* h, int B, int T, size_t* bytes) {
 int ns2vc_voc_decode(ns2vc_voc* h, const float* mel, long long mel_bstride, const int64_t* lengths, float* audio, int B, int T, void* ws,
                      ns2vc_stream stream) {
   NS_REQUIRE(h && mel && audio, "null argument");
-  NS_REQUIRE(h->finalized, "ns2vc_voc_finalize() has not been called");
-  NS_REQUIRE(ws != nullptr, "workspace is NULL");
   NS_REQUIRE(mel_bstride >= (long long)h->cfg.input_channels * T, "mel batch stride %lld shorter than a [%d, %d] row", mel_bstride,
              h->cfg.input_channels, T);
-  if (!(h->pB == B && h->pT == T && h->pws == ws)) {
-    const int rc = build_program(h, B, T, ws, nullptr);
-    if (rc) return rc;
-  }
+  const int rc = ensure_program(h, "ns2vc_voc", B, T, 0, false, ws, [&] { return build_program(h, B, T, ws, nullptr); });
+  if (rc) return rc;
   return run_program(h, mel, mel_bstride, reinterpret_cast<const long long*>(lengths), audio, (cudaStream_t)stream);
 }
 
@@ -573,15 +527,9 @@ int ns2vc_voc_istft(ns2vc_voc* h, const float* head_out, const int64_t* lengths,
   return launch_istft(h, head_out, h->cfg.n_fft + 2, reinterpret_cast<const long long*>(lengths), audio, B, T, (cudaStream_t)stream);
 }
 
-int ns2vc_voc_num_taps(const ns2vc_voc* h) { return h ? h->taps.size() : -1; }
-int ns2vc_voc_tap_info(const ns2vc_voc* h, int i, const char** name, int* rows, int* channels) {
-  NS_REQUIRE(h, "tap index %d out of range", i);
-  return h->taps.info(i, name, rows, channels);
-}
-int ns2vc_voc_set_tap(ns2vc_voc* h, int i, float* dst) {
-  NS_REQUIRE(h, "tap index %d out of range", i);
-  return h->taps.set(i, dst);
-}
-int ns2vc_voc_launch_count(const ns2vc_voc* h) { return h ? h->last_launches : -1; }
+int ns2vc_voc_num_taps(const ns2vc_voc* h) { return num_taps(h); }
+int ns2vc_voc_tap_info(const ns2vc_voc* h, int i, const char** name, int* rows, int* channels) { return tap_info(h, i, name, rows, channels); }
+int ns2vc_voc_set_tap(ns2vc_voc* h, int i, float* dst) { return set_tap(h, i, dst); }
+int ns2vc_voc_launch_count(const ns2vc_voc* h) { return launch_count(h); }
 
 }  // extern "C"

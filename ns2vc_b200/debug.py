@@ -14,28 +14,11 @@ def run_with_taps(unet, device: torch.device, B: int, T: int, run: Callable[[], 
     """Sets every tap of the engine's ACTIVE program (B, T: its batch and frame count), calls ``run()``, clears the taps.
     ``run`` must execute that program (the module call of the same shape, or ``DenoiserSession.forward`` of the session that
     prepared it) without building another one first.  Returns (run's result, {op name: activation [B,C,T_level]}) —
-    activations converted from the engine's token-major layout to the reference's channel-major layout; fresh buffers, so a
-    tap the program does not write is left uninitialised."""
-    L = _lib.lib()
-    h = unet.engine(device)
+    activations converted from the engine's token-major layout to the reference's channel-major layout; fresh zeroed
+    buffers, so a tap the program does not write reads 0."""
     Tl = level_lengths(T, len(unet.cfg.block_out_channels))
-    n = L.ns2vc_unet_num_taps(h)
-    bufs, names = [], []
-    try:
-        for i in range(n):
-            name, lvl, ch = C.c_char_p(), C.c_int(), C.c_int()
-            _lib.check(L.ns2vc_unet_tap_info(h, i, C.byref(name), C.byref(lvl), C.byref(ch)))
-            buf = torch.empty((B, Tl[lvl.value], ch.value), dtype=torch.float32, device=device)
-            _lib.check(L.ns2vc_unet_set_tap(h, i, buf.data_ptr()))
-            bufs.append(buf)
-            names.append(name.value.decode())
-        with torch.no_grad():
-            res = run()
-        torch.cuda.synchronize(device)
-    finally:
-        for i in range(n):
-            L.ns2vc_unet_set_tap(h, i, None)
-    return res, {k: v.permute(0, 2, 1).contiguous() for k, v in zip(names, bufs)}
+    res, bufs = unet._collect_taps(device, B, run, rows=lambda level: Tl[level])
+    return res, {k: v.permute(0, 2, 1).contiguous() for k, v in bufs.items()}
 
 
 def forward_with_taps(unet, sample: torch.Tensor, timestep, ehs: torch.Tensor,

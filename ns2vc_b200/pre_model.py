@@ -12,9 +12,8 @@ marshals pointers.  No CPU path; inference only (the reference's training forwar
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
-from typing import Dict, Optional, Tuple
+from typing import Dict, Tuple
 
 import torch
 import torch.nn as nn
@@ -76,7 +75,9 @@ def pre_param_shapes(cfg: dict) -> Dict[str, Tuple[int, ...]]:
     return shapes
 
 
-class Pre_model(nn.Module):
+class Pre_model(_lib.EngineModule):
+    _prefix, _cfg_struct, _requirement = "ns2vc_pre_", _lib.PreCfg, "these condition encoders need fp32 parameters on {device}"
+
     def __init__(self, cfg: dict) -> None:
         super().__init__()
         self.cfg = cfg
@@ -101,43 +102,16 @@ class Pre_model(nn.Module):
                     fan_in *= d
                 t = torch.empty(shape).uniform_(-1.0 / math.sqrt(fan_in), 1.0 / math.sqrt(fan_in))
             _insert(self, key, nn.Parameter(t))
-        self._handle: Optional[int] = None
-        self._handle_device = None
-        self._wsig = None
-        self._ws: Optional[torch.Tensor] = None
 
     # ------------------------------------------------------------------ engine management
     def _c_cfg(self) -> "_lib.PreCfg":
         pi, ph, po, pl = _enc_args(self.cfg["phoneme_encoder"], 512)
         ri, rh, ro, rl = _enc_args(self.cfg["prompt_encoder"], 256)
-        c = _lib.PreCfg()
+        c = self._cfg_struct()
         c.phone_in, c.phone_hidden, c.phone_out, c.phone_layers = pi, ph, po, pl
         c.prompt_in, c.prompt_hidden, c.prompt_out, c.prompt_layers = ri, rh, ro, rl
         c.ref_dim, c.ref_heads, c.n_heads, c.ffn_kernel = REF_DIM, 1, N_HEADS, FFN_KERNEL
         return c
-
-    def _release(self):
-        if _lib.release_engine(self, "ns2vc_pre_"):
-            self.__dict__["_ws"] = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
-
-    def engine(self, device: torch.device) -> int:
-        """Opaque engine handle with the current parameter values packed (re-packed when a parameter changed)."""
-        return _lib.engine_handle(self, "ns2vc_pre_", device, "these condition encoders need fp32 parameters on {device}")
-
-    def workspace(self, B: int, T: int, S: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.lib().ns2vc_pre_workspace_bytes(self.engine(device), B, T, S, C.byref(n)))
-        need = int(n.value)
-        ws = self._ws
-        if ws is None or ws.device != device or ws.numel() < need:
-            self._ws = ws = torch.empty(int(need * 1.25), dtype=torch.uint8, device=device)
-        return ws
 
     # ------------------------------------------------------------------ reference API
     @torch.no_grad()
@@ -199,27 +173,7 @@ class Pre_model(nn.Module):
     # diagnostics for the parity tests -------------------------------------------------------
     def taps(self, data, per_utterance: bool = False) -> Dict[str, torch.Tensor]:
         """Per-layer activations of one ``infer`` (token-major [B, rows, C]; the speaker vector as [B, 1, 100])."""
-        c_padded, refer_padded = data[0], data[1]
-        dev = c_padded.device
-        B, _, T = c_padded.shape
-        S = refer_padded.shape[2]
+        c_padded = data[0]
         self.infer(data, per_utterance=per_utterance)          # builds the program for this shape
-        L = _lib.lib()
-        h = self._handle
-        bufs = {}
-        for i in range(L.ns2vc_pre_num_taps(h)):
-            name, rows, ch = C.c_char_p(), C.c_int(), C.c_int()
-            _lib.check(L.ns2vc_pre_tap_info(h, i, C.byref(name), C.byref(rows), C.byref(ch)))
-            t = torch.zeros((B, rows.value, ch.value), dtype=torch.float32, device=dev)
-            _lib.check(L.ns2vc_pre_set_tap(h, i, t.data_ptr()))
-            bufs[name.value.decode()] = t
-        try:
-            self.infer(data, per_utterance=per_utterance)
-            torch.cuda.synchronize(dev)
-        finally:
-            for i in range(L.ns2vc_pre_num_taps(h)):
-                L.ns2vc_pre_set_tap(h, i, None)
+        _, bufs = self._collect_taps(c_padded.device, c_padded.shape[0], lambda: self.infer(data, per_utterance=per_utterance))
         return bufs
-
-    def launch_count(self) -> int:
-        return int(_lib.lib().ns2vc_pre_launch_count(self._handle)) if self._handle is not None else 0

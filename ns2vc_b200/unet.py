@@ -11,7 +11,6 @@ that would need gradients raises instead of silently detaching.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 import threading
 from collections import OrderedDict
@@ -105,7 +104,10 @@ class CallRecord:
     output: torch.Tensor
 
 
-class UNet1DConditionModel(nn.Module):
+class UNet1DConditionModel(_lib.EngineModule):
+    _prefix, _cfg_struct = "ns2vc_unet_", _lib.UNetCfg
+    _requirement = "this denoiser needs fp32 parameters on {device} (module.to('cuda'))"
+
     def __init__(
         self,
         sample_size: Optional[int] = None,
@@ -256,16 +258,10 @@ class UNet1DConditionModel(nn.Module):
                 t = torch.empty(shape).uniform_(-bound, bound)
             _insert(self, key, nn.Parameter(t))
 
-        self._handle: Optional[int] = None
-        self._wsig = None
-        self._ws: Dict[str, torch.Tensor] = {}
-        self._ws_need: Dict[Tuple[int, int, int], int] = {}
-        self._handle_device = None
-
     # ------------------------------------------------------------------ engine management
     def _c_cfg(self) -> _lib.UNetCfg:
         cfg = self.cfg
-        c = _lib.UNetCfg()
+        c = self._cfg_struct()
         c.in_channels, c.latent_channels, c.out_channels = cfg.in_channels, self.latent_channels, cfg.out_channels
         c.n_levels = len(cfg.block_out_channels)
         n = c.n_levels
@@ -281,47 +277,6 @@ class UNet1DConditionModel(nn.Module):
         c.add_embed_heads = cfg.addition_embed_type_num_heads
         c.flip_sin_to_cos, c.freq_shift = int(cfg.flip_sin_to_cos), float(cfg.freq_shift)
         return c
-
-    def _release(self):
-        if _lib.release_engine(self, "ns2vc_unet_"):
-            self.__dict__["_ws"] = {}
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
-
-    def engine(self, device: torch.device) -> int:
-        """Opaque engine handle with the current parameter values packed for the tensor cores
-        (re-packed when any parameter changed: optimizer step, load_state_dict, .to())."""
-        sig = self._wsig
-        h = _lib.engine_handle(self, "ns2vc_unet_", device, "this denoiser needs fp32 parameters on {device} (module.to('cuda'))")
-        if self._wsig is not sig:       # (re)loaded: the workspace sizes are asked again
-            self._ws_need = {}
-        return h
-
-    def workspace(self, B: int, T: int, S: int, device: torch.device) -> torch.Tensor:
-        """ONE grow-only scratch buffer per module, shared by every shape (the CLI feeds a different T per slice: a fresh
-        multi-hundred-MB allocation per shape was most of a cold call).  Calls are stream-ordered and never concurrent, and
-        every program re-runs prepare_cond after a shape switch, so shapes can alias the same memory.  Growing it invalidates
-        the captured loops that baked the old pointer (the sessions are dropped)."""
-        key = (B, T, S)
-        need = self._ws_need.get(key)
-        if need is None:
-            n = C.c_size_t()
-            _lib.check(_lib.lib().ns2vc_unet_workspace_bytes(self.engine(device), B, T, S, C.byref(n)))
-            need = int(n.value)
-            if len(self._ws_need) > 256:
-                self._ws_need.clear()
-            self._ws_need[key] = need
-        pool = self._ws.get("pool")
-        if pool is None or pool.device != device or pool.numel() < need:
-            self.__dict__.get("_sessions", {}).clear()
-            self._ws.pop("pool", None)
-            pool = None
-            self._ws["pool"] = pool = torch.empty(int(need * 1.25) if need < (8 << 30) else need, dtype=torch.uint8, device=device)
-        return pool
 
     def plan_string(self) -> str:
         return "".join(f"{o.kind}|{o.prefix}|{o.cin}|{o.cout}|{o.level}\n" for o in build_plan(self.cfg))

@@ -11,7 +11,6 @@ inference only.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional, Tuple
 
 import torch
@@ -59,7 +58,9 @@ def vocos_init(key: str, shape: Tuple[int, ...], num_layers: int, generator: Opt
     return torch.nn.init.trunc_normal_(torch.empty(shape), std=0.02, generator=generator)
 
 
-class Vocos(nn.Module):
+class Vocos(_lib.EngineModule):
+    _prefix, _cfg_struct, _requirement = "ns2vc_voc_", _lib.VocCfg, "this vocoder needs fp32 parameters on {device}"
+
     def __init__(self, input_channels: int = 100, dim: int = 512, intermediate_dim: int = 1536, num_layers: int = 8,
                  n_fft: int = 1024, hop_length: int = 256) -> None:
         super().__init__()
@@ -70,10 +71,6 @@ class Vocos(nn.Module):
         for key, shape in vocos_param_shapes(input_channels, dim, intermediate_dim, num_layers, n_fft).items():
             # the window is a buffer in the package; here it is a frozen parameter, so that a change re-packs the engine
             _insert(self, key, nn.Parameter(vocos_init(key, shape, num_layers), requires_grad=not key.endswith("istft.window")))
-        self._handle: Optional[int] = None
-        self._handle_device = None
-        self._wsig = None
-        self._ws: Optional[torch.Tensor] = None
 
     @property
     def hop_length(self) -> int:
@@ -103,16 +100,7 @@ class Vocos(nn.Module):
         if n_fft != 4 * hop_length:
             raise ValueError(f"head.out.weight gives n_fft {n_fft}; with hop_length {hop_length} only n_fft = 4 * hop_length is supported")
         m = cls(int(input_channels), int(dim), int(intermediate_dim), num_layers, int(n_fft), int(hop_length))
-        want = m.state_dict()
-        for k in want:
-            need(k)
-        for k, v in sd.items():
-            if k not in want:
-                raise ValueError(f"unexpected key {k} in the Vocos state_dict")
-            if tuple(v.shape) != tuple(want[k].shape):
-                raise ValueError(f"size mismatch for {k}: expected {tuple(want[k].shape)}, got {tuple(v.shape)}")
-        m.load_state_dict({k: v.detach().to(torch.float32) for k, v in sd.items()})
-        return m
+        return m._load_checked(sd, "Vocos")
 
     @classmethod
     def from_vocos(cls, obj) -> "Vocos":
@@ -126,36 +114,6 @@ class Vocos(nn.Module):
         m = cls.from_state_dict(sd, hop_length=int(istft.hop_length))
         dev = sd["head.out.weight"].device
         return m.to(dev)
-
-    # ------------------------------------------------------------------ engine management
-    def _c_cfg(self) -> "_lib.VocCfg":
-        c = _lib.VocCfg()
-        for k, v in self.cfg.items():
-            setattr(c, k, int(v))
-        return c
-
-    def _release(self):
-        if _lib.release_engine(self, "ns2vc_voc_"):
-            self.__dict__["_ws"] = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
-
-    def engine(self, device: torch.device) -> int:
-        """Opaque engine handle with the current parameter values packed (re-packed when a parameter changed)."""
-        return _lib.engine_handle(self, "ns2vc_voc_", device, "this vocoder needs fp32 parameters on {device}")
-
-    def workspace(self, B: int, T: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.lib().ns2vc_voc_workspace_bytes(self.engine(device), B, T, C.byref(n)))
-        need = int(n.value)
-        ws = self._ws
-        if ws is None or ws.device != device or ws.numel() < need:
-            self._ws = ws = torch.empty(int(need * 1.25), dtype=torch.uint8, device=device)
-        return ws
 
     def _lengths(self, lengths, B: int, T: int, dev: torch.device) -> Optional[torch.Tensor]:
         if lengths is None:
@@ -214,26 +172,9 @@ class Vocos(nn.Module):
     def taps(self, features_input: torch.Tensor, lengths=None) -> Dict[str, torch.Tensor]:
         """Activations of one ``decode`` (token-major [B, T, C]: after backbone.norm, each convnext block, final_layer_norm and
         head.out) plus its result under ``"audio"``."""
-        B, _, T = features_input.shape
-        dev = features_input.device
+        B = features_input.shape[0]
         self.decode(features_input, lengths)                     # builds the program for this shape
-        L = _lib.lib()
-        h = self._handle
-        bufs = {}
-        for i in range(L.ns2vc_voc_num_taps(h)):
-            name, rows, ch = C.c_char_p(), C.c_int(), C.c_int()
-            _lib.check(L.ns2vc_voc_tap_info(h, i, C.byref(name), C.byref(rows), C.byref(ch)))
-            t = torch.zeros((B, rows.value, ch.value), dtype=torch.float32, device=dev)
-            _lib.check(L.ns2vc_voc_set_tap(h, i, t.data_ptr()))
-            bufs[name.value.decode()] = t
-        try:
-            bufs["audio"] = self.decode(features_input, lengths)
-            torch.cuda.synchronize(dev)
-        finally:
-            for i in range(L.ns2vc_voc_num_taps(h)):
-                L.ns2vc_voc_set_tap(h, i, None)
+        audio, bufs = self._collect_taps(features_input.device, B, lambda: self.decode(features_input, lengths))
+        bufs["audio"] = audio
         bufs["head.out"] = bufs["head.out"][:, :, :self.cfg["n_fft"] + 2]
         return bufs
-
-    def launch_count(self) -> int:
-        return int(_lib.lib().ns2vc_voc_launch_count(self._handle)) if self._handle is not None else 0
