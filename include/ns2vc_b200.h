@@ -372,6 +372,33 @@ long long ns2vc_slice_rms_frames(long long n, int hop, int win);
 int ns2vc_slice_rms(const float* wav, long long wav_bstride, const int64_t* lengths, const int* hop_win, float* rms, int F, int B,
                     ns2vc_stream stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Training objective of NaturalSpeech2.forward (model.py:698-734) under no_grad, at K timesteps per batch of B rows.
+ * q_sample: x_start = spec * mask, noise_m = noise * mask, x[k] = sqrt_ac[t[k,b]] * x_start + sqrt_1mac[t[k,b]] * noise_m with
+ * mask[b, :, f] = (f < lengths[b]) as a 0/1 factor, every product and the sum rounded separately: bit-identical to the
+ * reference's torch expression on the device.  Inputs must be finite (a non-finite value past a length gives NaN there, as
+ * in the reference).
+ *   spec [B, C, T] fp32, lengths [B] int64, t [K, B] int64 (a value outside [0, timesteps) gives NaN), all device
+ *   noise [K, B, C, T] (noise_per_k != 0) or one [B, C, T] shared by every k (noise_per_k == 0)
+ *   sqrt_alphas_cumprod, sqrt_one_minus_alphas_cumprod [timesteps] fp32 device
+ *   x_start [B, C, T], x [K, B, C, T]; noise_masked: NULL, or the shape of noise
+ * Stream-ordered, allocates nothing, capturable. */
+int ns2vc_q_sample(const float* spec, const float* noise, int noise_per_k, const int64_t* lengths, const int64_t* t,
+                   const float* sqrt_alphas_cumprod, const float* sqrt_one_minus_alphas_cumprod, int timesteps, float* x_start,
+                   float* noise_masked, float* x, int K, int B, int C, int T, ns2vc_stream stream);
+/* Host-only: bytes of the scratch buffer ns2vc_mse_rows needs (its contents on entry do not matter). */
+int ns2vc_mse_workspace_bytes(int K, int B, int C, int T, size_t* bytes);
+/* loss_row[k, b] = mean over C * T of (out[k, b] - target[b])^2 (padded frames included, as F.mse_loss over the padded row),
+ * loss_weighted[k, b] = loss_row * w with w = loss_weight[t[k, b]], clamped to min_snr_gamma when that is > 0,
+ * loss[k] = mean_b(w) * mean_b(loss_row[k, b]): the number forward() returns, whose [B, C*T] x [B, 1, 1] product broadcasts over
+ * a second batch axis (model.py:723-726); it equals mean_b(loss_weighted) when every row has the same t.  out [K, B, C, T]; target [K, B, C, T] (target_per_k != 0) or [B, C, T];
+ * K * B <= 65535.  Sums run in fp64 over a partition and in an order that depend on C * T only, without atomics, so two
+ * launches give the same bits; every fp32 output is rounded once from fp64.  ws: 8-byte aligned device scratch.
+ * Stream-ordered, allocates nothing, capturable. */
+int ns2vc_mse_rows(const float* out, const float* target, int target_per_k, const int64_t* t, const float* loss_weight, int timesteps,
+                   float min_snr_gamma, float* loss_row, float* loss_weighted, float* loss, int K, int B, int C, int T, void* ws,
+                   ns2vc_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

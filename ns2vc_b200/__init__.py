@@ -7,6 +7,7 @@ Drop-in surface (same names as the reference):
     ns2vc_b200.pre_model.Pre_model                <- model.py:328-377 (condition encoders; ``install_pre_model(model)``)
     ns2vc_b200.frontend.repeat_expand_2d          <- utils.py:482-496 (feature stretch in front of the encoders)
     ns2vc_b200.diffusion.{p_sample_loop, ddim_sample} <- model.py:544-603 (DDPM / DDIM; ``install_diffusion(model)``)
+    ns2vc_b200.loss.diffusion_loss                <- model.py:706-734 (``NaturalSpeech2.forward``'s objective, no gradients)
 ``ns2vc_b200.install()`` aliases those module paths so the reference's model.py / infer.py import
 them unchanged (see INTEGRATION.md).
 """
@@ -63,7 +64,8 @@ def install_pre_model(model_module=None) -> None:
 
 def install_diffusion(model_module=None) -> None:
     """Make the reference's ``NaturalSpeech2.p_sample_loop`` / ``.ddim_sample`` (``sample_method='ddpm'`` / ``'ddim'``, model.py:544-603)
-    take the fused DDPM / DDIM loops when the denoiser is our UNet (``ns2vc_b200.diffusion``); call after ``import model``."""
+    take the fused DDPM / DDIM loops when the denoiser is our UNet (``ns2vc_b200.diffusion``), and add
+    ``NaturalSpeech2.validation_loss``: ``forward``'s objective under ``no_grad`` on the device path.  Call after ``import model``."""
     from . import diffusion
     if model_module is None:
         model_module = sys.modules.get("model")
@@ -71,3 +73,5 @@ def install_diffusion(model_module=None) -> None:
         raise RuntimeError("install_diffusion: import the reference's model.py first (or pass the module)")
     model_module.NaturalSpeech2.p_sample_loop = diffusion.p_sample_loop
     model_module.NaturalSpeech2.ddim_sample = diffusion.ddim_sample
+    # the training objective under no_grad (model.py:706-734); `forward` itself stays the reference's
+    model_module.NaturalSpeech2.validation_loss = diffusion.validation_loss

@@ -163,6 +163,10 @@ SIGNATURES = {
     # silence slicer (framewise RMS)
     "ns2vc_slice_rms_frames": (C.c_longlong, [C.c_longlong, C.c_int, C.c_int]),
     "ns2vc_slice_rms": (C.c_int, [_P, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, _P]),
+    # training objective (q_sample and the SNR-weighted per-row MSE)
+    "ns2vc_q_sample": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "ns2vc_mse_workspace_bytes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ns2vc_mse_rows": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_float, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -226,10 +226,13 @@ def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Op
 
 
 def __getattr__(name):
-    # waveform-to-waveform conversion lives in convert.py and live conversion in stream.py; both build on this module
+    # waveform-to-waveform conversion lives in convert.py and live conversion in stream.py; they build on this module
     if name in ("convert_utterances", "convert_slices", "convert_files"):
         from . import convert
         return getattr(convert, name)
+    if name in ("diffusion_loss", "loss_profile"):           # the training objective under no_grad lives in loss.py
+        from . import loss
+        return getattr(loss, name)
     if name == "StreamConverter":
         from . import stream
         return stream.StreamConverter

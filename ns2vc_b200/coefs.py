@@ -179,6 +179,24 @@ def diffusion_buffers(timesteps: int = 1000) -> dict:
     }
 
 
+def loss_buffers(timesteps: int = 1000, min_snr_gamma=None) -> dict:
+    """The schedule buffers ``NaturalSpeech2.forward`` reads (reference model.py:461-498), fp64 then cast to fp32 as
+    ``register_buffer`` does: ``sqrt_alphas_cumprod`` and ``sqrt_one_minus_alphas_cumprod`` (``q_sample``) and ``loss_weight``,
+    the SNR ``alphas_cumprod / (1 - alphas_cumprod)``, clamped to ``min_snr_gamma`` when given (``min_snr_loss_weight=True``)."""
+    scale = 1000 / timesteps
+    betas = torch.linspace(scale * 0.0001, scale * 0.02, timesteps, dtype=torch.float64)
+    alphas_cumprod = torch.cumprod(1. - betas, dim=0)
+    snr = alphas_cumprod / (1 - alphas_cumprod)
+    if min_snr_gamma is not None:
+        snr = snr.clamp(max=min_snr_gamma)
+    f32 = lambda v: v.to(torch.float32)
+    return {
+        "sqrt_alphas_cumprod": f32(torch.sqrt(alphas_cumprod)),
+        "sqrt_one_minus_alphas_cumprod": f32(torch.sqrt(1. - alphas_cumprod)),
+        "loss_weight": f32(snr),
+    }
+
+
 @dataclass
 class DdpmStep:
     t_input: float      # model time: the integer timestep t

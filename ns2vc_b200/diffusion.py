@@ -31,6 +31,41 @@ def _buffers_match(model) -> bool:
     return True
 
 
+def _loss_gamma(model):
+    """(True, gamma) when the model's ``q_sample`` / ``loss_weight`` buffers are the ones ``coefs.loss_buffers`` computes; gamma is
+    the clamp its ``loss_weight`` was built with (``min_snr_loss_weight=True``) or None.  A clamped weight table's maximum is
+    the clamp itself: the SNR at t = 0 is ~1e4."""
+    lw = getattr(model, "loss_weight", None)
+    if not torch.is_tensor(lw) or lw.dtype != torch.float32 or lw.shape != (1000,):
+        return False, None
+    plain = coefs.loss_buffers(1000)
+    gamma = None if torch.equal(lw.detach().cpu(), plain["loss_weight"]) else float(lw.max())
+    ours = plain if gamma is None else coefs.loss_buffers(1000, gamma)
+    for name, v in ours.items():
+        b = getattr(model, name, None)
+        if not torch.is_tensor(b) or b.dtype != torch.float32 or not torch.equal(b.detach().cpu(), v):
+            return False, None
+    return True, gamma
+
+
+def validation_loss(self, data, t=None, noise=None):
+    """``NaturalSpeech2.forward(data, vocos)`` (reference model.py:706-734) under ``no_grad`` through ``loss.diffusion_loss``: the
+    same 7-tuple ``(loss, loss_diff, 0, 0, 0, model_out, target)``, with ``t`` / ``noise`` drawn as ``forward`` draws them unless
+    given ([K, B] ``t`` gives [K] losses).  ``forward`` itself is untouched: training keeps the reference's modules.  Raises when
+    the object's modules or schedule buffers are not the ones the device path computes with."""
+    from .loss import diffusion_loss
+    from .pre_model import Pre_model
+    unet = getattr(self.diff_model, "unet", None)
+    if not isinstance(self.pre_model, Pre_model) or not isinstance(unet, UNet1DConditionModel):
+        raise TypeError("validation_loss needs ns2vc_b200's Pre_model and UNet1DConditionModel in the model (install() and "
+                        "install_pre_model() before it is constructed)")
+    ok, gamma = _loss_gamma(self)
+    if not (ok and _buffers_match(self)):
+        raise ValueError("validation_loss supports NaturalSpeech2's 1000-step linear-beta schedule buffers; this model's differ")
+    r = diffusion_loss(self.pre_model, unet, data, t=t, noise=noise, timesteps=1000, min_snr_gamma=gamma)
+    return r.loss, r.loss, 0, 0, 0, r.model_out, r.target
+
+
 def _our_call(recs, x: torch.Tensor, x_start: torch.Tensor, time: int):
     """The call record if the first model_predictions was one call of our UNet on cat([x, content]) at ``time`` whose output is
     x_start itself, else None (same test as fused._trace_first_call, for the reference's x_start parameterisation)."""

@@ -448,6 +448,37 @@ class DenoiserSession:
         return self._chain("ddim", x_T, ("ddim", S, eta), lambda: coefs.ddim_table(buf, total, S, eta), first_out, noise)
 
 
+    # ------------------------------------------------------------------ training objective: K evaluations behind one prepare
+    def eval_x_start(self, x_KBCT: torch.Tensor, t_KB: torch.Tensor, out_KBCT: torch.Tensor) -> torch.Tensor:
+        """The denoiser's x_start prediction of K noisy batches on this session's conditioning: ``out[k] = denoiser(x[k], t[k])``
+        with x [K, B, Cl, T] fp32 and t [K, B] (integer timesteps, any dtype) on the session device.  ``prepare()`` runs once
+        and the FiLM rows of all K * B times come from one ``time_table`` launch per CHUNK evaluations; each evaluation is the
+        ``forward`` the samplers run.  Eager (no CUDA graph).  Padded sessions only: ``NaturalSpeech2.forward`` averages its
+        loss over the padded rows."""
+        if self.ragged:
+            raise ValueError("eval_x_start runs the padded program (the reference's objective averages over padded rows)")
+        K = x_KBCT.shape[0]
+        if tuple(x_KBCT.shape) != (K, self.B, self.Cl, self.T) or tuple(t_KB.shape) != (K, self.B) \
+                or tuple(out_KBCT.shape) != (K, self.B, self.Co, self.T):
+            raise ValueError(f"expected x [K, {self.B}, {self.Cl}, {self.T}], t [K, {self.B}] and out [K, {self.B}, {self.Co}, {self.T}], "
+                             f"got {tuple(x_KBCT.shape)}, {tuple(t_KB.shape)}, {tuple(out_KBCT.shape)}")
+        for v in (x_KBCT, out_KBCT):
+            if v.dtype != torch.float32 or not v.is_contiguous() or v.device != self.dev:
+                raise ValueError("x and out must be contiguous fp32 tensors on the session device")
+        self._sync_engine()
+        self.prepare()
+        tvals = t_KB.to(self.dev, torch.float32).contiguous()
+        fw = int(self.L.ns2vc_unet_film_width(self.h))
+        n = min(K, self.CHUNK)
+        table = torch.empty(int(self.L.ns2vc_unet_time_table_floats(self.h, n * self.B)), dtype=torch.float32, device=self.dev)
+        for j in range(0, K, self.CHUNK):
+            L = min(self.CHUNK, K - j)
+            self.time_table(tvals[j:j + L], table)
+            for k in range(L):
+                self.forward(x_KBCT[j + k], None, out_KBCT[j + k], film_rows=table[k * self.B * fw:(k + 1) * self.B * fw])
+        return out_KBCT
+
+
 def check_lengths(lengths, B: int, limit: int, name: str) -> list:
     """Per-utterance lengths as a list of B ints in [1, limit]; ValueError otherwise."""
     vals = [int(v) for v in (lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)]
