@@ -399,6 +399,57 @@ int ns2vc_mse_rows(const float* out, const float* target, int target_per_k, cons
                    float min_snr_gamma, float* loss_row, float* loss_weighted, float* loss, int K, int B, int C, int T, void* ws,
                    ns2vc_stream stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Kernel checks (tests only): one weight packing, one wgmma GEMM or one flash attention through the engines' own host code
+ * and launchers, described by flat structs.  Every pointer is device memory; invalid combinations come back as the
+ * launchers' error codes.  `desc` (desc_len bytes, may be NULL) receives the kernel and template arguments launched.
+ * Stream-ordered (the GEMM allocates and frees its panel-affine descriptor on the stream). */
+typedef struct ns2vc_check_split {   /* a bf16 hi/lo split activation [B, T, ld] (16-bit elements), C valid channels */
+  const void* hi; const void* lo;
+  int T, C, ld;
+  long long bpitch;                  /* elements between batch entries; 0: T * ld */
+} ns2vc_check_split;
+typedef struct ns2vc_check_gemm_args {
+  int B, T_out;
+  int nsrc; ns2vc_check_split src[4];
+  int nseg; int seg[8][4];           /* plain segments: source, first channel, channels, row offset (tap) */
+  int nxs; int xseg[4][8];           /* panel segments: source, c0, channels, taps (1 | 3), k-block of tap 0, k-block stride of the
+                                        taps, normalise (0 | 1), first channel of the affine table */
+  const void* w_hi; const void* w_lo; /* packed weights (ns2vc_check_pack_b), N columns x nkb_w k-blocks */
+  int N, n_valid, nkb_w;
+  int flags;                         /* EPI_* bits of the GEMM epilogue (csrc/common.cuh) */
+  const float* bias; const float* rowbias; int rowbias_ld;
+  const float* res; int res_ld;
+  float* out; int out_ld;
+  void* out_hi; void* out_lo; int out_split_ld;
+  int f16_col0;                      /* split columns >= f16_col0 stored as fp16 hi/lo; < 0: none */
+  const double* ln_stats; const float* ln_g; int ln_C; float ln_eps;
+  double* row_stats; double* stat_sum; double* stat_sq;
+  const float* rowmask;
+  const int* row_len; int len_shift;
+  const float* pre_scale; const float* pre_shift; /* panel mode: the affine [B, pre_C] applied to the normalised segments */
+  int pre_mode;                      /* 1: x * scale + shift, 2: then SiLU */
+  int pre_C;
+  int ksplit;                        /* panel mode: 1 or 2 CTAs per tile */
+} ns2vc_check_gemm_args;
+typedef struct ns2vc_check_attn_args {
+  int B, H, Tq, Tk, dh;
+  float scale;
+  int v2;                            /* 1: the TMA-fed kernel over split q / k / v; 0: the fp32-input tensor-core kernel */
+  const float* q; int q_ld; const float* k; int k_ld; const float* v; int v_ld;
+  ns2vc_check_split qs, ks, vs;      /* v2; head h of x at channels [x_c0 + h dh, x_c0 + (h + 1) dh) */
+  int q_c0, k_c0, v_c0;
+  int p_split;
+  const int* key_len; int key_shift;
+  const float* bias;                 /* additive [B, Tk] or NULL */
+  float* out; int out_ld;
+  void* out_hi; void* out_lo; int out_split_ld;
+} ns2vc_check_attn_args;
+int ns2vc_check_pack_b(const float* w, int n_rows, int cin_total, int ktaps, int tap, int cin0, int ncin, int n_dst0, int kb0,
+                       int geglu_half, const float* cscale, void* w_hi, void* w_lo, int Npad, int nkb_total, ns2vc_stream stream);
+int ns2vc_check_gemm(const ns2vc_check_gemm_args* args, char* desc, int desc_len, ns2vc_stream stream);
+int ns2vc_check_attention(const ns2vc_check_attn_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -425,14 +425,6 @@ struct Builder : ProgramBuilder {
     Launch& l = ProgramBuilder::emit_gemm(g, w, in);
     if (g.pre_film || (g.flags & EPI_ROWBIAS)) l.reads_film = 1;
   }
-  // ---- panel mode (GemmOp::xmode): raw split sources normalised inside the GEMM
-  void xseg(GemmOp& g, int src, int c0, int nch, int ntap, int kb0, int kb_stride, int xf, int aff_c0) {
-    XSeg& x = g.xs[g.nxs++];
-    x.src = src; x.c0 = c0; x.ncb = nkb_of(nch); x.ntap = ntap; x.xf = xf; x.aff_c0 = aff_c0;
-    for (int j = 0; j < 3; ++j) x.kb_tap[j] = kb0 + j * kb_stride;
-    g.nkb_total += x.ncb * ntap;
-    g.xmode = 1;
-  }
   // GroupNorm parameters of a panel-mode GEMM (statistics of up to two concatenated producers), parked in the workspace
   const PrepOp* affine_desc(const double* st1, int C1, const double* st2, int C2, int Tn, int mode, float eps, const float* gamma,
                             const float* beta, int film_ld, int level) {

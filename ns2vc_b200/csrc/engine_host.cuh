@@ -234,6 +234,14 @@ struct ProgramBuilder {
     s.src = src; s.c0 = c0; s.nkb = nkb_of(nch); s.tap = tap;
     g.nkb_total += s.nkb;
   }
+  // ---- panel mode (GemmOp::xmode): raw split sources normalised inside the GEMM
+  void xseg(GemmOp& g, int src, int c0, int nch, int ntap, int kb0, int kb_stride, int xf, int aff_c0) {
+    XSeg& x = g.xs[g.nxs++];
+    x.src = src; x.c0 = c0; x.ncb = nkb_of(nch); x.ntap = ntap; x.xf = xf; x.aff_c0 = aff_c0;
+    for (int j = 0; j < 3; ++j) x.kb_tap[j] = kb0 + j * kb_stride;
+    g.nkb_total += x.ncb * ntap;
+    g.xmode = 1;
+  }
   // a linear layer: one unshifted segment over all channels of `in`
   GemmOp lin(const PackedB& w, const SplitBuf& in, int T_out) {
     GemmOp g = gemm_base(w, T_out);

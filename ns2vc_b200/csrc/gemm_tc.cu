@@ -826,7 +826,8 @@ int encode_tmaps(GemmOp& op) {
   // (one thread per row storing straight to global memory would cost 32 LSU wavefronts per 128-bit store instruction).
   op.tma_out = 0;
   if (!(op.flags & EPI_OUT_NCT)) {
-    if ((op.flags & EPI_OUT_F32) && op.out && (op.out_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(op.out) & 15) == 0) {
+    // (the GEGLU epilogue does not stage its fp32 chunk for a bulk store: its fp32 output takes the element-wise path)
+    if ((op.flags & EPI_OUT_F32) && !(op.flags & EPI_GEGLU) && op.out && (op.out_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(op.out) & 15) == 0) {
       int rc = encode_tmap_any(&op.tmap_out[0], op.out, 4, op.n_valid, op.T_out, op.B, op.out_ld, 32, 32, 128);
       if (rc) return rc;
       op.tma_out |= 1;

@@ -1,0 +1,151 @@
+// Test-only entry points into the product launchers: one weight packing, one wgmma GEMM and one flash attention, each
+// described by a flat C struct (include/ns2vc_b200.h, "kernel checks") and run through exactly the host code the engines use
+// (pack_seg, the ProgramBuilder helpers, plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention
+// dispatch).  tests/test_kernels_fp64.py drives them at the shapes and edges the models never reach.  Nothing here is a
+// kernel: every launch is the product's own.
+#include "engine_host.cuh"
+#include "../../include/ns2vc_b200.h"
+
+#include <cstdio>
+
+namespace ns2vc {
+namespace {
+
+SplitBuf to_split(const ns2vc_check_split& s) {
+  SplitBuf b{};
+  b.hi = (__nv_bfloat16*)s.hi; b.lo = (__nv_bfloat16*)s.lo; b.T = s.T; b.C = s.C; b.ld = s.ld; b.bpitch = s.bpitch;
+  return b;
+}
+
+// the kernel and template arguments a launch selected, for the caller's `desc` (may be null)
+template <class... A> void report(char* desc, int desc_len, const char* fmt, A... args) {
+  if (desc && desc_len > 0) snprintf(desc, (size_t)desc_len, fmt, args...);
+}
+
+}  // namespace
+}  // namespace ns2vc
+
+using namespace ns2vc;
+
+extern "C" {
+
+int ns2vc_check_pack_b(const float* w, int n_rows, int cin_total, int ktaps, int tap, int cin0, int ncin, int n_dst0, int kb0,
+                       int geglu_half, const float* cscale, void* w_hi, void* w_lo, int Npad, int nkb_total, ns2vc_stream stream) {
+  NS_REQUIRE(w && w_hi && w_lo, "check_pack_b: null argument");
+  NS_REQUIRE(n_rows >= 1 && ktaps >= 1 && tap >= 0 && tap < ktaps && cin0 >= 0 && ncin >= 1 && cin0 + ncin <= cin_total,
+             "check_pack_b: bad weight slice n_rows=%d cin=%d+%d of %d tap=%d of %d", n_rows, cin0, ncin, cin_total, tap, ktaps);
+  NS_REQUIRE(Npad % 128 == 0 && n_dst0 >= 0 && n_dst0 + n_rows <= Npad, "check_pack_b: columns %d+%d do not fit Npad=%d", n_dst0, n_rows, Npad);
+  NS_REQUIRE(kb0 >= 0 && kb0 + nkb_of(ncin) <= nkb_total, "check_pack_b: k-blocks %d+%d do not fit %d", kb0, nkb_of(ncin), nkb_total);
+  NS_REQUIRE(geglu_half == 0 || 2 * geglu_half == n_rows, "check_pack_b: a GEGLU weight has 2 * geglu_half rows");
+  PackedB pb;
+  pb.hi = (__nv_bfloat16*)w_hi; pb.lo = (__nv_bfloat16*)w_lo; pb.Npad = Npad; pb.nkb = nkb_total;
+  return pack_seg(pb, w, n_rows, cin_total, ktaps, tap, cin0, ncin, n_dst0, kb0, geglu_half, (cudaStream_t)stream, cscale);
+}
+
+int ns2vc_check_gemm(const ns2vc_check_gemm_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a, "check_gemm: null argument");
+  NS_REQUIRE(a->B >= 1 && a->T_out >= 1, "check_gemm: bad sizes B=%d T_out=%d", a->B, a->T_out);
+  NS_REQUIRE(a->nsrc >= 1 && a->nsrc <= kMaxSrc && a->nseg >= 0 && a->nseg <= kMaxSeg && a->nxs >= 0 && a->nxs <= kMaxXSeg,
+             "check_gemm: %d sources (1..%d), %d segments (0..%d), %d panel segments (0..%d)", a->nsrc, kMaxSrc, a->nseg, kMaxSeg,
+             a->nxs, kMaxXSeg);
+  NS_REQUIRE((a->nseg > 0) != (a->nxs > 0), "check_gemm: either plain segments or panel segments");
+  NS_REQUIRE(a->w_hi && a->w_lo, "check_gemm: null weights");
+  const int f = a->flags;
+  NS_REQUIRE(!(f & (EPI_OUT_F32 | EPI_OUT_NCT)) || a->out, "check_gemm: fp32 output without a buffer");
+  NS_REQUIRE(!(f & EPI_OUT_SPLIT) || (a->out_hi && a->out_lo), "check_gemm: split output without buffers");
+  NS_REQUIRE(!(f & (EPI_BIAS | EPI_GEGLU)) || a->bias, "check_gemm: bias flag without a bias");
+  NS_REQUIRE(!(f & EPI_RESIDUAL) || a->res, "check_gemm: residual flag without a residual");
+  NS_REQUIRE(!(f & EPI_ROWBIAS) || a->rowbias, "check_gemm: row-bias flag without a row bias");
+  NS_REQUIRE(!(f & EPI_LNFOLD) || (a->ln_stats && a->ln_g && a->ln_C > 0), "check_gemm: folded LayerNorm without statistics");
+  NS_REQUIRE(!(f & EPI_ROWSTATS) || a->row_stats, "check_gemm: row statistics without a buffer");
+  NS_REQUIRE(!(f & EPI_STATS) || (a->stat_sum && a->stat_sq), "check_gemm: column statistics without buffers");
+
+  PackedB w;
+  w.hi = (__nv_bfloat16*)a->w_hi; w.lo = (__nv_bfloat16*)a->w_lo; w.Npad = a->N; w.nkb = a->nkb_w; w.n_logical = a->n_valid;
+  ProgramBuilder bld{Arena{}, a->B, false, false, nullptr};
+  GemmOp g = bld.gemm_base(w, a->T_out);
+  for (int i = 0; i < a->nsrc; ++i) bld.add_src(g, to_split(a->src[i]));
+  for (int i = 0; i < a->nseg; ++i) {
+    const int* s = a->seg[i];
+    NS_REQUIRE(s[0] >= 0 && s[0] < a->nsrc && s[1] >= 0 && s[2] >= 1, "check_gemm: bad segment %d", i);
+    bld.seg(g, s[0], s[1], s[2], s[3]);
+  }
+  for (int i = 0; i < a->nxs; ++i) {
+    const int* x = a->xseg[i];
+    NS_REQUIRE(x[0] >= 0 && x[0] < a->nsrc && x[1] >= 0 && x[1] % 64 == 0 && x[2] >= 1 && (x[3] == 1 || x[3] == 3),
+               "check_gemm: bad panel segment %d", i);
+    NS_REQUIRE(!x[6] || (x[7] >= 0 && x[7] + nkb_of(x[2]) * 64 <= kXfMaxC), "check_gemm: panel segment %d outside the affine table", i);
+    bld.xseg(g, x[0], x[1], x[2], x[3], x[4], x[5], x[6], x[7]);
+  }
+  NS_REQUIRE(g.nkb_total == a->nkb_w, "check_gemm: the segments cover %d k-blocks, the weights %d", g.nkb_total, a->nkb_w);
+  if (g.xmode) for (int i = 0; i < g.nxs; ++i) for (int j = 0; j < g.xs[i].ntap; ++j)
+    NS_REQUIRE(g.xs[i].kb_tap[j] >= 0 && g.xs[i].kb_tap[j] + g.xs[i].ncb <= a->nkb_w, "check_gemm: panel segment %d tap %d outside the weights", i, j);
+  g.flags = f;
+  g.bias = a->bias; g.rowbias = a->rowbias; g.rowbias_ld = a->rowbias_ld; g.res = a->res; g.res_ld = a->res_ld;
+  g.out = a->out; g.out_ld = a->out_ld;
+  g.out_hi = (__nv_bfloat16*)a->out_hi; g.out_lo = (__nv_bfloat16*)a->out_lo; g.out_split_ld = a->out_split_ld;
+  if (a->f16_col0 >= 0) g.f16_col0 = a->f16_col0;
+  g.ln_stats = a->ln_stats; g.ln_g = a->ln_g; g.ln_C = a->ln_C; g.ln_eps = a->ln_eps;
+  g.row_stats = a->row_stats; g.stat_sum = a->stat_sum; g.stat_sq = a->stat_sq;
+  g.rowmask = a->rowmask; g.row_len = a->row_len; g.len_shift = a->len_shift;
+  g.ksplit = a->ksplit;
+
+  cudaStream_t st = (cudaStream_t)stream;
+  PrepOp* pre_dev = nullptr;
+  if (g.xmode && a->pre_scale) {
+    NS_REQUIRE(a->pre_shift && a->pre_C >= 1 && a->pre_C <= kXfMaxC, "check_gemm: panel affine needs scale, shift and 1..%d channels", kXfMaxC);
+    NS_REQUIRE(a->pre_mode == PREP_AFFINE || a->pre_mode == PREP_AFFINE_SILU, "check_gemm: panel affine mode %d", a->pre_mode);
+    PrepOp p; memset(&p, 0, sizeof(p));
+    p.C1 = a->pre_C; p.B = a->B; p.T_src = a->T_out; p.T_dst = a->T_out; p.mode = a->pre_mode;
+    p.scale = a->pre_scale; p.shift = a->pre_shift;
+    p.row_len = a->row_len; p.len_shift = a->len_shift;
+    NS_CHECK_CUDA(cudaMallocAsync((void**)&pre_dev, sizeof(PrepOp), st));
+    NS_CHECK_CUDA(cudaMemcpyAsync(pre_dev, &p, sizeof(PrepOp), cudaMemcpyHostToDevice, st));
+    g.pre = pre_dev;
+  }
+  plan_gemm(g);
+  int rc = encode_tmaps(g);
+  if (!rc) rc = launch_gemm_tc(g, st);
+  if (pre_dev) NS_CHECK_CUDA(cudaFreeAsync(pre_dev, st));
+  if (rc) return rc;
+  // the template arguments launch_gemm_tc selects for this operator
+  const bool voc = (f & EPI_GELU) != 0, enc = !voc && (f & (EPI_RELU | EPI_ROWMASK));
+  report(desc, desc_len, "gemm_tc<%d,LNF=%d,XF=%d,ENC=%d,RAG=%d,VOC=%d>", g.bn, (f & EPI_LNFOLD) ? 1 : 0, g.xmode ? 1 : 0, enc ? 1 : 0,
+         g.row_len ? 1 : 0, voc ? 1 : 0);
+  return 0;
+}
+
+int ns2vc_check_attention(const ns2vc_check_attn_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a, "check_attention: null argument");
+  NS_REQUIRE(a->B >= 1 && a->H >= 1 && a->dh >= 1, "check_attention: bad sizes B=%d H=%d dh=%d", a->B, a->H, a->dh);
+  NS_REQUIRE(a->out || (a->out_hi && a->out_lo), "check_attention: no output");
+  AttnOp op; memset(&op, 0, sizeof(op));
+  op.B = a->B; op.H = a->H; op.Tq = a->Tq; op.Tk = a->Tk; op.dh = a->dh; op.scale = a->scale;
+  op.bias = a->bias;
+  op.out = a->out; op.out_ld = a->out_ld;
+  op.out_hi = (__nv_bfloat16*)a->out_hi; op.out_lo = (__nv_bfloat16*)a->out_lo; op.out_split_ld = a->out_split_ld;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (a->v2) {
+    NS_REQUIRE(a->qs.hi && a->qs.lo && a->ks.hi && a->ks.lo && a->vs.hi && a->vs.lo, "check_attention: v2 needs split q / k / v");
+    op.v2 = 1;
+    op.qs = to_split(a->qs); op.ks = to_split(a->ks); op.vs = to_split(a->vs);
+    op.q_c0 = a->q_c0; op.k_c0 = a->k_c0; op.v_c0 = a->v_c0;
+    op.key_len = a->key_len; op.key_shift = a->key_shift; op.p_split = a->p_split;
+    int rc = encode_attn_tmaps(op);
+    if (!rc) rc = launch_attention_v2(op, st);
+    if (rc) return rc;
+    const bool pf16 = attention_v2_p_fp16() && !op.p_split;
+    report(desc, desc_len, "attn_v2<%d,PB=%d,BIAS=%d,PF16=%d,RAGK=%d>", op.dh, op.pb, op.bias ? 1 : 0, pf16 ? 1 : 0, op.key_len ? 1 : 0);
+    return 0;
+  }
+  NS_REQUIRE(a->q && a->k && a->v, "check_attention: v1 needs fp32 q / k / v");
+  NS_REQUIRE(!a->key_len, "check_attention: per-entry key counts are a v2 feature");
+  op.q = a->q; op.q_ld = a->q_ld; op.k = a->k; op.k_ld = a->k_ld; op.v = a->v; op.v_ld = a->v_ld;
+  const int rc = launch_attention(op, st, false);
+  if (rc) return rc;
+  const int dhp = a->dh <= 16 ? 16 : a->dh <= 32 ? 32 : a->dh <= 48 ? 48 : 64;
+  report(desc, desc_len, "attn_tc<%d>", dhp);
+  return 0;
+}
+
+}  // extern "C"
