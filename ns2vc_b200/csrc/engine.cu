@@ -37,7 +37,7 @@ struct ResnetSite {
 struct XformerSite {
   std::string p;
   int c;
-  PackedB proj_in, qkv, out1, q2, out2, ff1, ff2, proj_out;
+  PackedB proj_in, qkv, out1, q2, out2, ff1;
   // ff.net.2 and proj_out have no non-linearity between them (reference attention.py:203 -> transformer_1d.py:289-295):
   //   proj_out(ff2(g) + b2 + h) + bp = g (Wp W2)^T + h Wp^T + (Wp b2 + bp)
   // so both run as ONE GEMM over K = [GEGLU output (4C) | residual stream h (C)] with the product matrix packed at load time.
@@ -98,11 +98,7 @@ struct ns2vc_unet : EngineBase {
     static_bufs.clear();
   }
   bool profiling = false;
-  bool ksplit = true;        // split-K pairs for few-tile panel-mode launches (NS2VC_KSPLIT=0: one CTA per tile)
-  bool xf = true;            // GroupNorm(+FiLM)(+SiLU) of the conv / proj_in inputs applied inside the GEMM (panel mode; NS2VC_XF=0: prep launches)
-  bool merge_ff = true;      // ff.net.2 + proj_out as one GEMM (NS2VC_MERGE_FF=0: two launches)
   const float* film_ext = nullptr;   // caller-supplied FiLM rows for one forward (replace the active program's film_base)
-  bool lnfold = true;        // LayerNorms of the transformer folded into their consumer GEMMs (NS2VC_LNFOLD=0: separate LN kernels)
   unsigned long long* trace = nullptr; int trace_cap = 0;
   unsigned long long* attn_trace = nullptr; int attn_trace_cap = 0;
   unsigned long long* span = nullptr; int span_cap = 0;   // [launch][2] grid spans
@@ -311,32 +307,25 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       if ((rc = pack_named(h, x.proj_in, x.p + ".proj_in.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
       if ((rc = h->mem.alloc_packed(x.qkv, 3 * C, 3 * C, nk, h->simt))) return rc;
       const char* qkvn[3] = {".attn1.to_q.weight", ".attn1.to_k.weight", ".attn1.to_v.weight"};
-      const bool fold = h->lnfold;
       for (int i = 0; i < 3; ++i)
-        if ((rc = pack_named(h, x.qkv, b + qkvn[i], C, C, 1, 0, 0, C, i * C, 0, 0, st, fold ? h->weights.W(b + ".norm1.weight") : nullptr))) return rc;
-      if (fold) {
-        if (!(x.g_qkv = h->mem.alloc<float>((size_t)3 * C)) || !(x.bf_qkv = h->mem.alloc<float>((size_t)3 * C))) return -2;
-        if (!(x.g_q2 = h->mem.alloc<float>((size_t)C)) || !(x.bf_q2 = h->mem.alloc<float>((size_t)C))) return -2;
-        if (!(x.g_ff1 = h->mem.alloc<float>((size_t)8 * C)) || !(x.bf_ff1 = h->mem.alloc<float>((size_t)8 * C))) return -2;
-        for (int i = 0; i < 3; ++i)
-          if ((rc = ln_fold_vectors(h, b + qkvn[i], "", b + ".norm1", C, C, x.g_qkv, x.bf_qkv, i * C, st))) return rc;
-        if ((rc = ln_fold_vectors(h, b + ".attn2.to_q.weight", "", b + ".norm2", C, C, x.g_q2, x.bf_q2, 0, st))) return rc;
-        if ((rc = ln_fold_vectors(h, b + ".ff.net.0.proj.weight", b + ".ff.net.0.proj.bias", b + ".norm3", 8 * C, C, x.g_ff1, x.bf_ff1, 0, st))) return rc;
-      }
+        if ((rc = pack_named(h, x.qkv, b + qkvn[i], C, C, 1, 0, 0, C, i * C, 0, 0, st, h->weights.W(b + ".norm1.weight")))) return rc;
+      if (!(x.g_qkv = h->mem.alloc<float>((size_t)3 * C)) || !(x.bf_qkv = h->mem.alloc<float>((size_t)3 * C))) return -2;
+      if (!(x.g_q2 = h->mem.alloc<float>((size_t)C)) || !(x.bf_q2 = h->mem.alloc<float>((size_t)C))) return -2;
+      if (!(x.g_ff1 = h->mem.alloc<float>((size_t)8 * C)) || !(x.bf_ff1 = h->mem.alloc<float>((size_t)8 * C))) return -2;
+      for (int i = 0; i < 3; ++i)
+        if ((rc = ln_fold_vectors(h, b + qkvn[i], "", b + ".norm1", C, C, x.g_qkv, x.bf_qkv, i * C, st))) return rc;
+      if ((rc = ln_fold_vectors(h, b + ".attn2.to_q.weight", "", b + ".norm2", C, C, x.g_q2, x.bf_q2, 0, st))) return rc;
+      if ((rc = ln_fold_vectors(h, b + ".ff.net.0.proj.weight", b + ".ff.net.0.proj.bias", b + ".norm3", 8 * C, C, x.g_ff1, x.bf_ff1, 0, st))) return rc;
       if ((rc = h->mem.alloc_packed(x.out1, C, C, nk, h->simt))) return rc;
       if ((rc = pack_named(h, x.out1, b + ".attn1.to_out.0.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
       if ((rc = h->mem.alloc_packed(x.q2, C, C, nk, h->simt))) return rc;
-      if ((rc = pack_named(h, x.q2, b + ".attn2.to_q.weight", C, C, 1, 0, 0, C, 0, 0, 0, st, fold ? h->weights.W(b + ".norm2.weight") : nullptr))) return rc;
+      if ((rc = pack_named(h, x.q2, b + ".attn2.to_q.weight", C, C, 1, 0, 0, C, 0, 0, 0, st, h->weights.W(b + ".norm2.weight")))) return rc;
       if ((rc = h->mem.alloc_packed(x.out2, C, C, nk, h->simt))) return rc;
       if ((rc = pack_named(h, x.out2, b + ".attn2.to_out.0.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
       NS_REQUIRE((4 * C) % 64 == 0, "transformer width %d: 4C must be a multiple of 64", C);
       if ((rc = h->mem.alloc_packed(x.ff1, 4 * C, 8 * C, nk, h->simt))) return rc;
-      if ((rc = pack_named(h, x.ff1, b + ".ff.net.0.proj.weight", 8 * C, C, 1, 0, 0, C, 0, 0, 4 * C, st, fold ? h->weights.W(b + ".norm3.weight") : nullptr))) return rc;
-      if ((rc = h->mem.alloc_packed(x.ff2, C, C, nkb_of(4 * C), h->simt))) return rc;
-      if ((rc = pack_named(h, x.ff2, b + ".ff.net.2.weight", C, 4 * C, 1, 0, 0, 4 * C, 0, 0, 0, st))) return rc;
-      if ((rc = h->mem.alloc_packed(x.proj_out, C, C, nk, h->simt))) return rc;
-      if ((rc = pack_named(h, x.proj_out, x.p + ".proj_out.weight", C, C, 1, 0, 0, C, 0, 0, 0, st))) return rc;
-      if (h->merge_ff && fold) {
+      if ((rc = pack_named(h, x.ff1, b + ".ff.net.0.proj.weight", 8 * C, C, 1, 0, 0, C, 0, 0, 4 * C, st, h->weights.W(b + ".norm3.weight")))) return rc;
+      {
         // proj_out o ff.net.2 as one operator: K blocks [Wp W2 over the 4C GEGLU channels | Wp over the C residual channels]
         const float* Wp = h->weights.W(x.p + ".proj_out.weight"); const float* W2 = h->weights.W(b + ".ff.net.2.weight");
         NS_REQUIRE(Wp && W2, "pack: %s feed-forward / proj_out weights missing", x.p.c_str());
@@ -414,7 +403,7 @@ struct Builder : ProgramBuilder {
     for (int j = 0; j < 3; ++j) seg(g, i, 0, s.C, j - 1);
   }
   void emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
-    if (g.xmode && h->ksplit) {
+    if (g.xmode) {
       // few-tile, deep-K launches (the two coarsest levels at B = 8: 64 tiles of 24-64 k-blocks each): two CTAs per tile, each
       // half of the channel blocks; worth it when both halves still have a few panels and all pairs are resident at once
       const int tiles = B * ceil_div(g.T_out, 128) * (w.Npad / 64);
@@ -472,6 +461,24 @@ struct Builder : ProgramBuilder {
     p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / p.gn.G));
   }
 };
+
+// The timestep path over M rows of timesteps `t` as small linears into temb1, emb [M, ted] and film [M, film_total]; returns their
+// number (the FiLM projection only when some resnet has one).  Reference embeddings.py:24-64, 157-218 (sinusoid -> linear_1 ->
+// SiLU -> linear_2), unet_1d_condition.py:869-883 (+ aug_emb: row m adds row m % B of `aug`), resnet.py:619-629 (time_emb_proj
+// of SiLU(emb) for every resnet at once).
+int time_path_ops(const ns2vc_unet* h, const float* t, int M, int B, const float* aug, float* temb1, float* emb, float* film, LinOp ops[3]) {
+  const ns2vc_unet_cfg& c = h->cfg;
+  const int ted = h->ted;
+  ops[0] = linear_op(t, 1, M, c.block_out_channels[0], h->weights.W("time_embedding.linear_1.weight"), h->weights.W("time_embedding.linear_1.bias"),
+                     ted, temb1, ted);
+  ops[0].in_mode = LIN_SINUSOID; ops[0].flip_sin_to_cos = c.flip_sin_to_cos; ops[0].freq_shift = c.freq_shift; ops[0].out_silu = 1;
+  ops[1] = linear_op(temb1, ted, M, ted, h->weights.W("time_embedding.linear_2.weight"), h->weights.W("time_embedding.linear_2.bias"), ted, emb, ted);
+  if (c.add_embed_text) { ops[1].add = aug; ops[1].add_ld = ted; ops[1].add_rows = B; }
+  if (h->film_total <= 0) return 2;
+  ops[2] = linear_op(emb, ted, M, ted, h->film_W, h->film_b, h->film_total, film, h->film_total);
+  ops[2].in_mode = LIN_SILU;
+  return 3;
+}
 
 // Builds the programs of (B, T, S, ragged, ws) into *prog, or (ws == nullptr) sizes their workspace into *bytes_out.
 // A ragged program takes no more workspace than the padded one: its tables live in the program's static buffer.
@@ -592,7 +599,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   for (auto& o : h->plan) {
     if (o.kind == PlanOp::RESNET) stat_doubles += (size_t)4 * B * o.cout;
     else if (o.kind == PlanOp::XFORMER || o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) stat_doubles += (size_t)2 * B * o.cout;
-    if (o.kind == PlanOp::XFORMER && h->lnfold) stat_doubles += (size_t)3 * 2 * B * Tl[o.level];   // three LayerNorm row-statistics buffers
+    if (o.kind == PlanOp::XFORMER) stat_doubles += (size_t)3 * 2 * B * Tl[o.level];   // three LayerNorm row-statistics buffers
   }
   double* stat_arena = ar.get<double>(stat_doubles);
   size_t stat_used = 0;
@@ -617,8 +624,8 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   auto scratch_split = [&](size_t elems) { SplitBuf s{}; s.hi = ar.get<__nv_bfloat16>(elems); s.lo = ar.get<__nv_bfloat16>(elems); return s; };
   const SplitBuf SP_A = scratch_split(max_cat);      // conv1 / resample input
   const SplitBuf SP_R = scratch_split(max_cat);      // raw shortcut operand / odd rows of a stride-2 conv
-  const SplitBuf SP_H = scratch_split(max_act);      // conv2 input, ff2 output, out-head input
-  const SplitBuf SP_X = scratch_split(max_act);      // GN / LN normalised transformer activations
+  const SplitBuf SP_H = scratch_split(max_act);      // conv2 input, out-head input
+  const SplitBuf SP_X = scratch_split(max_act);      // GN-normalised transformer input (when the GroupNorm is a prep launch)
   const SplitBuf SP_ATT = scratch_split(max_act);    // attention output
   const SplitBuf SP_FF = scratch_split(max_ff);      // GEGLU output
   const SplitBuf SP_QKV = scratch_split(max_qkv);    // q | k | v of the self-attention (q of the cross-attention)
@@ -626,22 +633,16 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
 
   // entry: x -> split tokens, time path, conv_in
   { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::X; l.i0 = Cl; l.i1 = T; l.split = s_xin; l.lens = lens; bld.out->push_back(l); }
-  { LinOp o = linear_op(nullptr, 1, B, c0, h->weights.W("time_embedding.linear_1.weight"), h->weights.W("time_embedding.linear_1.bias"), ted, temb1, ted);
-    o.in_mode = LIN_SINUSOID; o.flip_sin_to_cos = c.flip_sin_to_cos; o.freq_shift = c.freq_shift; o.out_silu = 1;
-    bld.emit_linear(o, Launch::T, 1); }
-  { LinOp o = linear_op(temb1, ted, B, ted, h->weights.W("time_embedding.linear_2.weight"), h->weights.W("time_embedding.linear_2.bias"), ted, emb, ted);
-    if (c.add_embed_text) { o.add = aug; o.add_ld = ted; }
-    bld.emit_linear(o, Launch::NONE, 1); }
-  if (h->film_total > 0) {
-    LinOp o = linear_op(emb, ted, B, ted, h->film_W, h->film_b, h->film_total, film, h->film_total);
-    o.in_mode = LIN_SILU;
-    bld.emit_linear(o, Launch::NONE, 1);
+  {
+    LinOp tp[3];
+    const int n = time_path_ops(h, nullptr, B, B, aug, temb1, emb, film, tp);
+    for (int i = 0; i < n; ++i) bld.emit_linear(tp[i], i == 0 ? Launch::T : Launch::NONE, 1);
   }
 
   // An activation that leaves a block: fp32 token-major tensor, its raw bf16 hi/lo split (the A operand of the panel-mode
   // GEMMs that consume it; written by the same epilogue) and the per-(b, channel) sums for the consumer's GroupNorm.
   struct Act { float* p = nullptr; SplitBuf sp{}; int c = 0; double* st = nullptr; };
-  const bool xf_on = h->xf && !h->simt;
+  const bool xf_on = !h->simt;
   SplitBuf rot_sp[3];
   for (int i = 0; i < 3; ++i) rot_sp[i] = xf_on ? scratch_split(max_act) : SplitBuf{};
   std::vector<Act> skips;
@@ -769,23 +770,16 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
         const XformerSite& x = h->xformers[xi++];
         const int C = x.c, H = c.num_heads, dh = C / H;
         const std::string b = x.p + ".transformer_blocks.0";
-        const SplitBuf sx = Builder::view(SP_X, TL, C), satt = Builder::view(SP_ATT, TL, C), sff = Builder::view(SP_FF, TL, 4 * C),
-                       sh2 = Builder::view(SP_H, TL, C);
+        const SplitBuf sx = Builder::view(SP_X, TL, C), satt = Builder::view(SP_ATT, TL, C), sff = Builder::view(SP_FF, TL, 4 * C);
         const bool xin = xf_ok(C, 0);                        // GroupNorm(eps 1e-6) of the block input applied inside proj_in
         if (!xin) {
           bld.emit_prep_gn(cur.p, C, cur.st, nullptr, 0, nullptr, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), nullptr, 0, sx);
           rag_prep(lens, o.level);
         }
-        // Folded LayerNorms: the producer of each LN input also emits its raw bf16 split and the per-row sums; the consumer
-        // GEMM runs on the raw split with gamma folded into its weights and applies mean / rstd in its epilogue:
-        //   LN(x) W^T = rstd * (x (gamma*W)^T - mean * g) + (beta W^T + bias),   g[n] = sum_c gamma_c W[n,c]
-        // (reference attention.py:83,102,118 nn.LayerNorm eps 1e-5) - no LayerNorm kernel, no extra pass over the rows.
-        const bool fold = h->lnfold;
+        // Folded LayerNorms (reference attention.py:83,102,118 nn.LayerNorm): proj_in, out1 and out2 each emit the raw split of
+        // the residual stream into `sln` and its per-row sums; qkv, q2 and ff1 read `sln` - no LayerNorm kernel, no extra pass.
         const SplitBuf sln = Builder::view(SP_LN, TL, C);
-        double* rs1 = fold ? new_rowstats(rows) : nullptr; double* rs2 = fold ? new_rowstats(rows) : nullptr; double* rs3 = fold ? new_rowstats(rows) : nullptr;
-        auto emits_ln_input = [&](GemmOp& g, double* rs) { g.flags |= EPI_OUT_SPLIT | EPI_ROWSTATS; g.out_hi = sln.hi; g.out_lo = sln.lo; g.out_split_ld = sln.ld; g.row_stats = rs; };
-        auto consumes_ln = [&](GemmOp& g, const double* rs, const float* gv, const float* bf) {
-          g.flags |= EPI_LNFOLD | EPI_BIAS; g.ln_stats = rs; g.ln_g = gv; g.bias = bf; g.ln_C = C; g.ln_eps = 1e-5f; };
+        double* rs1 = new_rowstats(rows); double* rs2 = new_rowstats(rows); double* rs3 = new_rowstats(rows);
         { GemmOp g = xin ? bld.gemm_base(x.proj_in, TL) : bld.lin(x.proj_in, sx, TL);
           if (xin) {
             const int i0 = bld.add_src(g, cur.sp);
@@ -793,18 +787,16 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
             g.pre = bld.affine_desc(cur.st, C, nullptr, 0, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), 0, o.level);
           }
           g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(x.p + ".proj_in.bias"); g.out = T0; g.out_ld = C;
-          if (fold) emits_ln_input(g, rs1);
+          bld.emits_ln_input(g, sln, rs1);
           rag(g, o.level);
           bld.emit_gemm(g, x.proj_in); }
-        if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->weights.W(b + ".norm1.weight"), h->weights.W(b + ".norm1.bias"), sx);
-        const SplitBuf& sn = fold ? sln : sx;                // A operand of the LayerNorm consumers
         const bool av2 = !h->simt && attention_v2_supported(dh, TL, false) && attention_v2_supported(dh, S, true);
         const SplitBuf sqkv = Builder::view(SP_QKV, TL, 3 * C), sq2 = Builder::view(SP_QKV, TL, C);
-        { GemmOp g = bld.lin(x.qkv, sn, TL);
+        { GemmOp g = bld.lin(x.qkv, sln, TL);
           if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sqkv.hi; g.out_lo = sqkv.lo; g.out_split_ld = sqkv.ld;
                      if (p16(TL)) g.f16_col0 = 2 * C; }
           else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = 3 * C; }
-          if (fold) consumes_ln(g, rs1, x.g_qkv, x.bf_qkv);
+          bld.consumes_ln(g, rs1, x.g_qkv, x.bf_qkv, C);
           bld.emit_gemm(g, x.qkv); }
         { AttnOp a; memset(&a, 0, sizeof(a));
           a.q = QKV; a.q_ld = 3 * C; a.k = QKV + C; a.k_ld = 3 * C; a.v = QKV + 2 * C; a.v_ld = 3 * C;
@@ -816,13 +808,12 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           if (av2) { a.v2 = 1; a.p_split = p16(TL) ? 0 : 1; a.qs = sqkv; a.ks = sqkv; a.vs = sqkv; a.q_c0 = 0; a.k_c0 = C; a.v_c0 = 2 * C; }
           bld.emit_attention(a); }
         { GemmOp g = bld.lin(x.out1, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn1.to_out.0.bias"); g.res = T0; g.res_ld = C; g.out = T1; g.out_ld = C;
-          if (fold) emits_ln_input(g, rs2);
+          bld.emits_ln_input(g, sln, rs2);
           bld.emit_gemm(g, x.out1); }
-        if (!fold) bld.emit_ln_split(T1, C, (int)rows, C, h->weights.W(b + ".norm2.weight"), h->weights.W(b + ".norm2.bias"), sx);
-        { GemmOp g = bld.lin(x.q2, sn, TL);
+        { GemmOp g = bld.lin(x.q2, sln, TL);
           if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sq2.hi; g.out_lo = sq2.lo; g.out_split_ld = sq2.ld; }
           else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = C; }
-          if (fold) consumes_ln(g, rs2, x.g_q2, x.bf_q2);
+          bld.consumes_ln(g, rs2, x.g_q2, x.bf_q2, C);
           bld.emit_gemm(g, x.q2); }
         { AttnOp a; memset(&a, 0, sizeof(a));
           a.q = QKV; a.q_ld = C; a.k = kvc + x.kv_off; a.k_ld = h->kv_total; a.v = kvc + x.v_off; a.v_ld = h->kv_total; a.bias = maskbias;
@@ -832,28 +823,20 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
           if (ragged) { a.bias = pg.rt.prompt_bias; bld.emit_attention(a); }   // the prompt-length bias of the ragged tables
           else bld.emit_attention(a, Launch::MASK); }     // the key-padding bias comes from the call's mask (dropped without one)
         { GemmOp g = bld.lin(x.out2, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn2.to_out.0.bias"); g.res = T1; g.res_ld = C; g.out = T0; g.out_ld = C;
-          if (fold) emits_ln_input(g, rs3);
+          bld.emits_ln_input(g, sln, rs3);
           bld.emit_gemm(g, x.out2); }
-        if (!fold) bld.emit_ln_split(T0, C, (int)rows, C, h->weights.W(b + ".norm3.weight"), h->weights.W(b + ".norm3.bias"), sx);
-        { GemmOp g = bld.lin(x.ff1, sn, TL); g.flags = EPI_GEGLU | EPI_OUT_SPLIT; g.bias = h->weights.W(b + ".ff.net.0.proj.bias");
+        { GemmOp g = bld.lin(x.ff1, sln, TL); g.flags = EPI_GEGLU | EPI_OUT_SPLIT;
           g.out_hi = sff.hi; g.out_lo = sff.lo; g.out_split_ld = sff.ld;
-          if (fold) { consumes_ln(g, rs3, x.g_ff1, x.bf_ff1); g.flags &= ~EPI_BIAS; }   // GEGLU reads its (folded) biases through g.bias itself
+          bld.consumes_ln(g, rs3, x.g_ff1, x.bf_ff1, C); g.flags &= ~EPI_BIAS;   // GEGLU reads its (folded) biases through g.bias itself
           bld.emit_gemm(g, x.ff1); }
         Act outp = next_out(followed_by_push(pi), TL, C);
         outp.st = new_stats(C);
-        if (h->merge_ff && fold) {
-          // ff.net.2 + proj_out as one GEMM over K = [GEGLU output | residual stream]:  out = g (Wp W2)^T + h Wp^T + (Wp b2 + bp) + x_in
+        { // ff.net.2 + proj_out as one GEMM over K = [GEGLU output | residual stream]:  out = g (Wp W2)^T + h Wp^T + (Wp b2 + bp) + x_in
           GemmOp g = bld.gemm_base(x.ff2p, TL);
           const int i0 = bld.add_src(g, sff); bld.seg(g, i0, 0, 4 * C, 0);
           const int i1 = bld.add_src(g, sln); bld.seg(g, i1, 0, C, 0);          // raw split of the residual stream, written by out2's epilogue
           g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = x.bias_ff2p; g.res = cur.p; g.res_ld = C;
-          emits_block_out(g, outp); with_stats(g, outp.st, C); rag(g, o.level); bld.emit_gemm(g, x.ff2p);
-        } else {
-          { GemmOp g = bld.lin(x.ff2, sff, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_SPLIT; g.bias = h->weights.W(b + ".ff.net.2.bias"); g.res = T0; g.res_ld = C;
-            g.out_hi = sh2.hi; g.out_lo = sh2.lo; g.out_split_ld = sh2.ld; bld.emit_gemm(g, x.ff2); }
-          { GemmOp g = bld.lin(x.proj_out, sh2, TL); g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = h->weights.W(x.p + ".proj_out.bias"); g.res = cur.p; g.res_ld = C;
-            emits_block_out(g, outp); with_stats(g, outp.st, C); rag(g, o.level); bld.emit_gemm(g, x.proj_out); }
-        }
+          emits_block_out(g, outp); with_stats(g, outp.st, C); rag(g, o.level); bld.emit_gemm(g, x.ff2p); }
         cur = outp;
         bld.emit_tap(pg.taps, x.p, cur.p, o.level, C, TL);
         break;
@@ -1115,10 +1098,6 @@ int ns2vc_unet_create(const ns2vc_unet_cfg* cfg, ns2vc_unet** out) {
   h->ted = 4 * cfg->block_out_channels[0];
   const char* be = getenv("NS2VC_GEMM_BACKEND");
   h->simt = be && strcmp(be, "simt") == 0;
-  { const char* e = getenv("NS2VC_LNFOLD"); h->lnfold = !(e && e[0] == '0'); }
-  { const char* e = getenv("NS2VC_XF"); h->xf = !(e && e[0] == '0'); }
-  { const char* e = getenv("NS2VC_KSPLIT"); h->ksplit = !(e && e[0] == '0'); }
-  { const char* e = getenv("NS2VC_MERGE_FF"); h->merge_ff = !(e && e[0] == '0'); }
   build_plan(h);
   register_weights(h);
   *out = h;
@@ -1197,27 +1176,13 @@ int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float*
   if (rc) return rc;
   const Program& pg = h->progs[h->active];
   NS_REQUIRE(pg.cond_ready || !h->cfg.add_embed_text, "ns2vc_unet_prepare_cond() must precede ns2vc_unet_time_table() (the pooled prompt embedding is added to every row)");
-  const ns2vc_unet_cfg& c = h->cfg;
-  const int ted = h->ted, c0 = c.block_out_channels[0];
   float* film = table;
   float* temb1 = table + (size_t)n_rows * std::max(h->film_total, 1);
-  float* emb = temb1 + (size_t)n_rows * ted;
-  cudaStream_t st = (cudaStream_t)stream;
-  // reference embeddings.py:24-64, 157-218 (sinusoid -> linear_1 -> SiLU -> linear_2), unet_1d_condition.py:869-883 (+ aug_emb),
-  // resnet.py:619-629 (time_emb_proj of SiLU(emb) for all 22 resnets at once)
-  { LinOp o; memset(&o, 0, sizeof(o));
-    o.x = t_rows; o.x_ld = 1; o.M = n_rows; o.K = c0; o.W = h->weights.W("time_embedding.linear_1.weight"); o.bias = h->weights.W("time_embedding.linear_1.bias");
-    o.N = ted; o.out = temb1; o.out_ld = ted; o.in_mode = LIN_SINUSOID; o.flip_sin_to_cos = c.flip_sin_to_cos; o.freq_shift = c.freq_shift; o.out_silu = 1;
-    if ((rc = launch_small_linear(o, st))) return rc; }
-  { LinOp o; memset(&o, 0, sizeof(o));
-    o.x = temb1; o.x_ld = ted; o.M = n_rows; o.K = ted; o.W = h->weights.W("time_embedding.linear_2.weight"); o.bias = h->weights.W("time_embedding.linear_2.bias");
-    o.N = ted; o.out = emb; o.out_ld = ted; if (c.add_embed_text) { o.add = pg.aug; o.add_ld = ted; o.add_rows = B; }
-    if ((rc = launch_small_linear(o, st))) return rc; }
-  if (h->film_total > 0) {
-    LinOp o; memset(&o, 0, sizeof(o));
-    o.x = emb; o.x_ld = ted; o.M = n_rows; o.K = ted; o.W = h->film_W; o.bias = h->film_b; o.N = h->film_total; o.out = film; o.out_ld = h->film_total; o.in_mode = LIN_SILU;
-    if ((rc = launch_small_linear(o, st))) return rc;
-  }
+  float* emb = temb1 + (size_t)n_rows * h->ted;
+  LinOp tp[3];
+  const int n = time_path_ops(h, t_rows, n_rows, B, pg.aug, temb1, emb, film, tp);
+  for (int i = 0; i < n; ++i)
+    if ((rc = launch_small_linear(tp[i], (cudaStream_t)stream))) return rc;
   return 0;
 }
 

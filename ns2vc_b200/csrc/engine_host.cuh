@@ -248,6 +248,16 @@ struct ProgramBuilder {
     seg(g, add_src(g, in), 0, in.C, 0);
     return g;
   }
+  // ---- LayerNorm (eps 1e-5) folded into its consumer GEMM (EPI_LNFOLD):
+  //   LN(x) W^T = rstd * (x (gamma*W)^T - mean * g) + (beta W^T + bias),   g[n] = sum_c gamma_c W[n,c]
+  // The producer of x also writes its raw split `s` and the per-row sums `rs`; the consumer runs on `s` with gamma packed into
+  // its weights and applies mean / rstd over the C channels with the load-time vectors `gv` = g and `bf` = beta W^T + bias.
+  static void emits_ln_input(GemmOp& g, const SplitBuf& s, double* rs) {
+    g.flags |= EPI_OUT_SPLIT | EPI_ROWSTATS; g.out_hi = s.hi; g.out_lo = s.lo; g.out_split_ld = s.ld; g.row_stats = rs;
+  }
+  static void consumes_ln(GemmOp& g, const double* rs, const float* gv, const float* bf, int C) {
+    g.flags |= EPI_LNFOLD | EPI_BIAS; g.ln_stats = rs; g.ln_g = gv; g.bias = bf; g.ln_C = C; g.ln_eps = 1e-5f;
+  }
   Launch& emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
     Launch l; l.kind = Launch::GEMM; l.input = in;
     if (!dry) {

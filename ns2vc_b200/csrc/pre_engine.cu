@@ -183,9 +183,6 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
   const SplitBuf s_in = bld.split(Tn, e.cin), s_ln = bld.split(Tn, H), s_qkv = bld.split(Tn, 3 * H), s_att = bld.split(Tn, H),
                  s_y = bld.split(Tn, H), s_ff = bld.split(Tn, F);
   auto new_rowstats = [&]() { double* p = stat_cur; if (stat_cur) stat_cur += 2 * M; return p; };
-  auto emits_ln_input = [&](GemmOp& g, double* rs) { g.flags |= EPI_OUT_SPLIT | EPI_ROWSTATS; g.out_hi = s_ln.hi; g.out_lo = s_ln.lo; g.out_split_ld = s_ln.ld; g.row_stats = rs; };
-  auto consumes_ln = [&](GemmOp& g, const double* rs, const float* gv, const float* bf) {
-    g.flags |= EPI_LNFOLD | EPI_BIAS; g.ln_stats = rs; g.ln_g = gv; g.bias = bf; g.ln_C = H; g.ln_eps = 1e-5f; };
   auto masked = [&](GemmOp& g) { g.flags |= EPI_ROWMASK; g.rowmask = keep; };
 
   { Launch l; l.kind = Launch::SEQMASK; l.input = io.lengths; l.i0 = Tn; l.o = keep; l.o2 = kbias; l.mem = ilens; bld.out->push_back(l); }
@@ -194,7 +191,7 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
   double* rs = new_rowstats();
   { GemmOp g = bld.lin(e.pre, s_in, Tn);
     g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = w.W(e.p + ".pre.conv.bias"); g.out = XA; g.out_ld = H;
-    masked(g); emits_ln_input(g, rs);
+    masked(g); bld.emits_ln_input(g, s_ln, rs);
     bld.emit_gemm(g, e.pre); }
   bld.emit_tap(taps, e.p + ".pre", XA, Tn, H, Tn);
   const bool av2 = !h->simt && attention_v2_supported(dh, Tn, true);
@@ -204,7 +201,7 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
     { GemmOp g = bld.lin(ls.qkv, s_ln, Tn);
       if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = s_qkv.hi; g.out_lo = s_qkv.lo; g.out_split_ld = s_qkv.ld; }   // (V stays a bf16 split: p_split below)
       else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = 3 * H; }
-      consumes_ln(g, rs, ls.g_qkv, ls.bf_qkv);
+      bld.consumes_ln(g, rs, ls.g_qkv, ls.bf_qkv, H);
       bld.emit_gemm(g, ls.qkv); }
     { AttnOp a; memset(&a, 0, sizeof(a));
       a.q = QKV; a.q_ld = 3 * H; a.k = QKV + H; a.k_ld = 3 * H; a.v = QKV + 2 * H; a.v_ld = 3 * H; a.bias = kbias;
@@ -229,13 +226,13 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
     rs = new_rowstats();
     { GemmOp g = bld.lin(ls.ffn2, s_ff, Tn);
       g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = w.W(b + ".ffn.ffn_2.bias"); g.res = XB; g.res_ld = H; g.out = XA; g.out_ld = H;
-      masked(g); emits_ln_input(g, rs);
+      masked(g); bld.emits_ln_input(g, s_ln, rs);
       bld.emit_gemm(g, ls.ffn2); }
     bld.emit_tap(taps, e.p + ".layers." + std::to_string(i), XA, Tn, H, Tn);
   }
   { GemmOp g = bld.lin(e.outp, s_ln, Tn);
     g.flags = EPI_OUT_F32; g.out = OUTP; g.out_ld = e.cout;
-    consumes_ln(g, rs, e.g_out, e.bf_out);
+    bld.consumes_ln(g, rs, e.g_out, e.bf_out, H);
     bld.emit_gemm(g, e.outp); }
   { Launch l; l.kind = Launch::LN_MASK; l.input = io.out; l.a = OUTP; l.i0 = e.cout; l.i1 = (int)M; l.i2 = e.cout; l.f0 = 1e-5f;
     l.b = w.W(e.p + ".layer_norm.weight"); l.c = w.W(e.p + ".layer_norm.bias"); l.d = keep; bld.out->push_back(l); }

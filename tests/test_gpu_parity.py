@@ -551,8 +551,7 @@ def test_forward_with_large_gain_weights_and_offset_activations(gain, offset):
 
 
 # ------------------------------------------------------------------ every documented switch keeps parity
-@pytest.mark.parametrize("env", ["NS2VC_XF=0", "NS2VC_KSPLIT=0", "NS2VC_MERGE_FF=0", "NS2VC_LNFOLD=0", "NS2VC_ATTN_P=split",
-                                 "NS2VC_PDL=0", "NS2VC_GRAPH=0"])
+@pytest.mark.parametrize("env", ["NS2VC_ATTN_P=split", "NS2VC_PDL=0", "NS2VC_GRAPH=0"])
 def test_diagnostic_switches_keep_parity(env):
     """The environment switches of README.md (A/B paths and numerical fallbacks) are read once per process / engine, so each one is
     exercised in a child process on the per-op tap test, the reference full-config fixture and the tiny sampler fixtures."""
