@@ -230,10 +230,16 @@ int launch_ln_fold_vec(const float* W, const float* gamma, const float* beta, co
 
 int launch_prep_split(const PrepOp& op, cudaStream_t st);
 
-// LayerNorm + split in one pass (one warp per row): out = ((x-mean)*rstd*gamma + beta) as bf16 hi/lo; rows with keep[row] == 0
-// store zeros when `keep` is given
-int launch_ln_split(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta,
-                    SplitBuf out, cudaStream_t st, unsigned long long* span = nullptr, const float* keep = nullptr);
+// LayerNorm (eps) of M rows of C channels (row pitch ld), one warp per row
+struct LnOp {
+  const float* x; int ld, M, C; float eps;
+  const float* gamma; const float* beta;
+  const float* keep;           // [M] row keep factors or nullptr: ln_split stores zeros where keep == 0, ln_mask multiplies by keep
+  float* y; int y_ld;          // ln_apply / ln_mask: fp32 output
+  SplitBuf split;              // ln_split: bf16 hi/lo output
+};
+// LayerNorm + split in one pass: split = ((x-mean)*rstd*gamma + beta) as bf16 hi/lo
+int launch_ln_split(const LnOp& op, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------
 // Attention
@@ -280,20 +286,25 @@ int encode_tmap_any(TMap* out, const void* base, int elem_bytes, int C, int T, i
 // ---------------------------------------------------------------------------------------------
 // Norm statistics and small kernels (kernels_misc.cu)
 // ---------------------------------------------------------------------------------------------
-int launch_ln_stats(const float* x, int ld, int M, int C, float eps, float* stats /*[M,2]*/, cudaStream_t st);
-int launch_ln_apply(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta,
-                    float* y, int y_ld, cudaStream_t st);
+// y = (x-mean)*rstd*gamma + beta
+int launch_ln_apply(const LnOp& op, cudaStream_t st);
 
-// [B, C, T] (batch stride bstride) -> token-major [B, T, ldo] (channels >= C zero-filled up to Cpad)
-int launch_nct_to_tokens(const float* x, long long bstride, int B, int C, int T, float* out, int ldo, int Cpad,
-                         cudaStream_t st);
+// [B, C, T] fp32 (batch stride bstride) -> token-major fp32 [B, T, ld], channels >= C zero-filled up to ld
+struct TokensOp {
+  const float* x; long long bstride; int B, C, T;
+  float* out; int ld;
+  const float* rowbias;        // enc_input: + rowbias[b, c], or nullptr
+  const float* keep;           // enc_input: [B, T] rows with keep == 0 are stored as zeros
+};
+int launch_nct_to_tokens(const TokensOp& op, cudaStream_t st);
 // [B, C, T] fp32 -> split token-major [B, T, out.ld] (channels >= C zero-filled up to out.ld)
-// warm / warm_bytes: optional region prefetched into L2 by the same launch (the step's FiLM rows)
-// row_len: per-entry valid frames [B] (ragged programs): frames past them are written as zeros
-int launch_nct_to_split(const float* x, long long bstride, int B, int C, int T, SplitBuf out, cudaStream_t st, const void* warm = nullptr,
-                        long long warm_bytes = 0, const int* row_len = nullptr);
-// token-major [B, T, ld] -> [B, C, T]
-int launch_tokens_to_nct(const float* x, int ld, int B, int C, int T, float* out, cudaStream_t st);
+struct NctSplitOp {
+  const float* x; long long bstride; int B, C, T;
+  SplitBuf out;
+  const int* row_len;          // per-entry valid frames [B] (ragged programs): frames past them are written as zeros; or nullptr
+  const void* warm; long long warm_bytes;   // optional region prefetched into L2 by the same launch (the step's FiLM rows)
+};
+int launch_nct_to_split(const NctSplitOp& op, cudaStream_t st);
 
 enum LinIn : int { LIN_RAW = 0, LIN_SILU = 1, LIN_SINUSOID = 2 };
 // Small-M linear: out[m, n] = f(x[m, :]) . W[n, :] + bias[n] (+ add[m, n]);  W row-major [N, K].
@@ -312,11 +323,21 @@ int launch_small_linear(const LinOp& op, cudaStream_t st);
 
 // AttentionPooling pieces (reference embeddings.py:499-546)
 // lens: per-entry prompt lengths [B] (ragged programs: pool over the first lens[b] frames only), or nullptr (all S)
-int launch_pool_class_token(const float* xn /*[B,S,C] LN'd*/, const float* pos /*[C]*/, int B, int S, int C,
-                            float* tokens /*[B,S+1,C]: row0 = class token, rows 1.. = xn*/, cudaStream_t st, const int* lens = nullptr);
-int launch_pool_attend(const float* q /*[B,C]*/, const float* kv /*[B,S+1,2C] k|v*/, int B, int S1, int C, int heads,
-                       float* out /*[B,C]*/, cudaStream_t st, const int* lens = nullptr);
-int launch_mask_bias(const uint8_t* mask, int n, float* bias, cudaStream_t st);
+struct PoolClsOp {
+  const float* x; const float* pos; int B, S, C;   // x: [B, S, C] LayerNorm'd, pos: [C]
+  float* tokens;                                   // [B, S+1, C]: row 0 = class token, rows 1.. = x
+  const int* lens;
+};
+int launch_pool_class_token(const PoolClsOp& op, cudaStream_t st);
+// POOL_ATT (launch_pool_attend: head width <= 16) and POOL_ATT_WIDE (launch_pool_attend_wide: any head width)
+struct PoolAttOp {
+  const float* q; const float* kv; int B, S1, C, heads;   // q: [B, C], kv: [B, S1, 2C] k | v
+  float* out;                                             // [B, C]
+  const int* lens;
+};
+int launch_pool_attend(const PoolAttOp& op, cudaStream_t st);
+struct MaskBiasOp { const uint8_t* mask; int n; float* bias; };
+int launch_mask_bias(const MaskBiasOp& op, cudaStream_t st);
 
 // Ragged programs: per-utterance lengths -> the device tables the program reads (written by ns2vc_unet_prepare_cond_ragged).
 constexpr int kRagMaxLevels = 8;
@@ -377,12 +398,16 @@ int launch_ddim_step(const float* x, const float* x0, const float* noise, const 
 // ---------------------------------------------------------------------------------------------
 // Condition encoders (pre_kernels.cu; program in pre_engine.cu)
 // ---------------------------------------------------------------------------------------------
-int launch_seq_mask(const long long* len, int B, int T, float* keep, float* kbias, cudaStream_t st, int* ilen = nullptr);
-int launch_enc_input(const float* x, long long bstride, const float* rowbias, const float* keep, int B, int C, int T, float* out, int ld,
-                     cudaStream_t st);
-int launch_ln_mask(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta, const float* keep, float* y, int y_ld,
-                   cudaStream_t st);
-int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st, const int* lens = nullptr);
+struct SeqMaskOp {
+  const long long* len; int B, T;
+  float* keep; float* kbias;   // [B, T]
+  int* ilen;                   // the lengths as int [B], clamped to [1, T], or nullptr
+};
+int launch_seq_mask(const SeqMaskOp& op, cudaStream_t st);
+int launch_enc_input(const TokensOp& op, cudaStream_t st);
+// y = LayerNorm(x) * keep
+int launch_ln_mask(const LnOp& op, cudaStream_t st);
+int launch_pool_attend_wide(const PoolAttOp& op, cudaStream_t st);
 int launch_tbc_weight(const float* w, int k, int cin, int cout, float* o, cudaStream_t st);
 int launch_ffn_taps(const float* const* w, int k, int F, int H, int centre, float scale, float* o, cudaStream_t st);
 int launch_scale_vec(const float* a, float s, float* o, int n, cudaStream_t st);
@@ -390,8 +415,13 @@ int launch_scale_vec(const float* a, float s, float* o, int n, cudaStream_t st);
 // LayerNorm (eps) of token-major [B, T, C] rows (vocoder.cu's voc_norm_kernel; C a multiple of 128 up to 1024), optionally after
 // a 7-tap depthwise conv (dw: [C][8] taps and bias).  Rows at or past len[b] (int64 [B], clamped into [1, T]; nullptr: T) read
 // and store 0.  Outputs: fp32 `out` and / or the bf16 hi/lo `split`.
-int launch_voc_norm(const float* x, int B, int T, int C, const float* dw, const float* gamma, const float* beta, float eps, const long long* len,
-                    float* out, const SplitBuf& split, cudaStream_t st);
+struct VocNormOp {
+  const float* x; int B, T, C;
+  const float* dw; const float* gamma; const float* beta; float eps;
+  const long long* len;
+  float* out; SplitBuf split;
+};
+int launch_voc_norm(const VocNormOp& op, cudaStream_t st);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

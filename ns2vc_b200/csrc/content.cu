@@ -269,15 +269,10 @@ struct ns2vc_cv : SingleProgramEngine {
   std::vector<PackedB> pos;                                 // per positional-conv group
   std::vector<PackedB> qkv, out, fc1, fc2;
   std::vector<float*> qkv_b;
-  // what the cached program adds to the shared one
-  std::vector<SplitBuf> tap_split;                          // per tap: the split it converts (hi == nullptr: an fp32 tap)
-  std::vector<int> tap_rows;                                // per split tap: rows per entry of the split
-  LenTables lt{};                                           // the program's length tables (in its workspace)
+  LenTables lt{};                                           // the cached program's length tables (in its workspace)
 };
 
 namespace {
-
-enum CvKind { CV_LENS = 100, CV_GN_STATS, CV_CONV0, CV_NORM, CV_POS_WIN, CV_ADD, CV_SPLIT_TAP, CV_OUT };
 
 std::string layer(int i) { return "encoder.layers." + std::to_string(i); }
 std::string conv_key(int l) { return "feature_extractor.conv_layers." + std::to_string(l); }
@@ -386,8 +381,6 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
   const int T = Tl[kLevels - 1];
   std::vector<Launch> prog;
   TapSet taps;
-  std::vector<SplitBuf> tap_split;
-  std::vector<int> tap_rows;
   ProgramBuilder bld{Arena{(uint8_t*)ws, 0}, B, dry, false, &prog};
   Arena& ar = bld.ar;
   const WeightRegistry& w = h->weights;
@@ -416,27 +409,20 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
   __nv_bfloat16* win_hi = ar.get<__nv_bfloat16>(win_elems);
   __nv_bfloat16* win_lo = ar.get<__nv_bfloat16>(win_elems);
 
-  auto tap_f32 = [&](const std::string& name, const float* src, int C) {
-    if (dry) return;
-    bld.emit_tap(taps, name, src, T, C, T);
-    tap_split.push_back(SplitBuf{}); tap_rows.push_back(0);
-  };
+  auto tap_f32 = [&](const std::string& name, const float* src, int C) { bld.emit_tap(taps, name, src, T, C, T); };
   auto tap_split_of = [&](const std::string& name, const SplitBuf& s, int rws, int Tn) {
     if (dry) return;
-    Launch l; l.kind = (Launch::Kind)CV_SPLIT_TAP; l.tap_index = taps.add(name, Tn, C0); l.i0 = rws; l.i1 = Tn;
-    prog.push_back(l);
-    tap_split.push_back(s); tap_rows.push_back(rws);
+    bld.emit(Launch::CV_SPLIT_TAP, SplitTapOp{s, B, rws, Tn, C0}).tap_index = taps.add(name, Tn, C0);
   };
   auto norm = [&](const float* in, const std::string& ln, int C, float* out, const SplitBuf& split) {
-    Launch l; l.kind = (Launch::Kind)CV_NORM; l.a = in; l.b = w.W(ln + ".weight"); l.c = w.W(ln + ".bias"); l.f0 = 1e-5f;
-    l.i0 = T; l.i1 = C; l.o = out; l.split = split;
-    prog.push_back(l);
+    bld.emit(Launch::VOC_NORM, VocNormOp{in, B, T, C, nullptr, w.W(ln + ".weight"), w.W(ln + ".bias"), 1e-5f, lt.frames64, out, split});
   };
   auto rowmask = [&](GemmOp& g, int l) { g.flags |= EPI_ROWMASK; g.rowmask = lt.keep[l]; };
 
-  { Launch l; l.kind = (Launch::Kind)CV_LENS; prog.push_back(l); }
-  { Launch l; l.kind = (Launch::Kind)CV_GN_STATS; l.o = reinterpret_cast<float*>(gn); prog.push_back(l); }
-  { Launch l; l.kind = (Launch::Kind)CV_CONV0; l.i0 = rows[0]; l.a = reinterpret_cast<const float*>(gn); l.split = lv_even; prog.push_back(l); }
+  const float* w0 = w.W(conv_key(0) + ".0.weight");
+  bld.emit(Launch::CV_LENS, CvLensOp{B, N});
+  bld.emit(Launch::CV_GN_STATS, CvGnStatsOp{B, N, C0, w0, 1e-5f, gn});
+  bld.emit(Launch::CV_CONV0, CvConv0Op{B, N, rows[0], w0, gn, w.W(conv_key(0) + ".2.weight"), w.W(conv_key(0) + ".2.bias"), lv_even});
   tap_split_of(conv_key(0), lv_even, rows[0], Tl[0]);
   for (int l = 1; l < kLevels; ++l) {
     SplitBuf in = (l & 1) ? lv_even : lv_odd;                // level l - 1
@@ -461,8 +447,7 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
     rowmask(g, kLevels - 1);
     bld.emit_gemm(g, h->proj); }
   tap_f32("post_extract_proj", Fp, D);
-  { Launch l; l.kind = (Launch::Kind)CV_POS_WIN; l.a = Fp; l.i0 = T; l.i1 = D; l.i2 = G; l.i3 = gw; l.f0 = 0;
-    l.split = SplitBuf{win_hi, win_lo, Tw, kWinTaps * 64, kWinTaps * 64, 0}; prog.push_back(l); }
+  bld.emit(Launch::CV_POS_WIN, CvPosWinOp{Fp, B, T, D, G, gw, K, lt.frames64, SplitBuf{win_hi, win_lo, Tw, kWinTaps * 64, kWinTaps * 64, 0}});
   for (int g_ = 0; g_ < G; ++g_) {
     SplitBuf win{win_hi + (size_t)g_ * Tw * kWinTaps * 64, win_lo + (size_t)g_ * Tw * kWinTaps * 64, Tw, kWinTaps * 64, kWinTaps * 64,
                  (long long)G * Tw * kWinTaps * 64};
@@ -473,7 +458,7 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
     rowmask(g, kLevels - 1);
     bld.emit_gemm(g, h->pos[g_]);
   }
-  { Launch l; l.kind = (Launch::Kind)CV_ADD; l.o = P; l.a = Fp; l.mem_bytes = M * D * sizeof(float); prog.push_back(l); }
+  bld.emit(Launch::CV_ADD, CvAddOp{P, Fp, (long long)(M * D / 4)});
   tap_f32("encoder.pos_conv", P, D);
   norm(P, "encoder.layer_norm", D, X, s_x);
   tap_f32("encoder.layer_norm", X, D);
@@ -508,14 +493,12 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
     rowmask(g, kLevels - 1);
     bld.emit_gemm(g, h->fin); }
   tap_f32("final_proj", U, c.final_dim);
-  { Launch l; l.kind = (Launch::Kind)CV_OUT; l.input = Launch::OUT; l.a = U; l.mem_bytes = M * c.final_dim * sizeof(float); prog.push_back(l); }
+  bld.emit(Launch::COPY, CopyOp{U, M * c.final_dim * sizeof(float), nullptr}, Launch::OUT);
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
     h->cp.prog = std::move(prog);
     h->cp.taps = std::move(taps);
-    h->tap_split = std::move(tap_split);
-    h->tap_rows = std::move(tap_rows);
     h->lt = lt;
   }
   return 0;
@@ -531,42 +514,46 @@ int launch_check(cudaError_t e, const char* what) {
 }
 
 int run_program(ns2vc_cv* h, const float* wav, long long bstride, const long long* lengths, float* units, long long* frames_out, cudaStream_t st) {
-  const int B = h->cp.dims[0], N = h->cp.dims[1];
-  const ns2vc_cv_cfg& c = h->cfg;
-  const int C0 = c.conv_dim;
-  const WeightRegistry& w = h->weights;
-  const LenTables& lt = h->lt;
-  return run_cached(h, false, st, [&](const Launch& l) {
-    switch ((int)l.kind) {
-      case CV_LENS:
-        return launch_check(launch_k(cv_lengths_kernel, dim3(ceil_div(B * lt.rows[1], 256)), dim3(256), 0, st, lengths, B, N, lt, frames_out), "cv_lengths");
-      case CV_GN_STATS:
-        return launch_check(launch_k(cv_gn_stats_kernel, dim3(C0 / kStatCh, B), dim3(kStatCh * kStatLanes), 0, st, wav, bstride, lengths, N,
-                                     w.W(conv_key(0) + ".0.weight"), 1e-5f, C0, reinterpret_cast<float2*>(l.o)), "cv_gn_stats");
-      case CV_CONV0:
-        return launch_check(launch_k(cv_conv0_kernel, dim3(ceil_div(l.i0, kConv0Frames), B), dim3(C0 / 2), 0, st, wav, bstride, lengths, N, l.i0,
-                                     w.W(conv_key(0) + ".0.weight"), reinterpret_cast<const float2*>(l.a), w.W(conv_key(0) + ".2.weight"),
-                                     w.W(conv_key(0) + ".2.bias"), l.split), "cv_conv0");
-      case CV_NORM: return launch_voc_norm(l.a, B, l.i0, l.i1, nullptr, l.b, l.c, l.f0, lt.frames64, l.o, l.split, st);
-      case CV_POS_WIN:
-        return launch_check(launch_k(cv_pos_windows_kernel, dim3(l.split.T, l.i2, B), dim3(kWinTaps * 64 / 8), 0, st, l.a, l.i0, l.i1, l.i2, l.i3,
-                                     c.pos_conv_kernel, (const long long*)lt.frames64, l.split.hi, l.split.lo), "cv_pos_windows");
-      case CV_ADD: {
-        const long long n4 = (long long)(l.mem_bytes / sizeof(float4));
-        return launch_check(launch_k(cv_add_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(l.o),
-                                     reinterpret_cast<const float4*>(l.a), n4), "cv_add");
+  CallArgs in{};
+  in[Launch::OUT] = {units};
+  return run_cached(h, false, in, st, [&](const Launch& l) {
+    switch (l.kind) {
+      case Launch::CV_LENS: {
+        const CvLensOp& o = l.get<CvLensOp>();
+        const LenTables& lt = h->lt;
+        return launch_check(launch_k(cv_lengths_kernel, dim3(ceil_div(o.B * lt.rows[1], 256)), dim3(256), 0, st, lengths, o.B, o.N, lt, frames_out), "cv_lengths");
       }
-      case CV_SPLIT_TAP: {
+      case Launch::CV_GN_STATS: {
+        const CvGnStatsOp& o = l.get<CvGnStatsOp>();
+        return launch_check(launch_k(cv_gn_stats_kernel, dim3(o.C0 / kStatCh, o.B), dim3(kStatCh * kStatLanes), 0, st, wav, bstride, lengths, o.N,
+                                     o.w0, o.eps, o.C0, o.stats), "cv_gn_stats");
+      }
+      case Launch::CV_CONV0: {
+        const CvConv0Op& o = l.get<CvConv0Op>();
+        return launch_check(launch_k(cv_conv0_kernel, dim3(ceil_div(o.rows, kConv0Frames), o.B), dim3(o.out.C / 2), 0, st, wav, bstride, lengths, o.N,
+                                     o.rows, o.w0, o.stats, o.gamma, o.beta, o.out), "cv_conv0");
+      }
+      case Launch::CV_POS_WIN: {
+        const CvPosWinOp& o = l.get<CvPosWinOp>();
+        return launch_check(launch_k(cv_pos_windows_kernel, dim3(o.win.T, o.G, o.B), dim3(kWinTaps * 64 / 8), 0, st, o.x, o.T, o.D, o.G, o.gw, o.K,
+                                     o.frames, o.win.hi, o.win.lo), "cv_pos_windows");
+      }
+      case Launch::CV_ADD: {
+        const CvAddOp& o = l.get<CvAddOp>();
+        return launch_check(launch_k(cv_add_kernel, dim3((unsigned)((o.n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(o.p),
+                                     reinterpret_cast<const float4*>(o.x), o.n4), "cv_add");
+      }
+      case Launch::CV_SPLIT_TAP: {
         float* dst = h->cp.taps.dst[l.tap_index];
         if (dst) {
-          const long long n = (long long)B * l.i1 * C0;
-          cv_split_tap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(h->tap_split[l.tap_index], l.i0, l.i1, C0, dst, n);
+          const SplitTapOp& o = l.get<SplitTapOp>();
+          const long long n = (long long)o.B * o.T * o.C;
+          cv_split_tap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(o.s, o.rows, o.T, o.C, dst, n);
           NS_CV_LAUNCH_CHECK();
         }
         return 0;
       }
-      case CV_OUT: NS_CHECK_CUDA(cudaMemcpyAsync(units, l.a, l.mem_bytes, cudaMemcpyDeviceToDevice, st)); return 0;
-      default: return kSharedKind;
+      default: return no_launcher(l);
     }
   });
 }

@@ -441,19 +441,18 @@ struct Builder : ProgramBuilder {
   void emit_prep(const float* s1, int C1, const float* s2, int C2, int T_src, int T_dst, int mode, const float* scale,
                  const float* shift, const SplitBuf& o, const SplitBuf* raw = nullptr, int row_mul = 1, int row_add = 0,
                  const int* rowmap = nullptr, Launch::Input in = Launch::NONE) {
-    Launch l; l.kind = Launch::PREP; l.input = in;
-    PrepOp& p = l.prep; memset(&p, 0, sizeof(p));
+    PrepOp p; memset(&p, 0, sizeof(p));
     p.src1 = s1; p.ld1 = C1; p.C1 = C1; p.src2 = s2; p.ld2 = C2; p.C2 = C2; p.B = B; p.T_src = T_src; p.T_dst = T_dst;
     p.row_mul = row_mul; p.row_add = row_add; p.rowmap = rowmap; p.mode = mode; p.scale = scale; p.shift = shift; p.out = o;
     if (raw) p.raw = *raw;
-    out->push_back(l);
+    emit(Launch::PREP, p, in);
   }
   // GroupNorm(+FiLM)(+SiLU) prep whose statistics come from the producers' epilogues
   void emit_prep_gn(const float* s1, int C1, const double* st1, const float* s2, int C2, const double* st2, int Tn, int mode,
                     float eps, const float* gamma, const float* beta, const float* film, int film_ld, const SplitBuf& o,
                     const SplitBuf* raw = nullptr) {
     emit_prep(s1, C1, s2, C2, Tn, Tn, mode, nullptr, nullptr, o, raw);
-    PrepOp& p = out->back().prep;
+    PrepOp& p = out->back().get<PrepOp>();
     if (film) out->back().reads_film = 1;
     p.gn.sum1 = st1; p.gn.sq1 = st1 ? st1 + (size_t)B * C1 : nullptr;
     p.gn.sum2 = st2; p.gn.sq2 = st2 ? st2 + (size_t)B * C2 : nullptr;
@@ -538,7 +537,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   const int* lens = pg.rt.lens;
   const int* plens = lens ? lens + B : nullptr;
   auto rag = [&](GemmOp& g, int level) { g.row_len = lens; g.len_shift = level; };
-  auto rag_prep = [&](const int* len, int level) { PrepOp& p = bld.out->back().prep; p.row_len = len; p.len_shift = level; };
+  auto rag_prep = [&](const int* len, int level) { PrepOp& p = bld.out->back().get<PrepOp>(); p.row_len = len; p.len_shift = level; };
 
   // ---- persistent conditioning buffers
   float* P = (Cc > 0) ? ar.get<float>((size_t)B * T * c0) : nullptr;      // conv_in(content) + bias
@@ -568,13 +567,13 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
 
   // ================= conditioning program =================
   if (Cc > 0) {
-    { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::CONTENT; l.i0 = Cc; l.i1 = T; l.split = s_content; l.lens = lens; bld.out->push_back(l); }
+    bld.emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, Cc, T, s_content, lens, nullptr, 0}, Launch::CONTENT);
     GemmOp g = bld.gemm_base(h->convin_content, T);
     bld.conv3(g, s_content);
     g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W("conv_in.bias"); g.out = P; g.out_ld = c0;
     bld.emit_gemm(g, h->convin_content);
   }
-  { Launch l; l.kind = Launch::MASKBIAS; l.input = Launch::MASK; l.i0 = B * S; l.o = maskbias; bld.out->push_back(l); }
+  bld.emit(Launch::MASKBIAS, MaskBiasOp{nullptr, B * S, maskbias}, Launch::MASK);
   if (h->kv_total > 0) {
     bld.emit_prep(nullptr, xd, nullptr, 0, S, S, PREP_RAW, nullptr, nullptr, s_prompt, nullptr, 1, 0, nullptr, Launch::PROMPT);
     rag_prep(plens, 0);                                    // (ragged: prompt frames past S_b are zeros, so is their K / V)
@@ -632,7 +631,7 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   const SplitBuf SP_LN = scratch_split(max_act);     // raw (un-normalised) split of the transformer's residual stream (folded LayerNorms)
 
   // entry: x -> split tokens, time path, conv_in
-  { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::X; l.i0 = Cl; l.i1 = T; l.split = s_xin; l.lens = lens; bld.out->push_back(l); }
+  bld.emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, Cl, T, s_xin, lens, nullptr, 0}, Launch::X);
   {
     LinOp tp[3];
     const int n = time_path_ops(h, nullptr, B, B, aug, temb1, emb, film, tp);
@@ -927,82 +926,68 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
   return 0;
 }
 
-int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& prog, const float* x, long long x_bstride, const float* t,
-                float* out, const float* content, long long content_bstride, const float* prompt, const uint8_t* mask, cudaStream_t st) {
+// Runs `prog` over the call arguments `in`.  Before Runner launches a record, the denoiser's own patches go into a copy of it:
+// the FiLM rows of ns2vc_unet_forward_film, the cross-attention without a mask, and the span / trace / profiling diagnostics.
+int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& prog, const CallArgs& in, cudaStream_t st) {
   int rc = 0, count = 0, gemm_idx = 0, attn_idx = 0;
   // Precomputed FiLM rows (ns2vc_unet_time_table): the timestep path of this forward is skipped and every reader is rebased.
   const float* film_ext = h->film_ext;
   auto rebase = [&](const float* p) { return (film_ext && p) ? film_ext + (p - pg.film_base) : p; };
-  const Runner run{h->simt, pg.B, &pg.taps, st};
-  for (const Launch& l : prog) {
-    if (film_ext && l.time_path) continue;
+  const Runner run{h->simt, &pg.taps, st};
+  Launch tmp;
+  for (const Launch& rec : prog) {
+    if (film_ext && rec.time_path) continue;
     cudaEvent_t ev_a = nullptr, ev_b = nullptr;
-    const bool prof = h->profiling && l.kind != Launch::TAP;
+    const bool prof = h->profiling && rec.kind != Launch::TAP;
     if (prof) {
       cudaEventCreate(&ev_a); cudaEventCreate(&ev_b);
       cudaEventRecord(ev_a, st);
     }
     unsigned long long* span = (h->span && count < h->span_cap) ? h->span + 2 * count : nullptr;
-    switch (l.kind) {
-      case Launch::GEMM: {
-        const bool to_out = l.input == Launch::OUT;
-        if (to_out || h->trace || h->span || (film_ext && l.reads_film)) {
-          GemmOp g = l.gemm;
-          if (to_out) g.out = out;
-          if (film_ext && l.reads_film) {
-            g.rowbias = rebase(g.rowbias);
-            g.pre_film = rebase(g.pre_film);
-          }
-          if (span) g.span = span;
-          if (h->trace && gemm_idx < h->trace_cap) g.trace = h->trace + 32 * gemm_idx;
-          ++gemm_idx;
-          rc = run.gemm(g);
-        } else {
-          rc = run.gemm(l.gemm);
+    const Launch* l = bound(rec, in, tmp, rc);
+    auto patched = [&]() { if (l != &tmp) { tmp = rec; l = &tmp; } return &tmp; };
+    bool skip = false;
+    switch (rec.kind) {
+      case Launch::GEMM:
+        if (film_ext && rec.reads_film) {
+          GemmOp& g = patched()->get<GemmOp>();
+          g.rowbias = rebase(g.rowbias);
+          g.pre_film = rebase(g.pre_film);
         }
+        if (span) patched()->get<GemmOp>().span = span;
+        if (h->trace && gemm_idx < h->trace_cap) patched()->get<GemmOp>().trace = h->trace + 32 * gemm_idx;
+        ++gemm_idx;
         break;
-      }
-      case Launch::ATTN: {
-        AttnOp a = l.attn;
-        if (l.input == Launch::MASK && !pg.has_mask) a.bias = nullptr;
-        if (span) a.span = span;
-        if (h->attn_trace && attn_idx < h->attn_trace_cap) a.trace = h->attn_trace + 2048 * attn_idx;
+      case Launch::ATTN:
+        if (rec.input == Launch::MASK && !pg.has_mask) patched()->get<AttnOp>().bias = nullptr;
+        if (span) patched()->get<AttnOp>().span = span;
+        if (h->attn_trace && attn_idx < h->attn_trace_cap) patched()->get<AttnOp>().trace = h->attn_trace + 2048 * attn_idx;
         ++attn_idx;
-        rc = run.attn(a);
         break;
-      }
-      case Launch::NCT2SPLIT: {
-        const bool fwd = l.input == Launch::X;
-        const bool warm = fwd && film_ext != nullptr;
-        rc = launch_nct_to_split(fwd ? x : content, fwd ? x_bstride : content_bstride, pg.B, l.i0, l.i1, l.split, st, warm ? film_ext : nullptr,
-                                 warm ? (long long)pg.B * h->film_total * 4 : 0, l.lens);
+      case Launch::PREP:
+        if (film_ext && rec.reads_film) { PrepOp& p = patched()->get<PrepOp>(); p.gn.film = rebase(p.gn.film); }
+        if (span) patched()->get<PrepOp>().span = span;
         break;
-      }
-      case Launch::PREP: {
-        PrepOp p = l.prep;
-        if (l.input == Launch::PROMPT) p.src1 = prompt;
-        if (film_ext && l.reads_film) p.gn.film = rebase(p.gn.film);
-        if (span) p.span = span;
-        rc = launch_prep_split(p, st);
+      case Launch::NCT2SPLIT:   // the forward's first launch: it warms the step's FiLM rows into L2
+        if (film_ext && rec.input == Launch::X) { NctSplitOp& o = patched()->get<NctSplitOp>(); o.warm = film_ext; o.warm_bytes = (long long)pg.B * h->film_total * 4; }
         break;
-      }
-      case Launch::POOL_ATT: rc = launch_pool_attend(l.a, l.b, pg.B, l.i0, l.i1, l.i2, l.o, st, l.lens); break;
-      case Launch::MASKBIAS:
-        if (mask) rc = launch_mask_bias(mask, l.i0, l.o, st); else --count;
-        break;
-      case Launch::TAP: --count; rc = run.run(l); break;
-      default: rc = run.run(l, l.input == Launch::PROMPT ? prompt : l.input == Launch::T ? t : nullptr, span); break;
+      case Launch::MASKBIAS: skip = !in[Launch::MASK].p; break;   // no mask: the cross-attention runs without the bias
+      default: break;
+    }
+    if (!rc && !skip) {
+      rc = run.run(*l);
+      if (rc == kEngineKind) rc = no_launcher(rec);
     }
     if (prof) {
       cudaEventRecord(ev_b, st);
-      ns2vc_unet::ProfRec pr{(int)l.kind, ev_a, ev_b, 0, 0, 0, 0, 0};
-      if (l.kind == Launch::GEMM) { pr.M = l.gemm.B * l.gemm.T_out; pr.N = l.gemm.n_valid; pr.K = l.gemm.nkb_total * 64; pr.nseg = l.gemm.nseg; }
-      if (l.kind == Launch::PREP) { pr.M = l.prep.B * l.prep.T_dst; pr.N = l.prep.C1 + l.prep.C2; }
-      if (l.kind == Launch::ATTN) { pr.M = l.attn.Tq; pr.N = l.attn.Tk; pr.K = l.attn.dh; }
+      ns2vc_unet::ProfRec pr{(int)rec.kind, ev_a, ev_b, 0, 0, 0, 0, 0};
+      if (rec.kind == Launch::GEMM) { const GemmOp& g = rec.get<GemmOp>(); pr.M = g.B * g.T_out; pr.N = g.n_valid; pr.K = g.nkb_total * 64; pr.nseg = g.nseg; }
+      if (rec.kind == Launch::PREP) { const PrepOp& p = rec.get<PrepOp>(); pr.M = p.B * p.T_dst; pr.N = p.C1 + p.C2; }
+      if (rec.kind == Launch::ATTN) { const AttnOp& a = rec.get<AttnOp>(); pr.M = a.Tq; pr.N = a.Tk; pr.K = a.dh; }
       h->prof.push_back(pr);
     }
     if (rc) return rc;
-    ++count;
+    if (rec.tap_index < 0 && !skip) ++count;
   }
   h->last_launches = count;
   return 0;
@@ -1127,7 +1112,9 @@ int ns2vc_unet_prepare_cond(ns2vc_unet* h, const float* content, long long conte
   NS_REQUIRE(Cc == 0 || content != nullptr, "content is NULL but the model has %d content channels", Cc);
   Program& pg = h->progs[h->active];
   pg.has_mask = mask != nullptr;
-  rc = run_program(h, pg, pg.prog_cond, nullptr, 0, nullptr, nullptr, content, content_bstride, prompt, mask, (cudaStream_t)stream);
+  CallArgs in{};
+  in[Launch::CONTENT] = {content, content_bstride}; in[Launch::PROMPT] = {prompt}; in[Launch::MASK] = {mask};
+  rc = run_program(h, pg, pg.prog_cond, in, (cudaStream_t)stream);
   if (rc) return rc;
   pg.cond_ready = true;
   return 0;
@@ -1146,7 +1133,9 @@ int ns2vc_unet_prepare_cond_ragged(ns2vc_unet* h, const float* content, long lon
   rc = launch_ragged_tables(reinterpret_cast<const long long*>(content_lengths), reinterpret_cast<const long long*>(prompt_lengths), pg.rt,
                             (cudaStream_t)stream);
   if (rc) return rc;
-  rc = run_program(h, pg, pg.prog_cond, nullptr, 0, nullptr, nullptr, content, content_bstride, prompt, nullptr, (cudaStream_t)stream);
+  CallArgs in{};
+  in[Launch::CONTENT] = {content, content_bstride}; in[Launch::PROMPT] = {prompt};
+  rc = run_program(h, pg, pg.prog_cond, in, (cudaStream_t)stream);
   if (rc) return rc;
   pg.cond_ready = true;
   return 0;
@@ -1159,7 +1148,9 @@ int ns2vc_unet_forward(ns2vc_unet* h, const float* x, long long x_bstride, const
   if (rc0) return rc0;
   const Program& pg = h->progs[h->active];
   NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond%s() must be called with the same (B,T,S,workspace) before forward", pg.ragged ? "_ragged" : "");
-  return run_program(h, pg, pg.prog_fwd, x, x_bstride, t, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
+  CallArgs in{};
+  in[Launch::X] = {x, x_bstride}; in[Launch::T] = {t}; in[Launch::OUT] = {out};
+  return run_program(h, pg, pg.prog_fwd, in, (cudaStream_t)stream);
 }
 
 int ns2vc_unet_film_width(const ns2vc_unet* h) { return h ? h->film_total : -1; }
@@ -1195,7 +1186,9 @@ int ns2vc_unet_forward_film(ns2vc_unet* h, const float* x, long long x_bstride, 
   NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond%s() must be called with the same (B,T,S,workspace) before forward", pg.ragged ? "_ragged" : "");
   NS_REQUIRE(h->film_total > 0, "the model has no FiLM rows");
   h->film_ext = film_rows;
-  const int rc = run_program(h, pg, pg.prog_fwd, x, x_bstride, nullptr, out, nullptr, 0, nullptr, nullptr, (cudaStream_t)stream);
+  CallArgs in{};
+  in[Launch::X] = {x, x_bstride}; in[Launch::OUT] = {out};
+  const int rc = run_program(h, pg, pg.prog_fwd, in, (cudaStream_t)stream);
   h->film_ext = nullptr;
   return rc;
 }
@@ -1241,7 +1234,7 @@ int ns2vc_ddim_step(const float* x, const float* x0, const float* noise, const n
 
 int ns2vc_mask_bias(const uint8_t* mask, int n, float* bias, ns2vc_stream stream) {
   NS_REQUIRE(mask && bias && n >= 0, "bad argument");
-  return launch_mask_bias(mask, n, bias, (cudaStream_t)stream);
+  return launch_mask_bias(MaskBiasOp{mask, n, bias}, (cudaStream_t)stream);
 }
 
 int ns2vc_unet_num_taps(const ns2vc_unet* h) { return h ? (h->active >= 0 ? h->progs[h->active].taps.size() : 0) : -1; }

@@ -6,9 +6,11 @@
 #include "common.cuh"
 
 #include <algorithm>
+#include <array>
 #include <cstring>
 #include <string>
 #include <unordered_map>
+#include <variant>
 #include <vector>
 
 namespace ns2vc {
@@ -141,34 +143,67 @@ inline int concat_pool_kv(DeviceMem& mem, const WeightRegistry& w, const std::st
   return 0;
 }
 
-// One launch of a per-shape program.
+// The arguments of the launch kinds that run without a launcher of common.cuh: two copies, and the kernels private to
+// vocoder.cu and content.cu (whose hooks pass them the call arguments they read)
+struct MemsetOp { void* p; size_t bytes; };
+struct CopyOp { const float* src; size_t bytes; float* dst; };   // TAP: dst is the tap's buffer (TapSet); COPY: the call's output
+struct VocLensOp { int B, T; int* lens; float* keep; };          // lengths -> lens [B] and keep [B, T]
+struct IstftOp { const float* h; int ld, B, T; };                // head output [B, T, ld] -> audio
+struct CvLensOp { int B, N; };                                   // lengths -> the content encoder's length tables
+struct CvGnStatsOp { int B, N, C0; const float* w0; float eps; float2* stats; };
+struct CvConv0Op { int B, N, rows; const float* w0; const float2* stats; const float* gamma; const float* beta; SplitBuf out; };
+struct CvPosWinOp { const float* x; int B, T, D, G, gw, K; const long long* frames; SplitBuf win; };
+struct CvAddOp { float* p; const float* x; long long n4; };     // p += x over n4 float4
+struct SplitTapOp { SplitBuf s; int B, rows, T, C; };            // tap of a split [B, rows, s.ld]: its first T rows, C channels
+
+// One launch of a per-shape program: its kind and that kind's arguments.
 struct Launch {
   // The denoiser's kinds keep their numbers: ns2vc_unet_launch_kind() and ns2vc_profile_kind_name() expose them.  The
-  // condition encoders' own kinds follow TAP, the vocoder's follow theirs.
+  // condition encoders' own kinds follow TAP, then the vocoder's, then the content encoder's.
   enum Kind { GEMM, ATTN, LN_SPLIT, LN_APPLY, LINEAR, NCT2SPLIT, POOL_CLS, POOL_ATT, MASKBIAS, PREP, MEMSET, TAP,
               SEQMASK, ENC_INPUT, LN_MASK, NCT2TOK, POOL_ATT_WIDE,
-              VOC_LENS, VOC_NORM, VOC_ISTFT } kind;
-  // The call argument a launch reads or writes instead of a program buffer; each engine resolves them in its run_program.
+              VOC_LENS, VOC_NORM, VOC_ISTFT,
+              COPY, CV_LENS, CV_GN_STATS, CV_CONV0, CV_POS_WIN, CV_ADD, CV_SPLIT_TAP } kind = GEMM;
+  // The call argument a launch reads or writes instead of a program buffer (bind_input puts it into the payload)
   enum Input { NONE,
                X, T, OUT, CONTENT, PROMPT, MASK,                               // ns2vc_unet_prepare_cond / _forward
                C, REFER, LENGTHS, REFER_LENGTHS, CONTENT_OUT, PROMPT_OUT,      // ns2vc_pre_infer
-               MEL, AUDIO                                                     // ns2vc_voc_decode
+               MEL,                                                           // ns2vc_voc_decode (+ LENGTHS)
+               NUM_INPUTS                                                     // (ns2vc_cv_extract: OUT)
   } input = NONE;
-  GemmOp gemm;
-  AttnOp attn;
-  LinOp lin;
-  PrepOp prep;
-  SplitBuf split;
-  // generic small args
-  const float* a = nullptr; const float* b = nullptr; const float* c = nullptr; const float* d = nullptr;
-  float* o = nullptr; float* o2 = nullptr;
-  int i0 = 0, i1 = 0, i2 = 0, i3 = 0; float f0 = 0;
-  void* mem = nullptr; size_t mem_bytes = 0;
+  std::variant<std::monostate, GemmOp, AttnOp, LnOp, LinOp, NctSplitOp, TokensOp, PoolClsOp, PoolAttOp, MaskBiasOp, PrepOp, SeqMaskOp,
+               VocNormOp, MemsetOp, CopyOp, VocLensOp, IstftOp, CvLensOp, CvGnStatsOp, CvConv0Op, CvPosWinOp, CvAddOp, SplitTapOp> op;
   int tap_index = -1;
   int reads_film = 0;        // denoiser: reads the FiLM rows (pointers are rebased when the caller supplies precomputed rows)
   int time_path = 0;         // denoiser: timestep path (sinusoid -> MLP -> FiLM rows): skipped when the caller supplies precomputed FiLM rows
-  const int* lens = nullptr; // denoiser's ragged programs: per-entry lengths [B] of NCT2SPLIT frames / pooled prompt frames
+  template <class Op> Op& get() { return std::get<Op>(op); }
+  template <class Op> const Op& get() const { return std::get<Op>(op); }
 };
+
+// A call argument: its pointer and (the [B, C, T] inputs) its batch stride in elements.  Each C entry point fills the table of
+// the arguments its programs read.
+struct CallArg { const void* p = nullptr; long long bstride = 0; };
+using CallArgs = std::array<CallArg, Launch::NUM_INPUTS>;
+
+// Puts the call argument `a` into the field of l's payload that reads it.
+inline int bind_input(Launch& l, const CallArg& a) {
+  float* p = (float*)a.p;
+  switch (l.kind) {
+    case Launch::GEMM: l.get<GemmOp>().out = p; return 0;
+    case Launch::ATTN: return 0;   // MASK: the denoiser drops the key-padding bias when its prepare_cond had no mask
+    case Launch::LN_APPLY: l.get<LnOp>().x = p; return 0;
+    case Launch::LN_MASK: l.get<LnOp>().y = p; return 0;
+    case Launch::LINEAR: l.get<LinOp>().x = p; return 0;
+    case Launch::PREP: l.get<PrepOp>().src1 = p; return 0;
+    case Launch::NCT2SPLIT: { NctSplitOp& o = l.get<NctSplitOp>(); o.x = p; o.bstride = a.bstride; return 0; }
+    case Launch::ENC_INPUT: case Launch::NCT2TOK: { TokensOp& o = l.get<TokensOp>(); o.x = p; o.bstride = a.bstride; return 0; }
+    case Launch::MASKBIAS: l.get<MaskBiasOp>().mask = (const uint8_t*)a.p; return 0;
+    case Launch::SEQMASK: l.get<SeqMaskOp>().len = (const long long*)a.p; return 0;
+    case Launch::VOC_NORM: l.get<VocNormOp>().len = (const long long*)a.p; return 0;
+    case Launch::COPY: l.get<CopyOp>().dst = p; return 0;
+    default: set_error("internal: launch kind %d reads no call argument", (int)l.kind); return -1;
+  }
+}
 
 // Named activations a program can copy out after the launch that produced them (diagnostics: per-layer parity tests).
 struct TapSet {
@@ -194,7 +229,8 @@ struct TapSet {
   }
   int copy(const Launch& l, cudaStream_t st) const {
     if (l.tap_index >= 0 && l.tap_index < size() && dst[l.tap_index]) {
-      cudaError_t e = cudaMemcpyAsync(dst[l.tap_index], l.a, (size_t)l.i0 * sizeof(float), cudaMemcpyDeviceToDevice, st);
+      const CopyOp& c = l.get<CopyOp>();
+      cudaError_t e = cudaMemcpyAsync(dst[l.tap_index], c.src, c.bytes, cudaMemcpyDeviceToDevice, st);
       if (e != cudaSuccess) { set_error("tap copy failed: %s", cudaGetErrorString(e)); return -2; }
     }
     return 0;
@@ -258,44 +294,40 @@ struct ProgramBuilder {
   static void consumes_ln(GemmOp& g, const double* rs, const float* gv, const float* bf, int C) {
     g.flags |= EPI_LNFOLD | EPI_BIAS; g.ln_stats = rs; g.ln_g = gv; g.bias = bf; g.ln_C = C; g.ln_eps = 1e-5f;
   }
+  template <class Op> Launch& emit(Launch::Kind kind, const Op& op, Launch::Input in = Launch::NONE) {
+    Launch l; l.kind = kind; l.input = in; l.op = op;
+    out->push_back(l);
+    return out->back();
+  }
   Launch& emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
-    Launch l; l.kind = Launch::GEMM; l.input = in;
     if (!dry) {
       if (g.nkb_total != w.nkb) { set_error("internal: K mismatch %d vs %d", g.nkb_total, w.nkb); err = -1; }
       plan_gemm(g);
       if (!simt) { const int rc = encode_tmaps(g); if (rc) err = rc; }
     }
-    l.gemm = g;
-    out->push_back(l);
-    return out->back();
+    return emit(Launch::GEMM, g, in);
   }
   void emit_attention(const AttnOp& a, Launch::Input in = Launch::NONE) {
-    Launch l; l.kind = Launch::ATTN; l.input = in; l.attn = a;
-    if (a.v2 && !dry) { const int rc = encode_attn_tmaps(l.attn); if (rc) err = rc; }
-    out->push_back(l);
+    AttnOp& op = emit(Launch::ATTN, a, in).get<AttnOp>();
+    if (a.v2 && !dry) { const int rc = encode_attn_tmaps(op); if (rc) err = rc; }
   }
-  void emit_ln_split(const float* x, int ld, int M, int C, const float* gamma, const float* beta, const SplitBuf& o) {
-    Launch l; l.kind = Launch::LN_SPLIT; l.a = x; l.i0 = ld; l.i1 = M; l.i2 = C; l.f0 = 1e-5f; l.b = gamma; l.c = beta; l.split = o;
-    out->push_back(l);
+  // LayerNorm (eps 1e-5) of M rows of C channels at pitch ld; `keep`: rows whose factor is 0 are stored as zeros, or nullptr
+  void emit_ln_split(const float* x, int ld, int M, int C, const float* gamma, const float* beta, const SplitBuf& o, const float* keep = nullptr) {
+    LnOp op{x, ld, M, C, 1e-5f, gamma, beta, keep, nullptr, 0, o};
+    emit(Launch::LN_SPLIT, op);
   }
   void emit_ln_apply(const float* x, Launch::Input in, int M, int C, const float* gamma, const float* beta, float* y) {
-    Launch l; l.kind = Launch::LN_APPLY; l.input = in; l.a = x; l.i0 = C; l.i1 = M; l.i2 = C; l.f0 = 1e-5f; l.b = gamma; l.c = beta;
-    l.o = y; l.i3 = C;
-    out->push_back(l);
+    LnOp op{x, C, M, C, 1e-5f, gamma, beta, nullptr, y, C, SplitBuf{}};
+    emit(Launch::LN_APPLY, op, in);
   }
   void emit_linear(const LinOp& o, Launch::Input in = Launch::NONE, int time_path = 0) {
-    Launch l; l.kind = Launch::LINEAR; l.input = in; l.lin = o; l.time_path = time_path;
-    out->push_back(l);
+    emit(Launch::LINEAR, o, in).time_path = time_path;
   }
-  void emit_memset(void* p, size_t bytes) {
-    Launch l; l.kind = Launch::MEMSET; l.mem = p; l.mem_bytes = bytes;
-    out->push_back(l);
-  }
+  void emit_memset(void* p, size_t bytes) { emit(Launch::MEMSET, MemsetOp{p, bytes}); }
   // copy-out point of a named activation ([B, rows, C] fp32): only in real programs, whose taps can be read
   void emit_tap(TapSet& taps, const std::string& name, const float* src, int tap_rows, int C, int rows) {
     if (dry) return;
-    Launch l; l.kind = Launch::TAP; l.a = src; l.i0 = B * rows * C; l.tap_index = taps.add(name, tap_rows, C);
-    out->push_back(l);
+    emit(Launch::TAP, CopyOp{src, (size_t)B * rows * C * sizeof(float), nullptr}).tap_index = taps.add(name, tap_rows, C);
   }
 };
 
@@ -325,48 +357,71 @@ struct TextTimeEmbedding {
             int E, int heads, Launch::Kind attend, const PoolKV& pkv, float* y, const int* lens = nullptr) const {
     const int B = bld.B;
     bld.emit_ln_apply(x, x_in, B * S, R, w.W(p + ".norm1.weight"), w.W(p + ".norm1.bias"), norm);
-    { Launch l; l.kind = Launch::POOL_CLS; l.a = norm; l.b = w.W(p + ".pool.positional_embedding"); l.i0 = S; l.i1 = R; l.o = tok; l.lens = lens;
-      bld.out->push_back(l); }
+    bld.emit(Launch::POOL_CLS, PoolClsOp{norm, w.W(p + ".pool.positional_embedding"), B, S, R, tok, lens});
     bld.emit_linear(linear_op(tok, (S + 1) * R, B, R, w.W(p + ".pool.q_proj.weight"), w.W(p + ".pool.q_proj.bias"), R, q, R));
     bld.emit_linear(linear_op(tok, R, B * (S + 1), R, pkv.W, pkv.b, 2 * R, kv, 2 * R));
-    { Launch l; l.kind = attend; l.a = q; l.b = kv; l.i0 = S + 1; l.i1 = R; l.i2 = heads; l.o = pool; l.lens = lens; bld.out->push_back(l); }
+    bld.emit(attend, PoolAttOp{q, kv, B, S + 1, R, heads, pool, lens});
     bld.emit_linear(linear_op(pool, R, B, R, w.W(p + ".proj.weight"), w.W(p + ".proj.bias"), E, proj, E));
     bld.emit_ln_apply(proj, Launch::NONE, B, E, w.W(p + ".norm2.weight"), w.W(p + ".norm2.bias"), y);
   }
 };
 
-// Runs the launch kinds both engines use.  GEMM / ATTN launch the op they are given: the record's own or a copy the caller
-// patched.  `in` replaces the recorded input of LN_APPLY and LINEAR when the launch reads a call argument.
+// Launches every kind whose launcher common.cuh declares, with the arguments of the record (bound, patched or as built);
+// returns kEngineKind for the kinds an engine launches itself.
+constexpr int kEngineKind = 1;
 struct Runner {
   bool simt;
-  int B;
   const TapSet* taps;
   cudaStream_t st;
 
-  int gemm(const GemmOp& g) const { return simt ? launch_gemm_simt(g, st) : launch_gemm_tc(g, st); }
-  int attn(const AttnOp& a) const { return (a.v2 && !simt) ? launch_attention_v2(a, st) : launch_attention(a, st, simt); }
-  int run(const Launch& l, const float* in = nullptr, unsigned long long* span = nullptr) const {
+  int run(const Launch& l) const {
     switch (l.kind) {
-      case Launch::GEMM: return gemm(l.gemm);
-      case Launch::ATTN: return attn(l.attn);
-      case Launch::LN_SPLIT: return launch_ln_split(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.split, st, span, l.d);   // d: row keep factors, or nullptr
-      case Launch::LN_APPLY: return launch_ln_apply(in ? in : l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.o, l.i3, st);
-      case Launch::LINEAR: {
-        LinOp o = l.lin;
-        if (in) o.x = in;
-        return launch_small_linear(o, st);
-      }
-      case Launch::POOL_CLS: return launch_pool_class_token(l.a, l.b, B, l.i0, l.i1, l.o, st, l.lens);
+      case Launch::GEMM: { const GemmOp& g = l.get<GemmOp>(); return simt ? launch_gemm_simt(g, st) : launch_gemm_tc(g, st); }
+      case Launch::ATTN: { const AttnOp& a = l.get<AttnOp>(); return (a.v2 && !simt) ? launch_attention_v2(a, st) : launch_attention(a, st, simt); }
+      case Launch::LN_SPLIT: return launch_ln_split(l.get<LnOp>(), st);
+      case Launch::LN_APPLY: return launch_ln_apply(l.get<LnOp>(), st);
+      case Launch::LN_MASK: return launch_ln_mask(l.get<LnOp>(), st);
+      case Launch::LINEAR: return launch_small_linear(l.get<LinOp>(), st);
+      case Launch::NCT2SPLIT: return launch_nct_to_split(l.get<NctSplitOp>(), st);
+      case Launch::NCT2TOK: return launch_nct_to_tokens(l.get<TokensOp>(), st);
+      case Launch::ENC_INPUT: return launch_enc_input(l.get<TokensOp>(), st);
+      case Launch::POOL_CLS: return launch_pool_class_token(l.get<PoolClsOp>(), st);
+      case Launch::POOL_ATT: return launch_pool_attend(l.get<PoolAttOp>(), st);
+      case Launch::POOL_ATT_WIDE: return launch_pool_attend_wide(l.get<PoolAttOp>(), st);
+      case Launch::MASKBIAS: return launch_mask_bias(l.get<MaskBiasOp>(), st);
+      case Launch::PREP: return launch_prep_split(l.get<PrepOp>(), st);
+      case Launch::SEQMASK: return launch_seq_mask(l.get<SeqMaskOp>(), st);
+      case Launch::VOC_NORM: return launch_voc_norm(l.get<VocNormOp>(), st);
       case Launch::MEMSET: {
-        const cudaError_t e = cudaMemsetAsync(l.mem, 0, l.mem_bytes, st);
+        const MemsetOp& m = l.get<MemsetOp>();
+        const cudaError_t e = cudaMemsetAsync(m.p, 0, m.bytes, st);
         if (e != cudaSuccess) { set_error("memset failed: %s", cudaGetErrorString(e)); return -2; }
         return 0;
       }
+      case Launch::COPY: {
+        const CopyOp& c = l.get<CopyOp>();
+        NS_CHECK_CUDA(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToDevice, st));
+        return 0;
+      }
       case Launch::TAP: return taps->copy(l, st);
-      default: set_error("internal: launch kind %d is not a shared kind", (int)l.kind); return -1;
+      default: return kEngineKind;
     }
   }
 };
+
+inline int no_launcher(const Launch& l) {
+  set_error("internal: launch kind %d has no launcher", (int)l.kind);
+  return -1;
+}
+
+// The record to launch for `l`: `l` itself, or (when it reads a call argument) `tmp` holding a copy with the argument bound
+inline const Launch* bound(const Launch& l, const CallArgs& in, Launch& tmp, int& rc) {
+  rc = 0;
+  if (l.input == Launch::NONE) return &l;
+  tmp = l;
+  rc = bind_input(tmp, in[l.input]);
+  return &tmp;
+}
 
 // What every engine handle holds: the reference state_dict, the device memory of its packed weights, whether the loaded
 // weights are packed, and the number of launches of its last run.  Each handle also has a drop_programs() that forgets the
@@ -456,18 +511,20 @@ template <class Build> int ensure_program(SingleProgramEngine* h, const char* en
   return 0;
 }
 
-// Runs h->cp and records its launch count in h->last_launches.  `own(l)` launches the engine's own kinds and returns
-// kSharedKind for the kinds Runner launches.  Tap copies (the launches with a tap index) are not counted: they are
-// diagnostics, not part of the computation.
-constexpr int kSharedKind = 1;
-template <class Own> int run_cached(SingleProgramEngine* h, bool simt, cudaStream_t st, Own own) {
-  const Runner run{simt, h->cp.dims[0], &h->cp.taps, st};
+// Runs h->cp over the call arguments `in` and records its launch count in h->last_launches.  `own(l)` launches the kinds
+// Runner leaves to the engine.  Tap copies (the launches with a tap index) are not counted: they are diagnostics, not part of
+// the computation.
+template <class Own> int run_cached(SingleProgramEngine* h, bool simt, const CallArgs& in, cudaStream_t st, Own own) {
+  const Runner run{simt, &h->cp.taps, st};
+  Launch tmp;
   int count = 0;
-  for (const Launch& l : h->cp.prog) {
-    int rc = own(l);
-    if (rc == kSharedKind) rc = run.run(l);
+  for (const Launch& rec : h->cp.prog) {
+    int rc;
+    const Launch* l = bound(rec, in, tmp, rc);
+    if (!rc) rc = run.run(*l);
+    if (rc == kEngineKind) rc = own(*l);
     if (rc) return rc;
-    if (l.tap_index < 0) ++count;
+    if (rec.tap_index < 0) ++count;
   }
   h->last_launches = count;
   return 0;

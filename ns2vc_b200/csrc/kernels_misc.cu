@@ -58,31 +58,9 @@ __global__ void nct_to_tokens_kernel(const float* __restrict__ x, long long bstr
     if (t < T && c < Cpad) out[((long long)b * T + t) * ldo + c] = tile[threadIdx.x][i];
   }
 }
-int launch_nct_to_tokens(const float* x, long long bstride, int B, int C, int T, float* out, int ldo, int Cpad,
-                         cudaStream_t st) {
-  dim3 grid(ceil_div(T, 32), ceil_div(Cpad, 32), B), block(32, 8);
-  nct_to_tokens_kernel<<<grid, block, 0, st>>>(x, bstride, C, T, out, ldo, Cpad);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-__global__ void tokens_to_nct_kernel(const float* __restrict__ x, int ld, int C, int T, float* __restrict__ out) {
-  __shared__ float tile[32][33];
-  const int b = blockIdx.z;
-  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    int t = t0 + i, c = c0 + threadIdx.x;
-    tile[i][threadIdx.x] = (c < C && t < T) ? x[((long long)b * T + t) * ld + c] : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    int c = c0 + i, t = t0 + threadIdx.x;
-    if (c < C && t < T) out[((long long)b * C + c) * T + t] = tile[threadIdx.x][i];
-  }
-}
-int launch_tokens_to_nct(const float* x, int ld, int B, int C, int T, float* out, cudaStream_t st) {
-  dim3 grid(ceil_div(T, 32), ceil_div(C, 32), B), block(32, 8);
-  tokens_to_nct_kernel<<<grid, block, 0, st>>>(x, ld, C, T, out);
+int launch_nct_to_tokens(const TokensOp& op, cudaStream_t st) {
+  dim3 grid(ceil_div(op.T, 32), ceil_div(op.ld, 32), op.B), block(32, 8);
+  nct_to_tokens_kernel<<<grid, block, 0, st>>>(op.x, op.bstride, op.C, op.T, op.out, op.ld, op.ld);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -113,14 +91,8 @@ __global__ void __launch_bounds__(256) ln_kernel(const float* __restrict__ x, in
     stats[2 * row + 1] = rstd;
   }
 }
-int launch_ln_stats(const float* x, int ld, int M, int C, float eps, float* stats, cudaStream_t st) {
-  ln_kernel<false><<<ceil_div(M, 8), 256, 0, st>>>(x, ld, M, C, eps, stats, nullptr, nullptr, nullptr, 0);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-int launch_ln_apply(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta, float* y,
-                    int y_ld, cudaStream_t st) {
-  ln_kernel<true><<<ceil_div(M, 8), 256, 0, st>>>(x, ld, M, C, eps, nullptr, gamma, beta, y, y_ld);
+int launch_ln_apply(const LnOp& op, cudaStream_t st) {
+  ln_kernel<true><<<ceil_div(op.M, 8), 256, 0, st>>>(op.x, op.ld, op.M, op.C, op.eps, nullptr, op.gamma, op.beta, op.y, op.y_ld);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -263,11 +235,13 @@ __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__
   }
   span_end(span);
 }
-int launch_ln_split(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta, SplitBuf out,
-                    cudaStream_t st, unsigned long long* span, const float* keep) {
-  if (C > 1024 || (out.ld & 7) || out.ld > 1024) { set_error("ln_split: C=%d / pitch %d unsupported", C, out.ld); return -1; }
-  if (keep) launch_k(ln_split_kernel<true>, dim3(ceil_div(M, 8)), dim3(256), 0, st, x, ld, M, C, eps, gamma, beta, out, span, keep);
-  else launch_k(ln_split_kernel<false>, dim3(ceil_div(M, 8)), dim3(256), 0, st, x, ld, M, C, eps, gamma, beta, out, span, keep);
+int launch_ln_split(const LnOp& op, cudaStream_t st) {
+  const SplitBuf& out = op.split;
+  if (op.C > 1024 || (out.ld & 7) || out.ld > 1024) { set_error("ln_split: C=%d / pitch %d unsupported", op.C, out.ld); return -1; }
+  unsigned long long* span = nullptr;
+  const dim3 grid(ceil_div(op.M, 8)), block(256);
+  if (op.keep) launch_k(ln_split_kernel<true>, grid, block, 0, st, op.x, op.ld, op.M, op.C, op.eps, op.gamma, op.beta, out, span, op.keep);
+  else launch_k(ln_split_kernel<false>, grid, block, 0, st, op.x, op.ld, op.M, op.C, op.eps, op.gamma, op.beta, out, span, op.keep);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -306,11 +280,11 @@ __global__ void nct_to_split_kernel(const float* __restrict__ x, long long bstri
     }
   }
 }
-int launch_nct_to_split(const float* x, long long bstride, int B, int C, int T, SplitBuf out, cudaStream_t st, const void* warm,
-                        long long warm_bytes, const int* row_len) {
-  dim3 grid(ceil_div(T, 32), ceil_div(out.ld, 32), B), block(32, 8);
-  if (row_len) launch_k(nct_to_split_kernel<true>, grid, block, 0, st, x, bstride, C, T, out, (const char*)warm, warm_bytes, row_len);
-  else launch_k(nct_to_split_kernel<false>, grid, block, 0, st, x, bstride, C, T, out, (const char*)warm, warm_bytes, row_len);
+int launch_nct_to_split(const NctSplitOp& op, cudaStream_t st) {
+  dim3 grid(ceil_div(op.T, 32), ceil_div(op.out.ld, 32), op.B), block(32, 8);
+  const char* warm = (const char*)op.warm;
+  if (op.row_len) launch_k(nct_to_split_kernel<true>, grid, block, 0, st, op.x, op.bstride, op.C, op.T, op.out, warm, op.warm_bytes, op.row_len);
+  else launch_k(nct_to_split_kernel<false>, grid, block, 0, st, op.x, op.bstride, op.C, op.T, op.out, warm, op.warm_bytes, op.row_len);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -448,9 +422,9 @@ __global__ void pool_class_token_kernel(const float* __restrict__ xn, const floa
     for (int t = 0; t < S; ++t) tokens[((long long)b * (S + 1) + 1 + t) * C + c] = xn[((long long)b * S + t) * C + c];
   }
 }
-int launch_pool_class_token(const float* xn, const float* pos, int B, int S, int C, float* tokens, cudaStream_t st, const int* lens) {
-  if (lens) pool_class_token_kernel<true><<<B, 256, 0, st>>>(xn, pos, S, C, tokens, lens);
-  else pool_class_token_kernel<false><<<B, 256, 0, st>>>(xn, pos, S, C, tokens, lens);
+int launch_pool_class_token(const PoolClsOp& op, cudaStream_t st) {
+  if (op.lens) pool_class_token_kernel<true><<<op.B, 256, 0, st>>>(op.x, op.pos, op.S, op.C, op.tokens, op.lens);
+  else pool_class_token_kernel<false><<<op.B, 256, 0, st>>>(op.x, op.pos, op.S, op.C, op.tokens, op.lens);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -492,10 +466,10 @@ __global__ void pool_attend_kernel(const float* __restrict__ q, const float* __r
     if (lane == 0) out[(long long)b * C + h * dph + d] = a / den;
   }
 }
-int launch_pool_attend(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st, const int* lens) {
-  if (C % heads || C / heads > 16) { set_error("pool_attend: dim/head %d/%d unsupported", C, heads); return -1; }
-  if (lens) pool_attend_kernel<true><<<B * heads, 32, 0, st>>>(q, kv, S1, C, heads, out, lens);
-  else pool_attend_kernel<false><<<B * heads, 32, 0, st>>>(q, kv, S1, C, heads, out, lens);
+int launch_pool_attend(const PoolAttOp& op, cudaStream_t st) {
+  if (op.C % op.heads || op.C / op.heads > 16) { set_error("pool_attend: dim/head %d/%d unsupported", op.C, op.heads); return -1; }
+  if (op.lens) pool_attend_kernel<true><<<op.B * op.heads, 32, 0, st>>>(op.q, op.kv, op.S1, op.C, op.heads, op.out, op.lens);
+  else pool_attend_kernel<false><<<op.B * op.heads, 32, 0, st>>>(op.q, op.kv, op.S1, op.C, op.heads, op.out, op.lens);
   NS_LAUNCH_CHECK();
   return 0;
 }
@@ -505,8 +479,8 @@ __global__ void mask_bias_kernel(const uint8_t* __restrict__ mask, int n, float*
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) bias[i] = (1.0f - (mask[i] ? 1.0f : 0.0f)) * -10000.0f;
 }
-int launch_mask_bias(const uint8_t* mask, int n, float* bias, cudaStream_t st) {
-  mask_bias_kernel<<<ceil_div(n, 256), 256, 0, st>>>(mask, n, bias);
+int launch_mask_bias(const MaskBiasOp& op, cudaStream_t st) {
+  mask_bias_kernel<<<ceil_div(op.n, 256), 256, 0, st>>>(op.mask, op.n, op.bias);
   NS_LAUNCH_CHECK();
   return 0;
 }

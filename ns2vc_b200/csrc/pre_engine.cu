@@ -185,8 +185,8 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
   auto new_rowstats = [&]() { double* p = stat_cur; if (stat_cur) stat_cur += 2 * M; return p; };
   auto masked = [&](GemmOp& g) { g.flags |= EPI_ROWMASK; g.rowmask = keep; };
 
-  { Launch l; l.kind = Launch::SEQMASK; l.input = io.lengths; l.i0 = Tn; l.o = keep; l.o2 = kbias; l.mem = ilens; bld.out->push_back(l); }
-  { Launch l; l.kind = Launch::ENC_INPUT; l.input = io.in; l.b = spk; l.c = keep; l.i0 = e.cin; l.i1 = Tn; l.o = X0; l.i2 = ldin; bld.out->push_back(l); }
+  bld.emit(Launch::SEQMASK, SeqMaskOp{nullptr, B, Tn, keep, kbias, ilens}, io.lengths);
+  bld.emit(Launch::ENC_INPUT, TokensOp{nullptr, 0, B, e.cin, Tn, X0, ldin, spk, keep}, io.in);
   bld.emit_ln_split(X0, ldin, (int)M, e.cin, w.W(e.p + ".pre.layer_norm.weight"), w.W(e.p + ".pre.layer_norm.bias"), s_in);
   double* rs = new_rowstats();
   { GemmOp g = bld.lin(e.pre, s_in, Tn);
@@ -215,8 +215,7 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
       g.flags = EPI_RESIDUAL | EPI_OUT_F32; g.res = XA; g.res_ld = H; g.out = XB; g.out_ld = H;
       masked(g);
       bld.emit_gemm(g, ls.out); }
-    bld.emit_ln_split(XB, H, (int)M, H, w.W(b + ".layer_norm2.weight"), w.W(b + ".layer_norm2.bias"), s_y);
-    if (ragged) bld.out->back().d = keep;
+    bld.emit_ln_split(XB, H, (int)M, H, w.W(b + ".layer_norm2.weight"), w.W(b + ".layer_norm2.bias"), s_y, ragged ? keep : nullptr);
     { GemmOp g = bld.gemm_base(ls.ffn1, Tn);
       const int src = bld.add_src(g, s_y);
       for (int j = 0; j < k - 1; ++j) bld.seg(g, src, 0, H, j + 1 - (k - 1) / 2);     // row offsets -3 .. +4 for k = 9
@@ -234,8 +233,8 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
     g.flags = EPI_OUT_F32; g.out = OUTP; g.out_ld = e.cout;
     bld.consumes_ln(g, rs, e.g_out, e.bf_out, H);
     bld.emit_gemm(g, e.outp); }
-  { Launch l; l.kind = Launch::LN_MASK; l.input = io.out; l.a = OUTP; l.i0 = e.cout; l.i1 = (int)M; l.i2 = e.cout; l.f0 = 1e-5f;
-    l.b = w.W(e.p + ".layer_norm.weight"); l.c = w.W(e.p + ".layer_norm.bias"); l.d = keep; bld.out->push_back(l); }
+  bld.emit(Launch::LN_MASK, LnOp{OUTP, e.cout, (int)M, e.cout, 1e-5f, w.W(e.p + ".layer_norm.weight"), w.W(e.p + ".layer_norm.bias"), keep,
+                                 nullptr, e.cout, SplitBuf{}}, io.out);
 }
 
 // `ragged`: row b is the utterance c[b, :, :T_b], refer[b, :, :S_b] encoded alone (ns2vc_pre_infer_ragged).  Besides the masked
@@ -263,7 +262,7 @@ int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size
   tte.reserve(ar, B, S, R, R);
   float* g = ar.get<float>((size_t)B * R);
   float* spk = ar.get<float>((size_t)B * c.phone_hidden);
-  { Launch l; l.kind = Launch::NCT2TOK; l.input = Launch::REFER; l.i0 = R; l.i1 = S; l.o = rt; prog.push_back(l); }
+  bld.emit(Launch::NCT2TOK, TokensOp{nullptr, 0, B, R, S, rt, R, nullptr, nullptr}, Launch::REFER);
   tte.emit(bld, h->weights, "ref_enc", rt, Launch::NONE, S, R, R, c.ref_heads, Launch::POOL_ATT_WIDE, h->ref_kv, g, plens);
   bld.emit_tap(taps, "ref_enc", g, 1, R, 1);
   // spk_proj: Conv1d(100, hidden, 1) on g [B, 100, 1] (model.py:123, 127)
@@ -282,20 +281,13 @@ int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size
 
 int run_program(ns2vc_pre* h, const float* c, const float* refer, const long long* lengths, const long long* refer_lengths, float* content,
                 float* prompt, cudaStream_t st) {
-  const int B = h->cp.dims[0];
-  return run_cached(h, h->simt, st, [&](const Launch& l) {
-    switch (l.kind) {
-      case Launch::SEQMASK: return launch_seq_mask(l.input == Launch::LENGTHS ? lengths : refer_lengths, B, l.i0, l.o, l.o2, st, (int*)l.mem);
-      case Launch::ENC_INPUT: {
-        const float* src = l.input == Launch::C ? c : refer;
-        return launch_enc_input(src, (long long)l.i0 * l.i1, l.b, l.c, B, l.i0, l.i1, l.o, l.i2, st);
-      }
-      case Launch::LN_MASK: return launch_ln_mask(l.a, l.i0, l.i1, l.i2, l.f0, l.b, l.c, l.d, l.input == Launch::CONTENT_OUT ? content : prompt, l.i2, st);
-      case Launch::NCT2TOK: return launch_nct_to_tokens(refer, (long long)l.i0 * l.i1, B, l.i0, l.i1, l.o, l.i0, l.i0, st);
-      case Launch::POOL_ATT_WIDE: return launch_pool_attend_wide(l.a, l.b, B, l.i0, l.i1, l.i2, l.o, st, l.lens);
-      default: return kSharedKind;
-    }
-  });
+  const int T = h->cp.dims[1], S = h->cp.dims[2];
+  CallArgs in{};
+  in[Launch::C] = {c, (long long)h->cfg.phone_in * T};
+  in[Launch::REFER] = {refer, (long long)h->cfg.prompt_in * S};
+  in[Launch::LENGTHS] = {lengths}; in[Launch::REFER_LENGTHS] = {refer_lengths};
+  in[Launch::CONTENT_OUT] = {content}; in[Launch::PROMPT_OUT] = {prompt};
+  return run_cached(h, h->simt, in, st, no_launcher);
 }
 
 }  // namespace

@@ -44,8 +44,8 @@ __global__ void seq_mask_kernel(const long long* __restrict__ len, int B, int T,
   kbias[i] = (1.0f - k) * -10000.0f;
   if (ilen && t == 0) ilen[b] = (int)max(1LL, min((long long)T, len[b]));
 }
-int launch_seq_mask(const long long* len, int B, int T, float* keep, float* kbias, cudaStream_t st, int* ilen) {
-  seq_mask_kernel<<<ceil_div(B * T, 256), 256, 0, st>>>(len, B, T, keep, kbias, ilen);
+int launch_seq_mask(const SeqMaskOp& op, cudaStream_t st) {
+  seq_mask_kernel<<<ceil_div(op.B * op.T, 256), 256, 0, st>>>(op.len, op.B, op.T, op.keep, op.kbias, op.ilen);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }
@@ -73,10 +73,9 @@ __global__ void enc_input_kernel(const float* __restrict__ x, long long bstride,
     }
   }
 }
-int launch_enc_input(const float* x, long long bstride, const float* rowbias, const float* keep, int B, int C, int T, float* out, int ld,
-                     cudaStream_t st) {
-  dim3 grid(ceil_div(T, 32), ceil_div(ld, 32), B), block(32, 8);
-  enc_input_kernel<<<grid, block, 0, st>>>(x, bstride, rowbias, keep, C, T, out, ld);
+int launch_enc_input(const TokensOp& op, cudaStream_t st) {
+  dim3 grid(ceil_div(op.T, 32), ceil_div(op.ld, 32), op.B), block(32, 8);
+  enc_input_kernel<<<grid, block, 0, st>>>(op.x, op.bstride, op.rowbias, op.keep, op.C, op.T, op.out, op.ld);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }
@@ -98,9 +97,8 @@ __global__ void __launch_bounds__(256) ln_mask_kernel(const float* __restrict__ 
   float* yr = y + (long long)row * y_ld;
   for (int c = lane; c < C; c += 32) yr[c] = ((xr[c] - mean) * rstd * gamma[c] + beta[c]) * k;
 }
-int launch_ln_mask(const float* x, int ld, int M, int C, float eps, const float* gamma, const float* beta, const float* keep, float* y, int y_ld,
-                   cudaStream_t st) {
-  ln_mask_kernel<<<ceil_div(M, 8), 256, 0, st>>>(x, ld, M, C, eps, gamma, beta, keep, y, y_ld);
+int launch_ln_mask(const LnOp& op, cudaStream_t st) {
+  ln_mask_kernel<<<ceil_div(op.M, 8), 256, 0, st>>>(op.x, op.ld, op.M, op.C, op.eps, op.gamma, op.beta, op.keep, op.y, op.y_ld);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }
@@ -149,12 +147,12 @@ __global__ void __launch_bounds__(256) pool_attend_wide_kernel(const float* __re
     out[(long long)b * C + h * dph + d] = a / den;
   }
 }
-int launch_pool_attend_wide(const float* q, const float* kv, int B, int S1, int C, int heads, float* out, cudaStream_t st, const int* lens) {
-  if (heads < 1 || C % heads) { set_error("pool_attend: dim/heads %d/%d unsupported", C, heads); return -1; }
-  const size_t smem = (size_t)S1 * sizeof(float);
-  if (smem > 48 * 1024) { set_error("pool_attend: %d keys do not fit the score buffer", S1); return -1; }
-  if (lens) pool_attend_wide_kernel<true><<<B * heads, 256, smem, st>>>(q, kv, S1, C, heads, out, lens);
-  else pool_attend_wide_kernel<false><<<B * heads, 256, smem, st>>>(q, kv, S1, C, heads, out, lens);
+int launch_pool_attend_wide(const PoolAttOp& op, cudaStream_t st) {
+  if (op.heads < 1 || op.C % op.heads) { set_error("pool_attend: dim/heads %d/%d unsupported", op.C, op.heads); return -1; }
+  const size_t smem = (size_t)op.S1 * sizeof(float);
+  if (smem > 48 * 1024) { set_error("pool_attend: %d keys do not fit the score buffer", op.S1); return -1; }
+  if (op.lens) pool_attend_wide_kernel<true><<<op.B * op.heads, 256, smem, st>>>(op.q, op.kv, op.S1, op.C, op.heads, op.out, op.lens);
+  else pool_attend_wide_kernel<false><<<op.B * op.heads, 256, smem, st>>>(op.q, op.kv, op.S1, op.C, op.heads, op.out, op.lens);
   NS_PRE_LAUNCH_CHECK();
   return 0;
 }

@@ -288,11 +288,12 @@ __global__ void voc_layer_scale_kernel(const float* __restrict__ W, const float*
 }  // namespace
 
 // (also the content encoder's LayerNorms: content.cu)
-int launch_voc_norm(const float* x, int B, int T, int C, const float* dw, const float* gamma, const float* beta, float eps, const long long* len,
-                    float* out, const SplitBuf& split, cudaStream_t st) {
-  const dim3 grid(ceil_div(T, kNormRows), B), block(C / 4);
-  cudaError_t e = dw ? launch_k(voc_norm_kernel<true>, grid, block, 0, st, x, T, C, reinterpret_cast<const float4*>(dw), gamma, beta, eps, len, out, split)
-                     : launch_k(voc_norm_kernel<false>, grid, block, 0, st, x, T, C, (const float4*)nullptr, gamma, beta, eps, len, out, split);
+int launch_voc_norm(const VocNormOp& op, cudaStream_t st) {
+  const dim3 grid(ceil_div(op.T, kNormRows), op.B), block(op.C / 4);
+  cudaError_t e = op.dw ? launch_k(voc_norm_kernel<true>, grid, block, 0, st, op.x, op.T, op.C, reinterpret_cast<const float4*>(op.dw), op.gamma,
+                                   op.beta, op.eps, op.len, op.out, op.split)
+                        : launch_k(voc_norm_kernel<false>, grid, block, 0, st, op.x, op.T, op.C, (const float4*)nullptr, op.gamma, op.beta,
+                                   op.eps, op.len, op.out, op.split);
   if (e != cudaSuccess) { set_error("voc_norm launch failed: %s", cudaGetErrorString(e)); return -2; }
   return 0;
 }
@@ -415,12 +416,10 @@ int build_program(ns2vc_voc* h, int B, int T, void* ws, size_t* bytes_out) {
   float* y = ar.get<float>(M * D);
   float* H = ar.get<float>(M * ldh);
   auto norm = [&](const float* in, const float* dwp, const std::string& ln, float* out, const SplitBuf& split) {
-    Launch l; l.kind = Launch::VOC_NORM; l.a = in; l.d = dwp; l.b = w.W(ln + ".weight"); l.c = w.W(ln + ".bias"); l.f0 = 1e-6f;
-    l.i0 = T; l.o = out; l.split = split;
-    prog.push_back(l);
+    bld.emit(Launch::VOC_NORM, VocNormOp{in, B, T, D, dwp, w.W(ln + ".weight"), w.W(ln + ".bias"), 1e-6f, nullptr, out, split}, Launch::LENGTHS);
   };
-  { Launch l; l.kind = Launch::VOC_LENS; l.i0 = T; l.mem = lens; l.o = keep; prog.push_back(l); }
-  { Launch l; l.kind = Launch::NCT2SPLIT; l.input = Launch::MEL; l.i0 = c.input_channels; l.i1 = T; l.split = s_mel; l.lens = lens; prog.push_back(l); }
+  bld.emit(Launch::VOC_LENS, VocLensOp{B, T, lens, keep});
+  bld.emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, c.input_channels, T, s_mel, lens, nullptr, 0}, Launch::MEL);
   { GemmOp g = bld.gemm_base(h->embed, T);
     const int src = bld.add_src(g, s_mel);
     for (int j = 0; j < kTaps; ++j) bld.seg(g, src, 0, c.input_channels, j - kTaps / 2);
@@ -448,7 +447,7 @@ int build_program(ns2vc_voc* h, int B, int T, void* ws, size_t* bytes_out) {
     g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = w.W("head.out.bias"); g.out = H; g.out_ld = ldh;
     bld.emit_gemm(g, h->head); }
   bld.emit_tap(taps, "head.out", H, T, ldh, T);
-  { Launch l; l.kind = Launch::VOC_ISTFT; l.input = Launch::AUDIO; l.a = H; l.i0 = ldh; l.i1 = T; prog.push_back(l); }
+  bld.emit(Launch::VOC_ISTFT, IstftOp{H, ldh, B, T});
   if (bld.err) return bld.err;
   if (bytes_out) *bytes_out = ar.off + 256;
   if (!dry) {
@@ -459,17 +458,18 @@ int build_program(ns2vc_voc* h, int B, int T, void* ws, size_t* bytes_out) {
 }
 
 int run_program(ns2vc_voc* h, const float* mel, long long mel_bstride, const long long* lengths, float* audio, cudaStream_t st) {
-  const int B = h->cp.dims[0], T = h->cp.dims[1];
-  return run_cached(h, false, st, [&](const Launch& l) {
+  CallArgs in{};
+  in[Launch::MEL] = {mel, mel_bstride}; in[Launch::LENGTHS] = {lengths};
+  return run_cached(h, false, in, st, [&](const Launch& l) {
     switch (l.kind) {
-      case Launch::VOC_LENS:
-        voc_lengths_kernel<<<ceil_div(B * T, 256), 256, 0, st>>>(lengths, B, T, static_cast<int*>(l.mem), l.o);
+      case Launch::VOC_LENS: {
+        const VocLensOp& o = l.get<VocLensOp>();
+        voc_lengths_kernel<<<ceil_div(o.B * o.T, 256), 256, 0, st>>>(lengths, o.B, o.T, o.lens, o.keep);
         NS_VOC_LAUNCH_CHECK();
         return 0;
-      case Launch::NCT2SPLIT: return launch_nct_to_split(mel, mel_bstride, B, l.i0, l.i1, l.split, st, nullptr, 0, l.lens);
-      case Launch::VOC_NORM: return launch_voc_norm(l.a, B, l.i0, h->cfg.dim, l.d, l.b, l.c, l.f0, lengths, l.o, l.split, st);
-      case Launch::VOC_ISTFT: return launch_istft(h, l.a, l.i0, lengths, audio, B, l.i1, st);
-      default: return kSharedKind;
+      }
+      case Launch::VOC_ISTFT: { const IstftOp& o = l.get<IstftOp>(); return launch_istft(h, o.h, o.ld, lengths, audio, o.B, o.T, st); }
+      default: return no_launcher(l);
     }
   });
 }
