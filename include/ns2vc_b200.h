@@ -398,6 +398,18 @@ int ns2vc_mse_workspace_bytes(int K, int B, int C, int T, size_t* bytes);
 int ns2vc_mse_rows(const float* out, const float* target, int target_per_k, const int64_t* t, const float* loss_weight, int timesteps,
                    float min_snr_gamma, float* loss_row, float* loss_weighted, float* loss, int K, int B, int C, int T, void* ws,
                    ns2vc_stream stream);
+/* Host-only: bytes of the scratch buffer ns2vc_mse_rows_ragged needs (its contents on entry do not matter). */
+int ns2vc_mse_ragged_workspace_bytes(int K, int B, int C, int T, size_t* bytes);
+/* The per-utterance reduction of a ragged batch: loss_row[k, b] = mean over the C * T_b elements of frames f < T_b = lengths[b]
+ * of (out[k, b] - target[b])^2, loss_weighted[k, b] = loss_row * w with w as for ns2vc_mse_rows.  out, target as for
+ * ns2vc_mse_rows; lengths [B] int64 device (a length outside [1, T] gives NaN in its rows).  Nothing past a row's length is read,
+ * so non-finite padding has no effect.  The partition of a row and the order of every addition depend on (C, T_b) only: a row's
+ * result has the same bits whatever T, B or position it has (and equals ns2vc_mse_rows on the unpadded row).  No atomics;
+ * every fp32 output is rounded once from fp64.  K * B <= 65535.  ws: 8-byte aligned device scratch.
+ * Stream-ordered, allocates nothing, capturable. */
+int ns2vc_mse_rows_ragged(const float* out, const float* target, int target_per_k, const int64_t* lengths, const int64_t* t,
+                          const float* loss_weight, int timesteps, float min_snr_gamma, float* loss_row, float* loss_weighted, int K,
+                          int B, int C, int T, void* ws, ns2vc_stream stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Kernel checks (tests only): one weight packing, one wgmma GEMM or one flash attention through the engines' own host code

@@ -167,6 +167,9 @@ SIGNATURES = {
     "ns2vc_q_sample": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "ns2vc_mse_workspace_bytes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "ns2vc_mse_rows": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_float, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_mse_ragged_workspace_bytes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ns2vc_mse_rows_ragged": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_float, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        _P, _P]),
     # kernel checks (tests only; the argument structs are mirrored in tests/test_kernels_fp64.py)
     "ns2vc_check_pack_b": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                      C.c_int, C.c_int, _P]),

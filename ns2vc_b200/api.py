@@ -230,7 +230,7 @@ def __getattr__(name):
     if name in ("convert_utterances", "convert_slices", "convert_files"):
         from . import convert
         return getattr(convert, name)
-    if name in ("diffusion_loss", "loss_profile"):           # the training objective under no_grad lives in loss.py
+    if name in ("diffusion_loss", "loss_profile", "utterance_losses"):     # the training objective under no_grad lives in loss.py
         from . import loss
         return getattr(loss, name)
     if name == "StreamConverter":

@@ -9,6 +9,9 @@
 // The MSE is deterministic: every row is cut into chunks of kMseChunk elements, one CTA per chunk, fp64 accumulation in a fixed
 // order inside the CTA, the partial sums written to a workspace and added by mse_finish_kernel in index order.  No atomics: the
 // result depends on neither the launch nor the scheduling.
+//
+// The ragged MSE (per-utterance objective) applies the same scheme to each row's own C * T_b elements and reads nothing past a
+// row's length, so a row's value does not depend on the batch it sits in.
 #include "common.cuh"
 #include "../../include/ns2vc_b200.h"
 
@@ -106,6 +109,70 @@ __global__ void __launch_bounds__(kFinishThreads) mse_finish_kernel(const double
   }
 }
 
+// The ragged reduction: row r = k * B + b holds C * T_b valid elements, frame f < T_b of channel c at c * T + f of the padded
+// [C, T] row.  Element j of the row's own [C, T_b] order is cut into chunks of kMseChunk exactly as mse_rows_kernel cuts a row of
+// n = C * T_b, and every thread walks its chunk with the same stride, so the additions and their order depend on (C, T_b) only:
+// an utterance's value has the same bits whatever T, B or row it gets.  CTAs past the row's last chunk return at once.  A
+// length outside [1, T] gives NaN (mse_ragged_finish_kernel); nothing past a row's length is read.
+__global__ void __launch_bounds__(kMseThreads) mse_rows_ragged_kernel(const float* __restrict__ out,
+                                                                      const float* __restrict__ target, long long target_kstride,
+                                                                      const int64_t* __restrict__ lengths,
+                                                                      double* __restrict__ partial, int B, int T, int n) {
+  __shared__ double s_warp[kMseThreads / 32];
+  const int p = blockIdx.x, r = blockIdx.y;
+  const int k = r / B, b = r - k * B;
+  const long long len = lengths[b];
+  if (len < 1 || len > T) return;
+  const int Tb = (int)len;
+  const int nb = (n / T) * Tb;                             // C * T_b
+  const int lo = p * kMseChunk;
+  if (lo >= nb) return;
+  const int hi = min(nb, lo + kMseChunk);
+  const float* o = out + (long long)r * n;
+  const float* g = target + (long long)k * target_kstride + (long long)b * n;
+  double acc = 0.0;
+  for (int j = lo + threadIdx.x; j < hi; j += kMseThreads) {
+    const int c = j / Tb;
+    const int i = c * T + (j - c * Tb);
+    const double d = (double)o[i] - (double)g[i];
+    acc = fma(d, d, acc);
+  }
+  for (int w = 16; w > 0; w >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, w);
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sum = s_warp[0];
+    for (int j = 1; j < kMseThreads / 32; ++j) sum += s_warp[j];
+    partial[(long long)r * gridDim.x + p] = sum;
+  }
+}
+
+// One thread per row: the row's own chunks added in index order, / (C * T_b), the weight of its t.
+__global__ void __launch_bounds__(kFinishThreads) mse_ragged_finish_kernel(const double* __restrict__ partial,
+                                                                           const int64_t* __restrict__ lengths,
+                                                                           const int64_t* __restrict__ t,
+                                                                           const float* __restrict__ loss_weight, int timesteps,
+                                                                           float min_snr_gamma, float* __restrict__ loss_row,
+                                                                           float* __restrict__ loss_weighted, int rows, int B, int T,
+                                                                           int C, int P) {
+  const int r = blockIdx.x * kFinishThreads + threadIdx.x;
+  if (r >= rows) return;
+  const long long len = lengths[r % B];
+  double mean = nan("");
+  if (len >= 1 && len <= T) {
+    const int nb = C * (int)len;
+    const int pb = (nb + kMseChunk - 1) / kMseChunk;
+    double sum = 0.0;
+    for (int p = 0; p < pb; ++p) sum += partial[(long long)r * P + p];
+    mean = sum / (double)nb;
+  }
+  const long long tb = t[r];
+  float w = (tb >= 0 && tb < timesteps) ? loss_weight[tb] : nanf("");
+  if (min_snr_gamma > 0.0f) w = fminf(w, min_snr_gamma);
+  loss_row[r] = (float)mean;
+  loss_weighted[r] = (float)(mean * (double)w);
+}
+
 inline int mse_chunks(long long n) { return (int)((n + kMseChunk - 1) / kMseChunk); }
 
 }  // namespace
@@ -157,6 +224,33 @@ int ns2vc_mse_rows(const float* out, const float* target, int target_per_k, cons
   NS_CHECK_CUDA(cudaGetLastError());
   mse_finish_kernel<<<K, kFinishThreads, 0, (cudaStream_t)stream>>>(partial, rows, t, loss_weight, timesteps, min_snr_gamma,
                                                                    loss_row, loss_weighted, loss, B, P, (int)n);
+  NS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int ns2vc_mse_ragged_workspace_bytes(int K, int B, int C, int T, size_t* bytes) {
+  NS_REQUIRE(bytes != nullptr, "mse_ragged_workspace_bytes: null argument");
+  NS_REQUIRE(K >= 1 && B >= 1 && C >= 1 && T >= 1, "mse_ragged_workspace_bytes: bad sizes K=%d B=%d C=%d T=%d", K, B, C, T);
+  *bytes = (size_t)K * B * (size_t)mse_chunks((long long)C * T) * sizeof(double);
+  return 0;
+}
+
+int ns2vc_mse_rows_ragged(const float* out, const float* target, int target_per_k, const int64_t* lengths, const int64_t* t,
+                          const float* loss_weight, int timesteps, float min_snr_gamma, float* loss_row, float* loss_weighted, int K,
+                          int B, int C, int T, void* ws, ns2vc_stream stream) {
+  NS_REQUIRE(out && target && lengths && t && loss_weight && loss_row && loss_weighted && ws, "mse_rows_ragged: null argument");
+  NS_REQUIRE(K >= 1 && B >= 1 && (long long)K * B <= 65535 && C >= 1 && T >= 1 && timesteps >= 1,
+             "mse_rows_ragged: bad sizes K=%d B=%d (K * B <= 65535) C=%d T=%d timesteps=%d", K, B, C, T, timesteps);
+  const long long n = (long long)C * T;
+  NS_REQUIRE(n <= 0x7fffffffLL - kMseChunk, "mse_rows_ragged: C * T = %lld is too long for one row", n);
+  NS_REQUIRE(((uintptr_t)ws & 7) == 0, "mse_rows_ragged: the workspace must be 8-byte aligned");
+  const int P = mse_chunks(n);
+  const int rows = K * B;
+  mse_rows_ragged_kernel<<<dim3((unsigned)P, (unsigned)rows), kMseThreads, 0, (cudaStream_t)stream>>>(
+      out, target, target_per_k ? (long long)B * n : 0LL, lengths, (double*)ws, B, T, (int)n);
+  NS_CHECK_CUDA(cudaGetLastError());
+  mse_ragged_finish_kernel<<<(rows + kFinishThreads - 1) / kFinishThreads, kFinishThreads, 0, (cudaStream_t)stream>>>(
+      (const double*)ws, lengths, t, loss_weight, timesteps, min_snr_gamma, loss_row, loss_weighted, rows, B, T, C, P);
   NS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

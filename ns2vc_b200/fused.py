@@ -457,6 +457,17 @@ class DenoiserSession:
         loss over the padded rows."""
         if self.ragged:
             raise ValueError("eval_x_start runs the padded program (the reference's objective averages over padded rows)")
+        return self._eval_k(x_KBCT, t_KB, out_KBCT)
+
+    def eval_x_start_ragged(self, x_KBCT: torch.Tensor, t_KB: torch.Tensor, out_KBCT: torch.Tensor) -> torch.Tensor:
+        """``eval_x_start`` on a ragged session: ``out[k, b, :, :T_b]`` is the prediction for utterance b alone at ``t[k, b]``, from
+        ``x[k, b, :, :T_b]`` (values past T_b are never read; ``out`` past T_b is left unspecified).  The same one ``prepare()``
+        and one ``time_table`` per CHUNK evaluations, the forwards of the ragged program."""
+        if not self.ragged:
+            raise ValueError("eval_x_start_ragged needs a ragged session (get_session(..., content_lengths=...))")
+        return self._eval_k(x_KBCT, t_KB, out_KBCT)
+
+    def _eval_k(self, x_KBCT: torch.Tensor, t_KB: torch.Tensor, out_KBCT: torch.Tensor) -> torch.Tensor:
         K = x_KBCT.shape[0]
         if tuple(x_KBCT.shape) != (K, self.B, self.Cl, self.T) or tuple(t_KB.shape) != (K, self.B) \
                 or tuple(out_KBCT.shape) != (K, self.B, self.Co, self.T):

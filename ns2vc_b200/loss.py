@@ -9,17 +9,22 @@ one deterministic reduction (``csrc/loss.cu``).  Eval mode only: ``Pre_model.for
 The loss of a row is the mean over all ``C x T`` elements of the PADDED row, as in the reference (past a row's length the target
 is 0 and the prediction is whatever the network emits there).  Inputs must be finite: the length mask is a 0/1 factor, as in the
 reference, so a non-finite value past a length turns the row into NaN.
+
+``utterance_losses`` is the per-utterance reading: each utterance's loss is what ``forward`` returns for that utterance alone as an
+unpadded B = 1 batch, whatever batch it is evaluated in.  It runs ragged batches (the ragged encoders, the ragged denoiser program
+and a reduction over each row's own length), on one GPU or over the ranks of a process group.
 """
 from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import torch
+import torch.distributed as dist
 
-from . import _lib, coefs
-from .api import sequence_mask
+from . import _lib, coefs, shard
+from .api import batch_plan, pad_batch, sequence_mask
 from .fused import check_lengths, get_session
 from .unet import UNet1DConditionModel
 
@@ -105,6 +110,44 @@ def mse_rows(out: torch.Tensor, target: torch.Tensor, t: torch.Tensor, timesteps
     return loss_row, loss_weighted, loss
 
 
+def mse_rows_ragged(out: torch.Tensor, target: torch.Tensor, lengths, t: torch.Tensor, timesteps: int = 1000,
+                    min_snr_gamma: Optional[float] = None, ws: Optional[torch.Tensor] = None):
+    """The per-utterance reduction of a ragged batch: out [K, B, C, T], target [B, C, T] or [K, B, C, T] and t [K, B] int64 on one
+    CUDA device, ``lengths`` B host ints (or a tensor) in [1, T] -> (loss_row [K, B], loss_weighted [K, B]): the mean of
+    (out - target)^2 over row b's own C x T_b elements and that times ``loss_weight[t]``.  Nothing past a length is read, and a row's
+    bits depend on (C, T_b) only (see ``ns2vc_mse_rows_ragged``).  ``ws``: scratch to reuse (uint8, 8-byte aligned)."""
+    if out.dim() != 4:
+        raise ValueError(f"out must be [K, B, C, T], got {tuple(out.shape)}")
+    K, B, Cl, T = out.shape
+    if tuple(target.shape) not in ((B, Cl, T), (K, B, Cl, T)):
+        raise ValueError(f"target must be [{B}, {Cl}, {T}] or [{K}, {B}, {Cl}, {T}], got {tuple(target.shape)}")
+    if not torch.is_tensor(t) or t.dtype != torch.int64 or tuple(t.shape) != (K, B):
+        raise ValueError(f"t must be an int64 tensor [{K}, {B}]")
+    lens = check_lengths(lengths, B, T, "lengths")
+    for name, v in (("out", out), ("target", target), ("t", t)):
+        if not v.is_cuda or not v.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous CUDA tensor (no CPU path)")
+    if out.dtype != torch.float32 or target.dtype != torch.float32 or target.device != out.device or t.device != out.device:
+        raise ValueError("out and target must be fp32, and out, target and t on one device")
+    dev = out.device
+    L = _lib.lib()
+    need = C.c_size_t()
+    _lib.check(L.ns2vc_mse_ragged_workspace_bytes(K, B, Cl, T, C.byref(need)))
+    if ws is None:
+        ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+    elif ws.numel() < need.value:
+        raise ValueError(f"workspace of {ws.numel()} bytes, {need.value} needed")
+    len_d = torch.tensor(lens, dtype=torch.int64).to(dev, non_blocking=True)
+    loss_row = torch.empty((K, B), dtype=torch.float32, device=dev)
+    loss_weighted = torch.empty((K, B), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(L.ns2vc_mse_rows_ragged(out.data_ptr(), target.data_ptr(), int(target.dim() == 4), len_d.data_ptr(), t.data_ptr(),
+                                           _loss_buffers(timesteps, dev)["loss_weight"].data_ptr(), timesteps,
+                                           float(min_snr_gamma) if min_snr_gamma is not None else 0.0, loss_row.data_ptr(),
+                                           loss_weighted.data_ptr(), K, B, Cl, T, ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    return loss_row, loss_weighted
+
+
 def _check_args(unet, data, t, noise, timesteps, min_snr_gamma):
     """Host-side argument checks; returns (B, C, T, S)."""
     if len(data) != 8:
@@ -188,3 +231,164 @@ def loss_profile(pre_model, unet: UNet1DConditionModel, data, t_grid=range(0, 10
     B = data[3].shape[0]
     t = torch.tensor(grid, dtype=torch.int64)[:, None].expand(len(grid), B).contiguous()
     return diffusion_loss(pre_model, unet, data, t=t, noise=noise, timesteps=timesteps, min_snr_gamma=min_snr_gamma)
+
+
+# ------------------------------------------------------------------------------------------------ per-utterance (ragged) objective
+HOP = 256                # mel hop of 24 kHz audio: the cost rows of shard.plan_batches count 24 kHz samples (convert.frame_plan)
+
+
+@dataclass
+class UtteranceLosses:
+    """``loss``: each utterance's ``loss_weight[t] * mse``, [N] (or [K, N] for a ``t_grid`` of K timesteps); ``mse``: the
+    unweighted mean over the utterance's own 100 x T_i elements, same shape; ``t``: the timesteps, same shape, int64.  On the
+    models' device, in input order."""
+    loss: torch.Tensor
+    mse: torch.Tensor
+    t: torch.Tensor
+
+
+@torch.no_grad()
+def batch_utterance_losses(pre_model, unet: UNet1DConditionModel, c_padded: torch.Tensor, refer_padded: torch.Tensor,
+                           spec_padded: torch.Tensor, lengths, refer_lengths, t: torch.Tensor, noise: torch.Tensor,
+                           timesteps: int = 1000, min_snr_gamma: Optional[float] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """One ragged batch: c_padded [B, 256, T], refer_padded [B, 100, S], spec_padded [B, 100, T] fp32, t [K, B] int64 and noise
+    [B, 100, T] (shared by every k) or [K, B, 100, T], all on the models' device; lengths / refer_lengths: B host ints.  Returns
+    (mse [K, B], loss [K, B]); row b is utterance b's objective alone, and values past its lengths are never read.
+
+    ``Pre_model.infer(per_utterance=True)`` -> ``q_sample`` (masked by ``lengths``) -> the ragged session's
+    ``eval_x_start_ragged`` -> ``mse_rows_ragged``."""
+    dev = spec_padded.device
+    B, _, T = spec_padded.shape
+    S = refer_padded.shape[2]
+    tl = torch.tensor(check_lengths(lengths, B, T, "lengths"), dtype=torch.int64)
+    sl = torch.tensor(check_lengths(refer_lengths, B, S, "refer_lengths"), dtype=torch.int64)
+    content, prompt = pre_model.infer((c_padded, refer_padded, None, None, None, tl, sl, None), per_utterance=True)
+    x_start, x = q_sample(spec_padded, noise, tl.to(dev, non_blocking=True), t, timesteps)
+    sess = get_session(unet, content.permute(1, 2, 0), prompt.permute(1, 0, 2), None, content_lengths=tl, prompt_lengths=sl)
+    model_out = sess.eval_x_start_ragged(x, t, torch.empty_like(x))
+    mse, loss = mse_rows_ragged(model_out, x_start, tl, t, timesteps, min_snr_gamma)
+    return mse, loss
+
+
+def _check_items(unet, items, t, t_grid, noise, max_batch, timesteps, min_snr_gamma) -> Tuple[List[int], List[int], Optional[List[int]]]:
+    """Host-side argument checks of ``utterance_losses``; returns (T_i, S_i, the grid or None)."""
+    if len(items) == 0:
+        raise ValueError("items is empty")
+    Cl = unet.latent_channels
+    if unet.cfg.out_channels != Cl:
+        raise ValueError("the x_start objective needs a denoiser with out_channels equal to its latent channels")
+    tl, sl = [], []
+    for i, it in enumerate(items):
+        if not isinstance(it, (tuple, list)) or len(it) != 3 or not all(torch.is_tensor(v) for v in it):
+            raise ValueError(f"utterance {i}: expected a (c [C, T_i], spec [{Cl}, T_i], refer [C, S_i]) tuple of tensors")
+        c, spec, refer = it
+        if spec.dim() != 2 or spec.shape[0] != Cl or c.dim() != 2 or c.shape[1] != spec.shape[1] or refer.dim() != 2:
+            raise ValueError(f"utterance {i}: expected c [C, T_i], spec [{Cl}, T_i] and refer [C, S_i], got {tuple(c.shape)}, "
+                             f"{tuple(spec.shape)}, {tuple(refer.shape)}")
+        if spec.shape[1] < 1 or refer.shape[1] < 1:
+            raise ValueError(f"utterance {i}: T_i = {spec.shape[1]} and S_i = {refer.shape[1]} must be >= 1")
+        if c.shape[0] != items[0][0].shape[0] or refer.shape[0] != items[0][2].shape[0]:
+            raise ValueError(f"utterance {i}: channel counts differ from utterance 0's")
+        tl.append(int(spec.shape[1]))
+        sl.append(int(refer.shape[1]))
+    N = len(items)
+    if int(max_batch) < 1:
+        raise ValueError("max_batch must be >= 1")
+    if int(timesteps) < 1:
+        raise ValueError("timesteps must be >= 1")
+    if min_snr_gamma is not None and not float(min_snr_gamma) > 0:
+        raise ValueError("min_snr_gamma must be positive")
+    if t is not None and t_grid is not None:
+        raise ValueError("pass t (one timestep per utterance) or t_grid (the same K timesteps for every utterance), not both")
+    if t is not None:
+        if not torch.is_tensor(t) or t.dtype != torch.int64 or tuple(t.shape) != (N,):
+            raise ValueError(f"t must be an int64 tensor [{N}]")
+        if int(t.min()) < 0 or int(t.max()) >= timesteps:
+            raise ValueError(f"t must lie in [0, {timesteps})")
+    grid = None
+    if t_grid is not None:
+        grid = [int(v) for v in t_grid]
+        if not grid:
+            raise ValueError("t_grid is empty")
+        if min(grid) < 0 or max(grid) >= timesteps:
+            raise ValueError(f"t_grid must lie in [0, {timesteps})")
+        if len(grid) * min(int(max_batch), N) > 65535:
+            raise ValueError(f"t_grid of {len(grid)} points times max_batch rows exceeds 65535 evaluations per batch")
+    if noise is not None:
+        if len(noise) != N:
+            raise ValueError(f"{len(noise)} noise tensors for {N} utterances")
+        for i, (nz, T) in enumerate(zip(noise, tl)):
+            if not torch.is_tensor(nz) or tuple(nz.shape) != (Cl, T):
+                raise ValueError(f"noise {i}: expected [{Cl}, {T}], got {tuple(nz.shape) if torch.is_tensor(nz) else nz!r}")
+    return tl, sl, grid
+
+
+@torch.no_grad()
+def utterance_losses(pre_model, unet: UNet1DConditionModel, items: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]],
+                     t: Optional[torch.Tensor] = None, t_grid=None, noise: Optional[Sequence[torch.Tensor]] = None, max_batch: int = 8,
+                     group: Optional[dist.ProcessGroup] = None, timesteps: int = 1000,
+                     min_snr_gamma: Optional[float] = None) -> UtteranceLosses:
+    """Each utterance's own training objective: for ``items[i] = (c [256, T_i], spec [100, T_i], refer [100, S_i])`` the number
+    ``NaturalSpeech2.forward`` (reference model.py:706-734) returns for the unpadded B = 1 batch ``(c[None], refer[None], ...,
+    spec[None], lengths=[T_i], refer_lengths=[S_i])``: ``loss_weight[t] * mean((model_out - spec)^2)`` over its 100 x T_i
+    elements.  Unlike ``diffusion_loss`` on a padded batch, the value does not depend on the batch the utterance is evaluated in,
+    so it compares checkpoints on a held-out set, profiles the schedule per utterance, or ranks a corpus by fit.
+
+    ``t``: int64 [N], one timestep per utterance; ``t_grid``: K timesteps evaluated for every utterance with one noise tensor per
+    utterance shared by the grid (results [K, N]); neither: one drawn timestep each.  ``noise``: one [100, T_i] per utterance, or
+    None.  Default draws, per utterance in input order on the device's default generator: ``torch.randint(0, timesteps, (1,))``
+    when ``t`` and ``t_grid`` are None, then ``torch.randn_like(spec_i[None])`` when ``noise`` is None - the draws of the loop
+    ``for i: diffusion_loss(pre_model, unet, unpadded_batch_i)``, so after the same ``torch.manual_seed`` both give the same
+    values and leave the generator in the same state, whatever ``max_batch`` and ``group``.
+
+    The utterances run in ragged batches of at most ``max_batch`` (``api.batch_plan``, longest first): ``batch_utterance_losses``.
+    With a process ``group`` of more than one rank (one process per GPU, every rank making the same call with its models on its
+    own device), the batches are shared out by ``shard.plan_batches``, run by ``shard.run_sharded`` and all-gathered once; every
+    rank draws the defaults for all utterances, so every rank returns the one-GPU result and ends with the same generator state."""
+    tl, sl, grid = _check_items(unet, items, t, t_grid, noise, max_batch, timesteps, min_snr_gamma)
+    dev = next(unet.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("utterance_losses needs the models on a CUDA device (no CPU path)")
+    N, Cl = len(items), unet.latent_channels
+    sharded = group is not None and dist.get_world_size(group) > 1
+    if sharded and (t is None and grid is None or noise is None):
+        shard.check_generator(torch.cuda.default_generators[dev.index], group, dev)
+    # the default draws, utterance by utterance in input order (every rank draws all of them)
+    t_u = [None] * N if t is None else list(t.to(dev))
+    noise_u = [None] * N if noise is None else list(noise)
+    for i in range(N):
+        if t is None and grid is None:
+            t_u[i] = torch.randint(0, timesteps, (1,), device=dev).long()[0]
+        if noise is None:
+            noise_u[i] = torch.randn((1, Cl, tl[i]), device=dev)[0]
+    if grid is not None:
+        t_all = torch.tensor(grid, dtype=torch.int64, device=dev)[:, None].expand(len(grid), N).contiguous()
+    else:
+        t_all = torch.stack(t_u)[None].contiguous()
+    K = t_all.shape[0]
+
+    def work(idx: List[int]) -> List[torch.Tensor]:
+        spec, c, refer, _, _ = pad_batch([(items[i][1], items[i][0].t(), items[i][2].t()) for i in idx], range(len(idx)))
+        f32 = lambda v: v.to(dev, torch.float32, non_blocking=True).contiguous()
+        nz = torch.zeros((len(idx), Cl, max(tl[i] for i in idx)), dtype=torch.float32, device=dev)
+        for j, i in enumerate(idx):
+            nz[j, :, :tl[i]] = noise_u[i]
+        mse, loss = batch_utterance_losses(pre_model, unet, f32(c.permute(1, 2, 0)), f32(refer.permute(1, 2, 0)), f32(spec),
+                                           [tl[i] for i in idx], [sl[i] for i in idx], t_all[:, idx].contiguous(), nz, timesteps,
+                                           min_snr_gamma)
+        both = torch.stack([mse, loss])                                      # [2, K, B]
+        return [both[:, :, j] for j in range(len(idx))]
+
+    if sharded:
+        world = dist.get_world_size(group)
+        plan = shard.plan_batches([dict(n24=T * HOP, T=T) for T in tl], sl, world, int(max_batch))
+        rows = shard.run_sharded(work, plan, [(2, K)] * N, group, dev)
+    else:
+        rows: List[Optional[torch.Tensor]] = [None] * N
+        for idx in batch_plan(tl, int(max_batch)):
+            for i, r in zip(idx, work(idx)):
+                rows[i] = r
+    both = torch.stack([r.to(dev) for r in rows], dim=-1)                   # [2, K, N]
+    if grid is None:
+        return UtteranceLosses(loss=both[1, 0], mse=both[0, 0], t=t_all[0])
+    return UtteranceLosses(loss=both[1], mse=both[0], t=t_all)

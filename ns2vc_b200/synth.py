@@ -136,6 +136,15 @@ def make_pre_inputs(B: int, T: int, S: int, content_ch: int = 256, ragged: bool 
     return dict(c=c, refer=refer, lengths=lengths, refer_lengths=refer_lengths)
 
 
+def make_utterance_loss_inputs(T: int, S: int, seed: int) -> Dict[str, torch.Tensor]:
+    """One utterance of the per-utterance objective: c [256, T] and refer [100, S] (``make_pre_inputs`` at B = 1), the target
+    mel spec [100, T] ~ N(0,1) (seed+1) and the noise [100, T] ~ N(0,1) (seed+2)."""
+    pin = make_pre_inputs(1, T, S, seed=seed)
+    spec = torch.randn((1, 100, T), generator=torch.Generator().manual_seed(seed + 1))
+    noise = torch.randn((1, 100, T), generator=torch.Generator().manual_seed(seed + 2))
+    return dict(c=pin["c"][0], refer=pin["refer"][0], spec=spec[0], noise=noise[0])
+
+
 def state_dict_checksum(sd: Dict[str, torch.Tensor]) -> str:
     h = hashlib.sha256()
     for k in sorted(sd):
