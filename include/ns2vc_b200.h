@@ -443,6 +443,12 @@ typedef struct ns2vc_check_gemm_args {
   int pre_mode;                      /* 1: x * scale + shift, 2: then SiLU */
   int pre_C;
   int ksplit;                        /* panel mode: 1 or 2 CTAs per tile */
+  /* panel mode without pre_scale: the GroupNorm (mode pre_mode) of gn_C1 + gn_C2 channels in gn_G groups over T_out rows (row_len:
+     each entry's own rows) from per-(entry, channel) sums gn_stats1 [2][B][gn_C1] | gn_stats2 [2][B][gn_C2] (sums, then sums of
+     squares, as EPI_STATS writes them; NULL: no second source), with FiLM rows gn_film [B, gn_film_ld] (scale | shift) or NULL -
+     the descriptor the denoiser builds */
+  const double* gn_stats1; const double* gn_stats2; int gn_C1, gn_C2, gn_G; float gn_eps;
+  const float* gn_gamma; const float* gn_beta; const float* gn_film; int gn_film_ld;
 } ns2vc_check_gemm_args;
 typedef struct ns2vc_check_attn_args {
   int B, H, Tq, Tk, dh;
@@ -461,6 +467,76 @@ int ns2vc_check_pack_b(const float* w, int n_rows, int cin_total, int ktaps, int
                        int geglu_half, const float* cscale, void* w_hi, void* w_lo, int Npad, int nkb_total, ns2vc_stream stream);
 int ns2vc_check_gemm(const ns2vc_check_gemm_args* args, char* desc, int desc_len, ns2vc_stream stream);
 int ns2vc_check_attention(const ns2vc_check_attn_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* One activation prep (prep_split_kernel): concat(src1, src2) rows remapped -> [affine (+ SiLU)] -> split `out` (+ the untransformed
+ * split `raw`).  The affine is either given (scale / shift) or the GroupNorm (+ FiLM) of the sums, as the denoiser builds it. */
+typedef struct ns2vc_check_prep_args {
+  const float* src1; int ld1, C1;
+  const float* src2; int ld2, C2;    /* NULL / 0: no concat */
+  int B, T_src, T_dst;
+  int row_mul, row_add;              /* source row of output row t: rowmap ? rowmap[t] : t * row_mul + row_add */
+  const int* rowmap;                 /* [T_dst] or NULL; with row_len: the nearest-upsample rule of each entry's own lengths */
+  int mode;                          /* 0: raw, 1: affine, 2: affine then SiLU */
+  const float* scale; const float* shift; /* [B, C1 + C2], or NULL: GroupNorm from stats1 / stats2 */
+  const double* stats1; const double* stats2; /* [2][B][C1] / [2][B][C2]: sums, then sums of squares, over T_src rows */
+  const float* gamma; const float* beta; int G; float eps;
+  const float* film; int film_ld;    /* [B, film_ld]: scale at [b, c], shift at [b, C1 + C2 + c]; or NULL */
+  ns2vc_check_split out, raw;        /* raw.hi NULL: no raw output */
+  const int* row_len; int len_shift; /* ragged: level-0 lengths [B] or NULL */
+} ns2vc_check_prep_args;
+int ns2vc_check_prep(const ns2vc_check_prep_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* One LayerNorm launch of M rows of C channels (pitch ld): kind 0 ln_split (into `split`; keep: rows whose factor is 0 are stored
+ * as zeros, or NULL), 1 ln_apply (into y), 2 ln_mask (into y, times keep). */
+typedef struct ns2vc_check_ln_args {
+  int kind;
+  const float* x; int ld, M, C; float eps;
+  const float* gamma; const float* beta;
+  const float* keep;
+  float* y; int y_ld;
+  ns2vc_check_split split;
+} ns2vc_check_ln_args;
+int ns2vc_check_ln(const ns2vc_check_ln_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* One voc_norm_kernel launch: LayerNorm of token-major [B, T, C] rows, after the 7-tap depthwise conv dw ([C][8]: taps, bias) or
+ * not (NULL), rows at or past len[b] (int64, or NULL) zero; into out and / or split. */
+typedef struct ns2vc_check_voc_norm_args {
+  const float* x; int B, T, C;
+  const float* dw; const float* gamma; const float* beta; float eps;
+  const int64_t* len;
+  float* out; ns2vc_check_split split;
+} ns2vc_check_voc_norm_args;
+int ns2vc_check_voc_norm(const ns2vc_check_voc_norm_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* One small linear: out[m, n] = f(x[m, :]) . W[n, :] + bias[n] (+ add[m % add_rows (add_rows > 0) or m, n]) (then SiLU);
+ * in_mode 0: x, 1: SiLU(x), 2: the K-wide sinusoid of t = x[m * x_ld]. */
+typedef struct ns2vc_check_linear_args {
+  const float* x; int x_ld, M, K;
+  const float* W; const float* bias; int N;
+  const float* add; int add_ld, add_rows;
+  float* out; int out_ld;
+  int in_mode, flip_sin_to_cos; float freq_shift; int out_silu;
+} ns2vc_check_linear_args;
+int ns2vc_check_small_linear(const ns2vc_check_linear_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* AttentionPooling pieces: with `tokens`, the class token (mean of x's first lens[b] or S rows + pos) and the copied rows; with
+ * `out`, the attention of q [B, C] over kv [B, S + 1, 2C] (k | v) in `heads` heads (wide: the any-width kernel). */
+typedef struct ns2vc_check_pool_args {
+  const float* x; const float* pos; int B, S, C;
+  float* tokens;
+  const float* q; const float* kv; int heads, wide;
+  float* out;
+  const int* lens;
+} ns2vc_check_pool_args;
+int ns2vc_check_pool(const ns2vc_check_pool_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* [B, C, T] fp32 (batch stride bstride) -> split token-major [B, T, out.ld]; frames past row_len[b] (or NULL) are zeros. */
+typedef struct ns2vc_check_nct_split_args {
+  const float* x; long long bstride; int B, C, T;
+  ns2vc_check_split out;
+  const int* row_len;
+} ns2vc_check_nct_split_args;
+int ns2vc_check_nct_split(const ns2vc_check_nct_split_args* args, char* desc, int desc_len, ns2vc_stream stream);
 
 #ifdef __cplusplus
 }

@@ -420,10 +420,7 @@ struct Builder : ProgramBuilder {
     PrepOp p; memset(&p, 0, sizeof(p));
     p.C1 = C1; p.C2 = C2; p.B = B; p.T_src = Tn; p.T_dst = Tn; p.mode = mode;
     p.row_len = rag_lens; p.len_shift = level;
-    p.gn.sum1 = st1; p.gn.sq1 = st1 ? st1 + (size_t)B * C1 : nullptr;
-    p.gn.sum2 = st2; p.gn.sq2 = st2 ? st2 + (size_t)B * C2 : nullptr;
-    p.gn.gamma = gamma; p.gn.beta = beta; p.gn.film_ld = film_ld; p.gn.G = h->cfg.norm_num_groups; p.gn.eps = eps;
-    p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / p.gn.G));
+    set_group_norm(p, B, st1, C1, st2, C2, Tn, h->cfg.norm_num_groups, eps, gamma, beta, nullptr, film_ld);
     // all descriptors of a program sit in one workspace array and go to the device in ONE copy when the program is complete
     if ((int)aff_host.size() >= aff_cap) { err = -1; set_error("internal: affine descriptor table full"); return nullptr; }
     aff_host.push_back(p);
@@ -454,10 +451,7 @@ struct Builder : ProgramBuilder {
     emit_prep(s1, C1, s2, C2, Tn, Tn, mode, nullptr, nullptr, o, raw);
     PrepOp& p = out->back().get<PrepOp>();
     if (film) out->back().reads_film = 1;
-    p.gn.sum1 = st1; p.gn.sq1 = st1 ? st1 + (size_t)B * C1 : nullptr;
-    p.gn.sum2 = st2; p.gn.sq2 = st2 ? st2 + (size_t)B * C2 : nullptr;
-    p.gn.gamma = gamma; p.gn.beta = beta; p.gn.film = film; p.gn.film_ld = film_ld; p.gn.G = h->cfg.norm_num_groups; p.gn.eps = eps;
-    p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / p.gn.G));
+    set_group_norm(p, B, st1, C1, st2, C2, Tn, h->cfg.norm_num_groups, eps, gamma, beta, film, film_ld);
   }
 };
 

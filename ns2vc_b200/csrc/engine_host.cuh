@@ -331,6 +331,18 @@ struct ProgramBuilder {
   }
 };
 
+// The GroupNorm part of a prep descriptor over Tn rows of B entries: statistics of up to two concatenated producers (st1 / st2:
+// [B, C] sums | [B, C] sums of squares, as the producers' EPI_STATS epilogues lay them out; st2 nullptr without a concat), the
+// norm's weights, the FiLM rows (nullptr: none; the panel-mode GEMM passes its own as GemmOp::pre_film) and the group count.
+// The engines and the kernel checks fill every GroupNorm descriptor through this.
+inline void set_group_norm(PrepOp& p, int B, const double* st1, int C1, const double* st2, int C2, int Tn, int G, float eps,
+                           const float* gamma, const float* beta, const float* film, int film_ld) {
+  p.gn.sum1 = st1; p.gn.sq1 = st1 ? st1 + (size_t)B * C1 : nullptr;
+  p.gn.sum2 = st2; p.gn.sq2 = st2 ? st2 + (size_t)B * C2 : nullptr;
+  p.gn.gamma = gamma; p.gn.beta = beta; p.gn.film = film; p.gn.film_ld = film_ld; p.gn.G = G; p.gn.eps = eps;
+  p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / G));
+}
+
 inline LinOp linear_op(const float* x, int x_ld, int M, int K, const float* W, const float* bias, int N, float* y, int y_ld) {
   LinOp o; memset(&o, 0, sizeof(o));
   o.x = x; o.x_ld = x_ld; o.M = M; o.K = K; o.W = W; o.bias = bias; o.N = N; o.out = y; o.out_ld = y_ld;

@@ -1,8 +1,9 @@
-// Test-only entry points into the product launchers: one weight packing, one wgmma GEMM and one flash attention, each
-// described by a flat C struct (include/ns2vc_b200.h, "kernel checks") and run through exactly the host code the engines use
-// (pack_seg, the ProgramBuilder helpers, plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention
-// dispatch).  tests/test_kernels_fp64.py drives them at the shapes and edges the models never reach.  Nothing here is a
-// kernel: every launch is the product's own.
+// Test-only entry points into the product launchers: one weight packing, one wgmma GEMM, one flash attention, one activation
+// prep, one LayerNorm, one small linear, the AttentionPooling pieces and one [B, C, T] -> split conversion, each described by a
+// flat C struct (include/ns2vc_b200.h, "kernel checks") and run through exactly the host code the engines use (pack_seg, the
+// ProgramBuilder helpers, set_group_norm, linear_op, plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the
+// attention dispatch, the launchers of common.cuh).  tests/test_kernels_fp64.py and tests/test_norm_kernels_fp64.py drive them
+// at the shapes and edges the models never reach.  Nothing here is a kernel: every launch is the product's own.
 #include "engine_host.cuh"
 #include "../../include/ns2vc_b200.h"
 
@@ -92,12 +93,27 @@ int ns2vc_check_gemm(const ns2vc_check_gemm_args* a, char* desc, int desc_len, n
 
   cudaStream_t st = (cudaStream_t)stream;
   PrepOp* pre_dev = nullptr;
-  if (g.xmode && a->pre_scale) {
-    NS_REQUIRE(a->pre_shift && a->pre_C >= 1 && a->pre_C <= kXfMaxC, "check_gemm: panel affine needs scale, shift and 1..%d channels", kXfMaxC);
+  if (g.xmode && (a->pre_scale || a->gn_stats1)) {
     NS_REQUIRE(a->pre_mode == PREP_AFFINE || a->pre_mode == PREP_AFFINE_SILU, "check_gemm: panel affine mode %d", a->pre_mode);
     PrepOp p; memset(&p, 0, sizeof(p));
-    p.C1 = a->pre_C; p.B = a->B; p.T_src = a->T_out; p.T_dst = a->T_out; p.mode = a->pre_mode;
-    p.scale = a->pre_scale; p.shift = a->pre_shift;
+    p.B = a->B; p.T_src = a->T_out; p.T_dst = a->T_out; p.mode = a->pre_mode;
+    if (a->pre_scale) {
+      NS_REQUIRE(a->pre_shift && a->pre_C >= 1 && a->pre_C <= kXfMaxC, "check_gemm: panel affine needs scale, shift and 1..%d channels", kXfMaxC);
+      p.C1 = a->pre_C;
+      p.scale = a->pre_scale; p.shift = a->pre_shift;
+    } else {
+      // the GroupNorm descriptor as the denoiser's affine_desc builds it; the FiLM rows travel in GemmOp::pre_film
+      const int Cg = a->gn_C1 + a->gn_C2;
+      NS_REQUIRE(a->gn_C1 >= 1 && a->gn_C2 >= 0 && (a->gn_C2 == 0) == (a->gn_stats2 == nullptr) && Cg <= kXfMaxC,
+                 "check_gemm: GroupNorm sources %d + %d channels (up to %d)", a->gn_C1, a->gn_C2, kXfMaxC);
+      NS_REQUIRE(a->gn_G >= 1 && a->gn_G <= 64 && Cg % a->gn_G == 0 && a->gn_gamma && a->gn_beta,
+                 "check_gemm: GroupNorm of %d channels in %d groups", Cg, a->gn_G);
+      NS_REQUIRE(!a->gn_film || a->gn_film_ld >= 2 * Cg, "check_gemm: FiLM rows of %d < %d", a->gn_film_ld, 2 * Cg);
+      p.C1 = a->gn_C1; p.C2 = a->gn_C2;
+      set_group_norm(p, a->B, a->gn_stats1, a->gn_C1, a->gn_stats2, a->gn_C2, a->T_out, a->gn_G, a->gn_eps, a->gn_gamma, a->gn_beta,
+                     nullptr, a->gn_film_ld);
+      g.pre_film = a->gn_film;
+    }
     p.row_len = a->row_len; p.len_shift = a->len_shift;
     NS_CHECK_CUDA(cudaMallocAsync((void**)&pre_dev, sizeof(PrepOp), st));
     NS_CHECK_CUDA(cudaMemcpyAsync(pre_dev, &p, sizeof(PrepOp), cudaMemcpyHostToDevice, st));
@@ -145,6 +161,116 @@ int ns2vc_check_attention(const ns2vc_check_attn_args* a, char* desc, int desc_l
   if (rc) return rc;
   const int dhp = a->dh <= 16 ? 16 : a->dh <= 32 ? 32 : a->dh <= 48 ? 48 : 64;
   report(desc, desc_len, "attn_tc<%d>", dhp);
+  return 0;
+}
+
+int ns2vc_check_prep(const ns2vc_check_prep_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a, "check_prep: null argument");
+  NS_REQUIRE(a->B >= 1 && a->T_src >= 1 && a->T_dst >= 1 && a->C1 >= 1 && a->C2 >= 0 && a->src1 && (a->C2 == 0 || a->src2),
+             "check_prep: bad sizes B=%d T=%d->%d C=%d+%d", a->B, a->T_src, a->T_dst, a->C1, a->C2);
+  NS_REQUIRE(a->out.hi && a->out.lo, "check_prep: no output");
+  NS_REQUIRE(a->mode >= PREP_RAW && a->mode <= PREP_AFFINE_SILU, "check_prep: mode %d", a->mode);
+  PrepOp p; memset(&p, 0, sizeof(p));
+  p.src1 = a->src1; p.ld1 = a->ld1; p.C1 = a->C1; p.src2 = a->src2; p.ld2 = a->ld2; p.C2 = a->C2;
+  p.B = a->B; p.T_src = a->T_src; p.T_dst = a->T_dst;
+  p.row_mul = a->row_mul; p.row_add = a->row_add; p.rowmap = a->rowmap; p.mode = a->mode;
+  p.out = to_split(a->out);
+  if (a->raw.hi) p.raw = to_split(a->raw);
+  p.row_len = a->row_len; p.len_shift = a->len_shift;
+  if (a->mode != PREP_RAW) {
+    if (a->scale) {
+      NS_REQUIRE(a->shift, "check_prep: scale without shift");
+      p.scale = a->scale; p.shift = a->shift;
+    } else {
+      NS_REQUIRE(a->stats1 && (a->C2 == 0 || a->stats2) && a->gamma && a->beta && a->G >= 1, "check_prep: GroupNorm without its sums or weights");
+      set_group_norm(p, a->B, a->stats1, a->C1, a->C2 ? a->stats2 : nullptr, a->C2, a->T_src, a->G, a->eps, a->gamma, a->beta, a->film,
+                     a->film_ld);
+    }
+  }
+  const int rc = launch_prep_split(p, (cudaStream_t)stream);
+  if (rc) return rc;
+  report(desc, desc_len, "prep_split<RAG=%d>", p.row_len ? 1 : 0);
+  return 0;
+}
+
+int ns2vc_check_ln(const ns2vc_check_ln_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->x && a->gamma && a->beta, "check_ln: null argument");
+  NS_REQUIRE(a->M >= 1 && a->C >= 1 && a->ld >= a->C, "check_ln: bad sizes M=%d C=%d ld=%d", a->M, a->C, a->ld);
+  LnOp op{a->x, a->ld, a->M, a->C, a->eps, a->gamma, a->beta, a->keep, a->y, a->y_ld, to_split(a->split)};
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  switch (a->kind) {
+    case 0:
+      NS_REQUIRE(op.split.hi && op.split.lo, "check_ln: ln_split without a split output");
+      if ((rc = launch_ln_split(op, st))) return rc;
+      report(desc, desc_len, "ln_split<KEEP=%d>", op.keep ? 1 : 0);
+      return 0;
+    case 1:
+      NS_REQUIRE(op.y, "check_ln: ln_apply without an output");
+      if ((rc = launch_ln_apply(op, st))) return rc;
+      report(desc, desc_len, "%s", "ln_apply");
+      return 0;
+    case 2:
+      NS_REQUIRE(op.y && op.keep, "check_ln: ln_mask without an output or keep factors");
+      if ((rc = launch_ln_mask(op, st))) return rc;
+      report(desc, desc_len, "%s", "ln_mask");
+      return 0;
+  }
+  set_error("check_ln: kind %d", a->kind);
+  return -1;
+}
+
+int ns2vc_check_voc_norm(const ns2vc_check_voc_norm_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->x && a->gamma && a->beta, "check_voc_norm: null argument");
+  NS_REQUIRE(a->B >= 1 && a->T >= 1 && a->C >= 128 && a->C <= 1024 && a->C % 128 == 0, "check_voc_norm: bad sizes B=%d T=%d C=%d", a->B,
+             a->T, a->C);
+  NS_REQUIRE(a->out || (a->split.hi && a->split.lo), "check_voc_norm: no output");
+  VocNormOp op{a->x, a->B, a->T, a->C, a->dw, a->gamma, a->beta, a->eps, (const long long*)a->len, a->out, to_split(a->split)};
+  const int rc = launch_voc_norm(op, (cudaStream_t)stream);
+  if (rc) return rc;
+  report(desc, desc_len, "voc_norm<DW=%d>", a->dw ? 1 : 0);
+  return 0;
+}
+
+int ns2vc_check_small_linear(const ns2vc_check_linear_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->x && a->W && a->out, "check_small_linear: null argument");
+  NS_REQUIRE(a->M >= 1 && a->K >= 1 && a->N >= 1 && a->in_mode >= LIN_RAW && a->in_mode <= LIN_SINUSOID,
+             "check_small_linear: bad sizes M=%d K=%d N=%d mode %d", a->M, a->K, a->N, a->in_mode);
+  LinOp op = linear_op(a->x, a->x_ld, a->M, a->K, a->W, a->bias, a->N, a->out, a->out_ld);
+  op.add = a->add; op.add_ld = a->add_ld; op.add_rows = a->add_rows;
+  op.in_mode = a->in_mode; op.flip_sin_to_cos = a->flip_sin_to_cos; op.freq_shift = a->freq_shift; op.out_silu = a->out_silu;
+  const int rc = launch_small_linear(op, (cudaStream_t)stream);
+  if (rc) return rc;
+  report(desc, desc_len, "%s", "small_linear");
+  return 0;
+}
+
+int ns2vc_check_pool(const ns2vc_check_pool_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && (a->tokens || a->out), "check_pool: nothing to launch");
+  NS_REQUIRE(a->B >= 1 && a->S >= 1 && a->C >= 1, "check_pool: bad sizes B=%d S=%d C=%d", a->B, a->S, a->C);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (a->tokens) {
+    NS_REQUIRE(a->x && a->pos, "check_pool: class token without input");
+    if ((rc = launch_pool_class_token(PoolClsOp{a->x, a->pos, a->B, a->S, a->C, a->tokens, a->lens}, st))) return rc;
+  }
+  if (a->out) {
+    NS_REQUIRE(a->q && a->kv && a->heads >= 1, "check_pool: attention without q / kv");
+    const PoolAttOp op{a->q, a->kv, a->B, a->S + 1, a->C, a->heads, a->out, a->lens};
+    if ((rc = a->wide ? launch_pool_attend_wide(op, st) : launch_pool_attend(op, st))) return rc;
+  }
+  report(desc, desc_len, "%s%s%s<RAG=%d>", a->tokens ? "pool_class_token" : "", a->tokens && a->out ? "+" : "",
+         a->out ? (a->wide ? "pool_attend_wide" : "pool_attend") : "", a->lens ? 1 : 0);
+  return 0;
+}
+
+int ns2vc_check_nct_split(const ns2vc_check_nct_split_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->x && a->out.hi && a->out.lo, "check_nct_split: null argument");
+  NS_REQUIRE(a->B >= 1 && a->C >= 1 && a->T >= 1 && a->out.ld >= a->C && a->out.ld % 8 == 0, "check_nct_split: bad sizes B=%d C=%d T=%d ld=%d",
+             a->B, a->C, a->T, a->out.ld);
+  const int rc = launch_nct_to_split(NctSplitOp{a->x, a->bstride, a->B, a->C, a->T, to_split(a->out), a->row_len, nullptr, 0}, (cudaStream_t)stream);
+  if (rc) return rc;
+  report(desc, desc_len, "nct_to_split<RAG=%d>", a->row_len ? 1 : 0);
   return 0;
 }
 

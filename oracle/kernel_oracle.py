@@ -288,3 +288,147 @@ def ratio(err: torch.Tensor, bound: torch.Tensor) -> float:
 def rule_ratio(got: torch.Tensor, ref: torch.Tensor) -> float:
     """max |got - ref| / rule_tol(ref) (<= 1 passes)"""
     return ratio(got.to(F64) - ref, rule_tol(ref))
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# GroupNorm / LayerNorm / timestep / pooling launches (tests/test_norm_kernels_fp64.py).  Each reference is the operation in
+# the dtype of its arguments: fp64 on the kernel's fp32 input is the truth, fp32 gives e32 (the floor of the parity rule).
+# ---------------------------------------------------------------------------------------------------------------------------
+def parity_tol(ref: torch.Tensor, e32: float) -> torch.Tensor:
+    """the parity rule of the model-level files: max(1e-3 |ref| + 1e-4 rms(ref), 2 e32), e32 = max |fp32 - fp64| of the same
+    operation on the same input"""
+    return torch.clamp(rule_tol(ref), min=2 * e32)
+
+
+def group_norm_rows(x: torch.Tensor, G: int, gamma, beta, eps: float, rows: Sequence[int], film: Optional[torch.Tensor] = None,
+                    silu: bool = False, one_plus: bool = True, count: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """GroupNorm of token-major x [B, T, C] over each entry's first rows[b] rows (nn.GroupNorm on the unpadded entry), then
+    x * (1 + scale) + shift of film [B, >= 2C] (scale | shift), then SiLU; rows past rows[b] are 0.  In x's dtype.
+    one_plus=False (FiLM scale without 1+) and count (the rows the statistics are divided by) are defects for the sensitivity checks."""
+    B, T, C = x.shape
+    out = torch.zeros_like(x)
+    for b in range(B):
+        n = int(rows[b])
+        xb = x[b, :n].T[None]                                          # [1, C, n]
+        if count is None:
+            y = torch.nn.functional.group_norm(xb, G, gamma.to(x.dtype), beta.to(x.dtype), eps)[0].T
+        else:
+            g = xb.reshape(G, -1)
+            k = int(count[b]) * (C // G)
+            mean = g.sum(-1, keepdim=True) / k
+            var = (g * g).sum(-1, keepdim=True) / k - mean * mean
+            y = ((g - mean) / torch.sqrt(var.clamp_min(0) + eps)).reshape(C, n).T * gamma.to(x.dtype) + beta.to(x.dtype)
+        if film is not None:
+            s, sh = film[b, :C].to(x.dtype), film[b, C:2 * C].to(x.dtype)
+            y = y * ((1 + s) if one_plus else s) + sh
+        if silu:
+            y = y * torch.sigmoid(y)
+        out[b, :n] = y
+    return out
+
+
+def one_pass_variance_term(x: torch.Tensor, G: int, gamma, rows: Sequence[int], film: Optional[torch.Tensor], eps: float,
+                           partial: int = 32) -> torch.Tensor:
+    """Bound of what the producers' statistics add to a GroupNorm output, per element.  The producing GEMM epilogue (EPI_STATS)
+    sums each column in fp32 over `partial` rows, then adds the partial sums in fp64: a partial of p terms is within
+    (p - 1) 2^-24 of the sum of their magnitudes (the standard summation bound), so with S1 = sum |x| and S2 = sum x^2 over a
+    group of n elements
+        |d mean| <= (p - 1) 2^-24 S1 / n,      |d q / n| <= (p - 1) 2^-24 S2 / n,
+    and the one-pass variance q / n - mean^2 is off by |d var| <= (p - 1) 2^-24 (S2 / n + 2 |mean| S1 / n) + d mean^2.  Relative
+    to var that is ~ 3 (p - 1) 2^-24 (1 + r^2) for r = |mean| / std (a worst case; random roundings give ~ 2^-24 r^2 sqrt(p / n)).
+    An output y = (x - mean) rstd gamma (1 + s) then moves by
+        |gamma (1 + s)| rstd (|d mean| + |x - mean| |d var| / (2 (var + eps))).
+    Rows past rows[b] get 0 (the kernels store exact zeros there)."""
+    B, T, C = x.shape
+    u = (partial - 1) * 2.0 ** -24
+    out = torch.zeros_like(x)
+    for b in range(B):
+        n = int(rows[b])
+        g = x[b, :n].T.reshape(G, -1)
+        k = g.shape[1]
+        mean = g.sum(-1, keepdim=True) / k
+        var = ((g - mean) ** 2).sum(-1, keepdim=True) / k
+        s1, s2 = g.abs().sum(-1, keepdim=True) / k, (g * g).sum(-1, keepdim=True) / k
+        dmean = u * s1
+        dvar = u * (s2 + 2 * mean.abs() * s1) + dmean * dmean
+        e = ((dmean + (g - mean).abs() * dvar / (2 * (var + eps))) / torch.sqrt(var + eps)).reshape(C, n).T * gamma.abs()
+        if film is not None:
+            e = e * (1 + film[b, :C]).abs()
+        out[b, :n] = e
+    return out
+
+
+def affine_terms(x: torch.Tensor, G: int, gamma, beta, rows: Sequence[int], film: Optional[torch.Tensor], eps: float) -> torch.Tensor:
+    """The kernel's fp32 uncentred affine y = fma(x, a, b) with a = gamma rstd (1 + s), b = (beta - mean gamma rstd)(1 + s) + shift:
+    a few roundings of |x a| and |b|, which for a group offset r carry r |gamma (1 + s)| of the output - 8 * 2^-24 of those, plus
+    2^-17 |y| of the bf16 hi/lo split of the output."""
+    B, T, C = x.shape
+    out = torch.zeros_like(x)
+    for b in range(B):
+        n = int(rows[b])
+        g = x[b, :n].T.reshape(G, -1)
+        k = g.shape[1]
+        mean = g.sum(-1, keepdim=True) / k
+        var = ((g - mean) ** 2).sum(-1, keepdim=True) / k
+        a = (1.0 / torch.sqrt(var + eps)).expand(G, k).reshape(C, n).T * gamma
+        m = mean.expand(G, k).reshape(C, n).T
+        fs = (1 + film[b, :C]) if film is not None else 1.0
+        fb = film[b, C:2 * C] if film is not None else 0.0
+        bb = (beta - m * a) * fs + fb
+        y = x[b, :n] * a * fs + bb
+        out[b, :n] = 8 * 2.0 ** -24 * ((x[b, :n] * a * fs).abs() + bb.abs() + (beta * fs).abs()) + 2.0 ** -17 * y.abs()
+    return out
+
+
+def layer_norm_rows(x: torch.Tensor, gamma, beta, eps: float) -> torch.Tensor:
+    """LayerNorm over the last dim in x's dtype"""
+    return torch.nn.functional.layer_norm(x, (x.shape[-1],), gamma.to(x.dtype), beta.to(x.dtype), eps)
+
+
+def depthwise7(x: torch.Tensor, dw: torch.Tensor, L: Sequence[int]) -> torch.Tensor:
+    """ConvNeXt's depthwise conv (k = 7, padding 3) of token-major x [B, T, C] with dw [C, 8] (taps, bias), rows >= L[b] of the
+    input read as 0"""
+    B, T, C = x.shape
+    xm = x.clone()
+    for b in range(B):
+        xm[b, int(L[b]):] = 0
+    w = dw[:, :7].to(x.dtype)[:, None, :]
+    return torch.nn.functional.conv1d(xm.transpose(1, 2), w, dw[:, 7].to(x.dtype), padding=3, groups=C).transpose(1, 2)
+
+
+def sinusoid(t: torch.Tensor, K: int, flip: bool, freq_shift: float) -> torch.Tensor:
+    """the timestep embedding of embeddings.py:24-64 in t's dtype: [sin | cos] (flipped: [cos | sin]) of t * 10^(-4 i / (half -
+    shift)), zero-padded to an odd K"""
+    half = K // 2
+    ex = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=t.dtype, device=t.device) / (half - freq_shift))
+    arg = t[:, None] * ex[None, :]
+    emb = torch.cat([torch.cos(arg), torch.sin(arg)] if flip else [torch.sin(arg), torch.cos(arg)], -1)
+    return torch.nn.functional.pad(emb, (0, K - 2 * half))
+
+
+def small_linear(xin: torch.Tensor, W, bias, add: Optional[torch.Tensor], add_rows: int, out_silu: bool) -> torch.Tensor:
+    """xin [M, K] (already through the input mode) @ W^T + bias (+ add row m % add_rows, or m) (then SiLU), in xin's dtype"""
+    y = xin @ W.to(xin.dtype).T
+    if bias is not None:
+        y = y + bias.to(xin.dtype)
+    if add is not None:
+        idx = torch.arange(xin.shape[0], device=xin.device)
+        y = y + add.to(xin.dtype)[idx % add_rows if add_rows > 0 else idx]
+    return y * torch.sigmoid(y) if out_silu else y
+
+
+def pool_attend(q: torch.Tensor, kv: torch.Tensor, heads: int, keys: Sequence[int]) -> torch.Tensor:
+    """AttentionPooling's attention (embeddings.py:521-546): q [B, C], kv [B, S1, 2C]; entry b over its first keys[b] rows; both
+    q and k scaled by dph^-1/4; in q's dtype"""
+    B, C = q.shape
+    dph = C // heads
+    s4 = 1.0 / math.sqrt(math.sqrt(dph))
+    out = torch.zeros_like(q)
+    for b in range(B):
+        n = int(keys[b])
+        qh = (q[b] * s4).reshape(heads, dph)
+        k = (kv[b, :n, :C] * s4).reshape(n, heads, dph)
+        v = kv[b, :n, C:].reshape(n, heads, dph)
+        w = torch.softmax(torch.einsum("hd,nhd->hn", qh, k), -1)
+        out[b] = torch.einsum("hn,nhd->hd", w, v).reshape(C)
+    return out

@@ -69,7 +69,9 @@ class GemmArgs(C.Structure):
                 ("ln_stats", C.c_void_p), ("ln_g", C.c_void_p), ("ln_C", C.c_int), ("ln_eps", C.c_float), ("row_stats", C.c_void_p),
                 ("stat_sum", C.c_void_p), ("stat_sq", C.c_void_p), ("rowmask", C.c_void_p), ("row_len", C.c_void_p),
                 ("len_shift", C.c_int), ("pre_scale", C.c_void_p), ("pre_shift", C.c_void_p), ("pre_mode", C.c_int), ("pre_C", C.c_int),
-                ("ksplit", C.c_int)]
+                ("ksplit", C.c_int), ("gn_stats1", C.c_void_p), ("gn_stats2", C.c_void_p), ("gn_C1", C.c_int), ("gn_C2", C.c_int),
+                ("gn_G", C.c_int), ("gn_eps", C.c_float), ("gn_gamma", C.c_void_p), ("gn_beta", C.c_void_p), ("gn_film", C.c_void_p),
+                ("gn_film_ld", C.c_int)]
 
 
 class AttnArgs(C.Structure):
