@@ -131,6 +131,20 @@ int ns2vc_unipc_step(const float* x_prev, const float* x_eval, const float* unet
                      const ns2vc_unipc_coef* c, float* m_t, float* x_t, float* x_pred, size_t n, int* nan_flag,
                      ns2vc_stream stream);
 
+/* The two steps above for rows at different steps: row b of a [B, row_n] batch (row_n = Cl * T elements per row) takes step
+ * k[b] of a run whose coefficient structs are the DEVICE array coefs (one per step; k[b] must be below their count).
+ *   k [B] int32 device: each row's step, or -1 for an empty row.  An occupied row's results are bit-identical to the scalar entry
+ *     run on that row with struct coefs[k[b]]; an empty row writes 0 to every output and raises no flag.  Each occupied k[b] is
+ *     advanced by one, so a captured step replays with no host write in between.
+ *   nan_flags [B] int32 device (may be NULL): entry b is set to 1 when row b's x (x_eval) holds a NaN.
+ * Every buffer pointer is required (any row may need any operand).  UniPC: a row at its first step (corr_order == 0) writes
+ * x_t = x_eval, so the rotation m1 <- m0 <- m_t, x_prev <- x_t, x_eval <- x_pred is the same for every row. */
+int ns2vc_dpm_step_rows(const float* x, const float* unet_out, const float* m_prev, const ns2vc_dpm_coef* coefs, int* k, float* m_cur,
+                        float* x_next, size_t row_n, int B, int* nan_flags, ns2vc_stream stream);
+int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
+                          const ns2vc_unipc_coef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
+                          int* nan_flags, ns2vc_stream stream);
+
 /* DDPM p_sample (model.py:535-542) and DDIM (model.py:586-601) steps after the denoiser returned x0 = x_start.
  * UNLIKE the two entries above, `c` is a DEVICE pointer to one coefficient struct, read by the kernel: a captured chunk of
  * steps then serves every chunk of a long run (the host refills a device window of structs before each replay).

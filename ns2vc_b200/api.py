@@ -226,7 +226,7 @@ def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Op
 
 
 def __getattr__(name):
-    # waveform-to-waveform conversion lives in convert.py and live conversion in stream.py; they build on this module
+    # waveform-to-waveform conversion lives in convert.py, live conversion in stream.py and serving in serve.py; they build on this module
     if name in ("convert_utterances", "convert_slices", "convert_files"):
         from . import convert
         return getattr(convert, name)
@@ -236,4 +236,7 @@ def __getattr__(name):
     if name == "StreamConverter":
         from . import stream
         return stream.StreamConverter
+    if name == "ConversionServer":                          # requests served as they arrive (continuous batching)
+        from . import serve
+        return serve.ConversionServer
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

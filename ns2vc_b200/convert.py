@@ -92,6 +92,28 @@ def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.
     plans = _check_inputs(wavs, sr, list(prompts), list(x_T))
     dev = next(unet.parameters()).device
     B = len(wavs)
+    front = encode_front(content_model, pre_model, wavs, sr, prompts, plans, dev)
+    tl, content, prompt = front["tl"], front["content"], front["prompt"]
+    sl = [int(p.shape[1]) for p in prompts]
+    T = max(tl)
+    tl_h, sl_h = torch.tensor(tl, dtype=torch.int64), torch.tensor(sl, dtype=torch.int64)
+    x = torch.zeros((B, LATENT_CH, T), dtype=torch.float32, device=dev)
+    for j, xt in enumerate(x_T):
+        x[j, :, :tl[j]] = xt.reshape(LATENT_CH, tl[j]).to(dev, torch.float32)
+    lat = sample_latents(unet, x, content, prompt, sl_h, steps=steps, method=method, device=dev, content_lengths=tl_h)
+    audio = vocoder.decode(lat, tl_h)
+    return dict(units=front["units"], c=front["c"], content=[content[:tl[j], j] for j in range(B)],
+                prompt=[prompt[:sl[j], j] for j in range(B)], latent=[lat[j, :, :tl[j]] for j in range(B)],
+                audio=[audio[j, :tl[j] * HOP] for j in range(B)])
+
+
+@torch.no_grad()
+def encode_front(content_model, pre_model, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence[torch.Tensor],
+                 plans: Sequence[Dict[str, int]], dev: torch.device) -> Dict[str, object]:
+    """The encoders in front of the sampler, on ``wavs`` (checked by ``_check_inputs``, which gave ``plans``) as ONE ragged batch:
+    resampling, ContentVec, ``repeat_expand_2d`` and ``Pre_model.infer(per_utterance=True)``.  Returns ``units`` and ``c`` per
+    utterance, the frame counts ``tl``, and the encoders' padded outputs ``content`` [T, B, C] and ``prompt`` [S, B, C]."""
+    B = len(wavs)
     n = [int(w.shape[0]) for w in wavs]
     n24, tl = [p["n24"] for p in plans], [p["T"] for p in plans]
     n16, nu = [p["n16"] for p in plans], [p["units"] for p in plans]
@@ -115,13 +137,7 @@ def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.
         refer[j, :, :sl[j]] = p.to(dev, torch.float32)
     tl_h, sl_h = torch.tensor(tl, dtype=torch.int64), torch.tensor(sl, dtype=torch.int64)
     content, prompt = pre_model.infer((c, refer, None, None, None, tl_h, sl_h, None), per_utterance=True)
-    x = torch.zeros((B, LATENT_CH, T), dtype=torch.float32, device=dev)
-    for j, xt in enumerate(x_T):
-        x[j, :, :tl[j]] = xt.reshape(LATENT_CH, tl[j]).to(dev, torch.float32)
-    lat = sample_latents(unet, x, content, prompt, sl_h, steps=steps, method=method, device=dev, content_lengths=tl_h)
-    audio = vocoder.decode(lat, tl_h)
-    return dict(units=units, c=cs, content=[content[:tl[j], j] for j in range(B)], prompt=[prompt[:sl[j], j] for j in range(B)],
-                latent=[lat[j, :, :tl[j]] for j in range(B)], audio=[audio[j, :tl[j] * HOP] for j in range(B)])
+    return dict(units=units, c=cs, tl=tl, content=content, prompt=prompt)
 
 
 @torch.no_grad()

@@ -378,6 +378,13 @@ int launch_unipc_step(const float* x_prev, const float* x_eval, const float* une
                       const float* m1, const UniPcStepCoef& c, float* m_t, float* x_t, float* x_pred, size_t n,
                       int* nan_flag, cudaStream_t st);
 
+// Per-row steps: row b of [B, row_n] takes the DEVICE struct coefs[k[b]] (k[b] < 0: an empty row, zeros out); k[b] is advanced
+int launch_dpm_step_rows(const float* x, const float* unet_out, const float* m_prev, const DpmStepCoef* coefs, int* k, float* m_cur,
+                         float* x_next, size_t row_n, int B, int* nan_flags, cudaStream_t st);
+int launch_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
+                           const UniPcStepCoef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
+                           int* nan_flags, cudaStream_t st);
+
 // DDPM / DDIM steps: the coefficient struct is read from DEVICE memory (layout of ns2vc_ddpm_coef / ns2vc_ddim_coef)
 struct DdpmStepCoef {   // x_next = (c_x0*x0 + c_x*x) + (add_noise ? c_noise*noise : 0)
   float c_x0, c_x;             // posterior_mean_coef1[t], posterior_mean_coef2[t]

@@ -1209,6 +1209,29 @@ int ns2vc_unipc_step(const float* x_prev, const float* x_eval, const float* unet
   return launch_unipc_step(x_prev, x_eval, unet_out, m0, m1, k, m_t, x_t, x_pred, n, nan_flag, (cudaStream_t)stream);
 }
 
+static_assert(sizeof(ns2vc_dpm_coef) == sizeof(DpmStepCoef) && offsetof(ns2vc_dpm_coef, order) == offsetof(DpmStepCoef, order),
+              "ns2vc_dpm_coef and DpmStepCoef must share one layout (the row kernel reads the caller's structs from device memory)");
+static_assert(sizeof(ns2vc_unipc_coef) == sizeof(UniPcStepCoef) && offsetof(ns2vc_unipc_coef, corr_order) == offsetof(UniPcStepCoef, corr_order) &&
+              offsetof(ns2vc_unipc_coef, pred_order) == offsetof(UniPcStepCoef, pred_order),
+              "ns2vc_unipc_coef and UniPcStepCoef must share one layout (the row kernel reads the caller's structs from device memory)");
+
+int ns2vc_dpm_step_rows(const float* x, const float* unet_out, const float* m_prev, const ns2vc_dpm_coef* coefs, int* k, float* m_cur,
+                        float* x_next, size_t row_n, int B, int* nan_flags, ns2vc_stream stream) {
+  NS_REQUIRE(x && unet_out && m_prev && coefs && k && m_cur && x_next, "null argument");
+  NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
+  return launch_dpm_step_rows(x, unet_out, m_prev, reinterpret_cast<const DpmStepCoef*>(coefs), k, m_cur, x_next, row_n, B, nan_flags,
+                              (cudaStream_t)stream);
+}
+
+int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
+                          const ns2vc_unipc_coef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
+                          int* nan_flags, ns2vc_stream stream) {
+  NS_REQUIRE(x_prev && x_eval && unet_out && m0 && m1 && coefs && k && m_t && x_t && x_pred, "null argument");
+  NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
+  return launch_unipc_step_rows(x_prev, x_eval, unet_out, m0, m1, reinterpret_cast<const UniPcStepCoef*>(coefs), k, m_t, x_t, x_pred,
+                                row_n, B, nan_flags, (cudaStream_t)stream);
+}
+
 static_assert(sizeof(ns2vc_ddpm_coef) == sizeof(DdpmStepCoef) && offsetof(ns2vc_ddpm_coef, add_noise) == offsetof(DdpmStepCoef, add_noise),
               "ns2vc_ddpm_coef and DdpmStepCoef must share one layout (the kernel reads the caller's struct from device memory)");
 static_assert(sizeof(ns2vc_ddim_coef) == sizeof(DdimStepCoef) && offsetof(ns2vc_ddim_coef, last) == offsetof(DdimStepCoef, last),

@@ -1,0 +1,330 @@
+"""Conversion requests served as they arrive (continuous batching): the rows of one ragged denoiser batch at their own sampler steps.
+
+A ``ConversionServer`` owns a fixed set of *slots*, the rows of one ragged program of geometry B = slots, T = max_frames,
+S = max_prompt_frames.  It advances one *tick* at a time: one denoiser forward plus one sampler step for every occupied slot,
+each slot at its own step index.  Requests wait in a FIFO queue; at the start of a tick the queued ones are *admitted* into the
+free slots, and a request *retires* at the end of its ``steps``-th tick, leaving its slot free for the next one.  A request thus
+waits at most one tick for a slot (plus its own admission), never for another request's whole run.
+
+Each request's result equals ``convert.convert_batch`` of that request alone with the same x_T, because every stage keeps row b
+equal to utterance b run alone: the encoders run on the newcomers as one ragged batch, ``ns2vc_unet_prepare_cond_ragged`` keeps its
+lengths in device tables, the FiLM rows are per row, and the row step kernels (``ns2vc_dpm_step_rows`` / ``ns2vc_unipc_step_rows``)
+do the scalar step's arithmetic with each row's own coefficient struct.
+
+A tick costs one forward of the whole slots x max_frames geometry whatever the occupancy (the ragged GEMMs compute padded rows),
+so for a list known in advance ``convert.convert_utterances`` (longest-first batches) remains the faster call: the server buys
+latency under arrivals, not peak throughput.  DDPM / DDIM are refused: their per-step noise would need a generator stream per row.
+"""
+from __future__ import annotations
+
+import collections
+import os
+from typing import Dict, List, Optional, Tuple
+
+import torch
+
+from . import _lib, convert
+from .api import default_schedule
+from .convert import HOP, LATENT_CH
+from .fused import DenoiserSession, _step_table, schedule_signature
+
+NAN_MESSAGE = "NaN in the denoiser input during the fused sampling run (reference model.py:404)"
+
+
+class SlotTable:
+    """The host bookkeeping of a server: the FIFO queue of tickets, the ticket in each slot and the tick at whose end it retires.
+    No device state; every decision is made from tick numbers alone, so finding the finished rows needs no device sync."""
+
+    def __init__(self, slots: int, steps: int):
+        self.slots, self.steps = int(slots), int(steps)
+        self.queue: collections.deque = collections.deque()
+        self.ticket: List[Optional[int]] = [None] * self.slots
+        self.last: List[Optional[int]] = [None] * self.slots
+
+    def enqueue(self, ticket: int) -> None:
+        self.queue.append(ticket)
+
+    def free_slots(self) -> List[int]:
+        return [s for s in range(self.slots) if self.ticket[s] is None]
+
+    def admit(self, tick: int) -> List[Tuple[int, int]]:
+        """(slot, ticket) of the requests admitted at the start of ``tick``: the oldest queued ones, into the free slots in
+        ascending order.  Each will run ticks ``tick .. tick + steps - 1``."""
+        out = []
+        for s in self.free_slots():
+            if not self.queue:
+                break
+            t = self.queue.popleft()
+            self.ticket[s], self.last[s] = t, tick + self.steps - 1
+            out.append((s, t))
+        return out
+
+    def retire(self, tick: int) -> List[Tuple[int, int]]:
+        """(slot, ticket) of the requests whose last tick is ``tick``; their slots are free from the next tick on."""
+        out = [(s, self.ticket[s]) for s in range(self.slots) if self.ticket[s] is not None and self.last[s] == tick]
+        for s, _ in out:
+            self.ticket[s] = self.last[s] = None
+        return out
+
+    @property
+    def occupied(self) -> int:
+        return sum(t is not None for t in self.ticket)
+
+    @property
+    def idle(self) -> bool:
+        return not self.queue and self.occupied == 0
+
+
+class ConversionServer:
+    """Waveform-to-waveform conversion of requests that arrive at any time; the caller owns the loop::
+
+        srv = ConversionServer(content_model, pre_model, unet, vocoder, slots=8, max_frames=1024, max_prompt_frames=512)
+        ticket = srv.submit(wav, sr, prompt_mel)       # FIFO order
+        done = srv.tick()                              # {ticket: audio [T_b * 256]} of the requests that finished in this tick
+        done = srv.drain()                             # tick until the queue and the slots are empty
+
+    ``method`` is ``"unipc"`` (30 steps by default) or ``"dpmsolver"`` (40), as for ``convert_utterances``.  A request whose
+    denoiser input held a NaN comes back as an ``AssertionError`` (the reference's per-call guard, model.py:404) in place of its
+    audio; the others carry on.  ``last_latents`` holds the latents [100, T_b] of the requests that finished in the last tick.
+
+    The tick is captured as one CUDA graph on its ``DenoiserSession.CAPTURE_AFTER``-th run and replayed from then on
+    (``NS2VC_GRAPH=0``: eager).  It holds the FiLM-row gather, the forward, the row step and the sampler's buffer rotation as
+    stream-ordered device copies (see ``_body``)."""
+
+    def __init__(self, content_model, pre_model, unet, vocoder, slots: int = 8, max_frames: int = 1024, max_prompt_frames: int = 512,
+                 method: str = "unipc", steps: Optional[int] = None):
+        self.steps = convert._check_method(method, steps)
+        if self.steps < 1:
+            raise ValueError(f"steps must be >= 1, got {self.steps}")
+        for name, v in (("slots", slots), ("max_frames", max_frames), ("max_prompt_frames", max_prompt_frames)):
+            if int(v) < 1:
+                raise ValueError(f"{name} must be >= 1, got {v}")
+        self.models = (content_model, pre_model, unet, vocoder)
+        self.method, self.kind = method, ("dpm" if method == "dpmsolver" else "unipc")
+        self.B, self.T, self.S = int(slots), int(max_frames), int(max_prompt_frames)
+        self.table = SlotTable(self.B, self.steps)
+        self.ticks = 0                                      # ticks run so far (the index of the next one)
+        self.last_latents: Dict[int, torch.Tensor] = {}
+        self.admission_events: Optional[list] = None        # set to [] to record (start, end) CUDA events around each admission
+        self._requests: Dict[int, dict] = {}
+        self._next_ticket = 0
+        self._sess: Optional[DenoiserSession] = None        # device state: allocated by the first tick
+
+    # ------------------------------------------------------------------------------------------------ requests
+    def submit(self, wav: torch.Tensor, sr: int, prompt_mel: torch.Tensor, x_T: Optional[torch.Tensor] = None) -> int:
+        """Queues one 1-D waveform at ``sr`` with its prompt mel [100, S_b] and returns its ticket (increasing, FIFO).  ``x_T``
+        ([1, 100, T_b] or [100, T_b]) defaults to ``torch.randn((1, 100, T_b))`` on the model's device, drawn here: requests
+        submitted in list order get the draws ``convert_utterances`` makes for that list."""
+        plan = convert._check_inputs([wav], sr, [prompt_mel], None if x_T is None else [x_T])[0]
+        if plan["T"] > self.T:
+            raise ValueError(f"the waveform is {plan['T']} frames, more than max_frames={self.T}")
+        S_b = int(prompt_mel.shape[1])
+        if S_b > self.S:
+            raise ValueError(f"the prompt is {S_b} frames, more than max_prompt_frames={self.S}")
+        if x_T is None:
+            x_T = torch.randn((1, LATENT_CH, plan["T"]), device=self._device())
+        ticket = self._next_ticket
+        self._next_ticket += 1
+        self._requests[ticket] = dict(wav=wav, sr=int(sr), prompt=prompt_mel, x_T=x_T, plan=plan, T=plan["T"], S=S_b)
+        self.table.enqueue(ticket)
+        return ticket
+
+    @torch.no_grad()
+    def tick(self) -> Dict[int, object]:
+        """Admits queued requests into the free slots, runs one tick and returns {ticket: audio [T_b * 256]} (or an
+        ``AssertionError``) for the requests that finished in it.  Does nothing when the queue and the slots are empty."""
+        if self.table.idle:
+            return {}
+        t = self.ticks
+        new = self.table.admit(t)
+        stale = self._setup()
+        if new:
+            self._admit(new)
+        elif stale:
+            self._prepare_all()
+        elif not self._sess._prepared or self._unet.__dict__.get("_cond_owner") is not self._sess:
+            self._sess.prepare()                            # another caller used the module's shared workspace since the last tick
+        self._run_tick()
+        self.ticks += 1
+        return self._retire(t)
+
+    def drain(self) -> Dict[int, object]:
+        """Ticks until the queue and the slots are empty; returns every result."""
+        out: Dict[int, object] = {}
+        while not self.table.idle:
+            out.update(self.tick())
+        return out
+
+    # ------------------------------------------------------------------------------------------------ device state
+    @property
+    def _unet(self):
+        return self.models[2]
+
+    def _device(self) -> torch.device:
+        return next(self._unet.parameters()).device
+
+    def _setup(self) -> bool:
+        """Allocates the device state on the first call.  True when the weights were re-packed since the last tick: the captured
+        tick, the prepared conditioning and the FiLM table are then stale."""
+        sess = self._sess
+        if sess is not None:
+            wsig = sess._wsig
+            sess._sync_engine()
+            if sess._wsig == wsig:
+                return False
+            self._graph, self._runs = None, 0
+            return True
+        unet = self._unet
+        dev = self._device()
+        B, T, S = self.B, self.T, self.S
+        f32 = dict(dtype=torch.float32, device=dev)
+        Cc = unet.cfg.in_channels - unet.latent_channels
+        content = torch.zeros((B, Cc, T), **f32) if Cc > 0 else None
+        prompt = torch.zeros((B, S, unet.cfg.cross_attention_dim), **f32)
+        sess = DenoiserSession(unet, content, prompt, None, T=T, content_lengths=[1] * B, prompt_lengths=[1] * B)
+        if sess.Cl != sess.Co:
+            raise ValueError("the server needs out_channels == latent channels (x_start parameterisation)")
+        self._sess, self._L = sess, _lib.lib()
+        self._clen, self._plen = [1] * B, [1] * B
+        ns = default_schedule()
+        ts = torch.linspace(ns.T, 1.0 / ns.total_N, self.steps + 1)
+        extra = True if self.kind == "dpm" else "bh2"       # lower_order_final / variant, as sample_latents runs them
+        steps = _step_table(self.kind, ns, ts, extra, (self.kind, tuple(float(v) for v in ts), extra, schedule_signature(ns)))
+        if self.kind == "dpm":
+            arr = (_lib.DpmCoef * len(steps))(*[_lib.DpmCoef(s.alpha_s, s.sigma_s, s.c_x, s.c_m, s.c_d, s.inv_r0, s.order) for s in steps])
+        else:
+            arr = (_lib.UniPcCoef * len(steps))(*[_lib.UniPcCoef(s.alpha_t, s.sigma_t, s.c_x, s.c_m, s.ab, s.rk, s.rho0, s.rho1,
+                                                                 s.corr_order, s.n_c_x, s.n_c_m, s.nab, s.nrk, s.pred_order) for s in steps])
+        self._coef = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
+        self._tvals = torch.tensor([[s.t_input] * B for s in steps], dtype=torch.float32).to(dev)
+        L, h = self._L, sess.h
+        self._fw = int(L.ns2vc_unet_film_width(h))
+        self._film_table = torch.empty(int(L.ns2vc_unet_time_table_floats(h, self.steps * B)), **f32)
+        self._film_rows = self._film_table[:self.steps * B * self._fw].view(self.steps * B, self._fw)
+        self._film = torch.empty((B, self._fw), **f32)
+        self._rowbase = torch.arange(B, dtype=torch.int64, device=dev)
+        self._k = torch.full((B,), -1, dtype=torch.int32, device=dev)
+        self._nan = torch.zeros((B,), dtype=torch.int32, device=dev)
+        shape = (B, sess.Cl, T)
+        names = ("x", "x_next", "m_prev", "m_cur") if self.kind == "dpm" else ("x_prev", "x_eval", "m0", "m1", "m_t", "x_t", "x_pred")
+        self._buf = {n: torch.zeros(shape, **f32) for n in names + ("out",)}
+        self._x = self._buf["x" if self.kind == "dpm" else "x_eval"]      # the denoiser input; after a request's last tick, its latent
+        self._graph, self._runs = None, 0
+        return False
+
+    def _admit(self, new: List[Tuple[int, int]]):
+        """Encodes the newcomers as one ragged batch per input rate, writes them into their slots, and prepares every slot again."""
+        cm, pm, _, _ = self.models
+        sess, dev = self._sess, self._device()
+        ev = None
+        if self.admission_events is not None:
+            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+            ev[0].record()
+        by_rate: Dict[int, List[Tuple[int, int]]] = {}
+        for s, tk in new:
+            by_rate.setdefault(self._requests[tk]["sr"], []).append((s, tk))
+        for sr, group in by_rate.items():
+            reqs = [self._requests[tk] for _, tk in group]
+            front = convert.encode_front(cm, pm, [r["wav"] for r in reqs], sr, [r["prompt"] for r in reqs], [r["plan"] for r in reqs], dev)
+            for j, ((s, _), r) in enumerate(zip(group, reqs)):
+                Tb, Sb = r["T"], r["S"]
+                if sess.content is not None:
+                    sess.content[s].zero_()
+                    sess.content[s, :, :Tb] = front["content"][:Tb, j].t()
+                sess.prompt[s].zero_()
+                sess.prompt[s, :Sb] = front["prompt"][:Sb, j]
+                for b in self._buf.values():
+                    b[s].zero_()
+                self._x[s, :, :Tb] = r["x_T"].reshape(LATENT_CH, Tb).to(dev, torch.float32)
+                self._clen[s], self._plen[s] = Tb, Sb
+        occupied = {s for s in range(self.B) if self.table.ticket[s] is not None}
+        for s in range(self.B):
+            if s not in occupied:                           # empty slots: length 1, zero inputs
+                if sess.content is not None:
+                    sess.content[s].zero_()
+                sess.prompt[s].zero_()
+                for b in self._buf.values():
+                    b[s].zero_()
+                self._clen[s], self._plen[s] = 1, 1
+        slots = torch.tensor([s for s, _ in new], dtype=torch.int64, device=dev)
+        self._k.index_fill_(0, slots, 0)
+        self._nan.index_fill_(0, slots, 0)
+        self._prepare_all()
+        if ev is not None:
+            ev[1].record()
+            self.admission_events.append(ev)
+
+    def _prepare_all(self):
+        """The conditioning of every slot (ns2vc_unet_prepare_cond_ragged) and the FiLM rows of all steps x slots."""
+        sess = self._sess
+        sess.clen.copy_(torch.tensor(self._clen, dtype=torch.int64))
+        sess.plen.copy_(torch.tensor(self._plen, dtype=torch.int64))
+        sess.prepare()
+        sess.time_table(self._tvals, self._film_table)
+
+    def _body(self):
+        """One tick: the FiLM row (k_b, b) of every slot, the forward, the row step, then the rotation of the sampler's buffers.
+        The rotation is four (UniPC) or two (DPM-Solver++) device copies inside the one captured graph rather than a cycle of
+        graphs over rotating pointers: UniPC's 3-deep history and 2-deep state would need lcm(3, 2) = 6 captures of the whole
+        forward, and the copies move 4 x slots x 100 x max_frames floats, small next to one forward."""
+        sess, L, b = self._sess, self._L, self._buf
+        idx = self._k.clamp(min=0).to(torch.int64) * self.B + self._rowbase       # empty slots read step 0's row (their output is discarded)
+        torch.index_select(self._film_rows, 0, idx, out=self._film)
+        sess.forward(self._x, None, b["out"], film_rows=self._film)
+        n, stream = sess.Cl * self.T, sess._stream()
+        with torch.cuda.device(sess.dev):
+            if self.kind == "dpm":
+                _lib.check(L.ns2vc_dpm_step_rows(b["x"].data_ptr(), b["out"].data_ptr(), b["m_prev"].data_ptr(), self._coef.data_ptr(),
+                                                 self._k.data_ptr(), b["m_cur"].data_ptr(), b["x_next"].data_ptr(), n, self.B,
+                                                 self._nan.data_ptr(), stream))
+            else:
+                _lib.check(L.ns2vc_unipc_step_rows(b["x_prev"].data_ptr(), b["x_eval"].data_ptr(), b["out"].data_ptr(), b["m0"].data_ptr(),
+                                                   b["m1"].data_ptr(), self._coef.data_ptr(), self._k.data_ptr(), b["m_t"].data_ptr(),
+                                                   b["x_t"].data_ptr(), b["x_pred"].data_ptr(), n, self.B, self._nan.data_ptr(), stream))
+        if self.kind == "dpm":
+            b["x"].copy_(b["x_next"])
+            b["m_prev"].copy_(b["m_cur"])
+        else:
+            b["m1"].copy_(b["m0"])
+            b["m0"].copy_(b["m_t"])
+            b["x_prev"].copy_(b["x_t"])
+            b["x_eval"].copy_(b["x_pred"])
+
+    def _run_tick(self):
+        self._runs += 1
+        if os.environ.get("NS2VC_GRAPH", "1") == "0" or (self._graph is None and self._runs < DenoiserSession.CAPTURE_AFTER):
+            self._body()
+            return
+        if self._graph is None:
+            torch.cuda.synchronize(self._sess.dev)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._body()
+            self._graph = g
+        self._graph.replay()
+
+    def _retire(self, t: int) -> Dict[int, object]:
+        done = self.table.retire(t)
+        self.last_latents = {}
+        if not done:
+            return {}
+        dev = self._device()
+        slots = torch.tensor([s for s, _ in done], dtype=torch.int64, device=dev)
+        flags = self._nan.index_select(0, slots).tolist()
+        self._k.index_fill_(0, slots, -1)
+        out: Dict[int, object] = {}
+        ok = [(s, tk) for (s, tk), f in zip(done, flags) if f == 0]
+        if ok:
+            tl = [self._requests[tk]["T"] for _, tk in ok]
+            rows = torch.tensor([s for s, _ in ok], dtype=torch.int64, device=dev)
+            lat = self._x.index_select(0, rows)[:, :, :max(tl)].contiguous()
+            audio = self.models[3].decode(lat, torch.tensor(tl, dtype=torch.int64))
+            for j, (_, tk) in enumerate(ok):
+                out[tk] = audio[j, :tl[j] * HOP]
+                self.last_latents[tk] = lat[j, :, :tl[j]]
+        for (_, tk), f in zip(done, flags):
+            if f != 0:
+                out[tk] = AssertionError(NAN_MESSAGE)
+        for _, tk in done:
+            del self._requests[tk]
+        return dict(sorted(out.items()))
