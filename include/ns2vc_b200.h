@@ -426,8 +426,8 @@ int ns2vc_mse_rows_ragged(const float* out, const float* target, int target_per_
                           int B, int C, int T, void* ws, ns2vc_stream stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * Kernel checks (tests only): one weight packing, one wgmma GEMM or one flash attention through the engines' own host code
- * and launchers, described by flat structs.  Every pointer is device memory; invalid combinations come back as the
+ * Kernel checks (tests only): one weight packing, one wgmma GEMM, one flash attention or one other launch (or short run of
+ * launches) through the engines' own host code and launchers, described by flat structs.  Every pointer is device memory; invalid combinations come back as the
  * launchers' error codes.  `desc` (desc_len bytes, may be NULL) receives the kernel and template arguments launched.
  * Stream-ordered (the GEMM allocates and frees its panel-affine descriptor on the stream). */
 typedef struct ns2vc_check_split {   /* a bf16 hi/lo split activation [B, T, ld] (16-bit elements), C valid channels */
@@ -551,6 +551,39 @@ typedef struct ns2vc_check_nct_split_args {
   const int* row_len;
 } ns2vc_check_nct_split_args;
 int ns2vc_check_nct_split(const ns2vc_check_nct_split_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* The content encoder's first conv: the GroupNorm statistics launch (stats [B, C0] of (mean, 1 / std) float pairs over each row's
+ * own frames), then the conv 0 launch into the split `out` [B, rows, out.ld] (out.C = C0); wav [B, bstride], lengths int64 [B]
+ * (clamped into [400, N]) or NULL. */
+typedef struct ns2vc_check_cv_conv0_args {
+  const float* wav; long long bstride; const int64_t* lengths; int B, N, C0;
+  const float* w0; const float* gamma; const float* beta; float eps;   /* w0 [C0, 1, 10]; the GroupNorm's weights [C0] */
+  float* stats;
+  ns2vc_check_split out; int rows;
+} ns2vc_check_cv_conv0_args;
+int ns2vc_check_cv_conv0(const ns2vc_check_cv_conv0_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* The content encoder's positional conv out = x + GELU(SamePad(conv(x))) over x [B, T, D] with frames[b] (int64) valid rows:
+ * the window launch into win_hi / win_lo ([B, G, T + K, 1024] bf16 each), then (windows_only = 0) one GEMM per group over the
+ * folded weight w [D, D / G, K] packed as the engine packs it, with bias [D] and the row mask keep [B, T], then the residual add. */
+typedef struct ns2vc_check_cv_pos_conv_args {
+  const float* x; int B, T, D, G, K;
+  const int64_t* frames;
+  const float* w; const float* bias; const float* keep;
+  void* win_hi; void* win_lo;
+  float* out;
+  int windows_only;
+} ns2vc_check_cv_pos_conv_args;
+int ns2vc_check_cv_pos_conv(const ns2vc_check_cv_pos_conv_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* The vocoder's ISTFT of a head output h [B, T, ld] (log-magnitudes, then phases; ld >= n_fft + 2) with window [n_fft] and
+ * hop n_fft / 4 into audio [B, T * hop]; len int64 [B] (clamped into [1, T]) or NULL.  The twiddles are the engine's. */
+typedef struct ns2vc_check_istft_args {
+  const float* h; int ld; const int64_t* len; int B, T, n_fft;
+  const float* window;
+  float* audio;
+} ns2vc_check_istft_args;
+int ns2vc_check_istft(const ns2vc_check_istft_args* args, char* desc, int desc_len, ns2vc_stream stream);
 
 #ifdef __cplusplus
 }

@@ -172,7 +172,8 @@ SIGNATURES = {
     "ns2vc_mse_ragged_workspace_bytes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "ns2vc_mse_rows_ragged": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_float, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
                                         _P, _P]),
-    # kernel checks (tests only; the argument structs are mirrored in tests/test_kernels_fp64.py and tests/test_norm_kernels_fp64.py)
+    # kernel checks (tests only; the argument structs are mirrored in tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py and
+    # tests/test_audio_kernels_fp64.py)
     "ns2vc_check_pack_b": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                      C.c_int, C.c_int, _P]),
     "ns2vc_check_gemm": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
@@ -183,6 +184,9 @@ SIGNATURES = {
     "ns2vc_check_small_linear": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_pool": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_nct_split": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
+    "ns2vc_check_cv_conv0": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
+    "ns2vc_check_cv_pos_conv": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
+    "ns2vc_check_istft": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

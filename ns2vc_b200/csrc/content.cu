@@ -257,7 +257,58 @@ __global__ void cv_qkv_kernel(const float* __restrict__ qw, const float* __restr
   }
 }
 
+int launch_check(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) { set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return -2; }
+  return 0;
+}
+
 }  // namespace
+
+// The launchers of the kernels above (engine_host.cuh): run_program and the kernel checks launch them through these
+int launch_cv_gn_stats(const CvGnStatsOp& o, const float* wav, long long bstride, const long long* lengths, cudaStream_t st) {
+  return launch_check(launch_k(cv_gn_stats_kernel, dim3(o.C0 / kStatCh, o.B), dim3(kStatCh * kStatLanes), 0, st, wav, bstride, lengths, o.N,
+                               o.w0, o.eps, o.C0, o.stats), "cv_gn_stats");
+}
+
+int launch_cv_conv0(const CvConv0Op& o, const float* wav, long long bstride, const long long* lengths, cudaStream_t st) {
+  return launch_check(launch_k(cv_conv0_kernel, dim3(ceil_div(o.rows, kConv0Frames), o.B), dim3(o.out.C / 2), 0, st, wav, bstride, lengths, o.N,
+                               o.rows, o.w0, o.stats, o.gamma, o.beta, o.out), "cv_conv0");
+}
+
+int launch_cv_pos_windows(const CvPosWinOp& o, cudaStream_t st) {
+  return launch_check(launch_k(cv_pos_windows_kernel, dim3(o.win.T, o.G, o.B), dim3(kWinTaps * 64 / 8), 0, st, o.x, o.T, o.D, o.G, o.gw, o.K,
+                               o.frames, o.win.hi, o.win.lo), "cv_pos_windows");
+}
+
+int launch_cv_add(const CvAddOp& o, cudaStream_t st) {
+  return launch_check(launch_k(cv_add_kernel, dim3((unsigned)((o.n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(o.p),
+                               reinterpret_cast<const float4*>(o.x), o.n4), "cv_add");
+}
+
+// Group g's weights of the folded positional conv (wg: [gw, gw, K]) into pb (Npad 128, K k-blocks): k-block j = tap j
+int pack_cv_pos_group(PackedB& pb, const float* wg, int gw, int K, cudaStream_t st) {
+  for (int j = 0; j < K; ++j) {
+    const int rc = pack_seg(pb, wg, gw, gw, K, j, 0, gw, 0, j, 0, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// The positional conv's GEMM of group g over the windows `win` (CvPosWinOp::win: G groups of T + K rows): K / kWinTaps segments
+// of 1024 channels at row shifts kWinTaps a, bias + GELU, the row mask `keep` [B, T], fp32 out at column g gw of out [B, T, out_ld]
+GemmOp cv_pos_group_gemm(ProgramBuilder& bld, const PackedB& w, const SplitBuf& win, int G, int g, int gw, int T, int K, const float* bias,
+                         const float* keep, float* out, int out_ld) {
+  const size_t gsz = (size_t)win.T * kWinTaps * 64;
+  const SplitBuf s{win.hi + g * gsz, win.lo + g * gsz, win.T, kWinTaps * 64, kWinTaps * 64,
+                   (long long)G * win.T * kWinTaps * 64};
+  GemmOp op = bld.gemm_base(w, T);
+  const int src = bld.add_src(op, s);
+  for (int a = 0; a < K / kWinTaps; ++a) bld.seg(op, src, 0, kWinTaps * 64, kWinTaps * a);
+  op.flags = EPI_BIAS | EPI_GELU | EPI_OUT_F32 | EPI_ROWMASK; op.bias = bias + g * gw; op.out = out + g * gw; op.out_ld = out_ld;
+  op.rowmask = keep;
+  return op;
+}
+
 }  // namespace ns2vc
 
 using namespace ns2vc;
@@ -329,9 +380,8 @@ int pack_with(ns2vc_cv* h, cudaStream_t st, float* scratch) {
     NS_CV_LAUNCH_CHECK();
     h->pos.assign(G, PackedB());
     for (int g = 0; g < G; ++g) {
-      if ((rc = mem.alloc_packed(h->pos[g], gw, gw, K, false))) return rc;   // k-block j = tap j (gw <= 64 channels, zero beyond)
-      for (int j = 0; j < K; ++j)
-        if ((rc = pack_seg(h->pos[g], wpos + (size_t)g * gw * gw * K, gw, gw, K, j, 0, gw, 0, j, 0, st))) return rc;
+      if ((rc = mem.alloc_packed(h->pos[g], gw, gw, K, false))) return rc;   // gw <= 64 channels, zero beyond
+      if ((rc = pack_cv_pos_group(h->pos[g], wpos + (size_t)g * gw * gw * K, gw, K, st))) return rc;
     }
   }
   const int L = c.num_layers;
@@ -447,15 +497,10 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
     rowmask(g, kLevels - 1);
     bld.emit_gemm(g, h->proj); }
   tap_f32("post_extract_proj", Fp, D);
-  bld.emit(Launch::CV_POS_WIN, CvPosWinOp{Fp, B, T, D, G, gw, K, lt.frames64, SplitBuf{win_hi, win_lo, Tw, kWinTaps * 64, kWinTaps * 64, 0}});
+  const SplitBuf win{win_hi, win_lo, Tw, kWinTaps * 64, kWinTaps * 64, 0};
+  bld.emit(Launch::CV_POS_WIN, CvPosWinOp{Fp, B, T, D, G, gw, K, lt.frames64, win});
   for (int g_ = 0; g_ < G; ++g_) {
-    SplitBuf win{win_hi + (size_t)g_ * Tw * kWinTaps * 64, win_lo + (size_t)g_ * Tw * kWinTaps * 64, Tw, kWinTaps * 64, kWinTaps * 64,
-                 (long long)G * Tw * kWinTaps * 64};
-    GemmOp g = bld.gemm_base(h->pos[g_], T);
-    const int src = bld.add_src(g, win);
-    for (int a = 0; a < K / kWinTaps; ++a) bld.seg(g, src, 0, kWinTaps * 64, kWinTaps * a);
-    g.flags = EPI_BIAS | EPI_GELU | EPI_OUT_F32; g.bias = w.W("encoder.pos_conv.0.bias") + g_ * gw; g.out = P + g_ * gw; g.out_ld = D;
-    rowmask(g, kLevels - 1);
+    GemmOp g = cv_pos_group_gemm(bld, h->pos[g_], win, G, g_, gw, T, K, w.W("encoder.pos_conv.0.bias"), lt.keep[kLevels - 1], P, D);
     bld.emit_gemm(g, h->pos[g_]);
   }
   bld.emit(Launch::CV_ADD, CvAddOp{P, Fp, (long long)(M * D / 4)});
@@ -508,11 +553,6 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
 
 namespace {
 
-int launch_check(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) { set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return -2; }
-  return 0;
-}
-
 int run_program(ns2vc_cv* h, const float* wav, long long bstride, const long long* lengths, float* units, long long* frames_out, cudaStream_t st) {
   CallArgs in{};
   in[Launch::OUT] = {units};
@@ -523,26 +563,10 @@ int run_program(ns2vc_cv* h, const float* wav, long long bstride, const long lon
         const LenTables& lt = h->lt;
         return launch_check(launch_k(cv_lengths_kernel, dim3(ceil_div(o.B * lt.rows[1], 256)), dim3(256), 0, st, lengths, o.B, o.N, lt, frames_out), "cv_lengths");
       }
-      case Launch::CV_GN_STATS: {
-        const CvGnStatsOp& o = l.get<CvGnStatsOp>();
-        return launch_check(launch_k(cv_gn_stats_kernel, dim3(o.C0 / kStatCh, o.B), dim3(kStatCh * kStatLanes), 0, st, wav, bstride, lengths, o.N,
-                                     o.w0, o.eps, o.C0, o.stats), "cv_gn_stats");
-      }
-      case Launch::CV_CONV0: {
-        const CvConv0Op& o = l.get<CvConv0Op>();
-        return launch_check(launch_k(cv_conv0_kernel, dim3(ceil_div(o.rows, kConv0Frames), o.B), dim3(o.out.C / 2), 0, st, wav, bstride, lengths, o.N,
-                                     o.rows, o.w0, o.stats, o.gamma, o.beta, o.out), "cv_conv0");
-      }
-      case Launch::CV_POS_WIN: {
-        const CvPosWinOp& o = l.get<CvPosWinOp>();
-        return launch_check(launch_k(cv_pos_windows_kernel, dim3(o.win.T, o.G, o.B), dim3(kWinTaps * 64 / 8), 0, st, o.x, o.T, o.D, o.G, o.gw, o.K,
-                                     o.frames, o.win.hi, o.win.lo), "cv_pos_windows");
-      }
-      case Launch::CV_ADD: {
-        const CvAddOp& o = l.get<CvAddOp>();
-        return launch_check(launch_k(cv_add_kernel, dim3((unsigned)((o.n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(o.p),
-                                     reinterpret_cast<const float4*>(o.x), o.n4), "cv_add");
-      }
+      case Launch::CV_GN_STATS: return launch_cv_gn_stats(l.get<CvGnStatsOp>(), wav, bstride, lengths, st);
+      case Launch::CV_CONV0: return launch_cv_conv0(l.get<CvConv0Op>(), wav, bstride, lengths, st);
+      case Launch::CV_POS_WIN: return launch_cv_pos_windows(l.get<CvPosWinOp>(), st);
+      case Launch::CV_ADD: return launch_cv_add(l.get<CvAddOp>(), st);
       case Launch::CV_SPLIT_TAP: {
         float* dst = h->cp.taps.dst[l.tap_index];
         if (dst) {

@@ -343,6 +343,29 @@ inline void set_group_norm(PrepOp& p, int B, const double* st1, int C1, const do
   p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / G));
 }
 
+// The content encoder's launchers (content.cu), shared by its run_program and the kernel checks.  conv 0's two launches read the
+// call's waveform (batch stride bstride) and lengths; the positional conv is the windows, one GEMM per group
+// (cv_pos_group_gemm over the weights pack_cv_pos_group packs), then the residual add.
+int launch_cv_gn_stats(const CvGnStatsOp& o, const float* wav, long long bstride, const long long* lengths, cudaStream_t st);
+int launch_cv_conv0(const CvConv0Op& o, const float* wav, long long bstride, const long long* lengths, cudaStream_t st);
+int launch_cv_pos_windows(const CvPosWinOp& o, cudaStream_t st);
+int launch_cv_add(const CvAddOp& o, cudaStream_t st);
+int pack_cv_pos_group(PackedB& pb, const float* wg, int gw, int K, cudaStream_t st);
+GemmOp cv_pos_group_gemm(ProgramBuilder& bld, const PackedB& w, const SplitBuf& win, int G, int g, int gw, int T, int K, const float* bias,
+                         const float* keep, float* out, int out_ld);
+
+// The vocoder's ISTFT (vocoder.cu): its tables, and the launch of one head output [B, T, ld] -> audio [B, T hop] with them
+struct IstftTables {
+  const float* window;      // [n_fft] head.istft.window as loaded
+  const float2* tw_half;    // [M / 2] exp(+2 pi i j / M), M = n_fft / 2: the inverse complex FFT
+  const float2* tw_full;    // [M / 2 + 1] exp(+2 pi i k / n_fft): the split step of the real inverse
+};
+void istft_twiddles(int n_fft, std::vector<float2>& tw_half, std::vector<float2>& tw_full);
+int istft_log2m(int n_fft);
+size_t istft_smem_bytes(int n_fft);
+int launch_istft(const IstftTables& tb, const float* h, int ld, const long long* len, float* audio, int B, int T, int n_fft, int hop, int log2m,
+                 size_t smem, cudaStream_t st);
+
 inline LinOp linear_op(const float* x, int x_ld, int M, int K, const float* W, const float* bias, int N, float* y, int y_ld) {
   LinOp o; memset(&o, 0, sizeof(o));
   o.x = x; o.x_ld = x_ld; o.M = M; o.K = K; o.W = W; o.bias = bias; o.N = N; o.out = y; o.out_ld = y_ld;

@@ -1,13 +1,15 @@
 // Test-only entry points into the product launchers: one weight packing, one wgmma GEMM, one flash attention, one activation
-// prep, one LayerNorm, one small linear, the AttentionPooling pieces and one [B, C, T] -> split conversion, each described by a
-// flat C struct (include/ns2vc_b200.h, "kernel checks") and run through exactly the host code the engines use (pack_seg, the
-// ProgramBuilder helpers, set_group_norm, linear_op, plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the
-// attention dispatch, the launchers of common.cuh).  tests/test_kernels_fp64.py and tests/test_norm_kernels_fp64.py drive them
-// at the shapes and edges the models never reach.  Nothing here is a kernel: every launch is the product's own.
+// prep, one LayerNorm, one small linear, the AttentionPooling pieces, one [B, C, T] -> split conversion, the content encoder's
+// first conv and positional conv, and the vocoder's ISTFT, each described by a flat C struct (include/ns2vc_b200.h, "kernel
+// checks") and run through exactly the host code the engines use (pack_seg, the ProgramBuilder helpers, set_group_norm,
+// linear_op, plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention dispatch, the launchers of common.cuh
+// and engine_host.cuh).  tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py and tests/test_audio_kernels_fp64.py drive
+// them at the shapes and edges the models never reach.  Nothing here is a kernel: every launch is the product's own.
 #include "engine_host.cuh"
 #include "../../include/ns2vc_b200.h"
 
 #include <cstdio>
+#include <vector>
 
 namespace ns2vc {
 namespace {
@@ -271,6 +273,90 @@ int ns2vc_check_nct_split(const ns2vc_check_nct_split_args* a, char* desc, int d
   const int rc = launch_nct_to_split(NctSplitOp{a->x, a->bstride, a->B, a->C, a->T, to_split(a->out), a->row_len, nullptr, 0}, (cudaStream_t)stream);
   if (rc) return rc;
   report(desc, desc_len, "nct_to_split<RAG=%d>", a->row_len ? 1 : 0);
+  return 0;
+}
+
+int ns2vc_check_cv_conv0(const ns2vc_check_cv_conv0_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->wav && a->w0 && a->gamma && a->beta && a->stats && a->out.hi && a->out.lo, "check_cv_conv0: null argument");
+  NS_REQUIRE(a->B >= 1 && a->B <= 65535 && a->N >= 400 && a->bstride >= a->N && a->rows >= 1, "check_cv_conv0: bad sizes B=%d N=%d bstride=%lld rows=%d",
+             a->B, a->N, a->bstride, a->rows);
+  NS_REQUIRE(a->C0 >= 128 && a->C0 <= 1024 && a->C0 % 128 == 0 && a->out.C == a->C0 && a->out.ld >= a->C0 && a->out.ld % 8 == 0,
+             "check_cv_conv0: C0=%d (a multiple of 128 up to 1024), out C=%d ld=%d", a->C0, a->out.C, a->out.ld);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long* len = (const long long*)a->lengths;
+  float2* stats = (float2*)a->stats;
+  int rc = launch_cv_gn_stats(CvGnStatsOp{a->B, a->N, a->C0, a->w0, a->eps, stats}, a->wav, a->bstride, len, st);
+  if (rc) return rc;
+  rc = launch_cv_conv0(CvConv0Op{a->B, a->N, a->rows, a->w0, stats, a->gamma, a->beta, to_split(a->out)}, a->wav, a->bstride, len, st);
+  if (rc) return rc;
+  report(desc, desc_len, "cv_gn_stats+cv_conv0<%d>", a->C0 / 2);
+  return 0;
+}
+
+int ns2vc_check_cv_pos_conv(const ns2vc_check_cv_pos_conv_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->x && a->frames && a->win_hi && a->win_lo, "check_cv_pos_conv: null argument");
+  NS_REQUIRE(a->B >= 1 && a->B <= 65535 && a->T >= 1 && a->G >= 1 && a->D % a->G == 0 && a->D % 4 == 0, "check_cv_pos_conv: bad sizes B=%d T=%d D=%d G=%d",
+             a->B, a->T, a->D, a->G);
+  const int gw = a->D / a->G;
+  NS_REQUIRE(gw <= 64 && gw % 4 == 0 && a->K >= 16 && a->K <= 16 * kMaxSeg && a->K % 16 == 0, "check_cv_pos_conv: group width %d, K=%d", gw, a->K);
+  cudaStream_t st = (cudaStream_t)stream;
+  const SplitBuf win{(__nv_bfloat16*)a->win_hi, (__nv_bfloat16*)a->win_lo, a->T + a->K, 1024, 1024, 0};
+  int rc = launch_cv_pos_windows(CvPosWinOp{a->x, a->B, a->T, a->D, a->G, gw, a->K, (const long long*)a->frames, win}, st);
+  if (rc) return rc;
+  if (a->windows_only) {
+    report(desc, desc_len, "%s", "cv_pos_windows");
+    return 0;
+  }
+  NS_REQUIRE(a->w && a->bias && a->keep && a->out, "check_cv_pos_conv: the GEMMs need weights, bias, keep and out");
+  ProgramBuilder bld{Arena{}, a->B, false, false, nullptr};
+  PackedB pb;
+  pb.Npad = pad_to(gw, 128); pb.nkb = a->K; pb.n_logical = gw;
+  const size_t elems = (size_t)pb.nkb * pb.Npad * 64;
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&pb.hi, elems * sizeof(__nv_bfloat16), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&pb.lo, elems * sizeof(__nv_bfloat16), st));
+  int bn = 0;
+  for (int g = 0; g < a->G && !rc; ++g) {
+    if (cudaMemsetAsync(pb.hi, 0, elems * sizeof(__nv_bfloat16), st) != cudaSuccess || cudaMemsetAsync(pb.lo, 0, elems * sizeof(__nv_bfloat16), st) != cudaSuccess) {
+      set_error("check_cv_pos_conv: memset failed");
+      rc = -2;
+      break;
+    }
+    if ((rc = pack_cv_pos_group(pb, a->w + (size_t)g * gw * gw * a->K, gw, a->K, st))) break;
+    GemmOp op = cv_pos_group_gemm(bld, pb, win, a->G, g, gw, a->T, a->K, a->bias, a->keep, a->out, a->D);
+    plan_gemm(op);
+    bn = op.bn;
+    if (!(rc = encode_tmaps(op))) rc = launch_gemm_tc(op, st);
+  }
+  NS_CHECK_CUDA(cudaFreeAsync(pb.hi, st));
+  NS_CHECK_CUDA(cudaFreeAsync(pb.lo, st));
+  if (rc) return rc;
+  if ((rc = launch_cv_add(CvAddOp{a->out, a->x, (long long)a->B * a->T * a->D / 4}, st))) return rc;
+  report(desc, desc_len, "cv_pos_windows+%dxgemm_tc<%d,LNF=0,XF=0,ENC=0,RAG=0,VOC=1>+cv_add", a->G, bn);
+  return 0;
+}
+
+int ns2vc_check_istft(const ns2vc_check_istft_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->h && a->window && a->audio, "check_istft: null argument");
+  const int n_fft = a->n_fft, hop = n_fft / 4;
+  NS_REQUIRE(n_fft >= 64 && n_fft <= 2048 && (n_fft & (n_fft - 1)) == 0, "check_istft: n_fft %d (a power of two, 64 .. 2048)", n_fft);
+  NS_REQUIRE(a->B >= 1 && a->B <= 65535 && a->T >= 1 && (long long)a->T * hop <= INT32_MAX && a->ld >= n_fft + 2, "check_istft: bad sizes B=%d T=%d ld=%d",
+             a->B, a->T, a->ld);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<float2> th, tf;
+  istft_twiddles(n_fft, th, tf);
+  float2 *d_th = nullptr, *d_tf = nullptr;
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&d_th, th.size() * sizeof(float2), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&d_tf, tf.size() * sizeof(float2), st));
+  NS_CHECK_CUDA(cudaMemcpyAsync(d_th, th.data(), th.size() * sizeof(float2), cudaMemcpyHostToDevice, st));
+  NS_CHECK_CUDA(cudaMemcpyAsync(d_tf, tf.data(), tf.size() * sizeof(float2), cudaMemcpyHostToDevice, st));
+  const int log2m = istft_log2m(n_fft);
+  const size_t smem = istft_smem_bytes(n_fft);
+  const int rc = launch_istft(IstftTables{a->window, d_th, d_tf}, a->h, a->ld, (const long long*)a->len, a->audio, a->B, a->T, n_fft, hop, log2m,
+                              smem, st);
+  NS_CHECK_CUDA(cudaFreeAsync(d_th, st));
+  NS_CHECK_CUDA(cudaFreeAsync(d_tf, st));
+  if (rc) return rc;
+  report(desc, desc_len, "voc_istft<log2m=%d,smem=%zu>", log2m, smem);
   return 0;
 }
 

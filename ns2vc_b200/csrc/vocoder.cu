@@ -177,12 +177,6 @@ __global__ void __launch_bounds__(256) voc_norm_kernel(const float* __restrict__
   }
 }
 
-struct IstftTables {
-  const float* window;      // [n_fft] head.istft.window as loaded
-  const float2* tw_half;    // [M / 2] exp(+2 pi i j / M), M = n_fft / 2: the inverse complex FFT
-  const float2* tw_full;    // [M / 2 + 1] exp(+2 pi i k / n_fft): the split step of the real inverse
-};
-
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
 // Bin k of S = clip(exp(mag), max=100) * (cos p + i sin p) from the head's row (log-magnitudes [nb], then phases [nb]).  The
@@ -298,6 +292,39 @@ int launch_voc_norm(const VocNormOp& op, cudaStream_t st) {
   return 0;
 }
 
+// twiddles: fp64 formulas rounded to fp32 (the kernels evaluate no sin / cos besides the phases')
+void istft_twiddles(int n_fft, std::vector<float2>& th, std::vector<float2>& tf) {
+  const int M = n_fft / 2;
+  const double pi = 3.141592653589793;
+  th.resize(M / 2);
+  tf.resize(M / 2 + 1);
+  for (int j = 0; j < M / 2; ++j) th[j] = make_float2((float)std::cos(2.0 * pi * j / M), (float)std::sin(2.0 * pi * j / M));
+  for (int k = 0; k <= M / 2; ++k) tf[k] = make_float2((float)std::cos(2.0 * pi * k / n_fft), (float)std::sin(2.0 * pi * k / n_fft));
+}
+
+int istft_log2m(int n_fft) {                                 // M = n_fft / 2 = 2^log2m
+  int log2m = 0;
+  while ((2 << log2m) < n_fft) ++log2m;
+  return log2m;
+}
+
+size_t istft_smem_bytes(int n_fft) { return (size_t)kIstftFrames * n_fft * sizeof(float); }
+
+int launch_istft(const IstftTables& tb, const float* head_out, int ld, const long long* len, float* audio, int B, int T, int n_fft, int hop,
+                 int log2m, size_t smem, cudaStream_t st) {
+  static size_t smem_set = 0;
+  if (smem > 48 * 1024 && smem > smem_set) {
+    const cudaError_t e = cudaFuncSetAttribute(voc_istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("voc_istft: cannot set %zu B dynamic smem: %s", smem, cudaGetErrorString(e)); return -2; }
+    smem_set = smem;
+  }
+  constexpr int G = kIstftFrames - (kFramesPerSample - 1);
+  const cudaError_t e = launch_k(voc_istft_kernel, dim3(ceil_div(T + 1, G), B), dim3(kIstftThreads), smem, st, head_out, ld, T, len, audio, n_fft,
+                                 hop, log2m, tb);
+  if (e != cudaSuccess) { set_error("voc_istft launch failed: %s", cudaGetErrorString(e)); return -2; }
+  return 0;
+}
+
 }  // namespace ns2vc
 
 using namespace ns2vc;
@@ -367,12 +394,8 @@ int pack(ns2vc_voc* h, cudaStream_t st) {
   }
   if ((rc = mem.alloc_packed(h->head, c.n_fft + 2, c.n_fft + 2, nkb_of(D), false))) return rc;
   if ((rc = pack_seg(h->head, w.W("head.out.weight"), c.n_fft + 2, D, 1, 0, 0, D, 0, 0, 0, st))) return rc;
-  // twiddles: fp64 formulas rounded to fp32 (the kernels evaluate no sin / cos besides the phases')
-  const int M = c.n_fft / 2;
-  const double pi = 3.141592653589793;
-  std::vector<float2> th(M / 2), tf(M / 2 + 1);
-  for (int j = 0; j < M / 2; ++j) th[j] = make_float2((float)std::cos(2.0 * pi * j / M), (float)std::sin(2.0 * pi * j / M));
-  for (int k = 0; k <= M / 2; ++k) tf[k] = make_float2((float)std::cos(2.0 * pi * k / c.n_fft), (float)std::sin(2.0 * pi * k / c.n_fft));
+  std::vector<float2> th, tf;
+  istft_twiddles(c.n_fft, th, tf);
   if (!(h->tw_half = mem.alloc<float2>(th.size())) || !(h->tw_full = mem.alloc<float2>(tf.size()))) return -2;
   NS_CHECK_CUDA(cudaMemcpy(h->tw_half, th.data(), th.size() * sizeof(float2), cudaMemcpyHostToDevice));
   NS_CHECK_CUDA(cudaMemcpy(h->tw_full, tf.data(), tf.size() * sizeof(float2), cudaMemcpyHostToDevice));
@@ -380,18 +403,8 @@ int pack(ns2vc_voc* h, cudaStream_t st) {
 }
 
 int launch_istft(const ns2vc_voc* h, const float* head_out, int ld, const long long* len, float* audio, int B, int T, cudaStream_t st) {
-  static size_t smem_set = 0;
-  if (h->istft_smem > 48 * 1024 && h->istft_smem > smem_set) {
-    const cudaError_t e = cudaFuncSetAttribute(voc_istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->istft_smem);
-    if (e != cudaSuccess) { set_error("voc_istft: cannot set %zu B dynamic smem: %s", h->istft_smem, cudaGetErrorString(e)); return -2; }
-    smem_set = h->istft_smem;
-  }
   const IstftTables tb{h->weights.W("head.istft.window"), h->tw_half, h->tw_full};
-  constexpr int G = kIstftFrames - (kFramesPerSample - 1);
-  const cudaError_t e = launch_k(voc_istft_kernel, dim3(ceil_div(T + 1, G), B), dim3(kIstftThreads), h->istft_smem, st, head_out, ld, T, len,
-                                 audio, h->cfg.n_fft, h->cfg.hop_length, h->log2m, tb);
-  if (e != cudaSuccess) { set_error("voc_istft launch failed: %s", cudaGetErrorString(e)); return -2; }
-  return 0;
+  return launch_istft(tb, head_out, ld, len, audio, B, T, h->cfg.n_fft, h->cfg.hop_length, h->log2m, h->istft_smem, st);
 }
 
 int head_ld(const ns2vc_voc_cfg& c) { return pad_to(c.n_fft + 2, 4); }   // a TMA-storable row pitch for the head's output
@@ -489,8 +502,8 @@ int ns2vc_voc_create(const ns2vc_voc_cfg* cfg, ns2vc_voc** out) {
   NS_REQUIRE(cfg->n_fft >= 64 && cfg->n_fft <= 2048 && (cfg->n_fft & (cfg->n_fft - 1)) == 0, "n_fft %d unsupported (a power of two, 64 .. 2048)", cfg->n_fft);
   ns2vc_voc* h = new ns2vc_voc();
   h->cfg = *cfg;
-  while ((2 << h->log2m) < cfg->n_fft) ++h->log2m;           // M = n_fft / 2 = 2^log2m
-  h->istft_smem = (size_t)kIstftFrames * cfg->n_fft * sizeof(float);
+  h->log2m = istft_log2m(cfg->n_fft);
+  h->istft_smem = istft_smem_bytes(cfg->n_fft);
   register_weights(h);
   *out = h;
   return 0;

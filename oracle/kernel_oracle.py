@@ -432,3 +432,144 @@ def pool_attend(q: torch.Tensor, kv: torch.Tensor, heads: int, keys: Sequence[in
         w = torch.softmax(torch.einsum("hd,nhd->hn", qh, k), -1)
         out[b] = torch.einsum("hn,nhd->hd", w, v).reshape(C)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# The content encoder's first conv and positional conv, the vocoder's ISTFT (tests/test_audio_kernels_fp64.py).  The truth of
+# each is the pinned oracle's stage (content_oracle.conv_layer / pos_conv, vocos_oracle.head_istft); these restate the same
+# operations with a switch per defect, so the tests can show each bound would notice it, and derive the design's error terms.
+# ---------------------------------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24
+
+
+def conv0_rows(wav: torch.Tensor, n: int, w0: torch.Tensor, gamma, beta, eps: float, padded_stats: bool = False,
+               unbiased: bool = False, use_eps: bool = True) -> torch.Tensor:
+    """conv 0 (k 10, s 5) -> GroupNorm(C0, C0) -> erf-GELU of one row's first n samples of wav [>= n], [T0, C0] in wav's dtype.
+    Defects: padded_stats (the statistics over the frames of the whole zero-padded wav instead of the row's own), unbiased
+    (variance over T0 - 1), use_eps=False (eps dropped)."""
+    x = wav.clone()
+    x[n:] = 0
+    T0 = (n - 10) // 5 + 1
+    y = torch.nn.functional.conv1d(x[None, None], w0.to(x.dtype), stride=5)[0]          # [C0, frames of the whole wav]
+    ys = y if padded_stats else y[:, :T0]
+    mean = ys.mean(-1, keepdim=True)
+    var = ys.var(-1, unbiased=unbiased, keepdim=True)
+    z = (y[:, :T0] - mean) / torch.sqrt(var + (eps if use_eps else 0.0)) * gamma.to(x.dtype)[:, None] + beta.to(x.dtype)[:, None]
+    return gelu_erf(z).T
+
+
+def conv0_fp32(wav: torch.Tensor, n: int, w0: torch.Tensor) -> torch.Tensor:
+    """The kernel's fp32 conv 0 of a row, emulated: y = fmaf(w[j], x[5t + j], y) for j = 0 .. 9, each step rounded to fp32 once
+    (the fp64 sum of an exact fp64 product and an fp32 value, then rounded: the same value but for a double rounding in 2^-29 of
+    the steps).  [C0, T0] as fp64."""
+    T0 = (n - 10) // 5 + 1
+    x = wav[:5 * (T0 - 1) + 10].to(F64)
+    cols = torch.stack([x[j:j + 5 * (T0 - 1) + 1:5] for j in range(10)])                # [10, T0]
+    w = w0.reshape(w0.shape[0], 10).to(F64)
+    y = torch.zeros(w.shape[0], T0, dtype=F64, device=x.device)
+    for j in range(10):
+        y = (w[:, j:j + 1] * cols[j][None] + y).float().to(F64)
+    return y
+
+
+def conv0_stats_tol(y32: torch.Tensor) -> tuple:
+    """What the kernel's stored (mean, 1 / std) may differ from the fp64 statistics of its own fp32 conv y32 [C0, T0]: the fp32
+    rounding of each (2^-24 relative), and the one-pass fp64 sums (32 time lanes of T0 / 32 frames, then the lanes in order:
+    (T0 / 32 + 32) 2^-53 of sum |y| and sum y^2, which the variance q / T0 - mean^2 carries relative to mean^2 + var).
+    Returns (mean, var, mean_tol, var_err), each [C0]: var_err bounds the fp64 sums' error in the variance."""
+    T0 = y32.shape[1]
+    mean = y32.mean(-1)
+    var = y32.var(-1, unbiased=False)
+    n_add = T0 / 32 + 34
+    mean_tol = U32 * mean.abs() + n_add * 2.0 ** -53 * y32.abs().mean(-1)
+    return mean, var, mean_tol, n_add * 2.0 ** -52 * (mean * mean + var)
+
+
+def conv0_terms(wav: torch.Tensor, n: int, w0: torch.Tensor, gamma, beta, eps: float) -> torch.Tensor:
+    """The design's error terms of cv_gn_stats + cv_conv0 against the fp64 truth, per output of one row ([T0, C0]):
+      * the fp32 conv, ten fmaf in tap order: d = 10 2^-24 sum_j |w_j| |x_5t+j|, at the output and in each statistic;
+      * the fp32 mean and the fp32 subtraction y - mean: 2^-24 (|mean| + |y - mean|);
+      * rstd: its fp32 rounding, the conv's error in the variance (2 std max d + max d^2) and the fp64 one-pass sums
+        (conv0_stats_tol), relative to var + eps;
+    all times rstd |gamma|, then the affine's two fp32 roundings, GELU's slope (< 1.13) and erff / its products (4 2^-24 of
+    |z| + |GELU(z)|), and 2^-17 |out| of the bf16 hi/lo split.  Under a DC offset the first two are
+    (10 sum |w||x| + |mean|) 2^-24 rstd |gamma|: the cancellation the design accepts."""
+    T0 = (n - 10) // 5 + 1
+    x = wav[:5 * (T0 - 1) + 10].to(F64)
+    y = torch.nn.functional.conv1d(x[None, None], w0.to(F64), stride=5)[0]                # [C0, T0]
+    d = 10 * U32 * torch.nn.functional.conv1d(x.abs()[None, None], w0.to(F64).abs(), stride=5)[0]
+    mean = y.mean(-1, keepdim=True)
+    var = y.var(-1, unbiased=False, keepdim=True)
+    dmax = d.amax(-1, keepdim=True)
+    _, _, _, var_sum = conv0_stats_tol(y)
+    rstd = 1.0 / torch.sqrt(var + eps)
+    drel = U32 + (2 * torch.sqrt(var) * dmax + dmax * dmax + var_sum[:, None]) / (2 * (var + eps))
+    g = gamma.to(F64).abs()[:, None]
+    yh = (y - mean) * rstd
+    z = yh * gamma.to(F64)[:, None] + beta.to(F64)[:, None]
+    dz = g * rstd * (d + dmax + U32 * (mean.abs() + (y - mean).abs())) + g * yh.abs() * drel + 2 * U32 * ((g * yh).abs() + z.abs())
+    out = gelu_erf(z)
+    return (1.13 * dz + 4 * U32 * (z.abs() + out.abs()) + 2.0 ** -17 * out.abs()).T
+
+
+def pos_conv_rows(x: torch.Tensor, W: torch.Tensor, bias, L: Sequence[int], shift: int = 0, keep_last: bool = False) -> torch.Tensor:
+    """x + GELU(SamePad(pos_conv(x))) of token-major x [B, T, D] (W [D, D / G, K], bias [D]), row b on its first L[b] frames,
+    rows at or past L[b] equal to x.  In x's dtype.  Defects: shift (every tap reads one frame later), keep_last (SamePad's
+    dropped frame kept: row L[b] gets a conv output too)."""
+    B, T, D = x.shape
+    K, gw = W.shape[-1], W.shape[1]
+    out = x.clone()
+    for b in range(B):
+        n = int(L[b])
+        xb = torch.zeros(n + K + 2, D, dtype=x.dtype, device=x.device)
+        xb[:n] = x[b, :n]
+        # output t reads x[t - K / 2 + j + shift], j < K: pad K / 2 - shift in front
+        front = K // 2 - shift
+        xp = torch.cat([torch.zeros(front, D, dtype=x.dtype, device=x.device), xb], 0).T[None]
+        y = torch.nn.functional.conv1d(xp, W.to(x.dtype), bias.to(x.dtype), groups=D // gw)[0].T
+        m = min(n + (1 if keep_last else 0), T)
+        out[b, :m] = x[b, :m] + gelu_erf(y[:m])
+    return out
+
+
+def pos_conv_terms(x: torch.Tensor, W: torch.Tensor, bias, L: Sequence[int]) -> torch.Tensor:
+    """The design's error terms of the positional conv per output: the 3xBF16 product of the split windows and split weights
+    (each split exact to 2^-17 relative, the lo x lo product left out: 3 2^-18 of sum |w||x|), the fp32 accumulation over the
+    4 K k-steps of 16 (worst case (4 K + 16) 2^-24 of sum |w||x|), carried through GELU's slope with the epilogue's
+    polynomial erf (4e-7 (1 + |v|)) and its roundings, and the fp32 residual add (2^-24 |out|).  Rows past L[b]: 0 (exact)."""
+    B, T, D = x.shape
+    K, gw = W.shape[-1], W.shape[1]
+    out = torch.zeros_like(x, dtype=F64)
+    for b in range(B):
+        n = int(L[b])
+        xp = torch.nn.functional.pad(x[b, :n].to(F64).T[None], (K // 2, K // 2))
+        v = torch.nn.functional.conv1d(xp, W.to(F64), bias.to(F64), groups=D // gw)[0].T[:n]
+        a = torch.nn.functional.conv1d(xp.abs(), W.to(F64).abs(), groups=D // gw)[0].T[:n]
+        e = (3 * 2.0 ** -18 + (4 * K + 16) * U32) * a + 2 * U32 * v.abs()
+        e = gelu_erf_slope(v).abs() * e + 4e-7 * (1 + v.abs()) + 4 * U32 * gelu_erf(v).abs()
+        out[b, :n] = e + U32 * (x[b, :n].to(F64) + gelu_erf(v)).abs()
+    return out
+
+
+def istft_rows(h: torch.Tensor, window: torch.Tensor, hop: int, L: Sequence[int], env_all_frames: bool = False,
+               reverse_window: bool = False, clip_first: bool = False) -> torch.Tensor:
+    """The ISTFT head of h [B, T, >= n_fft + 2] (log-magnitudes, then phases), row b alone on its first L[b] frames, zero past
+    L[b] hop samples: [B, T hop] in h's dtype.  Defects: env_all_frames (the envelope counts all T frames), reverse_window,
+    clip_first (clip(h, max=100) before exp instead of clip(exp(h), max=100))."""
+    B, T, _ = h.shape
+    n = window.numel()
+    nb, pad = n // 2 + 1, (n - hop) // 2
+    w = window.to(h.dtype).flip(0) if reverse_window else window.to(h.dtype)
+    out = torch.zeros(B, T * hop, dtype=h.dtype, device=h.device)
+    for b in range(B):
+        Lb = int(L[b])
+        lm, p = h[b, :Lb, :nb], h[b, :Lb, nb:2 * nb]
+        mag = torch.exp(torch.clip(lm, max=100.0)) if clip_first else torch.clip(torch.exp(lm), max=1e2)
+        S = mag * (torch.cos(p) + 1j * torch.sin(p))
+        frames = torch.fft.irfft(S, n, dim=-1) * w                                        # [Lb, n]
+        Le = T if env_all_frames else Lb
+        y = torch.nn.functional.fold(frames.T[None], (1, (Lb - 1) * hop + n), (1, n), stride=(1, hop))[0, 0, 0]
+        env = torch.nn.functional.fold((w * w)[None, :, None].expand(1, n, Le), (1, (Le - 1) * hop + n), (1, n), stride=(1, hop))[0, 0, 0]
+        out[b, :Lb * hop] = y[pad:pad + Lb * hop] / env[pad:pad + Lb * hop]
+    return out
+

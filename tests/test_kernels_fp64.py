@@ -827,6 +827,7 @@ for dev in (0, 1):
         t.launch_attn(ac, t.build_attn(ac, torch.device('cuda', dev)), poison=False)
         ac = t.ATTN_CASES[-1]
         t.launch_attn(ac, t.build_attn(ac, torch.device('cuda', dev)), poison=False)
+        a = __import__('test_audio_kernels_fp64'); a.launch_istft((2048, 2, 0), a.build_istft((2048, 2, 0)), torch.device('cuda', dev))
 print('ok')
 """
 
