@@ -24,6 +24,8 @@ struct PlanOp {
   std::string prefix;
   int cin = 0, cout = 0, level = 0;
   int c1 = 0, c2 = 0;       // RESNET: channels of the running tensor and of the concatenated skip
+  int site = -1;            // RESNET / XFORMER / DOWN / UP: index of its ResnetSite / XformerSite / ConvSite (set by pack_all)
+  bool skip = false;        // its output is pushed as a skip (the next op is a PUSH)
 };
 
 struct ResnetSite {
@@ -117,7 +119,10 @@ void build_plan(ns2vc_unet* h) {
   const ns2vc_unet_cfg& c = h->cfg;
   const int n = c.n_levels;
   std::vector<int> skip;
-  auto push = [&](int ch, int level) { PlanOp o; o.kind = PlanOp::PUSH; o.cout = ch; o.level = level; h->plan.push_back(o); skip.push_back(ch); };
+  auto push = [&](int ch, int level) {
+    if (!h->plan.empty()) h->plan.back().skip = true;   // (the first push keeps conv_in's output, which precedes the plan)
+    PlanOp o; o.kind = PlanOp::PUSH; o.cout = ch; o.level = level; h->plan.push_back(o); skip.push_back(ch);
+  };
   int ch = c.block_out_channels[0], level = 0;
   push(ch, 0);
   for (int i = 0; i < n; ++i) {
@@ -298,6 +303,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       add_vec_kernel<<<ceil_div(s.cout, 256), 256, 0, st>>>(h->weights.W(s.p + ".conv2.bias"), s.shortcut ? h->weights.W(s.p + ".conv_shortcut.bias") : nullptr, s.bias2, s.cout);
       s.film_off = film_off;
       film_off += c.time_scale_shift ? 2 * s.cout : s.cout;
+      o.site = (int)h->resnets.size();
       h->resnets.push_back(s);
     } else if (o.kind == PlanOp::XFORMER) {
       XformerSite x; x.p = o.prefix; x.c = o.cout;
@@ -339,6 +345,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       }
       x.kv_off = kv_off;
       kv_off += C;
+      o.site = (int)h->xformers.size();
       h->xformers.push_back(x);
     } else if (o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) {
       ConvSite s; s.p = o.prefix; s.c = o.cout;
@@ -346,6 +353,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       if ((rc = h->mem.alloc_packed(s.w, s.c, s.c, 3 * nk, h->simt))) return rc;
       for (int j = 0; j < 3; ++j)
         if ((rc = pack_named(h, s.w, s.p + ".conv.weight", s.c, s.c, 3, j, 0, s.c, 0, j * nk, 0, st))) return rc;
+      o.site = (int)h->resamplers.size();
       h->resamplers.push_back(s);
     }
   }
@@ -393,68 +401,6 @@ __global__ void nearest_index_kernel(int t_in, int t_out, int* idx) {
   idx[i] = nearest_src_index(i, t_in, t_out);
 }
 
-struct Builder : ProgramBuilder {
-  ns2vc_unet* h;
-  Builder(ns2vc_unet* h_, void* ws, int B_, std::vector<Launch>* out_)
-      : ProgramBuilder{Arena{(uint8_t*)ws, 0}, B_, ws == nullptr, h_->simt, out_}, h(h_) {}
-
-  void conv3(GemmOp& g, const SplitBuf& s) {           // k=3, stride 1, pad 1 over one split source
-    const int i = add_src(g, s);
-    for (int j = 0; j < 3; ++j) seg(g, i, 0, s.C, j - 1);
-  }
-  void emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
-    if (g.xmode) {
-      // few-tile, deep-K launches (the two coarsest levels at B = 8: 64 tiles of 24-64 k-blocks each): two CTAs per tile, each
-      // half of the channel blocks; worth it when both halves still have a few panels and all pairs are resident at once
-      const int tiles = B * ceil_div(g.T_out, 128) * (w.Npad / 64);
-      int panels = 0;
-      for (int i = 0; i < g.nxs; ++i) panels += g.xs[i].ncb;
-      if (2 * tiles <= gemm_sm_count() && panels >= 8) g.ksplit = 2;
-    }
-    Launch& l = ProgramBuilder::emit_gemm(g, w, in);
-    if (g.pre_film || (g.flags & EPI_ROWBIAS)) l.reads_film = 1;
-  }
-  // GroupNorm parameters of a panel-mode GEMM (statistics of up to two concatenated producers), parked in the workspace
-  const PrepOp* affine_desc(const double* st1, int C1, const double* st2, int C2, int Tn, int mode, float eps, const float* gamma,
-                            const float* beta, int film_ld, int level) {
-    PrepOp p; memset(&p, 0, sizeof(p));
-    p.C1 = C1; p.C2 = C2; p.B = B; p.T_src = Tn; p.T_dst = Tn; p.mode = mode;
-    p.row_len = rag_lens; p.len_shift = level;
-    set_group_norm(p, B, st1, C1, st2, C2, Tn, h->cfg.norm_num_groups, eps, gamma, beta, nullptr, film_ld);
-    // all descriptors of a program sit in one workspace array and go to the device in ONE copy when the program is complete
-    if ((int)aff_host.size() >= aff_cap) { err = -1; set_error("internal: affine descriptor table full"); return nullptr; }
-    aff_host.push_back(p);
-    return aff_dev ? aff_dev + (aff_host.size() - 1) : reinterpret_cast<const PrepOp*>(uintptr_t(16));   // (dry run: any non-null value)
-  }
-  std::vector<PrepOp> aff_host; PrepOp* aff_dev = nullptr; int aff_cap = 0;
-  const int* rag_lens = nullptr;                           // ragged programs: content lengths [B] (device), else nullptr
-  Arena sar;                                               // the program's static buffer (see ns2vc_unet::static_bufs)
-  void reserve_affine(int n) { aff_cap = n; aff_dev = sar.get<PrepOp>((size_t)n); aff_host.reserve(n); }
-  int upload_affine(cudaStream_t st) {
-    if (dry || aff_host.empty()) return 0;
-    // pageable source: the runtime stages it before returning, so the vector may die with the builder
-    return cudaMemcpyAsync(aff_dev, aff_host.data(), aff_host.size() * sizeof(PrepOp), cudaMemcpyHostToDevice, st) == cudaSuccess ? 0 : -2;
-  }
-  void emit_prep(const float* s1, int C1, const float* s2, int C2, int T_src, int T_dst, int mode, const float* scale,
-                 const float* shift, const SplitBuf& o, const SplitBuf* raw = nullptr, int row_mul = 1, int row_add = 0,
-                 const int* rowmap = nullptr, Launch::Input in = Launch::NONE) {
-    PrepOp p; memset(&p, 0, sizeof(p));
-    p.src1 = s1; p.ld1 = C1; p.C1 = C1; p.src2 = s2; p.ld2 = C2; p.C2 = C2; p.B = B; p.T_src = T_src; p.T_dst = T_dst;
-    p.row_mul = row_mul; p.row_add = row_add; p.rowmap = rowmap; p.mode = mode; p.scale = scale; p.shift = shift; p.out = o;
-    if (raw) p.raw = *raw;
-    emit(Launch::PREP, p, in);
-  }
-  // GroupNorm(+FiLM)(+SiLU) prep whose statistics come from the producers' epilogues
-  void emit_prep_gn(const float* s1, int C1, const double* st1, const float* s2, int C2, const double* st2, int Tn, int mode,
-                    float eps, const float* gamma, const float* beta, const float* film, int film_ld, const SplitBuf& o,
-                    const SplitBuf* raw = nullptr) {
-    emit_prep(s1, C1, s2, C2, Tn, Tn, mode, nullptr, nullptr, o, raw);
-    PrepOp& p = out->back().get<PrepOp>();
-    if (film) out->back().reads_film = 1;
-    set_group_norm(p, B, st1, C1, st2, C2, Tn, h->cfg.norm_num_groups, eps, gamma, beta, film, film_ld);
-  }
-};
-
 // The timestep path over M rows of timesteps `t` as small linears into temb1, emb [M, ted] and film [M, film_total]; returns their
 // number (the FiLM projection only when some resnet has one).  Reference embeddings.py:24-64, 157-218 (sinusoid -> linear_1 ->
 // SiLU -> linear_2), unet_1d_condition.py:869-883 (+ aug_emb: row m adds row m % B of `aug`), resnet.py:619-629 (time_emb_proj
@@ -473,24 +419,437 @@ int time_path_ops(const ns2vc_unet* h, const float* t, int M, int B, const float
   return 3;
 }
 
+// An activation that leaves a block: fp32 token-major tensor, its raw bf16 hi/lo split (the A operand of the panel-mode
+// GEMMs that consume it; written by the same epilogue) and the per-(b, channel) sums for the consumer's GroupNorm.
+struct Act { float* p = nullptr; SplitBuf sp{}; int c = 0; double* st = nullptr; };
+
+// The forward's scratch, shared by every block: each block views these at its own level's rows and width (Builder::reserve_forward).
+struct Scratch {
+  float* rot[3]; SplitBuf rot_sp[3];   // outputs of the blocks whose output no skip keeps, in rotation, and their raw splits
+  float *H1, *T0, *T1, *QKV;
+  SplitBuf SP_A, SP_R, SP_H, SP_X, SP_ATT, SP_FF, SP_QKV, SP_LN;
+};
+
+// Builds the conditioning and forward programs of one (B, T, S, ragged, workspace) key into `pg`: emit_cond, then
+// reserve_forward, emit_entry, one emitter per plan op in plan order and emit_head.  Each step takes its buffers from the
+// workspace arena and the static buffer as it goes, so this order fixes every offset.
+struct Builder : ProgramBuilder {
+  ns2vc_unet* h;
+  Program& pg;
+  const int T, S;
+  const bool ragged;
+  std::vector<int> Tl;                                     // rows per entry at each level
+  const bool xf_on;                                        // panel mode is possible (wgmma backend)
+  const int* rag_lens = nullptr;                           // ragged programs: content lengths [B] (device), else nullptr
+  Arena sar;                                               // the program's static buffer (see ns2vc_unet::static_bufs)
+  // conditioning outputs the forward reads
+  float* P = nullptr;                                      // conv_in(content) + bias
+  float* kvc = nullptr;                                    // cross-attention K | V of every transformer
+  SplitBuf kvs{};                                          // the same cache as bf16 hi/lo (attention v2 reads it by TMA)
+  float* maskbias = nullptr;
+  float* aug = nullptr;                                    // add_embedding output [B, ted]
+  // per-step buffers of the forward
+  SplitBuf s_xin{};
+  float* temb1 = nullptr; float* emb = nullptr; float* film = nullptr;
+  // per-(b, channel) sum | sum-of-squares of every fp32 activation that feeds a GroupNorm, accumulated by the producing GEMM
+  // epilogues; one contiguous arena, zeroed by one memset at the top of the forward
+  double* stat_arena = nullptr;
+  size_t stat_doubles = 0, stat_used = 0;
+  Scratch sc{};
+  // the walk: the running activation, the skip stack and the skip popped for the next resnet's concat
+  Act cur, cat2;
+  std::vector<Act> skips;
+  int rot_i = 0;
+
+  Builder(ns2vc_unet* h_, Program& pg_, void* ws, int B_, int T_, int S_, bool ragged_)
+      : ProgramBuilder{Arena{(uint8_t*)ws, 0}, B_, ws == nullptr, h_->simt, &pg_.prog_cond}, h(h_), pg(pg_), T(T_), S(S_),
+        ragged(ragged_), Tl(h_->cfg.n_levels), xf_on(!h_->simt) {
+    for (int l = 0; l < (int)Tl.size(); ++l) Tl[l] = level_len(T, l);
+  }
+
+  void conv3(GemmOp& g, const SplitBuf& s) {           // k=3, stride 1, pad 1 over one split source
+    const int i = add_src(g, s);
+    for (int j = 0; j < 3; ++j) seg(g, i, 0, s.C, j - 1);
+  }
+  void emit_gemm(GemmOp& g, const PackedB& w, Launch::Input in = Launch::NONE) {
+    if (g.xmode) {
+      // few-tile, deep-K launches (the two coarsest levels at B = 8: 64 tiles of 24-64 k-blocks each): two CTAs per tile, each
+      // half of the channel blocks; worth it when both halves still have a few panels and all pairs are resident at once
+      const int tiles = B * ceil_div(g.T_out, 128) * (w.Npad / 64);
+      int panels = 0;
+      for (int i = 0; i < g.nxs; ++i) panels += g.xs[i].ncb;
+      if (2 * tiles <= gemm_sm_count() && panels >= 8) g.ksplit = 2;
+    }
+    Launch& l = ProgramBuilder::emit_gemm(g, w, in);
+    if (g.pre_film || (g.flags & EPI_ROWBIAS)) l.reads_film = 1;
+  }
+  // GroupNorm descriptors of the panel-mode GEMMs: one array in the static buffer, copied to the device in ONE copy when the
+  // program is complete
+  std::vector<PrepOp> aff_host; PrepOp* aff_dev = nullptr; int aff_cap = 0;
+  void reserve_affine(int n) { aff_cap = n; aff_dev = sar.get<PrepOp>((size_t)n); aff_host.reserve(n); }
+  int upload_affine(cudaStream_t st) {
+    if (dry || aff_host.empty()) return 0;
+    // pageable source: the runtime stages it before returning, so the vector may die with the builder
+    return cudaMemcpyAsync(aff_dev, aff_host.data(), aff_host.size() * sizeof(PrepOp), cudaMemcpyHostToDevice, st) == cudaSuccess ? 0 : -2;
+  }
+  void emit_prep(const float* s1, int C1, const float* s2, int C2, int T_src, int T_dst, int mode, const float* scale,
+                 const float* shift, const SplitBuf& o, const SplitBuf* raw = nullptr, int row_mul = 1, int row_add = 0,
+                 const int* rowmap = nullptr, Launch::Input in = Launch::NONE) {
+    PrepOp p; memset(&p, 0, sizeof(p));
+    p.src1 = s1; p.ld1 = C1; p.C1 = C1; p.src2 = s2; p.ld2 = C2; p.C2 = C2; p.B = B; p.T_src = T_src; p.T_dst = T_dst;
+    p.row_mul = row_mul; p.row_add = row_add; p.rowmap = rowmap; p.mode = mode; p.scale = scale; p.shift = shift; p.out = o;
+    if (raw) p.raw = *raw;
+    emit(Launch::PREP, p, in);
+  }
+
+  // ragged programs: rows past each entry's length (every level derives its own: ceil(T_b / 2^l)) are zeros
+  void rag(GemmOp& g, int level) const { g.row_len = rag_lens; g.len_shift = level; }
+  void rag_prep(const int* len, int level) { PrepOp& p = out->back().get<PrepOp>(); p.row_len = len; p.len_shift = level; }
+  double* new_stats(int C) { return new_rowstats((size_t)B * C); }   // per-(b, channel) sums | sums of squares
+  double* new_rowstats(size_t nrows) { double* p = stat_arena ? stat_arena + stat_used : nullptr; stat_used += 2 * nrows; return p; }
+  void with_stats(GemmOp& g, double* st_, int C) const { g.flags |= EPI_STATS; g.stat_sum = st_; g.stat_sq = st_ ? st_ + (size_t)B * C : nullptr; }
+  SplitBuf scratch_split(size_t elems) { SplitBuf s{}; s.hi = ar.get<__nv_bfloat16>(elems); s.lo = ar.get<__nv_bfloat16>(elems); return s; }
+
+  // fp16 softmax weights (one P x [V_hi | V_lo] MMA per k-step) only where enough keys average their 2^-12 rounding out: over a few
+  // dozen keys (short prompts, the coarsest levels of short utterances) the weights are a bf16 hi/lo split - those launches are
+  // cheap anyway.  Measured on the reference's 40-step pipeline fixture (S = 40): worst err/tol 1.35 with fp16 weights everywhere.
+  // Only self-attention uses fp16 weights.  Cross-attention keeps the split whatever its key count: a key count cannot see how
+  // sharp the prompt attention is, and with fp16 weights in both attentions, scores of std ~4 (tests/test_numerics_fp64.py,
+  // regime 'sharp' at B=4, T=1024, S=256) put the output at 1.51x the elementwise tolerance against fp64 on an H100.
+  // Ragged programs never use them: entry b of a self-attention attends over its own T_b,l keys, known only on the device, and
+  // one built program serves every length vector, so the padded T_l says nothing about how many keys average the rounding.
+  static constexpr int kFp16MinKeys = 256;
+  bool p16(int keys) const { return !ragged && attention_v2_p_fp16() && keys >= kFp16MinKeys; }
+
+  // Can the GroupNorm in front of a GEMM over (cur [+ skip]) channels run inside the GEMM?  (64-channel blocks may not
+  // straddle the concat seam; the affine table holds kXfMaxC channels)
+  bool xf_ok(int c1, int c2) const { return xf_on && (c2 == 0 || c1 % 64 == 0) && c1 + c2 <= kXfMaxC && h->cfg.norm_num_groups <= 64; }
+
+  // The GroupNorm(+FiLM)(+SiLU) of one or two concatenated producers (statistics from their epilogues) as the A operand of `g`,
+  // a conv of `taps` taps (3: k3 p1, or 1).  Panel mode (`panel`, which xf_ok allows): the GEMM reads the producers' raw splits
+  // and normalises them with the descriptor, parked in the static buffer; the FiLM rows travel in GemmOp::pre_film.  Otherwise
+  // the descriptor is a prep launch into `o` (with `raw`: also the input's raw split, for a prep-mode shortcut) and the GEMM
+  // reads `o` in plain segments.
+  void normed_input(GemmOp& g, bool panel, const Act& a1, const Act& a2, const std::string& norm, float eps, int mode,
+                    const float* film, int film_ld, int taps, int level, const SplitBuf& o, const SplitBuf* raw = nullptr) {
+    const int Tn = Tl[level], C = a1.c + a2.c;
+    PrepOp p; memset(&p, 0, sizeof(p));
+    p.C1 = a1.c; p.C2 = a2.c; p.B = B; p.T_src = Tn; p.T_dst = Tn; p.mode = mode; p.row_len = rag_lens; p.len_shift = level;
+    set_group_norm(p, B, a1.st, a1.c, a2.st, a2.c, Tn, h->cfg.norm_num_groups, eps, h->weights.W(norm + ".weight"),
+                   h->weights.W(norm + ".bias"), panel ? nullptr : film, film_ld);
+    if (panel) {
+      const int kb_stride = taps == 1 ? 0 : nkb_of(C);       // k-blocks per tap
+      const int i1 = add_src(g, a1.sp);
+      xseg(g, i1, 0, a1.c, taps, 0, kb_stride, 1, 0);
+      if (a2.c) { const int i2 = add_src(g, a2.sp); xseg(g, i2, 0, a2.c, taps, nkb_of(a1.c), kb_stride, 1, a1.c); }
+      g.pre_film = film;
+      if ((int)aff_host.size() >= aff_cap) { err = -1; set_error("internal: affine descriptor table full"); return; }
+      aff_host.push_back(p);
+      g.pre = aff_dev ? aff_dev + (aff_host.size() - 1) : reinterpret_cast<const PrepOp*>(uintptr_t(16));   // (dry run: any non-null value)
+    } else {
+      p.src1 = a1.p; p.ld1 = a1.c; p.src2 = a2.p; p.ld2 = a2.c; p.row_mul = 1; p.out = o;
+      if (raw) p.raw = *raw;
+      emit(Launch::PREP, p).reads_film = film != nullptr;
+      const int i = add_src(g, o);
+      for (int j = 0; j < taps; ++j) seg(g, i, 0, C, j - taps / 2);
+    }
+  }
+
+  // The GEMM `g` that ends a block at `level` writes the block's output of C channels: fp32, (panel mode) its raw split and its
+  // statistics, into a buffer of its own when a skip keeps it, else into the next of the three rotating ones; ragged rows past
+  // each entry's length are zeros.  The output becomes the running activation, tapped as `name`.
+  void emit_block_out(GemmOp& g, const PackedB& w, int level, int C, bool is_skip, const std::string& name) {
+    const int TL = Tl[level];
+    Act a; a.c = C;
+    if (is_skip) { a.p = ar.get<float>((size_t)B * TL * C); if (xf_on) a.sp = view(scratch_split((size_t)B * TL * pad_to(C, 8)), TL, C); }
+    else { a.p = sc.rot[rot_i]; if (xf_on) a.sp = view(sc.rot_sp[rot_i], TL, C); rot_i = (rot_i + 1) % 3; }
+    a.st = new_stats(C);
+    g.flags |= EPI_OUT_F32; g.out = a.p; g.out_ld = C;
+    if (xf_on) { g.flags |= EPI_OUT_SPLIT; g.out_hi = a.sp.hi; g.out_lo = a.sp.lo; g.out_split_ld = a.sp.ld; }
+    with_stats(g, a.st, C);
+    rag(g, level);
+    emit_gemm(g, w);
+    cur = a;
+    emit_tap(pg.taps, name, a.p, level, C, TL);
+  }
+
+  // ================= conditioning program =================
+  // conv_in of the content, the cross-attention K | V of every transformer over the prompt, the mask bias and the pooled prompt
+  // embedding; its outputs stay in the workspace for every forward
+  void emit_cond() {
+    const ns2vc_unet_cfg& c = h->cfg;
+    const int c0 = c.block_out_channels[0], Cc = c.in_channels - c.latent_channels, xd = c.cross_attention_dim, ted = h->ted;
+    const int* plens = rag_lens ? rag_lens + B : nullptr;   // ragged: prompt lengths
+    P = (Cc > 0) ? ar.get<float>((size_t)B * T * c0) : nullptr;
+    kvc = ar.get<float>((size_t)B * S * std::max(h->kv_total, 1));
+    kvs.T = S; kvs.C = std::max(h->kv_total, 8); kvs.ld = pad_to(kvs.C, 8);
+    kvs.hi = ar.get<__nv_bfloat16>((size_t)B * S * kvs.ld);
+    kvs.lo = ar.get<__nv_bfloat16>((size_t)B * S * kvs.ld);
+    maskbias = ar.get<float>((size_t)B * S);
+    aug = ar.get<float>((size_t)B * ted);
+    // conditioning scratch
+    const SplitBuf s_content = (Cc > 0) ? split(T, Cc) : SplitBuf{};
+    const SplitBuf s_prompt = split(S, xd);
+    TextTimeEmbedding tte;
+    tte.reserve(ar, B, S, xd, ted);
+
+    if (Cc > 0) {
+      emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, Cc, T, s_content, rag_lens, nullptr, 0}, Launch::CONTENT);
+      GemmOp g = gemm_base(h->convin_content, T);
+      conv3(g, s_content);
+      g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W("conv_in.bias"); g.out = P; g.out_ld = c0;
+      emit_gemm(g, h->convin_content);
+    }
+    emit(Launch::MASKBIAS, MaskBiasOp{nullptr, B * S, maskbias}, Launch::MASK);
+    if (h->kv_total > 0) {
+      emit_prep(nullptr, xd, nullptr, 0, S, S, PREP_RAW, nullptr, nullptr, s_prompt, nullptr, 1, 0, nullptr, Launch::PROMPT);
+      rag_prep(plens, 0);                                    // (ragged: prompt frames past S_b are zeros, so is their K / V)
+      GemmOp g = lin(h->kv_all, s_prompt, S);
+      g.flags = EPI_OUT_F32 | EPI_OUT_SPLIT; g.out = kvc; g.out_ld = h->kv_total;
+      g.out_hi = kvs.hi; g.out_lo = kvs.lo; g.out_split_ld = kvs.ld;   // (V stays a bf16 split: cross-attention weights are split)
+      emit_gemm(g, h->kv_all);
+    }
+    if (c.add_embed_text)   // TextTimeEmbedding of the prompt (embeddings.py:421-434)
+      tte.emit(*this, h->weights, "add_embedding", nullptr, Launch::PROMPT, S, xd, ted, c.add_embed_heads, Launch::POOL_ATT, h->pool_kv, aug, plens);
+  }
+
+  // ================= forward program =================
+  // per-step buffers, the statistics arena and the scratch the blocks share
+  void reserve_forward() {
+    const ns2vc_unet_cfg& c = h->cfg;
+    const int c0 = c.block_out_channels[0];
+    s_xin = split(T, c.latent_channels);
+    temb1 = ar.get<float>((size_t)B * h->ted);
+    emb = ar.get<float>((size_t)B * h->ted);
+    film = ar.get<float>((size_t)B * std::max(h->film_total, 1));
+    stat_doubles = (size_t)2 * B * c0;
+    for (auto& o : h->plan) {
+      if (o.kind == PlanOp::RESNET) stat_doubles += (size_t)4 * B * o.cout;
+      else if (o.kind == PlanOp::XFORMER || o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) stat_doubles += (size_t)2 * B * o.cout;
+      if (o.kind == PlanOp::XFORMER) stat_doubles += (size_t)3 * 2 * B * Tl[o.level];   // three LayerNorm row-statistics buffers
+    }
+    stat_arena = ar.get<double>(stat_doubles);
+    // activation buffers
+    size_t max_act = (size_t)B * T * c0, max_cat = 0, max_ff = 1, max_qkv = 1;
+    for (auto& o : h->plan) {
+      const size_t rows = (size_t)B * Tl[o.level];
+      if (o.kind == PlanOp::RESNET) { max_act = std::max(max_act, rows * o.cout); max_cat = std::max(max_cat, rows * o.cin); }
+      if (o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) { max_act = std::max(max_act, rows * o.cout); max_cat = std::max(max_cat, rows * o.cout); }
+      if (o.kind == PlanOp::XFORMER) { max_act = std::max(max_act, rows * o.cout); max_ff = std::max(max_ff, rows * 4 * o.cout); max_qkv = std::max(max_qkv, rows * 3 * o.cout); }
+    }
+    max_cat = std::max(max_cat, max_act);
+    for (int i = 0; i < 3; ++i) sc.rot[i] = ar.get<float>(max_act);
+    sc.H1 = ar.get<float>(max_act);
+    sc.T0 = ar.get<float>(max_act);
+    sc.T1 = ar.get<float>(max_act);
+    sc.QKV = ar.get<float>(max_qkv);
+    sc.SP_A = scratch_split(max_cat);      // conv1 / resample input
+    sc.SP_R = scratch_split(max_cat);      // raw shortcut operand / odd rows of a stride-2 conv
+    sc.SP_H = scratch_split(max_act);      // conv2 input, out-head input
+    sc.SP_X = scratch_split(max_act);      // GN-normalised transformer input (when the GroupNorm is a prep launch)
+    sc.SP_ATT = scratch_split(max_act);    // attention output
+    sc.SP_FF = scratch_split(max_ff);      // GEGLU output
+    sc.SP_QKV = scratch_split(max_qkv);    // q | k | v of the self-attention (q of the cross-attention)
+    sc.SP_LN = scratch_split(max_act);     // raw (un-normalised) split of the transformer's residual stream (folded LayerNorms)
+    for (int i = 0; i < 3; ++i) sc.rot_sp[i] = xf_on ? scratch_split(max_act) : SplitBuf{};   // (panel mode only)
+  }
+
+  // entry: the statistics memset, x -> split tokens, the time path and conv_in (whose output is the first skip)
+  void emit_entry() {
+    const ns2vc_unet_cfg& c = h->cfg;
+    const int c0 = c.block_out_channels[0], Cc = c.in_channels - c.latent_channels;
+    emit_memset(stat_arena, stat_doubles * sizeof(double));
+    emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, c.latent_channels, T, s_xin, rag_lens, nullptr, 0}, Launch::X);
+    LinOp tp[3];
+    const int n = time_path_ops(h, nullptr, B, B, aug, temb1, emb, film, tp);
+    for (int i = 0; i < n; ++i) emit_linear(tp[i], i == 0 ? Launch::T : Launch::NONE, 1);
+
+    GemmOp g = gemm_base(h->convin_lat, T);
+    conv3(g, s_xin);
+    if (Cc > 0) { g.flags |= EPI_RESIDUAL; g.res = P; g.res_ld = c0; }
+    else { g.flags |= EPI_BIAS; g.bias = h->weights.W("conv_in.bias"); }
+    emit_block_out(g, h->convin_lat, 0, c0, true, "conv_in");
+  }
+
+  // ResnetBlock1D (reference resnet.py:597-612): norm1 + SiLU -> conv1 (+ FiLM bias) -> norm2 (+ FiLM scale / shift) + SiLU ->
+  // conv2, plus the block input or its 1x1 conv_shortcut.  The input is the running tensor, concatenated in the up path with
+  // the popped skip.  Panel mode normalises both inputs inside the convs, with no fp32 h; the 1x1 shortcut reads the raw splits
+  // of the block input(s) as extra 1-tap segments.  Otherwise two prep launches, the first also writing the input's raw split
+  // for the shortcut.  The whole block takes one mode: conv2's shortcut reads the input as conv1's mode leaves it.
+  void emit_resnet(const PlanOp& o) {
+    const ns2vc_unet_cfg& c = h->cfg;
+    const ResnetSite& s = h->resnets[o.site];
+    const int TL = Tl[o.level];
+    const bool panel = xf_ok(s.c1, s.c2) && xf_ok(s.cout, 0);
+    const SplitBuf a_h = view(sc.SP_H, TL, s.cout), a_raw = view(sc.SP_R, TL, s.cin);
+    const Act h1{sc.H1, a_h, s.cout, new_stats(s.cout)};   // conv1's output: its raw split (panel mode) or fp32
+    {
+      GemmOp g = gemm_base(s.conv1, TL);
+      normed_input(g, panel, cur, cat2, s.p + ".norm1", c.norm_eps, PREP_AFFINE_SILU, nullptr, 0, 3, o.level, view(sc.SP_A, TL, s.cin),
+                   s.shortcut ? &a_raw : nullptr);
+      g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv1.bias");
+      if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
+      if (panel) { g.flags |= EPI_OUT_SPLIT; g.out_hi = a_h.hi; g.out_lo = a_h.lo; g.out_split_ld = a_h.ld; }
+      else { g.flags |= EPI_OUT_F32; g.out = h1.p; g.out_ld = s.cout; }
+      with_stats(g, h1.st, s.cout);
+      rag(g, o.level);
+      emit_gemm(g, s.conv1);
+    }
+    {
+      GemmOp g = gemm_base(s.conv2, TL);
+      // panel mode: the raw 1x1 shortcut panels go first: their MMAs run while the transform warps still derive the GroupNorm affine
+      if (s.shortcut && panel) {
+        const int no = nkb_of(s.cout), n1 = nkb_of(s.c1);
+        const int a0 = add_src(g, cur.sp);
+        xseg(g, a0, 0, s.c1, 1, 3 * no, 0, 0, 0);
+        if (s.c2) { const int a1 = add_src(g, cat2.sp); xseg(g, a1, 0, s.c2, 1, 3 * no + n1, 0, 0, 0); }
+      }
+      normed_input(g, panel, h1, Act{}, s.p + ".norm2", c.norm_eps, PREP_AFFINE_SILU, c.time_scale_shift ? film + s.film_off : nullptr,
+                   h->film_total, 3, o.level, a_h);
+      if (s.shortcut && !panel) { const int i = add_src(g, a_raw); seg(g, i, 0, s.cin, 0); }
+      g.flags |= EPI_BIAS; g.bias = s.bias2;
+      if (!s.shortcut) { g.flags |= EPI_RESIDUAL; g.res = cur.p; g.res_ld = s.c1; }
+      emit_block_out(g, s.conv2, o.level, s.cout, o.skip, s.p);
+    }
+    cat2 = Act{};
+  }
+
+  // Transformer1DModel with one BasicTransformerBlock (reference transformer_1d.py, attention.py)
+  void emit_xformer(const PlanOp& o) {
+    const XformerSite& x = h->xformers[o.site];
+    const int TL = Tl[o.level], C = x.c, H = h->cfg.num_heads, dh = C / H;
+    const size_t rows = (size_t)B * TL;
+    const std::string b = x.p + ".transformer_blocks.0";
+    const SplitBuf satt = view(sc.SP_ATT, TL, C), sff = view(sc.SP_FF, TL, 4 * C);
+    // Folded LayerNorms (reference attention.py:83,102,118 nn.LayerNorm): proj_in, out1 and out2 each emit the raw split of
+    // the residual stream into `sln` and its per-row sums; qkv, q2 and ff1 read `sln` - no LayerNorm kernel, no extra pass.
+    const SplitBuf sln = view(sc.SP_LN, TL, C);
+    double* rs1 = new_rowstats(rows); double* rs2 = new_rowstats(rows); double* rs3 = new_rowstats(rows);
+    { GemmOp g = gemm_base(x.proj_in, TL);              // GroupNorm (eps 1e-6) of the block input, then proj_in
+      normed_input(g, xf_ok(C, 0), cur, Act{}, x.p + ".norm", 1e-6f, PREP_AFFINE, nullptr, 0, 1, o.level, view(sc.SP_X, TL, C));
+      g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(x.p + ".proj_in.bias"); g.out = sc.T0; g.out_ld = C;
+      emits_ln_input(g, sln, rs1);
+      rag(g, o.level);
+      emit_gemm(g, x.proj_in); }
+    const bool av2 = !h->simt && attention_v2_supported(dh, TL, false) && attention_v2_supported(dh, S, true);
+    const SplitBuf sqkv = view(sc.SP_QKV, TL, 3 * C), sq2 = view(sc.SP_QKV, TL, C);
+    { GemmOp g = lin(x.qkv, sln, TL);
+      if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sqkv.hi; g.out_lo = sqkv.lo; g.out_split_ld = sqkv.ld;
+                 if (p16(TL)) g.f16_col0 = 2 * C; }
+      else { g.flags = EPI_OUT_F32; g.out = sc.QKV; g.out_ld = 3 * C; }
+      consumes_ln(g, rs1, x.g_qkv, x.bf_qkv, C);
+      emit_gemm(g, x.qkv); }
+    { AttnOp a; memset(&a, 0, sizeof(a));
+      a.q = sc.QKV; a.q_ld = 3 * C; a.k = sc.QKV + C; a.k_ld = 3 * C; a.v = sc.QKV + 2 * C; a.v_ld = 3 * C;
+      a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
+      a.B = B; a.H = H; a.Tq = TL; a.Tk = TL; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
+      // ragged: v2 attends over each entry's own keys (per-entry key count); the fp32 kernel takes a 0 / -inf key bias
+      if (ragged && av2) { a.key_len = rag_lens; a.key_shift = o.level; }
+      else if (ragged) a.bias = pg.rt.key_bias[o.level];
+      if (av2) { a.v2 = 1; a.p_split = p16(TL) ? 0 : 1; a.qs = sqkv; a.ks = sqkv; a.vs = sqkv; a.q_c0 = 0; a.k_c0 = C; a.v_c0 = 2 * C; }
+      emit_attention(a); }
+    { GemmOp g = lin(x.out1, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn1.to_out.0.bias"); g.res = sc.T0; g.res_ld = C; g.out = sc.T1; g.out_ld = C;
+      emits_ln_input(g, sln, rs2);
+      emit_gemm(g, x.out1); }
+    { GemmOp g = lin(x.q2, sln, TL);
+      if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sq2.hi; g.out_lo = sq2.lo; g.out_split_ld = sq2.ld; }
+      else { g.flags = EPI_OUT_F32; g.out = sc.QKV; g.out_ld = C; }
+      consumes_ln(g, rs2, x.g_q2, x.bf_q2, C);
+      emit_gemm(g, x.q2); }
+    { AttnOp a; memset(&a, 0, sizeof(a));
+      a.q = sc.QKV; a.q_ld = C; a.k = kvc + x.kv_off; a.k_ld = h->kv_total; a.v = kvc + x.v_off; a.v_ld = h->kv_total; a.bias = maskbias;
+      a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
+      a.B = B; a.H = H; a.Tq = TL; a.Tk = S; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
+      if (av2) { a.v2 = 1; a.p_split = 1; a.qs = sq2; a.ks = kvs; a.vs = kvs; a.q_c0 = 0; a.k_c0 = x.kv_off; a.v_c0 = x.v_off; }
+      if (ragged) { a.bias = pg.rt.prompt_bias; emit_attention(a); }   // the prompt-length bias of the ragged tables
+      else emit_attention(a, Launch::MASK); }     // the key-padding bias comes from the call's mask (dropped without one)
+    { GemmOp g = lin(x.out2, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn2.to_out.0.bias"); g.res = sc.T1; g.res_ld = C; g.out = sc.T0; g.out_ld = C;
+      emits_ln_input(g, sln, rs3);
+      emit_gemm(g, x.out2); }
+    { GemmOp g = lin(x.ff1, sln, TL); g.flags = EPI_GEGLU | EPI_OUT_SPLIT;
+      g.out_hi = sff.hi; g.out_lo = sff.lo; g.out_split_ld = sff.ld;
+      consumes_ln(g, rs3, x.g_ff1, x.bf_ff1, C); g.flags &= ~EPI_BIAS;   // GEGLU reads its (folded) biases through g.bias itself
+      emit_gemm(g, x.ff1); }
+    { // ff.net.2 + proj_out as one GEMM over K = [GEGLU output | residual stream]:  out = g (Wp W2)^T + h Wp^T + (Wp b2 + bp) + x_in
+      GemmOp g = gemm_base(x.ff2p, TL);
+      const int i0 = add_src(g, sff); seg(g, i0, 0, 4 * C, 0);
+      const int i1 = add_src(g, sln); seg(g, i1, 0, C, 0);          // raw split of the residual stream, written by out2's epilogue
+      g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = x.bias_ff2p; g.res = cur.p; g.res_ld = C;
+      emit_block_out(g, x.ff2p, o.level, C, o.skip, x.p); }
+  }
+
+  // Downsample1D: conv k3 s2 p1:  out[t] = W0 x[2t-1] + W1 x[2t] + W2 x[2t+1] = W0 O[t-1] + W1 E[t] + W2 O[t]
+  // with E[t] = x[2t], O[t] = x[2t+1] decimated by the prep kernel (unit-stride TMA windows).
+  void emit_down(const PlanOp& o) {
+    const ConvSite& s = h->resamplers[o.site];
+    const int TL = Tl[o.level], Tin = Tl[o.level - 1];
+    const int To = Tin / 2;                                  // odd-row count
+    SplitBuf ev = view(sc.SP_A, TL, s.c), od = view(sc.SP_R, std::max(To, 1), s.c);
+    if (xf_on && To >= 1) {
+      // no copy at all: the raw split of the block input seen as row PAIRS [B, ceil(Tin/2), 2*ld] - even rows are the first
+      // half of a pair, odd rows the second (one row fewer when Tin is odd: rows past it are the TMA unit's zero fill)
+      ev = cur.sp; ev.T = TL; ev.ld = 2 * cur.sp.ld; ev.bpitch = (long long)Tin * cur.sp.ld;
+      od = ev; od.hi += cur.sp.ld; od.lo += cur.sp.ld; od.T = To;
+    } else {
+      emit_prep(cur.p, s.c, nullptr, 0, Tin, TL, PREP_RAW, nullptr, nullptr, ev, nullptr, 2, 0);
+      emit_prep(cur.p, s.c, nullptr, 0, Tin, std::max(To, 1), PREP_RAW, nullptr, nullptr, od, nullptr, 2, 1);
+    }
+    GemmOp g = gemm_base(s.w, TL);
+    const int ie = add_src(g, ev), io = add_src(g, od);
+    seg(g, io, 0, s.c, -1); seg(g, ie, 0, s.c, 0); seg(g, io, 0, s.c, 0);
+    g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
+    emit_block_out(g, s.w, o.level, s.c, o.skip, s.p);
+  }
+
+  // Upsample1D: nearest-neighbour 2x (to the finer level's length), then conv k3 p1
+  int emit_up(const PlanOp& o, cudaStream_t st) {
+    const ConvSite& s = h->resamplers[o.site];
+    const int TL = Tl[o.level], Tin = Tl[o.level + 1];
+    // nearest-neighbour source rows of F.interpolate(size=TL) (reference resnet.py:160): a table in the static buffer, filled on
+    // the device with the same fp32 rule as ns2vc_nearest_index() (stream-ordered: no allocation, no host sync)
+    int* map_d = sar.get<int>((size_t)TL);
+    if (!dry) {
+      nearest_index_kernel<<<ceil_div(TL, 256), 256, 0, st>>>(Tin, TL, map_d);
+      NS_CHECK_CUDA(cudaGetLastError());
+    }
+    const SplitBuf up = view(sc.SP_A, TL, s.c);
+    emit_prep(cur.p, s.c, nullptr, 0, Tin, TL, PREP_RAW, nullptr, nullptr, up, nullptr, 1, 0, map_d);
+    // ragged: each entry's rows come from its OWN (T_b,l+1 -> T_b,l) nearest rule (the padded table can differ from it in
+    // fp32), and rows past the entry's length at this level are zeros
+    rag_prep(rag_lens, o.level);
+    GemmOp g = gemm_base(s.w, TL);
+    conv3(g, up);
+    g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
+    emit_block_out(g, s.w, o.level, s.c, o.skip, s.p);
+    return 0;
+  }
+
+  // output head: GN -> SiLU -> conv_out, stored channel-major [B, out_channels, T]
+  void emit_head() {
+    const ns2vc_unet_cfg& c = h->cfg;
+    const int c0 = c.block_out_channels[0];
+    GemmOp g = gemm_base(h->conv_out, T);
+    normed_input(g, xf_ok(c0, 0), cur, Act{}, "conv_norm_out", c.norm_eps, PREP_AFFINE_SILU, nullptr, 0, 3, 0, view(sc.SP_H, T, c0));
+    g.flags = EPI_BIAS | EPI_OUT_NCT; g.bias = h->weights.W("conv_out.bias"); g.out = nullptr;
+    rag(g, 0);                                             // (ragged: output frames past T_b are exact zeros)
+    emit_gemm(g, h->conv_out, Launch::OUT);
+  }
+};
+
 // Builds the programs of (B, T, S, ragged, ws) into *prog, or (ws == nullptr) sizes their workspace into *bytes_out.
 // A ragged program takes no more workspace than the padded one: its tables live in the program's static buffer.
 int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_out, Program* prog, cudaStream_t st = nullptr,
                    bool ragged = false) {
-  const ns2vc_unet_cfg& c = h->cfg;
+  const int nlev = h->cfg.n_levels;
   const bool dry = (ws == nullptr);
-  const int nlev = c.n_levels;
-  const int c0 = c.block_out_channels[0];
-  const int Cl = c.latent_channels, Cc = c.in_channels - Cl;
-  const int xd = c.cross_attention_dim, ted = h->ted;
-  std::vector<int> Tl(nlev);
-  for (int l = 0; l < nlev; ++l) Tl[l] = level_len(T, l);
+  Program pg;
+  Builder bld(h, pg, ws, B, T, S, ragged);
+  const std::vector<int>& Tl = bld.Tl;
   NS_REQUIRE(Tl[nlev - 1] >= 1 && T >= 1 && B >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
   NS_REQUIRE(!ragged || (!h->simt && nlev <= kRagMaxLevels), "ragged programs need the wgmma backend and at most %d levels", kRagMaxLevels);
   std::vector<bool> xf_level(nlev, false);                 // levels with a transformer (their self-attention needs a key bias)
   for (auto& o : h->plan) if (o.kind == PlanOp::XFORMER) xf_level[o.level] = true;
 
-  Program pg;
   if (!dry) {
     // building a program allocates its static tables and copies them to the device: illegal under stream capture (header contract:
     // run a new shape once eagerly first)
@@ -500,8 +859,6 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
       return -1;
     }
   }
-  Builder bld(h, ws, B, &pg.prog_cond);
-  Arena& ar = bld.ar;
   {
     const int n_aff = 2 * (int)h->resnets.size() + (int)h->xformers.size() + 2;
     size_t sbytes = 1024 + (size_t)n_aff * sizeof(PrepOp);
@@ -521,400 +878,35 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
       pg.ragged = true;
       RaggedTables& rt = pg.rt;
       rt.B = B; rt.T = T; rt.S = S; rt.nlev = nlev;
-      rt.lens = bld.sar.get<int>((size_t)2 * B);
+      rt.lens = bld.sar.get<int>((size_t)2 * B);           // content lengths [B] | prompt lengths [B]
       rt.prompt_bias = bld.sar.get<float>((size_t)B * S);
       for (int l = 0; l < nlev; ++l) { rt.Tl[l] = Tl[l]; rt.key_bias[l] = xf_level[l] ? bld.sar.get<float>((size_t)B * Tl[l]) : nullptr; }
       bld.rag_lens = rt.lens;
     }
   }
-  // ragged programs: content lengths (every level derives its own: ceil(T_b / 2^l)) and prompt lengths
-  const int* lens = pg.rt.lens;
-  const int* plens = lens ? lens + B : nullptr;
-  auto rag = [&](GemmOp& g, int level) { g.row_len = lens; g.len_shift = level; };
-  auto rag_prep = [&](const int* len, int level) { PrepOp& p = bld.out->back().get<PrepOp>(); p.row_len = len; p.len_shift = level; };
 
-  // ---- persistent conditioning buffers
-  float* P = (Cc > 0) ? ar.get<float>((size_t)B * T * c0) : nullptr;      // conv_in(content) + bias
-  float* kvc = ar.get<float>((size_t)B * S * std::max(h->kv_total, 1));
-  SplitBuf kvs{};                                                          // the same cache as bf16 hi/lo (attention v2 reads it by TMA)
-  kvs.T = S; kvs.C = std::max(h->kv_total, 8); kvs.ld = pad_to(kvs.C, 8);
-  kvs.hi = ar.get<__nv_bfloat16>((size_t)B * S * kvs.ld);
-  kvs.lo = ar.get<__nv_bfloat16>((size_t)B * S * kvs.ld);
-  float* maskbias = ar.get<float>((size_t)B * S);
-  float* aug = ar.get<float>((size_t)B * ted);
-  // ---- conditioning scratch
-  SplitBuf s_content = (Cc > 0) ? bld.split(T, Cc) : SplitBuf{};
-  SplitBuf s_prompt = bld.split(S, xd);
-  TextTimeEmbedding tte;
-  tte.reserve(ar, B, S, xd, ted);
-
-  // fp16 softmax weights (one P x [V_hi | V_lo] MMA per k-step) only where enough keys average their 2^-12 rounding out: over a few
-  // dozen keys (short prompts, the coarsest levels of short utterances) the weights are a bf16 hi/lo split - those launches are
-  // cheap anyway.  Measured on the reference's 40-step pipeline fixture (S = 40): worst err/tol 1.35 with fp16 weights everywhere.
-  // Only self-attention uses fp16 weights.  Cross-attention keeps the split whatever its key count: a key count cannot see how
-  // sharp the prompt attention is, and with fp16 weights in both attentions, scores of std ~4 (tests/test_numerics_fp64.py,
-  // regime 'sharp' at B=4, T=1024, S=256) put the output at 1.51x the elementwise tolerance against fp64 on an H100.
-  // Ragged programs never use them: entry b of a self-attention attends over its own T_b,l keys, known only on the device, and
-  // one built program serves every length vector, so the padded T_l says nothing about how many keys average the rounding.
-  constexpr int kFp16MinKeys = 256;
-  auto p16 = [&](int keys) { return !ragged && attention_v2_p_fp16() && keys >= kFp16MinKeys; };
-
-  // ================= conditioning program =================
-  if (Cc > 0) {
-    bld.emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, Cc, T, s_content, lens, nullptr, 0}, Launch::CONTENT);
-    GemmOp g = bld.gemm_base(h->convin_content, T);
-    bld.conv3(g, s_content);
-    g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W("conv_in.bias"); g.out = P; g.out_ld = c0;
-    bld.emit_gemm(g, h->convin_content);
-  }
-  bld.emit(Launch::MASKBIAS, MaskBiasOp{nullptr, B * S, maskbias}, Launch::MASK);
-  if (h->kv_total > 0) {
-    bld.emit_prep(nullptr, xd, nullptr, 0, S, S, PREP_RAW, nullptr, nullptr, s_prompt, nullptr, 1, 0, nullptr, Launch::PROMPT);
-    rag_prep(plens, 0);                                    // (ragged: prompt frames past S_b are zeros, so is their K / V)
-    GemmOp g = bld.lin(h->kv_all, s_prompt, S);
-    g.flags = EPI_OUT_F32 | EPI_OUT_SPLIT; g.out = kvc; g.out_ld = h->kv_total;
-    g.out_hi = kvs.hi; g.out_lo = kvs.lo; g.out_split_ld = kvs.ld;   // (V stays a bf16 split: cross-attention weights are split)
-    bld.emit_gemm(g, h->kv_all);
-  }
-  if (c.add_embed_text)   // TextTimeEmbedding of the prompt (embeddings.py:421-434)
-    tte.emit(bld, h->weights, "add_embedding", nullptr, Launch::PROMPT, S, xd, ted, c.add_embed_heads, Launch::POOL_ATT, h->pool_kv, aug, plens);
-
-  // ================= forward program =================
+  bld.emit_cond();
   bld.out = &pg.prog_fwd;
-  // per-step small buffers
-  SplitBuf s_xin = bld.split(T, Cl);
-  float* temb1 = ar.get<float>((size_t)B * ted);
-  float* emb = ar.get<float>((size_t)B * ted);
-  float* film = ar.get<float>((size_t)B * std::max(h->film_total, 1));
-  // per-(b, channel) sum | sum-of-squares of every fp32 activation that feeds a GroupNorm, accumulated by
-  // the producing GEMM epilogues; one contiguous arena, zeroed by one memset at the top of the forward
-  size_t stat_doubles = (size_t)2 * B * c0;
-  for (auto& o : h->plan) {
-    if (o.kind == PlanOp::RESNET) stat_doubles += (size_t)4 * B * o.cout;
-    else if (o.kind == PlanOp::XFORMER || o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) stat_doubles += (size_t)2 * B * o.cout;
-    if (o.kind == PlanOp::XFORMER) stat_doubles += (size_t)3 * 2 * B * Tl[o.level];   // three LayerNorm row-statistics buffers
-  }
-  double* stat_arena = ar.get<double>(stat_doubles);
-  size_t stat_used = 0;
-  auto new_stats = [&](int C) { double* p = stat_arena ? stat_arena + stat_used : nullptr; stat_used += (size_t)2 * B * C; return p; };
-  auto new_rowstats = [&](size_t nrows) { double* p = stat_arena ? stat_arena + stat_used : nullptr; stat_used += 2 * nrows; return p; };
-  auto with_stats = [&](GemmOp& g, double* st_, int C) { g.flags |= EPI_STATS; g.stat_sum = st_; g.stat_sq = st_ ? st_ + (size_t)B * C : nullptr; };
-  bld.emit_memset(stat_arena, stat_doubles * sizeof(double));
-  // activation buffers
-  size_t max_act = (size_t)B * T * c0, max_cat = 0, max_ff = 1, max_qkv = 1;
-  for (auto& o : h->plan) {
-    const size_t rows = (size_t)B * Tl[o.level];
-    if (o.kind == PlanOp::RESNET) { max_act = std::max(max_act, rows * o.cout); max_cat = std::max(max_cat, rows * o.cin); }
-    if (o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) { max_act = std::max(max_act, rows * o.cout); max_cat = std::max(max_cat, rows * o.cout); }
-    if (o.kind == PlanOp::XFORMER) { max_act = std::max(max_act, rows * o.cout); max_ff = std::max(max_ff, rows * 4 * o.cout); max_qkv = std::max(max_qkv, rows * 3 * o.cout); }
-  }
-  max_cat = std::max(max_cat, max_act);
-  float* rot[3]; for (int i = 0; i < 3; ++i) rot[i] = ar.get<float>(max_act);
-  float* H1 = ar.get<float>(max_act);
-  float* T0 = ar.get<float>(max_act);
-  float* T1 = ar.get<float>(max_act);
-  float* QKV = ar.get<float>(max_qkv);
-  auto scratch_split = [&](size_t elems) { SplitBuf s{}; s.hi = ar.get<__nv_bfloat16>(elems); s.lo = ar.get<__nv_bfloat16>(elems); return s; };
-  const SplitBuf SP_A = scratch_split(max_cat);      // conv1 / resample input
-  const SplitBuf SP_R = scratch_split(max_cat);      // raw shortcut operand / odd rows of a stride-2 conv
-  const SplitBuf SP_H = scratch_split(max_act);      // conv2 input, out-head input
-  const SplitBuf SP_X = scratch_split(max_act);      // GN-normalised transformer input (when the GroupNorm is a prep launch)
-  const SplitBuf SP_ATT = scratch_split(max_act);    // attention output
-  const SplitBuf SP_FF = scratch_split(max_ff);      // GEGLU output
-  const SplitBuf SP_QKV = scratch_split(max_qkv);    // q | k | v of the self-attention (q of the cross-attention)
-  const SplitBuf SP_LN = scratch_split(max_act);     // raw (un-normalised) split of the transformer's residual stream (folded LayerNorms)
-
-  // entry: x -> split tokens, time path, conv_in
-  bld.emit(Launch::NCT2SPLIT, NctSplitOp{nullptr, 0, B, Cl, T, s_xin, lens, nullptr, 0}, Launch::X);
-  {
-    LinOp tp[3];
-    const int n = time_path_ops(h, nullptr, B, B, aug, temb1, emb, film, tp);
-    for (int i = 0; i < n; ++i) bld.emit_linear(tp[i], i == 0 ? Launch::T : Launch::NONE, 1);
-  }
-
-  // An activation that leaves a block: fp32 token-major tensor, its raw bf16 hi/lo split (the A operand of the panel-mode
-  // GEMMs that consume it; written by the same epilogue) and the per-(b, channel) sums for the consumer's GroupNorm.
-  struct Act { float* p = nullptr; SplitBuf sp{}; int c = 0; double* st = nullptr; };
-  const bool xf_on = !h->simt;
-  SplitBuf rot_sp[3];
-  for (int i = 0; i < 3; ++i) rot_sp[i] = xf_on ? scratch_split(max_act) : SplitBuf{};
-  std::vector<Act> skips;
-  int rot_i = 0;
-  auto next_out = [&](bool is_skip, int TLn, int C) -> Act {
-    Act a; a.c = C;
-    const size_t elems = (size_t)B * TLn * C;
-    if (is_skip) { a.p = ar.get<float>(elems); if (xf_on) a.sp = Builder::view(scratch_split((size_t)B * TLn * pad_to(C, 8)), TLn, C); }
-    else { a.p = rot[rot_i]; if (xf_on) a.sp = Builder::view(rot_sp[rot_i], TLn, C); rot_i = (rot_i + 1) % 3; }
-    return a;
-  };
-  auto emits_block_out = [&](GemmOp& g, const Act& a) {       // fp32 + (panel mode) raw split of a block output
-    g.flags |= EPI_OUT_F32; g.out = a.p; g.out_ld = a.c;
-    if (xf_on) { g.flags |= EPI_OUT_SPLIT; g.out_hi = a.sp.hi; g.out_lo = a.sp.lo; g.out_split_ld = a.sp.ld; }
-  };
-  // Can the GroupNorm in front of a GEMM over (cur [+ skip]) channels run inside the GEMM?  (64-channel blocks may not
-  // straddle the concat seam; the affine table holds kXfMaxC channels)
-  auto xf_ok = [&](int c1, int c2) { return xf_on && (c2 == 0 || c1 % 64 == 0) && c1 + c2 <= kXfMaxC && c.norm_num_groups <= 64; };
-  auto followed_by_push = [&](size_t i) { return i + 1 < h->plan.size() && h->plan[i + 1].kind == PlanOp::PUSH; };
-
-  Act cur;
-  {
-    Act o = next_out(true, T, c0);                      // conv_in output is the first skip
-    GemmOp g = bld.gemm_base(h->convin_lat, T);
-    bld.conv3(g, s_xin);
-    if (Cc > 0) { g.flags |= EPI_RESIDUAL; g.res = P; g.res_ld = c0; }
-    else { g.flags |= EPI_BIAS; g.bias = h->weights.W("conv_in.bias"); }
-    emits_block_out(g, o);
-    o.st = new_stats(c0);
-    with_stats(g, o.st, c0);
-    rag(g, 0);
-    bld.emit_gemm(g, h->convin_lat);
-    cur = o;
-    bld.emit_tap(pg.taps, "conv_in", cur.p, 0, c0, T);
-  }
-  Act cat2;                                              // pending concat source
-  size_t ri = 0, xi = 0, si = 0;
-  for (size_t pi = 0; pi < h->plan.size(); ++pi) {
-    const PlanOp& o = h->plan[pi];
-    const int TL = Tl[o.level];
-    const size_t rows = (size_t)B * TL;
+  bld.reserve_forward();
+  bld.emit_entry();
+  for (const PlanOp& o : h->plan) {
     switch (o.kind) {
-      case PlanOp::PUSH: skips.push_back(cur); break;
-      case PlanOp::POP_CAT: cat2 = skips.back(); skips.pop_back(); break;
-      case PlanOp::RESNET: {
-        const ResnetSite& s = h->resnets[ri++];
-        const float* s1 = cur.p; const float* s2 = s.c2 ? cat2.p : nullptr;
-        const SplitBuf a_h = Builder::view(SP_H, TL, s.cout);
-        double* h1_st = new_stats(s.cout);
-        Act outp = next_out(followed_by_push(pi), TL, s.cout);
-        outp.st = new_stats(s.cout);
-        if (xf_ok(s.c1, s.c2) && s.cout <= kXfMaxC) {
-          // Panel mode: norm1 + SiLU inside conv1, norm2 (+FiLM) + SiLU inside conv2 (reference resnet.py:597-612); the
-          // 1x1 shortcut reads the raw splits of the block input(s) as extra 1-tap segments.  No prep launch, no fp32 h.
-          const int ni = nkb_of(s.cin), n1 = nkb_of(s.c1), no = nkb_of(s.cout);
-          {
-            GemmOp g = bld.gemm_base(s.conv1, TL);
-            const int i0 = bld.add_src(g, cur.sp);
-            bld.xseg(g, i0, 0, s.c1, 3, 0, ni, 1, 0);
-            if (s.c2) { const int i1 = bld.add_src(g, cat2.sp); bld.xseg(g, i1, 0, s.c2, 3, n1, ni, 1, s.c1); }
-            g.pre = bld.affine_desc(cur.st, s.c1, s.c2 ? cat2.st : nullptr, s.c2, TL, PREP_AFFINE_SILU, c.norm_eps,
-                                    h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), 0, o.level);
-            g.flags = EPI_BIAS | EPI_OUT_SPLIT; g.bias = h->weights.W(s.p + ".conv1.bias");
-            if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
-            g.out_hi = a_h.hi; g.out_lo = a_h.lo; g.out_split_ld = a_h.ld;
-            with_stats(g, h1_st, s.cout);
-            rag(g, o.level);
-            bld.emit_gemm(g, s.conv1);
-          }
-          {
-            GemmOp g = bld.gemm_base(s.conv2, TL);
-            g.flags = EPI_BIAS; g.bias = s.bias2;
-            // the raw 1x1 shortcut panels go first: their MMAs run while the transform warps still derive the GroupNorm affine
-            if (s.shortcut) {
-              const int a0 = bld.add_src(g, cur.sp);
-              bld.xseg(g, a0, 0, s.c1, 1, 3 * no, 0, 0, 0);
-              if (s.c2) { const int a1 = bld.add_src(g, cat2.sp); bld.xseg(g, a1, 0, s.c2, 1, 3 * no + n1, 0, 0, 0); }
-            } else { g.flags |= EPI_RESIDUAL; g.res = s1; g.res_ld = s.c1; }
-            const int j0 = bld.add_src(g, a_h);
-            bld.xseg(g, j0, 0, s.cout, 3, 0, no, 1, 0);
-            g.pre = bld.affine_desc(h1_st, s.cout, nullptr, 0, TL, PREP_AFFINE_SILU, c.norm_eps, h->weights.W(s.p + ".norm2.weight"),
-                                    h->weights.W(s.p + ".norm2.bias"), h->film_total, o.level);
-            g.pre_film = c.time_scale_shift ? film + s.film_off : nullptr;
-            emits_block_out(g, outp);
-            with_stats(g, outp.st, s.cout);
-            rag(g, o.level);
-            bld.emit_gemm(g, s.conv2);
-          }
-        } else {
-          const SplitBuf a_in = Builder::view(SP_A, TL, s.cin), a_raw = Builder::view(SP_R, TL, s.cin);
-          bld.emit_prep_gn(s1, s.c1, cur.st, s2, s.c2, s.c2 ? cat2.st : nullptr, TL, PREP_AFFINE_SILU, c.norm_eps,
-                           h->weights.W(s.p + ".norm1.weight"), h->weights.W(s.p + ".norm1.bias"), nullptr, 0, a_in, s.shortcut ? &a_raw : nullptr);
-          rag_prep(lens, o.level);
-          {
-            GemmOp g = bld.gemm_base(s.conv1, TL);
-            bld.conv3(g, a_in);
-            g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(s.p + ".conv1.bias");
-            if (!c.time_scale_shift) { g.flags |= EPI_ROWBIAS; g.rowbias = film + s.film_off; g.rowbias_ld = h->film_total; }
-            g.out = H1; g.out_ld = s.cout;
-            with_stats(g, h1_st, s.cout);
-            rag(g, o.level);
-            bld.emit_gemm(g, s.conv1);
-          }
-          // norm2 (+FiLM scale/shift) + SiLU (reference resnet.py:602-612)
-          bld.emit_prep_gn(H1, s.cout, h1_st, nullptr, 0, nullptr, TL, PREP_AFFINE_SILU, c.norm_eps, h->weights.W(s.p + ".norm2.weight"),
-                           h->weights.W(s.p + ".norm2.bias"), c.time_scale_shift ? film + s.film_off : nullptr, h->film_total, a_h);
-          rag_prep(lens, o.level);
-          {
-            GemmOp g = bld.gemm_base(s.conv2, TL);
-            bld.conv3(g, a_h);
-            g.flags = EPI_BIAS; g.bias = s.bias2;
-            if (s.shortcut) { const int i = bld.add_src(g, a_raw); bld.seg(g, i, 0, s.cin, 0); }
-            else { g.flags |= EPI_RESIDUAL; g.res = s1; g.res_ld = s.c1; }
-            emits_block_out(g, outp);
-            with_stats(g, outp.st, s.cout);
-            rag(g, o.level);
-            bld.emit_gemm(g, s.conv2);
-          }
-        }
-        cur = outp; cat2 = Act{};
-        bld.emit_tap(pg.taps, s.p, cur.p, o.level, cur.c, TL);
-        break;
-      }
-      case PlanOp::XFORMER: {
-        const XformerSite& x = h->xformers[xi++];
-        const int C = x.c, H = c.num_heads, dh = C / H;
-        const std::string b = x.p + ".transformer_blocks.0";
-        const SplitBuf sx = Builder::view(SP_X, TL, C), satt = Builder::view(SP_ATT, TL, C), sff = Builder::view(SP_FF, TL, 4 * C);
-        const bool xin = xf_ok(C, 0);                        // GroupNorm(eps 1e-6) of the block input applied inside proj_in
-        if (!xin) {
-          bld.emit_prep_gn(cur.p, C, cur.st, nullptr, 0, nullptr, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), nullptr, 0, sx);
-          rag_prep(lens, o.level);
-        }
-        // Folded LayerNorms (reference attention.py:83,102,118 nn.LayerNorm): proj_in, out1 and out2 each emit the raw split of
-        // the residual stream into `sln` and its per-row sums; qkv, q2 and ff1 read `sln` - no LayerNorm kernel, no extra pass.
-        const SplitBuf sln = Builder::view(SP_LN, TL, C);
-        double* rs1 = new_rowstats(rows); double* rs2 = new_rowstats(rows); double* rs3 = new_rowstats(rows);
-        { GemmOp g = xin ? bld.gemm_base(x.proj_in, TL) : bld.lin(x.proj_in, sx, TL);
-          if (xin) {
-            const int i0 = bld.add_src(g, cur.sp);
-            bld.xseg(g, i0, 0, C, 1, 0, 0, 1, 0);
-            g.pre = bld.affine_desc(cur.st, C, nullptr, 0, TL, PREP_AFFINE, 1e-6f, h->weights.W(x.p + ".norm.weight"), h->weights.W(x.p + ".norm.bias"), 0, o.level);
-          }
-          g.flags = EPI_BIAS | EPI_OUT_F32; g.bias = h->weights.W(x.p + ".proj_in.bias"); g.out = T0; g.out_ld = C;
-          bld.emits_ln_input(g, sln, rs1);
-          rag(g, o.level);
-          bld.emit_gemm(g, x.proj_in); }
-        const bool av2 = !h->simt && attention_v2_supported(dh, TL, false) && attention_v2_supported(dh, S, true);
-        const SplitBuf sqkv = Builder::view(SP_QKV, TL, 3 * C), sq2 = Builder::view(SP_QKV, TL, C);
-        { GemmOp g = bld.lin(x.qkv, sln, TL);
-          if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sqkv.hi; g.out_lo = sqkv.lo; g.out_split_ld = sqkv.ld;
-                     if (p16(TL)) g.f16_col0 = 2 * C; }
-          else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = 3 * C; }
-          bld.consumes_ln(g, rs1, x.g_qkv, x.bf_qkv, C);
-          bld.emit_gemm(g, x.qkv); }
-        { AttnOp a; memset(&a, 0, sizeof(a));
-          a.q = QKV; a.q_ld = 3 * C; a.k = QKV + C; a.k_ld = 3 * C; a.v = QKV + 2 * C; a.v_ld = 3 * C;
-          a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
-          a.B = B; a.H = H; a.Tq = TL; a.Tk = TL; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
-          // ragged: v2 attends over each entry's own keys (per-entry key count); the fp32 kernel takes a 0 / -inf key bias
-          if (ragged && av2) { a.key_len = lens; a.key_shift = o.level; }
-          else if (ragged) a.bias = pg.rt.key_bias[o.level];
-          if (av2) { a.v2 = 1; a.p_split = p16(TL) ? 0 : 1; a.qs = sqkv; a.ks = sqkv; a.vs = sqkv; a.q_c0 = 0; a.k_c0 = C; a.v_c0 = 2 * C; }
-          bld.emit_attention(a); }
-        { GemmOp g = bld.lin(x.out1, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn1.to_out.0.bias"); g.res = T0; g.res_ld = C; g.out = T1; g.out_ld = C;
-          bld.emits_ln_input(g, sln, rs2);
-          bld.emit_gemm(g, x.out1); }
-        { GemmOp g = bld.lin(x.q2, sln, TL);
-          if (av2) { g.flags = EPI_OUT_SPLIT; g.out_hi = sq2.hi; g.out_lo = sq2.lo; g.out_split_ld = sq2.ld; }
-          else { g.flags = EPI_OUT_F32; g.out = QKV; g.out_ld = C; }
-          bld.consumes_ln(g, rs2, x.g_q2, x.bf_q2, C);
-          bld.emit_gemm(g, x.q2); }
-        { AttnOp a; memset(&a, 0, sizeof(a));
-          a.q = QKV; a.q_ld = C; a.k = kvc + x.kv_off; a.k_ld = h->kv_total; a.v = kvc + x.v_off; a.v_ld = h->kv_total; a.bias = maskbias;
-          a.out_hi = satt.hi; a.out_lo = satt.lo; a.out_split_ld = satt.ld;
-          a.B = B; a.H = H; a.Tq = TL; a.Tk = S; a.dh = dh; a.scale = 1.0f / sqrtf((float)dh);
-          if (av2) { a.v2 = 1; a.p_split = 1; a.qs = sq2; a.ks = kvs; a.vs = kvs; a.q_c0 = 0; a.k_c0 = x.kv_off; a.v_c0 = x.v_off; }
-          if (ragged) { a.bias = pg.rt.prompt_bias; bld.emit_attention(a); }   // the prompt-length bias of the ragged tables
-          else bld.emit_attention(a, Launch::MASK); }     // the key-padding bias comes from the call's mask (dropped without one)
-        { GemmOp g = bld.lin(x.out2, satt, TL); g.flags = EPI_BIAS | EPI_RESIDUAL | EPI_OUT_F32; g.bias = h->weights.W(b + ".attn2.to_out.0.bias"); g.res = T1; g.res_ld = C; g.out = T0; g.out_ld = C;
-          bld.emits_ln_input(g, sln, rs3);
-          bld.emit_gemm(g, x.out2); }
-        { GemmOp g = bld.lin(x.ff1, sln, TL); g.flags = EPI_GEGLU | EPI_OUT_SPLIT;
-          g.out_hi = sff.hi; g.out_lo = sff.lo; g.out_split_ld = sff.ld;
-          bld.consumes_ln(g, rs3, x.g_ff1, x.bf_ff1, C); g.flags &= ~EPI_BIAS;   // GEGLU reads its (folded) biases through g.bias itself
-          bld.emit_gemm(g, x.ff1); }
-        Act outp = next_out(followed_by_push(pi), TL, C);
-        outp.st = new_stats(C);
-        { // ff.net.2 + proj_out as one GEMM over K = [GEGLU output | residual stream]:  out = g (Wp W2)^T + h Wp^T + (Wp b2 + bp) + x_in
-          GemmOp g = bld.gemm_base(x.ff2p, TL);
-          const int i0 = bld.add_src(g, sff); bld.seg(g, i0, 0, 4 * C, 0);
-          const int i1 = bld.add_src(g, sln); bld.seg(g, i1, 0, C, 0);          // raw split of the residual stream, written by out2's epilogue
-          g.flags = EPI_BIAS | EPI_RESIDUAL; g.bias = x.bias_ff2p; g.res = cur.p; g.res_ld = C;
-          emits_block_out(g, outp); with_stats(g, outp.st, C); rag(g, o.level); bld.emit_gemm(g, x.ff2p); }
-        cur = outp;
-        bld.emit_tap(pg.taps, x.p, cur.p, o.level, C, TL);
-        break;
-      }
-      case PlanOp::DOWN: {
-        // conv k3 s2 p1:  out[t] = W0 x[2t-1] + W1 x[2t] + W2 x[2t+1] = W0 O[t-1] + W1 E[t] + W2 O[t]
-        // with E[t] = x[2t], O[t] = x[2t+1] decimated by the prep kernel (unit-stride TMA windows).
-        const ConvSite& s = h->resamplers[si++];
-        const int Tin = Tl[o.level - 1];
-        const int To = Tin / 2;                                  // odd-row count
-        SplitBuf ev = Builder::view(SP_A, TL, s.c), od = Builder::view(SP_R, std::max(To, 1), s.c);
-        if (xf_on && To >= 1) {
-          // no copy at all: the raw split of the block input seen as row PAIRS [B, ceil(Tin/2), 2*ld] - even rows are the first
-          // half of a pair, odd rows the second (one row fewer when Tin is odd: rows past it are the TMA unit's zero fill)
-          ev = cur.sp; ev.T = TL; ev.ld = 2 * cur.sp.ld; ev.bpitch = (long long)Tin * cur.sp.ld;
-          od = ev; od.hi += cur.sp.ld; od.lo += cur.sp.ld; od.T = To;
-        } else {
-          bld.emit_prep(cur.p, s.c, nullptr, 0, Tin, TL, PREP_RAW, nullptr, nullptr, ev, nullptr, 2, 0);
-          bld.emit_prep(cur.p, s.c, nullptr, 0, Tin, std::max(To, 1), PREP_RAW, nullptr, nullptr, od, nullptr, 2, 1);
-        }
-        Act outp = next_out(followed_by_push(pi), TL, s.c);
-        outp.st = new_stats(s.c);
-        GemmOp g = bld.gemm_base(s.w, TL);
-        const int ie = bld.add_src(g, ev), io = bld.add_src(g, od);
-        bld.seg(g, io, 0, s.c, -1); bld.seg(g, ie, 0, s.c, 0); bld.seg(g, io, 0, s.c, 0);
-        g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
-        emits_block_out(g, outp); with_stats(g, outp.st, s.c);
-        rag(g, o.level);
-        bld.emit_gemm(g, s.w);
-        cur = outp;
-        bld.emit_tap(pg.taps, s.p, cur.p, o.level, s.c, TL);
-        break;
-      }
-      case PlanOp::UP: {
-        const ConvSite& s = h->resamplers[si++];
-        const int Tin = Tl[o.level + 1];
-        // nearest-neighbour source rows of F.interpolate(size=TL) (reference resnet.py:160): a table in the workspace, filled on
-        // the device with the same fp32 rule as ns2vc_nearest_index() (stream-ordered: no allocation, no host sync)
-        int* map_d = bld.sar.get<int>((size_t)TL);
-        if (!dry) {
-          nearest_index_kernel<<<ceil_div(TL, 256), 256, 0, st>>>(Tin, TL, map_d);
-          NS_CHECK_CUDA(cudaGetLastError());
-        }
-        const SplitBuf up = Builder::view(SP_A, TL, s.c);
-        bld.emit_prep(cur.p, s.c, nullptr, 0, Tin, TL, PREP_RAW, nullptr, nullptr, up, nullptr, 1, 0, map_d);
-        // ragged: each entry's rows come from its OWN (T_b,l+1 -> T_b,l) nearest rule (the padded table can differ from it in
-        // fp32), and rows past the entry's length at this level are zeros
-        rag_prep(lens, o.level);
-        Act outp = next_out(followed_by_push(pi), TL, s.c);
-        outp.st = new_stats(s.c);
-        GemmOp g = bld.gemm_base(s.w, TL);
-        bld.conv3(g, up);
-        g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
-        emits_block_out(g, outp); with_stats(g, outp.st, s.c);
-        rag(g, o.level);
-        bld.emit_gemm(g, s.w);
-        cur = outp;
-        bld.emit_tap(pg.taps, s.p, cur.p, o.level, s.c, TL);
-        break;
-      }
+      case PlanOp::PUSH: bld.skips.push_back(bld.cur); break;
+      case PlanOp::POP_CAT: bld.cat2 = bld.skips.back(); bld.skips.pop_back(); break;
+      case PlanOp::RESNET: bld.emit_resnet(o); break;
+      case PlanOp::XFORMER: bld.emit_xformer(o); break;
+      case PlanOp::DOWN: bld.emit_down(o); break;
+      case PlanOp::UP: { const int rc = bld.emit_up(o, st); if (rc) return rc; break; }
     }
   }
-  // output head: GN -> SiLU -> conv_out, stored channel-major [B, out_channels, T]
-  {
-    const SplitBuf a_h = Builder::view(SP_H, T, c0);
-    GemmOp g = bld.gemm_base(h->conv_out, T);
-    if (xf_ok(c0, 0)) {
-      const int i0 = bld.add_src(g, cur.sp);
-      bld.xseg(g, i0, 0, c0, 3, 0, nkb_of(c0), 1, 0);
-      g.pre = bld.affine_desc(cur.st, c0, nullptr, 0, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), 0, 0);
-    } else {
-      bld.emit_prep_gn(cur.p, c0, cur.st, nullptr, 0, nullptr, T, PREP_AFFINE_SILU, c.norm_eps, h->weights.W("conv_norm_out.weight"), h->weights.W("conv_norm_out.bias"), nullptr, 0, a_h);
-      rag_prep(lens, 0);
-      bld.conv3(g, a_h);
-    }
-    g.flags = EPI_BIAS | EPI_OUT_NCT; g.bias = h->weights.W("conv_out.bias"); g.out = nullptr;
-    rag(g, 0);                                             // (ragged: output frames past T_b are exact zeros)
-    bld.emit_gemm(g, h->conv_out, Launch::OUT);
-  }
+  bld.emit_head();
+
   if (!bld.err && bld.upload_affine(st)) { set_error("affine descriptor upload failed"); return -2; }
   if (bld.err) return bld.err;
-  if (bytes_out) *bytes_out = ar.off + 256;
+  if (bytes_out) *bytes_out = bld.ar.off + 256;
   if (!dry) {
     pg.B = B; pg.T = T; pg.S = S; pg.ws = ws;
-    pg.film_base = film; pg.aug = aug;
+    pg.film_base = bld.film; pg.aug = bld.aug;
     *prog = std::move(pg);
   }
   return 0;

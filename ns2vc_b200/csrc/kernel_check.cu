@@ -104,7 +104,7 @@ int ns2vc_check_gemm(const ns2vc_check_gemm_args* a, char* desc, int desc_len, n
       p.C1 = a->pre_C;
       p.scale = a->pre_scale; p.shift = a->pre_shift;
     } else {
-      // the GroupNorm descriptor as the denoiser's affine_desc builds it; the FiLM rows travel in GemmOp::pre_film
+      // the GroupNorm descriptor as the denoiser's normed_input builds it in panel mode; the FiLM rows travel in GemmOp::pre_film
       const int Cg = a->gn_C1 + a->gn_C2;
       NS_REQUIRE(a->gn_C1 >= 1 && a->gn_C2 >= 0 && (a->gn_C2 == 0) == (a->gn_stats2 == nullptr) && Cg <= kXfMaxC,
                  "check_gemm: GroupNorm sources %d + %d channels (up to %d)", a->gn_C1, a->gn_C2, kXfMaxC);
