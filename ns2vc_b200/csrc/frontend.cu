@@ -226,7 +226,8 @@ log_mel_kernel(const float* __restrict__ x, long long x_bstride, long long n, co
       const float* w = t.weights + __ldg(t.band_off + m);
       float acc = 0.f;
       for (int i = 0; i < band.y; ++i) acc = fmaf(__ldg(w + i), mag[band.x + i], acc);
-      s_mel[m * kMelPitch + f] = logf(fmaxf(acc, 1e-7f));
+      // torch.clip(., min=1e-7) keeps NaN (fmaxf would return 1e-7 for it): a NaN sample reaches the prompt mel as NaN
+      s_mel[m * kMelPitch + f] = logf(acc < 1e-7f ? 1e-7f : acc);
     }
   }
   __syncthreads();
@@ -305,7 +306,7 @@ int ns2vc_resampler_create(int orig_freq, int new_freq, ns2vc_resampler** out) {
       range.push_back(make_int2(lo, hi));
     }
   }
-  const Ratio& r = h->r;
+  const Ratio r = h->r;                                     // a copy: the refusal below reads it after deleting h
   h->window = (int)std::min<long long>((long long)((kResThreads - 1) / r.nw + 1) * r.orig + r.taps, INT32_MAX);
   if (h->window > kResMaxWindow) {
     delete h;

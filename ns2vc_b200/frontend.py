@@ -159,7 +159,11 @@ def resample(wav: torch.Tensor, orig_freq: int, new_freq: int,
 
     Row b equals ``torchaudio.transforms.Resample(orig_freq, new_freq)(wav[b, :lengths[b]])`` (sinc_interp_hann,
     lowpass_filter_width 6, rolloff 0.99) up to fp32 summation order; samples at or past ``out_lengths[b]`` are exactly 0.
-    ``N_out = resample_out_length(orig_freq, new_freq, N)``.  orig_freq == new_freq gives a copy."""
+    ``N_out = resample_out_length(orig_freq, new_freq, N)``.  orig_freq == new_freq gives a copy.
+
+    A NaN input sample makes NaN exactly the outputs whose nonzero taps cover it; the others are unchanged.  torchaudio also
+    multiplies the exact-zero taps at each phase's ends, so there a NaN reaches a few samples further; downstream the
+    utterance is NaN either way."""
     if int(orig_freq) <= 0 or int(new_freq) <= 0:
         raise ValueError(f"resample: bad rates {orig_freq} -> {new_freq}")
     x, squeeze, host = _rows(wav, lengths)
@@ -179,7 +183,12 @@ def log_mel_spectrogram(wav: torch.Tensor, sample_rate: int = MEL_SAMPLE_RATE,
     hop_length=256, n_mels=100, center=True, power=1)`` of ``wav[b, :lengths[b]]`` with the reflect padding at that row's own
     ends, then ``log(max(., 1e-7))``.  ``frame_lengths[b] = 1 + len24k[b] // 256``; frames past it are exactly 0 (the layout of
     the reference's collate, dataset.py:151-173), ``S = 1 + N24k // 256``.  A 24 kHz row of 512 samples or fewer raises
-    ValueError, as torch's reflect padding does."""
+    ValueError, as torch's reflect padding does.
+
+    The clip keeps NaN, as ``torch.clip`` does: a NaN 24 kHz sample makes NaN every band of exactly the frames whose
+    reflect-padded window holds it (mirrored positions near both ends included), and +-Inf makes those frames non-finite in
+    every band with a nonzero weight; every other frame is unchanged.  A NaN prompt mel then fails its conversion with the
+    reference's AssertionError (model.py:404) rather than passing as silence."""
     sr = int(sample_rate)
     if sr <= 0:
         raise ValueError(f"log_mel_spectrogram: bad sample rate {sample_rate}")

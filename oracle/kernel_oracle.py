@@ -573,3 +573,257 @@ def istft_rows(h: torch.Tensor, window: torch.Tensor, hop: int, L: Sequence[int]
         out[b, :Lb * hop] = y[pad:pad + Lb * hop] / env[pad:pad + Lb * hop]
     return out
 
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Prompt-mel front end: resample_kernel and log_mel_kernel (csrc/frontend.cu), tests/test_frontend_kernels_fp64.py.  Each
+# reference takes one row alone, in fp64 on the kernel's own fp32 input and fp32 tables, with a switch per defect so the tests
+# can show each bound would notice it.
+# ---------------------------------------------------------------------------------------------------------------------------
+U53 = 2.0 ** -53
+MEL_CLIP = float(torch.tensor(1e-7, dtype=torch.float32))          # the kernel's 1e-7f; torch.clip(fp32, 1e-7) clips at it too
+
+
+def resample_trim(table: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(first, last) nonzero tap of each phase of a [nw, taps] table: the range the kernel's loop runs over"""
+    nz = table != 0
+    taps = table.shape[1]
+    idx = torch.arange(taps, device=table.device)
+    lo = torch.where(nz, idx, taps).amin(1)
+    hi = torch.where(nz, idx, -1).amax(1)
+    return lo, hi
+
+
+def resample_width(orig: int, nw: int) -> int:
+    """lowpass width of the reduced ratio orig:nw, ceil(6 orig / (0.99 min(orig, nw))) as the host computes it; 0 for the
+    identity"""
+    return 0 if orig == nw else math.ceil(6.0 * orig / (min(orig, nw) * 0.99))
+
+
+def sinc_table64(orig: int, nw: int, width: int) -> torch.Tensor:
+    """torchaudio's phase table of the reduced ratio orig:nw built for lowpass width `width` (fp32 phase offsets, the rest in
+    fp64, not rounded): [nw, 2 width + orig] fp64.  At the ratio's own width it is the fp64 value of the handle's table."""
+    base = min(orig, nw) * 0.99
+    idx = torch.arange(-width, width + orig, dtype=F64)[None] / orig
+    t = (torch.arange(0, -nw, -1, dtype=torch.float32)[:, None] / nw).to(F64) + idx
+    t = (t * base).clamp(-6, 6)
+    window = torch.cos(t * math.pi / 6 / 2) ** 2
+    t = t * math.pi
+    k = torch.where(t == 0, torch.ones((), dtype=F64), t.sin() / t)
+    return k * (window * (base / orig))
+
+
+def resample_out_len(orig: int, nw: int, n: int) -> int:
+    """ceil(fp32(nw n / orig)), the fp64 quotient rounded to fp32 (torchaudio's length rule); n for the identity"""
+    if orig == nw:
+        return n
+    return int(math.ceil(float(torch.tensor(nw * n / orig, dtype=torch.float32))))
+
+
+def _resample_windows(x: torch.Tensor, L: int, orig: int, width: int, taps: int, K: int, shift: int = 0) -> torch.Tensor:
+    """[K, taps] fp64: window k holds x[k orig - width + shift + i], i < taps, zero outside [0, L)"""
+    front = width + 1
+    xp = torch.zeros(front + (K - 1) * orig + taps + 2, dtype=F64, device=x.device)
+    n = max(0, min(L, xp.numel() - front))
+    xp[front:front + n] = x[:n].to(F64)
+    return xp[1 + shift:].unfold(0, taps, orig)[:K]
+
+
+def resample_rows(x: torch.Tensor, L: int, table: torch.Tensor, orig: int, nw: int, width: int, n_out: int, shift: int = 0,
+                  phase_plus_one: bool = False, width_delta: int = 0, fp32_acc: bool = False) -> torch.Tensor:
+    """One row of resample_kernel: output j < L_out (the length rule at the row's L) is sum_i table[j mod nw][i] x[(j div nw) orig
+    - width + i] over the row's first L samples, later outputs 0.  [n_out] fp64.  table [nw, taps] (fp32 values: truth A; the
+    fp64 table: truth B's arithmetic).  Defects: shift (every tap reads one input sample later), phase_plus_one (phase p reads
+    table row p + 1), width_delta (a table built for width + delta applied at the handle's width), fp32_acc (the sum in fp32,
+    one fmaf per tap in tap order)."""
+    if width_delta:
+        table = sinc_table64(orig, nw, width + width_delta)
+    if phase_plus_one:
+        table = table.roll(-1, 0)
+    taps = table.shape[1]
+    L_out = min(resample_out_len(orig, nw, L), n_out)
+    out = torch.zeros(n_out, dtype=F64, device=x.device)
+    if L_out <= 0:
+        return out
+    K = (L_out + nw - 1) // nw
+    win = _resample_windows(x, L, orig, width, taps, K, shift)
+    w = table.to(F64)
+    if fp32_acc:
+        acc = torch.zeros(K, nw, dtype=F64, device=x.device)
+        for i in range(taps):
+            acc = (win[:, i:i + 1] * w[None, :, i] + acc).float().to(F64)
+        y = acc
+    else:
+        y = win @ w.T
+    out[:L_out] = y.reshape(-1)[:L_out]
+    return out
+
+
+def resample_abs_sum(x: torch.Tensor, L: int, table: torch.Tensor, orig: int, nw: int, width: int, n_out: int) -> torch.Tensor:
+    """sum_i |table[p][i]| |x[...]| of each output, the scale of every rounding of the convolution: [n_out] fp64"""
+    return resample_rows(x.abs(), L, table.abs(), orig, nw, width, n_out)
+
+
+def resample_terms_a(y: torch.Tensor, absum: torch.Tensor, taps: int) -> torch.Tensor:
+    """The kernel's error against truth A (the fp64 convolution on its own fp32 table), per output: it multiplies and adds in
+    fp64 (each fma rounds at 2^-53 of a partial sum no larger than sum |w||x|: taps 2^-53 sum |w||x|) and rounds once to fp32
+    (2^-24 |y|, and 2^-150 below fp32's normal range).  The fp64 reference's own summation adds the same taps 2^-53 sum |w||x|
+    again."""
+    return U32 * y.abs() + 2 * taps * U53 * absum + 2.0 ** -150
+
+
+def resample_terms_b(absum: torch.Tensor) -> torch.Tensor:
+    """What truth B (the recipe in fp64 on the fp64 table) adds to the parity rule: the table's rounding to fp32, 2^-24 of each
+    |w|, so 2^-24 sum |w||x|"""
+    return U32 * absum
+
+
+def _reflect_index(L: int, F: int, frame_offset: int = 0, about_L: bool = False, device=None) -> torch.Tensor:
+    """[F, 1024] sample index of tap t of frame f: 256 f + t - 512 reflected about sample 0 and about sample L - 1 (center=True,
+    pad_mode='reflect'), clamped into the row as the kernel does.  Defects: frame_offset (frames start that many samples
+    later), about_L (the right end reflected about L instead of L - 1)."""
+    p = torch.arange(F, device=device)[:, None] * 256 + torch.arange(1024, device=device)[None, :] - 512 + frame_offset
+    s = p.abs()
+    s = torch.where(s >= L, (2 * L if about_L else 2 * (L - 1)) - s, s)
+    return s.clamp(0, L - 1)
+
+
+def log_mel_frames(L: int, S: int) -> int:
+    """frames log_mel_kernel computes for a row of L samples in a launch of S frames"""
+    return min(1 + L // 256, S)
+
+
+def mel_band_bins(fb: torch.Tensor) -> torch.Tensor:
+    """[100] bins from each band's first to its last nonzero weight (the kernel's loop length; 0 for an all-zero band)"""
+    lo, hi = resample_trim(fb.T)
+    return (hi - lo + 1).clamp_min(0)
+
+
+def log_mel_rows(x: torch.Tensor, L: int, window: torch.Tensor, fb: torch.Tensor, S: int, reflect_about_L: bool = False,
+                 frame_offset: int = 0, symmetric_window: bool = False, band_shift: int = 0, power: int = 1,
+                 clip: float = MEL_CLIP, tap_scale: Optional[Tuple[int, float]] = None, magnitudes: bool = False):
+    """One row of log_mel_kernel: log(max(fb^T |rfft(window * frame)|, clip)) of the reflect-padded frames of x[:L], [100, S] fp64
+    with frames past log_mel_frames(L, S) 0.  window [1024] and fb [513, 100] are the kernel's fp32 tables.  magnitudes=True
+    also returns (|X| [F, 513], the windowed frames [F, 1024]).  Defects: reflect_about_L, frame_offset, symmetric_window (the
+    symmetric Hann window in place of `window`), band_shift (every band one bin higher), power, clip, tap_scale (i, s):
+    window tap i times s."""
+    F = log_mel_frames(L, S)
+    dev = x.device
+    w = (torch.hann_window(1024, periodic=False, dtype=torch.float32) if symmetric_window else window).to(dev, F64).clone()
+    if tap_scale is not None:
+        w[tap_scale[0]] *= tap_scale[1]
+    fr = x[:L].to(F64)[_reflect_index(L, F, frame_offset, reflect_about_L, dev)] * w                  # [F, 1024]
+    mag = torch.fft.rfft(fr, dim=-1).abs()                                                              # [F, 513]
+    fbd = fb.to(dev, F64)
+    if band_shift:
+        fbd = fbd.roll(band_shift, 0)
+    mel = (mag ** power) @ fbd                                                                          # [F, 100]
+    out = torch.zeros(100, S, dtype=F64, device=dev)
+    out[:, :F] = torch.log(torch.clip(mel, min=clip)).T
+    if magnitudes:
+        return out, mag, fr
+    return out
+
+
+def _twiddles(n: int, count: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(exact exp(-2 pi i k / n), the kernel's fp32 table of it) for k < count, complex128"""
+    k = torch.arange(count, dtype=F64)
+    ex = torch.complex(torch.cos(2 * math.pi * k / n), -torch.sin(2 * math.pi * k / n))
+    return ex, torch.complex(ex.real.float().to(F64), ex.imag.float().to(F64))
+
+
+def _l1(z: torch.Tensor) -> torch.Tensor:
+    return z.real.abs() + z.imag.abs()
+
+
+def _cmul_error(c: torch.Tensor, ex: torch.Tensor, t32: torch.Tensor) -> torch.Tensor:
+    """What the kernel's fp32 complex product c x t32 (cmul: two products and a sum per part, or one of them fused) adds to
+    the exact c x ex, given c exactly: the twiddle's own rounding |c| |t32 - ex|, 2^-24 of every product that is not exact (a
+    factor 0 or +-1 is exact) and 2^-24 of each part of the result."""
+    tr, ti = t32.real, t32.imag
+    inexact_r = ((tr != 0) & (tr.abs() != 1)).to(F64)
+    inexact_i = ((ti != 0) & (ti.abs() != 1)).to(F64)
+    prods = (c.real.abs() + c.imag.abs()) * (tr.abs() * inexact_r + ti.abs() * inexact_i)
+    return c.abs() * (t32 - ex).abs() + U32 * prods + U32 * _l1(c * ex)
+
+
+def fft_magnitude_bound(fr: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """|rfft| [F, 513] of windowed frames fr [F, 1024] (fp64 products of the kernel's fp32 samples and window) and, per bin,
+    a bound on how far log_mel_kernel's fp32 magnitude may lie from it.
+
+    The bound follows the kernel's own passes in fp64, carrying per node an error bound E next to the exact node value:
+      * z[q] = x[2q] w[2q] + i x[2q+1] w[2q+1], rounded to fp32: E = 2^-24 (|Re z| + |Im z|), stored bit-reversed;
+      * each radix-2 stage (half = 1 .. 256): a, c -> a +- c W, W the fp32 twiddle.  E(c W) = E(c) (1 + u) + _cmul_error, and
+        each output adds E(a) + E(c W) + 2^-24 of its parts (the fp32 add), times (1 + 2u) for the second-order terms;
+      * the split step: Xe = (Z_k + conj Z_(512-k)) / 2 and Xo = (Z_k - conj Z_(512-k)) / 2i (the halving is exact), the
+        product with the fp32 tw1024 and the sum / difference, each bounded the same way;
+      * |X| = sqrtf(ar^2 + ai^2): two squares, a sum and the root, 3 2^-24 |X|.
+    Every rounding is charged at the magnitude of the value it rounds, node by node, not at the frame's sum |x w|: a bin that
+    is weak within a loud frame gets a bound of its own size wherever the passes leading to it carry little."""
+    u = U32
+    F, dev = fr.shape[0], fr.device
+    z = torch.complex(fr[:, 0::2], fr[:, 1::2])                                                         # [F, 512]
+    brev = torch.tensor([int(f"{i:09b}"[::-1], 2) for i in range(512)], device=dev)
+    Z, E = z[:, brev], u * _l1(z)[:, brev]
+    ex512, t512 = (t.to(dev) for t in _twiddles(512, 256))
+    half = 1
+    while half < 512:
+        tws = 256 // half
+        Zr, Er = Z.reshape(F, 512 // (2 * half), 2, half), E.reshape(F, 512 // (2 * half), 2, half)
+        a, c, Ea, Ec = Zr[:, :, 0], Zr[:, :, 1], Er[:, :, 0], Er[:, :, 1]
+        idx = torch.arange(half, device=dev) * tws
+        ct = c * ex512[idx]
+        Ect = Ec * (1 + u) + _cmul_error(c, ex512[idx], t512[idx])
+        o0, o1 = a + ct, a - ct
+        E0 = (Ea + Ect + u * _l1(o0)) * (1 + 2 * u)
+        E1 = (Ea + Ect + u * _l1(o1)) * (1 + 2 * u)
+        Z = torch.stack([o0, o1], 2).reshape(F, 512)
+        E = torch.stack([E0, E1], 2).reshape(F, 512)
+        half *= 2
+    k = torch.arange(257, device=dev)
+    n = (512 - k) % 512
+    zk, zn, Ek, En = Z[:, k], Z[:, n], E[:, k], E[:, n]
+    xe, xo = (zk + zn.conj()) / 2, (zk - zn.conj()) / 2j
+    Exe, Exo = 0.5 * (Ek + En) + u * _l1(xe), 0.5 * (Ek + En) + u * _l1(xo)
+    ex1024, t1024 = (t.to(dev) for t in _twiddles(1024, 257))
+    wx = ex1024 * xo
+    Ewx = Exo * (1 + u) + _cmul_error(xo, ex1024, t1024)
+    Xk, Xn = xe + wx, xe - wx
+    Bk = (Exe + Ewx + u * _l1(Xk)) * (1 + 2 * u) + 3 * u * Xk.abs()
+    Bn = (Exe + Ewx + u * _l1(Xn)) * (1 + 2 * u) + 3 * u * Xn.abs()
+    mag = torch.zeros(F, 513, dtype=F64, device=dev)
+    bound = torch.zeros(F, 513, dtype=F64, device=dev)
+    mag[:, :257], bound[:, :257] = Xk.abs(), Bk
+    mag[:, 512 - k], bound[:, 512 - k] = Xn.abs(), Bn                                                   # bins 256 .. 512
+    bound[:, 256] = torch.maximum(Bk[:, 256], Bn[:, 256])                                               # written twice
+    return mag, bound
+
+
+def log_mel_terms(x: torch.Tensor, L: int, window: torch.Tensor, fb: torch.Tensor, S: int):
+    """The fp64 truth of log_mel_kernel on one row and the interval its fp32 output must lie in: (ref, lo, hi), each [100, S].
+
+    Magnitude per bin: fft_magnitude_bound, the kernel's FFT, split step and |.| followed node by node.  Band m: sum fb x the
+    magnitude bound, plus the fmaf chain over its n_m bins from the first to the last nonzero weight, n_m 2^-24 sum fb M.  The
+    interval [mel - d, mel + d] maps through log(max(., 1e-7f)), so an entry whose whole interval is clipped is exact, and then
+    widens by logf's 1 ulp (2^-23 |log|)."""
+    ref, _, fr = log_mel_rows(x, L, window, fb, S, magnitudes=True)
+    F = fr.shape[0]
+    mag, dM = fft_magnitude_bound(fr)
+    fbd = fb.to(x.device, F64)
+    mel = mag @ fbd
+    d = dM @ fbd + mel_band_bins(fb).to(x.device, F64)[None, :] * U32 * ((mag + dM) @ fbd)
+    lo_m, hi_m = (mel - d).clamp_min(MEL_CLIP), (mel + d).clamp_min(MEL_CLIP)
+    lo, hi = ref.clone(), ref.clone()
+    lo_l, hi_l = torch.log(lo_m), torch.log(hi_m)
+    clipped = hi_m <= MEL_CLIP
+    lo_l = torch.where(clipped, lo_l, lo_l - 2.0 ** -23 * lo_l.abs())
+    hi_l = torch.where(clipped, hi_l, hi_l + 2.0 ** -23 * hi_l.abs())
+    lo[:, :F], hi[:, :F] = lo_l.T, hi_l.T
+    return ref, lo, hi
+
+
+def interval_ratio(got: torch.Tensor, ref: torch.Tensor, lo: torch.Tensor, hi: torch.Tensor) -> torch.Tensor:
+    """|got - ref| over the side of [lo, hi] it lies towards, elementwise (0 where got == ref, inf past a zero-width side)"""
+    e = got.to(F64) - ref
+    side = torch.where(e > 0, hi - ref, ref - lo)
+    return torch.where(e == 0, torch.zeros_like(e), e.abs() / side)

@@ -54,6 +54,7 @@ def resample(x: torch.Tensor, orig_freq: int, new_freq: int, dtype: torch.dtype 
     g = math.gcd(orig_freq, new_freq)
     orig, new = orig_freq // g, new_freq // g
     kernel, width = sinc_kernel(orig, new, dtype)
+    kernel = kernel.to(x.device)
     xp = F.pad(x[None, None], (width, width + orig))
     y = F.conv1d(xp, kernel, stride=orig).transpose(1, 2).reshape(-1)
     return y[:out_length(orig_freq, new_freq, x.shape[-1])]
@@ -76,12 +77,28 @@ def mel_filterbank() -> torch.Tensor:
     return torch.max(torch.zeros(1), torch.min(down, up))
 
 
-def log_mel_24k(x24: torch.Tensor, dtype: torch.dtype = torch.float64) -> torch.Tensor:
-    """One 24 kHz utterance [N] (N > 512) -> log-mel [100, 1 + N // 256] in dtype."""
-    x24 = x24.to(dtype)
-    spec = torch.stft(x24, N_FFT, HOP, window=hann_window().to(dtype), center=True, pad_mode="reflect", return_complex=True).abs()
-    mel = torch.matmul(spec.transpose(-1, -2), mel_filterbank().to(dtype)).transpose(-1, -2)
+def stft_magnitude(x24: torch.Tensor, window: Optional[torch.Tensor] = None, dtype: torch.dtype = torch.float64) -> torch.Tensor:
+    """|STFT| [513, 1 + N // 256] of one 24 kHz utterance [N] (N > 512): reflect centring, ``window`` [1024] (default the
+    periodic Hann window), in dtype."""
+    w = hann_window() if window is None else window
+    return torch.stft(x24.to(dtype), N_FFT, HOP, window=w.to(dtype), center=True, pad_mode="reflect", return_complex=True).abs()
+
+
+def mel_project(spec: torch.Tensor, fb: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """[513, frames] magnitudes -> [100, frames] through ``fb`` [513, 100] (default the HTK filterbank), in spec's dtype."""
+    fb = mel_filterbank() if fb is None else fb
+    return torch.matmul(spec.transpose(-1, -2), fb.to(spec.dtype)).transpose(-1, -2)
+
+
+def log_clip(mel: torch.Tensor) -> torch.Tensor:
+    """log(clip(., 1e-7)): torch.clip keeps NaN"""
     return torch.log(torch.clip(mel, min=1e-7))
+
+
+def log_mel_24k(x24: torch.Tensor, dtype: torch.dtype = torch.float64, window: Optional[torch.Tensor] = None,
+                fb: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One 24 kHz utterance [N] (N > 512) -> log-mel [100, 1 + N // 256] in dtype, with the recipe's tables unless given."""
+    return log_clip(mel_project(stft_magnitude(x24, window, dtype), fb))
 
 
 def log_mel(x: torch.Tensor, sample_rate: int, dtype: torch.dtype = torch.float64) -> torch.Tensor:

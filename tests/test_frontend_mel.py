@@ -151,19 +151,6 @@ def test_resampler_on_fixture_cases(fx):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("orig,new", [(16000, 24000), (22050, 24000), (48000, 24000), (44100, 24000), (44100, 16000)])
-def test_resampler_rate_pairs(fx, orig, new):
-    """Every tabled rate pair on the reference's 2.wav read as if it were at `orig` Hz: fp64 oracle, e_ref from the fp32 oracle."""
-    x = case_wav(fx["cases"]["2.wav"])
-    want = mel_oracle.resample(x, orig, new, torch.float64)
-    e_ref = (mel_oracle.resample(x, orig, new, torch.float32).double() - want).abs().max().item()
-    y, out_len = frontend.resample(x.cuda(), orig, new)
-    assert out_len.tolist() == [want.shape[0]] and y.shape == want.shape
-    err = (y.cpu().double() - want).abs().max().item()
-    assert err <= 4 * e_ref, (orig, new, err, e_ref)
-
-
-@pytest.mark.gpu
 def test_resample_same_rate_is_a_copy():
     w = torch.randn(3, 1000).cuda()
     y, n = frontend.resample(w, 24000, 24000, torch.tensor([1000, 10, 0]).cuda())

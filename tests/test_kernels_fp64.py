@@ -819,6 +819,7 @@ _TWO_DEVICES = r"""
 import sys, torch
 sys.path.insert(0, sys.argv[1]); sys.path.insert(0, sys.argv[1] + '/tests')
 import test_kernels_fp64 as t
+front = []
 for dev in (0, 1):
     with torch.cuda.device(dev):
         gc = t.GEMM_CASES[0]
@@ -828,13 +829,19 @@ for dev in (0, 1):
         ac = t.ATTN_CASES[-1]
         t.launch_attn(ac, t.build_attn(ac, torch.device('cuda', dev)), poison=False)
         a = __import__('test_audio_kernels_fp64'); a.launch_istft((2048, 2, 0), a.build_istft((2048, 2, 0)), torch.device('cuda', dev))
+        f = __import__('test_frontend_kernels_fp64'); sp = torch.randn(4000, generator=torch.Generator().manual_seed(0))
+        rc = f.RES_CASES[13]; front.append(f.launch_res(rc, f.build_res(rc, sp), torch.device('cuda', dev)).cpu())
+        mc = f.MEL_CASES[1]; front.append(f.launch_mel(mc, f.build_mel(mc, sp), torch.device('cuda', dev), f.MelHandle(mc)).cpu())
+# each handle reads the tables of its own device: device 1's front-end outputs equal device 0's bit for bit
+assert torch.equal(front[0], front[2]) and torch.equal(front[1], front[3])
 print('ok')
 """
 
 
 @gpu
 def test_launchers_on_two_devices_in_one_process():
-    """The launchers set each kernel's dynamic shared-memory attribute once per process; CUDA keeps it per device."""
+    """The launchers set each kernel's dynamic shared-memory attribute once per process; CUDA keeps it per device.  The front
+    end's resampler and log-mel handles keep their tables on the device they were created on."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two GPUs")
     r = subprocess.run([sys.executable, "-c", _TWO_DEVICES, REPO], capture_output=True, text=True, timeout=600)

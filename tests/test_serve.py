@@ -318,3 +318,26 @@ def test_a_nan_prompt_fails_only_its_own_request(chain):
     assert isinstance(res[2], AssertionError) and "model.py:404" in str(res[2])
     assert 2 not in lat
     _check_parity(models, wavs, prompt, xs, "unipc", res, lat, skip=(2,))
+
+
+@pytest.mark.gpu
+def test_a_nan_voice_sample_fails_only_its_own_request(chain):
+    """One NaN sample in a voice recording reaches its prompt mel (torch.clip keeps NaN) and so fails that request with the
+    reference's AssertionError, as a NaN prompt does; the requests with the clean voice are bit-identical to a run without it."""
+    models, wavs, _, xs = chain
+    g = torch.Generator().manual_seed(11)
+    voice = (0.2 * torch.randn(11000, generator=g)).float()                   # 16 kHz: 16500 samples, 65 frames at 24 kHz
+    bad_voice = voice.clone()
+    bad_voice[5000] = float("nan")
+    clean, bad = convert.voice_mels([(voice, 16000), (bad_voice, 16000)], torch.device("cuda"))
+    hit = bad.isnan().any(0)
+    assert bad.isnan()[:, hit].all() and 0 < int(hit.sum()) < 8 and torch.equal(bad[:, ~hit], clean[:, ~hit])
+    prompts = [clean.cpu()] * len(wavs)
+    ref, ref_lat, _ = _script(models, wavs, clean.cpu(), xs, "unipc", prompts=prompts)
+    prompts[2] = bad.cpu()
+    res, lat, _ = _script(models, wavs, clean.cpu(), xs, "unipc", prompts=prompts)
+    assert isinstance(res[2], AssertionError) and "model.py:404" in str(res[2])
+    assert 2 not in lat
+    for i in range(len(wavs)):
+        if i != 2:
+            assert torch.equal(lat[i], ref_lat[i]) and torch.equal(res[i], ref[i]), f"request {i} changed"
