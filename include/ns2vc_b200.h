@@ -274,6 +274,9 @@ long long ns2vc_resample_out_length(int orig_freq, int new_freq, long long n);
 int ns2vc_resample_table(int orig_freq, int new_freq, int* phases, int* taps, int* width, float* table);
 /* Host-only: the dense fp32 mel filterbank [513][100] (torchaudio melscale_fbanks at the parameters above). */
 int ns2vc_mel_filterbank(float* fb);
+/* Host-only, no GPU: 0 when ns2vc_resampler_create accepts the rate pair, else -1 with the reason (a bad rate, or a ratio whose
+ * input window per CTA exceeds 48 KB of shared memory), so a caller can reject an input before any device work. */
+int ns2vc_resample_check(int orig_freq, int new_freq);
 int ns2vc_resampler_create(int orig_freq, int new_freq, ns2vc_resampler** out);   /* orig == new: a copy */
 void ns2vc_resampler_destroy(ns2vc_resampler* h);
 /* x [B, n] fp32 (batch stride x_bstride floats), lengths [B] int64 device (each <= n; NULL: every row n)

@@ -154,6 +154,7 @@ SIGNATURES = {
     "ns2vc_resample_out_length": (C.c_longlong, [C.c_int, C.c_int, C.c_longlong]),
     "ns2vc_resample_table": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "ns2vc_mel_filterbank": (C.c_int, [_P]),
+    "ns2vc_resample_check": (C.c_int, [C.c_int, C.c_int]),
     "ns2vc_resampler_create": (C.c_int, [C.c_int, C.c_int, C.POINTER(_P)]),
     "ns2vc_resampler_destroy": (None, [_P]),
     "ns2vc_resample": (C.c_int, [_P, _P, C.c_longlong, C.c_longlong, _P, _P, C.c_longlong, C.c_longlong, C.c_int, _P]),

@@ -233,6 +233,9 @@ def __getattr__(name):
     if name in ("diffusion_loss", "loss_profile", "utterance_losses"):     # the training objective under no_grad lives in loss.py
         from . import loss
         return getattr(loss, name)
+    if name in ("preprocess_utterances", "dataset_item"):   # a corpus to the reference's training files lives in preprocess.py
+        from . import preprocess
+        return getattr(preprocess, name)
     if name == "StreamConverter":
         from . import stream
         return stream.StreamConverter

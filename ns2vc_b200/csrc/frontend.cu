@@ -103,6 +103,11 @@ long long out_length(const Ratio& r, long long n) {
   return (long long)std::ceil((float)((double)(r.nw * n) / (double)r.orig));
 }
 
+// input floats a resample CTA stages for its kResThreads outputs; a ratio whose window passes kResMaxWindow is refused
+long long resample_window(const Ratio& r) {
+  return (long long)((kResThreads - 1) / r.nw + 1) * r.orig + r.taps;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Kernels
 // ---------------------------------------------------------------------------------------------------------------------
@@ -284,6 +289,15 @@ int ns2vc_mel_filterbank(float* fb) {
   return 0;
 }
 
+int ns2vc_resample_check(int orig_freq, int new_freq) {
+  NS_REQUIRE(orig_freq > 0 && new_freq > 0, "resample_check: bad rates %d -> %d", orig_freq, new_freq);
+  if (orig_freq == new_freq) return 0;
+  const Ratio r = resample_ratio(orig_freq, new_freq);
+  NS_REQUIRE(resample_window(r) <= kResMaxWindow, "resample_check: %d -> %d Hz reduces to %d:%d, whose %lld-sample input window per %d "
+             "outputs exceeds %d", orig_freq, new_freq, r.orig, r.nw, resample_window(r), kResThreads, kResMaxWindow);
+  return 0;
+}
+
 int ns2vc_resampler_create(int orig_freq, int new_freq, ns2vc_resampler** out) {
   NS_REQUIRE(out, "resampler_create: null argument");
   NS_REQUIRE(orig_freq > 0 && new_freq > 0, "resampler_create: bad rates %d -> %d", orig_freq, new_freq);
@@ -307,11 +321,11 @@ int ns2vc_resampler_create(int orig_freq, int new_freq, ns2vc_resampler** out) {
     }
   }
   const Ratio r = h->r;                                     // a copy: the refusal below reads it after deleting h
-  h->window = (int)std::min<long long>((long long)((kResThreads - 1) / r.nw + 1) * r.orig + r.taps, INT32_MAX);
+  h->window = (int)std::min<long long>(resample_window(r), INT32_MAX);
   if (h->window > kResMaxWindow) {
     delete h;
     set_error("resampler_create: %d -> %d Hz reduces to %d:%d, whose %d-sample input window per %d outputs exceeds %d",
-              orig_freq, new_freq, r.orig, r.nw, (int)((kResThreads - 1) / r.nw + 1) * r.orig + r.taps, kResThreads, kResMaxWindow);
+              orig_freq, new_freq, r.orig, r.nw, (int)resample_window(r), kResThreads, kResMaxWindow);
     return -1;
   }
   cudaError_t e = cudaMalloc(&h->table, table.size() * sizeof(float));

@@ -72,6 +72,13 @@ def resample_out_length(orig_freq: int, new_freq: int, n: int) -> int:
     return r
 
 
+def resample_check(orig_freq: int, new_freq: int) -> None:
+    """Raises ValueError, on the host and before any device work, unless ``resample`` accepts the rate pair: both rates
+    positive, and a reduced ratio whose input window per CTA fits in 48 KB of shared memory (46:1 is the first refused)."""
+    if _lib.lib().ns2vc_resample_check(int(orig_freq), int(new_freq)) != 0:
+        raise ValueError((_lib.lib().ns2vc_last_error() or b"").decode("utf-8", "replace"))
+
+
 def _rows(wav: torch.Tensor, lengths: Optional[torch.Tensor]):
     """[B, N] or [N] float32 (+ optional int64 [B] lengths) -> (2-D view, was 1-D, host lengths)."""
     if wav.dim() not in (1, 2):

@@ -78,6 +78,16 @@ def plan_batches(plans: Sequence[Dict[str, int]], prompt_lengths: Sequence[int],
     if world == 1:
         return [batches]
     cost = [len(b) * sample_step_flops(max(plans[i]["T"] for i in b), max(int(prompt_lengths[i]) for i in b)) for b in batches]
+    return assign_batches(batches, cost, world)
+
+
+def assign_batches(batches: Sequence[List[int]], cost: Sequence[int], world: int) -> List[List[List[int]]]:
+    """Whole batches to ranks by LPT, ``out[rank] = [batch, ...]``: the costliest batch first (input order on ties), to the
+    least-loaded rank, the lowest rank on ties.  ``cost[k]`` is batch k's work in any unit the caller's workload scales with."""
+    if world < 1:
+        raise ValueError(f"bad world size {world}")
+    if len(cost) != len(batches):
+        raise ValueError(f"{len(cost)} costs for {len(batches)} batches")
     out: List[List[List[int]]] = [[] for _ in range(world)]
     load = [0] * world
     for k in sorted(range(len(batches)), key=lambda k: -cost[k]):
