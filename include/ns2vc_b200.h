@@ -89,6 +89,16 @@ int ns2vc_unet_prepare_cond_ragged(ns2vc_unet* h, const float* content, long lon
                                    const int64_t* content_lengths, const int64_t* prompt_lengths, int B, int T, int S, void* ws,
                                    ns2vc_stream stream);
 
+/* ns2vc_unet_prepare_cond_ragged for the n_rows entries listed in rows (host array of distinct indices in [0, B)) only:
+ * their length and key-bias tables, content conditioning, pooled prompt embedding and cross-attention K/V are recomputed
+ * from the same arguments (content_lengths / prompt_lengths are the full int64 [B] device arrays) and written exactly as
+ * the full call writes them; no byte of any other entry changes.  The ragged program of (B, T, S, workspace) must already
+ * have been prepared by ns2vc_unet_prepare_cond_ragged (and no other key run on the handle since).  Each listed entry is
+ * its own launches at B = 1 (listing every entry runs the full program once).  Stream-ordered, no host sync. */
+int ns2vc_unet_prepare_cond_rows(ns2vc_unet* h, const float* content, long long content_bstride, const float* prompt,
+                                 const int64_t* content_lengths, const int64_t* prompt_lengths, const int* rows, int n_rows,
+                                 int B, int T, int S, void* ws, ns2vc_stream stream);
+
 /* UNet1DConditionModel.forward (unet_1d_condition.py:743-1037) given prepared conditioning.
  *   x [B, latent_channels, T] fp32 (batch stride x_bstride floats), t [B] fp32 -> out [B, out_channels, T] */
 int ns2vc_unet_forward(ns2vc_unet* h, const float* x, long long x_bstride, const float* t, float* out, int B, int T,
@@ -104,6 +114,12 @@ int ns2vc_unet_film_width(const ns2vc_unet* h);
 size_t ns2vc_unet_time_table_floats(const ns2vc_unet* h, int n_rows);
 int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float* table, int B, int T, int S, void* ws,
                           ns2vc_stream stream);
+/* The FiLM rows k * B + b of such a table for the entries b listed in rows (host array of n_rows distinct indices in [0, B))
+ * and every step k < n_steps, bit-identical to what ns2vc_unet_time_table(t_rows, n_steps * B, ...) writes there; every
+ * other FiLM row is left as it was.  t_rows and table are laid out as for that call.  Each listed entry is three launches
+ * of n_steps rows (listing every entry computes the whole table in three launches). */
+int ns2vc_unet_time_table_rows(ns2vc_unet* h, const float* t_rows, int n_steps, const int* rows, int n_rows, float* table, int B,
+                               int T, int S, void* ws, ns2vc_stream stream);
 /* ns2vc_unet_forward with the timestep path taken from B rows of such a table (film_rows = table + step * B * film_width). */
 int ns2vc_unet_forward_film(ns2vc_unet* h, const float* x, long long x_bstride, const float* film_rows, float* out, int B,
                             int T, int S, void* ws, ns2vc_stream stream);

@@ -79,10 +79,13 @@ SIGNATURES = {
     "ns2vc_unet_workspace_bytes": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "ns2vc_unet_prepare_cond": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_unet_prepare_cond_ragged": (C.c_int, [_P, _P, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_unet_prepare_cond_rows": (C.c_int, [_P, _P, C.c_longlong, _P, _P, _P, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int,
+                                               C.c_int, _P, _P]),
     "ns2vc_unet_forward": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_unet_film_width": (C.c_int, [_P]),
     "ns2vc_unet_time_table_floats": (C.c_size_t, [_P, C.c_int]),
     "ns2vc_unet_time_table": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_unet_time_table_rows": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int), C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_unet_forward_film": (C.c_int, [_P, _P, C.c_longlong, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_dpm_step": (C.c_int, [_P, _P, _P, C.POINTER(DpmCoef), _P, _P, C.c_size_t, _P, _P]),
     "ns2vc_unipc_step": (C.c_int, [_P, _P, _P, _P, _P, C.POINTER(UniPcCoef), _P, _P, _P, C.c_size_t, _P, _P]),

@@ -348,7 +348,9 @@ struct RaggedTables {
   float* key_bias[kRagMaxLevels];     // [B, Tl] 0 / -inf key bias of the self-attention at level l (nullptr: no transformer there)
   int Tl[kRagMaxLevels];
 };
-int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st);
+// Entries [b0, b0 + n) (n = 0: all B); the lengths are read at the same entries.
+int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st,
+                         int b0 = 0, int n = 0);
 
 // Fused sampler steps (element-wise, bit-exact op order; see kernels_misc.cu)
 struct DpmStepCoef {   // DPM-Solver++(2M): one post-UNet step

@@ -62,6 +62,9 @@ struct Program {
   bool has_mask = false;
   bool cond_ready = false;   // the conditioning program has run for this key since it last became active
   std::vector<Launch> prog_cond, prog_fwd;
+  // ragged: entry b's conditioning alone (ns2vc_unet_prepare_cond_rows), built when b is first asked for; empty until then
+  std::vector<std::vector<Launch>> prog_cond_row;
+  size_t cond_end = 0;                                    // workspace offset where the conditioning's buffers end
   float* film_base = nullptr;                             // FiLM rows [B, film_total] (workspace)
   float* aug = nullptr;                                   // add_embedding output [B, ted] (workspace)
   TapSet taps;
@@ -441,6 +444,7 @@ struct Builder : ProgramBuilder {
   std::vector<int> Tl;                                     // rows per entry at each level
   const bool xf_on;                                        // panel mode is possible (wgmma backend)
   const int* rag_lens = nullptr;                           // ragged programs: content lengths [B] (device), else nullptr
+  const int* rag_plens = nullptr;                          // ragged programs: prompt lengths [B] (device), else nullptr
   Arena sar;                                               // the program's static buffer (see ns2vc_unet::static_bufs)
   // conditioning outputs the forward reads
   float* P = nullptr;                                      // conv_in(content) + bias
@@ -579,7 +583,7 @@ struct Builder : ProgramBuilder {
   void emit_cond() {
     const ns2vc_unet_cfg& c = h->cfg;
     const int c0 = c.block_out_channels[0], Cc = c.in_channels - c.latent_channels, xd = c.cross_attention_dim, ted = h->ted;
-    const int* plens = rag_lens ? rag_lens + B : nullptr;   // ragged: prompt lengths
+    const int* plens = rag_plens;
     P = (Cc > 0) ? ar.get<float>((size_t)B * T * c0) : nullptr;
     kvc = ar.get<float>((size_t)B * S * std::max(h->kv_total, 1));
     kvs.T = S; kvs.C = std::max(h->kv_total, 8); kvs.ld = pad_to(kvs.C, 8);
@@ -882,10 +886,12 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
       rt.prompt_bias = bld.sar.get<float>((size_t)B * S);
       for (int l = 0; l < nlev; ++l) { rt.Tl[l] = Tl[l]; rt.key_bias[l] = xf_level[l] ? bld.sar.get<float>((size_t)B * Tl[l]) : nullptr; }
       bld.rag_lens = rt.lens;
+      bld.rag_plens = rt.lens + B;
     }
   }
 
   bld.emit_cond();
+  pg.cond_end = bld.ar.off;
   bld.out = &pg.prog_fwd;
   bld.reserve_forward();
   bld.emit_entry();
@@ -908,6 +914,39 @@ int build_programs(ns2vc_unet* h, int B, int T, int S, void* ws, size_t* bytes_o
     pg.B = B; pg.T = T; pg.S = S; pg.ws = ws;
     pg.film_base = bld.film; pg.aug = bld.aug;
     *prog = std::move(pg);
+  }
+  return 0;
+}
+
+// Entry b's conditioning program of the ragged program `pg`: emit_cond at B = 1 over row b of every buffer the full program
+// placed there (an Arena row view of the same workspace), reading entry b's lengths.  Each of its launches is row-local:
+// the GEMMs' tiles, the split and prep rows, the LayerNorm rows, the small linears' rows and the pooling CTAs each cover one
+// entry, and no ragged launch reads another entry's length.  So it writes the bytes the full program writes for row b, and
+// nothing of any other row.
+int build_cond_row(ns2vc_unet* h, Program& pg, int b) {
+  Builder rb(h, pg, pg.ws, 1, pg.T, pg.S, true);
+  rb.ar.rows = (size_t)pg.B; rb.ar.row = (size_t)b;
+  std::vector<Launch> prog;
+  rb.out = &prog;
+  rb.rag_lens = pg.rt.lens + b;
+  rb.rag_plens = pg.rt.lens + pg.B + b;
+  rb.emit_cond();
+  if (rb.err) return rb.err;
+  // every buffer emit_cond takes must be [B, ...]: then the row view ends where the full build's conditioning ended
+  NS_REQUIRE(rb.ar.off == pg.cond_end, "internal: entry %d's conditioning ends at workspace offset %zu, the full program's at %zu",
+             b, rb.ar.off, pg.cond_end);
+  pg.prog_cond_row[b] = std::move(prog);
+  return 0;
+}
+
+// Checks a caller's list of n distinct entries of a batch of B.
+int check_rows(const int* rows, int n, int B, const char* fn) {
+  NS_REQUIRE(n >= 0 && n <= B && (rows || n == 0), "%s: %d rows of a batch of %d", fn, n, B);
+  std::vector<char> seen((size_t)B, 0);
+  for (int i = 0; i < n; ++i) {
+    NS_REQUIRE(rows[i] >= 0 && rows[i] < B, "%s: row %d out of range [0, %d)", fn, rows[i], B);
+    NS_REQUIRE(!seen[rows[i]], "%s: row %d listed twice", fn, rows[i]);
+    seen[rows[i]] = 1;
   }
   return 0;
 }
@@ -1127,6 +1166,44 @@ int ns2vc_unet_prepare_cond_ragged(ns2vc_unet* h, const float* content, long lon
   return 0;
 }
 
+int ns2vc_unet_prepare_cond_rows(ns2vc_unet* h, const float* content, long long content_bstride, const float* prompt,
+                                 const int64_t* content_lengths, const int64_t* prompt_lengths, const int* rows, int n_rows, int B,
+                                 int T, int S, void* ws, ns2vc_stream stream) {
+  NS_REQUIRE(h && prompt && content_lengths && prompt_lengths, "null argument");
+  int rc = check_rows(rows, n_rows, B, "ns2vc_unet_prepare_cond_rows");
+  if (rc) return rc;
+  rc = ensure_program(h, B, T, S, ws, (cudaStream_t)stream, true);
+  if (rc) return rc;
+  const int Cc = h->cfg.in_channels - h->cfg.latent_channels;
+  NS_REQUIRE(Cc == 0 || content != nullptr, "content is NULL but the model has %d content channels", Cc);
+  Program& pg = h->progs[h->active];
+  NS_REQUIRE(pg.cond_ready, "ns2vc_unet_prepare_cond_ragged() must have prepared the same (B,T,S,workspace) before ns2vc_unet_prepare_cond_rows()");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const long long* clen = reinterpret_cast<const long long*>(content_lengths);
+  const long long* plen = reinterpret_cast<const long long*>(prompt_lengths);
+  if (n_rows == B) {                                       // every entry: the full program writes exactly these rows
+    if ((rc = launch_ragged_tables(clen, plen, pg.rt, st))) return rc;
+    CallArgs in{};
+    in[Launch::CONTENT] = {content, content_bstride}; in[Launch::PROMPT] = {prompt};
+    return run_program(h, pg, pg.prog_cond, in, st);
+  }
+  if (pg.prog_cond_row.empty()) pg.prog_cond_row.resize(B);
+  const size_t prompt_row = (size_t)S * h->cfg.cross_attention_dim;
+  int launches = 0;
+  for (int i = 0; i < n_rows; ++i) {
+    const int b = rows[i];
+    if (pg.prog_cond_row[b].empty() && (rc = build_cond_row(h, pg, b))) return rc;
+    if ((rc = launch_ragged_tables(clen, plen, pg.rt, st, b, 1))) return rc;
+    CallArgs in{};
+    in[Launch::CONTENT] = {content ? content + (size_t)b * content_bstride : nullptr, content_bstride};
+    in[Launch::PROMPT] = {prompt + (size_t)b * prompt_row};
+    if ((rc = run_program(h, pg, pg.prog_cond_row[b], in, st))) return rc;
+    launches += 1 + h->last_launches;
+  }
+  h->last_launches = launches;
+  return 0;
+}
+
 int ns2vc_unet_forward(ns2vc_unet* h, const float* x, long long x_bstride, const float* t, float* out, int B, int T, int S, void* ws,
                        ns2vc_stream stream) {
   NS_REQUIRE(h && x && t && out, "null argument");
@@ -1160,6 +1237,43 @@ int ns2vc_unet_time_table(ns2vc_unet* h, const float* t_rows, int n_rows, float*
   const int n = time_path_ops(h, t_rows, n_rows, B, pg.aug, temb1, emb, film, tp);
   for (int i = 0; i < n; ++i)
     if ((rc = launch_small_linear(tp[i], (cudaStream_t)stream))) return rc;
+  return 0;
+}
+
+int ns2vc_unet_time_table_rows(ns2vc_unet* h, const float* t_rows, int n_steps, const int* rows, int n_rows, float* table, int B, int T,
+                               int S, void* ws, ns2vc_stream stream) {
+  NS_REQUIRE(h && t_rows && table, "null argument");
+  NS_REQUIRE(n_steps > 0, "time table rows: %d steps", n_steps);
+  int rc = check_rows(rows, n_rows, B, "ns2vc_unet_time_table_rows");
+  if (rc) return rc;
+  rc = ensure_program_for_call(h, B, T, S, ws, (cudaStream_t)stream);
+  if (rc) return rc;
+  const Program& pg = h->progs[h->active];
+  NS_REQUIRE(pg.cond_ready || !h->cfg.add_embed_text, "ns2vc_unet_prepare_cond() must precede ns2vc_unet_time_table_rows() (the pooled prompt embedding is added to every row)");
+  // ns2vc_unet_time_table's layout for n_steps x B rows; entry b's rows k * B + b are one strided M = n_steps pass per linear
+  // (the small linear computes each row on its own, so a row is the same at any M and pitch)
+  const int M = n_steps * B, ted = h->ted, fw = h->film_total;
+  float* film = table;
+  float* temb1 = table + (size_t)M * std::max(fw, 1);
+  float* emb = temb1 + (size_t)M * ted;
+  if (n_rows == B) {                                       // every entry: the whole table, three launches
+    LinOp tp[3];
+    const int n = time_path_ops(h, t_rows, M, B, pg.aug, temb1, emb, film, tp);
+    for (int j = 0; j < n; ++j)
+      if ((rc = launch_small_linear(tp[j], (cudaStream_t)stream))) return rc;
+    return 0;
+  }
+  for (int i = 0; i < n_rows; ++i) {
+    const int b = rows[i];
+    LinOp tp[3];
+    const int n = time_path_ops(h, t_rows + b, n_steps, 1, pg.aug ? pg.aug + (size_t)b * ted : nullptr, temb1 + (size_t)b * ted,
+                                emb + (size_t)b * ted, film + (size_t)b * std::max(fw, 1), tp);
+    tp[0].x_ld = B; tp[0].out_ld = B * ted;
+    tp[1].x_ld = B * ted; tp[1].out_ld = B * ted;
+    if (n > 2) { tp[2].x_ld = B * ted; tp[2].out_ld = B * fw; }
+    for (int j = 0; j < n; ++j)
+      if ((rc = launch_small_linear(tp[j], (cudaStream_t)stream))) return rc;
+  }
   return 0;
 }
 

@@ -25,13 +25,17 @@ struct PackedB {
 inline int pad_to(int v, int m) { return (v + m - 1) / m * m; }
 inline int nkb_of(int c) { return (c + 63) / 64; }
 
-struct Arena {           // bump allocator over the caller's workspace (or a dry run when base == nullptr)
+// Bump allocator over the caller's workspace (or a dry run when base == nullptr).  A row view (rows > 1) replays the
+// allocations of a build at B = rows from a build at B = 1: each request of n elements reserves n * rows, as the B = rows
+// build did, and returns the start of row `row` of that [rows, n] buffer.
+struct Arena {
   uint8_t* base = nullptr;
   size_t off = 0;
+  size_t rows = 1, row = 0;
   template <class T> T* get(size_t n) {
     off = (off + 255) & ~(size_t)255;
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * sizeof(T);
+    T* p = base ? reinterpret_cast<T*>(base + off) + row * n : nullptr;
+    off += n * rows * sizeof(T);
     return p;
   }
 };

@@ -489,8 +489,9 @@ int launch_mask_bias(const MaskBiasOp& op, cudaStream_t st) {
 // Ragged programs: one block per batch entry turns its content / prompt lengths into the program's tables.  The key biases are
 // -inf (not the reference mask's -10000): the attention kernels already stage -inf for keys past Tk, so a masked key contributes
 // exactly 0 to the online softmax, and the staged bias row of a short utterance equals that of the utterance run alone.
-__global__ void ragged_tables_kernel(const long long* __restrict__ clen, const long long* __restrict__ plen, RaggedTables r) {
-  const int b = blockIdx.x;
+// Block i fills entry b0 + i, so one entry's tables can be rewritten without touching the others'.
+__global__ void ragged_tables_kernel(const long long* __restrict__ clen, const long long* __restrict__ plen, RaggedTables r, int b0) {
+  const int b = b0 + blockIdx.x;
   const int T = (int)min(max(clen[b], 1LL), (long long)r.T), S = (int)min(max(plen[b], 1LL), (long long)r.S);
   if (threadIdx.x == 0) { r.lens[b] = T; r.lens[r.B + b] = S; }
   for (int s = threadIdx.x; s < r.S; s += blockDim.x) r.prompt_bias[(long long)b * r.S + s] = s < S ? 0.f : -INFINITY;
@@ -500,9 +501,12 @@ __global__ void ragged_tables_kernel(const long long* __restrict__ clen, const l
     for (int t = threadIdx.x; t < Tl; t += blockDim.x) r.key_bias[l][(long long)b * Tl + t] = t < tb ? 0.f : -INFINITY;
   }
 }
-int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st) {
+int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st,
+                         int b0, int n) {
   if (r.nlev > kRagMaxLevels) { set_error("ragged tables: %d levels", r.nlev); return -1; }
-  ragged_tables_kernel<<<r.B, 256, 0, st>>>(content_lengths, prompt_lengths, r);
+  if (n <= 0) n = r.B;
+  if (b0 < 0 || b0 + n > r.B) { set_error("ragged tables: entries [%d, %d) of %d", b0, b0 + n, r.B); return -1; }
+  ragged_tables_kernel<<<n, 256, 0, st>>>(content_lengths, prompt_lengths, r, b0);
   NS_LAUNCH_CHECK();
   return 0;
 }

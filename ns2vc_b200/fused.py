@@ -15,7 +15,7 @@ import collections
 import ctypes as C
 import hashlib
 import os
-from typing import Optional
+from typing import Optional, Sequence
 
 import torch
 
@@ -167,11 +167,36 @@ class DenoiserSession:
                 _lib.check(self.L.ns2vc_unet_forward(self.h, x.data_ptr(), self.Cl * self.T, t.data_ptr(), out.data_ptr(),
                                                      self.B, self.T, self.S, self.ws.data_ptr(), self._stream()))
 
+    def prepare_rows(self, rows: Sequence[int]):
+        """Ragged sessions: the conditioning of the listed rows only (``ns2vc_unet_prepare_cond_rows``), from the static buffers
+        and length tensors as they stand now; every other row keeps what the last ``prepare()`` wrote.  Needs that prepare()
+        to be this session's and the last one on the module's workspace."""
+        if not self.ragged:
+            raise ValueError("prepare_rows needs a ragged session")
+        if not self._prepared or self.unet.__dict__.get("_cond_owner") is not self:
+            raise RuntimeError("prepare_rows() needs this session's prepare() first")
+        rows = [int(r) for r in rows]
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.ns2vc_unet_prepare_cond_rows(
+                self.h, self.content.data_ptr() if self.content is not None else None,
+                (self.Cc * self.T) if self.content is not None else 0, self.prompt.data_ptr(), self.clen.data_ptr(),
+                self.plen.data_ptr(), (C.c_int * len(rows))(*rows), len(rows), self.B, self.T, self.S, self.ws.data_ptr(),
+                self._stream()))
+
     def time_table(self, tvals: torch.Tensor, table: torch.Tensor):
         """FiLM rows of every evaluation time of a run (tvals [steps, B] fp32) into ``table`` (needs prepare())."""
         with torch.cuda.device(self.dev):
             _lib.check(self.L.ns2vc_unet_time_table(self.h, tvals.data_ptr(), tvals.numel(), table.data_ptr(), self.B, self.T, self.S,
                                                     self.ws.data_ptr(), self._stream()))
+
+    def time_table_rows(self, tvals: torch.Tensor, table: torch.Tensor, rows: Sequence[int]):
+        """``time_table`` for the listed rows only: FiLM rows k * B + b for b in ``rows`` and every step k; the others are
+        left as they are."""
+        rows = [int(r) for r in rows]
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.ns2vc_unet_time_table_rows(self.h, tvals.data_ptr(), tvals.numel() // self.B, (C.c_int * len(rows))(*rows),
+                                                         len(rows), table.data_ptr(), self.B, self.T, self.S, self.ws.data_ptr(),
+                                                         self._stream()))
 
     # ------------------------------------------------------------------ loop bodies (eager or under capture)
     def _film(self, ent, k):

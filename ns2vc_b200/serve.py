@@ -11,6 +11,12 @@ equal to utterance b run alone: the encoders run on the newcomers as one ragged 
 lengths in device tables, the FiLM rows are per row, and the row step kernels (``ns2vc_dpm_step_rows`` / ``ns2vc_unipc_step_rows``)
 do the scalar step's arithmetic with each row's own coefficient struct.
 
+An admission re-prepares only the rows it changes: the newcomers' slots and the slots freed since the last admission, which
+go back to length 1 and zero inputs (``ns2vc_unet_prepare_cond_rows`` and ``ns2vc_unet_time_table_rows`` write those rows
+exactly as the full prepare and FiLM table would, and nothing else).  The residents' conditioning and FiLM rows stay as they
+are, so an admission costs in proportion to its newcomers, not to the slot count.  Every slot is prepared again after the
+weights are re-packed or when another caller has used the module's shared workspace.
+
 A tick costs one forward of the whole slots x max_frames geometry whatever the occupancy (the ragged GEMMs compute padded rows),
 so for a list known in advance ``convert.convert_utterances`` (longest-first batches) remains the faster call: the server buys
 latency under arrivals, not peak throughput.  DDPM / DDIM are refused: their per-step noise would need a generator stream per row.
@@ -19,11 +25,12 @@ from __future__ import annotations
 
 import collections
 import os
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
+import torch.distributed as dist
 
-from . import _lib, convert
+from . import _lib, convert, shard
 from .api import default_schedule
 from .convert import HOP, LATENT_CH
 from .fused import DenoiserSession, _step_table, schedule_signature
@@ -75,6 +82,45 @@ class SlotTable:
         return not self.queue and self.occupied == 0
 
 
+HEADER_FIELDS = 7          # per admission: ticket, rank, slot, samples, sr, T_b, S_b
+
+
+def place_requests(free: Sequence[int], n: int) -> List[int]:
+    """The rank of each of the first queued requests, in FIFO order, on a server spread over several ranks: each goes to the
+    rank with the most free slots (the lowest rank on ties), which then has one fewer.  Stops when no rank has a free slot, so
+    the result has at most ``min(n, sum(free))`` entries."""
+    free = [int(f) for f in free]
+    out: List[int] = []
+    for _ in range(int(n)):
+        r = max(range(len(free)), key=lambda r: (free[r], -r)) if free else 0
+        if not free or free[r] <= 0:
+            break
+        out.append(r)
+        free[r] -= 1
+    return out
+
+
+def pack_header(admissions: Sequence[Sequence[int]], idle: bool, capacity: int) -> torch.Tensor:
+    """One tick's int64 header: [count, idle, then HEADER_FIELDS values per admission], padded to ``capacity`` admissions so
+    that every rank receives a tensor of one known size."""
+    if len(admissions) > capacity:
+        raise ValueError(f"{len(admissions)} admissions in a header for {capacity}")
+    h = torch.zeros(2 + HEADER_FIELDS * capacity, dtype=torch.int64)
+    h[0], h[1] = len(admissions), int(bool(idle))
+    for i, a in enumerate(admissions):
+        if len(a) != HEADER_FIELDS:
+            raise ValueError(f"an admission has {len(a)} fields, not {HEADER_FIELDS}")
+        h[2 + HEADER_FIELDS * i:2 + HEADER_FIELDS * (i + 1)] = torch.tensor([int(v) for v in a], dtype=torch.int64)
+    return h
+
+
+def unpack_header(h: torch.Tensor) -> Tuple[List[Tuple[int, ...]], bool]:
+    """(admissions, idle) of ``pack_header``'s tensor."""
+    v = h.cpu().tolist()
+    n = int(v[0])
+    return [tuple(v[2 + HEADER_FIELDS * i:2 + HEADER_FIELDS * (i + 1)]) for i in range(n)], bool(v[1])
+
+
 class ConversionServer:
     """Waveform-to-waveform conversion of requests that arrive at any time; the caller owns the loop::
 
@@ -89,10 +135,22 @@ class ConversionServer:
 
     The tick is captured as one CUDA graph on its ``DenoiserSession.CAPTURE_AFTER``-th run and replayed from then on
     (``NS2VC_GRAPH=0``: eager).  It holds the FiLM-row gather, the forward, the row step and the sampler's buffer rotation as
-    stream-ordered device copies (see ``_body``)."""
+    stream-ordered device copies (see ``_body``).
+
+    With a process ``group`` of more than one rank (one process per GPU, each rank with its models on its own device, every
+    rank constructing the server with the same arguments), ``slots`` are per rank.  Rank 0 is the front: only it may
+    ``submit``, and it places each newcomer, FIFO, on the rank with the most free slots (``place_requests``).  Every rank calls
+    ``tick()`` and ``drain()`` in lockstep and mirrors the whole placement, so each knows every retirement tick.  Per tick, one
+    int64 header broadcast from rank 0 carries the admissions and a global idle flag; when something is admitted, one float32
+    broadcast carries the newcomers' wav | prompt | x_T.  Each rank admits and ticks its own slots, the ranks exchange one status
+    flag (an exception on any rank raises a RuntimeError on every rank), and on ticks where something retires one ragged gather
+    (``shard.gather_ragged``) brings each result's NaN flag, latent and audio to rank 0.  Rank 0 returns the results and holds
+    ``last_latents``; the other ranks return {}.  The default x_T is drawn on rank 0 at ``submit``, as on one GPU, so every
+    result equals the one-GPU server's.  Waveforms and prompts travel as float32.  ``group=None`` or a world of 1 is the
+    one-GPU server."""
 
     def __init__(self, content_model, pre_model, unet, vocoder, slots: int = 8, max_frames: int = 1024, max_prompt_frames: int = 512,
-                 method: str = "unipc", steps: Optional[int] = None):
+                 method: str = "unipc", steps: Optional[int] = None, group: Optional[dist.ProcessGroup] = None):
         self.steps = convert._check_method(method, steps)
         if self.steps < 1:
             raise ValueError(f"steps must be >= 1, got {self.steps}")
@@ -109,12 +167,26 @@ class ConversionServer:
         self._requests: Dict[int, dict] = {}
         self._next_ticket = 0
         self._sess: Optional[DenoiserSession] = None        # device state: allocated by the first tick
+        self._freed: set = set()                            # slots retired since the last admission (their rows still hold the request)
+        self.group = group
+        self.world = dist.get_world_size(group) if group is not None else 1
+        self.rank = dist.get_rank(group) if self.world > 1 else 0
+        if self.world > 1:
+            self.tables = [SlotTable(self.B, self.steps) for _ in range(self.world)]   # every rank's slots, mirrored on every rank
+            self.table = self.tables[self.rank]
+            self._pending: collections.deque = collections.deque()                     # rank 0: tickets not yet placed
+            self._frames: Dict[int, int] = {}                                          # T_b of every placed request
+            self._checked = False
+            self._idle = True
+            self.served = 0                                                            # requests retired on any rank so far
 
     # ------------------------------------------------------------------------------------------------ requests
     def submit(self, wav: torch.Tensor, sr: int, prompt_mel: torch.Tensor, x_T: Optional[torch.Tensor] = None) -> int:
         """Queues one 1-D waveform at ``sr`` with its prompt mel [100, S_b] and returns its ticket (increasing, FIFO).  ``x_T``
         ([1, 100, T_b] or [100, T_b]) defaults to ``torch.randn((1, 100, T_b))`` on the model's device, drawn here: requests
-        submitted in list order get the draws ``convert_utterances`` makes for that list."""
+        submitted in list order get the draws ``convert_utterances`` makes for that list.  On several ranks only rank 0 submits."""
+        if self.world > 1 and self.rank != 0:
+            raise RuntimeError(f"submit() on rank {self.rank}: only rank 0 of the server's group takes requests")
         plan = convert._check_inputs([wav], sr, [prompt_mel], None if x_T is None else [x_T])[0]
         if plan["T"] > self.T:
             raise ValueError(f"the waveform is {plan['T']} frames, more than max_frames={self.T}")
@@ -126,34 +198,157 @@ class ConversionServer:
         ticket = self._next_ticket
         self._next_ticket += 1
         self._requests[ticket] = dict(wav=wav, sr=int(sr), prompt=prompt_mel, x_T=x_T, plan=plan, T=plan["T"], S=S_b)
-        self.table.enqueue(ticket)
+        if self.world > 1:
+            self._pending.append(ticket)
+        else:
+            self.table.enqueue(ticket)
         return ticket
 
     @torch.no_grad()
     def tick(self) -> Dict[int, object]:
         """Admits queued requests into the free slots, runs one tick and returns {ticket: audio [T_b * 256]} (or an
         ``AssertionError``) for the requests that finished in it.  Does nothing when the queue and the slots are empty."""
+        if self.world > 1:
+            return self._tick_group()
         if self.table.idle:
             return {}
         t = self.ticks
-        new = self.table.admit(t)
-        stale = self._setup()
-        if new:
-            self._admit(new)
-        elif stale:
-            self._prepare_all()
-        elif not self._sess._prepared or self._unet.__dict__.get("_cond_owner") is not self._sess:
-            self._sess.prepare()                            # another caller used the module's shared workspace since the last tick
-        self._run_tick()
+        self._step(self.table.admit(t))
         self.ticks += 1
         return self._retire(t)
 
     def drain(self) -> Dict[int, object]:
-        """Ticks until the queue and the slots are empty; returns every result."""
+        """Ticks until the queue and the slots are empty (on several ranks: everywhere, and every rank returns in the same
+        tick); returns every result."""
         out: Dict[int, object] = {}
+        if self.world > 1:
+            while True:
+                out.update(self.tick())
+                if self._idle:
+                    return out
         while not self.table.idle:
             out.update(self.tick())
         return out
+
+    def _step(self, new: List[Tuple[int, int]]):
+        """The device work of one tick on this server's slots: the admission of ``new`` (slot, ticket), then the tick."""
+        stale = self._setup()
+        if new:
+            self._admit(new, full=stale or not self._owns_cond())
+        elif stale:
+            self._prepare_all()
+        elif not self._owns_cond():
+            self._sess.prepare()                            # another caller used the module's shared workspace since the last tick
+        self._run_tick()
+
+    # ------------------------------------------------------------------------------------------------ several ranks
+    def _coll_device(self) -> Optional[torch.device]:
+        return self._device() if "nccl" in str(dist.get_backend(self.group)) else None
+
+    def _broadcast(self, t: torch.Tensor) -> torch.Tensor:
+        dev = self._coll_device()
+        t = t.to(dev) if dev is not None else t.cpu()
+        dist.broadcast(t, src=dist.get_global_rank(self.group, 0), group=self.group)
+        return t.cpu()
+
+    def _check_group_args(self):
+        """Raises ValueError on every rank unless every rank built the server with the same arguments (one all-gather)."""
+        key = torch.tensor([self.B, self.T, self.S, self.steps, int(self.kind == "dpm")], dtype=torch.int64)
+        keys = shard._all_gather(key, self.group, self._coll_device()).view(self.world, -1).cpu()
+        self._checked = True
+        if not bool((keys == keys[0]).all()):
+            raise ValueError("the ranks built their servers with different arguments (slots, max_frames, max_prompt_frames, steps, "
+                             f"dpmsolver per rank: {keys.tolist()})")
+
+    def _header(self, t: int) -> torch.Tensor:
+        """Rank 0: places the queued requests and packs the tick's header."""
+        free = {r: tab.free_slots() for r, tab in enumerate(self.tables)}
+        adm = []
+        for r in place_requests([len(free[r]) for r in range(self.world)], len(self._pending)):
+            tk = self._pending.popleft()
+            q = self._requests[tk]
+            adm.append((tk, r, free[r].pop(0), q["wav"].numel(), q["sr"], q["T"], q["S"]))
+        idle = not adm and all(tab.occupied == 0 for tab in self.tables)
+        return pack_header(adm, idle, self.world * self.B)
+
+    def _payload(self, adm) -> List[torch.Tensor]:
+        """Every newcomer's (wav, prompt [100, S_b], x_T [1, 100, T_b]) as sent by rank 0 in one float32 broadcast."""
+        sizes = [(n, LATENT_CH * Sb, LATENT_CH * Tb) for _, _, _, n, _, Tb, Sb in adm]
+        if self.rank == 0:
+            parts = []
+            for tk, *_ in adm:
+                q = self._requests[tk]
+                parts += [q["wav"].reshape(-1), q["prompt"].reshape(-1), q["x_T"].reshape(-1)]
+            dev = self._coll_device()
+            flat = torch.cat([p.to(dev if dev is not None else "cpu", torch.float32) for p in parts])
+        else:
+            flat = torch.empty(sum(sum(z) for z in sizes), dtype=torch.float32)
+        flat = self._broadcast(flat)
+        out, off = [], 0
+        for (n, np_, nx), (_, _, _, _, _, Tb, Sb) in zip(sizes, adm):
+            out.append((flat[off:off + n], flat[off + n:off + n + np_].view(LATENT_CH, Sb),
+                        flat[off + n + np_:off + n + np_ + nx].view(1, LATENT_CH, Tb)))
+            off += n + np_ + nx
+        return out
+
+    def _tick_group(self) -> Dict[int, object]:
+        if not self._checked:
+            self._check_group_args()
+        t = self.ticks
+        hdr = self._header(t) if self.rank == 0 else torch.zeros(2 + HEADER_FIELDS * self.world * self.B, dtype=torch.int64)
+        adm, self._idle = unpack_header(self._broadcast(hdr))
+        self.last_latents = {}
+        if self._idle:
+            return {}
+        payload = self._payload(adm) if adm else []
+        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T) in zip(adm, payload):
+            self.tables[r].enqueue(tk)
+            self._frames[tk] = Tb
+            if r == self.rank and self.rank != 0:
+                plan = convert._check_inputs([wav], sr, [prompt], [x_T])[0]
+                self._requests[tk] = dict(wav=wav, sr=sr, prompt=prompt, x_T=x_T, plan=plan, T=Tb, S=Sb)
+            elif r != self.rank:
+                self._requests.pop(tk, None)               # (rank 0: placed elsewhere)
+        news = [tab.admit(t) for tab in self.tables]
+        placed = sorted((r, s, tk) for r, new in enumerate(news) for s, tk in new)
+        if placed != sorted((r, s, tk) for tk, r, s, *_ in adm):
+            raise RuntimeError(f"rank {self.rank}: the mirrored placement {placed} differs from rank 0's")
+        err: Optional[Exception] = None
+        local: List[torch.Tensor] = []
+        dones: List[List[Tuple[int, int]]] = [[] for _ in range(self.world)]
+        try:
+            if self.table.occupied:
+                self._step(news[self.rank])
+            dones = [tab.retire(t) for tab in self.tables]   # (after the step: an admission zeroes the slots it sees free)
+            for flag, lat, audio in self._collect(dones[self.rank]):
+                local.append(torch.cat([torch.tensor([float(flag)], device=lat.device), lat.reshape(-1), audio.reshape(-1)]))
+        except Exception as e:                              # noqa: BLE001 (re-raised below on every rank)
+            err = e
+        failed = shard._all_gather(torch.tensor([err is not None], dtype=torch.int32), self.group,
+                                   self._coll_device()).nonzero().flatten().tolist()
+        if failed:
+            mine = f"; rank {self.rank} raised {type(err).__name__}: {err}" if err is not None else ""
+            raise RuntimeError(f"server tick {t} failed on rank(s) {failed}{mine}") from err
+        self.ticks += 1
+        if not any(dones):
+            return {}
+        order = [tk for done in dones for _, tk in done]
+        index = {tk: i for i, tk in enumerate(order)}
+        plan = [[[index[tk] for _, tk in done]] if done else [] for done in dones]
+        sizes = [1 + (LATENT_CH + HOP) * self._frames[tk] for tk in order]
+        got = shard.gather_ragged(local, plan, sizes, self.group, self._coll_device())
+        frames = [self._frames.pop(tk) for tk in order]
+        self.served += len(order)
+        if self.rank != 0:
+            return {}
+        out: Dict[int, object] = {}
+        for tk, Tb, v in zip(order, frames, got):
+            if v[0].item() != 0:
+                out[tk] = AssertionError(NAN_MESSAGE)
+                continue
+            self.last_latents[tk] = v[1:1 + LATENT_CH * Tb].view(LATENT_CH, Tb)
+            out[tk] = v[1 + LATENT_CH * Tb:]
+        return dict(sorted(out.items()))
 
     # ------------------------------------------------------------------------------------------------ device state
     @property
@@ -162,6 +357,10 @@ class ConversionServer:
 
     def _device(self) -> torch.device:
         return next(self._unet.parameters()).device
+
+    def _owns_cond(self) -> bool:
+        """True while the module's shared workspace holds this server's prepared conditioning."""
+        return self._sess._prepared and self._unet.__dict__.get("_cond_owner") is self._sess
 
     def _setup(self) -> bool:
         """Allocates the device state on the first call.  True when the weights were re-packed since the last tick: the captured
@@ -212,8 +411,9 @@ class ConversionServer:
         self._graph, self._runs = None, 0
         return False
 
-    def _admit(self, new: List[Tuple[int, int]]):
-        """Encodes the newcomers as one ragged batch per input rate, writes them into their slots, and prepares every slot again."""
+    def _admit(self, new: List[Tuple[int, int]], full: bool):
+        """Encodes the newcomers as one ragged batch per input rate and writes them into their slots.  Then prepares the rows
+        of the newcomers and of the slots freed since the last admission (``full``: every slot)."""
         cm, pm, _, _ = self.models
         sess, dev = self._sess, self._device()
         ev = None
@@ -249,7 +449,11 @@ class ConversionServer:
         slots = torch.tensor([s for s, _ in new], dtype=torch.int64, device=dev)
         self._k.index_fill_(0, slots, 0)
         self._nan.index_fill_(0, slots, 0)
-        self._prepare_all()
+        if full:
+            self._prepare_all()
+        else:
+            self._prepare_rows(sorted({s for s, _ in new} | (self._freed - occupied)))
+        self._freed.clear()
         if ev is not None:
             ev[1].record()
             self.admission_events.append(ev)
@@ -261,6 +465,14 @@ class ConversionServer:
         sess.plen.copy_(torch.tensor(self._plen, dtype=torch.int64))
         sess.prepare()
         sess.time_table(self._tvals, self._film_table)
+
+    def _prepare_rows(self, rows: List[int]):
+        """The conditioning and the FiLM rows (every step) of the listed slots only; the other slots' stay as they are."""
+        sess = self._sess
+        sess.clen.copy_(torch.tensor(self._clen, dtype=torch.int64))
+        sess.plen.copy_(torch.tensor(self._plen, dtype=torch.int64))
+        sess.prepare_rows(rows)
+        sess.time_table_rows(self._tvals, self._film_table, rows)
 
     def _body(self):
         """One tick: the FiLM row (k_b, b) of every slot, the forward, the row step, then the rotation of the sampler's buffers.
@@ -308,11 +520,26 @@ class ConversionServer:
         self.last_latents = {}
         if not done:
             return {}
+        out: Dict[int, object] = {}
+        for (_, tk), (flag, lat, audio) in zip(done, self._collect(done)):
+            if flag != 0:
+                out[tk] = AssertionError(NAN_MESSAGE)
+            else:
+                out[tk] = audio
+                self.last_latents[tk] = lat
+        return dict(sorted(out.items()))
+
+    def _collect(self, done: List[Tuple[int, int]]) -> List[Tuple[int, torch.Tensor, torch.Tensor]]:
+        """(NaN flag, latent [100, T_b], audio [T_b * 256]) of each retired (slot, ticket), in order; a flagged request's
+        latent and audio are zeros.  Frees the slots and forgets the requests."""
+        if not done:
+            return []
         dev = self._device()
         slots = torch.tensor([s for s, _ in done], dtype=torch.int64, device=dev)
         flags = self._nan.index_select(0, slots).tolist()
         self._k.index_fill_(0, slots, -1)
-        out: Dict[int, object] = {}
+        self._freed.update(s for s, _ in done)
+        res: Dict[int, Tuple[torch.Tensor, torch.Tensor]] = {}
         ok = [(s, tk) for (s, tk), f in zip(done, flags) if f == 0]
         if ok:
             tl = [self._requests[tk]["T"] for _, tk in ok]
@@ -320,11 +547,12 @@ class ConversionServer:
             lat = self._x.index_select(0, rows)[:, :, :max(tl)].contiguous()
             audio = self.models[3].decode(lat, torch.tensor(tl, dtype=torch.int64))
             for j, (_, tk) in enumerate(ok):
-                out[tk] = audio[j, :tl[j] * HOP]
-                self.last_latents[tk] = lat[j, :, :tl[j]]
+                res[tk] = (lat[j, :, :tl[j]], audio[j, :tl[j] * HOP])
+        out = []
         for (_, tk), f in zip(done, flags):
-            if f != 0:
-                out[tk] = AssertionError(NAN_MESSAGE)
+            Tb = self._requests[tk]["T"]
+            lat, audio = res.get(tk, (torch.zeros((LATENT_CH, Tb), device=dev), torch.zeros(Tb * HOP, device=dev)))
+            out.append((int(f), lat, audio))
         for _, tk in done:
             del self._requests[tk]
-        return dict(sorted(out.items()))
+        return out
