@@ -128,9 +128,14 @@ int ns2vc_unet_forward_film(ns2vc_unet* h, const float* x, long long x_bstride, 
  * DPM-Solver++(2M): model_wrapper x_start->noise (sampler/dpm_solver.py:291-292), data_prediction_fn
  * (:437-439), dpm_solver_first_update (:569-576), multistep_dpm_solver_second_update (:813-831). */
 typedef struct ns2vc_dpm_coef {
-  float alpha_s, sigma_s, c_x, c_m, c_d, inv_r0;
+  float alpha_s, sigma_s;     /* at the time the UNet was evaluated (x0 round trip)                */
+  float c_x;                  /* sigma_t / sigma_s                                                 */
+  float c_m;                  /* alpha_t * expm1(-h)                                               */
+  float c_d;                  /* 0.5 * c_m                                                         */
+  float inv_r0;               /* 1 / r0 (order 2 only)                                             */
   int order;                  /* 0: x0 round trip only; 1 / 2: + first / second order update       */
 } ns2vc_dpm_coef;
+/* x_next = (c_x*x - c_m*m_cur) - c_d*(inv_r0*(m_cur - m_prev)), the last term at order 2 only */
 /* nan_flag (device int, may be NULL): set to 1 when x holds a NaN - the reference asserts on that every denoiser call
  * (model.py:404); the fused loop checks the flag once after the run instead of syncing every step. */
 int ns2vc_dpm_step(const float* x, const float* unet_out, const float* m_prev, const ns2vc_dpm_coef* c, float* m_cur,
@@ -138,10 +143,17 @@ int ns2vc_dpm_step(const float* x, const float* unet_out, const float* m_prev, c
 
 /* UniPC-bh2 (sampler/uni_pc.py:471-588): corrector at t and predictor to the next time. */
 typedef struct ns2vc_unipc_coef {
-  float alpha_t, sigma_t, c_x, c_m, ab, rk, rho0, rho1;
-  int corr_order;
-  float n_c_x, n_c_m, nab, nrk;
-  int pred_order;
+  float alpha_t, sigma_t;     /* x0 round trip at t                                                */
+  /* corrector at t from (x_prev, m0, m1): x_t = xbar - ab*(rho0*D1 + rho1*(m_t - m0))                */
+  float c_x, c_m;             /* xbar = c_x*x_prev - c_m*m0                                        */
+  float ab;                   /* alpha_t * B_h                                                     */
+  float rk;                   /* D1 = (m1 - m0) / rk (order-2 corrector)                           */
+  float rho0, rho1;
+  int corr_order;             /* 0: no corrector (the first step: history only), 1, 2              */
+  /* predictor to the next time from (x_t, m_t, m0): x_pred = nbar - nab*(0.5*D1n), D1n = (m0 - m_t)/nrk */
+  float n_c_x, n_c_m;         /* nbar = n_c_x*x_t - n_c_m*m_t                                      */
+  float nab, nrk;
+  int pred_order;             /* 0: none, 1: nbar only, 2: with D1n                                */
 } ns2vc_unipc_coef;
 int ns2vc_unipc_step(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
                      const ns2vc_unipc_coef* c, float* m_t, float* x_t, float* x_pred, size_t n, int* nan_flag,

@@ -8,11 +8,13 @@ The reference spends ~165 micro-kernels per step on this (SURVEY §2.3 K17).
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
-from typing import List
+from typing import List, Tuple
 
 import torch
 
+from . import _lib
 from .schedule import NoiseScheduleVP
 
 
@@ -257,3 +259,26 @@ def ddim_table(buffers: dict, total: int, sampling_timesteps: int, eta: float = 
             st.c, st.sigma = _f(c), _f(sigma)
         out.append(st)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------- C-ABI structs
+_C_STRUCTS = {DpmStep: _lib.DpmCoef, UniPcStep: _lib.UniPcCoef, DdpmStep: _lib.DdpmCoef, DdimStep: _lib.DdimCoef}
+
+
+def c_struct(step):
+    """The step's coefficient struct of the C-ABI (``ns2vc_dpm_coef``, ``ns2vc_unipc_coef``, ``ns2vc_ddpm_coef`` or
+    ``ns2vc_ddim_coef``), every field taken by name from the step record."""
+    cls = _C_STRUCTS[type(step)]
+    return cls(**{name: int(getattr(step, name)) if ctype is C.c_int else getattr(step, name) for name, ctype in cls._fields_})
+
+
+def c_table(steps, device) -> Tuple[torch.Tensor, int]:
+    """The steps' structs back to back in a device byte table (the row steps and the DDPM / DDIM steps read their struct from
+    device memory), and the size of one struct in bytes."""
+    arr = (_C_STRUCTS[type(steps[0])] * len(steps))(*[c_struct(s) for s in steps])
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(device), C.sizeof(arr) // len(steps)
+
+
+def t_inputs(steps, B: int, device) -> torch.Tensor:
+    """The model time of every step for each of B rows: [steps, B] fp32 on ``device``, the step-major rows of the FiLM table."""
+    return torch.tensor([[s.t_input] * B for s in steps], dtype=torch.float32).to(device)

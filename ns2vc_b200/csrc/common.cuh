@@ -352,58 +352,6 @@ struct RaggedTables {
 int launch_ragged_tables(const long long* content_lengths, const long long* prompt_lengths, const RaggedTables& r, cudaStream_t st,
                          int b0 = 0, int n = 0);
 
-// Fused sampler steps (element-wise, bit-exact op order; see kernels_misc.cu)
-struct DpmStepCoef {   // DPM-Solver++(2M): one post-UNet step
-  float alpha_s, sigma_s;      // at the time the UNet was evaluated (x0 round trip)
-  float c_x;                   // sigma_t / sigma_s
-  float c_m;                   // alpha_t * expm1(-h)
-  float c_d;                   // 0.5 * c_m
-  float inv_r0;                // 1 / r0        (order 2 only)
-  int order;                   // 0: round trip only, 1: first-order update, 2: second-order update
-};
-int launch_dpm_step(const float* x, const float* unet_out, const float* m_prev, const DpmStepCoef& c,
-                    float* m_cur, float* x_next, size_t n, int* nan_flag, cudaStream_t st);
-
-struct UniPcStepCoef {  // UniPC-bh2, data prediction: corrector at t (+ predictor to t_next)
-  float alpha_t, sigma_t;      // x0 round trip at t
-  // corrector at t from (x_prev at t_p0, m0, m1):  x_t = xbar - ab*(rho0*D1 + rho1*(m_t - m0))
-  float c_x, c_m;              // xbar = c_x * x_prev - c_m * m0
-  float ab;                    // alpha_t * B_h
-  float rk;                    // D1 = (m1 - m0) / rk   (order-2 corrector)
-  float rho0, rho1;
-  int corr_order;              // 0: no corrector (first call: history only), 1, 2
-  // predictor to t_next from (x_t, m_t, m0):  x_pred = nbar - nab*(0.5*D1n), D1n = (m0 - m_t)/nrk
-  float n_c_x, n_c_m, nab, nrk;
-  int pred_order;              // 0: none, 1: xbar only, 2: with D1n
-};
-int launch_unipc_step(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0,
-                      const float* m1, const UniPcStepCoef& c, float* m_t, float* x_t, float* x_pred, size_t n,
-                      int* nan_flag, cudaStream_t st);
-
-// Per-row steps: row b of [B, row_n] takes the DEVICE struct coefs[k[b]] (k[b] < 0: an empty row, zeros out); k[b] is advanced
-int launch_dpm_step_rows(const float* x, const float* unet_out, const float* m_prev, const DpmStepCoef* coefs, int* k, float* m_cur,
-                         float* x_next, size_t row_n, int B, int* nan_flags, cudaStream_t st);
-int launch_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
-                           const UniPcStepCoef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
-                           int* nan_flags, cudaStream_t st);
-
-// DDPM / DDIM steps: the coefficient struct is read from DEVICE memory (layout of ns2vc_ddpm_coef / ns2vc_ddim_coef)
-struct DdpmStepCoef {   // x_next = (c_x0*x0 + c_x*x) + (add_noise ? c_noise*noise : 0)
-  float c_x0, c_x;             // posterior_mean_coef1[t], posterior_mean_coef2[t]
-  float c_noise;               // exp(0.5 * posterior_log_variance_clipped[t])
-  int add_noise;               // t > 0
-};
-int launch_ddpm_step(const float* x, const float* x0, const float* noise, const DdpmStepCoef* c, float* x_next, size_t n,
-                     int* nan_flag, cudaStream_t st);
-
-struct DdimStepCoef {   // pn = (sqrt_recip*x - x0)/sqrt_recipm1 ; x_next = (x0*sqrt_alpha_next + c*pn) + sigma*noise, or x0 if last
-  float sqrt_recip, sqrt_recipm1;
-  float sqrt_alpha_next, c, sigma;
-  int last;                    // the pair (t, -1)
-};
-int launch_ddim_step(const float* x, const float* x0, const float* noise, const DdimStepCoef* c, float* x_next, size_t n,
-                     int* nan_flag, cudaStream_t st);
-
 // ---------------------------------------------------------------------------------------------
 // Condition encoders (pre_kernels.cu; program in pre_engine.cu)
 // ---------------------------------------------------------------------------------------------

@@ -1293,68 +1293,6 @@ int ns2vc_unet_forward_film(ns2vc_unet* h, const float* x, long long x_bstride, 
   return rc;
 }
 
-int ns2vc_dpm_step(const float* x, const float* unet_out, const float* m_prev, const ns2vc_dpm_coef* c, float* m_cur, float* x_next,
-                   size_t n, int* nan_flag, ns2vc_stream stream) {
-  NS_REQUIRE(x && unet_out && c && m_cur, "null argument");
-  NS_REQUIRE(c->order == 0 || x_next, "x_next is NULL");
-  NS_REQUIRE(c->order < 2 || m_prev, "m_prev is NULL for a second-order step");
-  DpmStepCoef k; k.alpha_s = c->alpha_s; k.sigma_s = c->sigma_s; k.c_x = c->c_x; k.c_m = c->c_m; k.c_d = c->c_d; k.inv_r0 = c->inv_r0; k.order = c->order;
-  return launch_dpm_step(x, unet_out, m_prev, k, m_cur, x_next, n, nan_flag, (cudaStream_t)stream);
-}
-
-int ns2vc_unipc_step(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
-                     const ns2vc_unipc_coef* c, float* m_t, float* x_t, float* x_pred, size_t n, int* nan_flag, ns2vc_stream stream) {
-  NS_REQUIRE(x_eval && unet_out && c && m_t, "null argument");
-  NS_REQUIRE(c->corr_order == 0 || (x_prev && m0 && x_t), "corrector inputs missing");
-  NS_REQUIRE(c->corr_order < 2 || m1, "m1 is NULL for an order-2 corrector");
-  NS_REQUIRE(c->pred_order == 0 || x_pred, "x_pred is NULL");
-  NS_REQUIRE(c->pred_order < 2 || c->corr_order > 0, "order-2 predictor needs the previous model output");
-  UniPcStepCoef k;
-  k.alpha_t = c->alpha_t; k.sigma_t = c->sigma_t; k.c_x = c->c_x; k.c_m = c->c_m; k.ab = c->ab; k.rk = c->rk; k.rho0 = c->rho0; k.rho1 = c->rho1;
-  k.corr_order = c->corr_order; k.n_c_x = c->n_c_x; k.n_c_m = c->n_c_m; k.nab = c->nab; k.nrk = c->nrk; k.pred_order = c->pred_order;
-  return launch_unipc_step(x_prev, x_eval, unet_out, m0, m1, k, m_t, x_t, x_pred, n, nan_flag, (cudaStream_t)stream);
-}
-
-static_assert(sizeof(ns2vc_dpm_coef) == sizeof(DpmStepCoef) && offsetof(ns2vc_dpm_coef, order) == offsetof(DpmStepCoef, order),
-              "ns2vc_dpm_coef and DpmStepCoef must share one layout (the row kernel reads the caller's structs from device memory)");
-static_assert(sizeof(ns2vc_unipc_coef) == sizeof(UniPcStepCoef) && offsetof(ns2vc_unipc_coef, corr_order) == offsetof(UniPcStepCoef, corr_order) &&
-              offsetof(ns2vc_unipc_coef, pred_order) == offsetof(UniPcStepCoef, pred_order),
-              "ns2vc_unipc_coef and UniPcStepCoef must share one layout (the row kernel reads the caller's structs from device memory)");
-
-int ns2vc_dpm_step_rows(const float* x, const float* unet_out, const float* m_prev, const ns2vc_dpm_coef* coefs, int* k, float* m_cur,
-                        float* x_next, size_t row_n, int B, int* nan_flags, ns2vc_stream stream) {
-  NS_REQUIRE(x && unet_out && m_prev && coefs && k && m_cur && x_next, "null argument");
-  NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_dpm_step_rows(x, unet_out, m_prev, reinterpret_cast<const DpmStepCoef*>(coefs), k, m_cur, x_next, row_n, B, nan_flags,
-                              (cudaStream_t)stream);
-}
-
-int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
-                          const ns2vc_unipc_coef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
-                          int* nan_flags, ns2vc_stream stream) {
-  NS_REQUIRE(x_prev && x_eval && unet_out && m0 && m1 && coefs && k && m_t && x_t && x_pred, "null argument");
-  NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_unipc_step_rows(x_prev, x_eval, unet_out, m0, m1, reinterpret_cast<const UniPcStepCoef*>(coefs), k, m_t, x_t, x_pred,
-                                row_n, B, nan_flags, (cudaStream_t)stream);
-}
-
-static_assert(sizeof(ns2vc_ddpm_coef) == sizeof(DdpmStepCoef) && offsetof(ns2vc_ddpm_coef, add_noise) == offsetof(DdpmStepCoef, add_noise),
-              "ns2vc_ddpm_coef and DdpmStepCoef must share one layout (the kernel reads the caller's struct from device memory)");
-static_assert(sizeof(ns2vc_ddim_coef) == sizeof(DdimStepCoef) && offsetof(ns2vc_ddim_coef, last) == offsetof(DdimStepCoef, last),
-              "ns2vc_ddim_coef and DdimStepCoef must share one layout (the kernel reads the caller's struct from device memory)");
-
-int ns2vc_ddpm_step(const float* x, const float* x0, const float* noise, const ns2vc_ddpm_coef* c, float* x_next, size_t n,
-                    int* nan_flag, ns2vc_stream stream) {
-  NS_REQUIRE(x && x0 && c && x_next, "null argument");
-  return launch_ddpm_step(x, x0, noise, reinterpret_cast<const DdpmStepCoef*>(c), x_next, n, nan_flag, (cudaStream_t)stream);
-}
-
-int ns2vc_ddim_step(const float* x, const float* x0, const float* noise, const ns2vc_ddim_coef* c, float* x_next, size_t n,
-                    int* nan_flag, ns2vc_stream stream) {
-  NS_REQUIRE(x && x0 && c && x_next, "null argument");
-  return launch_ddim_step(x, x0, noise, reinterpret_cast<const DdimStepCoef*>(c), x_next, n, nan_flag, (cudaStream_t)stream);
-}
-
 int ns2vc_mask_bias(const uint8_t* mask, int n, float* bias, ns2vc_stream stream) {
   NS_REQUIRE(mask && bias && n >= 0, "bad argument");
   return launch_mask_bias(MaskBiasOp{mask, n, bias}, (cudaStream_t)stream);

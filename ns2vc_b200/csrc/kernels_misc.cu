@@ -1,10 +1,9 @@
 // Small HBM/L2-bound kernels of the denoiser step: layout conversion, GroupNorm/LayerNorm
-// statistics, the timestep/FiLM GEMV, AttentionPooling pieces, and the fused sampler updates.
+// statistics, the timestep/FiLM GEMV and AttentionPooling pieces.
 // All are coalesced/vectorised; none is worth tensor cores.
 #include "gemm_common.cuh"
 #include "prep_common.cuh"
 #include "launch.cuh"
-#include <cooperative_groups.h>
 #include <cstdarg>
 #include <cstdio>
 #include <math.h>
@@ -507,281 +506,6 @@ int launch_ragged_tables(const long long* content_lengths, const long long* prom
   if (n <= 0) n = r.B;
   if (b0 < 0 || b0 + n > r.B) { set_error("ragged tables: entries [%d, %d) of %d", b0, b0 + n, r.B); return -1; }
   ragged_tables_kernel<<<n, 256, 0, st>>>(content_lengths, prompt_lengths, r, b0);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Fused sampler steps.  Every arithmetic op uses the round-to-nearest intrinsics so that the
-// compiler cannot contract a*b+c into an FMA: the reference evaluates each product and sum as a
-// separate fp32 tensor op (dpm_solver.py:291-292, 437-439, 569-576, 813-831), and the result
-// here is bit-identical to that sequence.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float x0_round_trip(float x, float o, float alpha, float sigma) {
-  // noise = (x - alpha*out)/sigma  (model_wrapper, x_start)  ;  x0 = (x - sigma*noise)/alpha
-  float noise = __fdiv_rn(__fsub_rn(x, __fmul_rn(alpha, o)), sigma);
-  return __fdiv_rn(__fsub_rn(x, __fmul_rn(sigma, noise)), alpha);
-}
-
-__global__ void __launch_bounds__(256) dpm_step_kernel(const float* __restrict__ x, const float* __restrict__ o,
-                                                       const float* __restrict__ mp, DpmStepCoef c,
-                                                       float* __restrict__ mc, float* __restrict__ xn, size_t n, int* nan_flag) {
-  pdl_trigger();
-  pdl_wait();
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  bool bad = false;
-  for (; i < n; i += stride) {
-    const float xv = x[i];
-    bad |= (xv != xv);                                     // the reference asserts on NaN in the denoiser input every call (model.py:404)
-    const float m0 = x0_round_trip(xv, o[i], c.alpha_s, c.sigma_s);
-    mc[i] = m0;
-    if (c.order == 0) continue;
-    float r = __fsub_rn(__fmul_rn(c.c_x, xv), __fmul_rn(c.c_m, m0));
-    if (c.order == 2) {
-      float d1 = __fmul_rn(c.inv_r0, __fsub_rn(m0, mp[i]));
-      r = __fsub_rn(r, __fmul_rn(c.c_d, d1));
-    }
-    xn[i] = r;
-  }
-  if (bad && nan_flag) atomicOr(nan_flag, 1);
-}
-int launch_dpm_step(const float* x, const float* unet_out, const float* m_prev, const DpmStepCoef& c, float* m_cur,
-                    float* x_next, size_t n, int* nan_flag, cudaStream_t st) {
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  launch_k(dpm_step_kernel, dim3(blocks), dim3(256), 0, st, x, unet_out, m_prev, c, m_cur, x_next, n, nan_flag);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-__global__ void __launch_bounds__(256) unipc_step_kernel(const float* __restrict__ xp, const float* __restrict__ xe,
-                                                         const float* __restrict__ o, const float* __restrict__ m0p,
-                                                         const float* __restrict__ m1p, UniPcStepCoef c,
-                                                         float* __restrict__ mt_out, float* __restrict__ xt_out,
-                                                         float* __restrict__ xpred_out, size_t n, int* nan_flag) {
-  pdl_trigger();
-  pdl_wait();
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  bool bad = false;
-  for (; i < n; i += stride) {
-    const float xev = xe[i];
-    bad |= (xev != xev);                                   // NaN guard of the denoiser input (model.py:404)
-    const float mt = x0_round_trip(xev, o[i], c.alpha_t, c.sigma_t);
-    mt_out[i] = mt;
-    float xt = xev;
-    float m0 = 0.f;
-    if (c.corr_order > 0) {
-      m0 = m0p[i];
-      // uni_pc.py:533-536, 561-567
-      const float xbar = __fsub_rn(__fmul_rn(c.c_x, xp[i]), __fmul_rn(c.c_m, m0));
-      const float d1t = __fsub_rn(mt, m0);
-      float inner;
-      if (c.corr_order == 2) {
-        const float d1 = __fdiv_rn(__fsub_rn(m1p[i], m0), c.rk);
-        inner = __fadd_rn(__fmul_rn(c.rho0, d1), __fmul_rn(c.rho1, d1t));
-      } else {
-        inner = __fmul_rn(c.rho1, d1t);     // 0 + 0.5*D1_t
-      }
-      xt = __fsub_rn(xbar, __fmul_rn(c.ab, inner));
-      xt_out[i] = xt;
-    }
-    if (c.pred_order > 0) {
-      const float nbar = __fsub_rn(__fmul_rn(c.n_c_x, xt), __fmul_rn(c.n_c_m, mt));
-      float xpred = nbar;
-      if (c.pred_order == 2) {
-        const float d1n = __fdiv_rn(__fsub_rn(m0, mt), c.nrk);
-        xpred = __fsub_rn(nbar, __fmul_rn(c.nab, __fmul_rn(0.5f, d1n)));
-      }
-      xpred_out[i] = xpred;
-    }
-  }
-  if (bad && nan_flag) atomicOr(nan_flag, 1);
-}
-int launch_unipc_step(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0,
-                      const float* m1, const UniPcStepCoef& c, float* m_t, float* x_t, float* x_pred, size_t n,
-                      int* nan_flag, cudaStream_t st) {
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  launch_k(unipc_step_kernel, dim3(blocks), dim3(256), 0, st, x_prev, x_eval, unet_out, m0, m1, c, m_t, x_t, x_pred, n, nan_flag);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-// Per-row sampler steps: row b of a [B, row_n] batch takes step k[b] of a run whose coefficient structs sit in device memory,
-// so the rows of one batch can be at different steps (requests that joined at different ticks).  Each row is one cluster of
-// kRowCtas CTAs (grid kRowCtas x B); an occupied row does exactly the scalar kernel's arithmetic with struct k[b], an empty row
-// (k[b] < 0) writes zeros and raises nothing.  Every CTA reads k[b] before the cluster barrier and CTA 0 advances it after, so
-// a captured tick replays with no host write in between.  The NaN flag is per row.
-constexpr int kRowCtas = 8;
-
-__global__ void __launch_bounds__(256) dpm_step_rows_kernel(const float* __restrict__ x, const float* __restrict__ o,
-                                                            const float* __restrict__ mp, const DpmStepCoef* __restrict__ cs,
-                                                            int* k, float* __restrict__ mc, float* __restrict__ xn, size_t row_n,
-                                                            int* nan_flags) {
-  pdl_trigger();
-  pdl_wait();
-  const int b = blockIdx.y;
-  const int kb = k[b];
-  const size_t off = (size_t)b * row_n;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  if (kb < 0) {
-    for (; i < row_n; i += stride) { mc[off + i] = 0.f; xn[off + i] = 0.f; }
-  } else {
-    const DpmStepCoef c = cs[kb];
-    bool bad = false;
-    for (; i < row_n; i += stride) {
-      const size_t j = off + i;
-      const float xv = x[j];
-      bad |= (xv != xv);
-      const float m0 = x0_round_trip(xv, o[j], c.alpha_s, c.sigma_s);
-      mc[j] = m0;
-      if (c.order == 0) continue;
-      float r = __fsub_rn(__fmul_rn(c.c_x, xv), __fmul_rn(c.c_m, m0));
-      if (c.order == 2) {
-        float d1 = __fmul_rn(c.inv_r0, __fsub_rn(m0, mp[j]));
-        r = __fsub_rn(r, __fmul_rn(c.c_d, d1));
-      }
-      xn[j] = r;
-    }
-    if (bad && nan_flags) atomicOr(nan_flags + b, 1);
-  }
-  cooperative_groups::this_cluster().sync();               // every CTA of the row has read k[b]
-  if (kb >= 0 && blockIdx.x == 0 && threadIdx.x == 0) k[b] = kb + 1;
-}
-int launch_dpm_step_rows(const float* x, const float* unet_out, const float* m_prev, const DpmStepCoef* coefs, int* k, float* m_cur,
-                         float* x_next, size_t row_n, int B, int* nan_flags, cudaStream_t st) {
-  launch_kc(dpm_step_rows_kernel, dim3(kRowCtas, B), dim3(256), 0, st, dim3(kRowCtas, 1, 1), x, unet_out, m_prev, coefs, k, m_cur,
-            x_next, row_n, nan_flags);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-// UniPC rows.  A row at its first step (corr_order == 0) writes x_t = x_eval, so the caller's rotation (m1 <- m0 <- m_t,
-// x_prev <- x_t, x_eval <- x_pred) is the same for every row whatever its step.
-__global__ void __launch_bounds__(256) unipc_step_rows_kernel(const float* __restrict__ xp, const float* __restrict__ xe,
-                                                              const float* __restrict__ o, const float* __restrict__ m0p,
-                                                              const float* __restrict__ m1p, const UniPcStepCoef* __restrict__ cs,
-                                                              int* k, float* __restrict__ mt_out, float* __restrict__ xt_out,
-                                                              float* __restrict__ xpred_out, size_t row_n, int* nan_flags) {
-  pdl_trigger();
-  pdl_wait();
-  const int b = blockIdx.y;
-  const int kb = k[b];
-  const size_t off = (size_t)b * row_n;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  if (kb < 0) {
-    for (; i < row_n; i += stride) { mt_out[off + i] = 0.f; xt_out[off + i] = 0.f; xpred_out[off + i] = 0.f; }
-  } else {
-    const UniPcStepCoef c = cs[kb];
-    bool bad = false;
-    for (; i < row_n; i += stride) {
-      const size_t j = off + i;
-      const float xev = xe[j];
-      bad |= (xev != xev);
-      const float mt = x0_round_trip(xev, o[j], c.alpha_t, c.sigma_t);
-      mt_out[j] = mt;
-      float xt = xev;
-      float m0 = 0.f;
-      if (c.corr_order > 0) {
-        m0 = m0p[j];
-        const float xbar = __fsub_rn(__fmul_rn(c.c_x, xp[j]), __fmul_rn(c.c_m, m0));
-        const float d1t = __fsub_rn(mt, m0);
-        float inner;
-        if (c.corr_order == 2) {
-          const float d1 = __fdiv_rn(__fsub_rn(m1p[j], m0), c.rk);
-          inner = __fadd_rn(__fmul_rn(c.rho0, d1), __fmul_rn(c.rho1, d1t));
-        } else {
-          inner = __fmul_rn(c.rho1, d1t);
-        }
-        xt = __fsub_rn(xbar, __fmul_rn(c.ab, inner));
-      }
-      xt_out[j] = xt;
-      if (c.pred_order > 0) {
-        const float nbar = __fsub_rn(__fmul_rn(c.n_c_x, xt), __fmul_rn(c.n_c_m, mt));
-        float xpred = nbar;
-        if (c.pred_order == 2) {
-          const float d1n = __fdiv_rn(__fsub_rn(m0, mt), c.nrk);
-          xpred = __fsub_rn(nbar, __fmul_rn(c.nab, __fmul_rn(0.5f, d1n)));
-        }
-        xpred_out[j] = xpred;
-      }
-    }
-    if (bad && nan_flags) atomicOr(nan_flags + b, 1);
-  }
-  cooperative_groups::this_cluster().sync();
-  if (kb >= 0 && blockIdx.x == 0 && threadIdx.x == 0) k[b] = kb + 1;
-}
-int launch_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
-                           const UniPcStepCoef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
-                           int* nan_flags, cudaStream_t st) {
-  launch_kc(unipc_step_rows_kernel, dim3(kRowCtas, B), dim3(256), 0, st, dim3(kRowCtas, 1, 1), x_prev, x_eval, unet_out, m0, m1, coefs,
-            k, m_t, x_t, x_pred, row_n, nan_flags);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-// DDPM p_sample and DDIM steps (model.py:535-542, 586-601).  The scalars are read from device memory (one struct per step), so a
-// captured chunk of steps serves any window of a run: the host refills the coefficient window before each replay.  x_next may
-// be x itself (each element is read before it is written), which keeps a run's latents in one buffer.
-__global__ void __launch_bounds__(256) ddpm_step_kernel(const float* x, const float* __restrict__ x0, const float* __restrict__ noise,
-                                                        const DdpmStepCoef* __restrict__ cp, float* x_next, size_t n, int* nan_flag) {
-  pdl_trigger();
-  pdl_wait();
-  const DdpmStepCoef c = *cp;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  bool bad = false;
-  for (; i < n; i += stride) {
-    const float xv = x[i];
-    bad |= (xv != xv);                                     // NaN guard of the denoiser input (model.py:404)
-    // q_posterior mean (:509-512), then mean + exp(0.5 * logvar) * noise; at t == 0 the reference adds exp(.) * 0. (:540-541)
-    const float mean = __fadd_rn(__fmul_rn(c.c_x0, x0[i]), __fmul_rn(c.c_x, xv));
-    x_next[i] = __fadd_rn(mean, c.add_noise ? __fmul_rn(c.c_noise, noise[i]) : 0.0f);
-  }
-  if (bad && nan_flag) atomicOr(nan_flag, 1);
-}
-int launch_ddpm_step(const float* x, const float* x0, const float* noise, const DdpmStepCoef* c, float* x_next, size_t n,
-                     int* nan_flag, cudaStream_t st) {
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  launch_k(ddpm_step_kernel, dim3(blocks), dim3(256), 0, st, x, x0, noise, c, x_next, n, nan_flag);
-  NS_LAUNCH_CHECK();
-  return 0;
-}
-
-__global__ void __launch_bounds__(256) ddim_step_kernel(const float* x, const float* __restrict__ x0, const float* __restrict__ noise,
-                                                        const DdimStepCoef* __restrict__ cp, float* x_next, size_t n, int* nan_flag) {
-  pdl_trigger();
-  pdl_wait();
-  const DdimStepCoef c = *cp;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  bool bad = false;
-  for (; i < n; i += stride) {
-    const float xv = x[i];
-    bad |= (xv != xv);                                     // NaN guard of the denoiser input (model.py:404)
-    const float x0v = x0[i];
-    if (c.last) {                                          // the pair (t, -1): img = x_start (:589-592)
-      x_next[i] = x0v;
-      continue;
-    }
-    // predict_noise_from_start (:498-503), then x0 * sqrt(a_next) + c * pred_noise + sigma * noise (:599-601); the sigma term is
-    // kept at eta = 0: it decides the sign of zero results
-    const float pn = __fdiv_rn(__fsub_rn(__fmul_rn(c.sqrt_recip, xv), x0v), c.sqrt_recipm1);
-    const float r = __fadd_rn(__fmul_rn(x0v, c.sqrt_alpha_next), __fmul_rn(c.c, pn));
-    x_next[i] = __fadd_rn(r, __fmul_rn(c.sigma, noise[i]));
-  }
-  if (bad && nan_flag) atomicOr(nan_flag, 1);
-}
-int launch_ddim_step(const float* x, const float* x0, const float* noise, const DdimStepCoef* c, float* x_next, size_t n,
-                     int* nan_flag, cudaStream_t st) {
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  launch_k(ddim_step_kernel, dim3(blocks), dim3(256), 0, st, x, x0, noise, c, x_next, n, nan_flag);
   NS_LAUNCH_CHECK();
   return 0;
 }

@@ -214,7 +214,7 @@ class DenoiserSession:
                 out.copy_(self.first_out)
             else:
                 self.forward(x, ent["tvals"][k], out, film_rows=self._film(ent, k))
-            c = _lib.DpmCoef(st.alpha_s, st.sigma_s, st.c_x, st.c_m, st.c_d, st.inv_r0, st.order)
+            c = coefs.c_struct(st)
             with torch.cuda.device(self.dev):
                 _lib.check(self.L.ns2vc_dpm_step(x.data_ptr(), out.data_ptr(), m_b.data_ptr(), C.byref(c), m_a.data_ptr(),
                                                  x_next.data_ptr(), n, self.nan_flag.data_ptr(), stream))
@@ -237,8 +237,7 @@ class DenoiserSession:
             m_t = torch.empty_like(x_prev)
             x_t = torch.empty_like(x_prev) if st.corr_order > 0 else None
             x_pred = torch.empty_like(x_prev)
-            c = _lib.UniPcCoef(st.alpha_t, st.sigma_t, st.c_x, st.c_m, st.ab, st.rk, st.rho0, st.rho1, st.corr_order,
-                               st.n_c_x, st.n_c_m, st.nab, st.nrk, st.pred_order)
+            c = coefs.c_struct(st)
             with torch.cuda.device(self.dev):
                 _lib.check(self.L.ns2vc_unipc_step(
                     x_prev.data_ptr(), x_eval.data_ptr(), out.data_ptr(), m0.data_ptr() if m0 is not None else None,
@@ -289,7 +288,7 @@ class DenoiserSession:
         ent = self._graphs.get(key)
         if ent is None:
             steps = _step_table(kind, ns, ts, extra, key[:4])
-            tvals = torch.tensor([[st.t_input] * self.B for st in steps], dtype=torch.float32).to(self.dev)
+            tvals = coefs.t_inputs(steps, self.B, self.dev)
             nrows = tvals.numel()
             table = torch.empty(int(self.L.ns2vc_unet_time_table_floats(self.h, nrows)), dtype=torch.float32, device=self.dev)
             ent = {"steps": steps, "tvals": tvals, "table": table, "film_width": int(self.L.ns2vc_unet_film_width(self.h)),
@@ -387,17 +386,10 @@ class DenoiserSession:
         ent = self._chains.get(key)
         if ent is None:
             steps = make_steps()
-            if kind == "ddpm":
-                arr = (_lib.DdpmCoef * len(steps))(*[_lib.DdpmCoef(s.c_x0, s.c_x, s.c_noise, int(s.add_noise)) for s in steps])
-                draws = tuple(s.add_noise for s in steps)
-            else:
-                arr = (_lib.DdimCoef * len(steps))(*[_lib.DdimCoef(s.sqrt_recip, s.sqrt_recipm1, s.sqrt_alpha_next, s.c, s.sigma,
-                                                                   int(s.last)) for s in steps])
-                draws = tuple(not s.last for s in steps)
-            ent = {"n": len(steps), "draws": draws, "csize": C.sizeof(arr) // len(steps),
-                   "coef": torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev),
-                   "tvals": torch.tensor([[s.t_input] * self.B for s in steps], dtype=torch.float32).reshape(-1).to(self.dev),
-                   "runs": 0}
+            draws = tuple(s.add_noise for s in steps) if kind == "ddpm" else tuple(not s.last for s in steps)
+            coef, csize = coefs.c_table(steps, self.dev)
+            ent = {"n": len(steps), "draws": draws, "csize": csize, "coef": coef,
+                   "tvals": coefs.t_inputs(steps, self.B, self.dev).reshape(-1), "runs": 0}
             self._chains[key] = ent
             while len(self._chains) > self.MAX_GRAPHS:
                 self._chains.popitem(last=False)

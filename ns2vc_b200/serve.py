@@ -30,7 +30,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 import torch.distributed as dist
 
-from . import _lib, convert, shard
+from . import _lib, coefs, convert, shard
 from .api import default_schedule
 from .convert import HOP, LATENT_CH
 from .fused import DenoiserSession, _step_table, schedule_signature
@@ -389,13 +389,8 @@ class ConversionServer:
         ts = torch.linspace(ns.T, 1.0 / ns.total_N, self.steps + 1)
         extra = True if self.kind == "dpm" else "bh2"       # lower_order_final / variant, as sample_latents runs them
         steps = _step_table(self.kind, ns, ts, extra, (self.kind, tuple(float(v) for v in ts), extra, schedule_signature(ns)))
-        if self.kind == "dpm":
-            arr = (_lib.DpmCoef * len(steps))(*[_lib.DpmCoef(s.alpha_s, s.sigma_s, s.c_x, s.c_m, s.c_d, s.inv_r0, s.order) for s in steps])
-        else:
-            arr = (_lib.UniPcCoef * len(steps))(*[_lib.UniPcCoef(s.alpha_t, s.sigma_t, s.c_x, s.c_m, s.ab, s.rk, s.rho0, s.rho1,
-                                                                 s.corr_order, s.n_c_x, s.n_c_m, s.nab, s.nrk, s.pred_order) for s in steps])
-        self._coef = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
-        self._tvals = torch.tensor([[s.t_input] * B for s in steps], dtype=torch.float32).to(dev)
+        self._coef, _ = coefs.c_table(steps, dev)
+        self._tvals = coefs.t_inputs(steps, B, dev)
         L, h = self._L, sess.h
         self._fw = int(L.ns2vc_unet_film_width(h))
         self._film_table = torch.empty(int(L.ns2vc_unet_time_table_floats(h, self.steps * B)), **f32)

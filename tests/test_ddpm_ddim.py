@@ -198,8 +198,7 @@ def test_step_kernels_bit_exact():
     dbuf = {k: v.cuda() for k, v in buf.items()}
     for t in (999, 500, 1, 0):
         st = coefs.ddpm_table(buf, [t])[0]
-        c = _lib.DdpmCoef(st.c_x0, st.c_x, st.c_noise, int(st.add_noise))
-        cdev = torch.frombuffer(bytearray(bytes(c)), dtype=torch.uint8).cuda()
+        cdev, _ = coefs.c_table([st], "cuda")
         out = torch.full_like(x, float("nan"))
         _lib.check(L.ns2vc_ddpm_step(x.data_ptr(), x0.data_ptr(), nz.data_ptr(), cdev.data_ptr(), out.data_ptr(), x.numel(), None, None))
         inplace = x.clone()
@@ -214,8 +213,7 @@ def test_step_kernels_bit_exact():
     for S, eta in ((6, 0.0), (10, 0.5), (1000, 0.5)):
         tab = coefs.ddim_table(buf, 1000, S, eta)
         for st in (tab[0], tab[len(tab) // 2], tab[-2], tab[-1]):
-            c = _lib.DdimCoef(st.sqrt_recip, st.sqrt_recipm1, st.sqrt_alpha_next, st.c, st.sigma, int(st.last))
-            cdev = torch.frombuffer(bytearray(bytes(c)), dtype=torch.uint8).cuda()
+            cdev, _ = coefs.c_table([st], "cuda")
             out = torch.full_like(x, float("nan"))
             _lib.check(L.ns2vc_ddim_step(x.data_ptr(), x0.data_ptr(), nz.data_ptr(), cdev.data_ptr(), out.data_ptr(), x.numel(), None, None))
             bt = torch.full((3,), st.time, dtype=torch.long, device="cuda")

@@ -1,10 +1,13 @@
 """Drop-in sampler classes (generic Python path) against fixtures produced by the reference's own
-DPM_Solver / UniPC classes; and the host-side coefficient tables of the fused CUDA sampler against
-the same classes through a Python emulation of the fused kernels' arithmetic.  CPU only."""
+DPM_Solver / UniPC classes; the host-side coefficient tables of the fused CUDA sampler against
+the same classes through a Python emulation of the fused kernels' arithmetic; and the C-ABI structs
+built from those tables.  CPU only."""
+import ctypes as C
+
 import pytest
 import torch
 
-from ns2vc_b200 import coefs
+from ns2vc_b200 import _lib, coefs
 from ns2vc_b200 import dpm_solver as our_dpm
 from ns2vc_b200 import uni_pc as our_upc
 from ns2vc_b200.schedule import NoiseScheduleVP, interpolate_fn
@@ -89,7 +92,7 @@ def test_unipc_matches_reference(gold):
     assert kept >= 2 and kept + rejected == 18, (kept, rejected)
 
 
-# ---- Python emulation of the fused kernels (kernels_misc.cu dpm_step_kernel / unipc_step_kernel) ----
+# ---- Python emulation of the fused kernels (sampler.cu dpm_step_kernel / unipc_step_kernel) ----
 def _rt(x, o, a, s):
     noise = (x - a * o) / s
     return (x - s * noise) / a
@@ -154,3 +157,32 @@ def test_unipc_coef_table_bit_exact(steps, variant):
     fn = our_upc.model_wrapper(toy, ns, model_type="x_start")
     ref = our_upc.UniPC(fn, ns, variant=variant).sample(xT, steps=steps, order=2, skip_type="time_uniform", method="multistep")
     assert torch.equal(_emulate_unipc(table, xT, 1), ref)
+
+
+# ---- the C-ABI structs of the step records ----
+def _positional(st):
+    """The struct of a step record with its fields written out in the order of include/ns2vc_b200.h."""
+    if isinstance(st, coefs.DpmStep):
+        return _lib.DpmCoef(st.alpha_s, st.sigma_s, st.c_x, st.c_m, st.c_d, st.inv_r0, st.order)
+    if isinstance(st, coefs.UniPcStep):
+        return _lib.UniPcCoef(st.alpha_t, st.sigma_t, st.c_x, st.c_m, st.ab, st.rk, st.rho0, st.rho1, st.corr_order,
+                              st.n_c_x, st.n_c_m, st.nab, st.nrk, st.pred_order)
+    if isinstance(st, coefs.DdpmStep):
+        return _lib.DdpmCoef(st.c_x0, st.c_x, st.c_noise, int(st.add_noise))
+    return _lib.DdimCoef(st.sqrt_recip, st.sqrt_recipm1, st.sqrt_alpha_next, st.c, st.sigma, int(st.last))
+
+
+def test_c_structs_fill_every_field_by_name():
+    ns = NoiseScheduleVP("discrete", betas=linear_betas(1000))
+    buf = coefs.diffusion_buffers(1000)
+    tables = []
+    for steps in (6, 20):                      # lower-order final steps at 6, none at 20
+        ts = torch.linspace(1.0, 1e-3, steps + 1)
+        tables += [coefs.dpmpp_2m_table(ns, ts), coefs.unipc_bh2_table(ns, ts)]
+    tables += [coefs.ddpm_table(buf, range(999, -1, -1)), coefs.ddpm_table(buf, range(999, -1, -111))]
+    tables += [coefs.ddim_table(buf, 1000, 6, 0.0), coefs.ddim_table(buf, 1000, 50, 0.5)]
+    for tab in tables:
+        want = [bytes(_positional(s)) for s in tab]
+        assert [bytes(coefs.c_struct(s)) for s in tab] == want, type(tab[0]).__name__
+        table, size = coefs.c_table(tab, "cpu")
+        assert size == len(want[0]) and table.numpy().tobytes() == b"".join(want)

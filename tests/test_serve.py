@@ -111,15 +111,6 @@ def chain():
     return (cv, pre, unet, voc), wavs, prompt, xs
 
 
-def _coef_array(kind, steps):
-    if kind == "dpm":
-        arr = (_lib.DpmCoef * len(steps))(*[_lib.DpmCoef(s.alpha_s, s.sigma_s, s.c_x, s.c_m, s.c_d, s.inv_r0, s.order) for s in steps])
-    else:
-        arr = (_lib.UniPcCoef * len(steps))(*[_lib.UniPcCoef(s.alpha_t, s.sigma_t, s.c_x, s.c_m, s.ab, s.rk, s.rho0, s.rho1, s.corr_order,
-                                                             s.n_c_x, s.n_c_m, s.nab, s.nrk, s.pred_order) for s in steps])
-    return arr, torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to("cuda")
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", ["dpm", "unipc"])
 def test_row_steps_equal_the_scalar_steps_bit_for_bit(kind):
@@ -127,7 +118,7 @@ def test_row_steps_equal_the_scalar_steps_bit_for_bit(kind):
     ns = api.default_schedule()
     ts = torch.linspace(ns.T, 1.0 / ns.total_N, STEPS + 1)
     steps = coefs.dpmpp_2m_table(ns, ts, True) if kind == "dpm" else coefs.unipc_bh2_table(ns, ts, "bh2")
-    arr, dev_coef = _coef_array(kind, steps)
+    dev_coef, _ = coefs.c_table(steps, "cuda")
     ks = [0, 3, STEPS - 1, -1]                 # first step, a middle step, the lower-order final step, an empty row
     B, Cl, T = len(ks), 100, 97
     n = Cl * T
@@ -159,7 +150,7 @@ def test_row_steps_equal_the_scalar_steps_bit_for_bit(kind):
                 assert torch.count_nonzero(outs[name][b]) == 0, f"empty row: {name} is not exactly 0"
             continue
         ref = {name: torch.full((Cl, T), 7.0, device="cuda") for name in outs_names}
-        c = arr[kb]
+        c = coefs.c_struct(steps[kb])
         if kind == "dpm":
             _lib.check(L.ns2vc_dpm_step(ins["x"][b].data_ptr(), ins["o"][b].data_ptr(), ins["mp"][b].data_ptr(), C.byref(c),
                                         ref["mc"].data_ptr(), ref["xn"].data_ptr(), n, None, None))
