@@ -607,6 +607,36 @@ typedef struct ns2vc_check_cv_pos_conv_args {
 } ns2vc_check_cv_pos_conv_args;
 int ns2vc_check_cv_pos_conv(const ns2vc_check_cv_pos_conv_args* args, char* desc, int desc_len, ns2vc_stream stream);
 
+/* The denoiser's Downsample1D (conv k3 s2 p1 + bias) of x [B, Tin, C] as the engine launches it: one GEMM over row-pair views of
+ * the raw split (in_hi / in_lo [B, Tin, ld], ld a multiple of 8 >= C), or (force_prep, or Tin = 1) two prep launches decimating
+ * the fp32 x into dense even / odd splits first.  w [C, C, 3] is packed as the engine packs it.  Outputs [B, ceil(Tin / 2), C]:
+ * fp32 `out` and / or the split out_hi / out_lo (row pitch pad_to(C, 8)); ragged: level-0 lengths row_len [B] (int32) and the
+ * output level len_shift >= 1 (rows past each entry's own length are zeros), or NULL. */
+typedef struct ns2vc_check_down_conv_args {
+  int B, Tin, C;
+  const float* x;
+  const void* in_hi; const void* in_lo; int ld;
+  const float* w; const float* bias;
+  const int* row_len; int len_shift;
+  float* out;
+  void* out_hi; void* out_lo;
+  int force_prep;
+} ns2vc_check_down_conv_args;
+int ns2vc_check_down_conv(const ns2vc_check_down_conv_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
+/* The content encoder's conv l (1 .. 6: k 3, or 2 for l >= 5; stride 2, no bias) + GELU as the engine launches it: one GEMM over
+ * the row-pair view of the previous level's split in_hi / in_lo [B, rows_in, C0] (rows_in even), the row mask keep [B, rows_out],
+ * into the split out_hi / out_lo or the fp32 out ([B, rows_out, C0], exactly one of them).  w [C0, C0, k] is packed as the
+ * engine packs it; C0 a multiple of 128 up to 1024. */
+typedef struct ns2vc_check_cv_conv_args {
+  int B, rows_in, rows_out, C0, l;
+  const void* in_hi; const void* in_lo;
+  const float* w; const float* keep;
+  float* out;
+  void* out_hi; void* out_lo;
+} ns2vc_check_cv_conv_args;
+int ns2vc_check_cv_conv(const ns2vc_check_cv_conv_args* args, char* desc, int desc_len, ns2vc_stream stream);
+
 /* The vocoder's ISTFT of a head output h [B, T, ld] (log-magnitudes, then phases; ld >= n_fft + 2) with window [n_fft] and
  * hop n_fft / 4 into audio [B, T * hop]; len int64 [B] (clamped into [1, T]) or NULL.  The twiddles are the engine's. */
 typedef struct ns2vc_check_istft_args {

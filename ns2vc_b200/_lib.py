@@ -190,6 +190,8 @@ SIGNATURES = {
     "ns2vc_check_nct_split": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_cv_conv0": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_cv_pos_conv": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
+    "ns2vc_check_down_conv": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
+    "ns2vc_check_cv_conv": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_istft": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
 }
 

@@ -285,6 +285,36 @@ int launch_cv_add(const CvAddOp& o, cudaStream_t st) {
                                reinterpret_cast<const float4*>(o.x), o.n4), "cv_add");
 }
 
+int cv_conv_taps(int l) { return conv_k(l); }
+
+// Conv l's weights (w: [C0, C0, k]) into pb (Npad C0, k nkb(C0) k-blocks): tap j at k-block j nkb(C0), so that taps 0, 1 are
+// one row pair's channels in order
+int pack_cv_conv(PackedB& pb, const float* w, int C0, int l, cudaStream_t st) {
+  for (int j = 0; j < conv_k(l); ++j) {
+    const int rc = pack_seg(pb, w, C0, C0, conv_k(l), j, 0, C0, 0, j * nkb_of(C0), 0, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// Conv l (1 .. 6: k 3 or 2, stride 2, no bias) + GELU over level l - 1's split `in` [B, rows_in, C0] (ld C0; rows_in even, so
+// that no pair straddles two entries) seen as row pairs [B, rows_in / 2, 2 C0]: output row t reads pair t (taps 0, 1) and, for
+// k = 3, the next pair's first row (tap 2).  Rows whose factor in keep [B, rows_out] is 0 are stored as zeros; the output is
+// the split `out_split` [B, rows_out, C0] (hi non-null) or fp32 `out` [B, rows_out, C0].
+GemmOp cv_conv_gemm(ProgramBuilder& bld, const PackedB& w, const SplitBuf& in, int rows_in, int rows_out, int l, const float* keep,
+                    const SplitBuf& out_split, float* out) {
+  const SplitBuf pairs = ProgramBuilder::view(in, rows_in / 2, 2 * in.C);
+  const int C0 = in.C;
+  GemmOp g = bld.gemm_base(w, rows_out);
+  const int src = bld.add_src(g, pairs);
+  bld.seg(g, src, 0, 2 * C0, 0);                             // taps 0, 1: the pair itself
+  if (conv_k(l) == 3) bld.seg(g, src, 0, C0, 1);             // tap 2: the next pair's first row
+  g.flags = EPI_GELU | EPI_ROWMASK; g.rowmask = keep;
+  if (out_split.hi) { g.flags |= EPI_OUT_SPLIT; g.out_hi = out_split.hi; g.out_lo = out_split.lo; g.out_split_ld = out_split.ld; }
+  else { g.flags |= EPI_OUT_F32; g.out = out; g.out_ld = C0; }
+  return g;
+}
+
 // Group g's weights of the folded positional conv (wg: [gw, gw, K]) into pb (Npad 128, K k-blocks): k-block j = tap j
 int pack_cv_pos_group(PackedB& pb, const float* wg, int gw, int K, cudaStream_t st) {
   for (int j = 0; j < K; ++j) {
@@ -370,8 +400,7 @@ int pack_with(ns2vc_cv* h, cudaStream_t st, float* scratch) {
   for (int l = 1; l < kLevels; ++l) {
     PackedB& pb = h->conv[l];
     if ((rc = mem.alloc_packed(pb, C0, C0, conv_k(l) * nkb_of(C0), false))) return rc;
-    for (int j = 0; j < conv_k(l); ++j)
-      if ((rc = pack_seg(pb, w.W(conv_key(l) + ".0.weight"), C0, C0, conv_k(l), j, 0, C0, 0, j * nkb_of(C0), 0, st))) return rc;
+    if ((rc = pack_cv_conv(pb, w.W(conv_key(l) + ".0.weight"), C0, l, st))) return rc;
   }
   if ((rc = pack_lin(mem, h->proj, w.W("post_extract_proj.weight"), D, C0, st))) return rc;
   {
@@ -475,17 +504,9 @@ int build_program(ns2vc_cv* h, int B, int N, void* ws, size_t* bytes_out) {
   bld.emit(Launch::CV_CONV0, CvConv0Op{B, N, rows[0], w0, gn, w.W(conv_key(0) + ".2.weight"), w.W(conv_key(0) + ".2.bias"), lv_even});
   tap_split_of(conv_key(0), lv_even, rows[0], Tl[0]);
   for (int l = 1; l < kLevels; ++l) {
-    SplitBuf in = (l & 1) ? lv_even : lv_odd;                // level l - 1
-    in = ProgramBuilder::view(in, rows[l - 1] / 2, 2 * C0);  // row pairs [B, rows / 2, 2 C0]
+    const SplitBuf in = (l & 1) ? lv_even : lv_odd;          // level l - 1
     const SplitBuf out = ProgramBuilder::view((l & 1) ? lv_odd : lv_even, rows[l], C0);
-    GemmOp g = bld.gemm_base(h->conv[l], rows[l]);
-    const int src = bld.add_src(g, in);
-    bld.seg(g, src, 0, 2 * C0, 0);                           // taps 0, 1: the pair itself
-    if (conv_k(l) == 3) bld.seg(g, src, 0, C0, 1);           // tap 2: the next pair's first row
-    g.flags = EPI_GELU;
-    rowmask(g, l);
-    if (l + 1 < kLevels) { g.flags |= EPI_OUT_SPLIT; g.out_hi = out.hi; g.out_lo = out.lo; g.out_split_ld = out.ld; }
-    else { g.flags |= EPI_OUT_F32; g.out = H6; g.out_ld = C0; }
+    GemmOp g = cv_conv_gemm(bld, h->conv[l], in, rows[l - 1], rows[l], l, lt.keep[l], l + 1 < kLevels ? out : SplitBuf{}, H6);
     bld.emit_gemm(g, h->conv[l]);
     if (l + 1 < kLevels) tap_split_of(conv_key(l), out, rows[l], Tl[l]);
     else tap_f32(conv_key(l), H6, C0);

@@ -111,6 +111,46 @@ struct ns2vc_unet : EngineBase {
   std::vector<ProfRec> prof;
 };
 
+namespace ns2vc {
+
+// A resampler's (Downsample1D's, Upsample1D's) conv weights [C, C, 3]: tap j at k-block j nkb(C)
+int pack_resample_conv(PackedB& pb, const float* w, int C, cudaStream_t st) {
+  for (int j = 0; j < 3; ++j) {
+    const int rc = pack_seg(pb, w, C, C, 3, j, 0, C, 0, j * nkb_of(C), 0, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+DownConv down_conv(ProgramBuilder& bld, const PackedB& w, const float* bias, const float* x, const SplitBuf& raw, int Tin, int C,
+                   bool views, const SplitBuf& e_buf, const SplitBuf& o_buf) {
+  const int TL = (Tin - 1) / 2 + 1, To = Tin / 2;          // even rows, odd rows
+  DownConv d;
+  memset(&d, 0, sizeof(d));
+  SplitBuf ev = e_buf, od = o_buf;
+  if (views && To >= 1) {
+    // the raw split seen as row PAIRS [B, ceil(Tin/2), 2*ld]: even rows are the first half of a pair, odd rows the second
+    // (one row fewer when Tin is odd: rows past it are the TMA unit's zero fill).  The entries stay Tin rows apart.
+    ev = raw; ev.T = TL; ev.ld = 2 * raw.ld; ev.bpitch = (long long)Tin * raw.ld;
+    od = ev; od.hi += raw.ld; od.lo += raw.ld; od.T = To;
+  } else {
+    // E[t] = x[2t], O[t] = x[2t+1] decimated into dense splits (Tin = 1: O is one row of zeros past the input)
+    for (int j = 0; j < 2; ++j) {
+      PrepOp& p = d.prep[j];
+      p.src1 = x; p.ld1 = C; p.C1 = C; p.B = bld.B; p.T_src = Tin; p.T_dst = j ? std::max(To, 1) : TL;
+      p.row_mul = 2; p.row_add = j; p.mode = PREP_RAW; p.out = j ? od : ev;
+    }
+    d.nprep = 2;
+  }
+  d.g = bld.gemm_base(w, TL);
+  const int ie = bld.add_src(d.g, ev), io = bld.add_src(d.g, od);
+  bld.seg(d.g, io, 0, C, -1); bld.seg(d.g, ie, 0, C, 0); bld.seg(d.g, io, 0, C, 0);
+  d.g.flags = EPI_BIAS; d.g.bias = bias;
+  return d;
+}
+
+}  // namespace ns2vc
+
 namespace {
 
 int level_len(int T, int level) {
@@ -352,10 +392,10 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       h->xformers.push_back(x);
     } else if (o.kind == PlanOp::DOWN || o.kind == PlanOp::UP) {
       ConvSite s; s.p = o.prefix; s.c = o.cout;
-      const int nk = nkb_of(s.c);
-      if ((rc = h->mem.alloc_packed(s.w, s.c, s.c, 3 * nk, h->simt))) return rc;
-      for (int j = 0; j < 3; ++j)
-        if ((rc = pack_named(h, s.w, s.p + ".conv.weight", s.c, s.c, 3, j, 0, s.c, 0, j * nk, 0, st))) return rc;
+      const float* w = h->weights.W(s.p + ".conv.weight");
+      NS_REQUIRE(w != nullptr, "pack: weight %s missing", (s.p + ".conv.weight").c_str());
+      if ((rc = h->mem.alloc_packed(s.w, s.c, s.c, 3 * nkb_of(s.c), h->simt))) return rc;
+      if ((rc = pack_resample_conv(s.w, w, s.c, st))) return rc;
       o.site = (int)h->resamplers.size();
       h->resamplers.push_back(s);
     }
@@ -782,27 +822,15 @@ struct Builder : ProgramBuilder {
       emit_block_out(g, x.ff2p, o.level, C, o.skip, x.p); }
   }
 
-  // Downsample1D: conv k3 s2 p1:  out[t] = W0 x[2t-1] + W1 x[2t] + W2 x[2t+1] = W0 O[t-1] + W1 E[t] + W2 O[t]
-  // with E[t] = x[2t], O[t] = x[2t+1] decimated by the prep kernel (unit-stride TMA windows).
+  // Downsample1D: conv k3 s2 p1 (down_conv): in panel mode over row-pair views of the block input's raw split, else (and at
+  // Tin = 1) over its even and odd rows decimated by two prep launches.
   void emit_down(const PlanOp& o) {
     const ConvSite& s = h->resamplers[o.site];
     const int TL = Tl[o.level], Tin = Tl[o.level - 1];
-    const int To = Tin / 2;                                  // odd-row count
-    SplitBuf ev = view(sc.SP_A, TL, s.c), od = view(sc.SP_R, std::max(To, 1), s.c);
-    if (xf_on && To >= 1) {
-      // no copy at all: the raw split of the block input seen as row PAIRS [B, ceil(Tin/2), 2*ld] - even rows are the first
-      // half of a pair, odd rows the second (one row fewer when Tin is odd: rows past it are the TMA unit's zero fill)
-      ev = cur.sp; ev.T = TL; ev.ld = 2 * cur.sp.ld; ev.bpitch = (long long)Tin * cur.sp.ld;
-      od = ev; od.hi += cur.sp.ld; od.lo += cur.sp.ld; od.T = To;
-    } else {
-      emit_prep(cur.p, s.c, nullptr, 0, Tin, TL, PREP_RAW, nullptr, nullptr, ev, nullptr, 2, 0);
-      emit_prep(cur.p, s.c, nullptr, 0, Tin, std::max(To, 1), PREP_RAW, nullptr, nullptr, od, nullptr, 2, 1);
-    }
-    GemmOp g = gemm_base(s.w, TL);
-    const int ie = add_src(g, ev), io = add_src(g, od);
-    seg(g, io, 0, s.c, -1); seg(g, ie, 0, s.c, 0); seg(g, io, 0, s.c, 0);
-    g.flags = EPI_BIAS; g.bias = h->weights.W(s.p + ".conv.bias");
-    emit_block_out(g, s.w, o.level, s.c, o.skip, s.p);
+    DownConv d = down_conv(*this, s.w, h->weights.W(s.p + ".conv.bias"), cur.p, cur.sp, Tin, s.c, xf_on, view(sc.SP_A, TL, s.c),
+                           view(sc.SP_R, std::max(Tin / 2, 1), s.c));
+    for (int i = 0; i < d.nprep; ++i) emit(Launch::PREP, d.prep[i]);
+    emit_block_out(d.g, s.w, o.level, s.c, o.skip, s.p);
   }
 
   // Upsample1D: nearest-neighbour 2x (to the finer level's length), then conv k3 p1

@@ -347,13 +347,29 @@ inline void set_group_norm(PrepOp& p, int B, const double* st1, int C1, const do
   p.gn.inv_n = 1.0 / ((double)Tn * ((C1 + C2) / G));
 }
 
+// The denoiser's Downsample1D (engine.cu), shared by its emit_down and the kernel checks: conv k3 s2 p1 of a [B, Tin, C] input
+// as one GEMM over its even rows E[t] = x[2t] and odd rows O[t] = x[2t+1] (bias included; the caller adds the outputs):
+//   out[t] = W0 O[t-1] + W1 E[t] + W2 O[t],   t < ceil(Tin / 2)
+// With `views` and Tin >= 2, E and O are views of the raw split `raw` [B, Tin, raw.ld] as row pairs (no copy, nprep = 0);
+// otherwise the two prep launches prep[0..1] decimate the fp32 input x [B, Tin, C] into e_buf / o_buf first.  The weights are
+// [C, C, 3] packed by pack_resample_conv (which packs Upsample1D's conv too).
+struct DownConv { GemmOp g; PrepOp prep[2]; int nprep; };
+int pack_resample_conv(PackedB& pb, const float* w, int C, cudaStream_t st);
+DownConv down_conv(ProgramBuilder& bld, const PackedB& w, const float* bias, const float* x, const SplitBuf& raw, int Tin, int C,
+                   bool views, const SplitBuf& e_buf, const SplitBuf& o_buf);
+
 // The content encoder's launchers (content.cu), shared by its run_program and the kernel checks.  conv 0's two launches read the
-// call's waveform (batch stride bstride) and lengths; the positional conv is the windows, one GEMM per group
-// (cv_pos_group_gemm over the weights pack_cv_pos_group packs), then the residual add.
+// call's waveform (batch stride bstride) and lengths; convs 1-6 are one GEMM each (cv_conv_gemm over the weights pack_cv_conv
+// packs); the positional conv is the windows, one GEMM per group (cv_pos_group_gemm over the weights pack_cv_pos_group packs),
+// then the residual add.
 int launch_cv_gn_stats(const CvGnStatsOp& o, const float* wav, long long bstride, const long long* lengths, cudaStream_t st);
 int launch_cv_conv0(const CvConv0Op& o, const float* wav, long long bstride, const long long* lengths, cudaStream_t st);
 int launch_cv_pos_windows(const CvPosWinOp& o, cudaStream_t st);
 int launch_cv_add(const CvAddOp& o, cudaStream_t st);
+int cv_conv_taps(int l);
+int pack_cv_conv(PackedB& pb, const float* w, int C0, int l, cudaStream_t st);
+GemmOp cv_conv_gemm(ProgramBuilder& bld, const PackedB& w, const SplitBuf& in, int rows_in, int rows_out, int l, const float* keep,
+                    const SplitBuf& out_split, float* out);
 int pack_cv_pos_group(PackedB& pb, const float* wg, int gw, int K, cudaStream_t st);
 GemmOp cv_pos_group_gemm(ProgramBuilder& bld, const PackedB& w, const SplitBuf& win, int G, int g, int gw, int T, int K, const float* bias,
                          const float* keep, float* out, int out_ld);

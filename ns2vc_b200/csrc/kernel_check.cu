@@ -1,10 +1,12 @@
 // Test-only entry points into the product launchers: one weight packing, one wgmma GEMM, one flash attention, one activation
 // prep, one LayerNorm, one small linear, the AttentionPooling pieces, one [B, C, T] -> split conversion, the content encoder's
-// first conv and positional conv, and the vocoder's ISTFT, each described by a flat C struct (include/ns2vc_b200.h, "kernel
-// checks") and run through exactly the host code the engines use (pack_seg, the ProgramBuilder helpers, set_group_norm,
-// linear_op, plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention dispatch, the launchers of common.cuh
-// and engine_host.cuh).  tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py and tests/test_audio_kernels_fp64.py drive
-// them at the shapes and edges the models never reach.  Nothing here is a kernel: every launch is the product's own.
+// first conv, strided convs 1-6 and positional conv, the denoiser's Downsample1D conv, and the vocoder's ISTFT, each described
+// by a flat C struct (include/ns2vc_b200.h, "kernel checks") and run through exactly the host code the engines use (pack_seg,
+// the ProgramBuilder helpers, set_group_norm, linear_op, down_conv / pack_resample_conv, cv_conv_gemm / pack_cv_conv,
+// plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention dispatch, the launchers of common.cuh and
+// engine_host.cuh).  tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py, tests/test_audio_kernels_fp64.py and
+// tests/test_strided_conv_fp64.py drive them at the shapes and edges the models never reach.  Nothing here is a kernel: every
+// launch is the product's own.
 #include "engine_host.cuh"
 #include "../../include/ns2vc_b200.h"
 
@@ -332,6 +334,82 @@ int ns2vc_check_cv_pos_conv(const ns2vc_check_cv_pos_conv_args* a, char* desc, i
   if (rc) return rc;
   if ((rc = launch_cv_add(CvAddOp{a->out, a->x, (long long)a->B * a->T * a->D / 4}, st))) return rc;
   report(desc, desc_len, "cv_pos_windows+%dxgemm_tc<%d,LNF=0,XF=0,ENC=0,RAG=0,VOC=1>+cv_add", a->G, bn);
+  return 0;
+}
+
+int ns2vc_check_down_conv(const ns2vc_check_down_conv_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->x && a->in_hi && a->in_lo && a->w && a->bias, "check_down_conv: null argument");
+  NS_REQUIRE(a->B >= 1 && a->B <= 65535 && a->Tin >= 1 && a->C >= 1, "check_down_conv: bad sizes B=%d Tin=%d C=%d", a->B, a->Tin, a->C);
+  NS_REQUIRE(a->ld >= a->C && a->ld % 8 == 0, "check_down_conv: input ld=%d (a multiple of 8, at least C=%d)", a->ld, a->C);
+  NS_REQUIRE(a->out || (a->out_hi && a->out_lo), "check_down_conv: no output");
+  NS_REQUIRE(!a->row_len || a->len_shift >= 1, "check_down_conv: ragged output level %d (at least 1)", a->len_shift);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int C = a->C, Cp = pad_to(C, 8), TL = (a->Tin - 1) / 2 + 1, To = std::max(a->Tin / 2, 1);
+  PackedB pb;
+  pb.Npad = pad_to(C, 128); pb.nkb = 3 * nkb_of(C); pb.n_logical = C;
+  const size_t welems = (size_t)pb.nkb * pb.Npad * 64;
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&pb.hi, welems * sizeof(__nv_bfloat16), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&pb.lo, welems * sizeof(__nv_bfloat16), st));
+  // the prep path's dense even / odd splits (allocated either way: the views do not touch them)
+  SplitBuf e{}, o{};
+  e.T = TL; o.T = To; e.C = o.C = C; e.ld = o.ld = Cp;
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&e.hi, (size_t)a->B * TL * Cp * sizeof(__nv_bfloat16), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&e.lo, (size_t)a->B * TL * Cp * sizeof(__nv_bfloat16), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&o.hi, (size_t)a->B * To * Cp * sizeof(__nv_bfloat16), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&o.lo, (size_t)a->B * To * Cp * sizeof(__nv_bfloat16), st));
+  int rc = 0;
+  if (cudaMemsetAsync(pb.hi, 0, welems * sizeof(__nv_bfloat16), st) != cudaSuccess || cudaMemsetAsync(pb.lo, 0, welems * sizeof(__nv_bfloat16), st) != cudaSuccess) {
+    set_error("check_down_conv: memset failed");
+    rc = -2;
+  }
+  if (!rc) rc = pack_resample_conv(pb, a->w, C, st);
+  ProgramBuilder bld{Arena{}, a->B, false, false, nullptr};
+  const SplitBuf raw{(__nv_bfloat16*)a->in_hi, (__nv_bfloat16*)a->in_lo, a->Tin, C, a->ld, 0};
+  DownConv d = down_conv(bld, pb, a->bias, a->x, raw, a->Tin, C, !a->force_prep, e, o);
+  for (int i = 0; i < d.nprep && !rc; ++i) rc = launch_prep_split(d.prep[i], st);
+  GemmOp& g = d.g;
+  if (a->out) { g.flags |= EPI_OUT_F32; g.out = a->out; g.out_ld = C; }
+  if (a->out_hi) { g.flags |= EPI_OUT_SPLIT; g.out_hi = (__nv_bfloat16*)a->out_hi; g.out_lo = (__nv_bfloat16*)a->out_lo; g.out_split_ld = Cp; }
+  g.row_len = a->row_len; g.len_shift = a->len_shift;
+  if (!rc) {
+    plan_gemm(g);
+    if (!(rc = encode_tmaps(g))) rc = launch_gemm_tc(g, st);
+  }
+  for (void* p : {(void*)pb.hi, (void*)pb.lo, (void*)e.hi, (void*)e.lo, (void*)o.hi, (void*)o.lo}) NS_CHECK_CUDA(cudaFreeAsync(p, st));
+  if (rc) return rc;
+  report(desc, desc_len, "%sgemm_tc<%d,LNF=0,XF=0,ENC=0,RAG=%d,VOC=0>", d.nprep ? "2xprep_split<RAG=0>+" : "", g.bn, g.row_len ? 1 : 0);
+  return 0;
+}
+
+int ns2vc_check_cv_conv(const ns2vc_check_cv_conv_args* a, char* desc, int desc_len, ns2vc_stream stream) {
+  NS_REQUIRE(a && a->in_hi && a->in_lo && a->w && a->keep, "check_cv_conv: null argument");
+  NS_REQUIRE(a->l >= 1 && a->l <= 6, "check_cv_conv: conv index %d (1 .. 6)", a->l);
+  NS_REQUIRE(a->C0 >= 128 && a->C0 <= 1024 && a->C0 % 128 == 0, "check_cv_conv: C0=%d (a multiple of 128 up to 1024)", a->C0);
+  NS_REQUIRE(a->B >= 1 && a->B <= 65535 && a->rows_in >= 2 && a->rows_out >= 1, "check_cv_conv: bad sizes B=%d rows_in=%d rows_out=%d", a->B,
+             a->rows_in, a->rows_out);
+  NS_REQUIRE(a->rows_in % 2 == 0, "check_cv_conv: rows_in=%d is odd (a row pair would straddle two entries)", a->rows_in);
+  NS_REQUIRE((a->out != nullptr) != (a->out_hi != nullptr) && (a->out_hi != nullptr) == (a->out_lo != nullptr),
+             "check_cv_conv: exactly one output, fp32 or split");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int C0 = a->C0;
+  PackedB pb;
+  pb.Npad = C0; pb.nkb = cv_conv_taps(a->l) * nkb_of(C0); pb.n_logical = C0;
+  const size_t welems = (size_t)pb.nkb * pb.Npad * 64;
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&pb.hi, welems * sizeof(__nv_bfloat16), st));
+  NS_CHECK_CUDA(cudaMallocAsync((void**)&pb.lo, welems * sizeof(__nv_bfloat16), st));
+  int rc = pack_cv_conv(pb, a->w, C0, a->l, st);
+  ProgramBuilder bld{Arena{}, a->B, false, false, nullptr};
+  const SplitBuf in{(__nv_bfloat16*)a->in_hi, (__nv_bfloat16*)a->in_lo, a->rows_in, C0, C0, 0};
+  const SplitBuf out{(__nv_bfloat16*)a->out_hi, (__nv_bfloat16*)a->out_lo, a->rows_out, C0, C0, 0};
+  GemmOp g = cv_conv_gemm(bld, pb, in, a->rows_in, a->rows_out, a->l, a->keep, out, a->out);
+  if (!rc) {
+    plan_gemm(g);
+    if (!(rc = encode_tmaps(g))) rc = launch_gemm_tc(g, st);
+  }
+  NS_CHECK_CUDA(cudaFreeAsync(pb.hi, st));
+  NS_CHECK_CUDA(cudaFreeAsync(pb.lo, st));
+  if (rc) return rc;
+  report(desc, desc_len, "gemm_tc<%d,LNF=0,XF=0,ENC=0,RAG=0,VOC=1>", g.bn);
   return 0;
 }
 
