@@ -173,6 +173,32 @@ int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float*
                           const ns2vc_unipc_coef* coefs, int* k, float* m_t, float* x_t, float* x_pred, size_t row_n, int B,
                           int* nan_flags, ns2vc_stream stream);
 
+/* One row step for rows of either method: row b of a [B, row_n] batch takes step k[b] of its own schedule.
+ *   method [B] int32 device: NS2VC_ROW_DPM (DPM-Solver++) or NS2VC_ROW_UNIPC (UniPC-bh2); read only for occupied rows.
+ *   base [B] int32 device: where row b's schedule starts in its method's table, so row b's struct is
+ *     dpm_coefs[base[b] + k[b]] or unipc_coefs[base[b] + k[b]].  Each table holds the structs of every schedule of that method
+ *     in use, back to back; a table no occupied row selects may be NULL.
+ *   k [B] int32 device: each row's step within its schedule, or -1 for an empty row; each occupied k[b] is advanced by one.
+ *   nan_flags [B] int32 device (may be NULL): entry b is set to 1 when row b's x_in holds a NaN.
+ * Both methods use one buffer layout, so the rotation after the step is the same four copies for every row:
+ *   plane     DPM-Solver++   UniPC
+ *   x_in      x              x_eval      (the denoiser input)
+ *   m0        m_prev         m0
+ *   m1        -              m1
+ *   x_prev    -              x_prev
+ *   m_new     m_cur          m_t         (written)
+ *   x_t       -              x_t         (written; x_eval at a row's first step)
+ *   x_new     x_next         x_pred      (written)
+ * and the rotation is m1 <- m0, m0 <- m_new, x_prev <- x_t, x_in <- x_new.  A DPM row never reads m1 or x_prev and never writes
+ * x_t.  An occupied row's results are bit-identical to ns2vc_dpm_step / ns2vc_unipc_step run on that row with its struct; an
+ * empty row writes 0 to m_new, x_t and x_new and raises no flag.  Every pointer except nan_flags and one of the tables is
+ * required.  ns2vc_dpm_step_rows and ns2vc_unipc_step_rows are this step with one method and one schedule (base 0). */
+#define NS2VC_ROW_DPM 0
+#define NS2VC_ROW_UNIPC 1
+int ns2vc_sampler_step_rows(const float* x_in, const float* unet_out, const float* m0, const float* m1, const float* x_prev,
+                            const ns2vc_dpm_coef* dpm_coefs, const ns2vc_unipc_coef* unipc_coefs, const int* method, const int* base,
+                            int* k, float* m_new, float* x_t, float* x_new, size_t row_n, int B, int* nan_flags, ns2vc_stream stream);
+
 /* DDPM p_sample (model.py:535-542) and DDIM (model.py:586-601) steps after the denoiser returned x0 = x_start.
  * UNLIKE the two entries above, `c` is a DEVICE pointer to one coefficient struct, read by the kernel: a captured chunk of
  * steps then serves every chunk of a long run (the host refills a device window of structs before each replay).

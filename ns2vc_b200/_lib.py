@@ -91,6 +91,7 @@ SIGNATURES = {
     "ns2vc_unipc_step": (C.c_int, [_P, _P, _P, _P, _P, C.POINTER(UniPcCoef), _P, _P, _P, C.c_size_t, _P, _P]),
     "ns2vc_dpm_step_rows": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_int, _P, _P]),   # (device coefficient arrays)
     "ns2vc_unipc_step_rows": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_int, _P, _P]),
+    "ns2vc_sampler_step_rows": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_int, _P, _P]),
     "ns2vc_ddpm_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P, _P]),     # (the coefficient struct is a device pointer)
     "ns2vc_ddim_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P, _P]),
     "ns2vc_mask_bias": (C.c_int, [_P, C.c_int, _P, _P]),

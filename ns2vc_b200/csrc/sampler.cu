@@ -110,33 +110,6 @@ __device__ __forceinline__ void batch_step(size_t n, int* nan_flag, const Update
   if (bad && nan_flag) atomicOr(nan_flag, 1);
 }
 
-// The row kernels: row b of a [B, row_n] batch takes step k[b] of a run whose coefficient structs sit in device memory, so the
-// rows of one batch can be at different steps (requests that joined at different ticks).  Each row is one cluster of kRowCtas
-// CTAs (grid kRowCtas x B); an occupied row runs update(bad, c, j) with struct c = cs[k[b]], an empty row (k[b] < 0) runs zero(j)
-// and raises nothing.  Every CTA reads k[b] before the cluster barrier and CTA 0 advances it after, so a captured tick replays
-// with no host write in between.  The NaN flag is per row.
-constexpr int kRowCtas = 8;
-
-template <class Coef, class Update, class Zero>
-__device__ __forceinline__ void row_step(const Coef* __restrict__ cs, int* k, size_t row_n, int* nan_flags, const Update& update,
-                                         const Zero& zero) {
-  const int b = blockIdx.y;
-  const int kb = k[b];
-  const size_t off = (size_t)b * row_n;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  if (kb < 0) {
-    for (; i < row_n; i += stride) zero(off + i);
-  } else {
-    const Coef c = cs[kb];
-    bool bad = false;
-    for (; i < row_n; i += stride) update(bad, c, off + i);
-    if (bad && nan_flags) atomicOr(nan_flags + b, 1);
-  }
-  cooperative_groups::this_cluster().sync();               // every CTA of the row has read k[b]
-  if (kb >= 0 && blockIdx.x == 0 && threadIdx.x == 0) k[b] = kb + 1;
-}
-
 // Every kernel waits for its predecessor (programmatic dependent launch) before it reads global memory.
 __global__ void __launch_bounds__(256) dpm_step_kernel(const float* __restrict__ x, const float* __restrict__ o,
                                                        const float* __restrict__ mp, ns2vc_dpm_coef c, float* __restrict__ mc,
@@ -157,29 +130,51 @@ __global__ void __launch_bounds__(256) unipc_step_kernel(const float* __restrict
              [&](bool& bad, size_t i) { unipc_update<false>(bad, xp, xe, o, m0p, m1p, c, mt_out, xt_out, xpred_out, i); });
 }
 
-__global__ void __launch_bounds__(256) dpm_step_rows_kernel(const float* __restrict__ x, const float* __restrict__ o,
-                                                            const float* __restrict__ mp, const ns2vc_dpm_coef* __restrict__ cs,
-                                                            int* k, float* __restrict__ mc, float* __restrict__ xn, size_t row_n,
-                                                            int* nan_flags) {
-  pdl_trigger();
-  pdl_wait();
-  row_step(cs, k, row_n, nan_flags,
-           [&](bool& bad, const ns2vc_dpm_coef& c, size_t j) { dpm_update(bad, x, o, mp, c, mc, xn, j); },
-           [&](size_t j) { mc[j] = 0.f; xn[j] = 0.f; });
-}
+// The row kernel: row b of a [B, row_n] batch takes step k[b] of its own run, so the rows of one batch can be at different steps
+// (requests that joined at different ticks) and of different methods.  Row b's method is method[b] (uniform_method for every row
+// when method is NULL) and its struct is dpm[base[b] + k[b]] or unipc[base[b] + k[b]] (base NULL: 0), so one device table per
+// struct type holds every schedule in use.  Both methods share one buffer layout (see ns2vc_sampler_step_rows in the header);
+// a DPM row never reads m1 or x_prev and never writes x_t.  Each row is one cluster of kRowCtas CTAs (grid kRowCtas x B); an
+// empty row (k[b] < 0) zeroes m_new, x_t (when given) and x_new and raises nothing.  Every CTA reads k[b] before the cluster
+// barrier and CTA 0 advances it after, so a captured tick replays with no host write in between.  The NaN flag is per row.
+constexpr int kRowCtas = 8;
 
-__global__ void __launch_bounds__(256) unipc_step_rows_kernel(const float* __restrict__ xp, const float* __restrict__ xe,
-                                                              const float* __restrict__ o, const float* __restrict__ m0p,
-                                                              const float* __restrict__ m1p, const ns2vc_unipc_coef* __restrict__ cs,
-                                                              int* k, float* __restrict__ mt_out, float* __restrict__ xt_out,
-                                                              float* __restrict__ xpred_out, size_t row_n, int* nan_flags) {
+__global__ void __launch_bounds__(256) sampler_step_rows_kernel(const float* __restrict__ x_in, const float* __restrict__ o,
+                                                                const float* __restrict__ m0, const float* __restrict__ m1,
+                                                                const float* __restrict__ x_prev,
+                                                                const ns2vc_dpm_coef* __restrict__ dpm,
+                                                                const ns2vc_unipc_coef* __restrict__ unipc,
+                                                                const int* __restrict__ method, int uniform_method,
+                                                                const int* __restrict__ base, int* k, float* __restrict__ m_new,
+                                                                float* __restrict__ x_t, float* __restrict__ x_new, size_t row_n,
+                                                                int* nan_flags) {
   pdl_trigger();
   pdl_wait();
-  row_step(cs, k, row_n, nan_flags,
-           [&](bool& bad, const ns2vc_unipc_coef& c, size_t j) {
-             unipc_update<true>(bad, xp, xe, o, m0p, m1p, c, mt_out, xt_out, xpred_out, j);
-           },
-           [&](size_t j) { mt_out[j] = 0.f; xt_out[j] = 0.f; xpred_out[j] = 0.f; });
+  const int b = blockIdx.y;
+  const int kb = k[b];
+  const size_t off = (size_t)b * row_n;
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  if (kb < 0) {
+    for (; i < row_n; i += stride) {
+      m_new[off + i] = 0.f;
+      if (x_t) x_t[off + i] = 0.f;
+      x_new[off + i] = 0.f;
+    }
+  } else {
+    const int entry = (base ? base[b] : 0) + kb;
+    bool bad = false;
+    if ((method ? method[b] : uniform_method) == NS2VC_ROW_DPM) {
+      const ns2vc_dpm_coef c = dpm[entry];
+      for (; i < row_n; i += stride) dpm_update(bad, x_in, o, m0, c, m_new, x_new, off + i);
+    } else {
+      const ns2vc_unipc_coef c = unipc[entry];
+      for (; i < row_n; i += stride) unipc_update<true>(bad, x_prev, x_in, o, m0, m1, c, m_new, x_t, x_new, off + i);
+    }
+    if (bad && nan_flags) atomicOr(nan_flags + b, 1);
+  }
+  cooperative_groups::this_cluster().sync();               // every CTA of the row has read k[b]
+  if (kb >= 0 && blockIdx.x == 0 && threadIdx.x == 0) k[b] = kb + 1;
 }
 
 // DDPM and DDIM read their struct from device memory, so a captured chunk of steps serves any window of a run: the host refills
@@ -212,9 +207,12 @@ int launch_batch(void (*kernel)(KArgs...), size_t n, int* nan_flag, ns2vc_stream
   return 0;
 }
 
-template <typename... KArgs, typename... Args>
-int launch_rows(void (*kernel)(KArgs...), int B, ns2vc_stream stream, Args... args) {
-  launch_kc(kernel, dim3(kRowCtas, B), dim3(256), 0, (cudaStream_t)stream, dim3(kRowCtas, 1, 1), args...);
+// The row kernel over B rows.  dpm_step_rows and unipc_step_rows are this launch with one method for every row and one schedule.
+int launch_rows(int B, ns2vc_stream stream, const float* x_in, const float* unet_out, const float* m0, const float* m1,
+                const float* x_prev, const ns2vc_dpm_coef* dpm, const ns2vc_unipc_coef* unipc, const int* method, int uniform_method,
+                const int* base, int* k, float* m_new, float* x_t, float* x_new, size_t row_n, int* nan_flags) {
+  launch_kc(sampler_step_rows_kernel, dim3(kRowCtas, B), dim3(256), 0, (cudaStream_t)stream, dim3(kRowCtas, 1, 1), x_in, unet_out, m0,
+            m1, x_prev, dpm, unipc, method, uniform_method, base, k, m_new, x_t, x_new, row_n, nan_flags);
   NS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -248,7 +246,8 @@ int ns2vc_dpm_step_rows(const float* x, const float* unet_out, const float* m_pr
                         float* x_next, size_t row_n, int B, int* nan_flags, ns2vc_stream stream) {
   NS_REQUIRE(x && unet_out && m_prev && coefs && k && m_cur && x_next, "null argument");
   NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_rows(dpm_step_rows_kernel, B, stream, x, unet_out, m_prev, coefs, k, m_cur, x_next, row_n, nan_flags);
+  return launch_rows(B, stream, x, unet_out, m_prev, nullptr, nullptr, coefs, nullptr, nullptr, NS2VC_ROW_DPM, nullptr, k, m_cur,
+                     nullptr, x_next, row_n, nan_flags);
 }
 
 int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
@@ -256,7 +255,17 @@ int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float*
                           int* nan_flags, ns2vc_stream stream) {
   NS_REQUIRE(x_prev && x_eval && unet_out && m0 && m1 && coefs && k && m_t && x_t && x_pred, "null argument");
   NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_rows(unipc_step_rows_kernel, B, stream, x_prev, x_eval, unet_out, m0, m1, coefs, k, m_t, x_t, x_pred, row_n,
+  return launch_rows(B, stream, x_eval, unet_out, m0, m1, x_prev, nullptr, coefs, nullptr, NS2VC_ROW_UNIPC, nullptr, k, m_t, x_t,
+                     x_pred, row_n, nan_flags);
+}
+
+int ns2vc_sampler_step_rows(const float* x_in, const float* unet_out, const float* m0, const float* m1, const float* x_prev,
+                            const ns2vc_dpm_coef* dpm_coefs, const ns2vc_unipc_coef* unipc_coefs, const int* method, const int* base,
+                            int* k, float* m_new, float* x_t, float* x_new, size_t row_n, int B, int* nan_flags, ns2vc_stream stream) {
+  NS_REQUIRE(x_in && unet_out && m0 && m1 && x_prev && method && base && k && m_new && x_t && x_new, "null argument");
+  NS_REQUIRE(dpm_coefs || unipc_coefs, "no coefficient table");
+  NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
+  return launch_rows(B, stream, x_in, unet_out, m0, m1, x_prev, dpm_coefs, unipc_coefs, method, -1, base, k, m_new, x_t, x_new, row_n,
                      nan_flags);
 }
 

@@ -6,10 +6,15 @@ each slot at its own step index.  Requests wait in a FIFO queue; at the start of
 free slots, and a request *retires* at the end of its ``steps``-th tick, leaving its slot free for the next one.  A request thus
 waits at most one tick for a slot (plus its own admission), never for another request's whole run.
 
+Each request brings its own sampler: DPM-Solver++ or UniPC at its own step count, rows of both methods side by side in one tick.
+The coefficient structs of every schedule in use sit in one device table per method, each slot holds its schedule's base in
+that table and its method tag, and its FiLM rows hold its own model times; a schedule not yet resident grows the tables and
+re-captures the tick once.
+
 Each request's result equals ``convert.convert_batch`` of that request alone with the same x_T, because every stage keeps row b
 equal to utterance b run alone: the encoders run on the newcomers as one ragged batch, ``ns2vc_unet_prepare_cond_ragged`` keeps its
-lengths in device tables, the FiLM rows are per row, and the row step kernels (``ns2vc_dpm_step_rows`` / ``ns2vc_unipc_step_rows``)
-do the scalar step's arithmetic with each row's own coefficient struct.
+lengths in device tables, the FiLM rows are per row, and the row step kernel (``ns2vc_sampler_step_rows``) does the scalar step's
+arithmetic with each row's own method and coefficient struct.
 
 An admission re-prepares only the rows it changes: the newcomers' slots and the slots freed since the last admission, which
 go back to length 1 and zero inputs (``ns2vc_unet_prepare_cond_rows`` and ``ns2vc_unet_time_table_rows`` write those rows
@@ -40,29 +45,35 @@ NAN_MESSAGE = "NaN in the denoiser input during the fused sampling run (referenc
 
 class SlotTable:
     """The host bookkeeping of a server: the FIFO queue of tickets, the ticket in each slot and the tick at whose end it retires.
-    No device state; every decision is made from tick numbers alone, so finding the finished rows needs no device sync."""
+    No device state; every decision is made from tick numbers alone, so finding the finished rows needs no device sync.
+    ``steps`` is the step count of a request enqueued without its own."""
 
     def __init__(self, slots: int, steps: int):
         self.slots, self.steps = int(slots), int(steps)
         self.queue: collections.deque = collections.deque()
         self.ticket: List[Optional[int]] = [None] * self.slots
         self.last: List[Optional[int]] = [None] * self.slots
+        self._steps: Dict[int, int] = {}                    # queued ticket -> its step count
 
-    def enqueue(self, ticket: int) -> None:
+    def enqueue(self, ticket: int, steps: Optional[int] = None) -> None:
+        steps = self.steps if steps is None else int(steps)
+        if steps < 1:
+            raise ValueError(f"steps must be >= 1, got {steps}")
         self.queue.append(ticket)
+        self._steps[ticket] = steps
 
     def free_slots(self) -> List[int]:
         return [s for s in range(self.slots) if self.ticket[s] is None]
 
     def admit(self, tick: int) -> List[Tuple[int, int]]:
         """(slot, ticket) of the requests admitted at the start of ``tick``: the oldest queued ones, into the free slots in
-        ascending order.  Each will run ticks ``tick .. tick + steps - 1``."""
+        ascending order.  Each will run ticks ``tick .. tick + steps_b - 1``, steps_b its own step count."""
         out = []
         for s in self.free_slots():
             if not self.queue:
                 break
             t = self.queue.popleft()
-            self.ticket[s], self.last[s] = t, tick + self.steps - 1
+            self.ticket[s], self.last[s] = t, tick + self._steps.pop(t) - 1
             out.append((s, t))
         return out
 
@@ -83,6 +94,9 @@ class SlotTable:
 
 
 HEADER_FIELDS = 7          # per admission: ticket, rank, slot, samples, sr, T_b, S_b
+_METHODS = ("dpmsolver", "unipc")                    # a row's method tag (NS2VC_ROW_DPM, NS2VC_ROW_UNIPC) and its name
+_METHOD_CODE = {m: i for i, m in enumerate(_METHODS)}
+_KIND = {"dpmsolver": "dpm", "unipc": "unipc"}       # the sampler tables' name of each method
 
 
 def place_requests(free: Sequence[int], n: int) -> List[int]:
@@ -129,7 +143,8 @@ class ConversionServer:
         done = srv.tick()                              # {ticket: audio [T_b * 256]} of the requests that finished in this tick
         done = srv.drain()                             # tick until the queue and the slots are empty
 
-    ``method`` is ``"unipc"`` (30 steps by default) or ``"dpmsolver"`` (40), as for ``convert_utterances``.  A request whose
+    ``method`` is ``"unipc"`` (30 steps by default) or ``"dpmsolver"`` (40), as for ``convert_utterances``: the sampler of a
+    request submitted without its own (``submit(..., method=, steps=)``).  A request whose
     denoiser input held a NaN comes back as an ``AssertionError`` (the reference's per-call guard, model.py:404) in place of its
     audio; the others carry on.  ``last_latents`` holds the latents [100, T_b] of the requests that finished in the last tick.
 
@@ -142,7 +157,7 @@ class ConversionServer:
     ``submit``, and it places each newcomer, FIFO, on the rank with the most free slots (``place_requests``).  Every rank calls
     ``tick()`` and ``drain()`` in lockstep and mirrors the whole placement, so each knows every retirement tick.  Per tick, one
     int64 header broadcast from rank 0 carries the admissions and a global idle flag; when something is admitted, one float32
-    broadcast carries the newcomers' wav | prompt | x_T.  Each rank admits and ticks its own slots, the ranks exchange one status
+    broadcast carries the newcomers' wav | prompt | x_T and one int64 broadcast their (method, steps).  Each rank admits and ticks its own slots, the ranks exchange one status
     flag (an exception on any rank raises a RuntimeError on every rank), and on ticks where something retires one ragged gather
     (``shard.gather_ragged``) brings each result's NaN flag, latent and audio to rank 0.  Rank 0 returns the results and holds
     ``last_latents``; the other ranks return {}.  The default x_T is drawn on rank 0 at ``submit``, as on one GPU, so every
@@ -181,12 +196,20 @@ class ConversionServer:
             self.served = 0                                                            # requests retired on any rank so far
 
     # ------------------------------------------------------------------------------------------------ requests
-    def submit(self, wav: torch.Tensor, sr: int, prompt_mel: torch.Tensor, x_T: Optional[torch.Tensor] = None) -> int:
+    def submit(self, wav: torch.Tensor, sr: int, prompt_mel: torch.Tensor, x_T: Optional[torch.Tensor] = None,
+               method: Optional[str] = None, steps: Optional[int] = None) -> int:
         """Queues one 1-D waveform at ``sr`` with its prompt mel [100, S_b] and returns its ticket (increasing, FIFO).  ``x_T``
         ([1, 100, T_b] or [100, T_b]) defaults to ``torch.randn((1, 100, T_b))`` on the model's device, drawn here: requests
-        submitted in list order get the draws ``convert_utterances`` makes for that list.  On several ranks only rank 0 submits."""
+        submitted in list order get the draws ``convert_utterances`` makes for that list.  On several ranks only rank 0 submits.
+
+        ``method`` (``"unipc"`` or ``"dpmsolver"``) and ``steps`` are this request's sampler; ``None`` takes the server's
+        ``method`` / ``steps``.  The result equals ``convert_batch`` of the request alone with that method and step count."""
         if self.world > 1 and self.rank != 0:
             raise RuntimeError(f"submit() on rank {self.rank}: only rank 0 of the server's group takes requests")
+        method = self.method if method is None else method
+        steps = convert._check_method(method, self.steps if steps is None else steps)
+        if steps < 1:
+            raise ValueError(f"steps must be >= 1, got {steps}")
         plan = convert._check_inputs([wav], sr, [prompt_mel], None if x_T is None else [x_T])[0]
         if plan["T"] > self.T:
             raise ValueError(f"the waveform is {plan['T']} frames, more than max_frames={self.T}")
@@ -197,11 +220,12 @@ class ConversionServer:
             x_T = torch.randn((1, LATENT_CH, plan["T"]), device=self._device())
         ticket = self._next_ticket
         self._next_ticket += 1
-        self._requests[ticket] = dict(wav=wav, sr=int(sr), prompt=prompt_mel, x_T=x_T, plan=plan, T=plan["T"], S=S_b)
+        self._requests[ticket] = dict(wav=wav, sr=int(sr), prompt=prompt_mel, x_T=x_T, plan=plan, T=plan["T"], S=S_b, method=method,
+                                      steps=steps)
         if self.world > 1:
             self._pending.append(ticket)
         else:
-            self.table.enqueue(ticket)
+            self.table.enqueue(ticket, steps)
         return ticket
 
     @torch.no_grad()
@@ -233,6 +257,7 @@ class ConversionServer:
     def _step(self, new: List[Tuple[int, int]]):
         """The device work of one tick on this server's slots: the admission of ``new`` (slot, ticket), then the tick."""
         stale = self._setup()
+        stale = self._resident([(self._requests[tk]["method"], self._requests[tk]["steps"]) for _, tk in new]) or stale
         if new:
             self._admit(new, full=stale or not self._owns_cond())
         elif stale:
@@ -291,6 +316,17 @@ class ConversionServer:
             off += n + np_ + nx
         return out
 
+    def _settings(self, adm) -> List[Tuple[str, int]]:
+        """Every newcomer's (method, steps) as sent by rank 0 in one int64 broadcast: each rank needs them to mirror the
+        retirements, and the newcomer's rank to run its schedule."""
+        if self.rank == 0:
+            flat = torch.tensor([v for tk, *_ in adm for v in (_METHOD_CODE[self._requests[tk]["method"]], self._requests[tk]["steps"])],
+                                dtype=torch.int64)
+        else:
+            flat = torch.zeros(2 * len(adm), dtype=torch.int64)
+        v = self._broadcast(flat).tolist()
+        return [(_METHODS[v[2 * i]], int(v[2 * i + 1])) for i in range(len(adm))]
+
     def _tick_group(self) -> Dict[int, object]:
         if not self._checked:
             self._check_group_args()
@@ -301,12 +337,13 @@ class ConversionServer:
         if self._idle:
             return {}
         payload = self._payload(adm) if adm else []
-        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T) in zip(adm, payload):
-            self.tables[r].enqueue(tk)
+        settings = self._settings(adm) if adm else []
+        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T), (method, steps) in zip(adm, payload, settings):
+            self.tables[r].enqueue(tk, steps)
             self._frames[tk] = Tb
             if r == self.rank and self.rank != 0:
                 plan = convert._check_inputs([wav], sr, [prompt], [x_T])[0]
-                self._requests[tk] = dict(wav=wav, sr=sr, prompt=prompt, x_T=x_T, plan=plan, T=Tb, S=Sb)
+                self._requests[tk] = dict(wav=wav, sr=sr, prompt=prompt, x_T=x_T, plan=plan, T=Tb, S=Sb, method=method, steps=steps)
             elif r != self.rank:
                 self._requests.pop(tk, None)               # (rank 0: placed elsewhere)
         news = [tab.admit(t) for tab in self.tables]
@@ -385,26 +422,53 @@ class ConversionServer:
             raise ValueError("the server needs out_channels == latent channels (x_start parameterisation)")
         self._sess, self._L = sess, _lib.lib()
         self._clen, self._plen = [1] * B, [1] * B
-        ns = default_schedule()
-        ts = torch.linspace(ns.T, 1.0 / ns.total_N, self.steps + 1)
-        extra = True if self.kind == "dpm" else "bh2"       # lower_order_final / variant, as sample_latents runs them
-        steps = _step_table(self.kind, ns, ts, extra, (self.kind, tuple(float(v) for v in ts), extra, schedule_signature(ns)))
-        self._coef, _ = coefs.c_table(steps, dev)
-        self._tvals = coefs.t_inputs(steps, B, dev)
-        L, h = self._L, sess.h
-        self._fw = int(L.ns2vc_unet_film_width(h))
-        self._film_table = torch.empty(int(L.ns2vc_unet_time_table_floats(h, self.steps * B)), **f32)
-        self._film_rows = self._film_table[:self.steps * B * self._fw].view(self.steps * B, self._fw)
+        self._fw = int(self._L.ns2vc_unet_film_width(sess.h))
+        self._sched: Dict[Tuple[str, int], dict] = {}        # (method, steps) -> its tag, its base in its method's table, its t column
+        self._tab: Dict[str, list] = {"dpm": [], "unipc": []}   # the step records of every resident schedule, per method
+        self._coef: Dict[str, Optional[torch.Tensor]] = {"dpm": None, "unipc": None}
+        self._tvals = torch.zeros((0, B), **f32)           # [K, B]: the model time of slot b's request at its step k
         self._film = torch.empty((B, self._fw), **f32)
         self._rowbase = torch.arange(B, dtype=torch.int64, device=dev)
         self._k = torch.full((B,), -1, dtype=torch.int32, device=dev)
+        self._tag, self._base = [0] * B, [0] * B            # each slot's method tag and schedule base (host copies)
+        self._row_tag = torch.zeros((B,), dtype=torch.int32, device=dev)
+        self._row_base = torch.zeros((B,), dtype=torch.int32, device=dev)
         self._nan = torch.zeros((B,), dtype=torch.int32, device=dev)
         shape = (B, sess.Cl, T)
-        names = ("x", "x_next", "m_prev", "m_cur") if self.kind == "dpm" else ("x_prev", "x_eval", "m0", "m1", "m_t", "x_t", "x_pred")
-        self._buf = {n: torch.zeros(shape, **f32) for n in names + ("out",)}
-        self._x = self._buf["x" if self.kind == "dpm" else "x_eval"]      # the denoiser input; after a request's last tick, its latent
-        self._graph, self._runs = None, 0
+        self._buf = {n: torch.zeros(shape, **f32) for n in ("x_in", "m0", "m1", "x_prev", "m_new", "x_t", "x_new", "out")}
+        self._x = self._buf["x_in"]                         # the denoiser input; after a request's last tick, its latent
+        self._resident([(self.method, self.steps)])
+        self._tvals.copy_(self._sched[(self.method, self.steps)]["t"][:, None].expand(self.steps, B))
         return False
+
+    def _resident(self, settings: Sequence[Tuple[str, int]]) -> bool:
+        """Makes every (method, steps) schedule of ``settings`` resident.  The tables only grow: a schedule not yet resident
+        appends its coefficient structs to its method's table (the residents keep their bases), re-allocates that table and,
+        when it is the longest yet, the FiLM table, and drops the captured tick.  True when that happened: the FiLM rows of
+        every slot must then be written again (``_prepare_all``)."""
+        new = [st for st in dict.fromkeys(settings) if st not in self._sched]
+        if not new:
+            return False
+        ns, dev, B = default_schedule(), self._device(), self.B
+        for method, steps in new:
+            kind = _KIND[method]
+            ts = torch.linspace(ns.T, 1.0 / ns.total_N, steps + 1)
+            extra = True if kind == "dpm" else "bh2"       # lower_order_final / variant, as sample_latents runs them
+            tab = _step_table(kind, ns, ts, extra, (kind, tuple(float(v) for v in ts), extra, schedule_signature(ns)))
+            self._sched[(method, steps)] = dict(tag=_METHOD_CODE[method], base=len(self._tab[kind]),
+                                                t=torch.tensor([st.t_input for st in tab], dtype=torch.float32))
+            self._tab[kind] = self._tab[kind] + list(tab)
+            self._coef[kind] = coefs.c_table(self._tab[kind], dev)[0]
+        K = max(steps for _, steps in self._sched)
+        if K > self._tvals.shape[0]:
+            tv = torch.zeros((K, B), dtype=torch.float32, device=dev)
+            tv[:self._tvals.shape[0]] = self._tvals
+            self._tvals = tv
+            L, h = self._L, self._sess.h
+            self._film_table = torch.empty(int(L.ns2vc_unet_time_table_floats(h, K * B)), dtype=torch.float32, device=dev)
+            self._film_rows = self._film_table[:K * B * self._fw].view(K * B, self._fw)
+        self._graph, self._runs = None, 0
+        return True
 
     def _admit(self, new: List[Tuple[int, int]], full: bool):
         """Encodes the newcomers as one ragged batch per input rate and writes them into their slots.  Then prepares the rows
@@ -432,6 +496,9 @@ class ConversionServer:
                     b[s].zero_()
                 self._x[s, :, :Tb] = r["x_T"].reshape(LATENT_CH, Tb).to(dev, torch.float32)
                 self._clen[s], self._plen[s] = Tb, Sb
+                sched = self._sched[(r["method"], r["steps"])]
+                self._tvals[:r["steps"], s] = sched["t"].to(dev)          # the FiLM rows (k, s) hold this request's own times
+                self._tag[s], self._base[s] = sched["tag"], sched["base"]
         occupied = {s for s in range(self.B) if self.table.ticket[s] is not None}
         for s in range(self.B):
             if s not in occupied:                           # empty slots: length 1, zero inputs
@@ -442,6 +509,8 @@ class ConversionServer:
                     b[s].zero_()
                 self._clen[s], self._plen[s] = 1, 1
         slots = torch.tensor([s for s, _ in new], dtype=torch.int64, device=dev)
+        self._row_tag.copy_(torch.tensor(self._tag, dtype=torch.int32))
+        self._row_base.copy_(torch.tensor(self._base, dtype=torch.int32))
         self._k.index_fill_(0, slots, 0)
         self._nan.index_fill_(0, slots, 0)
         if full:
@@ -470,32 +539,27 @@ class ConversionServer:
         sess.time_table_rows(self._tvals, self._film_table, rows)
 
     def _body(self):
-        """One tick: the FiLM row (k_b, b) of every slot, the forward, the row step, then the rotation of the sampler's buffers.
-        The rotation is four (UniPC) or two (DPM-Solver++) device copies inside the one captured graph rather than a cycle of
-        graphs over rotating pointers: UniPC's 3-deep history and 2-deep state would need lcm(3, 2) = 6 captures of the whole
-        forward, and the copies move 4 x slots x 100 x max_frames floats, small next to one forward."""
+        """One tick: the FiLM row (k_b, b) of every slot, the forward, the row step of every slot with its own method and
+        schedule (``ns2vc_sampler_step_rows``), then the rotation of the sampler's buffers: m1 <- m0 <- m_new, x_prev <- x_t,
+        x_in <- x_new, the same for both methods (a DPM-Solver++ row never reads m1 or x_prev).  The rotation is four device
+        copies inside the one captured graph rather than a cycle of graphs over rotating pointers: UniPC's 3-deep history and
+        2-deep state would need lcm(3, 2) = 6 captures of the whole forward, and the copies move 4 x slots x 100 x max_frames
+        floats, small next to one forward."""
         sess, L, b = self._sess, self._L, self._buf
         idx = self._k.clamp(min=0).to(torch.int64) * self.B + self._rowbase       # empty slots read step 0's row (their output is discarded)
         torch.index_select(self._film_rows, 0, idx, out=self._film)
-        sess.forward(self._x, None, b["out"], film_rows=self._film)
+        sess.forward(b["x_in"], None, b["out"], film_rows=self._film)
         n, stream = sess.Cl * self.T, sess._stream()
+        dpm, unipc = (t.data_ptr() if t is not None else None for t in (self._coef["dpm"], self._coef["unipc"]))
         with torch.cuda.device(sess.dev):
-            if self.kind == "dpm":
-                _lib.check(L.ns2vc_dpm_step_rows(b["x"].data_ptr(), b["out"].data_ptr(), b["m_prev"].data_ptr(), self._coef.data_ptr(),
-                                                 self._k.data_ptr(), b["m_cur"].data_ptr(), b["x_next"].data_ptr(), n, self.B,
-                                                 self._nan.data_ptr(), stream))
-            else:
-                _lib.check(L.ns2vc_unipc_step_rows(b["x_prev"].data_ptr(), b["x_eval"].data_ptr(), b["out"].data_ptr(), b["m0"].data_ptr(),
-                                                   b["m1"].data_ptr(), self._coef.data_ptr(), self._k.data_ptr(), b["m_t"].data_ptr(),
-                                                   b["x_t"].data_ptr(), b["x_pred"].data_ptr(), n, self.B, self._nan.data_ptr(), stream))
-        if self.kind == "dpm":
-            b["x"].copy_(b["x_next"])
-            b["m_prev"].copy_(b["m_cur"])
-        else:
-            b["m1"].copy_(b["m0"])
-            b["m0"].copy_(b["m_t"])
-            b["x_prev"].copy_(b["x_t"])
-            b["x_eval"].copy_(b["x_pred"])
+            _lib.check(L.ns2vc_sampler_step_rows(b["x_in"].data_ptr(), b["out"].data_ptr(), b["m0"].data_ptr(), b["m1"].data_ptr(),
+                                                 b["x_prev"].data_ptr(), dpm, unipc, self._row_tag.data_ptr(), self._row_base.data_ptr(),
+                                                 self._k.data_ptr(), b["m_new"].data_ptr(), b["x_t"].data_ptr(), b["x_new"].data_ptr(), n,
+                                                 self.B, self._nan.data_ptr(), stream))
+        b["m1"].copy_(b["m0"])
+        b["m0"].copy_(b["m_new"])
+        b["x_prev"].copy_(b["x_t"])
+        b["x_in"].copy_(b["x_new"])
 
     def _run_tick(self):
         self._runs += 1
