@@ -672,6 +672,20 @@ typedef struct ns2vc_check_istft_args {
 } ns2vc_check_istft_args;
 int ns2vc_check_istft(const ns2vc_check_istft_args* args, char* desc, int desc_len, ns2vc_stream stream);
 
+/* The packed-weight record: the operands engine `kind` (0 denoiser ns2vc_unet, 1 condition encoders ns2vc_pre, 2 content encoder
+ * ns2vc_cv, 3 vocoder ns2vc_voc) built at its last finalize, in packing order, each with its site name and the load-time vectors
+ * (folded LayerNorm vectors, merged biases and operators, concatenations) read beside it.  Errors: another kind, a null handle,
+ * weights not packed since the last load, an index out of range, a name buffer shorter than the name and its NUL.
+ * _count returns the number of operands (-1 on error).  _packed: name (or NULL), the packed image's Npad columns (0: an entry of
+ * vectors only), nkb k-blocks and n_logical columns, nvec vectors; hi_out / lo_out (device, nkb * Npad * 64 bf16 each, or NULL)
+ * receive the swizzled hi / lo images.  _fold_vector: vector j of operand i, its name (or NULL), length n and (out: device
+ * fp32 [n], or NULL) values.  Stream-ordered copies. */
+int ns2vc_check_packed_count(int kind, const void* handle);
+int ns2vc_check_packed(int kind, const void* handle, int i, char* name, int name_len, int* Npad, int* nkb, int* n_logical, int* nvec,
+                       void* hi_out, void* lo_out, ns2vc_stream stream);
+int ns2vc_check_fold_vector(int kind, const void* handle, int i, int j, char* name, int name_len, long long* n, float* out,
+                            ns2vc_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

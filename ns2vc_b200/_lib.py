@@ -194,6 +194,10 @@ SIGNATURES = {
     "ns2vc_check_down_conv": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_cv_conv": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
     "ns2vc_check_istft": (C.c_int, [_P, C.c_char_p, C.c_int, _P]),
+    # the packed-weight record (tests/test_packed_weights_fp64.py)
+    "ns2vc_check_packed_count": (C.c_int, [C.c_int, _P]),
+    "ns2vc_check_packed": (C.c_int, [C.c_int, _P, C.c_int, C.c_char_p, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
+    "ns2vc_check_fold_vector": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_char_p, C.c_int, _P, _P, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

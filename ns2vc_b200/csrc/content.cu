@@ -353,6 +353,10 @@ struct ns2vc_cv : SingleProgramEngine {
   LenTables lt{};                                           // the cached program's length tables (in its workspace)
 };
 
+namespace ns2vc {
+const EngineBase* engine_base(const ns2vc_cv* h) { return h; }
+}  // namespace ns2vc
+
 namespace {
 
 std::string layer(int i) { return "encoder.layers." + std::to_string(i); }
@@ -401,8 +405,10 @@ int pack_with(ns2vc_cv* h, cudaStream_t st, float* scratch) {
     PackedB& pb = h->conv[l];
     if ((rc = mem.alloc_packed(pb, C0, C0, conv_k(l) * nkb_of(C0), false))) return rc;
     if ((rc = pack_cv_conv(pb, w.W(conv_key(l) + ".0.weight"), C0, l, st))) return rc;
+    h->packed.add(conv_key(l), pb);
   }
   if ((rc = pack_lin(mem, h->proj, w.W("post_extract_proj.weight"), D, C0, st))) return rc;
+  h->packed.add("post_extract_proj", h->proj);
   {
     float* wpos = scratch;
     cv_weight_norm_kernel<<<K, 256, 0, st>>>(w.W("encoder.pos_conv.0.weight_g"), w.W("encoder.pos_conv.0.weight_v"), D * gw, K, wpos);
@@ -411,6 +417,7 @@ int pack_with(ns2vc_cv* h, cudaStream_t st, float* scratch) {
     for (int g = 0; g < G; ++g) {
       if ((rc = mem.alloc_packed(h->pos[g], gw, gw, K, false))) return rc;   // gw <= 64 channels, zero beyond
       if ((rc = pack_cv_pos_group(h->pos[g], wpos + (size_t)g * gw * gw * K, gw, K, st))) return rc;
+      h->packed.add("encoder.pos_conv." + std::to_string(g), h->pos[g]);
     }
   }
   const int L = c.num_layers;
@@ -429,8 +436,14 @@ int pack_with(ns2vc_cv* h, cudaStream_t st, float* scratch) {
     if ((rc = pack_lin(mem, h->out[i], w.W(p + "out_proj.weight"), D, D, st))) return rc;
     if ((rc = pack_lin(mem, h->fc1[i], w.W(layer(i) + ".fc1.weight"), c.ffn_dim, D, st))) return rc;
     if ((rc = pack_lin(mem, h->fc2[i], w.W(layer(i) + ".fc2.weight"), D, c.ffn_dim, st))) return rc;
+    h->packed.add(layer(i) + ".qkv", h->qkv[i], {{"bias", h->qkv_b[i], 3 * D}});
+    h->packed.add(layer(i) + ".out_proj", h->out[i]);
+    h->packed.add(layer(i) + ".fc1", h->fc1[i]);
+    h->packed.add(layer(i) + ".fc2", h->fc2[i]);
   }
-  return pack_lin(mem, h->fin, w.W("final_proj.weight"), c.final_dim, D, st);
+  if ((rc = pack_lin(mem, h->fin, w.W("final_proj.weight"), c.final_dim, D, st))) return rc;
+  h->packed.add("final_proj", h->fin);
+  return 0;
 }
 
 // Packs every operator; the load-time scratch is freed again in stream order, whatever the outcome

@@ -113,6 +113,8 @@ struct ns2vc_unet : EngineBase {
 
 namespace ns2vc {
 
+const EngineBase* engine_base(const ns2vc_unet* h) { return h; }
+
 // A resampler's (Downsample1D's, Upsample1D's) conv weights [C, C, 3]: tap j at k-block j nkb(C)
 int pack_resample_conv(PackedB& pb, const float* w, int C, cudaStream_t st) {
   for (int j = 0; j < 3; ++j) {
@@ -319,11 +321,13 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
     if ((rc = h->mem.alloc_packed(h->convin_lat, c0, c0, 3 * nl, h->simt))) return rc;
     for (int j = 0; j < 3; ++j)
       if ((rc = pack_named(h, h->convin_lat, "conv_in.weight", c0, c.in_channels, 3, j, 0, Cl, 0, j * nl, 0, st))) return rc;
+    h->packed.add("conv_in.latent", h->convin_lat);
     if (Cc > 0) {
       const int nc = nkb_of(Cc);
       if ((rc = h->mem.alloc_packed(h->convin_content, c0, c0, 3 * nc, h->simt))) return rc;
       for (int j = 0; j < 3; ++j)
         if ((rc = pack_named(h, h->convin_content, "conv_in.weight", c0, c.in_channels, 3, j, Cl, Cc, 0, j * nc, 0, st))) return rc;
+      h->packed.add("conv_in.content", h->convin_content);
     }
   }
   // resnets / transformers / resamplers in plan order
@@ -344,6 +348,8 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
         if ((rc = pack_named(h, s.conv2, s.p + ".conv_shortcut.weight", s.cout, s.cin, 1, 0, 0, s.cin, 0, 3 * no, 0, st))) return rc;
       if (!(s.bias2 = h->mem.alloc<float>(s.cout))) return -2;
       add_vec_kernel<<<ceil_div(s.cout, 256), 256, 0, st>>>(h->weights.W(s.p + ".conv2.bias"), s.shortcut ? h->weights.W(s.p + ".conv_shortcut.bias") : nullptr, s.bias2, s.cout);
+      h->packed.add(s.p + ".conv1", s.conv1);
+      h->packed.add(s.p + ".conv2", s.conv2, {{"bias2", s.bias2, s.cout}});
       s.film_off = film_off;
       film_off += c.time_scale_shift ? 2 * s.cout : s.cout;
       o.site = (int)h->resnets.size();
@@ -385,6 +391,13 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
         if ((rc = h->mem.alloc_packed(x.ff2p, C, C, nkb_of(4 * C) + nk, h->simt))) return rc;
         if ((rc = pack_seg(x.ff2p, Wm, C, 4 * C, 1, 0, 0, 4 * C, 0, 0, 0, st))) return rc;
         if ((rc = pack_named(h, x.ff2p, x.p + ".proj_out.weight", C, C, 1, 0, 0, C, 0, nkb_of(4 * C), 0, st))) return rc;
+        h->packed.add(x.p + ".proj_in", x.proj_in);
+        h->packed.add(x.p + ".qkv", x.qkv, {{"g_qkv", x.g_qkv, 3 * C}, {"bf_qkv", x.bf_qkv, 3 * C}});
+        h->packed.add(x.p + ".out1", x.out1);
+        h->packed.add(x.p + ".q2", x.q2, {{"g_q2", x.g_q2, C}, {"bf_q2", x.bf_q2, C}});
+        h->packed.add(x.p + ".out2", x.out2);
+        h->packed.add(x.p + ".ff1", x.ff1, {{"g_ff1", x.g_ff1, 8 * C}, {"bf_ff1", x.bf_ff1, 8 * C}});
+        h->packed.add(x.p + ".ff2p", x.ff2p, {{"Wm", Wm, (long long)C * 4 * C}, {"bias_ff2p", x.bias_ff2p, C}});
       }
       x.kv_off = kv_off;
       kv_off += C;
@@ -396,6 +409,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       NS_REQUIRE(w != nullptr, "pack: weight %s missing", (s.p + ".conv.weight").c_str());
       if ((rc = h->mem.alloc_packed(s.w, s.c, s.c, 3 * nkb_of(s.c), h->simt))) return rc;
       if ((rc = pack_resample_conv(s.w, w, s.c, st))) return rc;
+      h->packed.add(s.p + ".conv", s.w);
       o.site = (int)h->resamplers.size();
       h->resamplers.push_back(s);
     }
@@ -410,6 +424,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
     if ((rc = h->mem.alloc_packed(h->conv_out, c.out_channels, c.out_channels, 3 * nk, h->simt))) return rc;
     for (int j = 0; j < 3; ++j)
       if ((rc = pack_named(h, h->conv_out, "conv_out.weight", c.out_channels, c0, 3, j, 0, c0, 0, j * nk, 0, st))) return rc;
+    h->packed.add("conv_out", h->conv_out);
   }
   // all cross-attention K|V projections as one GEMM over the prompt
   if (h->kv_total > 0) {
@@ -420,6 +435,7 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
       if ((rc = pack_named(h, h->kv_all, b + ".attn2.to_k.weight", x.c, xd, 1, 0, 0, xd, x.kv_off, 0, 0, st))) return rc;
       if ((rc = pack_named(h, h->kv_all, b + ".attn2.to_v.weight", x.c, xd, 1, 0, 0, xd, x.v_off, 0, 0, st))) return rc;
     }
+    h->packed.add("kv_all", h->kv_all);
   }
   // concatenated FiLM projection [film_total, ted]
   if (!(h->film_W = h->mem.alloc<float>((size_t)h->film_total * h->ted))) return -2;
@@ -429,8 +445,12 @@ int pack_all(ns2vc_unet* h, cudaStream_t st) {
     NS_CHECK_CUDA(cudaMemcpyAsync(h->film_W + (size_t)s.film_off * h->ted, h->weights.W(s.p + ".time_emb_proj.weight"), (size_t)rows * h->ted * 4, cudaMemcpyDeviceToDevice, st));
     NS_CHECK_CUDA(cudaMemcpyAsync(h->film_b + s.film_off, h->weights.W(s.p + ".time_emb_proj.bias"), (size_t)rows * 4, cudaMemcpyDeviceToDevice, st));
   }
-  if (c.add_embed_text)
-    if ((rc = concat_pool_kv(h->mem, h->weights, "add_embedding.pool", c.cross_attention_dim, h->pool_kv, st))) return rc;
+  h->packed.add("time_emb_proj", PackedB{}, {{"film_W", h->film_W, (long long)h->film_total * h->ted}, {"film_b", h->film_b, h->film_total}});
+  if (c.add_embed_text) {
+    const int xd = c.cross_attention_dim;
+    if ((rc = concat_pool_kv(h->mem, h->weights, "add_embedding.pool", xd, h->pool_kv, st))) return rc;
+    h->packed.add("add_embedding.pool.kv", PackedB{}, {{"W", h->pool_kv.W, 2LL * xd * xd}, {"b", h->pool_kv.b, 2LL * xd}});
+  }
   return 0;
 }
 

@@ -478,12 +478,24 @@ inline const Launch* bound(const Launch& l, const CallArgs& in, Launch& tmp, int
   return &tmp;
 }
 
-// What every engine handle holds: the reference state_dict, the device memory of its packed weights, whether the loaded
-// weights are packed, and the number of launches of its last run.  Each handle also has a drop_programs() that forgets the
-// launch programs built over the packed weights.
+// The operands a packer built, in packing order: each under its site name, with the load-time vectors (folded LayerNorm
+// vectors, merged biases and operators, concatenations) the launch programs read beside it.  Host bookkeeping only: the
+// pointers are the engine's own device memory and stay valid until the next finalize.  The kernel checks read it back
+// (ns2vc_check_packed), so that the tests can compare every packed image and fold with an fp64 fold of the state_dict.
+struct PackedRecord {
+  struct Vec { std::string name; const float* p; long long n; };
+  struct Entry { std::string name; PackedB pb; std::vector<Vec> vecs; };   // pb.Npad == 0: vectors only
+  std::vector<Entry> entries;
+  void add(const std::string& name, const PackedB& pb, std::vector<Vec> vecs = {}) { entries.push_back(Entry{name, pb, std::move(vecs)}); }
+};
+
+// What every engine handle holds: the reference state_dict, the device memory of its packed weights and their record, whether
+// the loaded weights are packed, and the number of launches of its last run.  Each handle also has a drop_programs() that
+// forgets the launch programs built over the packed weights.
 struct EngineBase {
   WeightRegistry weights;
   DeviceMem mem;
+  PackedRecord packed;
   bool finalized = false;
   int last_launches = 0;
 };
@@ -510,6 +522,7 @@ template <class Engine, class Pack> int finalize_engine(Engine* h, Pack pack) {
   int rc = h->weights.require_all_loaded();
   if (rc) return rc;
   h->mem.release();
+  h->packed.entries.clear();
   h->drop_programs();
   if ((rc = pack())) return rc;
   NS_CHECK_CUDA(cudaGetLastError());
@@ -585,4 +598,14 @@ template <class Own> int run_cached(SingleProgramEngine* h, bool simt, const Cal
   return 0;
 }
 
+}  // namespace ns2vc
+
+struct ns2vc_unet; struct ns2vc_pre; struct ns2vc_cv; struct ns2vc_voc;
+
+namespace ns2vc {
+// The EngineBase of each handle type, defined beside the type (kernel_check.cu sees the handles as opaque)
+const EngineBase* engine_base(const ns2vc_unet* h);
+const EngineBase* engine_base(const ns2vc_pre* h);
+const EngineBase* engine_base(const ns2vc_cv* h);
+const EngineBase* engine_base(const ns2vc_voc* h);
 }  // namespace ns2vc

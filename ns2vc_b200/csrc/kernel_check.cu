@@ -6,11 +6,14 @@
 // plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention dispatch, the launchers of common.cuh and
 // engine_host.cuh).  tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py, tests/test_audio_kernels_fp64.py and
 // tests/test_strided_conv_fp64.py drive them at the shapes and edges the models never reach.  Nothing here is a kernel: every
-// launch is the product's own.
+// launch is the product's own.  The packed-weight record (ns2vc_check_packed, ns2vc_check_fold_vector) gives back what each
+// engine's packer built, for tests/test_packed_weights_fp64.py.
 #include "engine_host.cuh"
 #include "../../include/ns2vc_b200.h"
 
 #include <cstdio>
+#include <cstring>
+#include <string>
 #include <vector>
 
 namespace ns2vc {
@@ -20,6 +23,30 @@ SplitBuf to_split(const ns2vc_check_split& s) {
   SplitBuf b{};
   b.hi = (__nv_bfloat16*)s.hi; b.lo = (__nv_bfloat16*)s.lo; b.T = s.T; b.C = s.C; b.ld = s.ld; b.bpitch = s.bpitch;
   return b;
+}
+
+// The packed record of the handle of engine `kind` (0 denoiser, 1 condition encoders, 2 content encoder, 3 vocoder); nullptr
+// (the error is set) for another kind, a null handle, or weights that are not packed
+const PackedRecord* packed_record(int kind, const void* handle) {
+  const EngineBase* e = nullptr;
+  switch (kind) {
+    case 0: e = engine_base((const ns2vc_unet*)handle); break;
+    case 1: e = engine_base((const ns2vc_pre*)handle); break;
+    case 2: e = engine_base((const ns2vc_cv*)handle); break;
+    case 3: e = engine_base((const ns2vc_voc*)handle); break;
+    default: set_error("check_packed: engine kind %d (0 denoiser, 1 condition encoders, 2 content encoder, 3 vocoder)", kind); return nullptr;
+  }
+  if (!handle) { set_error("check_packed: null handle"); return nullptr; }
+  if (!e->finalized) { set_error("check_packed: the weights are not packed (finalize has not run since the last load)"); return nullptr; }
+  return &e->packed;
+}
+
+// copies `name` into the caller's buffer (may be null)
+int copy_name(const std::string& name, char* out, int out_len) {
+  if (!out) return 0;
+  NS_REQUIRE(out_len > (int)name.size(), "check_packed: name buffer of %d bytes for %s (%d + 1 needed)", out_len, name.c_str(), (int)name.size());
+  memcpy(out, name.c_str(), name.size() + 1);
+  return 0;
 }
 
 // the kernel and template arguments a launch selected, for the caller's `desc` (may be null)
@@ -435,6 +462,45 @@ int ns2vc_check_istft(const ns2vc_check_istft_args* a, char* desc, int desc_len,
   NS_CHECK_CUDA(cudaFreeAsync(d_tf, st));
   if (rc) return rc;
   report(desc, desc_len, "voc_istft<log2m=%d,smem=%zu>", log2m, smem);
+  return 0;
+}
+
+int ns2vc_check_packed_count(int kind, const void* handle) {
+  const PackedRecord* r = packed_record(kind, handle);
+  return r ? (int)r->entries.size() : -1;
+}
+
+int ns2vc_check_packed(int kind, const void* handle, int i, char* name, int name_len, int* Npad, int* nkb, int* n_logical, int* nvec,
+                       void* hi_out, void* lo_out, ns2vc_stream stream) {
+  const PackedRecord* r = packed_record(kind, handle);
+  if (!r) return -1;
+  NS_REQUIRE(i >= 0 && i < (int)r->entries.size(), "check_packed: operand %d out of range (%d recorded)", i, (int)r->entries.size());
+  const PackedRecord::Entry& e = r->entries[i];
+  int rc = copy_name(e.name, name, name_len);
+  if (rc) return rc;
+  if (Npad) *Npad = e.pb.Npad;
+  if (nkb) *nkb = e.pb.nkb;
+  if (n_logical) *n_logical = e.pb.n_logical;
+  if (nvec) *nvec = (int)e.vecs.size();
+  const size_t bytes = (size_t)e.pb.nkb * e.pb.Npad * 64 * sizeof(__nv_bfloat16);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (hi_out && bytes) NS_CHECK_CUDA(cudaMemcpyAsync(hi_out, e.pb.hi, bytes, cudaMemcpyDeviceToDevice, st));
+  if (lo_out && bytes) NS_CHECK_CUDA(cudaMemcpyAsync(lo_out, e.pb.lo, bytes, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+int ns2vc_check_fold_vector(int kind, const void* handle, int i, int j, char* name, int name_len, long long* n, float* out,
+                            ns2vc_stream stream) {
+  const PackedRecord* r = packed_record(kind, handle);
+  if (!r) return -1;
+  NS_REQUIRE(i >= 0 && i < (int)r->entries.size(), "check_fold_vector: operand %d out of range (%d recorded)", i, (int)r->entries.size());
+  const PackedRecord::Entry& e = r->entries[i];
+  NS_REQUIRE(j >= 0 && j < (int)e.vecs.size(), "check_fold_vector: vector %d of %s out of range (%d recorded)", j, e.name.c_str(), (int)e.vecs.size());
+  const PackedRecord::Vec& v = e.vecs[j];
+  int rc = copy_name(v.name, name, name_len);
+  if (rc) return rc;
+  if (n) *n = v.n;
+  if (out && v.n) NS_CHECK_CUDA(cudaMemcpyAsync(out, v.p, (size_t)v.n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return 0;
 }
 

@@ -58,6 +58,10 @@ struct ns2vc_pre : SingleProgramEngine {
   PoolKV ref_kv;                                       // ref_enc.pool k_proj | v_proj as one [2R, R] operator
 };
 
+namespace ns2vc {
+const EngineBase* engine_base(const ns2vc_pre* h) { return h; }
+}  // namespace ns2vc
+
 namespace {
 
 // reference parameter names / shapes (model.py:98-127, 156-172; operations.py:784-797, 304-340, 644-663)
@@ -108,6 +112,7 @@ int pack_encoder(ns2vc_pre* h, EncSite& e, const std::string& p, int cin, int H,
     if ((rc = launch_tbc_weight(w, 1, cin, H, wt, st))) return rc;
     if ((rc = mem.alloc_packed(e.pre, H, H, nkb_of(cin), h->simt))) return rc;
     if ((rc = pack_seg(e.pre, wt, H, cin, 1, 0, 0, cin, 0, 0, 0, st))) return rc;
+    h->packed.add(p + ".pre", e.pre);
   }
   for (int i = 0; i < L; ++i) {
     const std::string b = p + ".layers." + std::to_string(i) + ".op";
@@ -136,6 +141,11 @@ int pack_encoder(ns2vc_pre* h, EncSite& e, const std::string& p, int cin, int H,
     const float* w2 = need(b + ".ffn.ffn_2.weight"); if (!w2) return -1;
     if ((rc = mem.alloc_packed(ls.ffn2, H, H, nkb_of(F), h->simt))) return rc;
     if ((rc = pack_seg(ls.ffn2, w2, H, F, 1, 0, 0, F, 0, 0, 0, st))) return rc;
+    const std::string site = p + ".layers." + std::to_string(i);
+    h->packed.add(site + ".qkv", ls.qkv, {{"g_qkv", ls.g_qkv, 3 * H}, {"bf_qkv", ls.bf_qkv, 3 * H}});
+    h->packed.add(site + ".out", ls.out);
+    h->packed.add(site + ".ffn1", ls.ffn1, {{"b_ffn1", ls.b_ffn1, F}});
+    h->packed.add(site + ".ffn2", ls.ffn2);
     e.layers.push_back(ls);
   }
   // out_proj: LayerNorm folded into the k=1 ConvTBC
@@ -149,6 +159,7 @@ int pack_encoder(ns2vc_pre* h, EncSite& e, const std::string& p, int cin, int H,
     if ((rc = pack_seg(e.outp, wt, cout, H, 1, 0, 0, H, 0, 0, 0, st, go))) return rc;
     if (!(e.g_out = mem.alloc<float>((size_t)cout)) || !(e.bf_out = mem.alloc<float>((size_t)cout))) return -2;
     if ((rc = launch_ln_fold_vec(wt, go, bo, cb, e.g_out, e.bf_out, cout, H, st))) return rc;
+    h->packed.add(p + ".out_proj", e.outp, {{"g_out", e.g_out, cout}, {"bf_out", e.bf_out, cout}});
   }
   return 0;
 }
@@ -158,7 +169,9 @@ int pack(ns2vc_pre* h, cudaStream_t st) {
   int rc;
   if ((rc = pack_encoder(h, h->phone, "phoneme_encoder", c.phone_in, c.phone_hidden, c.phone_out, c.phone_layers, true, st))) return rc;
   if ((rc = pack_encoder(h, h->prompt, "prompt_encoder", c.prompt_in, c.prompt_hidden, c.prompt_out, c.prompt_layers, false, st))) return rc;
-  return concat_pool_kv(h->mem, h->weights, "ref_enc.pool", c.ref_dim, h->ref_kv, st);
+  if ((rc = concat_pool_kv(h->mem, h->weights, "ref_enc.pool", c.ref_dim, h->ref_kv, st))) return rc;
+  h->packed.add("ref_enc.pool.kv", PackedB{}, {{"W", h->ref_kv.W, 2LL * c.ref_dim * c.ref_dim}, {"b", h->ref_kv.b, 2LL * c.ref_dim}});
+  return 0;
 }
 
 // The call arguments of one encoder: its lengths, its [B, C, T] input and its [B, T, C_out] output.

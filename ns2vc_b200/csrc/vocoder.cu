@@ -340,6 +340,10 @@ struct ns2vc_voc : SingleProgramEngine {
   size_t istft_smem = 0;
 };
 
+namespace ns2vc {
+const EngineBase* engine_base(const ns2vc_voc* h) { return h; }
+}  // namespace ns2vc
+
 namespace {
 
 std::string blk(int i) { return "backbone.convnext." + std::to_string(i); }
@@ -371,6 +375,7 @@ int pack(ns2vc_voc* h, cudaStream_t st) {
   if ((rc = mem.alloc_packed(h->embed, D, D, kTaps * nkb_of(cin), false))) return rc;
   for (int j = 0; j < kTaps; ++j)
     if ((rc = pack_seg(h->embed, w.W("backbone.embed.weight"), D, cin, kTaps, j, 0, cin, 0, j * nkb_of(cin), 0, st))) return rc;
+  h->packed.add("backbone.embed", h->embed);
   h->pw1.assign(c.num_layers, PackedB()); h->pw2.assign(c.num_layers, PackedB());
   h->b2.assign(c.num_layers, nullptr); h->dw.assign(c.num_layers, nullptr);
   float* scaled = c.num_layers ? mem.alloc<float>((size_t)D * F) : nullptr;   // scratch: gamma * W2 of one block at a time (stream order)
@@ -385,6 +390,8 @@ int pack(ns2vc_voc* h, cudaStream_t st) {
     NS_VOC_LAUNCH_CHECK();
     if ((rc = mem.alloc_packed(h->pw2[i], D, D, nkb_of(F), false))) return rc;
     if ((rc = pack_seg(h->pw2[i], scaled, D, F, 1, 0, 0, F, 0, 0, 0, st))) return rc;
+    h->packed.add(p + ".pw1", h->pw1[i]);
+    h->packed.add(p + ".pw2", h->pw2[i], {{"bias", h->b2[i], D}});
     float* d = h->dw[i] = mem.alloc<float>((size_t)D * 8);
     if (!d) return -2;
     NS_CHECK_CUDA(cudaMemcpy2DAsync(d, 8 * sizeof(float), w.W(p + ".dwconv.weight"), kTaps * sizeof(float), kTaps * sizeof(float), D,
@@ -394,6 +401,7 @@ int pack(ns2vc_voc* h, cudaStream_t st) {
   }
   if ((rc = mem.alloc_packed(h->head, c.n_fft + 2, c.n_fft + 2, nkb_of(D), false))) return rc;
   if ((rc = pack_seg(h->head, w.W("head.out.weight"), c.n_fft + 2, D, 1, 0, 0, D, 0, 0, 0, st))) return rc;
+  h->packed.add("head.out", h->head);
   std::vector<float2> th, tf;
   istft_twiddles(c.n_fft, th, tf);
   if (!(h->tw_half = mem.alloc<float2>(th.size())) || !(h->tw_full = mem.alloc<float2>(tf.size()))) return -2;
