@@ -286,6 +286,8 @@ int ns2vc_pre_num_weights(const ns2vc_pre* h);                                  
 int ns2vc_pre_weight_info(const ns2vc_pre* h, int i, const char** name, int64_t shape[4], int* ndim);
 int ns2vc_pre_load_weight(ns2vc_pre* h, const char* key, const float* dptr, const int64_t* shape, int ndim, ns2vc_stream stream);
 int ns2vc_pre_finalize(ns2vc_pre* h, ns2vc_stream stream);                      /* strict: fails on a missing key                   */
+/* One size serves every program of the handle at (B, T, S): ns2vc_pre_infer, _infer_ragged, _encode_voices_ragged of (B, S) and
+ * _infer_content_ragged of (B, T). */
 int ns2vc_pre_workspace_bytes(const ns2vc_pre* h, int B, int T, int S, size_t* bytes);
 /* Pre_model.infer:
  *   c [B, phone_in, T] fp32, refer [B, prompt_in, S] fp32 (contiguous), lengths / refer_lengths [B] int64 (device, each >= 1)
@@ -298,11 +300,24 @@ int ns2vc_pre_infer(ns2vc_pre* h, const float* c, const float* refer, const int6
  * never read.  A second program per (B, T, S, workspace); the workspace size above serves both. */
 int ns2vc_pre_infer_ragged(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths,
                            float* content, float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream);
+/* The ragged program in two halves, so that a target voice is encoded once and reused with any content:
+ * the voice half reads refer [B, prompt_in, S] and refer_lengths [B] (S_b in [1, S]) and writes
+ *   spk [B, phone_hidden]           phoneme_encoder.spk_proj(ref_enc(refer)), the one vector by which the voice enters the content,
+ *   prompt [B, S, prompt_out]        the prompt encoder's output, exactly 0 past S_b;
+ * the content half reads c [B, phone_in, T], lengths [B] (T_b in [1, T]) and row b's speaker vector spk[b] and writes
+ *   content [B, T, phone_out]        exactly 0 past T_b.
+ * Row b of each equals, byte for byte, the same row of ns2vc_pre_infer_ragged on that prompt and content: both halves are its
+ * launches, split after spk_proj.  Each is one more program per shape and workspace (size: ns2vc_pre_workspace_bytes above), and
+ * each zeroes its own LayerNorm statistics, so their launch counts add up to ns2vc_pre_infer_ragged's plus one. */
+int ns2vc_pre_encode_voices_ragged(ns2vc_pre* h, const float* refer, const int64_t* refer_lengths, float* spk, float* prompt, int B, int S,
+                                   void* ws, ns2vc_stream stream);
+int ns2vc_pre_infer_content_ragged(ns2vc_pre* h, const float* c, const int64_t* lengths, const float* spk, float* content, int B, int T,
+                                   void* ws, ns2vc_stream stream);
 /* Diagnostics for the parity tests: per-layer activations (token-major [B, rows, channels]; rows = 1 for the speaker vector). */
 int ns2vc_pre_num_taps(const ns2vc_pre* h);
 int ns2vc_pre_tap_info(const ns2vc_pre* h, int i, const char** name, int* rows, int* channels);
 int ns2vc_pre_set_tap(ns2vc_pre* h, int i, float* dst);
-int ns2vc_pre_launch_count(const ns2vc_pre* h);   /* kernels launched by the last infer */
+int ns2vc_pre_launch_count(const ns2vc_pre* h);   /* kernels launched by the last call of any of the four programs */
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Prompt-mel front end: the recipe of reference inference/infer_tool.py:170-181 (and preprocess.py:27-31, 49-59) per

@@ -122,6 +122,8 @@ SIGNATURES = {
     "ns2vc_pre_workspace_bytes": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "ns2vc_pre_infer": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "ns2vc_pre_infer_ragged": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_pre_encode_voices_ragged": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "ns2vc_pre_infer_content_ragged": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
     "ns2vc_pre_num_taps": (C.c_int, [_P]),
     "ns2vc_pre_tap_info": (C.c_int, [_P, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ns2vc_pre_set_tap": (C.c_int, [_P, C.c_int, _P]),

@@ -196,6 +196,27 @@ def decode_utterances(vocoder, latents: Sequence[torch.Tensor], max_batch: int =
     return out
 
 
+@torch.no_grad()
+def encode_voices(pre_model, mels: Sequence[torch.Tensor], max_batch: int = 8) -> list:
+    """Encodes target voices once for reuse: each prompt mel [100, S_v] of ``mels`` goes through ``pre_model.encode_voices`` in
+    ragged batches of at most ``max_batch`` (longest first), and one ``pre_model.Voice`` per mel is returned in input order.
+    The conversion entry points take a ``Voice`` wherever they take a prompt mel, and skip the voice's encoders."""
+    from .pre_model import REF_DIM
+    for k, m in enumerate(mels):
+        if not isinstance(m, torch.Tensor) or m.dim() != 2 or m.shape[0] != REF_DIM or m.shape[1] < 1:
+            raise ValueError(f"mel {k}: expected a mel [{REF_DIM}, S_v] with S_v >= 1, got {tuple(getattr(m, 'shape', ()))}")
+    dev = next(pre_model.parameters()).device
+    out: list = [None] * len(mels)
+    for idx in batch_plan([int(m.shape[1]) for m in mels], max_batch):
+        sl = [int(mels[i].shape[1]) for i in idx]
+        refer = torch.zeros((len(idx), REF_DIM, max(sl)), dtype=torch.float32, device=dev)
+        for j, i in enumerate(idx):
+            refer[j, :, :sl[j]] = mels[i]
+        for i, v in zip(idx, pre_model.encode_voices(refer, torch.tensor(sl, dtype=torch.int64))):
+            out[i] = v
+    return out
+
+
 def content_utterances(model, wavs16k: Sequence[torch.Tensor], target_frames: Optional[Sequence[int]] = None,
                        max_batch: int = 8) -> List[torch.Tensor]:
     """Content units of a list of 1-D 16 kHz waveforms of different lengths with a ``content.ContentVec``, in ragged batches of

@@ -7,7 +7,8 @@ Per utterance the chain is ``Svc.get_unit_f0_code`` + ``NaturalSpeech2.sample``:
 2. T = N24 // 256, the frame count of ``compute_f0_parselmouth`` (``utils.py:159-160``).  f0 itself is not read by the model
    (``model.py:349-375``) and the transposition only scales f0, so neither enters here;
 3. resample 24 -> 16 kHz, ContentVec units (``content.ContentVec.extract``), stretched to T frames (``repeat_expand_2d``);
-4. the condition encoders (``Pre_model.infer(per_utterance=True)``);
+4. the condition encoders (``Pre_model.infer(per_utterance=True)``), as its two halves: the prompt mel's ``Pre_model.encode_voices``
+   and the units' ``Pre_model.infer_content``, so that a prompt given as an encoded ``Voice`` is not encoded again;
 5. UniPC (30 steps, what ``Svc.infer`` runs) or DPM-Solver++ (40 steps) from x_T ~ N(0, 1) [1, 100, T];
 6. the vocoder (``Vocos.decode``): T * 256 samples at 24 kHz.
 
@@ -26,8 +27,9 @@ import torch
 import torch.distributed as dist
 
 from . import frontend, shard
-from .api import batch_plan, sample_latents
+from .api import batch_plan, encode_voices, sample_latents
 from .content import MIN_SAMPLES, num_frames
+from .pre_model import Voice
 
 TARGET_SR = 24000        # config data.sampling_rate: the rate of the converted audio
 HOP = 256                # config data.hop_length
@@ -53,6 +55,28 @@ def _check_method(method: str, steps: Optional[int]) -> int:
     return DEFAULT_STEPS[method] if steps is None else int(steps)
 
 
+def prompt_frames(p) -> int:
+    """S_b of a prompt: a mel [100, S_b] or a ``Voice``."""
+    return p.S_v if isinstance(p, Voice) else int(p.shape[1])
+
+
+def check_voices(pre_model, prompts, dev: torch.device) -> None:
+    """ValueError unless every ``Voice`` among ``prompts`` was encoded by ``pre_model`` on ``dev``."""
+    for k, p in enumerate(prompts):
+        if isinstance(p, Voice):
+            pre_model.check_voice(p, dev, f"prompt {k}")
+
+
+class FrontCache:
+    """What the encoders computed during one conversion call, keyed by the identity of its input tensors: the units and
+    stretched units of each waveform, and the ``Voice`` of each prompt mel.  Rows that repeat a waveform or a mel object share
+    them.  The call holds every input it was given, so no identity is reused while the cache lives."""
+
+    def __init__(self) -> None:
+        self.units: Dict[int, Tuple[torch.Tensor, torch.Tensor]] = {}
+        self.voices: Dict[int, Voice] = {}
+
+
 def _check_inputs(wavs: Sequence[torch.Tensor], sr: int, prompt, x_T) -> List[Dict[str, int]]:
     if len(wavs) == 0:
         raise ValueError("wavs is empty")
@@ -71,8 +95,10 @@ def _check_inputs(wavs: Sequence[torch.Tensor], sr: int, prompt, x_T) -> List[Di
     if len(prompts) != len(wavs):
         raise ValueError(f"{len(prompts)} prompts for {len(wavs)} waveforms")
     for k, p in enumerate(prompts):
-        if p.dim() != 2 or p.shape[0] != LATENT_CH or p.shape[1] < 1:
-            raise ValueError(f"prompt {k}: expected a mel [{LATENT_CH}, S], got {tuple(p.shape)}")
+        if isinstance(p, Voice):
+            continue
+        if not isinstance(p, torch.Tensor) or p.dim() != 2 or p.shape[0] != LATENT_CH or p.shape[1] < 1:
+            raise ValueError(f"prompt {k}: expected a mel [{LATENT_CH}, S] or a Voice, got {tuple(getattr(p, 'shape', ()))}")
     if x_T is not None:
         if len(x_T) != len(wavs):
             raise ValueError(f"{len(x_T)} x_T tensors for {len(wavs)} waveforms")
@@ -83,18 +109,21 @@ def _check_inputs(wavs: Sequence[torch.Tensor], sr: int, prompt, x_T) -> List[Di
 
 
 @torch.no_grad()
-def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence[torch.Tensor],
-                  x_T: Sequence[torch.Tensor], method: str = "unipc", steps: Optional[int] = None) -> Dict[str, List[torch.Tensor]]:
-    """Converts ``wavs`` (1-D, at ``sr``) as ONE ragged batch, each with its prompt mel [100, S_b] and x_T [1, 100, T_b], and returns
-    every stage per utterance, unpadded: ``units`` [D, units_b], ``c`` [D, T_b] (stretched), ``content`` [T_b, C], ``prompt``
-    [S_b, C] (the encoders' outputs), ``latent`` [100, T_b] and ``audio`` [T_b * 256]."""
+def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence,
+                  x_T: Sequence[torch.Tensor], method: str = "unipc", steps: Optional[int] = None,
+                  cache: Optional[FrontCache] = None) -> Dict[str, List[torch.Tensor]]:
+    """Converts ``wavs`` (1-D, at ``sr``) as ONE ragged batch, each with its prompt (a mel [100, S_b] or a ``Voice``) and x_T
+    [1, 100, T_b], and returns every stage per utterance, unpadded: ``units`` [D, units_b], ``c`` [D, T_b] (stretched), ``content``
+    [T_b, C], ``prompt`` [S_b, C] (the encoders' outputs), ``latent`` [100, T_b] and ``audio`` [T_b * 256].  ``cache``: see
+    ``encode_front``."""
     steps = _check_method(method, steps)
     plans = _check_inputs(wavs, sr, list(prompts), list(x_T))
     dev = next(unet.parameters()).device
+    check_voices(pre_model, prompts, dev)
     B = len(wavs)
-    front = encode_front(content_model, pre_model, wavs, sr, prompts, plans, dev)
+    front = encode_front(content_model, pre_model, wavs, sr, prompts, plans, dev, cache)
     tl, content, prompt = front["tl"], front["content"], front["prompt"]
-    sl = [int(p.shape[1]) for p in prompts]
+    sl = [prompt_frames(p) for p in prompts]
     T = max(tl)
     tl_h, sl_h = torch.tensor(tl, dtype=torch.int64), torch.tensor(sl, dtype=torch.int64)
     x = torch.zeros((B, LATENT_CH, T), dtype=torch.float32, device=dev)
@@ -107,47 +136,69 @@ def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.
                 audio=[audio[j, :tl[j] * HOP] for j in range(B)])
 
 
+def _first_rows(xs: Sequence, known: Dict[int, object]) -> List[int]:
+    """The first row of each distinct object of ``xs`` (by identity) that ``known`` does not hold yet."""
+    first: Dict[int, int] = {}
+    for j, x in enumerate(xs):
+        if id(x) not in known and id(x) not in first:
+            first[id(x)] = j
+    return list(first.values())
+
+
 @torch.no_grad()
-def encode_front(content_model, pre_model, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence[torch.Tensor],
-                 plans: Sequence[Dict[str, int]], dev: torch.device) -> Dict[str, object]:
+def encode_front(content_model, pre_model, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence,
+                 plans: Sequence[Dict[str, int]], dev: torch.device, cache: Optional[FrontCache] = None) -> Dict[str, object]:
     """The encoders in front of the sampler, on ``wavs`` (checked by ``_check_inputs``, which gave ``plans``) as ONE ragged batch:
-    resampling, ContentVec, ``repeat_expand_2d`` and ``Pre_model.infer(per_utterance=True)``.  Returns ``units`` and ``c`` per
-    utterance, the frame counts ``tl``, and the encoders' padded outputs ``content`` [T, B, C] and ``prompt`` [S, B, C]."""
+    resampling, ContentVec and ``repeat_expand_2d`` once per distinct waveform, ``Pre_model.encode_voices`` once per distinct
+    prompt mel (a ``Voice`` is used as it is), then ``Pre_model.infer_content`` on every row.  Waveforms and mels are matched by
+    tensor identity, within the call and with what ``cache`` (a ``FrontCache``, which this call extends) already holds.  Each
+    row equals ``Pre_model.infer(per_utterance=True)`` on it.  Returns ``units`` and ``c`` per utterance, the frame counts
+    ``tl``, and the encoders' padded outputs ``content`` [T, B, C] and ``prompt`` [S, B, C]."""
+    cache = FrontCache() if cache is None else cache
     B = len(wavs)
-    n = [int(w.shape[0]) for w in wavs]
-    n24, tl = [p["n24"] for p in plans], [p["T"] for p in plans]
-    n16, nu = [p["n16"] for p in plans], [p["units"] for p in plans]
-    sl = [int(p.shape[1]) for p in prompts]
-    T, S = max(tl), max(sl)
-    wav = torch.zeros((B, max(n)), dtype=torch.float32, device=dev)
-    for j, w in enumerate(wavs):
-        wav[j, :n[j]] = w.to(dev, torch.float32)
-    w24, _ = frontend.resample(wav, sr, TARGET_SR, torch.tensor(n, dtype=torch.int64))
-    w16, _ = frontend.resample(w24, TARGET_SR, CONTENT_SR, torch.tensor(n24, dtype=torch.int64))
-    units_all, _ = content_model.extract(w16, torch.tensor(n16, dtype=torch.int64))
-    D = units_all.shape[2]
-    units = [units_all[j, :nu[j]].t() for j in range(B)]
-    c = torch.zeros((B, D, T), dtype=torch.float32, device=dev)
-    cs = []
+    tl = [p["T"] for p in plans]
+    todo = _first_rows(wavs, cache.units)
+    if todo:
+        n = [int(wavs[j].shape[0]) for j in todo]
+        n24, n16, nu = ([plans[j][k] for j in todo] for k in ("n24", "n16", "units"))
+        wav = torch.zeros((len(todo), max(n)), dtype=torch.float32, device=dev)
+        for i, j in enumerate(todo):
+            wav[i, :n[i]] = wavs[j].to(dev, torch.float32)
+        w24, _ = frontend.resample(wav, sr, TARGET_SR, torch.tensor(n, dtype=torch.int64))
+        w16, _ = frontend.resample(w24, TARGET_SR, CONTENT_SR, torch.tensor(n24, dtype=torch.int64))
+        units_all, _ = content_model.extract(w16, torch.tensor(n16, dtype=torch.int64))
+        for i, j in enumerate(todo):
+            u = units_all[i, :nu[i]].t()
+            cache.units[id(wavs[j])] = (u, frontend.repeat_expand_2d(u, tl[j]))
+    mels = [p for p in prompts if not isinstance(p, Voice)]
+    todo = _first_rows(mels, cache.voices)
+    for j, v in zip(todo, encode_voices(pre_model, [mels[j] for j in todo], max_batch=max(len(todo), 1))):
+        cache.voices[id(mels[j])] = v
+    voices = [p if isinstance(p, Voice) else cache.voices[id(p)] for p in prompts]
+    units = [cache.units[id(w)][0] for w in wavs]
+    cs = [cache.units[id(w)][1] for w in wavs]
+    T, S = max(tl), max(v.S_v for v in voices)
+    c = torch.zeros((B, cs[0].shape[0], T), dtype=torch.float32, device=dev)
     for j in range(B):
-        cs.append(frontend.repeat_expand_2d(units[j], tl[j]))
         c[j, :, :tl[j]] = cs[j]
-    refer = torch.zeros((B, LATENT_CH, S), dtype=torch.float32, device=dev)
-    for j, p in enumerate(prompts):
-        refer[j, :, :sl[j]] = p.to(dev, torch.float32)
-    tl_h, sl_h = torch.tensor(tl, dtype=torch.int64), torch.tensor(sl, dtype=torch.int64)
-    content, prompt = pre_model.infer((c, refer, None, None, None, tl_h, sl_h, None), per_utterance=True)
+    content = pre_model.infer_content(c, torch.tensor(tl, dtype=torch.int64), voices)
+    prompt = torch.zeros((S, B, voices[0].prompt.shape[1]), dtype=torch.float32, device=dev)
+    for j, v in enumerate(voices):
+        prompt[:v.S_v, j] = v.prompt
     return dict(units=units, c=cs, tl=tl, content=content, prompt=prompt)
 
 
 @torch.no_grad()
 def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int,
-                       prompt: Union[torch.Tensor, Sequence[torch.Tensor]], method: str = "unipc", steps: Optional[int] = None,
+                       prompt: Union[torch.Tensor, Voice, Sequence], method: str = "unipc", steps: Optional[int] = None,
                        max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None,
                        group: Optional[dist.ProcessGroup] = None) -> List[torch.Tensor]:
-    """Converts 1-D float32 waveforms at ``sr`` with one prompt mel [100, S] (or one per waveform) and returns one 24 kHz
-    waveform [T_b * 256] per input, in input order, T_b = resample_out_length(sr, 24000, len) // 256.  The waveforms run in
-    ragged batches of at most ``max_batch`` (longest first); each result equals that waveform converted alone.
+    """Converts 1-D float32 waveforms at ``sr`` with one prompt (or one per waveform) and returns one 24 kHz waveform
+    [T_b * 256] per input, in input order, T_b = resample_out_length(sr, 24000, len) // 256.  The waveforms run in ragged
+    batches of at most ``max_batch`` (longest first); each result equals that waveform converted alone.
+
+    A prompt is a mel [100, S] or a ``Voice`` from ``api.encode_voices``.  Each distinct mel (by tensor identity) is encoded
+    once per call, and each distinct waveform object goes through ContentVec once per call, whichever batches it lands in.
 
     ``x_T`` (one [1, 100, T_b] per waveform) defaults to ``torch.randn((1, 100, T_b), device=dev)`` drawn per waveform in input
     order before any batching: the shape and order in which ``Svc.infer`` draws it once per slice (``model.py:633-635``), so after
@@ -160,14 +211,16 @@ def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[t
     plans = _check_inputs(wavs, sr, prompt, x_T)
     prompts = list(prompt) if isinstance(prompt, (list, tuple)) else [prompt] * len(wavs)
     dev = next(unet.parameters()).device
+    check_voices(pre_model, prompts, dev)
     if group is not None and dist.get_world_size(group) > 1:
         return _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts, plans, method, steps, max_batch, x_T, group, dev)
     if x_T is None:
         x_T = [torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans]
     out: List[Optional[torch.Tensor]] = [None] * len(wavs)
+    cache = FrontCache()
     for idx in batch_plan([int(w.shape[0]) for w in wavs], max_batch):
         r = convert_batch(content_model, pre_model, unet, vocoder, [wavs[i] for i in idx], sr, [prompts[i] for i in idx],
-                          [x_T[i] for i in idx], method, steps)
+                          [x_T[i] for i in idx], method, steps, cache)
         for j, i in enumerate(idx):
             out[i] = r["audio"][j]
     return out
@@ -182,13 +235,14 @@ def _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts,
     the x_T of the one-GPU call and every rank's generator ends where that call leaves it.  The ranks' CUDA generators must
     therefore start equal, which one all-gather of their seed and offset checks first."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
-    plan = shard.plan_batches(plans, [int(p.shape[1]) for p in prompts], world, max_batch)
+    plan = shard.plan_batches(plans, [prompt_frames(p) for p in prompts], world, max_batch)
     if x_T is None:
         shard.check_generator(torch.cuda.default_generators[dev.index], group, dev)
         mine = {i for b in plan[rank] for i in b}
         x_T = [x if i in mine else None for i, x in enumerate([torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans])]
+    cache = FrontCache()
     return shard.run_sharded(lambda idx: convert_batch(content_model, pre_model, unet, vocoder, [wavs[i] for i in idx], sr,
-                                                       [prompts[i] for i in idx], [x_T[i] for i in idx], method, steps)["audio"],
+                                                       [prompts[i] for i in idx], [x_T[i] for i in idx], method, steps, cache)["audio"],
                              plan, [p["T"] * HOP for p in plans], group, dev)
 
 
@@ -260,12 +314,12 @@ def stitch(audio_data, audio_sr: int, converted: Sequence[np.ndarray], pad_secon
 
 
 @torch.no_grad()
-def convert_slices(content_model, pre_model, unet, vocoder, audio_data, audio_sr: int, prompt: torch.Tensor, pad_seconds: float = 0.5,
+def convert_slices(content_model, pre_model, unet, vocoder, audio_data, audio_sr: int, prompt: Union[torch.Tensor, Voice], pad_seconds: float = 0.5,
                    clip_seconds: float = 0, linear_gradient: float = 0, linear_gradient_retain: float = 0.75, method: str = "unipc",
                    steps: Optional[int] = None, max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None,
                    group: Optional[dist.ProcessGroup] = None) -> np.ndarray:
     """Converts one file given as ``slicer.chunks2audio``'s list of (is_silence, samples) at ``audio_sr`` with one prompt mel
-    [100, S] and returns the float64 24 kHz array ``infer.py`` writes for it.  Every voice sub-slice goes through one
+    [100, S] (or a ``Voice``) and returns the float64 24 kHz array ``infer.py`` writes for it.  Every voice sub-slice goes through one
     ``convert_utterances`` call (``x_T``, if given, holds one tensor per sub-slice in order); stitching is ``stitch``.  With a
     ``group`` of more than one rank, the sub-slices are shared out over its ranks and every rank returns the stitched file."""
     _check_method(method, steps)
@@ -324,9 +378,11 @@ def convert_files(content_model, pre_model, unet, vocoder, files: Sequence[Tuple
     ``files`` are ``(wav, sr)`` pairs of 1-D float32 samples (as ``librosa.load(sr=None)`` returns them); each is cut at its
     silences by ``slicer.cut_batch`` (``slice_db``, min_len 5000 ms, as ``infer.py:83`` calls ``slicer.cut``; one RMS launch for
     all files) and split into voice sub-slices as ``convert_slices`` does.  ``voices`` are ``(wav, sr)`` reference recordings
-    (1-D, or [channels, N] of which channel 0 is used); their prompt mels come from ``voice_mels``.  Every (file, voice,
-    sub-slice) item of one input rate goes through ONE ``convert_utterances`` call, so the slices of different files and voices
-    share ragged batches (files at several rates take one call per rate); each file is stitched per voice by ``stitch``.
+    (1-D, or [channels, N] of which channel 0 is used); their prompt mels come from ``voice_mels`` and are encoded once, by
+    ``api.encode_voices``.  Every (file, voice, sub-slice) item of one input rate goes through ONE ``convert_utterances`` call,
+    so the slices of different files and voices share ragged batches (files at several rates take one call per rate); the V
+    items of one sub-slice share its ContentVec units, which each rank computes once, for the sub-slices of its own batches.
+    Each file is stitched per voice by ``stitch``.
 
     ``x_T`` (``x_T[f][v]``: one [1, 100, T] per voice sub-slice of file f) defaults to ``torch.randn((1, 100, T))`` per item drawn
     in the CLI's order - file, then voice, then sub-slice - before any conversion, so after the same ``torch.manual_seed`` every
@@ -349,7 +405,7 @@ def convert_files(content_model, pre_model, unet, vocoder, files: Sequence[Tuple
     audio_data = [slicer.chunks2audio(w, c) for w, c in zip(wavs, chunks)]
     subs = [_plan_slices(a, sr, pad_seconds, clip_seconds, linear_gradient) for a, sr in zip(audio_data, srs)]
     sub_T = [[frame_plan(len(s), sr)["T"] for s in ss] for ss, sr in zip(subs, srs)]
-    mels = voice_mels(voices, dev)
+    encoded = encode_voices(pre_model, voice_mels(voices, dev), max_batch=max_batch)
     V = len(voices)
     if x_T is None:
         if group is not None and dist.get_world_size(group) > 1:
@@ -358,13 +414,13 @@ def convert_files(content_model, pre_model, unet, vocoder, files: Sequence[Tuple
     elif len(x_T) != len(files) or any(len(xf) != V or any(len(xv) != len(ss) for xv in xf) for xf, ss in zip(x_T, subs)):
         raise ValueError("x_T must hold x_T[f][v], one tensor per voice sub-slice of file f, for every file and voice")
     converted: Dict[Tuple[int, int], List[np.ndarray]] = {(f, v): [] for f in range(len(files)) for v in range(V)}
+    sources = [[torch.from_numpy(s.astype(np.float32)) for s in ss] for ss in subs]     # one tensor per sub-slice: its V items share it
     for sr in dict.fromkeys(srs):
         items = [(f, v, k) for f in range(len(files)) if srs[f] == sr for v in range(V) for k in range(len(subs[f]))]
         if not items:
             continue
-        outs = convert_utterances(content_model, pre_model, unet, vocoder,
-                                  [torch.from_numpy(subs[f][k].astype(np.float32)) for f, _, k in items], sr,
-                                  [mels[v] for _, v, _ in items], method=method, steps=steps, max_batch=max_batch,
+        outs = convert_utterances(content_model, pre_model, unet, vocoder, [sources[f][k] for f, _, k in items], sr,
+                                  [encoded[v] for _, v, _ in items], method=method, steps=steps, max_batch=max_batch,
                                   x_T=[x_T[f][v][k] for f, v, k in items], group=group)
         for (f, v, _), o in zip(items, outs):
             converted[(f, v)].append(o.cpu().numpy())

@@ -172,9 +172,11 @@ struct Launch {
   enum Input { NONE,
                X, T, OUT, CONTENT, PROMPT, MASK,                               // ns2vc_unet_prepare_cond / _forward
                C, REFER, LENGTHS, REFER_LENGTHS, CONTENT_OUT, PROMPT_OUT,      // ns2vc_pre_infer
+               SPK,                                                           // ns2vc_pre_encode_voices_ragged / _infer_content_ragged
                MEL,                                                           // ns2vc_voc_decode (+ LENGTHS)
                NUM_INPUTS                                                     // (ns2vc_cv_extract: OUT)
   } input = NONE;
+  Input input2 = NONE;       // a second call argument (the condition encoders' content program: ENC_INPUT's speaker rows, SPK)
   std::variant<std::monostate, GemmOp, AttnOp, LnOp, LinOp, NctSplitOp, TokensOp, PoolClsOp, PoolAttOp, MaskBiasOp, PrepOp, SeqMaskOp,
                VocNormOp, MemsetOp, CopyOp, VocLensOp, IstftOp, CvLensOp, CvGnStatsOp, CvConv0Op, CvPosWinOp, CvAddOp, SplitTapOp> op;
   int tap_index = -1;
@@ -189,9 +191,14 @@ struct Launch {
 struct CallArg { const void* p = nullptr; long long bstride = 0; };
 using CallArgs = std::array<CallArg, Launch::NUM_INPUTS>;
 
-// Puts the call argument `a` into the field of l's payload that reads it.
-inline int bind_input(Launch& l, const CallArg& a) {
+// Puts the call argument `a` (the one named `which`) into the field of l's payload that reads it.
+inline int bind_input(Launch& l, Launch::Input which, const CallArg& a) {
   float* p = (float*)a.p;
+  if (which == Launch::SPK) {     // the speaker rows [B, phone_hidden]: written by spk_proj, or added to the content encoder's input
+    if (l.kind == Launch::LINEAR) { l.get<LinOp>().out = p; return 0; }
+    if (l.kind == Launch::ENC_INPUT) { l.get<TokensOp>().rowbias = p; return 0; }
+    set_error("internal: launch kind %d reads no speaker rows", (int)l.kind); return -1;
+  }
   switch (l.kind) {
     case Launch::GEMM: l.get<GemmOp>().out = p; return 0;
     case Launch::ATTN: return 0;   // MASK: the denoiser drops the key-padding bias when its prepare_cond had no mask
@@ -472,9 +479,10 @@ inline int no_launcher(const Launch& l) {
 // The record to launch for `l`: `l` itself, or (when it reads a call argument) `tmp` holding a copy with the argument bound
 inline const Launch* bound(const Launch& l, const CallArgs& in, Launch& tmp, int& rc) {
   rc = 0;
-  if (l.input == Launch::NONE) return &l;
+  if (l.input == Launch::NONE && l.input2 == Launch::NONE) return &l;
   tmp = l;
-  rc = bind_input(tmp, in[l.input]);
+  if (l.input != Launch::NONE) rc = bind_input(tmp, l.input, in[l.input]);
+  if (!rc && l.input2 != Launch::NONE) rc = bind_input(tmp, l.input2, in[l.input2]);
   return &tmp;
 }
 

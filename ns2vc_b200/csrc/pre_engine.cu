@@ -174,8 +174,9 @@ int pack(ns2vc_pre* h, cudaStream_t st) {
   return 0;
 }
 
-// The call arguments of one encoder: its lengths, its [B, C, T] input and its [B, T, C_out] output.
-struct EncIo { Launch::Input lengths, in, out; };
+// The call arguments of one encoder: its lengths, its [B, C, T] input, its [B, T, C_out] output and (SPK or NONE) the speaker
+// rows added to its input when the call supplies them.
+struct EncIo { Launch::Input lengths, in, out, spk = Launch::NONE; };
 
 // One encoder over Tn frames.  `ragged`: LN2's split is 0 on rows past the entry's length, so the conv-FFN reads zeros there as
 // an unpadded run reads its zero padding.  `ilens`: where SEQMASK also writes the lengths as int [B], clamped to [1, Tn], or nullptr.
@@ -199,7 +200,7 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
   auto masked = [&](GemmOp& g) { g.flags |= EPI_ROWMASK; g.rowmask = keep; };
 
   bld.emit(Launch::SEQMASK, SeqMaskOp{nullptr, B, Tn, keep, kbias, ilens}, io.lengths);
-  bld.emit(Launch::ENC_INPUT, TokensOp{nullptr, 0, B, e.cin, Tn, X0, ldin, spk, keep}, io.in);
+  bld.emit(Launch::ENC_INPUT, TokensOp{nullptr, 0, B, e.cin, Tn, X0, ldin, spk, keep}, io.in).input2 = io.spk;
   bld.emit_ln_split(X0, ldin, (int)M, e.cin, w.W(e.p + ".pre.layer_norm.weight"), w.W(e.p + ".pre.layer_norm.bias"), s_in);
   double* rs = new_rowstats();
   { GemmOp g = bld.lin(e.pre, s_in, Tn);
@@ -253,10 +254,24 @@ void build_encoder(ns2vc_pre* h, ProgramBuilder& bld, TapSet& taps, const EncSit
 // `ragged`: row b is the utterance c[b, :, :T_b], refer[b, :, :S_b] encoded alone (ns2vc_pre_infer_ragged).  Besides the masked
 // LN2 splits, ref_enc pools over each entry's 1 + S_b tokens; the prompt encoder runs first so that its SEQMASK launch writes the
 // int prompt lengths ref_enc reads.  Same launches as the padded program.
+// The two halves of the ragged program, each the same launches as its part of it:
+//   T = 0: the voice program (ns2vc_pre_encode_voices_ragged): prompt encoder, ref_enc and spk_proj, which writes the call's SPK;
+//   S = 0: the content program (ns2vc_pre_infer_content_ragged): the phone encoder, whose input adds the call's SPK rows.
+// Each half zeroes its own LayerNorm statistics, so their launch counts add up to the ragged program's plus one memset.
+int finish_program(ns2vc_pre* h, const ProgramBuilder& bld, std::vector<Launch> prog, TapSet taps, size_t* bytes_out) {
+  if (bld.err) return bld.err;
+  if (bytes_out) *bytes_out = bld.ar.off + 256;
+  if (!bld.dry) {
+    h->cp.prog = std::move(prog);
+    h->cp.taps = std::move(taps);
+  }
+  return 0;
+}
+
 int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size_t* bytes_out) {
   const ns2vc_pre_cfg& c = h->cfg;
   const bool dry = ws == nullptr;
-  NS_REQUIRE(B >= 1 && T >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
+  NS_REQUIRE(B >= 1 && T >= 0 && S >= 0 && T + S >= 1 && (ragged || (T >= 1 && S >= 1)), "bad shape B=%d T=%d S=%d", B, T, S);
   std::vector<Launch> prog;
   TapSet taps;
   ProgramBuilder bld{Arena{(uint8_t*)ws, 0}, B, dry, h->simt, &prog};
@@ -266,6 +281,10 @@ int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size
   double* stat_arena = ar.get<double>(stat_doubles);
   double* stat_cur = stat_arena;
   bld.emit_memset(stat_arena, stat_doubles * sizeof(double));
+  if (S == 0) {
+    build_encoder(h, bld, taps, h->phone, T, {Launch::LENGTHS, Launch::C, Launch::CONTENT_OUT, Launch::SPK}, nullptr, stat_cur, true, nullptr);
+    return finish_program(h, bld, std::move(prog), std::move(taps), bytes_out);
+  }
   int* plens = ragged ? ar.get<int>(B) : nullptr;
   if (ragged) build_encoder(h, bld, taps, h->prompt, S, {Launch::REFER_LENGTHS, Launch::REFER, Launch::PROMPT_OUT}, nullptr, stat_cur, true, plens);
   // ---- ref_enc: TextTimeEmbedding over ALL S prompt frames (the reference does not mask them: model.py:362), or S_b when ragged
@@ -280,26 +299,20 @@ int build_program(ns2vc_pre* h, int B, int T, int S, bool ragged, void* ws, size
   bld.emit_tap(taps, "ref_enc", g, 1, R, 1);
   // spk_proj: Conv1d(100, hidden, 1) on g [B, 100, 1] (model.py:123, 127)
   bld.emit_linear(linear_op(g, R, B, R, h->weights.W("phoneme_encoder.spk_proj.weight"), h->weights.W("phoneme_encoder.spk_proj.bias"),
-                            c.phone_hidden, spk, c.phone_hidden));
+                            c.phone_hidden, spk, c.phone_hidden), T == 0 ? Launch::SPK : Launch::NONE);
   if (!ragged) build_encoder(h, bld, taps, h->prompt, S, {Launch::REFER_LENGTHS, Launch::REFER, Launch::PROMPT_OUT}, nullptr, stat_cur, false, nullptr);
-  build_encoder(h, bld, taps, h->phone, T, {Launch::LENGTHS, Launch::C, Launch::CONTENT_OUT}, spk, stat_cur, ragged, nullptr);
-  if (bld.err) return bld.err;
-  if (bytes_out) *bytes_out = ar.off + 256;
-  if (!dry) {
-    h->cp.prog = std::move(prog);
-    h->cp.taps = std::move(taps);
-  }
-  return 0;
+  if (T > 0) build_encoder(h, bld, taps, h->phone, T, {Launch::LENGTHS, Launch::C, Launch::CONTENT_OUT}, spk, stat_cur, ragged, nullptr);
+  return finish_program(h, bld, std::move(prog), std::move(taps), bytes_out);
 }
 
 int run_program(ns2vc_pre* h, const float* c, const float* refer, const long long* lengths, const long long* refer_lengths, float* content,
-                float* prompt, cudaStream_t st) {
+                float* prompt, float* spk, cudaStream_t st) {
   const int T = h->cp.dims[1], S = h->cp.dims[2];
   CallArgs in{};
   in[Launch::C] = {c, (long long)h->cfg.phone_in * T};
   in[Launch::REFER] = {refer, (long long)h->cfg.prompt_in * S};
   in[Launch::LENGTHS] = {lengths}; in[Launch::REFER_LENGTHS] = {refer_lengths};
-  in[Launch::CONTENT_OUT] = {content}; in[Launch::PROMPT_OUT] = {prompt};
+  in[Launch::CONTENT_OUT] = {content}; in[Launch::PROMPT_OUT] = {prompt}; in[Launch::SPK] = {spk};
   return run_cached(h, h->simt, in, st, no_launcher);
 }
 
@@ -340,23 +353,28 @@ int ns2vc_pre_finalize(ns2vc_pre* h, ns2vc_stream stream) { return finalize_engi
 int ns2vc_pre_workspace_bytes(const ns2vc_pre* h, int B, int T, int S, size_t* bytes) {
   NS_REQUIRE(h && bytes, "null argument");
   NS_REQUIRE(h->finalized, "ns2vc_pre_finalize() has not been called");
-  // one workspace serves both programs of a shape
-  size_t padded = 0, ragged = 0;
-  int rc = build_program(const_cast<ns2vc_pre*>(h), B, T, S, false, nullptr, &padded);
-  if (!rc) rc = build_program(const_cast<ns2vc_pre*>(h), B, T, S, true, nullptr, &ragged);
-  if (!rc) *bytes = std::max(padded, ragged);
+  // one workspace serves every program of a shape: the padded and ragged ones, the voice program of (B, S) and the content
+  // program of (B, T)
+  size_t need[4] = {0, 0, 0, 0};
+  ns2vc_pre* hm = const_cast<ns2vc_pre*>(h);
+  int rc = build_program(hm, B, T, S, false, nullptr, &need[0]);
+  if (!rc) rc = build_program(hm, B, T, S, true, nullptr, &need[1]);
+  if (!rc) rc = build_program(hm, B, 0, S, true, nullptr, &need[2]);
+  if (!rc) rc = build_program(hm, B, T, 0, true, nullptr, &need[3]);
+  if (!rc) *bytes = *std::max_element(need, need + 4);
   return rc;
 }
 
 }  // extern "C"
 
 namespace {
+// T = 0 / S = 0: the voice / content program (build_program), cached under that shape like the others
 int infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content, float* prompt,
-          int B, int T, int S, void* ws, bool ragged, cudaStream_t st) {
-  NS_REQUIRE(h && c && refer && lengths && refer_lengths && content && prompt, "null argument");
+          float* spk, int B, int T, int S, void* ws, bool ragged, cudaStream_t st) {
   const int rc = ensure_program(h, "ns2vc_pre", B, T, S, ragged, ws, [&] { return build_program(h, B, T, S, ragged, ws, nullptr); });
   if (rc) return rc;
-  return run_program(h, c, refer, reinterpret_cast<const long long*>(lengths), reinterpret_cast<const long long*>(refer_lengths), content, prompt, st);
+  return run_program(h, c, refer, reinterpret_cast<const long long*>(lengths), reinterpret_cast<const long long*>(refer_lengths), content,
+                     prompt, spk, st);
 }
 }  // namespace
 
@@ -364,12 +382,30 @@ extern "C" {
 
 int ns2vc_pre_infer(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content,
                     float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream) {
-  return infer(h, c, refer, lengths, refer_lengths, content, prompt, B, T, S, ws, false, (cudaStream_t)stream);
+  NS_REQUIRE(h && c && refer && lengths && refer_lengths && content && prompt, "null argument");
+  NS_REQUIRE(T >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
+  return infer(h, c, refer, lengths, refer_lengths, content, prompt, nullptr, B, T, S, ws, false, (cudaStream_t)stream);
 }
 
 int ns2vc_pre_infer_ragged(ns2vc_pre* h, const float* c, const float* refer, const int64_t* lengths, const int64_t* refer_lengths, float* content,
                            float* prompt, int B, int T, int S, void* ws, ns2vc_stream stream) {
-  return infer(h, c, refer, lengths, refer_lengths, content, prompt, B, T, S, ws, true, (cudaStream_t)stream);
+  NS_REQUIRE(h && c && refer && lengths && refer_lengths && content && prompt, "null argument");
+  NS_REQUIRE(T >= 1 && S >= 1, "bad shape B=%d T=%d S=%d", B, T, S);
+  return infer(h, c, refer, lengths, refer_lengths, content, prompt, nullptr, B, T, S, ws, true, (cudaStream_t)stream);
+}
+
+int ns2vc_pre_encode_voices_ragged(ns2vc_pre* h, const float* refer, const int64_t* refer_lengths, float* spk, float* prompt, int B, int S,
+                                   void* ws, ns2vc_stream stream) {
+  NS_REQUIRE(h && refer && refer_lengths && spk && prompt, "null argument");
+  NS_REQUIRE(S >= 1, "bad shape B=%d S=%d", B, S);
+  return infer(h, nullptr, refer, nullptr, refer_lengths, nullptr, prompt, spk, B, 0, S, ws, true, (cudaStream_t)stream);
+}
+
+int ns2vc_pre_infer_content_ragged(ns2vc_pre* h, const float* c, const int64_t* lengths, const float* spk, float* content, int B, int T,
+                                   void* ws, ns2vc_stream stream) {
+  NS_REQUIRE(h && c && lengths && spk && content, "null argument");
+  NS_REQUIRE(T >= 1, "bad shape B=%d T=%d", B, T);
+  return infer(h, c, nullptr, lengths, nullptr, content, nullptr, const_cast<float*>(spk), B, T, 0, ws, true, (cudaStream_t)stream);
 }
 
 int ns2vc_pre_num_taps(const ns2vc_pre* h) { return num_taps(h); }

@@ -13,7 +13,8 @@ marshals pointers.  No CPU path; inference only (the reference's training forwar
 from __future__ import annotations
 
 import math
-from typing import Dict, Tuple
+from dataclasses import dataclass
+from typing import Dict, List, Sequence, Tuple
 
 import torch
 import torch.nn as nn
@@ -73,6 +74,25 @@ def pre_param_shapes(cfg: dict) -> Dict[str, Tuple[int, ...]]:
     shapes["ref_enc.proj.weight"] = (R, R); shapes["ref_enc.proj.bias"] = (R,)
     shapes["ref_enc.norm2.weight"] = (R,); shapes["ref_enc.norm2.bias"] = (R,)
     return shapes
+
+
+@dataclass(eq=False)
+class Voice:
+    """A target voice encoded once by ``Pre_model.encode_voices``: everything the condition encoders derive from its prompt mel.
+    ``spk`` [phone_hidden] is ``phoneme_encoder.spk_proj(ref_enc(mel))``, the one vector by which the voice enters the content
+    encoder; ``prompt`` [S_v, prompt_out] is the prompt encoder's output.  Both live on the device of the ``Pre_model`` that
+    encoded them, and only that module (on that device) may use them."""
+    spk: torch.Tensor
+    prompt: torch.Tensor
+    pre_model: "Pre_model"
+
+    @property
+    def S_v(self) -> int:
+        return int(self.prompt.shape[0])
+
+    @property
+    def device(self) -> torch.device:
+        return self.prompt.device
 
 
 class Pre_model(_lib.EngineModule):
@@ -161,6 +181,77 @@ class Pre_model(_lib.EngineModule):
                                          prompt.data_ptr(), B, T, S, ws.data_ptr(), stream))
         # the reference's layouts are the [T, B, C] / [S, B, C] views of the same values (model.py:147, 189)
         return content.transpose(0, 1).to(c_padded.dtype), prompt.transpose(0, 1).to(c_padded.dtype)
+
+    def voice_widths(self) -> Tuple[int, int]:
+        """(phone_hidden, prompt_out): the widths of a ``Voice``'s ``spk`` and ``prompt`` rows."""
+        return _enc_args(self.cfg["phoneme_encoder"], 512)[1], _enc_args(self.cfg["prompt_encoder"], 256)[2]
+
+    def check_voice(self, v, device: torch.device, what: str = "voice") -> Voice:
+        """``v`` if it is a ``Voice`` this module encoded on ``device``; ValueError otherwise."""
+        ph, ro = self.voice_widths()
+        if not isinstance(v, Voice):
+            raise ValueError(f"{what}: expected a Voice, got {type(v).__name__}")
+        if v.pre_model is not self:
+            raise ValueError(f"{what}: this Voice was encoded by another Pre_model")
+        if v.spk.device != device or v.prompt.device != device:
+            raise ValueError(f"{what}: this Voice lives on {v.device}, the call runs on {device}")
+        if tuple(v.spk.shape) != (ph,) or v.prompt.dim() != 2 or v.prompt.shape[1] != ro or v.S_v < 1:
+            raise ValueError(f"{what}: expected spk [{ph}] and prompt [S_v >= 1, {ro}], got {tuple(v.spk.shape)} and {tuple(v.prompt.shape)}")
+        return v
+
+    @torch.no_grad()
+    def encode_voices(self, refer: torch.Tensor, refer_lengths: torch.Tensor) -> List[Voice]:
+        """The voice half of ``infer(per_utterance=True)``: refer [B, 100, S] (mel prompts, zero-padded), refer_lengths [B] in
+        [1, S] -> one ``Voice`` per row, whose ``prompt`` is row b of ``infer``'s prompt output cut to S_b frames and whose
+        ``spk`` is the speaker vector its content rows add; both equal those of the fused call byte for byte."""
+        if not refer.is_cuda:
+            raise RuntimeError("ns2vc_b200.Pre_model has no CPU path: move the module and inputs to an H100 ('cuda')")
+        dev = refer.device
+        _pi, ph, _po, _pl = _enc_args(self.cfg["phoneme_encoder"], 512)
+        ri, _rh, ro, _rl = _enc_args(self.cfg["prompt_encoder"], 256)
+        if refer.dim() != 3 or refer.shape[1] != ri:
+            raise ValueError(f"refer must be [B, {ri}, S], got {tuple(refer.shape)}")
+        B, _, S = refer.shape
+        from .fused import check_lengths
+        sl = check_lengths(refer_lengths, B, S, "refer_lengths")
+        ref = refer.to(torch.float32).contiguous()
+        len_r = refer_lengths.to(dev, torch.int64).contiguous()
+        h = self.engine(dev)
+        ws = self.workspace(B, 1, S, dev)
+        spk = torch.empty((B, ph), dtype=torch.float32, device=dev)
+        prompt = torch.empty((B, S, ro), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().ns2vc_pre_encode_voices_ragged(h, ref.data_ptr(), len_r.data_ptr(), spk.data_ptr(), prompt.data_ptr(),
+                                                                 B, S, ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        return [Voice(spk[b], prompt[b, :int(sl[b])], self) for b in range(B)]
+
+    @torch.no_grad()
+    def infer_content(self, c: torch.Tensor, lengths: torch.Tensor, voices: Sequence[Voice]) -> torch.Tensor:
+        """The content half of ``infer(per_utterance=True)``: c [B, C, T] (stretched ContentVec units), lengths [B] in [1, T] and
+        row b's ``Voice`` -> content [T, B, C_out], row b equal byte for byte to ``infer``'s content row for that voice's prompt
+        mel; frames past T_b are exactly 0."""
+        dev = c.device
+        voices = [self.check_voice(v, dev, f"voice {b}") for b, v in enumerate(voices)]
+        if not c.is_cuda:
+            raise RuntimeError("ns2vc_b200.Pre_model has no CPU path: move the module and inputs to an H100 ('cuda')")
+        pi, _ph, po, _pl = _enc_args(self.cfg["phoneme_encoder"], 512)
+        if c.dim() != 3 or c.shape[1] != pi:
+            raise ValueError(f"c must be [B, {pi}, T], got {tuple(c.shape)}")
+        B, _, T = c.shape
+        if len(voices) != B:
+            raise ValueError(f"{len(voices)} voices for {B} rows")
+        from .fused import check_lengths
+        check_lengths(lengths, B, T, "lengths")
+        cc = c.to(torch.float32).contiguous()
+        len_c = lengths.to(dev, torch.int64).contiguous()
+        spk = torch.stack([v.spk for v in voices]).contiguous()
+        h = self.engine(dev)
+        ws = self.workspace(B, T, 1, dev)
+        content = torch.empty((B, T, po), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().ns2vc_pre_infer_content_ragged(h, cc.data_ptr(), len_c.data_ptr(), spk.data_ptr(), content.data_ptr(),
+                                                                 B, T, ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        return content.transpose(0, 1)
 
     def forward(self, data, g=None):
         """``Pre_model.forward`` (model.py:341-359) in eval mode: (content, audio_prompt, lf0, lf0_pred) with lf0 = lf0_pred = 0."""

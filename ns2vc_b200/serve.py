@@ -39,6 +39,7 @@ from . import _lib, coefs, convert, shard
 from .api import default_schedule
 from .convert import HOP, LATENT_CH
 from .fused import DenoiserSession, _step_table, schedule_signature
+from .pre_model import Voice
 
 NAN_MESSAGE = "NaN in the denoiser input during the fused sampling run (reference model.py:404)"
 
@@ -157,7 +158,8 @@ class ConversionServer:
     ``submit``, and it places each newcomer, FIFO, on the rank with the most free slots (``place_requests``).  Every rank calls
     ``tick()`` and ``drain()`` in lockstep and mirrors the whole placement, so each knows every retirement tick.  Per tick, one
     int64 header broadcast from rank 0 carries the admissions and a global idle flag; when something is admitted, one float32
-    broadcast carries the newcomers' wav | prompt | x_T and one int64 broadcast their (method, steps).  Each rank admits and ticks its own slots, the ranks exchange one status
+    broadcast carries the newcomers' wav | prompt | x_T and one int64 broadcast their (method, steps, prompt kind).  A prompt
+    travels as its mel, or, for a ``Voice``, as its encoded spk | prompt rows, which the admitting rank uses without encoding.  Each rank admits and ticks its own slots, the ranks exchange one status
     flag (an exception on any rank raises a RuntimeError on every rank), and on ticks where something retires one ragged gather
     (``shard.gather_ragged``) brings each result's NaN flag, latent and audio to rank 0.  Rank 0 returns the results and holds
     ``last_latents``; the other ranks return {}.  The default x_T is drawn on rank 0 at ``submit``, as on one GPU, so every
@@ -196,9 +198,11 @@ class ConversionServer:
             self.served = 0                                                            # requests retired on any rank so far
 
     # ------------------------------------------------------------------------------------------------ requests
-    def submit(self, wav: torch.Tensor, sr: int, prompt_mel: torch.Tensor, x_T: Optional[torch.Tensor] = None,
+    def submit(self, wav: torch.Tensor, sr: int, prompt_mel, x_T: Optional[torch.Tensor] = None,
                method: Optional[str] = None, steps: Optional[int] = None) -> int:
-        """Queues one 1-D waveform at ``sr`` with its prompt mel [100, S_b] and returns its ticket (increasing, FIFO).  ``x_T``
+        """Queues one 1-D waveform at ``sr`` with its prompt and returns its ticket (increasing, FIFO).  The prompt is a mel
+        [100, S_b], encoded at admission, or a ``Voice`` of this server's ``pre_model`` (``api.encode_voices``), used as it is;
+        S_b may not exceed ``max_prompt_frames``.  ``x_T``
         ([1, 100, T_b] or [100, T_b]) defaults to ``torch.randn((1, 100, T_b))`` on the model's device, drawn here: requests
         submitted in list order get the draws ``convert_utterances`` makes for that list.  On several ranks only rank 0 submits.
 
@@ -211,9 +215,11 @@ class ConversionServer:
         if steps < 1:
             raise ValueError(f"steps must be >= 1, got {steps}")
         plan = convert._check_inputs([wav], sr, [prompt_mel], None if x_T is None else [x_T])[0]
+        if isinstance(prompt_mel, Voice):
+            self.models[1].check_voice(prompt_mel, self._device(), "prompt")
         if plan["T"] > self.T:
             raise ValueError(f"the waveform is {plan['T']} frames, more than max_frames={self.T}")
-        S_b = int(prompt_mel.shape[1])
+        S_b = convert.prompt_frames(prompt_mel)
         if S_b > self.S:
             raise ValueError(f"the prompt is {S_b} frames, more than max_prompt_frames={self.S}")
         if x_T is None:
@@ -296,36 +302,48 @@ class ConversionServer:
         idle = not adm and all(tab.occupied == 0 for tab in self.tables)
         return pack_header(adm, idle, self.world * self.B)
 
-    def _payload(self, adm) -> List[torch.Tensor]:
-        """Every newcomer's (wav, prompt [100, S_b], x_T [1, 100, T_b]) as sent by rank 0 in one float32 broadcast."""
-        sizes = [(n, LATENT_CH * Sb, LATENT_CH * Tb) for _, _, _, n, _, Tb, Sb in adm]
+    def _payload(self, adm, voiced: Sequence[bool]) -> List[Tuple[torch.Tensor, object, torch.Tensor]]:
+        """Every newcomer's (wav, prompt, x_T [1, 100, T_b]) as sent by rank 0 in one float32 broadcast.  The prompt is its mel
+        [100, S_b], or (``voiced``) its ``Voice``, sent as its spk | prompt rows and rebuilt on this rank's device with this
+        rank's ``pre_model``."""
+        pm = self.models[1]
+        ph, ro = pm.voice_widths() if any(voiced) else (0, 0)
+        sizes = [(n, ph + Sb * ro if v else LATENT_CH * Sb, LATENT_CH * Tb) for (_, _, _, n, _, Tb, Sb), v in zip(adm, voiced)]
         if self.rank == 0:
             parts = []
             for tk, *_ in adm:
                 q = self._requests[tk]
-                parts += [q["wav"].reshape(-1), q["prompt"].reshape(-1), q["x_T"].reshape(-1)]
+                p = q["prompt"]
+                prompt = [p.spk, p.prompt.reshape(-1)] if isinstance(p, Voice) else [p.reshape(-1)]
+                parts += [q["wav"].reshape(-1)] + prompt + [q["x_T"].reshape(-1)]
             dev = self._coll_device()
             flat = torch.cat([p.to(dev if dev is not None else "cpu", torch.float32) for p in parts])
         else:
             flat = torch.empty(sum(sum(z) for z in sizes), dtype=torch.float32)
         flat = self._broadcast(flat)
         out, off = [], 0
-        for (n, np_, nx), (_, _, _, _, _, Tb, Sb) in zip(sizes, adm):
-            out.append((flat[off:off + n], flat[off + n:off + n + np_].view(LATENT_CH, Sb),
-                        flat[off + n + np_:off + n + np_ + nx].view(1, LATENT_CH, Tb)))
+        for (n, np_, nx), (_, _, _, _, _, Tb, Sb), v in zip(sizes, adm, voiced):
+            p = flat[off + n:off + n + np_]
+            if v:
+                dev = self._device()
+                p = Voice(p[:ph].to(dev), p[ph:].view(Sb, ro).to(dev), pm)
+            else:
+                p = p.view(LATENT_CH, Sb)
+            out.append((flat[off:off + n], p, flat[off + n + np_:off + n + np_ + nx].view(1, LATENT_CH, Tb)))
             off += n + np_ + nx
         return out
 
-    def _settings(self, adm) -> List[Tuple[str, int]]:
-        """Every newcomer's (method, steps) as sent by rank 0 in one int64 broadcast: each rank needs them to mirror the
-        retirements, and the newcomer's rank to run its schedule."""
+    def _settings(self, adm) -> List[Tuple[str, int, bool]]:
+        """Every newcomer's (method, steps, whether its prompt is a ``Voice``) as sent by rank 0 in one int64 broadcast: each rank
+        needs them to mirror the retirements, and the newcomer's rank to run its schedule and read its prompt."""
         if self.rank == 0:
-            flat = torch.tensor([v for tk, *_ in adm for v in (_METHOD_CODE[self._requests[tk]["method"]], self._requests[tk]["steps"])],
+            flat = torch.tensor([v for tk, *_ in adm for v in (_METHOD_CODE[self._requests[tk]["method"]], self._requests[tk]["steps"],
+                                                                int(isinstance(self._requests[tk]["prompt"], Voice)))],
                                 dtype=torch.int64)
         else:
-            flat = torch.zeros(2 * len(adm), dtype=torch.int64)
+            flat = torch.zeros(3 * len(adm), dtype=torch.int64)
         v = self._broadcast(flat).tolist()
-        return [(_METHODS[v[2 * i]], int(v[2 * i + 1])) for i in range(len(adm))]
+        return [(_METHODS[v[3 * i]], int(v[3 * i + 1]), bool(v[3 * i + 2])) for i in range(len(adm))]
 
     def _tick_group(self) -> Dict[int, object]:
         if not self._checked:
@@ -336,9 +354,9 @@ class ConversionServer:
         self.last_latents = {}
         if self._idle:
             return {}
-        payload = self._payload(adm) if adm else []
         settings = self._settings(adm) if adm else []
-        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T), (method, steps) in zip(adm, payload, settings):
+        payload = self._payload(adm, [v for _, _, v in settings]) if adm else []
+        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T), (method, steps, _) in zip(adm, payload, settings):
             self.tables[r].enqueue(tk, steps)
             self._frames[tk] = Tb
             if r == self.rank and self.rank != 0:

@@ -19,8 +19,10 @@ import numpy as np
 import torch
 
 from . import _lib, convert
+from .api import encode_voices
 from .content import MIN_SAMPLES
 from .convert import HOP, LATENT_CH, TARGET_SR
+from .pre_model import Voice
 
 # (2 Nc + Ns) fp32 samples staged in shared memory by the SOLA kernel
 SOLA_MAX_SAMPLES = 47 * 1024 // 4
@@ -79,6 +81,8 @@ def fade_in_table(Nc: int) -> np.ndarray:
 
 
 def _check_prompt(p, what: str) -> None:
+    if isinstance(p, Voice):
+        return
     if not isinstance(p, torch.Tensor) or p.dim() != 2 or p.shape[0] != LATENT_CH or p.shape[1] < 1:
         raise ValueError(f"{what}: expected a mel [{LATENT_CH}, S], got {tuple(getattr(p, 'shape', ()))}")
 
@@ -106,8 +110,10 @@ def sola(seg: torch.Tensor, tail: torch.Tensor, fade_in: torch.Tensor, Nb: int, 
 
 class StreamConverter:
     """Converts ``len(prompts)`` live streams at input rate ``sr`` in ticks of ``block_frames`` output frames (0.48 s by default),
-    stream b with the target voice of ``prompts[b]`` (a mel [100, S_b]).  Geometry as ``stream_plan``; ``method`` / ``steps`` as
-    ``convert.convert_utterances`` (UniPC-30 by default, or DPM-Solver++).  Every window and SOLA tail starts as zeros.
+    stream b with the target voice of ``prompts[b]`` (a mel [100, S_b] or a ``Voice``).  Geometry as ``stream_plan``; ``method``
+    / ``steps`` as ``convert.convert_utterances`` (UniPC-30 by default, or DPM-Solver++).  Every window and SOLA tail starts as
+    zeros.  Each prompt mel is encoded once (``api.encode_voices``, at the first tick after it is given), so a tick runs only
+    the content side of the condition encoders.
 
     Attributes after each ``push``: ``seg`` [B, Nb + Nc + Ns] (the end of each converted window that SOLA joined) and
     ``offsets`` [B] int32 (the chosen SOLA offsets)."""
@@ -126,7 +132,8 @@ class StreamConverter:
         self.models = (content_model, pre_model, unet, vocoder)
         self.sr = self.plan["sr"]
         self.device = next(unet.parameters()).device
-        self.prompts = [p.to(self.device, torch.float32) for p in prompts]
+        self.prompts = [p if isinstance(p, Voice) else p.to(self.device, torch.float32) for p in prompts]
+        self.voices = [p if isinstance(p, Voice) else None for p in self.prompts]     # None: encoded at the next tick
         self.B = len(prompts)
         self.window = torch.zeros((self.B, self.plan["W_in"]), dtype=torch.float32, device=self.device)
         self.tail = torch.zeros((self.B, self.plan["Nc"]), dtype=torch.float32, device=self.device)
@@ -155,20 +162,24 @@ class StreamConverter:
         self.window = torch.cat((self.window[:, p["block_in"]:], block.to(dev, torch.float32)), dim=1)
         if x_T is None:
             x_T = [torch.randn((1, LATENT_CH, T), device=dev) for _ in range(B)]
-        r = convert.convert_batch(*self.models, list(self.window.unbind(0)), self.sr, self.prompts, x_T, self.method, self.steps)
+        todo = [b for b, v in enumerate(self.voices) if v is None]
+        for b, v in zip(todo, encode_voices(self.models[1], [self.prompts[b] for b in todo], max_batch=max(len(todo), 1))):
+            self.voices[b] = v
+        r = convert.convert_batch(*self.models, list(self.window.unbind(0)), self.sr, self.voices, x_T, self.method, self.steps)
         audio = torch.stack(r["audio"])
         self.seg = audio[:, T * HOP - p["seg"]:]
         out, self.offsets = sola(self.seg, self.tail, self.fade_in, p["Nb"], p["Nc"], p["Ns"])
         return out.to(block.device)
 
     def reset(self, slot: int, prompt: Optional[torch.Tensor] = None) -> None:
-        """Starts stream ``slot`` again from silence: zeroes its window and SOLA tail and, if given, replaces its prompt mel
-        [100, S] (a prompt longer than the others makes the next tick run a new shape)."""
+        """Starts stream ``slot`` again from silence: zeroes its window and SOLA tail and, if given, replaces its prompt (a mel
+        [100, S] or a ``Voice``; a prompt longer than the others makes the next tick run a new shape)."""
         slot = operator.index(slot)
         if not 0 <= slot < self.B:
             raise IndexError(f"slot {slot} out of range for {self.B} streams")
         if prompt is not None:
             _check_prompt(prompt, "prompt")
-            self.prompts[slot] = prompt.to(self.device, torch.float32)
+            self.prompts[slot] = prompt if isinstance(prompt, Voice) else prompt.to(self.device, torch.float32)
+            self.voices[slot] = prompt if isinstance(prompt, Voice) else None
         self.window[slot].zero_()
         self.tail[slot].zero_()

@@ -114,7 +114,8 @@ def main():
     timer = StageTimer()
     frontend.resample = timer.wrap("resample", frontend.resample)
     cv.extract = timer.wrap("content", cv.extract)
-    pre.infer = timer.wrap("encoders", pre.infer)
+    pre.encode_voices = timer.wrap("encoders", pre.encode_voices)
+    pre.infer_content = timer.wrap("encoders", pre.infer_content)
     convert.sample_latents = timer.wrap("sampler", convert.sample_latents)
     voc.decode = timer.wrap("vocoder", voc.decode)
 
