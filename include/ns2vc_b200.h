@@ -226,6 +226,32 @@ typedef struct ns2vc_ddim_coef {
 int ns2vc_ddim_step(const float* x, const float* x0, const float* noise, const ns2vc_ddim_coef* c, float* x_next, size_t n,
                     int* nan_flag, ns2vc_stream stream);
 
+/* Seeded sampler noise (csrc/philox.cuh): the normal at (seed, step, c, t) is a pure function of those four values, Philox4x32-10
+ * keyed by the 64-bit seed with counter (t >> 2, c, step, 0) and a Box-Muller transform of its outputs, so an utterance's noise does
+ * not depend on its batch, slot, padding or launch.  Step NS2VC_XT_STEP is reserved for the utterance's x_T.
+ *   ns2vc_noise_normal_rows: out [B, C, T] fp32 device, out[b, c, t] = the normal at (seeds[b], step, c, t) for t < T_b and 0 past
+ *   it; seeds [B] int64 device (>= 0), lengths [B] int64 device (T_b in [1, T]) or NULL (every T_b = T). */
+#define NS2VC_XT_STEP 0xFFFFFFFFu
+int ns2vc_noise_normal_rows(const int64_t* seeds, uint32_t step, int C, int T, const int64_t* lengths, float* out, int B,
+                            ns2vc_stream stream);
+
+/* ns2vc_sampler_step_rows with seeded DDPM and DDIM rows as well: method[b] may also be
+ *   NS2VC_ROW_DDPM: struct ddpm_coefs[base[b] + k[b]];  NS2VC_ROW_DDIM: struct ddim_coefs[base[b] + k[b]].
+ * Such a row reads x_in (x) and unet_out (x0) only and writes x_new only (x_new may equal x_in); it never reads m0, m1 or x_prev
+ * and never writes m_new or x_t, so the four-copy rotation above stays the same for every row.  Its step noise is drawn
+ * in-register at (seeds[b], k[b], c, t), where row element i = c * T + t (row_n = C * T), bit-identical to
+ * ns2vc_noise_normal_rows(seeds, k[b], ...); its x_next is bit-identical to ns2vc_ddpm_step / ns2vc_ddim_step fed with that
+ * tensor.  seeds [B] int64 device is required when a DDPM or DDIM table is given; m0, m1, x_prev, m_new and x_t when a DPM-Solver++
+ * or UniPC table is.  A table no occupied row selects may be NULL.  DPM-Solver++ and UniPC rows, empty rows, k and the NaN flags are
+ * as for ns2vc_sampler_step_rows (an empty row leaves a NULL m_new or x_t alone). */
+#define NS2VC_ROW_DDPM 2
+#define NS2VC_ROW_DDIM 3
+int ns2vc_sampler_step_rows_seeded(const float* x_in, const float* unet_out, const float* m0, const float* m1, const float* x_prev,
+                                   const ns2vc_dpm_coef* dpm_coefs, const ns2vc_unipc_coef* unipc_coefs, const ns2vc_ddpm_coef* ddpm_coefs,
+                                   const ns2vc_ddim_coef* ddim_coefs, const int64_t* seeds, int T, const int* method, const int* base,
+                                   int* k, float* m_new, float* x_t, float* x_new, size_t row_n, int B, int* nan_flags,
+                                   ns2vc_stream stream);
+
 /* Bit-exact index helpers (host, no GPU): nearest-neighbour source index of F.interpolate(size=)
  * (reference resnet.py:160) and the stride-2 conv length rule (resnet.py:200). */
 int ns2vc_nearest_index(int t_in, int t_out, int* idx /* [t_out] */);
@@ -700,6 +726,10 @@ int ns2vc_check_packed(int kind, const void* handle, int i, char* name, int name
                        void* hi_out, void* lo_out, ns2vc_stream stream);
 int ns2vc_check_fold_vector(int kind, const void* handle, int i, int j, char* name, int name_len, long long* n, float* out,
                             ns2vc_stream stream);
+
+/* The sampler noise's generator (ns2vc_noise_normal_rows): for each of n entries, raw [n, 4] = Philox4x32-10 of counters [n, 4]
+ * under keys [n, 2] (key lo, hi), and normals [n, 4] = the Box-Muller pair (z0, z1) of outputs (x, y), then of (z, w). */
+int ns2vc_check_philox(const uint32_t* counters, const uint32_t* keys, int n, uint32_t* raw, float* normals, ns2vc_stream stream);
 
 #ifdef __cplusplus
 }

@@ -56,6 +56,10 @@ class UniPcCoef(C.Structure):
                 ("n_c_x", C.c_float), ("n_c_m", C.c_float), ("nab", C.c_float), ("nrk", C.c_float), ("pred_order", C.c_int)]
 
 
+# the row step's methods (NS2VC_ROW_* of the header)
+ROW_DPM, ROW_UNIPC, ROW_DDPM, ROW_DDIM = 0, 1, 2, 3
+
+
 class DdpmCoef(C.Structure):
     _fields_ = [("c_x0", C.c_float), ("c_x", C.c_float), ("c_noise", C.c_float), ("add_noise", C.c_int)]
 
@@ -94,6 +98,9 @@ SIGNATURES = {
     "ns2vc_sampler_step_rows": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_int, _P, _P]),
     "ns2vc_ddpm_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P, _P]),     # (the coefficient struct is a device pointer)
     "ns2vc_ddim_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P, _P]),
+    "ns2vc_sampler_step_rows_seeded": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P, _P, _P, C.c_size_t,
+                                                 C.c_int, _P, _P]),
+    "ns2vc_noise_normal_rows": (C.c_int, [_P, C.c_uint32, C.c_int, C.c_int, _P, _P, C.c_int, _P]),
     "ns2vc_mask_bias": (C.c_int, [_P, C.c_int, _P, _P]),
     "ns2vc_nearest_index": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "ns2vc_down_length": (C.c_int, [C.c_int]),
@@ -200,6 +207,8 @@ SIGNATURES = {
     "ns2vc_check_packed_count": (C.c_int, [C.c_int, _P]),
     "ns2vc_check_packed": (C.c_int, [C.c_int, _P, C.c_int, C.c_char_p, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
     "ns2vc_check_fold_vector": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_char_p, C.c_int, _P, _P, _P]),
+    # the sampler noise's generator (tests/test_seeded_noise.py)
+    "ns2vc_check_philox": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

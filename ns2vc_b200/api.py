@@ -13,6 +13,7 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 
 from .fused import check_lengths, get_session
+from .noise import check_seeds
 from .schedule import NoiseScheduleVP
 from .synth import linear_betas
 from .unet import UNet1DConditionModel
@@ -38,11 +39,14 @@ def sample_latents(unet: UNet1DConditionModel, x_T: torch.Tensor, content_TBC: t
                    prompt_lengths: Optional[torch.Tensor], steps: Optional[int] = None, method: str = "dpmsolver",
                    device: Optional[torch.device] = None, out_device: Optional[torch.device] = None,
                    noise_schedule: Optional[NoiseScheduleVP] = None, skip_type: str = "time_uniform", eta: float = 0.0,
-                   noise: Optional[torch.Tensor] = None, content_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   noise: Optional[torch.Tensor] = None, content_lengths: Optional[torch.Tensor] = None,
+                   noise_seeds: Optional[Sequence[int]] = None) -> torch.Tensor:
     """``method``: ``"dpmsolver"`` / ``"unipc"`` (``steps`` solver steps, default 50), ``"ddim"`` (``steps`` = the reference's
     ``sampling_timesteps``, default 100 as in ``sample()``; ``eta`` = ``ddim_sampling_eta``) or ``"ddpm"`` (``p_sample_loop``: every
     timestep 999 .. 0; ``steps`` may be left unset or be 1000).  DDPM / DDIM draw their noise with ``torch.randn_like`` on the
-    device's default generator, in the reference's order, unless ``noise`` [N, B, 100, T] (one tensor per step) is given.
+    device's default generator, in the reference's order, unless ``noise`` [N, B, 100, T] (one tensor per step) is given, or
+    ``noise_seeds`` (one int in [0, 2**63) per utterance): row b's noise is then drawn on the GPU from its own seed
+    (``ns2vc_b200.noise``), the same bits whatever batch the utterance runs in.
 
     ``content_lengths`` [B] (opt-in): sample a ragged batch.  Row b of the result is then utterance b sampled alone on
     x_T[b, :, :T_b], content[:T_b, b], prompt[:S_b, b] with S_b = ``prompt_lengths[b]`` (S when None), and its frames >= T_b
@@ -60,8 +64,14 @@ def sample_latents(unet: UNet1DConditionModel, x_T: torch.Tensor, content_TBC: t
             raise ValueError(f"method {method!r} uses NaturalSpeech2's own schedule buffers; noise_schedule applies to dpmsolver / unipc")
         if method == "ddpm" and steps not in (None, 1000):
             raise ValueError("method 'ddpm' runs every one of the 1000 timesteps (p_sample_loop); use 'ddim' for fewer steps")
-    elif noise is not None or eta != 0.0:
-        raise ValueError("eta and noise apply to the ddpm / ddim methods")
+        if noise_seeds is not None:
+            if noise is not None:
+                raise ValueError("noise and noise_seeds are mutually exclusive")
+            if not 0.0 <= eta <= 1.0:
+                raise ValueError(f"eta must lie in [0, 1], got {eta}")
+            noise_seeds = check_seeds(noise_seeds, x_T.shape[0], "noise_seeds")
+    elif noise is not None or eta != 0.0 or noise_seeds is not None:
+        raise ValueError("eta, noise and noise_seeds apply to the ddpm / ddim methods")
     if steps is None:
         steps = 100 if method == "ddim" else 50
     dev = torch.device(device) if device is not None else next(unet.parameters()).device
@@ -80,10 +90,10 @@ def sample_latents(unet: UNet1DConditionModel, x_T: torch.Tensor, content_TBC: t
             mask = sequence_mask(prompt_lengths.to(dev, non_blocking=nb), prompt_SBC.shape[0])
         sess = get_session(unet, content, prompt, mask)
     if method == "ddpm":
-        out = sess.sample_ddpm(x, noise=noise)
+        out = sess.sample_ddpm(x, noise=noise, seeds=noise_seeds)
         return out.to(out_device) if out_device is not None else out
     if method == "ddim":
-        out = sess.sample_ddim(x, steps, eta=eta, noise=noise)
+        out = sess.sample_ddim(x, steps, eta=eta, noise=noise, seeds=noise_seeds)
         return out.to(out_device) if out_device is not None else out
     t_T, t_0 = ns.T, 1.0 / ns.total_N
     if skip_type != "time_uniform":
@@ -152,10 +162,13 @@ def pad_batch(items: Sequence[Utterance], idx: Sequence[int]):
 @torch.no_grad()
 def sample_utterances(unet: UNet1DConditionModel, items: Sequence[Utterance], steps: Optional[int] = None, method: str = "dpmsolver",
                       max_batch: int = 8, device: Optional[torch.device] = None, out_device: Optional[torch.device] = None,
-                      noise_schedule: Optional[NoiseScheduleVP] = None, eta: float = 0.0) -> List[torch.Tensor]:
+                      noise_schedule: Optional[NoiseScheduleVP] = None, eta: float = 0.0,
+                      noise_seeds: Optional[Sequence[int]] = None) -> List[torch.Tensor]:
     """Samples a list of utterances of different lengths, ``(x_T [100, T_b], content [T_b, C], prompt [S_b, C])`` each, in
     ragged batches of at most ``max_batch`` (longest first) and returns their latents [100, T_b] in input order.  Each result
-    equals ``sample_latents`` on that utterance alone (DDPM / DDIM: up to the noise draws, see ``DenoiserSession``).
+    equals ``sample_latents`` on that utterance alone.  DDPM / DDIM with ``noise_seeds`` (one per utterance): equal bit for bit
+    to ``sample_latents(noise_seeds=[seed])`` on that utterance alone; without seeds their noise comes from the default
+    generator, drawn over each padded batch, so a result then depends on the batch it ran in.
     The slices of one file (the reference CLI's ``infer.py`` loop) go in as one call."""
     for k, (x, c, p) in enumerate(items):
         if x.dim() != 2 or c.dim() != 2 or p.dim() != 2 or x.shape[1] != c.shape[0]:
@@ -163,11 +176,14 @@ def sample_utterances(unet: UNet1DConditionModel, items: Sequence[Utterance], st
                              f"{tuple(x.shape)}, {tuple(c.shape)}, {tuple(p.shape)}")
         if x.shape[1] < 1 or p.shape[0] < 1:
             raise ValueError(f"utterance {k}: empty content or prompt")
+    if noise_seeds is not None:
+        noise_seeds = check_seeds(noise_seeds, len(items), "noise_seeds")
     out: List[Optional[torch.Tensor]] = [None] * len(items)
     for idx in batch_plan([x.shape[1] for x, _, _ in items], max_batch):
         x, c, p, tl, sl = pad_batch(items, idx)
         lat = sample_latents(unet, x, c, p, sl, steps=steps, method=method, device=device, out_device=out_device,
-                             noise_schedule=noise_schedule, eta=eta, content_lengths=tl)
+                             noise_schedule=noise_schedule, eta=eta, content_lengths=tl,
+                             noise_seeds=[noise_seeds[i] for i in idx] if noise_seeds is not None else None)
         for j, i in enumerate(idx):
             out[i] = lat[j, :, :int(tl[j])]
     return out

@@ -26,7 +26,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import frontend, shard
+from . import frontend, noise, shard
 from .api import batch_plan, encode_voices, sample_latents
 from .content import MIN_SAMPLES, num_frames
 from .pre_model import Voice
@@ -46,7 +46,19 @@ def frame_plan(n: int, sr: int) -> Dict[str, int]:
     return dict(n24=n24, T=n24 // HOP, n16=n16, units=num_frames(n16))
 
 
-def _check_method(method: str, steps: Optional[int]) -> int:
+def _check_method(method: str, steps: Optional[int], seeded: bool = False) -> int:
+    """The step count of ``method``.  DDPM and DDIM are accepted only for seeded rows (``seeded``: each row draws its noise
+    from its own seed, so a row equals its own conversion): DDPM runs all 1000 timesteps (``steps`` None or 1000), DDIM
+    ``steps`` pairs (default 100, ``sample()``'s ``sampling_timesteps``)."""
+    if method in ("ddpm", "ddim") and seeded:
+        if method == "ddpm":
+            if steps not in (None, 1000):
+                raise ValueError("method 'ddpm' runs every one of the 1000 timesteps (p_sample_loop); use 'ddim' for fewer steps")
+            return 1000
+        steps = 100 if steps is None else int(steps)
+        if steps < 1:
+            raise ValueError(f"steps must be >= 1, got {steps}")
+        return steps
     if method in ("ddpm", "ddim"):
         raise ValueError(f"method {method!r}: its per-step noise of a ragged batch is drawn over the padded tensor, so a slice would "
                          "not equal its own conversion; use 'unipc' or 'dpmsolver'")
@@ -75,6 +87,15 @@ class FrontCache:
     def __init__(self) -> None:
         self.units: Dict[int, Tuple[torch.Tensor, torch.Tensor]] = {}
         self.voices: Dict[int, Voice] = {}
+
+
+def _check_seeds(noise_seeds, eta: float, method: str, n: int) -> Optional[List[int]]:
+    """The seeds as n ints (or None), after the checks of ``eta``: in [0, 1], and 0 unless the method is DDIM."""
+    if not 0.0 <= float(eta) <= 1.0:
+        raise ValueError(f"eta must lie in [0, 1], got {eta}")
+    if eta != 0.0 and method != "ddim":
+        raise ValueError("eta applies to the ddim method")
+    return None if noise_seeds is None else noise.check_seeds(noise_seeds, n, "noise_seeds")
 
 
 def _check_inputs(wavs: Sequence[torch.Tensor], sr: int, prompt, x_T) -> List[Dict[str, int]]:
@@ -110,14 +131,22 @@ def _check_inputs(wavs: Sequence[torch.Tensor], sr: int, prompt, x_T) -> List[Di
 
 @torch.no_grad()
 def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int, prompts: Sequence,
-                  x_T: Sequence[torch.Tensor], method: str = "unipc", steps: Optional[int] = None,
-                  cache: Optional[FrontCache] = None) -> Dict[str, List[torch.Tensor]]:
+                  x_T: Optional[Sequence[torch.Tensor]], method: str = "unipc", steps: Optional[int] = None,
+                  cache: Optional[FrontCache] = None, noise_seeds: Optional[Sequence[int]] = None,
+                  eta: float = 0.0) -> Dict[str, List[torch.Tensor]]:
     """Converts ``wavs`` (1-D, at ``sr``) as ONE ragged batch, each with its prompt (a mel [100, S_b] or a ``Voice``) and x_T
     [1, 100, T_b], and returns every stage per utterance, unpadded: ``units`` [D, units_b], ``c`` [D, T_b] (stretched), ``content``
     [T_b, C], ``prompt`` [S_b, C] (the encoders' outputs), ``latent`` [100, T_b] and ``audio`` [T_b * 256].  ``cache``: see
-    ``encode_front``."""
-    steps = _check_method(method, steps)
-    plans = _check_inputs(wavs, sr, list(prompts), list(x_T))
+    ``encode_front``.
+
+    ``noise_seeds`` (one int in [0, 2**63) per waveform): each row's x_T, when ``x_T`` is None, is ``noise.x_T`` of its seed, and
+    ``ddpm`` / ``ddim`` (``eta``: the reference's ``ddim_sampling_eta``) are accepted, each row drawing its step noise from its
+    seed; a row then equals that waveform converted alone with its seed, bit for bit."""
+    steps = _check_method(method, steps, seeded=noise_seeds is not None)
+    noise_seeds = _check_seeds(noise_seeds, eta, method, len(wavs))
+    if x_T is None and noise_seeds is None:
+        raise ValueError("x_T is required without noise_seeds")
+    plans = _check_inputs(wavs, sr, list(prompts), None if x_T is None else list(x_T))
     dev = next(unet.parameters()).device
     check_voices(pre_model, prompts, dev)
     B = len(wavs)
@@ -126,10 +155,15 @@ def convert_batch(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.
     sl = [prompt_frames(p) for p in prompts]
     T = max(tl)
     tl_h, sl_h = torch.tensor(tl, dtype=torch.int64), torch.tensor(sl, dtype=torch.int64)
-    x = torch.zeros((B, LATENT_CH, T), dtype=torch.float32, device=dev)
-    for j, xt in enumerate(x_T):
-        x[j, :, :tl[j]] = xt.reshape(LATENT_CH, tl[j]).to(dev, torch.float32)
-    lat = sample_latents(unet, x, content, prompt, sl_h, steps=steps, method=method, device=dev, content_lengths=tl_h)
+    if x_T is None:
+        x = noise.x_T(noise_seeds, LATENT_CH, tl, dev)
+    else:
+        x = torch.zeros((B, LATENT_CH, T), dtype=torch.float32, device=dev)
+        for j, xt in enumerate(x_T):
+            x[j, :, :tl[j]] = xt.reshape(LATENT_CH, tl[j]).to(dev, torch.float32)
+    seeded = method in ("ddpm", "ddim")
+    lat = sample_latents(unet, x, content, prompt, sl_h, steps=None if method == "ddpm" else steps, method=method, device=dev,
+                         content_lengths=tl_h, eta=eta, noise_seeds=noise_seeds if seeded else None)
     audio = vocoder.decode(lat, tl_h)
     return dict(units=front["units"], c=front["c"], content=[content[:tl[j], j] for j in range(B)],
                 prompt=[prompt[:sl[j], j] for j in range(B)], latent=[lat[j, :, :tl[j]] for j in range(B)],
@@ -192,7 +226,8 @@ def encode_front(content_model, pre_model, wavs: Sequence[torch.Tensor], sr: int
 def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[torch.Tensor], sr: int,
                        prompt: Union[torch.Tensor, Voice, Sequence], method: str = "unipc", steps: Optional[int] = None,
                        max_batch: int = 8, x_T: Optional[Sequence[torch.Tensor]] = None,
-                       group: Optional[dist.ProcessGroup] = None) -> List[torch.Tensor]:
+                       group: Optional[dist.ProcessGroup] = None, noise_seeds: Optional[Sequence[int]] = None,
+                       eta: float = 0.0) -> List[torch.Tensor]:
     """Converts 1-D float32 waveforms at ``sr`` with one prompt (or one per waveform) and returns one 24 kHz waveform
     [T_b * 256] per input, in input order, T_b = resample_out_length(sr, 24000, len) // 256.  The waveforms run in ragged
     batches of at most ``max_batch`` (longest first); each result equals that waveform converted alone.
@@ -206,43 +241,53 @@ def convert_utterances(content_model, pre_model, unet, vocoder, wavs: Sequence[t
 
     With a process ``group`` of more than one rank (one process per GPU, each with its models on its own device, every rank
     making the same call) the waveforms are shared out by ``shard.plan_batches`` and every rank returns the full list; see
-    ``_convert_sharded``."""
-    steps = _check_method(method, steps)
+    ``_convert_sharded``.
+
+    ``noise_seeds`` (one int in [0, 2**63) per waveform) and ``eta``: as for ``convert_batch``.  With seeds, ``ddpm`` and ``ddim``
+    are accepted and an x_T not given comes from each waveform's seed (no draw on the default generator, on any rank); each
+    result equals that waveform converted alone with its seed, bit for bit."""
+    steps = _check_method(method, steps, seeded=noise_seeds is not None)
+    noise_seeds = _check_seeds(noise_seeds, eta, method, len(wavs))
     plans = _check_inputs(wavs, sr, prompt, x_T)
     prompts = list(prompt) if isinstance(prompt, (list, tuple)) else [prompt] * len(wavs)
     dev = next(unet.parameters()).device
     check_voices(pre_model, prompts, dev)
     if group is not None and dist.get_world_size(group) > 1:
-        return _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts, plans, method, steps, max_batch, x_T, group, dev)
-    if x_T is None:
+        return _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts, plans, method, steps, max_batch, x_T, group, dev,
+                                noise_seeds, eta)
+    if x_T is None and noise_seeds is None:
         x_T = [torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans]
     out: List[Optional[torch.Tensor]] = [None] * len(wavs)
     cache = FrontCache()
     for idx in batch_plan([int(w.shape[0]) for w in wavs], max_batch):
         r = convert_batch(content_model, pre_model, unet, vocoder, [wavs[i] for i in idx], sr, [prompts[i] for i in idx],
-                          [x_T[i] for i in idx], method, steps, cache)
+                          None if x_T is None else [x_T[i] for i in idx], method, steps, cache,
+                          None if noise_seeds is None else [noise_seeds[i] for i in idx], eta)
         for j, i in enumerate(idx):
             out[i] = r["audio"][j]
     return out
 
 
 def _convert_sharded(content_model, pre_model, unet, vocoder, wavs, sr, prompts, plans, method, steps, max_batch, x_T, group,
-                     dev) -> List[torch.Tensor]:
+                     dev, noise_seeds=None, eta=0.0) -> List[torch.Tensor]:
     """``convert_utterances`` over the ranks of ``group``: each rank runs its batches of ``shard.plan_batches`` through
     ``convert_batch`` and ``shard.run_sharded`` gathers the audio of all ranks (one status exchange, one all-gather).
 
     The default x_T: every rank draws all of them, in input order on its own device, and keeps its own, so each waveform gets
     the x_T of the one-GPU call and every rank's generator ends where that call leaves it.  The ranks' CUDA generators must
-    therefore start equal, which one all-gather of their seed and offset checks first."""
+    therefore start equal, which one all-gather of their seed and offset checks first.  With ``noise_seeds`` each rank draws only
+    its own rows' x_T, from their seeds, and the generators are neither read nor checked."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     plan = shard.plan_batches(plans, [prompt_frames(p) for p in prompts], world, max_batch)
-    if x_T is None:
+    if x_T is None and noise_seeds is None:
         shard.check_generator(torch.cuda.default_generators[dev.index], group, dev)
         mine = {i for b in plan[rank] for i in b}
         x_T = [x if i in mine else None for i, x in enumerate([torch.randn((1, LATENT_CH, p["T"]), device=dev) for p in plans])]
     cache = FrontCache()
     return shard.run_sharded(lambda idx: convert_batch(content_model, pre_model, unet, vocoder, [wavs[i] for i in idx], sr,
-                                                       [prompts[i] for i in idx], [x_T[i] for i in idx], method, steps, cache)["audio"],
+                                                       [prompts[i] for i in idx], None if x_T is None else [x_T[i] for i in idx],
+                                                       method, steps, cache,
+                                                       None if noise_seeds is None else [noise_seeds[i] for i in idx], eta)["audio"],
                              plan, [p["T"] * HOP for p in plans], group, dev)
 
 

@@ -7,8 +7,10 @@
 // engine_host.cuh).  tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py, tests/test_audio_kernels_fp64.py and
 // tests/test_strided_conv_fp64.py drive them at the shapes and edges the models never reach.  Nothing here is a kernel: every
 // launch is the product's own.  The packed-weight record (ns2vc_check_packed, ns2vc_check_fold_vector) gives back what each
-// engine's packer built, for tests/test_packed_weights_fp64.py.
+// engine's packer built, for tests/test_packed_weights_fp64.py.  The one kernel here, philox_check_kernel, runs the sampler
+// noise's device functions (philox.cuh) on a list of counters and keys for tests/test_seeded_noise.py.
 #include "engine_host.cuh"
+#include "philox.cuh"
 #include "../../include/ns2vc_b200.h"
 
 #include <cstdio>
@@ -58,6 +60,21 @@ template <class... A> void report(char* desc, int desc_len, const char* fmt, A..
 }  // namespace ns2vc
 
 using namespace ns2vc;
+
+namespace ns2vc {
+// Entry j: raw[j] = Philox4x32-10(counters[j], keys[j]); normals[j] = (z0, z1) of the pair (x, y), then of (z, w).
+__global__ void philox_check_kernel(const uint32_t* counters, const uint32_t* keys, int n, uint32_t* raw, float* normals) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t* c = counters + 4 * (size_t)j;
+  const PhiloxOut o = philox4x32_10(c[0], c[1], c[2], c[3], keys[2 * (size_t)j], keys[2 * (size_t)j + 1]);
+  uint32_t* r = raw + 4 * (size_t)j;
+  r[0] = o.x; r[1] = o.y; r[2] = o.z; r[3] = o.w;
+  float* z = normals + 4 * (size_t)j;
+  z[0] = box_muller(o.x, o.y, false); z[1] = box_muller(o.x, o.y, true);
+  z[2] = box_muller(o.z, o.w, false); z[3] = box_muller(o.z, o.w, true);
+}
+}  // namespace ns2vc
 
 extern "C" {
 
@@ -501,6 +518,13 @@ int ns2vc_check_fold_vector(int kind, const void* handle, int i, int j, char* na
   if (rc) return rc;
   if (n) *n = v.n;
   if (out && v.n) NS_CHECK_CUDA(cudaMemcpyAsync(out, v.p, (size_t)v.n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+
+int ns2vc_check_philox(const uint32_t* counters, const uint32_t* keys, int n, uint32_t* raw, float* normals, ns2vc_stream stream) {
+  NS_REQUIRE(counters && keys && raw && normals && n >= 1, "check_philox: null argument or n = %d", n);
+  philox_check_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(counters, keys, n, raw, normals);
+  NS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 

@@ -6,6 +6,7 @@
 // elements with one coefficient struct, the row kernels over the rows of a batch that are at different steps.
 #include "common.cuh"
 #include "launch.cuh"
+#include "philox.cuh"
 #include "../../include/ns2vc_b200.h"
 
 #include <cooperative_groups.h>
@@ -74,18 +75,19 @@ __device__ __forceinline__ void unipc_update(bool& bad, const float* xp, const f
   }
 }
 
-// x_next may be x itself: each element is read before it is written.
-__device__ __forceinline__ void ddpm_update(bool& bad, const float* x, const float* x0, const float* noise,
-                                            const ns2vc_ddpm_coef& c, float* x_next, size_t i) {
+// x_next may be x itself: each element is read before it is written.  `noise` is element i's noise value, a load or an
+// in-register draw; it is produced (and used) only where the step adds noise (add_noise / !last), which the caller tests.
+__device__ __forceinline__ void ddpm_update(bool& bad, const float* x, const float* x0, float noise, const ns2vc_ddpm_coef& c,
+                                            float* x_next, size_t i) {
   const float xv = x[i];
   bad |= (xv != xv);
   // q_posterior mean (:509-512), then mean + exp(0.5 * logvar) * noise; at t == 0 the reference adds exp(.) * 0. (:540-541)
   const float mean = __fadd_rn(__fmul_rn(c.c_x0, x0[i]), __fmul_rn(c.c_x, xv));
-  x_next[i] = __fadd_rn(mean, c.add_noise ? __fmul_rn(c.c_noise, noise[i]) : 0.0f);
+  x_next[i] = __fadd_rn(mean, c.add_noise ? __fmul_rn(c.c_noise, noise) : 0.0f);
 }
 
-__device__ __forceinline__ void ddim_update(bool& bad, const float* x, const float* x0, const float* noise,
-                                            const ns2vc_ddim_coef& c, float* x_next, size_t i) {
+__device__ __forceinline__ void ddim_update(bool& bad, const float* x, const float* x0, float noise, const ns2vc_ddim_coef& c,
+                                            float* x_next, size_t i) {
   const float xv = x[i];
   bad |= (xv != xv);
   const float x0v = x0[i];
@@ -96,7 +98,7 @@ __device__ __forceinline__ void ddim_update(bool& bad, const float* x, const flo
     // kept at eta = 0: it decides the sign of zero results
     const float pn = __fdiv_rn(__fsub_rn(__fmul_rn(c.sqrt_recip, xv), x0v), c.sqrt_recipm1);
     const float r = __fadd_rn(__fmul_rn(x0v, c.sqrt_alpha_next), __fmul_rn(c.c, pn));
-    x_next[i] = __fadd_rn(r, __fmul_rn(c.sigma, noise[i]));
+    x_next[i] = __fadd_rn(r, __fmul_rn(c.sigma, noise));
   }
 }
 
@@ -132,21 +134,26 @@ __global__ void __launch_bounds__(256) unipc_step_kernel(const float* __restrict
 
 // The row kernel: row b of a [B, row_n] batch takes step k[b] of its own run, so the rows of one batch can be at different steps
 // (requests that joined at different ticks) and of different methods.  Row b's method is method[b] (uniform_method for every row
-// when method is NULL) and its struct is dpm[base[b] + k[b]] or unipc[base[b] + k[b]] (base NULL: 0), so one device table per
+// when method is NULL) and its struct is dpm, unipc, ddpm or ddim[base[b] + k[b]] (base NULL: 0), so one device table per
 // struct type holds every schedule in use.  Both methods share one buffer layout (see ns2vc_sampler_step_rows in the header);
-// a DPM row never reads m1 or x_prev and never writes x_t.  Each row is one cluster of kRowCtas CTAs (grid kRowCtas x B); an
-// empty row (k[b] < 0) zeroes m_new, x_t (when given) and x_new and raises nothing.  Every CTA reads k[b] before the cluster
+// a DPM row never reads m1 or x_prev and never writes x_t.  A DDPM or DDIM row reads x_in and o (its x0) only, writes x_new only
+// (which may be x_in itself: each element is read before it is written) and draws its noise in-register at (seeds[b], k[b], c,
+// t) with row element i = c * T + t.  Each row is one cluster of kRowCtas CTAs (grid kRowCtas x B); an
+// empty row (k[b] < 0) zeroes m_new and x_t (when given) and x_new and raises nothing.  Every CTA reads k[b] before the cluster
 // barrier and CTA 0 advances it after, so a captured tick replays with no host write in between.  The NaN flag is per row.
 constexpr int kRowCtas = 8;
 
-__global__ void __launch_bounds__(256) sampler_step_rows_kernel(const float* __restrict__ x_in, const float* __restrict__ o,
+__global__ void __launch_bounds__(256) sampler_step_rows_kernel(const float* x_in, const float* __restrict__ o,
                                                                 const float* __restrict__ m0, const float* __restrict__ m1,
                                                                 const float* __restrict__ x_prev,
                                                                 const ns2vc_dpm_coef* __restrict__ dpm,
                                                                 const ns2vc_unipc_coef* __restrict__ unipc,
+                                                                const ns2vc_ddpm_coef* __restrict__ ddpm,
+                                                                const ns2vc_ddim_coef* __restrict__ ddim,
+                                                                const int64_t* __restrict__ seeds, unsigned T,
                                                                 const int* __restrict__ method, int uniform_method,
                                                                 const int* __restrict__ base, int* k, float* __restrict__ m_new,
-                                                                float* __restrict__ x_t, float* __restrict__ x_new, size_t row_n,
+                                                                float* __restrict__ x_t, float* x_new, size_t row_n,
                                                                 int* nan_flags) {
   pdl_trigger();
   pdl_wait();
@@ -157,19 +164,30 @@ __global__ void __launch_bounds__(256) sampler_step_rows_kernel(const float* __r
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   if (kb < 0) {
     for (; i < row_n; i += stride) {
-      m_new[off + i] = 0.f;
+      if (m_new) m_new[off + i] = 0.f;
       if (x_t) x_t[off + i] = 0.f;
       x_new[off + i] = 0.f;
     }
   } else {
     const int entry = (base ? base[b] : 0) + kb;
+    const int m = method ? method[b] : uniform_method;
     bool bad = false;
-    if ((method ? method[b] : uniform_method) == NS2VC_ROW_DPM) {
+    if (m == NS2VC_ROW_DPM) {
       const ns2vc_dpm_coef c = dpm[entry];
       for (; i < row_n; i += stride) dpm_update(bad, x_in, o, m0, c, m_new, x_new, off + i);
-    } else {
+    } else if (m == NS2VC_ROW_UNIPC) {
       const ns2vc_unipc_coef c = unipc[entry];
       for (; i < row_n; i += stride) unipc_update<true>(bad, x_prev, x_in, o, m0, m1, c, m_new, x_t, x_new, off + i);
+    } else if (m == NS2VC_ROW_DDPM) {
+      const ns2vc_ddpm_coef c = ddpm[entry];
+      const uint64_t seed = (uint64_t)seeds[b];
+      for (; i < row_n; i += stride)
+        ddpm_update(bad, x_in, o, c.add_noise ? seeded_normal(seed, kb, (unsigned)i / T, (unsigned)i % T) : 0.f, c, x_new, off + i);
+    } else {
+      const ns2vc_ddim_coef c = ddim[entry];
+      const uint64_t seed = (uint64_t)seeds[b];
+      for (; i < row_n; i += stride)
+        ddim_update(bad, x_in, o, c.last ? 0.f : seeded_normal(seed, kb, (unsigned)i / T, (unsigned)i % T), c, x_new, off + i);
     }
     if (bad && nan_flags) atomicOr(nan_flags + b, 1);
   }
@@ -184,7 +202,7 @@ __global__ void __launch_bounds__(256) ddpm_step_kernel(const float* x, const fl
   pdl_trigger();
   pdl_wait();
   const ns2vc_ddpm_coef c = *cp;
-  batch_step(n, nan_flag, [&](bool& bad, size_t i) { ddpm_update(bad, x, x0, noise, c, x_next, i); });
+  batch_step(n, nan_flag, [&](bool& bad, size_t i) { ddpm_update(bad, x, x0, c.add_noise ? noise[i] : 0.f, c, x_next, i); });
 }
 
 __global__ void __launch_bounds__(256) ddim_step_kernel(const float* x, const float* __restrict__ x0, const float* __restrict__ noise,
@@ -192,7 +210,23 @@ __global__ void __launch_bounds__(256) ddim_step_kernel(const float* x, const fl
   pdl_trigger();
   pdl_wait();
   const ns2vc_ddim_coef c = *cp;
-  batch_step(n, nan_flag, [&](bool& bad, size_t i) { ddim_update(bad, x, x0, noise, c, x_next, i); });
+  batch_step(n, nan_flag, [&](bool& bad, size_t i) { ddim_update(bad, x, x0, c.last ? 0.f : noise[i], c, x_next, i); });
+}
+
+// out[b, c, t] = the normal at (seeds[b], step, c, t) for t < T_b (lengths[b], or T), 0 past it.  Grid (x: elements, y: rows).
+__global__ void __launch_bounds__(256) noise_normal_rows_kernel(const int64_t* __restrict__ seeds, uint32_t step, int C, int T,
+                                                                const int64_t* __restrict__ lengths, float* __restrict__ out) {
+  pdl_trigger();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const uint64_t seed = (uint64_t)seeds[b];
+  const int64_t Tb = lengths ? lengths[b] : T;
+  const size_t row_n = (size_t)C * T;
+  float* row = out + (size_t)b * row_n;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < row_n; i += (size_t)gridDim.x * blockDim.x) {
+    const unsigned c = (unsigned)i / (unsigned)T, t = (unsigned)i % (unsigned)T;
+    row[i] = (int64_t)t < Tb ? seeded_normal(seed, step, c, t) : 0.f;
+  }
 }
 
 namespace {
@@ -208,11 +242,13 @@ int launch_batch(void (*kernel)(KArgs...), size_t n, int* nan_flag, ns2vc_stream
 }
 
 // The row kernel over B rows.  dpm_step_rows and unipc_step_rows are this launch with one method for every row and one schedule.
+// Every row entry is this launch: the tables, seeds and T an entry does not take are NULL / 0.
 int launch_rows(int B, ns2vc_stream stream, const float* x_in, const float* unet_out, const float* m0, const float* m1,
-                const float* x_prev, const ns2vc_dpm_coef* dpm, const ns2vc_unipc_coef* unipc, const int* method, int uniform_method,
-                const int* base, int* k, float* m_new, float* x_t, float* x_new, size_t row_n, int* nan_flags) {
+                const float* x_prev, const ns2vc_dpm_coef* dpm, const ns2vc_unipc_coef* unipc, const ns2vc_ddpm_coef* ddpm,
+                const ns2vc_ddim_coef* ddim, const int64_t* seeds, int T, const int* method, int uniform_method, const int* base, int* k,
+                float* m_new, float* x_t, float* x_new, size_t row_n, int* nan_flags) {
   launch_kc(sampler_step_rows_kernel, dim3(kRowCtas, B), dim3(256), 0, (cudaStream_t)stream, dim3(kRowCtas, 1, 1), x_in, unet_out, m0,
-            m1, x_prev, dpm, unipc, method, uniform_method, base, k, m_new, x_t, x_new, row_n, nan_flags);
+            m1, x_prev, dpm, unipc, ddpm, ddim, seeds, (unsigned)T, method, uniform_method, base, k, m_new, x_t, x_new, row_n, nan_flags);
   NS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -246,8 +282,8 @@ int ns2vc_dpm_step_rows(const float* x, const float* unet_out, const float* m_pr
                         float* x_next, size_t row_n, int B, int* nan_flags, ns2vc_stream stream) {
   NS_REQUIRE(x && unet_out && m_prev && coefs && k && m_cur && x_next, "null argument");
   NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_rows(B, stream, x, unet_out, m_prev, nullptr, nullptr, coefs, nullptr, nullptr, NS2VC_ROW_DPM, nullptr, k, m_cur,
-                     nullptr, x_next, row_n, nan_flags);
+  return launch_rows(B, stream, x, unet_out, m_prev, nullptr, nullptr, coefs, nullptr, nullptr, nullptr, nullptr, 0, nullptr,
+                     NS2VC_ROW_DPM, nullptr, k, m_cur, nullptr, x_next, row_n, nan_flags);
 }
 
 int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float* unet_out, const float* m0, const float* m1,
@@ -255,8 +291,8 @@ int ns2vc_unipc_step_rows(const float* x_prev, const float* x_eval, const float*
                           int* nan_flags, ns2vc_stream stream) {
   NS_REQUIRE(x_prev && x_eval && unet_out && m0 && m1 && coefs && k && m_t && x_t && x_pred, "null argument");
   NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_rows(B, stream, x_eval, unet_out, m0, m1, x_prev, nullptr, coefs, nullptr, NS2VC_ROW_UNIPC, nullptr, k, m_t, x_t,
-                     x_pred, row_n, nan_flags);
+  return launch_rows(B, stream, x_eval, unet_out, m0, m1, x_prev, nullptr, coefs, nullptr, nullptr, nullptr, 0, nullptr,
+                     NS2VC_ROW_UNIPC, nullptr, k, m_t, x_t, x_pred, row_n, nan_flags);
 }
 
 int ns2vc_sampler_step_rows(const float* x_in, const float* unet_out, const float* m0, const float* m1, const float* x_prev,
@@ -265,8 +301,34 @@ int ns2vc_sampler_step_rows(const float* x_in, const float* unet_out, const floa
   NS_REQUIRE(x_in && unet_out && m0 && m1 && x_prev && method && base && k && m_new && x_t && x_new, "null argument");
   NS_REQUIRE(dpm_coefs || unipc_coefs, "no coefficient table");
   NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
-  return launch_rows(B, stream, x_in, unet_out, m0, m1, x_prev, dpm_coefs, unipc_coefs, method, -1, base, k, m_new, x_t, x_new, row_n,
-                     nan_flags);
+  return launch_rows(B, stream, x_in, unet_out, m0, m1, x_prev, dpm_coefs, unipc_coefs, nullptr, nullptr, nullptr, 0, method, -1, base,
+                     k, m_new, x_t, x_new, row_n, nan_flags);
+}
+
+int ns2vc_sampler_step_rows_seeded(const float* x_in, const float* unet_out, const float* m0, const float* m1, const float* x_prev,
+                                   const ns2vc_dpm_coef* dpm_coefs, const ns2vc_unipc_coef* unipc_coefs, const ns2vc_ddpm_coef* ddpm_coefs,
+                                   const ns2vc_ddim_coef* ddim_coefs, const int64_t* seeds, int T, const int* method, const int* base,
+                                   int* k, float* m_new, float* x_t, float* x_new, size_t row_n, int B, int* nan_flags,
+                                   ns2vc_stream stream) {
+  NS_REQUIRE(x_in && unet_out && method && base && k && x_new, "null argument");
+  NS_REQUIRE(dpm_coefs || unipc_coefs || ddpm_coefs || ddim_coefs, "no coefficient table");
+  NS_REQUIRE(!(dpm_coefs || unipc_coefs) || (m0 && m1 && x_prev && m_new && x_t), "DPM-Solver++ / UniPC buffers missing");
+  NS_REQUIRE(!(ddpm_coefs || ddim_coefs) || seeds, "seeds is NULL with a DDPM / DDIM table");
+  NS_REQUIRE(B >= 1 && B <= 65535 && row_n >= 1, "bad row batch %d x %zu", B, row_n);
+  NS_REQUIRE(T >= 1 && row_n % (size_t)T == 0 && row_n <= 0xFFFFFFFFu, "row_n %zu is not C * T with T = %d", row_n, T);
+  return launch_rows(B, stream, x_in, unet_out, m0, m1, x_prev, dpm_coefs, unipc_coefs, ddpm_coefs, ddim_coefs, seeds, T, method, -1,
+                     base, k, m_new, x_t, x_new, row_n, nan_flags);
+}
+
+int ns2vc_noise_normal_rows(const int64_t* seeds, uint32_t step, int C, int T, const int64_t* lengths, float* out, int B,
+                            ns2vc_stream stream) {
+  NS_REQUIRE(seeds && out, "null argument");
+  NS_REQUIRE(B >= 1 && B <= 65535 && C >= 1 && T >= 1 && (size_t)C * T <= 0xFFFFFFFFu, "bad noise shape [%d, %d, %d]", B, C, T);
+  int blocks = (int)(((size_t)C * T + 255) / 256);
+  if (blocks > 64) blocks = 64;
+  launch_k(noise_normal_rows_kernel, dim3(blocks, B), dim3(256), 0, (cudaStream_t)stream, seeds, step, C, T, lengths, out);
+  NS_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }
 
 int ns2vc_ddpm_step(const float* x, const float* x0, const float* noise, const ns2vc_ddpm_coef* c, float* x_next, size_t n,

@@ -19,7 +19,7 @@ from typing import Optional, Sequence
 
 import torch
 
-from . import _lib, coefs
+from . import _lib, coefs, noise as seeded_noise
 from .unet import UNet1DConditionModel, trace_calls
 
 
@@ -65,9 +65,10 @@ class DenoiserSession:
     the session runs the engine's ragged program, for every sampling method.  Row b of a result is then utterance b
     sampled alone on x_T[b, :, :T_b], content[b, :, :T_b], prompt[b, :S_b]; its frames >= T_b are exactly 0 and input
     values past the lengths are never read.  x_T's padding is zeroed on entry and the denoiser output is zero there, so
-    the DPM-Solver++ / UniPC state stays zero in the padding.  DDPM / DDIM noise is still ``randn_like`` over the padded
-    [B, C, T] tensor (the default generator advances as for one padded call, not as for B separate runs): a row equals its
-    B = 1 run when the caller injects the per-row noise (``noise``), or with the deterministic samplers."""
+    the DPM-Solver++ / UniPC state stays zero in the padding.  DDPM / DDIM noise is by default ``randn_like`` over the padded
+    [B, C, T] tensor (the default generator advances as for one padded call, not as for B separate runs): a row then equals its
+    B = 1 run when the caller injects the per-row noise (``noise``).  With ``seeds`` (one per row) each row draws its own noise
+    in the step kernel from its seed (``ns2vc_b200.noise``), and row b equals utterance b run alone with seeds[b], bit for bit."""
 
     MAX_GRAPHS = 4                                           # LRU bound of captured loops per session
     CAPTURE_AFTER = 3                                        # the loop is captured on its third run, replayed from the fourth
@@ -263,8 +264,8 @@ class DenoiserSession:
             x.masked_fill_(~self.keep, 0.0)
         return x
 
-    def _check_nan(self):
-        if int(self.nan_flag.item()) != 0:
+    def _check_nan(self, flags=None):
+        if int((self.nan_flag if flags is None else flags).max().item()) != 0:
             # same exception type as the reference's per-call guard (model.py:404)
             raise AssertionError("NaN in the denoiser input during the fused sampling run (reference model.py:404)")
 
@@ -272,6 +273,8 @@ class DenoiserSession:
         if self.unet._wsig != self._wsig:                  # weights were re-packed: captured graphs are stale
             self._graphs.clear()
             self._chunk_graphs.clear()
+            for ent in self._chains.values():
+                ent["graphs"].clear()
             self.h = self.unet.engine(self.dev)
             self._wsig = self.unet._wsig
             self._prepared = False
@@ -353,6 +356,12 @@ class DenoiserSession:
                 "x": torch.empty((B, self.Cl, self.T), **f32),
                 "x0": torch.empty((B, self.Co, self.T), **f32),
                 "noise": torch.empty((B, self.Cl, self.T), **f32),
+                # seeded runs: the row step's per-row operands (k advanced by the kernel) and NaN flags
+                "seeds": torch.empty((B,), dtype=torch.int64, device=self.dev),
+                "method": torch.empty((B,), dtype=torch.int32, device=self.dev),
+                "base": torch.zeros((B,), dtype=torch.int32, device=self.dev),
+                "k": torch.empty((B,), dtype=torch.int32, device=self.dev),
+                "nan_rows": torch.empty((B,), dtype=torch.int32, device=self.dev),
             }
         return self._chunk
 
@@ -363,6 +372,26 @@ class DenoiserSession:
         with torch.cuda.device(self.dev):
             _lib.check(fn(x.data_ptr(), cb["x0"].data_ptr(), noise_ptr, coef_ptr, x.data_ptr(), x.numel(), self.nan_flag.data_ptr(),
                           self._stream()))
+
+    def _seeded_step(self, kind, ent):
+        """One step of a seeded run: the row kernel with every row at step k (on the device) of the run's full table."""
+        cb = self._chunk
+        x = cb["x"]
+        tab = ent["coef"].data_ptr()
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.ns2vc_sampler_step_rows_seeded(
+                x.data_ptr(), cb["x0"].data_ptr(), None, None, None, None, None, tab if kind == "ddpm" else None,
+                tab if kind == "ddim" else None, cb["seeds"].data_ptr(), self.T, cb["method"].data_ptr(), cb["base"].data_ptr(),
+                cb["k"].data_ptr(), None, None, x.data_ptr(), self.Cl * self.T, self.B, cb["nan_rows"].data_ptr(), self._stream()))
+
+    def _seeded_body(self, kind, ent, L):
+        """L steps of a seeded run from the time window; the steps' structs and noise follow the device counter k."""
+        cb = self._chunk
+        B, fw = self.B, cb["film_width"]
+        self.time_table(cb["tvals"][:L * B], cb["table"])
+        for k in range(L):
+            self.forward(cb["x"], None, cb["x0"], film_rows=cb["table"][k * B * fw:(k + 1) * B * fw])
+            self._seeded_step(kind, ent)
 
     def _chunk_body(self, kind, draws, noise, j, csize):
         """Steps j .. j+len(draws)-1 of a run, scalars and times from the windows.  noise: the injected [N, B, C, T] tensor or
@@ -380,8 +409,12 @@ class DenoiserSession:
                 nz = None
             self._chain_step(kind, cb["coef"].data_ptr() + k * csize, nz)
 
-    def _chain(self, kind, x_T, key, make_steps, first_out, noise):
+    def _chain(self, kind, x_T, key, make_steps, first_out, noise, seeds=None):
         assert self.Cl == self.Co, "x_start parameterisation needs out_channels == latent channels"
+        if seeds is not None:
+            if noise is not None:
+                raise ValueError("seeds and noise are mutually exclusive: seeded rows draw their own noise")
+            seeds = seeded_noise.check_seeds(seeds, self.B)
         self._sync_engine()
         ent = self._chains.get(key)
         if ent is None:
@@ -389,7 +422,7 @@ class DenoiserSession:
             draws = tuple(s.add_noise for s in steps) if kind == "ddpm" else tuple(not s.last for s in steps)
             coef, csize = coefs.c_table(steps, self.dev)
             ent = {"n": len(steps), "draws": draws, "csize": csize, "coef": coef,
-                   "tvals": coefs.t_inputs(steps, self.B, self.dev).reshape(-1), "runs": 0}
+                   "tvals": coefs.t_inputs(steps, self.B, self.dev).reshape(-1), "runs": 0, "seeded_runs": 0, "graphs": {}}
             self._chains[key] = ent
             while len(self._chains) > self.MAX_GRAPHS:
                 self._chains.popitem(last=False)
@@ -400,11 +433,14 @@ class DenoiserSession:
             if tuple(noise.shape) != (N, B, self.Cl, self.T):
                 raise ValueError(f"noise must be [{N}, {B}, {self.Cl}, {self.T}] (one tensor per step), got {tuple(noise.shape)}")
             noise = noise.to(self.dev, torch.float32).contiguous()
-        else:
-            ent["runs"] += 1
-        use_graph = noise is None and os.environ.get("NS2VC_GRAPH", "1") != "0" and ent["runs"] >= self.CAPTURE_AFTER
+        runs = "seeded_runs" if seeds is not None else "runs"    # (counted apart: each path's first runs are eager)
+        if noise is None:
+            ent[runs] += 1
+        use_graph = noise is None and os.environ.get("NS2VC_GRAPH", "1") != "0" and ent[runs] >= self.CAPTURE_AFTER
         cb = self._chunk_buffers()
         self._unpad(cb["x"].copy_(x_T, non_blocking=True))
+        if seeds is not None:
+            return self._seeded_chain(kind, ent, first_out, seeds, use_graph)
         self.nan_flag.zero_()
         self.prepare()
         j = 0
@@ -439,30 +475,69 @@ class DenoiserSession:
         self._check_nan()
         return self._unpad(res)
 
+    def _seeded_chain(self, kind, ent, first_out, seeds, use_graph):
+        """A seeded run (x_T already in the static x): every step is the row kernel over the run's full coefficient table, its
+        struct and noise picked by the device counter k, so one captured chunk of L steps serves every chunk of that length of
+        this run's schedule.  Those captures bake the table's pointer and live in the run's own entry (dropped with it)."""
+        cb = self._chunk
+        N, B = ent["n"], self.B
+        cb["seeds"].copy_(torch.tensor(seeds, dtype=torch.int64), non_blocking=False)
+        cb["method"].fill_(_lib.ROW_DDPM if kind == "ddpm" else _lib.ROW_DDIM)
+        cb["k"].zero_()
+        cb["nan_rows"].zero_()
+        self.prepare()
+        j = 0
+        if first_out is not None:
+            cb["x0"].copy_(first_out, non_blocking=True)
+            self._seeded_step(kind, ent)
+            j = 1
+        while j < N:
+            L = min(self.CHUNK, N - j)
+            cb["tvals"][:L * B].copy_(ent["tvals"][j * B:(j + L) * B], non_blocking=True)
+            if not use_graph:
+                self._seeded_body(kind, ent, L)
+            else:
+                g = ent["graphs"].get(L)
+                if g is None:
+                    torch.cuda.synchronize(self.dev)
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        self._seeded_body(kind, ent, L)
+                    ent["graphs"][L] = g
+                g.replay()
+            j += L
+        res = cb["x"].clone()
+        self._check_nan(cb["nan_rows"])
+        return self._unpad(res)
+
     def sample_ddpm(self, x_T: torch.Tensor, timesteps=None, noise: Optional[torch.Tensor] = None,
-                    first_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    first_out: Optional[torch.Tensor] = None, seeds=None) -> torch.Tensor:
         """DDPM ancestral sampling, one ``p_sample`` (reference model.py:535-542) per integer t of ``timesteps`` (descending;
         default 999 .. 0: ``p_sample_loop``, :544-561).  Noise: ``torch.randn_like(x)`` on the device's default generator for every
         step with t > 0, in the reference's order, or the injected ``noise`` [N, B, C, T] (row k for step k; the run is then
-        eager).  ``first_out``: the model output at timesteps[0] if the caller already evaluated it."""
+        eager), or with ``seeds`` ([B] ints in [0, 2**63)) row b's step-k noise ``noise.normal_rows(seeds[b], step=k)`` drawn in
+        the step kernel (captured and replayed like the default path).  ``first_out``: the model output at timesteps[0] if the
+        caller already evaluated it."""
         buf = _diffusion_buffers()
         total = buf["betas"].shape[0]
         ts = tuple(range(total - 1, -1, -1)) if timesteps is None else tuple(int(t) for t in timesteps)
         if not ts or any(not 0 <= t < total for t in ts):
             raise ValueError(f"timesteps must be a non-empty list of integers in [0, {total})")
-        return self._chain("ddpm", x_T, ("ddpm", ts), lambda: coefs.ddpm_table(buf, ts), first_out, noise)
+        return self._chain("ddpm", x_T, ("ddpm", ts), lambda: coefs.ddpm_table(buf, ts), first_out, noise, seeds)
 
     def sample_ddim(self, x_T: torch.Tensor, sampling_timesteps: int, eta: float = 0.0, noise: Optional[torch.Tensor] = None,
-                    first_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    first_out: Optional[torch.Tensor] = None, seeds=None) -> torch.Tensor:
         """DDIM (reference ``ddim_sample``, model.py:563-603) over ``sampling_timesteps`` pairs with ``ddim_sampling_eta = eta``.
         Noise: ``torch.randn_like(x)`` once per pair except the last (also at eta = 0, as the reference draws it), or the
-        injected ``noise`` [N, B, C, T]."""
+        injected ``noise`` [N, B, C, T], or drawn per row from ``seeds`` as for ``sample_ddpm`` (eta must then lie in [0, 1])."""
         buf = _diffusion_buffers()
         total = buf["betas"].shape[0]
         S, eta = int(sampling_timesteps), float(eta)
         if S < 1:
             raise ValueError("sampling_timesteps must be >= 1")
-        return self._chain("ddim", x_T, ("ddim", S, eta), lambda: coefs.ddim_table(buf, total, S, eta), first_out, noise)
+        if seeds is not None and not 0.0 <= eta <= 1.0:
+            raise ValueError(f"eta must lie in [0, 1], got {eta}")
+        return self._chain("ddim", x_T, ("ddim", S, eta), lambda: coefs.ddim_table(buf, total, S, eta), first_out, noise, seeds)
 
 
     # ------------------------------------------------------------------ training objective: K evaluations behind one prepare

@@ -13,7 +13,7 @@ re-captures the tick once.
 
 Each request's result equals ``convert.convert_batch`` of that request alone with the same x_T, because every stage keeps row b
 equal to utterance b run alone: the encoders run on the newcomers as one ragged batch, ``ns2vc_unet_prepare_cond_ragged`` keeps its
-lengths in device tables, the FiLM rows are per row, and the row step kernel (``ns2vc_sampler_step_rows``) does the scalar step's
+lengths in device tables, the FiLM rows are per row, and the row step kernel (``ns2vc_sampler_step_rows_seeded``) does the scalar step's
 arithmetic with each row's own method and coefficient struct.
 
 An admission re-prepares only the rows it changes: the newcomers' slots and the slots freed since the last admission, which
@@ -24,21 +24,27 @@ weights are re-packed or when another caller has used the module's shared worksp
 
 A tick costs one forward of the whole slots x max_frames geometry whatever the occupancy (the ragged GEMMs compute padded rows),
 so for a list known in advance ``convert.convert_utterances`` (longest-first batches) remains the faster call: the server buys
-latency under arrivals, not peak throughput.  DDPM / DDIM are refused: their per-step noise would need a generator stream per row.
+latency under arrivals, not peak throughput.
+
+A seeded request (``submit(..., seed=)``) may also use DDPM or DDIM: its row draws its step noise in the row step kernel from its
+own seed (``ns2vc_b200.noise``), so its audio is the same whatever else is in flight, and its x_T defaults to its seed's reserved
+stream.  Unseeded DDPM / DDIM requests are refused as ``convert_utterances`` refuses them.  A DDPM request (1000 steps) grows the
+FiLM table to 1000 x slots rows of ``ns2vc_unet_film_width`` floats each (see DESIGN.md §5 for its size at the real config).
 """
 from __future__ import annotations
 
 import collections
 import os
+import struct
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
 
-from . import _lib, coefs, convert, shard
+from . import _lib, coefs, convert, noise, shard
 from .api import default_schedule
 from .convert import HOP, LATENT_CH
-from .fused import DenoiserSession, _step_table, schedule_signature
+from .fused import DenoiserSession, _diffusion_buffers, _step_table, schedule_signature
 from .pre_model import Voice
 
 NAN_MESSAGE = "NaN in the denoiser input during the fused sampling run (reference model.py:404)"
@@ -95,9 +101,18 @@ class SlotTable:
 
 
 HEADER_FIELDS = 7          # per admission: ticket, rank, slot, samples, sr, T_b, S_b
-_METHODS = ("dpmsolver", "unipc")                    # a row's method tag (NS2VC_ROW_DPM, NS2VC_ROW_UNIPC) and its name
+_METHODS = ("dpmsolver", "unipc", "ddpm", "ddim")    # a row's method tag (NS2VC_ROW_DPM, _UNIPC, _DDPM, _DDIM) and its name
 _METHOD_CODE = {m: i for i, m in enumerate(_METHODS)}
-_KIND = {"dpmsolver": "dpm", "unipc": "unipc"}       # the sampler tables' name of each method
+_KIND = {"dpmsolver": "dpm", "unipc": "unipc", "ddpm": "ddpm", "ddim": "ddim"}   # the sampler tables' name of each method
+SETTINGS_FIELDS = 6        # per admission: method, steps, prompt is a Voice, seeded, seed, eta (its float64 bits)
+
+
+def _eta_bits(eta: float) -> int:
+    return struct.unpack("<q", struct.pack("<d", float(eta)))[0]
+
+
+def _eta_of(bits: int) -> float:
+    return struct.unpack("<d", struct.pack("<q", int(bits)))[0]
 
 
 def place_requests(free: Sequence[int], n: int) -> List[int]:
@@ -199,7 +214,7 @@ class ConversionServer:
 
     # ------------------------------------------------------------------------------------------------ requests
     def submit(self, wav: torch.Tensor, sr: int, prompt_mel, x_T: Optional[torch.Tensor] = None,
-               method: Optional[str] = None, steps: Optional[int] = None) -> int:
+               method: Optional[str] = None, steps: Optional[int] = None, seed: Optional[int] = None, eta: float = 0.0) -> int:
         """Queues one 1-D waveform at ``sr`` with its prompt and returns its ticket (increasing, FIFO).  The prompt is a mel
         [100, S_b], encoded at admission, or a ``Voice`` of this server's ``pre_model`` (``api.encode_voices``), used as it is;
         S_b may not exceed ``max_prompt_frames``.  ``x_T``
@@ -207,13 +222,22 @@ class ConversionServer:
         submitted in list order get the draws ``convert_utterances`` makes for that list.  On several ranks only rank 0 submits.
 
         ``method`` (``"unipc"`` or ``"dpmsolver"``) and ``steps`` are this request's sampler; ``None`` takes the server's
-        ``method`` / ``steps``.  The result equals ``convert_batch`` of the request alone with that method and step count."""
+        ``method`` / ``steps``.  The result equals ``convert_batch`` of the request alone with that method and step count.
+
+        ``seed`` (an int in [0, 2**63)): the request's x_T, when not given, is ``noise.x_T`` of its seed, and ``method`` may also be
+        ``"ddpm"`` (1000 steps) or ``"ddim"`` (``steps`` pairs, default 100; ``eta``: the reference's ``ddim_sampling_eta``), whose
+        step noise the row draws from its seed.  The result then equals ``convert_batch(..., noise_seeds=[seed], eta=eta)`` of the
+        request alone, bit for bit, whatever else is in flight."""
         if self.world > 1 and self.rank != 0:
             raise RuntimeError(f"submit() on rank {self.rank}: only rank 0 of the server's group takes requests")
         method = self.method if method is None else method
-        steps = convert._check_method(method, self.steps if steps is None else steps)
+        if steps is None and method not in ("ddpm", "ddim"):
+            steps = self.steps
+        steps = convert._check_method(method, steps, seeded=seed is not None)
         if steps < 1:
             raise ValueError(f"steps must be >= 1, got {steps}")
+        seeds = convert._check_seeds(None if seed is None else [seed], eta, method, 1)
+        eta = float(eta)
         plan = convert._check_inputs([wav], sr, [prompt_mel], None if x_T is None else [x_T])[0]
         if isinstance(prompt_mel, Voice):
             self.models[1].check_voice(prompt_mel, self._device(), "prompt")
@@ -223,11 +247,12 @@ class ConversionServer:
         if S_b > self.S:
             raise ValueError(f"the prompt is {S_b} frames, more than max_prompt_frames={self.S}")
         if x_T is None:
-            x_T = torch.randn((1, LATENT_CH, plan["T"]), device=self._device())
+            x_T = noise.x_T(seeds, LATENT_CH, [plan["T"]], self._device()) if seeds is not None \
+                else torch.randn((1, LATENT_CH, plan["T"]), device=self._device())
         ticket = self._next_ticket
         self._next_ticket += 1
         self._requests[ticket] = dict(wav=wav, sr=int(sr), prompt=prompt_mel, x_T=x_T, plan=plan, T=plan["T"], S=S_b, method=method,
-                                      steps=steps)
+                                      steps=steps, seed=None if seeds is None else seeds[0], eta=eta)
         if self.world > 1:
             self._pending.append(ticket)
         else:
@@ -263,7 +288,7 @@ class ConversionServer:
     def _step(self, new: List[Tuple[int, int]]):
         """The device work of one tick on this server's slots: the admission of ``new`` (slot, ticket), then the tick."""
         stale = self._setup()
-        stale = self._resident([(self._requests[tk]["method"], self._requests[tk]["steps"]) for _, tk in new]) or stale
+        stale = self._resident([self._setting(self._requests[tk]) for _, tk in new]) or stale
         if new:
             self._admit(new, full=stale or not self._owns_cond())
         elif stale:
@@ -333,17 +358,23 @@ class ConversionServer:
             off += n + np_ + nx
         return out
 
-    def _settings(self, adm) -> List[Tuple[str, int, bool]]:
-        """Every newcomer's (method, steps, whether its prompt is a ``Voice``) as sent by rank 0 in one int64 broadcast: each rank
-        needs them to mirror the retirements, and the newcomer's rank to run its schedule and read its prompt."""
+    def _settings(self, adm) -> List[Tuple[str, int, bool, Optional[int], float]]:
+        """Every newcomer's (method, steps, whether its prompt is a ``Voice``, seed or None, eta) as sent by rank 0 in one int64
+        broadcast (eta as its float64 bits): each rank needs them to mirror the retirements, and the newcomer's rank to run its
+        schedule, draw its noise and read its prompt."""
+        F = SETTINGS_FIELDS
         if self.rank == 0:
-            flat = torch.tensor([v for tk, *_ in adm for v in (_METHOD_CODE[self._requests[tk]["method"]], self._requests[tk]["steps"],
-                                                                int(isinstance(self._requests[tk]["prompt"], Voice)))],
-                                dtype=torch.int64)
+            vals = []
+            for tk, *_ in adm:
+                q = self._requests[tk]
+                vals += [_METHOD_CODE[q["method"]], q["steps"], int(isinstance(q["prompt"], Voice)), int(q["seed"] is not None),
+                         q["seed"] or 0, _eta_bits(q["eta"])]
+            flat = torch.tensor(vals, dtype=torch.int64)
         else:
-            flat = torch.zeros(3 * len(adm), dtype=torch.int64)
+            flat = torch.zeros(F * len(adm), dtype=torch.int64)
         v = self._broadcast(flat).tolist()
-        return [(_METHODS[v[3 * i]], int(v[3 * i + 1]), bool(v[3 * i + 2])) for i in range(len(adm))]
+        return [(_METHODS[v[F * i]], int(v[F * i + 1]), bool(v[F * i + 2]), int(v[F * i + 4]) if v[F * i + 3] else None,
+                 _eta_of(v[F * i + 5])) for i in range(len(adm))]
 
     def _tick_group(self) -> Dict[int, object]:
         if not self._checked:
@@ -355,13 +386,14 @@ class ConversionServer:
         if self._idle:
             return {}
         settings = self._settings(adm) if adm else []
-        payload = self._payload(adm, [v for _, _, v in settings]) if adm else []
-        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T), (method, steps, _) in zip(adm, payload, settings):
+        payload = self._payload(adm, [v for _, _, v, _, _ in settings]) if adm else []
+        for (tk, r, slot, _, sr, Tb, Sb), (wav, prompt, x_T), (method, steps, _, seed, eta) in zip(adm, payload, settings):
             self.tables[r].enqueue(tk, steps)
             self._frames[tk] = Tb
             if r == self.rank and self.rank != 0:
                 plan = convert._check_inputs([wav], sr, [prompt], [x_T])[0]
-                self._requests[tk] = dict(wav=wav, sr=sr, prompt=prompt, x_T=x_T, plan=plan, T=Tb, S=Sb, method=method, steps=steps)
+                self._requests[tk] = dict(wav=wav, sr=sr, prompt=prompt, x_T=x_T, plan=plan, T=Tb, S=Sb, method=method, steps=steps,
+                                          seed=seed, eta=eta)
             elif r != self.rank:
                 self._requests.pop(tk, None)               # (rank 0: placed elsewhere)
         news = [tab.admit(t) for tab in self.tables]
@@ -441,9 +473,9 @@ class ConversionServer:
         self._sess, self._L = sess, _lib.lib()
         self._clen, self._plen = [1] * B, [1] * B
         self._fw = int(self._L.ns2vc_unet_film_width(sess.h))
-        self._sched: Dict[Tuple[str, int], dict] = {}        # (method, steps) -> its tag, its base in its method's table, its t column
-        self._tab: Dict[str, list] = {"dpm": [], "unipc": []}   # the step records of every resident schedule, per method
-        self._coef: Dict[str, Optional[torch.Tensor]] = {"dpm": None, "unipc": None}
+        self._sched: Dict[Tuple[str, int, float], dict] = {}  # (method, steps, eta) -> its tag, its base in its method's table, its t column
+        self._tab: Dict[str, list] = {k: [] for k in ("dpm", "unipc", "ddpm", "ddim")}   # the step records of every resident schedule
+        self._coef: Dict[str, Optional[torch.Tensor]] = {k: None for k in self._tab}
         self._tvals = torch.zeros((0, B), **f32)           # [K, B]: the model time of slot b's request at its step k
         self._film = torch.empty((B, self._fw), **f32)
         self._rowbase = torch.arange(B, dtype=torch.int64, device=dev)
@@ -452,15 +484,21 @@ class ConversionServer:
         self._row_tag = torch.zeros((B,), dtype=torch.int32, device=dev)
         self._row_base = torch.zeros((B,), dtype=torch.int32, device=dev)
         self._nan = torch.zeros((B,), dtype=torch.int32, device=dev)
+        self._seeds = torch.zeros((B,), dtype=torch.int64, device=dev)   # each slot's noise seed (read by DDPM / DDIM rows only)
         shape = (B, sess.Cl, T)
         self._buf = {n: torch.zeros(shape, **f32) for n in ("x_in", "m0", "m1", "x_prev", "m_new", "x_t", "x_new", "out")}
         self._x = self._buf["x_in"]                         # the denoiser input; after a request's last tick, its latent
-        self._resident([(self.method, self.steps)])
-        self._tvals.copy_(self._sched[(self.method, self.steps)]["t"][:, None].expand(self.steps, B))
+        self._resident([(self.method, self.steps, 0.0)])
+        self._tvals.copy_(self._sched[(self.method, self.steps, 0.0)]["t"][:, None].expand(self.steps, B))
         return False
 
-    def _resident(self, settings: Sequence[Tuple[str, int]]) -> bool:
-        """Makes every (method, steps) schedule of ``settings`` resident.  The tables only grow: a schedule not yet resident
+    @staticmethod
+    def _setting(q: dict) -> Tuple[str, int, float]:
+        """A request's schedule key (method, steps, eta)."""
+        return q["method"], q["steps"], q["eta"]
+
+    def _resident(self, settings: Sequence[Tuple[str, int, float]]) -> bool:
+        """Makes every (method, steps, eta) schedule of ``settings`` resident.  The tables only grow: a schedule not yet resident
         appends its coefficient structs to its method's table (the residents keep their bases), re-allocates that table and,
         when it is the longest yet, the FiLM table, and drops the captured tick.  True when that happened: the FiLM rows of
         every slot must then be written again (``_prepare_all``)."""
@@ -468,16 +506,22 @@ class ConversionServer:
         if not new:
             return False
         ns, dev, B = default_schedule(), self._device(), self.B
-        for method, steps in new:
+        for method, steps, eta in new:
             kind = _KIND[method]
-            ts = torch.linspace(ns.T, 1.0 / ns.total_N, steps + 1)
-            extra = True if kind == "dpm" else "bh2"       # lower_order_final / variant, as sample_latents runs them
-            tab = _step_table(kind, ns, ts, extra, (kind, tuple(float(v) for v in ts), extra, schedule_signature(ns)))
-            self._sched[(method, steps)] = dict(tag=_METHOD_CODE[method], base=len(self._tab[kind]),
-                                                t=torch.tensor([st.t_input for st in tab], dtype=torch.float32))
+            if kind == "ddpm":
+                tab = coefs.ddpm_table(_diffusion_buffers(), range(steps - 1, -1, -1))
+            elif kind == "ddim":
+                buf = _diffusion_buffers()
+                tab = coefs.ddim_table(buf, buf["betas"].shape[0], steps, eta)
+            else:
+                ts = torch.linspace(ns.T, 1.0 / ns.total_N, steps + 1)
+                extra = True if kind == "dpm" else "bh2"   # lower_order_final / variant, as sample_latents runs them
+                tab = _step_table(kind, ns, ts, extra, (kind, tuple(float(v) for v in ts), extra, schedule_signature(ns)))
+            self._sched[(method, steps, eta)] = dict(tag=_METHOD_CODE[method], base=len(self._tab[kind]),
+                                                     t=coefs.t_inputs(tab, 1, "cpu")[:, 0])
             self._tab[kind] = self._tab[kind] + list(tab)
             self._coef[kind] = coefs.c_table(self._tab[kind], dev)[0]
-        K = max(steps for _, steps in self._sched)
+        K = max(steps for _, steps, _ in self._sched)
         if K > self._tvals.shape[0]:
             tv = torch.zeros((K, B), dtype=torch.float32, device=dev)
             tv[:self._tvals.shape[0]] = self._tvals
@@ -514,7 +558,8 @@ class ConversionServer:
                     b[s].zero_()
                 self._x[s, :, :Tb] = r["x_T"].reshape(LATENT_CH, Tb).to(dev, torch.float32)
                 self._clen[s], self._plen[s] = Tb, Sb
-                sched = self._sched[(r["method"], r["steps"])]
+                sched = self._sched[self._setting(r)]
+                self._seeds[s] = r["seed"] or 0
                 self._tvals[:r["steps"], s] = sched["t"].to(dev)          # the FiLM rows (k, s) hold this request's own times
                 self._tag[s], self._base[s] = sched["tag"], sched["base"]
         occupied = {s for s in range(self.B) if self.table.ticket[s] is not None}
@@ -558,7 +603,7 @@ class ConversionServer:
 
     def _body(self):
         """One tick: the FiLM row (k_b, b) of every slot, the forward, the row step of every slot with its own method and
-        schedule (``ns2vc_sampler_step_rows``), then the rotation of the sampler's buffers: m1 <- m0 <- m_new, x_prev <- x_t,
+        schedule (``ns2vc_sampler_step_rows_seeded``; DDPM / DDIM rows draw their noise from their seeds), then the rotation of the sampler's buffers: m1 <- m0 <- m_new, x_prev <- x_t,
         x_in <- x_new, the same for both methods (a DPM-Solver++ row never reads m1 or x_prev).  The rotation is four device
         copies inside the one captured graph rather than a cycle of graphs over rotating pointers: UniPC's 3-deep history and
         2-deep state would need lcm(3, 2) = 6 captures of the whole forward, and the copies move 4 x slots x 100 x max_frames
@@ -568,12 +613,13 @@ class ConversionServer:
         torch.index_select(self._film_rows, 0, idx, out=self._film)
         sess.forward(b["x_in"], None, b["out"], film_rows=self._film)
         n, stream = sess.Cl * self.T, sess._stream()
-        dpm, unipc = (t.data_ptr() if t is not None else None for t in (self._coef["dpm"], self._coef["unipc"]))
+        dpm, unipc, ddpm, ddim = (self._coef[k].data_ptr() if self._coef[k] is not None else None
+                                  for k in ("dpm", "unipc", "ddpm", "ddim"))
         with torch.cuda.device(sess.dev):
-            _lib.check(L.ns2vc_sampler_step_rows(b["x_in"].data_ptr(), b["out"].data_ptr(), b["m0"].data_ptr(), b["m1"].data_ptr(),
-                                                 b["x_prev"].data_ptr(), dpm, unipc, self._row_tag.data_ptr(), self._row_base.data_ptr(),
-                                                 self._k.data_ptr(), b["m_new"].data_ptr(), b["x_t"].data_ptr(), b["x_new"].data_ptr(), n,
-                                                 self.B, self._nan.data_ptr(), stream))
+            _lib.check(L.ns2vc_sampler_step_rows_seeded(
+                b["x_in"].data_ptr(), b["out"].data_ptr(), b["m0"].data_ptr(), b["m1"].data_ptr(), b["x_prev"].data_ptr(), dpm, unipc,
+                ddpm, ddim, self._seeds.data_ptr(), self.T, self._row_tag.data_ptr(), self._row_base.data_ptr(), self._k.data_ptr(),
+                b["m_new"].data_ptr(), b["x_t"].data_ptr(), b["x_new"].data_ptr(), n, self.B, self._nan.data_ptr(), stream))
         b["m1"].copy_(b["m0"])
         b["m0"].copy_(b["m_new"])
         b["x_prev"].copy_(b["x_t"])
