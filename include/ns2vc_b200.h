@@ -561,6 +561,8 @@ typedef struct ns2vc_check_gemm_args {
      the descriptor the denoiser builds */
   const double* gn_stats1; const double* gn_stats2; int gn_C1, gn_C2, gn_G; float gn_eps;
   const float* gn_gamma; const float* gn_beta; const float* gn_film; int gn_film_ld;
+  int bn, tma_out;                   /* the launch hook's report of the N tile and TMA stores a program chose (ignored by
+                                        ns2vc_check_gemm, which plans its own) */
 } ns2vc_check_gemm_args;
 typedef struct ns2vc_check_attn_args {
   int B, H, Tq, Tk, dh;
@@ -574,6 +576,7 @@ typedef struct ns2vc_check_attn_args {
   const float* bias;                 /* additive [B, Tk] or NULL */
   float* out; int out_ld;
   void* out_hi; void* out_lo; int out_split_ld;
+  int pb;                            /* the launch hook's report of the v2 box width (ignored by ns2vc_check_attention) */
 } ns2vc_check_attn_args;
 int ns2vc_check_pack_b(const float* w, int n_rows, int cin_total, int ktaps, int tap, int cin0, int ncin, int n_dst0, int kb0,
                        int geglu_half, const float* cscale, void* w_hi, void* w_lo, int Npad, int nkb_total, ns2vc_stream stream);
@@ -726,6 +729,18 @@ int ns2vc_check_packed(int kind, const void* handle, int i, char* name, int name
                        void* hi_out, void* lo_out, ns2vc_stream stream);
 int ns2vc_check_fold_vector(int kind, const void* handle, int i, int j, char* name, int name_len, long long* n, float* out,
                             ns2vc_stream stream);
+
+/* The launch observer of engine `kind` (numbered as for ns2vc_check_packed): while set, every run of the handle's programs
+ * calls fn(user, index, phase, launch_kind, gemm, attn, desc) before (phase 0) and after (phase 1) each launch, with the stream
+ * synchronised, index the launch's position in its program and launch_kind its kind (ns2vc_unet_launch_kind numbering).  For a
+ * GEMM, `gemm` describes the launch as bound to the call's arguments (plain or panel segments; a panel GroupNorm as gn_*), for
+ * an attention `attn`; the other is NULL, and both are NULL for the other kinds.  desc: the kernel and template arguments, as
+ * ns2vc_check_gemm / ns2vc_check_attention report them ("" for the other kinds).  A nonzero return from fn ends the run with an
+ * error.  fn NULL removes the observer.  A run on a capturing stream fails while an observer is set.  Errors: another kind, a
+ * null handle. */
+typedef int (*ns2vc_check_launch_fn)(void* user, int index, int phase, int launch_kind, const ns2vc_check_gemm_args* gemm,
+                                     const ns2vc_check_attn_args* attn, const char* desc);
+int ns2vc_check_set_launch_hook(int kind, void* handle, ns2vc_check_launch_fn fn, void* user);
 
 /* The sampler noise's generator (ns2vc_noise_normal_rows): for each of n entries, raw [n, 4] = Philox4x32-10 of counters [n, 4]
  * under keys [n, 2] (key lo, hi), and normals [n, 4] = the Box-Muller pair (z0, z1) of outputs (x, y), then of (z, w). */

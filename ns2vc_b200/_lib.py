@@ -207,6 +207,8 @@ SIGNATURES = {
     "ns2vc_check_packed_count": (C.c_int, [C.c_int, _P]),
     "ns2vc_check_packed": (C.c_int, [C.c_int, _P, C.c_int, C.c_char_p, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
     "ns2vc_check_fold_vector": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_char_p, C.c_int, _P, _P, _P]),
+    # the run loops' launch observer (tests/test_program_launches_fp64.py)
+    "ns2vc_check_set_launch_hook": (C.c_int, [C.c_int, _P, _P, _P]),
     # the sampler noise's generator (tests/test_seeded_noise.py)
     "ns2vc_check_philox": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
 }

@@ -1047,10 +1047,13 @@ int run_program(ns2vc_unet* h, const Program& pg, const std::vector<Launch>& pro
       case Launch::MASKBIAS: skip = !in[Launch::MASK].p; break;   // no mask: the cross-attention runs without the bias
       default: break;
     }
+    const int index = (int)(&rec - prog.data());
+    if (!rc && !skip && h->hook.fn) rc = observe_launch(h->hook, index, 0, *l, st);
     if (!rc && !skip) {
       rc = run.run(*l);
       if (rc == kEngineKind) rc = no_launcher(rec);
     }
+    if (!rc && !skip && h->hook.fn) rc = observe_launch(h->hook, index, 1, *l, st);
     if (prof) {
       cudaEventRecord(ev_b, st);
       ns2vc_unet::ProfRec pr{(int)rec.kind, ev_a, ev_b, 0, 0, 0, 0, 0};

@@ -497,15 +497,22 @@ struct PackedRecord {
   void add(const std::string& name, const PackedB& pb, std::vector<Vec> vecs = {}) { entries.push_back(Entry{name, pb, std::move(vecs)}); }
 };
 
+// A test-only observer of the run loops (ns2vc_check_set_launch_hook): while `fn` is set, every launch of a run is preceded
+// (phase 0) and followed (phase 1) by observe_launch(), which synchronises the stream and hands the record as launched (index:
+// its position in the program) to the caller's function.  Unset, the loops do what they do without it.
+struct LaunchHook { void* fn = nullptr; void* user = nullptr; };
+int observe_launch(const LaunchHook& hook, int index, int phase, const Launch& l, cudaStream_t st);   // kernel_check.cu
+
 // What every engine handle holds: the reference state_dict, the device memory of its packed weights and their record, whether
-// the loaded weights are packed, and the number of launches of its last run.  Each handle also has a drop_programs() that
-// forgets the launch programs built over the packed weights.
+// the loaded weights are packed, the number of launches of its last run, and the launch observer.  Each handle also has a
+// drop_programs() that forgets the launch programs built over the packed weights.
 struct EngineBase {
   WeightRegistry weights;
   DeviceMem mem;
   PackedRecord packed;
   bool finalized = false;
   int last_launches = 0;
+  LaunchHook hook;
 };
 
 // The C-ABI's <engine>_num_weights / _weight_info / _load_weight / _launch_count
@@ -593,12 +600,15 @@ template <class Build> int ensure_program(SingleProgramEngine* h, const char* en
 template <class Own> int run_cached(SingleProgramEngine* h, bool simt, const CallArgs& in, cudaStream_t st, Own own) {
   const Runner run{simt, &h->cp.taps, st};
   Launch tmp;
-  int count = 0;
+  int count = 0, index = 0;
   for (const Launch& rec : h->cp.prog) {
     int rc;
     const Launch* l = bound(rec, in, tmp, rc);
+    if (!rc && h->hook.fn) rc = observe_launch(h->hook, index, 0, *l, st);
     if (!rc) rc = run.run(*l);
     if (rc == kEngineKind) rc = own(*l);
+    if (!rc && h->hook.fn) rc = observe_launch(h->hook, index, 1, *l, st);
+    ++index;
     if (rc) return rc;
     if (rec.tap_index < 0) ++count;
   }

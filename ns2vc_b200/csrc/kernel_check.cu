@@ -5,14 +5,18 @@
 // the ProgramBuilder helpers, set_group_norm, linear_op, down_conv / pack_resample_conv, cv_conv_gemm / pack_cv_conv,
 // plan_gemm / encode_tmaps / launch_gemm_tc, encode_attn_tmaps / the attention dispatch, the launchers of common.cuh and
 // engine_host.cuh).  tests/test_kernels_fp64.py, tests/test_norm_kernels_fp64.py, tests/test_audio_kernels_fp64.py and
-// tests/test_strided_conv_fp64.py drive them at the shapes and edges the models never reach.  Nothing here is a kernel: every
-// launch is the product's own.  The packed-weight record (ns2vc_check_packed, ns2vc_check_fold_vector) gives back what each
-// engine's packer built, for tests/test_packed_weights_fp64.py.  The one kernel here, philox_check_kernel, runs the sampler
+// tests/test_strided_conv_fp64.py drive them at the shapes and edges the models never reach.  The launches the models make are
+// checked through the launch observer (ns2vc_check_set_launch_hook, observe_launch): the run loops hand each GEMM and attention
+// record, as bound to the call, to tests/test_program_launches_fp64.py in the same flat structs, before and after it runs (the
+// programs that module steps through are listed in its docstring and in DESIGN.md).  Nothing here is a kernel: every launch
+// is the product's own.  The packed-weight record (ns2vc_check_packed, ns2vc_check_fold_vector) gives back what each engine's
+// packer built, for tests/test_packed_weights_fp64.py.  The one kernel here, philox_check_kernel, runs the sampler
 // noise's device functions (philox.cuh) on a list of counters and keys for tests/test_seeded_noise.py.
 #include "engine_host.cuh"
 #include "philox.cuh"
 #include "../../include/ns2vc_b200.h"
 
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -27,18 +31,25 @@ SplitBuf to_split(const ns2vc_check_split& s) {
   return b;
 }
 
-// The packed record of the handle of engine `kind` (0 denoiser, 1 condition encoders, 2 content encoder, 3 vocoder); nullptr
-// (the error is set) for another kind, a null handle, or weights that are not packed
-const PackedRecord* packed_record(int kind, const void* handle) {
+// The EngineBase of the handle of engine `kind` (0 denoiser, 1 condition encoders, 2 content encoder, 3 vocoder); nullptr (the
+// error, prefixed by `fn`, is set) for another kind or a null handle
+const EngineBase* base_of(int kind, const void* handle, const char* fn) {
   const EngineBase* e = nullptr;
   switch (kind) {
     case 0: e = engine_base((const ns2vc_unet*)handle); break;
     case 1: e = engine_base((const ns2vc_pre*)handle); break;
     case 2: e = engine_base((const ns2vc_cv*)handle); break;
     case 3: e = engine_base((const ns2vc_voc*)handle); break;
-    default: set_error("check_packed: engine kind %d (0 denoiser, 1 condition encoders, 2 content encoder, 3 vocoder)", kind); return nullptr;
+    default: set_error("%s: engine kind %d (0 denoiser, 1 condition encoders, 2 content encoder, 3 vocoder)", fn, kind); return nullptr;
   }
-  if (!handle) { set_error("check_packed: null handle"); return nullptr; }
+  if (!handle) { set_error("%s: null handle", fn); return nullptr; }
+  return e;
+}
+
+// The packed record of the handle of engine `kind`; nullptr (the error is set) as for base_of, or for weights that are not packed
+const PackedRecord* packed_record(int kind, const void* handle) {
+  const EngineBase* e = base_of(kind, handle, "check_packed");
+  if (!e) return nullptr;
   if (!e->finalized) { set_error("check_packed: the weights are not packed (finalize has not run since the last load)"); return nullptr; }
   return &e->packed;
 }
@@ -56,7 +67,114 @@ template <class... A> void report(char* desc, int desc_len, const char* fmt, A..
   if (desc && desc_len > 0) snprintf(desc, (size_t)desc_len, fmt, args...);
 }
 
+// the template arguments launch_gemm_tc selects for a planned operator
+void report_gemm(const GemmOp& g, char* desc, int desc_len) {
+  const int f = g.flags;
+  const bool voc = (f & EPI_GELU) != 0, enc = !voc && (f & (EPI_RELU | EPI_ROWMASK));
+  report(desc, desc_len, "gemm_tc<%d,LNF=%d,XF=%d,ENC=%d,RAG=%d,VOC=%d>", g.bn, (f & EPI_LNFOLD) ? 1 : 0, g.xmode ? 1 : 0, enc ? 1 : 0,
+         g.row_len ? 1 : 0, voc ? 1 : 0);
+}
+
+// the kernel the attention dispatch launches for an operator (v2: after encode_attn_tmaps)
+void report_attn(const AttnOp& op, char* desc, int desc_len) {
+  if (op.v2) {
+    const bool pf16 = attention_v2_p_fp16() && !op.p_split;
+    report(desc, desc_len, "attn_v2<%d,PB=%d,BIAS=%d,PF16=%d,RAGK=%d>", op.dh, op.pb, op.bias ? 1 : 0, pf16 ? 1 : 0, op.key_len ? 1 : 0);
+  } else {
+    const int dhp = op.dh <= 16 ? 16 : op.dh <= 32 ? 32 : op.dh <= 48 ? 48 : 64;
+    report(desc, desc_len, "attn_tc<%d>", dhp);
+  }
+}
+
+ns2vc_check_split from_split(const SplitBuf& s) { return ns2vc_check_split{s.hi, s.lo, s.T, s.C, s.ld, s.bpitch}; }
+
+// The flat description of a program's GEMM: its segments as ns2vc_check_gemm takes them, and (panel mode) the affine of its
+// device-side descriptor, read back (the stream is synchronised)
+int flat_gemm(const GemmOp& g, ns2vc_check_gemm_args& a) {
+  memset(&a, 0, sizeof(a));
+  a.B = g.B; a.T_out = g.T_out;
+  a.nsrc = g.nsrc;
+  for (int i = 0; i < g.nsrc; ++i) a.src[i] = from_split(g.src[i]);
+  a.nseg = g.nseg;
+  for (int i = 0; i < g.nseg; ++i) {
+    const GSeg& s = g.seg[i];
+    a.seg[i][0] = s.src; a.seg[i][1] = s.c0; a.seg[i][2] = 64 * s.nkb; a.seg[i][3] = s.tap;
+  }
+  a.nxs = g.xmode ? g.nxs : 0;
+  for (int i = 0; i < a.nxs; ++i) {
+    const XSeg& x = g.xs[i];
+    const int v[8] = {x.src, x.c0, 64 * x.ncb, x.ntap, x.kb_tap[0], x.ntap > 1 ? x.kb_tap[1] - x.kb_tap[0] : 0, x.xf, x.aff_c0};
+    memcpy(a.xseg[i], v, sizeof(v));
+  }
+  a.w_hi = g.w_hi; a.w_lo = g.w_lo; a.N = g.N; a.n_valid = g.n_valid; a.nkb_w = g.nkb_total;
+  a.flags = g.flags;
+  a.bias = g.bias; a.rowbias = g.rowbias; a.rowbias_ld = g.rowbias_ld; a.res = g.res; a.res_ld = g.res_ld;
+  a.out = g.out; a.out_ld = g.out_ld; a.out_hi = g.out_hi; a.out_lo = g.out_lo; a.out_split_ld = g.out_split_ld;
+  a.f16_col0 = g.f16_col0 == 0x7fffffff ? -1 : g.f16_col0;
+  a.ln_stats = g.ln_stats; a.ln_g = g.ln_g; a.ln_C = g.ln_C; a.ln_eps = g.ln_eps;
+  a.row_stats = g.row_stats; a.stat_sum = g.stat_sum; a.stat_sq = g.stat_sq;
+  a.rowmask = g.rowmask; a.row_len = g.row_len; a.len_shift = g.len_shift;
+  a.ksplit = g.ksplit; a.bn = g.bn; a.tma_out = g.tma_out;
+  if (!g.xmode || !g.pre) return 0;
+  PrepOp p;
+  NS_CHECK_CUDA(cudaMemcpy(&p, g.pre, sizeof(p), cudaMemcpyDeviceToHost));
+  a.pre_mode = p.mode;
+  if (p.scale) {
+    a.pre_scale = p.scale; a.pre_shift = p.shift; a.pre_C = p.C1 + p.C2;
+    return 0;
+  }
+  // the flat record carries what set_group_norm derives from its arguments: check that this descriptor is one it built
+  const int Cg = p.C1 + p.C2;
+  NS_REQUIRE(p.gn.G >= 1 && Cg % p.gn.G == 0 && p.gn.sq1 == p.gn.sum1 + (size_t)g.B * p.C1 &&
+             (p.C2 ? p.gn.sq2 == p.gn.sum2 + (size_t)g.B * p.C2 : !p.gn.sum2) &&
+             std::fabs(p.gn.inv_n * (double)g.T_out * (Cg / p.gn.G) - 1.0) < 1e-12,
+             "launch hook: a panel GroupNorm descriptor the flat record cannot express");
+  a.gn_stats1 = p.gn.sum1; a.gn_stats2 = p.gn.sum2; a.gn_C1 = p.C1; a.gn_C2 = p.C2; a.gn_G = p.gn.G; a.gn_eps = p.gn.eps;
+  a.gn_gamma = p.gn.gamma; a.gn_beta = p.gn.beta; a.gn_film = g.pre_film; a.gn_film_ld = p.gn.film_ld;
+  return 0;
+}
+
+void flat_attn(const AttnOp& op, ns2vc_check_attn_args& a) {
+  memset(&a, 0, sizeof(a));
+  a.B = op.B; a.H = op.H; a.Tq = op.Tq; a.Tk = op.Tk; a.dh = op.dh; a.scale = op.scale; a.v2 = op.v2;
+  a.q = op.q; a.q_ld = op.q_ld; a.k = op.k; a.k_ld = op.k_ld; a.v = op.v; a.v_ld = op.v_ld;
+  a.qs = from_split(op.qs); a.ks = from_split(op.ks); a.vs = from_split(op.vs);
+  a.q_c0 = op.q_c0; a.k_c0 = op.k_c0; a.v_c0 = op.v_c0;
+  a.p_split = op.p_split; a.key_len = op.key_len; a.key_shift = op.key_shift; a.bias = op.bias;
+  a.out = op.out; a.out_ld = op.out_ld; a.out_hi = op.out_hi; a.out_lo = op.out_lo; a.out_split_ld = op.out_split_ld;
+  a.pb = op.pb;
+}
+
 }  // namespace
+
+int observe_launch(const LaunchHook& hook, int index, int phase, const Launch& l, cudaStream_t st) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  NS_CHECK_CUDA(cudaStreamIsCapturing(st, &cs));
+  NS_REQUIRE(cs == cudaStreamCaptureStatusNone, "launch hook: the stream is capturing (the observer synchronises it: remove it to capture)");
+  NS_CHECK_CUDA(cudaStreamSynchronize(st));
+  ns2vc_check_gemm_args ga;
+  ns2vc_check_attn_args aa;
+  const ns2vc_check_gemm_args* gp = nullptr;
+  const ns2vc_check_attn_args* ap = nullptr;
+  char desc[96] = "";
+  if (l.kind == Launch::GEMM) {
+    const GemmOp& g = l.get<GemmOp>();
+    const int rc = flat_gemm(g, ga);
+    if (rc) return rc;
+    report_gemm(g, desc, sizeof(desc));
+    gp = &ga;
+  } else if (l.kind == Launch::ATTN) {
+    const AttnOp& a = l.get<AttnOp>();
+    flat_attn(a, aa);
+    report_attn(a, desc, sizeof(desc));
+    ap = &aa;
+  }
+  const int r = ((ns2vc_check_launch_fn)hook.fn)(hook.user, index, phase, (int)l.kind, gp, ap, desc);
+  NS_REQUIRE(r == 0, "launch hook: the observer returned %d at launch %d (phase %d)", r, index, phase);
+  NS_CHECK_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
 }  // namespace ns2vc
 
 using namespace ns2vc;
@@ -172,10 +290,7 @@ int ns2vc_check_gemm(const ns2vc_check_gemm_args* a, char* desc, int desc_len, n
   if (!rc) rc = launch_gemm_tc(g, st);
   if (pre_dev) NS_CHECK_CUDA(cudaFreeAsync(pre_dev, st));
   if (rc) return rc;
-  // the template arguments launch_gemm_tc selects for this operator
-  const bool voc = (f & EPI_GELU) != 0, enc = !voc && (f & (EPI_RELU | EPI_ROWMASK));
-  report(desc, desc_len, "gemm_tc<%d,LNF=%d,XF=%d,ENC=%d,RAG=%d,VOC=%d>", g.bn, (f & EPI_LNFOLD) ? 1 : 0, g.xmode ? 1 : 0, enc ? 1 : 0,
-         g.row_len ? 1 : 0, voc ? 1 : 0);
+  report_gemm(g, desc, desc_len);
   return 0;
 }
 
@@ -198,8 +313,7 @@ int ns2vc_check_attention(const ns2vc_check_attn_args* a, char* desc, int desc_l
     int rc = encode_attn_tmaps(op);
     if (!rc) rc = launch_attention_v2(op, st);
     if (rc) return rc;
-    const bool pf16 = attention_v2_p_fp16() && !op.p_split;
-    report(desc, desc_len, "attn_v2<%d,PB=%d,BIAS=%d,PF16=%d,RAGK=%d>", op.dh, op.pb, op.bias ? 1 : 0, pf16 ? 1 : 0, op.key_len ? 1 : 0);
+    report_attn(op, desc, desc_len);
     return 0;
   }
   NS_REQUIRE(a->q && a->k && a->v, "check_attention: v1 needs fp32 q / k / v");
@@ -207,8 +321,7 @@ int ns2vc_check_attention(const ns2vc_check_attn_args* a, char* desc, int desc_l
   op.q = a->q; op.q_ld = a->q_ld; op.k = a->k; op.k_ld = a->k_ld; op.v = a->v; op.v_ld = a->v_ld;
   const int rc = launch_attention(op, st, false);
   if (rc) return rc;
-  const int dhp = a->dh <= 16 ? 16 : a->dh <= 32 ? 32 : a->dh <= 48 ? 48 : 64;
-  report(desc, desc_len, "attn_tc<%d>", dhp);
+  report_attn(op, desc, desc_len);
   return 0;
 }
 
@@ -518,6 +631,14 @@ int ns2vc_check_fold_vector(int kind, const void* handle, int i, int j, char* na
   if (rc) return rc;
   if (n) *n = v.n;
   if (out && v.n) NS_CHECK_CUDA(cudaMemcpyAsync(out, v.p, (size_t)v.n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+
+int ns2vc_check_set_launch_hook(int kind, void* handle, ns2vc_check_launch_fn fn, void* user) {
+  EngineBase* e = const_cast<EngineBase*>(base_of(kind, handle, "check_set_launch_hook"));
+  if (!e) return -1;
+  e->hook.fn = (void*)fn;
+  e->hook.user = fn ? user : nullptr;
   return 0;
 }
 

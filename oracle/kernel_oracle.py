@@ -161,10 +161,12 @@ def gemm_truth(A: torch.Tensor, W: torch.Tensor, ep: Dict) -> torch.Tensor:
     return gemm_epilogue(A.to(F64) @ W.to(F64).T, ep)
 
 
-def gemm_emulate(A: torch.Tensor, W: torch.Tensor, ep: Dict, drop: Optional[int] = None, a_split: Optional[Tuple] = None):
-    """(emulation, bound): A as bf16 hi/lo (or the given split pair), W fp32 as bf16 hi/lo, 3-term product, epilogue."""
+def gemm_emulate(A: torch.Tensor, W: torch.Tensor, ep: Dict, drop: Optional[int] = None, a_split: Optional[Tuple] = None,
+                 w_split: Optional[Tuple] = None):
+    """(emulation, bound): A as bf16 hi/lo (or the given split pair), W fp32 as bf16 hi/lo (or the given packed pair), 3-term
+    product, epilogue."""
     ah, al = a_split if a_split is not None else split_f64(A)
-    wh, wl = split_f64(W)
+    wh, wl = w_split if w_split is not None else split_f64(W)
     acc = product3(ah, al, wh, wl, drop)
     if drop is not None:
         return gemm_epilogue(acc, ep), None
@@ -204,22 +206,28 @@ def attention_design_terms(q, k, v, scale: float, bias, nkeys, out: torch.Tensor
 
 
 def attention_emulate(q, k, v, scale: float, bias: Optional[torch.Tensor], nkeys: Sequence[int], mode: str,
-                      drop: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                      drop: Optional[int] = None, splits: Optional[Tuple] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """(emulation, bound) of one flash launch.  mode: "f16" (v2, fp16 P, V as fp16 hi/lo), "split" (v2, bf16 hi/lo P and V),
-    "v1" (attn_tc_kernel: q pre-scaled in fp32 before its split, bf16 hi/lo P and V).  q/k/v fp32 [B, H, T, dh]."""
+    "v1" (attn_tc_kernel: q pre-scaled in fp32 before its split, bf16 hi/lo P and V).  q/k/v fp32 [B, H, T, dh].  splits (v2):
+    the launch's own (qh, ql, kh, kl, vh, vl) in fp64 instead of the splits of q / k / v (a producer's split of x need not be
+    the split of fp32(hi + lo): where lo is half an ulp of hi, round-to-even may split the sum the other way)."""
     dev = q.device
     B, H, Tq, dh = q.shape
     Tk = k.shape[2]
     qs32 = torch.tensor(scale, dtype=torch.float32) * torch.tensor(LOG2E, dtype=torch.float32)
-    if mode == "v1":
-        qh, ql = split_f64(q.float() * qs32.to(dev))
-        qs = 1.0
-    else:
-        qh, ql = split_f64(q)
-        qs = float(qs32)
-    kh, kl = split_f64(k)
     vdt = torch.float16 if mode == "f16" else torch.bfloat16
-    vh, vl = split_f64(v, vdt)
+    if splits is not None:
+        qh, ql, kh, kl, vh, vl = splits
+        qs = float(qs32)
+    else:
+        if mode == "v1":
+            qh, ql = split_f64(q.float() * qs32.to(dev))
+            qs = 1.0
+        else:
+            qh, ql = split_f64(q)
+            qs = float(qs32)
+        kh, kl = split_f64(k)
+        vh, vl = split_f64(v, vdt)
     raw = product3(qh, ql, kh, kl, drop)                      # [B, H, Tq, Tk]
     s = raw * qs
     if bias is not None:
@@ -234,7 +242,9 @@ def attention_emulate(q, k, v, scale: float, bias: Optional[torch.Tensor], nkeys
     m = torch.full((B, H, Tq, 1), float("-inf"), dtype=F64, device=dev)
     l = torch.zeros((B, H, Tq, 1), dtype=F64, device=dev)
     o = torch.zeros((B, H, Tq, dh), dtype=F64, device=dev)
-    # fp16 weights within the kernel's error of a rounding midpoint may round the other way there: one fp16 ulp each
+    # A weight within the kernel's error of a rounding boundary of its 16-bit form may round the other way there: one fp16 ulp
+    # of an fp16 weight (numerator and row sum), 2^-16 p of a bf16 hi/lo weight near a boundary of its hi or lo half
+    # (numerator only: the row sum adds the fp32 weights)
     flip_o = torch.zeros((B, H, Tq, dh), dtype=F64, device=dev)
     flip_l = torch.zeros((B, H, Tq, 1), dtype=F64, device=dev)
     for j0 in range(0, Tk, KEYS):
@@ -244,22 +254,27 @@ def attention_emulate(q, k, v, scale: float, bias: Optional[torch.Tensor], nkeys
         l, o, flip_o, flip_l = l * corr, o * corr, flip_o * corr, flip_l * corr
         p = torch.exp2(st - mn).float()                        # the kernel's fp32 weights
         vj_h, vj_l = vh[..., j0:j0 + KEYS, :], vl[..., j0:j0 + KEYS, :]
+        p64 = p.to(F64)
+        err_p = p64 * (4 * u + math.log(2.0) * ds[..., j0:j0 + KEYS])
         if mode == "f16":
-            p64 = p.to(F64)
             p16 = p.to(torch.float16).to(F64)
             l = l + p16.sum(-1, keepdim=True)
             o = o + p16 @ (vj_h + vj_l)
             ulp = torch.where(p64 >= 2.0 ** -14, 2.0 ** (torch.floor(torch.log2(p64.clamp_min(2.0 ** -14))) - 10),
                               torch.full_like(p64, 2.0 ** -24))
-            err_p = p64 * (4 * u + math.log(2.0) * ds[..., j0:j0 + KEYS])
             near = ((ulp / 2 - (p64 - p16).abs()) <= err_p) & (p64 > 0)
             fu = torch.where(near, ulp, torch.zeros_like(ulp))
-            flip_o = flip_o + fu @ absv[..., j0:j0 + KEYS, :]
             flip_l = flip_l + fu.sum(-1, keepdim=True)
         else:
             ph, pl = split_f64(p)
-            l = l + p.to(F64).sum(-1, keepdim=True)
+            l = l + p64.sum(-1, keepdim=True)
             o = o + ph @ vj_h + pl @ vj_h + ph @ vj_l
+            ulp_of = lambda x: 2.0 ** (torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -140))) - 7)
+            r = p64 - ph
+            near_hi = (ulp_of(p64) / 2 - r.abs()) <= err_p
+            near_lo = (r != 0) & ((ulp_of(r) / 2 - (r - pl).abs()) <= err_p)
+            fu = torch.where((near_hi | near_lo) & (p64 > 0), 2.0 ** -16 * p64, torch.zeros_like(p64))
+        flip_o = flip_o + fu @ absv[..., j0:j0 + KEYS, :]
         m = mn
     out = o / l
     # bound: fp32 accumulation of the weighted |v|, the score errors (a score error ds moves a weight by p ln2 ds), the flips
